@@ -1,13 +1,16 @@
 # -*- coding: utf-8 -*-
-"""bench.py -- images/sec of the LFD hot path (forward + device post-process) on B200.
+"""bench.py -- images/sec of the LFD hot path (forward + device post-process) on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config WIDERFACE_S]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config WIDERFACE_S] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 Workload (BASELINE.json configs[1]): WIDERFACE-S, 1280x720, batch 8 per GPU, bf16, synthetic frames and synthetic
 weights (tests/synth.py; no network for datasets / checkpoints).  One step = one batch: backbone + neck + head
 (CUDA-graph replay of the layer plan) + score / decode / NMS (lfd_postprocess).  Multi-GPU: the batch dimension
 shards across ranks, one process per GPU, no collective on the inference path (weak scaling: 8 frames per GPU).
+
+Exactly K steps are timed, after W warm-up steps.  --dump-outputs DIR writes what the timed path computed in its last step
+(rank 0) as DIR/<name>.npy; the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 
 Prints ONE JSON line (rank 0).  `value` = images/s with the uint8 frames already resident in HBM; `e2e` = the same
 through StreamingDetector with HOST (pinned) frames in and HOST detections out; `roofline` = the dominant kernel of the
@@ -41,7 +44,7 @@ WORKLOADS = {
     # configs[4]: fp16 4K throughput sweep, batch-sharded (2 frames per GPU per step)
     'WIDERFACE_XS_4K': dict(cfg='WIDERFACE_XS', N=2, H=2160, W=3840, dtype='fp16', name='WIDERFACE-XS inference 3840x2160 batch=2 per GPU', pool=4),
 }
-POOL = 8          # device-resident input batches rotated through (8 x 22 MB = 177 MB > 126 MB L2)
+POOL = 8          # device-resident input batches rotated through (8 x 22 MB = 177 MB > 50 MB L2)
 IOU_THR = 0.3     # WIDERFACE_train/predict.py:22
 PASS_FRACTION = 0.005
 
@@ -51,7 +54,7 @@ def peaks():
     if os.path.exists(path):
         d = json.load(open(path))
         return dict(hbm_gbs=float(d['hbm_gbs']), bf16_tflops=float(d.get('bf16_tflops_sustained', d['bf16_tflops'])), source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm_gbs=6650.0, bf16_tflops=1400.0, source='fallback (B200_PROFILING.md)')
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, source='H100 SXM data sheet (dense bf16, 700 W); not measured')
 
 
 class ClockSampler(object):
@@ -131,21 +134,6 @@ class ClockSampler(object):
                     source='nvidia-smi')
 
 
-def ncu_traffic(cfg, dtype, kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel`, from the committed `ncu --set full` capture:
-    profiles/ncu_traffic.json is written by profiles/ncu_parse.py from the .ncu-rep that profiles/ncu_run.sh produces
-    (re-run both after a kernel change).  None when that kernel has no capture."""
-    path = os.path.join(ROOT, 'profiles', 'ncu_traffic.json')
-    if not os.path.exists(path):
-        return None
-    try:
-        table = json.load(open(path))
-    except Exception:
-        return None
-    e = table.get('%s/%s' % (cfg, dtype), {}).get(kernel)
-    return None if e is None else int(e['dram_bytes_read'] + e['dram_bytes_write'])
-
-
 def op_algorithmic(row, N, input_bytes_per_px):
     """(bytes, flops) one launch must move / compute: input once, output once, residual once, weights once."""
     k, cin, cout = row['ksize'], row['Cin'], row['Cout']
@@ -199,6 +187,25 @@ def directional_peaks(dev):
     r = best(lambda: a.sum())
     del a
     return dict(write_only_gbs=w, read_only_gbs=r, how='torch fill_ / sum over 512 MB fp32, best of 5')
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """arrays: name -> float32 / float64 numpy array.  Arrays are written whole while they fit in 64 MB together; beyond that the
+    largest ones are replaced by a fixed, seeded sample of their flattened elements (same sample for the same shape)."""
+    os.makedirs(out_dir, exist_ok=True)
+    budget = DUMP_BYTES - 256 * len(arrays)     # room for the .npy headers
+    for name in sorted(arrays, key=lambda k: arrays[k].nbytes):
+        a = np.ascontiguousarray(arrays[name])
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        share = budget // max(1, len(arrays) - sorted(arrays, key=lambda k: arrays[k].nbytes).index(name))
+        if a.nbytes > share:
+            idx = np.sort(np.random.RandomState(0).choice(a.size, share // a.itemsize, replace=False))
+            a, name = a.reshape(-1)[idx], name + '_sample'
+        np.save(os.path.join(out_dir, name + '.npy'), a)
+        budget -= a.nbytes
 
 
 def op_name(row):
@@ -403,42 +410,31 @@ def train_main(args):
     for i in range(max(warmup, 3)):           # W warm-up steps (the first ones also capture the forward / backward CUDA graphs)
         lv = step(i)
     sync_all()
-    p0, p1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    p0.record()
-    step(0)
-    p1.record()
-    sync_all()
-    est_ms = max(p0.elapsed_time(p1), 1e-3)
-    blocks = int(min(50, max(1, -(-args.min_timed_s * 1e3 // (est_ms * args.steps)))))
-    tb = torch.tensor([blocks], dtype=torch.int64, device=dev)
-    if world > 1:
-        dist.all_reduce(tb, op=dist.ReduceOp.MAX)
-    blocks = int(tb.item())
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
-    block_ms, losses = [], []
-    for b in range(blocks):
-        sync_all()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for i in range(args.steps):
-            lv = step(b * args.steps + i)
-        e1.record()
-        sync_all()
-        block_ms.append(e0.elapsed_time(e1))
-        losses.append(lv['loss'])
+    sync_all()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for i in range(args.steps):                # exactly K timed steps
+        lv = step(i)
+    e1.record()
+    sync_all()
     clocks = sampler.stop() if rank == 0 else None
-    t = torch.tensor(block_ms, dtype=torch.float64, device=dev)
+    t = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
-    block_ms = [float(v) for v in t.tolist()]
-    ms_total = float(sum(block_ms))
-    ms_step = ms_total / (args.steps * blocks)
-    value = world * N * args.steps * blocks / (ms_total / 1e3)
+    ms_total = float(t.item())
+    ms_step = ms_total / args.steps
+    value = world * N * args.steps / (ms_total / 1e3)
+    if args.dump_outputs and rank == 0:        # what the last timed step computed: its loss values and the updated parameters
+        flat = model._flat_parameters
+        dump_outputs(args.dump_outputs, dict({'loss_' + k: np.array([float(v)], np.float64) for k, v in lv.items()},
+                                             parameters=flat.data.detach().float().cpu().numpy(),
+                                             gradients=flat.grad.detach().float().cpu().numpy()))
 
     # ---- end to end: pinned host uint8 crops in (H2D inside the timed region), loss values out (the reference's three .item() reads)
-    e2e_steps = args.steps * blocks
+    e2e_steps = args.steps
     copy_stream = torch.cuda.Stream(device=dev)
     stage = [torch.empty((N, H, W, 3), dtype=torch.uint8, device=dev) for _ in range(2)]
     sync_all()
@@ -521,7 +517,7 @@ def train_main(args):
         e = by_kind.setdefault(kname, dict(ms=0.0, bound_ms=0.0, launches=0))
         e['ms'] += r['ms']; e['bound_ms'] += r['t_bound_ms']; e['launches'] += 1
     net_bound_ms = float(sum(r['t_bound_ms'] for r in table))
-    roofline = dict(bound='hbm' if hbm_bound else 'tensor', achieved=achieved, peak=peak, unit=unit, frac=achieved / peak, traffic=None,
+    roofline = dict(bound='hbm' if hbm_bound else 'tensor', achieved=achieved, peak=peak, unit=unit, frac=achieved / peak,
                     peak_source=pk['source'], kernel='%s (%s)' % (train_op_name(top['op']), top['which']), kernel_ms=top['ms'],
                     kernel_share_of_step=top['ms'] / sum_ms, algorithmic_bytes=top['bytes'], algorithmic_flops=top['flops'],
                     net=dict(layerwise_bound_ms=net_bound_ms, plan_ms_eager_sum=sum_ms, frac_of_layerwise_bound=net_bound_ms / sum_ms,
@@ -534,7 +530,7 @@ def train_main(args):
     launches = len(plan.fwd_ops) + len(plan.bwd_ops) + 5 + 2      # + assign, 2 loss kernels, 2 memsets; + sqnorm, sgd
     line = dict(metric=metric, value=value, unit='images/s', n_gpus=world, steps=args.steps, warmup=warmup, ms_per_step=ms_step, higher_is_better=True,
                 scaling='weak', vs_baseline=None, dtype=wl['dtype'], data='synthetic', config=config,
-                impl_detail=dict(timed_blocks=blocks, block_ms=[round(v, 3) for v in block_ms[:16]], timed_s=ms_total / 1e3, loss_first_last=[losses[0], losses[-1]],
+                impl_detail=dict(timed_s=ms_total / 1e3, loss_last_step=lv['loss'],
                                  cuda_graph=bool(model.use_cuda_graph_training), launches_per_step=launches,
                                  side_branch_ctas={k: {str(b): c for b, c in v['ctas'].items()} for k, v in tuned.items()},
                                  workspace_gb=plan.workspace_bytes / 1e9, parameters=int(flat.numel),
@@ -543,7 +539,7 @@ def train_main(args):
                                  label_assign_note='native lfd_assign_targets incl. the H2D copy of the boxes vs the oracle restatement of '
                                                    'annotation_to_target (lfd.py:109-259) on the host, same batch',
                                  allreduce_us=ar_us, allreduce_bytes=int(flat.numel * 4)),
-                clocks=clocks, gpu_launches=launches * args.steps * blocks,
+                clocks=clocks, gpu_launches=launches * args.steps,
                 e2e=dict(value=e2e_value, unit='images/s', h2d_bytes_per_step=N * H * W * 3 + ann_bytes, d2h_bytes_per_step=12, steps=e2e_steps,
                          host_numa_node=numa_node, note='pinned host uint8 crops -> device (prefetched on a copy stream) -> training step -> loss values on the host'),
                 roofline=roofline)
@@ -648,7 +644,8 @@ def main():
     ap.add_argument('--no-graph', action='store_true')
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-autotune', action='store_true', help='skip InferencePlan.autotune (CTA bounds of the side-branch convs)')
-    ap.add_argument('--min-timed-s', type=float, default=0.5, help='the K-step timed block is repeated until this much time has been timed')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help="after the timed steps, write what the last step computed as DIR/<name>.npy (float32 / float64, <= 64 MB in all)")
     ap.add_argument('--profile-ops', action='store_true', help='print the per-op timing table to stderr')
     ap.add_argument('--ncu-step', action='store_true',
                     help='for `ncu --profile-from-start off`: warm up, then ONE eager step between cudaProfilerStart/Stop, and exit')
@@ -720,7 +717,7 @@ def main():
     pipe = ForwardPostPipeline(model, plan, post, score_thr, IOU_THR)
 
     def step(i):
-        pipe.enqueue(pool[i % npool])
+        return pipe.enqueue(pool[i % npool])
 
     def sync_all():
         torch.cuda.synchronize()
@@ -746,45 +743,41 @@ def main():
         for i in range(npool):
             step(i)
         sync_all()
-        # size the number of timed blocks from a short probe so that >= min_timed_s are timed whatever --steps is
-        p0, p1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        p0.record(pipe.fwd_stream)
         for i in range(warmup):                # the W warm-up steps
             step(i)
-        p1.record(pipe.post_stream)
-        sync_all()
-        est_ms = max(p0.elapsed_time(p1) / warmup, 1e-3)
-        blocks = int(min(200, max(1, -(-args.min_timed_s * 1e3 // (est_ms * args.steps)))))
-        tb = torch.tensor([blocks], dtype=torch.int64, device=dev)
-        if world > 1:
-            dist.all_reduce(tb, op=dist.ReduceOp.MAX)   # every rank times the same number of blocks
-        blocks = int(tb.item())
         sampler = ClockSampler(local)
         if rank == 0:
             sampler.start()
-        block_ms = []
-        for b in range(blocks):                # every block: EXACTLY K steps between a barrier + synchronize on both sides
-            sync_all()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(pipe.fwd_stream)
-            for i in range(args.steps):
-                step(b * args.steps + i)
-            e1.record(pipe.post_stream)
-            sync_all()
-            block_ms.append(e0.elapsed_time(e1))
+        sync_all()                             # EXACTLY K timed steps between a barrier + synchronize on both sides
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(pipe.fwd_stream)
+        for i in range(args.steps):
+            results = step(i)
+        e1.record(pipe.post_stream)
+        sync_all()
         clocks = sampler.stop() if rank == 0 else None
         counts = post.count.tolist()
-    t = torch.tensor(block_ms, dtype=torch.float64, device=dev)
+        if args.dump_outputs and rank == 0:
+            # what a caller of the timed path receives for the last step: the raw head outputs of its batch and the detections
+            # (the kept rows of every image, in order); steps rotate over the pool, so the last one saw pool[(K - 1) % npool]
+            cls_last, reg_last = plan.outputs((pipe.k - 1) % pipe.n_slots)
+            dets, labels, _, count = results
+            n_keep = [int(c) for c in count[:N].tolist()]
+            dump_outputs(args.dump_outputs, dict(
+                cls=cls_last.float().cpu().numpy(), reg=reg_last.float().cpu().numpy(),
+                det_boxes_scores=np.concatenate([dets[b, :n_keep[b]].float().cpu().numpy() for b in range(N)]).reshape(-1, 5),
+                det_labels=np.concatenate([labels[b, :n_keep[b]].cpu().numpy() for b in range(N)]).astype(np.float64),
+                det_counts=np.asarray(n_keep, np.float64)))
+    t = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=dev)
     if world > 1:
-        dist.all_reduce(t, op=dist.ReduceOp.MAX)       # per block: the slowest rank
-    block_ms = [float(v) for v in t.tolist()]
-    ms_total = float(sum(block_ms))
-    ms_step = ms_total / (args.steps * blocks)
-    value = world * N * args.steps * blocks / (ms_total / 1e3)
+        dist.all_reduce(t, op=dist.ReduceOp.MAX)       # the slowest rank
+    ms_total = float(t.item())
+    ms_step = ms_total / args.steps
+    value = world * N * args.steps / (ms_total / 1e3)
 
     # ---- end to end: pinned host frames in, host detections out, copies inside the timed region
     det = StreamingDetector(model, N, H, W, score_thr, IOU_THR, max_out=1024, device=dev)
-    e2e_steps = args.steps * blocks
+    e2e_steps = args.steps
     with torch.no_grad():
         for i in range(3):
             det.infer(host_pool[i % 2])
@@ -865,7 +858,6 @@ def main():
         dir_bound_ms += r['t_dir_ms']
     kname = op_name(top['row'])
     roofline = dict(bound='hbm' if hbm_bound else 'tensor', achieved=achieved, peak=peak, unit=unit, frac=achieved / peak,
-                    traffic=ncu_traffic(args.config, dtype, kname),
                     peak_source=pk['source'],
                     kernel=kname,
                     kernel_ms=top['ms'], kernel_share_of_step=top['ms'] / sum_ms, algorithmic_bytes=top['bytes'], algorithmic_flops=top['flops'],
@@ -894,7 +886,7 @@ def main():
                 higher_is_better=True, scaling='weak', vs_baseline=None, dtype=dtype, data='synthetic',
                 config=config,
                 impl_detail=dict(score_thr=score_thr, detections_last_step=counts[:N],
-                                 timed_blocks=blocks, block_ms=[round(v, 4) for v in block_ms[:16]], timed_s=ms_total / 1e3,
+                                 timed_s=ms_total / 1e3,
                                  setup_steps=2 * npool + 1,
                                  l2='inputs rotate over a %d-batch pool (%.0f MB > L2); the %.0f MB activation workspace is rewritten every step'
                                     % (npool, npool * N * H * W * 3 / 1e6, plan.workspace_bytes / 1e6),
@@ -902,7 +894,7 @@ def main():
                                  side_branch_ctas={str(b): c for b, c in plan.side_ctas.items()},
                                  autotune=[(k, round(v, 4)) for k, v in getattr(plan, 'autotune_log', [])],
                                  pipelining='post-process of batch i overlaps the forward of batch i+1 (two streams, two output slots)'),
-                clocks=clocks, gpu_launches=(plan.num_launches + 2) * args.steps * blocks,
+                clocks=clocks, gpu_launches=(plan.num_launches + 2) * args.steps,
                 e2e=dict(value=e2e_value, unit='images/s', h2d_bytes_per_step=det.h2d_bytes, d2h_bytes_per_step=det.d2h_bytes, steps=e2e_steps,
                          h2d_copy_alone_ms=h2d_ms, h2d_gbps=det.h2d_bytes / (h2d_ms * 1e-3) / 1e9, h2d_gbps_per_rank=h2d_per_rank,
                          copy_streams=len(det.copy_streams), host_numa_node=numa_node, host_submit_ms_per_step=host_submit_s / e2e_steps * 1e3,

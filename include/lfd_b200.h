@@ -1,11 +1,11 @@
-/* lfd_b200.h -- C-ABI of liblfd_b200.so: the B200 (sm_100a) implementation of the LFD dense-conv hot path.
+/* lfd_b200.h -- C-ABI of liblfd_b200.so: the H100 (sm_90a) implementation of the LFD dense-conv hot path.
  *
  * Conventions
  *   - plain C: raw device pointers, explicit shapes, a cudaStream_t passed as void*; no torch / C++ types.
  *   - nothing is allocated inside: the caller supplies outputs and workspaces (sizes via the *_bytes queries).
  *   - every function returns 0 (LFD_OK) or an lfd_status; lfd_last_error() gives a thread-local message.
  *     No exceptions cross the boundary.  Calls are asynchronous on the given stream unless stated otherwise.
- *   - there is no CPU fallback: every entry point launches CUDA kernels and fails if no sm_100 device is present.
+ *   - there is no CPU fallback: every entry point launches CUDA kernels and fails if no sm_90 device is present.
  *
  * Reference interfaces replaced (paths relative to the reference repository root):
  *   lfd_plan_*                     LFD.forward                         lfd/model/lfd.py:511-542
@@ -69,7 +69,7 @@ enum { LFD_DTYPE_BF16 = 0, LFD_DTYPE_FP16 = 1 };
  *   STEM0      3x3/s2 conv on the 3-channel image + shift (+ReLU), scale folded into the weights like CONV; in_off ignored (reads the external input);
  *              weight = bf16 packed [kh][2][Cout][8]: element (kh, kc, n, j) = weight of output n, input channel j % 4, filter
  *              column kw = 2*kc + j/4 (zero for kw = 3 and for the padded 4th channel): the kernel keeps the image patch as
- *              4-channel bf16 pixels and lets the UMMA address generator do the im2col (K = 16 per filter row).
+ *              4-channel bf16 pixels and lets the wgmma address generator do the im2col (K = 16 per filter row).
  *   CONV       ksize in {1,3}, stride in {1,2}, pad = ksize/2; y = conv(x) + shift (+res) (ReLU) -> bf16;
  *              weight = bf16 packed [Cin/cc][ksize^2][cc/8][Cout][8] with cc from lfd_conv_query, ALREADY MULTIPLIED by the
  *              per-output-channel scale (folded BatchNorm); `scale` must be NULL; `shift` (fp32 [Cout], may be NULL) is rounded
@@ -119,7 +119,7 @@ typedef struct lfd_op {
     const float* ds_shift;
 } lfd_op;
 
-/* Tile / pipeline configuration the tcgen05 kernel will use for a conv (host only, no launch).
+/* Tile / pipeline configuration the wgmma kernel will use for a conv (host only, no launch).
  * cc = input-channel chunk the weights must be packed with. */
 int lfd_conv_query(int N, int H, int W, int Cin, int Ho, int Wo, int Cout, int ksize, int stride, int tail_cout, int ds_cout, int* cc,
                    int* stages, int* weights_resident, int* num_tiles, int64_t* smem_bytes);
@@ -137,7 +137,7 @@ int lfd_plan_forward(lfd_plan* plan, const void* input, int input_format, void* 
  * Synchronises the stream.  Used by bench.py for the live per-kernel roofline. */
 int lfd_plan_profile(lfd_plan* plan, const void* input, int input_format, void* workspace, float* cls_out, float* reg_out,
                      float* ms_per_op, lfd_stream stream);
-/* Debugging aid: device buffer long long[4][32][4] that CTA 0 of every following tcgen05 conv launch fills with a
+/* Debugging aid: device buffer long long[4][32][4] that CTA 0 of every following wgmma conv launch fills with a
  * clock64() timeline (role 0 producer / 1 MMA issuer / 2 epilogue, per tile); NULL switches it off. */
 int lfd_debug_set_trace(void* device_buffer);
 /* Debugging aid (LFD_B200_TIMELINE builds): device buffer unsigned long long[2 * lfd_plan_num_launches()], pre-set by the caller

@@ -42,7 +42,7 @@ static int sm_count() {   // of the CURRENT device (cached per device ordinal)
 
 struct PlannedOp {
     lfd_op op;
-    UmmaConvParams cp;  // CONV via tcgen05
+    UmmaConvParams cp;  // CONV via wgmma
     size_t smem;
     int grid;
 };
@@ -125,8 +125,8 @@ extern "C" int lfd_conv_query(int N, int H, int W, int Cin, int Ho, int Wo, int 
     UmmaConvParams p;
     size_t smem = 0;
     int grid = 0;
-    int rc = umma_conv_configure(g, 148, &p, &smem, &grid);
-    if (rc) return fail(LFD_ERR_UNSUPPORTED, "conv %dx%d s%d Cin=%d Cout=%d not supported by the tcgen05 kernel (rc=%d)", ksize, ksize, stride, Cin, Cout, rc);
+    int rc = umma_conv_configure(g, 132, &p, &smem, &grid);
+    if (rc) return fail(LFD_ERR_UNSUPPORTED, "conv %dx%d s%d Cin=%d Cout=%d not supported by the wgmma kernel (rc=%d)", ksize, ksize, stride, Cin, Cout, rc);
     if (cc) *cc = p.Cc;
     if (stages) *stages = p.stages;
     if (weights_resident) *weights_resident = p.b_resident;
@@ -167,7 +167,7 @@ static int check_op(const lfd_op& o) {
 
 // GN_APPLY / HEAD_FINAL size their grids from the SM count: a max_ctas bound (side-branch layers, see lfd_op) scales them the same way
 static int bounded_sms(int max_ctas) {
-    const int sms = sm_count() > 0 ? sm_count() : 148;
+    const int sms = sm_count() > 0 ? sm_count() : 132;
     return max_ctas > 0 && max_ctas < sms ? max_ctas : sms;
 }
 
@@ -178,7 +178,7 @@ static int plan_op(const lfd_op& o, int conv_impl, PlannedOp* out) {
     out->smem = 0;
     out->grid = 0;
     if (o.kind == LFD_OP_CONV || o.kind == LFD_OP_STEM0) {
-        rc = umma_conv_configure(geom_of(o), sm_count() > 0 ? sm_count() : 148, &out->cp, &out->smem, &out->grid);
+        rc = umma_conv_configure(geom_of(o), sm_count() > 0 ? sm_count() : 132, &out->cp, &out->smem, &out->grid);
         if (rc) return fail(LFD_ERR_UNSUPPORTED, "conv %dx%d s%d Cin=%d Cout=%d unsupported (rc=%d)", o.ksize, o.ksize, o.stride, o.Cin, o.Cout, rc);
         if (o.kind == LFD_OP_CONV && out->cp.Cc != o.cc) return fail(LFD_ERR_INVALID, "weights packed with cc=%d but the kernel needs cc=%d", o.cc, out->cp.Cc);
         if (o.max_ctas < 0) return fail(LFD_ERR_INVALID, "max_ctas = %d", o.max_ctas);
@@ -658,7 +658,7 @@ extern "C" int lfd_sigmoid_focal_loss_backward(const float* logits, const int64_
 // ------------------------------------------------------------------------------------------------ training plan
 struct PlannedTop {
     lfd_top op;
-    PlannedOp conv;   // STEM0 / CONV: the tcgen05 configuration (same kernels as the inference plan)
+    PlannedOp conv;   // STEM0 / CONV: the wgmma configuration (same kernels as the inference plan)
 };
 
 struct lfd_train_plan {
@@ -701,7 +701,7 @@ static int plan_top(const lfd_top& t, int64_t ws_bytes, PlannedTop* out) {
         case LFD_TOP_WGRAD: {
             WgradGeom g = {t.N, t.H, t.W, t.Cin, t.Ho, t.Wo, t.Cout, t.ksize, t.stride};
             if (t.impl == LFD_WGRAD_UMMA && !wgrad_umma_supported(g))
-                return fail(LFD_ERR_UNSUPPORTED, "wgrad %dx%d s%d Cin=%d Cout=%d unsupported by the tcgen05 kernel", t.ksize, t.ksize, t.stride, t.Cin, t.Cout);
+                return fail(LFD_ERR_UNSUPPORTED, "wgrad %dx%d s%d Cin=%d Cout=%d unsupported by the wgmma kernel", t.ksize, t.ksize, t.stride, t.Cin, t.Cout);
             break;
         }
         case LFD_TOP_PACK: case LFD_TOP_UNPACK:

@@ -13,10 +13,10 @@ enum { MODE_FLAT = 0, MODE_3X3S1 = 1, MODE_3X3S2 = 2, MODE_1X1S2 = 3, MODE_STEM 
 static constexpr int kMaxStages = 8;
 static constexpr int kMaxDevices = 64;   // per-device state (function attributes, SM counts) is indexed by the device ordinal
 // dynamic shared memory map of conv_umma_kernel (bytes)
-static constexpr int kSmemBarOff = 0;        // mbarriers + TMEM slot
-static constexpr int kSmemOnesOff = 512;      // constant A operand [2 k-chunks][128 rows][16 B]: column 0 = 1, everything else 0
-// behind it, at offsets chosen per layer (UmmaConvParams::smem_*_off): halo pixel table (modes that need it), the bias B
-// operands [2][Cout][16 B] of the conv and of the fused tail, then the 1024-byte aligned staging regions [warp][buffer]
+static constexpr int kSmemBarOff = 0;        // mbarriers
+static constexpr int kSmemTableOff = 512;    // first per-layer region
+// from there, at offsets chosen per layer (UmmaConvParams::smem_*_off): halo pixel table (modes that need it), the fp32 shifts
+// of the conv and of the fused tail, then the 1024-byte aligned staging regions [warpgroup][buffer]
 
 struct ConvGeom {
     int N, H, W, Cin, Ho, Wo, Cout, ksize, stride;
@@ -29,13 +29,13 @@ struct alignas(64) UmmaConvParams {
     CUtensorMap tm_out;         // TMA descriptor of the stored tensor (epilogue tile store)
     CUtensorMap tm_res;         // TMA descriptor of the residual tensor (same geometry)
     CUtensorMap tm_out3;        // TMA descriptor of the fused shortcut conv's output (same geometry)
-    int stg_nbuf;               // staging buffers per epilogue warp (2: the store of tile t overlaps the conversion of tile t+1)
+    int stg_nbuf;               // staging buffers per warpgroup (2: the store of tile t overlaps the conversion of tile t+1)
     const __nv_bfloat16* in;
     __nv_bfloat16* out;
     const void* in_raw;         // MODE_STEM: the image, fp32 NCHW (input_format 0) or uint8 NHWC (1)
     const __nv_bfloat16* res;   // optional residual (same shape as out)
     const __nv_bfloat16* w;     // packed [cc][tap][kc][Cout][8]
-    const float* shift;         // [Cout] fp32 or null; added on the tensor core as bf16 (BatchNorm scale is folded into w)
+    const float* shift;         // [Cout] fp32 or null; rounded to the 16-bit type and added to the accumulator (BatchNorm scale is folded into w)
     // fused trailing 1x1 conv ("tail"): out = act2(scale2 * (W2 . act(scale * conv(x) + shift)) + shift2); `out`, `res`,
     // `stats` then refer to the tail's output (Cf channels) and the intermediate never leaves the SM
     const __nv_bfloat16* w2;    // packed [Cout/8][Cout2][8]
@@ -44,7 +44,7 @@ struct alignas(64) UmmaConvParams {
     // fused 1x1/s2 shortcut conv (MODE_3X3S2, no tail): out3 = W3 . x[centre tap] + shift3; its weights / shift travel in w2 / shift2
     int Cout3;
     __nv_bfloat16* out3;
-    uint32_t smem_w2_off, smem_a2_off, a2_bytes, n_a2;
+    uint32_t smem_w2_off;
     double* stats;              // optional [N][groups][2] (sum, sumsq) of the stored output
     unsigned long long* tl;     // debugging: [start, end] of the launch in %globaltimer ns (LFD_B200_TIMELINE builds), normally null
     long long* trace;           // debugging: clock64() timeline of CTA 0 ([role 0..2][tile < 32][4]), normally null
@@ -54,16 +54,16 @@ struct alignas(64) UmmaConvParams {
     unsigned long long magic_tpi, magic_tx;   // ceil(2^40 / d) for division-free tile decomposition
     int n_px;                   // halo pixels loaded per stage
     int Cc, stages, b_resident;
-    int log2_cpc, log2_cpr, log2_rp128, tmem_cols, ctas_per_sm;
+    int log2_cpc, log2_cpr;
     uint32_t lbo_a, sbo_a;
     uint32_t a_stage_bytes, b_slice_bytes, stage_bytes, w_total_bytes;
     uint32_t smem_table_off, smem_bias_off, smem_bias2_off, smem_staging_off;
     uint32_t smem_w_off, smem_ring_off;
     int input_format;
-    int f16;                    // activation / weight type: 0 = bf16, 1 = IEEE fp16 (same bytes, kind::f16 either way)
+    int f16;                    // activation / weight type: 0 = bf16, 1 = IEEE fp16 (same bytes, same tensor-core rate)
 };
 
-// returns 0 when the geometry is supported by the tcgen05 kernel
+// returns 0 when the geometry is supported by the wgmma kernel
 int umma_conv_configure(const ConvGeom& g, int num_sms, UmmaConvParams* out, size_t* smem_bytes, int* grid);
 cudaError_t umma_conv_launch(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st);
 // fills p->tm_out / p->tm_res from p->out / p->res (host, no launch); returns 0 on success

@@ -1,5 +1,5 @@
 // conv_simt.cu -- the bandwidth-bound / narrow kernels of the LFD forward that are not GEMM shaped, plus a
-// SIMT cross-check of the tcgen05 convolution:
+// SIMT cross-check of the wgmma convolution:
 //   stem0_kernel       3x3 stride-2 conv on the 3-channel image (K = 27): direct, fused BN scale/shift + ReLU,
 //                      reads fp32 NCHW (reference `forward(x)` input) or uint8 HWC BGR with the
 //                      (x/255-0.5)/0.5 normalisation fused (reference predict path,
@@ -303,7 +303,7 @@ cudaError_t head_final_launch(const HeadFinalParams& p, int num_sms, cudaStream_
     }
     if (smem > 64 * 1024) return cudaErrorInvalidValue;
     const int tiles = (p.HW + kHfPixPerBlock - 1) / kHfPixPerBlock;
-    int bx = (4 * num_sms + p.N - 1) / p.N;              // about four blocks per SM over all images (201 registers: two resident, two queued; 1 / 2 / 4 per SM measured alike)
+    int bx = (4 * num_sms + p.N - 1) / p.N;              // about four blocks per SM over all images
     if (bx > tiles) bx = tiles;
     const dim3 grid(bx < 1 ? 1 : bx, p.N);
     if (p.f16) head_final_kernel<true><<<grid, kHfThreads, smem, st>>>(p);
@@ -376,7 +376,7 @@ cudaError_t simt_conv_launch(const ConvGeom& g, int Cc, const __nv_bfloat16* in,
                              int relu, int f16, cudaStream_t st) {
     const size_t total = (size_t)g.N * g.Ho * g.Wo * (g.Cout >> 3);
     size_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     if (blocks < 1) blocks = 1;
     simt_conv_kernel<<<(int)blocks, 256, 0, st>>>(g, Cc, in, out, res, w, shift, stats, gn_groups, relu, f16);
     return cudaGetLastError();

@@ -1,37 +1,37 @@
-// conv_umma.cu -- implicit-GEMM convolution on 5th-gen tensor cores (tcgen05 / TMEM), sm_100a only.
+// conv_umma.cu -- implicit-GEMM convolution on Hopper tensor cores (wgmma), sm_90a.
 //
 // Replaces, for the LFD hot path, every nn.Conv2d(+BatchNorm2d)(+residual)(+ReLU) of the reference's
 // backbone / neck / head towers (lfd/model/backbone/lfd_resnet.py:96-154,354-473,
 // lfd/model/neck/simple_neck.py:35-47, lfd/model/head/lfd_head.py:85-135), which the reference runs
 // as separate cuDNN / ATen kernels in NCHW fp32.
 //
-// Formulation (NHWC bf16 activations, fp32 accumulate in TMEM):
+// Formulation (NHWC bf16 activations, fp32 accumulate in registers):
 //   D[128 output pixels, Cout] = sum over taps (kh,kw) and channel chunks of  A_tap[128, 16] * W_tap[16, Cout]
-//   * persistent CTAs (1 per SM for 3x3, 2 per SM for the 1x1 layers and the stem), warp-specialised:
-//       warps 0..E-1  epilogue   : TMEM -> regs -> (+residual) (+ReLU) -> bf16 -> the warp's own staging rows -> the warp's
-//                                  own TMA tensor store (+ optional GroupNorm partial statistics of the stored tensor);
-//                                  E = 4 (one warp per TMEM lane quarter) or 8 (two warps per quarter, each half the columns)
-//       warp  E       MMA issuer : one lane issues tcgen05.mma with pre-built descriptors, commits to mbarriers
-//       warps E+1..   producers  : cp.async (16 B, zero-fill = conv padding) of the input halo tile into the A ring;
-//                                  completion is signalled by cp.async.mbarrier.arrive (no thread waits on its own copies)
-//   * BatchNorm is folded on the host: scale into the bf16 weights, shift into one extra K=16 MMA against a constant
-//     "ones" operand, so the accumulator already holds scale * conv + shift.
+//   * persistent CTAs (one per SM), warp-specialised:
+//       warpgroups 0, 1  consumers : rows 0..63 / 64..127 of the tile; wgmma.mma_async (m64 x Cout x k16) with pre-built
+//                                    descriptors into register accumulators, then the epilogue from the same registers:
+//                                    (+shift) (+residual) (+ReLU) -> bf16 -> the warpgroup's own staging rows -> its own TMA
+//                                    tensor store (+ optional GroupNorm partial statistics of the stored tensor)
+//       warps 8..11      producers : cp.async (16 B, zero-fill = conv padding) of the input halo tile into the A ring;
+//                                    completion is signalled by cp.async.mbarrier.arrive (no thread waits on its own copies)
+//   * BatchNorm is folded on the host: scale into the bf16 weights; the shift, rounded to the 16-bit type, is added to the
+//     fp32 accumulator in the epilogue.
 //   * the input halo tile is loaded ONCE per (tile, channel-chunk) into "pixel planes"
 //       plane[k-chunk][pixel][8 channels = 16 B]
-//     which is exactly the UMMA K-major / no-swizzle canonical layout (8-row core matrices of 16 B rows,
+//     which is exactly the wgmma K-major / no-swizzle canonical layout (8-row core matrices of 16 B rows,
 //     SBO between 8-row groups, LBO between 16-byte K chunks).  A 3x3 tap is then just a *shifted view*
 //     (start address += tap offset, SBO = halo row pitch), so the 9 taps re-read shared memory, never L2.
 //     Stride-2 convolutions de-interleave the halo into 4 row/column parity planes so that every tap is
 //     again a unit-stride view.  The plane pitch (LBO) is an ODD multiple of 16 B so that the 8 channel
 //     chunks of one pixel land in 8 different bank groups (conflict-free cp.async writes).
 //   * MODE_STEM: the 3-channel stem conv's im2col is done by the same address generator (see kStem* below).
-//   * optional second GEMM in the same launch: a trailing 1x1 conv fed from shared memory ("tail": stem0->stem1,
-//     stem2->stem3), or the residual block's 1x1/s2 shortcut conv on the centre tap (MODE_3X3S2, second output tensor).
+//   * optional second GEMM in the same launch: a trailing 1x1 conv whose A operand is the first accumulator, rounded to
+//     16 bits, straight from registers ("tail": stem0->stem1, stem2->stem3), or the residual block's 1x1/s2 shortcut conv on
+//     the centre tap (MODE_3X3S2, second output tensor).
 //   * weights: pre-packed on the host in [channel-chunk][tap][k-chunk][Cout][8] order and brought in by
-//     the TMA engine as 1-D bulk copies (cp.async.bulk -> UBLKCP), either once (resident) or per stage
+//     the TMA engine as 1-D bulk copies (cp.async.bulk), either once (resident) or per stage
 //     (streamed, for 3x3x128x128 which does not fit next to the A ring).
-//   * two TMEM accumulator stages so the epilogue of tile i overlaps the MMAs of tile i+1.
-//   * programmatic dependent launch: the prologue (barriers, TMEM allocation, weight fetch) overlaps the previous layer.
+//   * programmatic dependent launch: the prologue (barriers, weight fetch) overlaps the previous layer.
 #include <stdlib.h>
 
 #include "conv_common.cuh"
@@ -40,17 +40,11 @@
 namespace lfd {
 
 static constexpr int kProdThreads = 128;
-// The 3x3/s2 layers are bound by the issue latency of the halo copies (561 pixels x Cc/8 scattered 16-byte cp.async per stage, each behind a
-// shared-memory table read).  Measured (profiles/r02_tuning_notes.md): 128 / 192 / 256 producer threads give 0.109 / 0.107 / 0.106 ms for the
-// 64->64 @180x320 layer -- the layer is NOT issue-bound but bound by 64-byte (half-line) segment fetches; four warps stay the default.
-#ifndef LFD_B200_S2_PROD
-#define LFD_B200_S2_PROD 128
-#endif
-template <int MODE> struct ProdThreads { static constexpr int value = (MODE == MODE_3X3S2) ? LFD_B200_S2_PROD : kProdThreads; };
+static constexpr int kConsumerThreads = 256;                        // two warpgroups
+static constexpr int kConvThreads = kConsumerThreads + kProdThreads;
 
-// The role bodies are lambdas that capture ~30 locals by reference.  If the compiler decides NOT to inline one of them (it did,
-// as soon as a lambda had three call sites or a second instantiation of the template existed) the closure is materialised in
-// local memory and the kernel runs 2-3x slower (a 230-byte stack frame in ptxas -v is the symptom).  Force it.
+// The role bodies are lambdas that capture many locals by reference.  If the compiler decides NOT to inline one of them the
+// closure is materialised in local memory and the kernel runs 2-3x slower (a large stack frame in ptxas -v is the symptom).  Force it.
 #define LFD_LAMBDA_INLINE __attribute__((always_inline))
 
 // clock64() timeline of CTA 0 (tests/debug_trace.py); compiled in only with -DLFD_B200_TRACE (LFD_B200_TRACE=1 python build.py)
@@ -70,7 +64,7 @@ struct PxEntry {  // one halo pixel: where it comes from and where it goes
 };
 struct PxDelta { int8_t dy, dx; };  // the same pixel relative to the tile's input origin, for tiles that touch the border
 
-// MODE_STEM: the im2col of the 3-channel stem conv is done by the UMMA address generator.  The producers write the raw-image
+// MODE_STEM: the im2col of the 3-channel stem conv is done by the wgmma address generator.  The producers write the raw-image
 // patch of one 16x8 output tile (33 rows x 18 pixels) to shared memory as bf16 with the channels padded to 4
 // ([row][pixel][b g r 0] = 8 B per pixel, already normalised / rounded = rounding point R0).  Output pixel (oy, ox) and filter row
 // kh need the 3 input pixels 2ox-1 .. 2ox+1 of input row 2oy+kh-1 = 12 of the 16 consecutive bf16 values that start at patch
@@ -84,54 +78,29 @@ static constexpr int kStemRowBytes = kStemCols * 8;                             
 static constexpr int kStemPerThread = (kStemPix + kProdThreads - 1) / kProdThreads;             // 5
 static constexpr int kStemPatchBytes = ((kStemRows * kStemRowBytes + 127) / 128) * 128;         // 4864
 
-// pitch (bytes) between the 16-byte channel chunks of the fused tail's A operand [chunk][128 rows + 1][16 B]
-static constexpr uint32_t kA2Pitch = 129 * 16;
-
-// 8 accumulator columns (+ 8 residual values) -> packed bf16; ReLU is fused into the conversion (cvt.rn.relu)
-template <bool RELU, bool F16>
-LFD_DEVINL uint4 pack8(const float* v) {
-    uint4 o;
-    if (RELU) { o.x = pack2_relu<F16>(v[0], v[1]); o.y = pack2_relu<F16>(v[2], v[3]); o.z = pack2_relu<F16>(v[4], v[5]); o.w = pack2_relu<F16>(v[6], v[7]); }
-    else { o.x = pack2<F16>(v[0], v[1]); o.y = pack2<F16>(v[2], v[3]); o.z = pack2<F16>(v[4], v[5]); o.w = pack2<F16>(v[6], v[7]); }
-    return o;
-}
-template <bool RELU, bool F16>
-LFD_DEVINL uint4 pack8_res(const float* v, uint4 rv) {
-    float o[8] = {v[0] + up_lo<F16>(rv.x), v[1] + up_hi<F16>(rv.x), v[2] + up_lo<F16>(rv.y), v[3] + up_hi<F16>(rv.y),
-                  v[4] + up_lo<F16>(rv.z), v[5] + up_hi<F16>(rv.z), v[6] + up_lo<F16>(rv.w), v[7] + up_hi<F16>(rv.w)};
-    return pack8<RELU, F16>(o);
+// c ? a : b as one selp: the compiler would otherwise select between the two ADDRESSES of an array element in warp_multi_reduce,
+// which sends the array to local memory
+LFD_DEVINL float selp_f32(bool c, float a, float b) {
+    float r;
+    asm("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %3, 0;\n\tselp.f32 %0, %1, %2, p;\n\t}" : "=f"(r) : "f"(a), "f"(b), "r"((uint32_t)c));
+    return r;
 }
 
-// Epilogue inner loop of one warp: NC accumulator columns of its TMEM lane quarter (row = lane) -> (+residual) (+ReLU) -> bf16
-// -> shared memory, fully unrolled so that every address is `base` plus / xor a literal.
-//   OPERAND = false: staging row in TMA swizzle layout, chunk k (8 channels, 16 B) at (base ^ ((k & 7) << 4)) + (k >> 3) * 4096;
-//                    RES adds the residual chunk found at the same place (TMA-loaded before), STATS accumulates the sum and
-//                    the sum of squares of the stored values per chunk into st[k] / st[NC/8 + k] (rows with !valid count 0)
-//   OPERAND = true : K-major A operand of the fused tail, chunk k at base + k * kA2Pitch
-template <int NC, bool RELU, bool RES, bool STATS, bool OPERAND, int MAXB, bool F16>
-LFD_DEVINL void drain(uint32_t taddr, uint32_t base, bool valid, float* st) {
-    constexpr int BATCH = NC < MAXB ? NC : MAXB;   // columns in flight per tcgen05.wait::ld
+// One step of the transposing butterfly of warp_multi_reduce: N live values -> N / 2 (compile-time recursion keeps every array
+// index a constant, so the values stay in registers)
+template <int NV, int N>
+LFD_DEVINL void butterfly_step(float* val, int lane) {
+    if constexpr (N > 1) {
+        constexpr int off = 16 * N / NV;
+        const bool upper = (lane & off) != 0;
 #pragma unroll
-    for (int c0 = 0; c0 < NC; c0 += BATCH) {
-        float v[BATCH];
-#pragma unroll
-        for (int j = 0; j < BATCH; j += 16) tmem_ld16(taddr + c0 + j, v + j);
-        tmem_ld_wait();
-#pragma unroll
-        for (int h = 0; h < BATCH / 8; ++h) {
-            const int k = (c0 >> 3) + h;
-            const uint32_t addr = OPERAND ? base + k * kA2Pitch : (base ^ (uint32_t)((k & 7) << 4)) + (uint32_t)(k >> 3) * 4096u;
-            const uint4 o = RES ? pack8_res<RELU, F16>(v + h * 8, lds128(addr)) : pack8<RELU, F16>(v + h * 8);
-            sts128(addr, o);
-            if (STATS) {
-                const float f[8] = {up_lo<F16>(o.x), up_hi<F16>(o.x), up_lo<F16>(o.y), up_hi<F16>(o.y), up_lo<F16>(o.z), up_hi<F16>(o.z), up_lo<F16>(o.w), up_hi<F16>(o.w)};
-                float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) { s1 += f[j]; s2 = fmaf(f[j], f[j], s2); }
-                st[k] = valid ? s1 : 0.f;
-                st[NC / 8 + k] = valid ? s2 : 0.f;
-            }
+        for (int i = 0; i < N / 2; ++i) {
+            const float lo = val[i], hi = val[i + N / 2];
+            const float send = selp_f32(upper, lo, hi);
+            const float keep = selp_f32(upper, hi, lo);
+            val[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
         }
+        butterfly_step<NV, N / 2>(val, lane);
     }
 }
 
@@ -139,17 +108,7 @@ LFD_DEVINL void drain(uint32_t taddr, uint32_t base, bool valid, float* st) {
 // halves the number of live values).  Returns, in every lane, the total of value index (lane * NV / 32).
 template <int NV>
 LFD_DEVINL float warp_multi_reduce(float* val, int lane) {
-    int off = 16;
-#pragma unroll
-    for (int n = NV; n > 1; n >>= 1, off >>= 1) {
-        const bool upper = (lane & off) != 0;
-#pragma unroll
-        for (int i = 0; i < n / 2; ++i) {
-            const float send = upper ? val[i] : val[i + n / 2];
-            const float keep = upper ? val[i + n / 2] : val[i];
-            val[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-        }
-    }
+    butterfly_step<NV, NV>(val, lane);
     float r = val[0];
 #pragma unroll
     for (int o = 16 / NV; o >= 1; o >>= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
@@ -158,7 +117,7 @@ LFD_DEVINL float warp_multi_reduce(float* val, int lane) {
 
 // GroupNorm partial statistics of one warp's NC stored channels: st = [sum per 8-channel chunk | sum of squares per chunk]
 template <int NC>
-LFD_DEVINL void stats_flush(float* st, int lane, double* dst) {   // dst: (sum, sumsq) pair of the warp's first group
+LFD_DEVINL void stats_flush(float* st, int lane, double* dst) {   // dst: (sum, sumsq) pair of the first group
     constexpr int NV = NC / 4, PER = 32 / NV, G = NV / 2;
     const float r = warp_multi_reduce<NV>(st, lane);
     if ((lane & (PER - 1)) == 0) {
@@ -178,34 +137,105 @@ __device__ __forceinline__ constexpr int tap_view(int tap) {  // pixel offset of
     return 0;
 }
 
-template <int MODE, int EPI_WARPS, bool F16>
-__global__ void __launch_bounds__(EPI_WARPS * 32 + 32 + ProdThreads<MODE>::value, (EPI_WARPS == 4 ? 2 : 1))
-conv_umma_kernel(const __grid_constant__ UmmaConvParams p) {
-    constexpr int kEpiThreads = EPI_WARPS * 32;
-    constexpr int kMmaWarp = EPI_WARPS;
-    constexpr int kProd = ProdThreads<MODE>::value;     // producer threads of this instantiation (the stem code below assumes kProdThreads)
-    constexpr int kThreads = kEpiThreads + 32 + kProd;
+LFD_DEVINL void wg_bar_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }   // the 128 threads of warpgroup wg
+
+// Where the epilogue of one warpgroup writes and what it stores
+struct EpiCtx {
+    uint32_t stg;          // this warpgroup's staging region: [buffer][64 rows x Cf x 2 B]
+    uint32_t stg_bytes;    // bytes of one staging buffer
+    int nbuf;
+    int r0, tq;            // this thread's first row (second: r0 + 8) within the warpgroup's 64, column pair index (lane % 4)
+    int wtid;              // thread index within the warpgroup
+    int wg, lane;
+};
+
+// Register accumulators (rows r0 / r0 + 8, NC <= NCMAX columns) (+shift) (+residual) (+ReLU) -> 16-bit staging rows in the TMA swizzle
+// layout -> one TMA tensor store per 64-channel panel (+ GroupNorm partial statistics of the stored values, NC == 128 only).
+// Staging rows are laid out the way the TMA engine expects for its swizzle modes: 128-byte panels [panel][64 rows][128 B] with the
+// 16-byte chunk index XORed by (row & 7) (SWIZZLE_128B); 64 / 32-byte rows use the 64B / 32B patterns.
+template <int MODE, int NCMAX, bool F16>
+LFD_DEVINL void store_tile(const EpiCtx& e, const float* acc, int nc, const float* bias, bool relu, bool res, double* stats,
+                           const CUtensorMap* tmap, const CUtensorMap* tmres, int c0, int c1, int n, bool v0, bool v1,
+                           uint64_t* res_bar, uint32_t& store_count, uint32_t& res_count) {
+    const uint32_t buf = e.stg + (e.nbuf == 2 ? (store_count & 1) * e.stg_bytes : 0u);
+    ++store_count;
+    const int row_bytes = nc >= 64 ? 128 : nc * 2;
+    const int n_panels = nc >= 64 ? nc / 64 : 1;
+    if (e.wtid == 0) {
+        // this staging buffer was the source of an earlier store: the TMA engine must be done reading it
+        if (e.nbuf == 2) bulk_wait_read<1>(); else bulk_wait_read<0>();
+        if (res) {   // residual rows -> staging (out-of-map rows / columns arrive as zeros), added in place below
+            mbar_arrive_expect_tx(res_bar, 64u * nc * 2u);
+            for (int pn = 0; pn < n_panels; ++pn) {
+                if (MODE == MODE_FLAT) tma_load_3d(buf + pn * 8192, tmres, pn * 64, c0, n, res_bar);
+                else tma_load_4d(buf + pn * 8192, tmres, pn * 64, c0, c1, n, res_bar);
+            }
+        }
+    }
+    wg_bar_sync(e.wg);
+    if (res) { mbar_wait(res_bar, res_count & 1); ++res_count; }
+    float st[NCMAX == 128 ? 32 : 1];
+    const bool stat = NCMAX == 128 && stats != nullptr;
+#pragma unroll
+    for (int j = 0; j < NCMAX / 8; ++j) {
+        if (j < nc / 8) {
+            const int c = 8 * j + 2 * e.tq;
+            const float b0 = bias[c], b1 = bias[c + 1];
+            float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = e.r0 + 8 * h;
+                const uint32_t swz = row_bytes == 128 ? (row & 7) : (row_bytes == 64 ? ((row >> 1) & 3) : ((row >> 2) & 1));
+                const uint32_t addr = buf + (uint32_t)(j >> 3) * 8192u + (uint32_t)(row * row_bytes) + ((((uint32_t)j & 7u) ^ swz) << 4) + 4u * e.tq;
+                float x0 = acc[4 * j + 2 * h] + b0, x1 = acc[4 * j + 2 * h + 1] + b1;
+                if (res) {
+                    uint32_t rv;
+                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(rv) : "r"(addr) : "memory");
+                    x0 += up_lo<F16>(rv); x1 += up_hi<F16>(rv);
+                }
+                const uint32_t o = relu ? pack2_relu<F16>(x0, x1) : pack2<F16>(x0, x1);
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(o) : "memory");
+                if (stat && (h ? v1 : v0)) {
+                    const float f0 = up_lo<F16>(o), f1 = up_hi<F16>(o);
+                    s1 += f0 + f1;
+                    s2 = fmaf(f0, f0, fmaf(f1, f1, s2));
+                }
+            }
+            if (NCMAX == 128) { st[j] = s1; st[16 + j] = s2; }
+        }
+    }
+    fence_proxy_async_smem();             // st.shared (generic proxy) -> TMA store (async proxy)
+    wg_bar_sync(e.wg);
+    if (e.wtid == 0) {
+        for (int pn = 0; pn < n_panels; ++pn) {   // rows / columns outside the map are clipped by the TMA engine
+            if (MODE == MODE_FLAT) tma_store_3d(tmap, buf + pn * 8192, pn * 64, c0, n);
+            else tma_store_4d(tmap, buf + pn * 8192, pn * 64, c0, c1, n);
+        }
+        bulk_commit();
+    }
+    if (NCMAX == 128 && stat) stats_flush<128>(st, e.lane, stats);
+}
+
+template <int MODE, int COUT, bool F16>
+__global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid_constant__ UmmaConvParams p) {
+    constexpr int kProd = kProdThreads;
+    constexpr int kThreads = kConvThreads;
     constexpr int TAPS = (MODE == MODE_3X3S1 || MODE == MODE_3X3S2) ? 9 : (MODE == MODE_STEM ? 3 : 1);
-    extern __shared__ __align__(128) uint8_t smem[];
+    extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + kSmemBarOff);
     uint64_t* empty = full + kMaxStages;
-    uint64_t* tfull = empty + kMaxStages;
-    uint64_t* tempty = tfull + 2;
-    uint64_t* wbar = tempty + 2;
-    uint64_t* a2_full = wbar + 1;     // tail: intermediate operand written by the epilogue warps
-    uint64_t* a2_empty = a2_full + 2; //       ... consumed by the tail MMAs
-    uint64_t* tfull2 = a2_empty + 2;  //       tail accumulator ready
-    uint64_t* tempty2 = tfull2 + 2;   //       tail accumulator drained
-    uint64_t* res_bar = tempty2 + 2;  // [8] residual rows of one epilogue warp landed (TMA load)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_bar + 8);
+    uint64_t* wbar = empty + kMaxStages;
+    uint64_t* res_bar = wbar + 1;     // [2] residual rows of one warpgroup landed (TMA load)
     PxEntry* table = reinterpret_cast<PxEntry*>(smem + p.smem_table_off);
     PxDelta* delta = reinterpret_cast<PxDelta*>(smem + p.smem_table_off + (size_t)p.n_px * sizeof(PxEntry));
+    float* bias = reinterpret_cast<float*>(smem + p.smem_bias_off);
+    float* bias2 = reinterpret_cast<float*>(smem + p.smem_bias2_off);
     uint8_t* staging = smem + p.smem_staging_off;
     uint8_t* wres = smem + p.smem_w_off;        // resident weights (if any)
     uint8_t* ring = smem + p.smem_ring_off;     // stages: [A chunk | B slice (streaming only)]
 
-    // Programmatic dependent launch: let the next kernel of the stream start its prologue (barrier init, TMEM allocation,
-    // weight fetch) while this one is still running; everything that touches upstream results waits at pdl_wait().
+    // Programmatic dependent launch: let the next kernel of the stream start its prologue (barrier init, weight fetch) while
+    // this one is still running; everything that touches upstream results waits at pdl_wait().
     pdl_launch_dependents();
     LFD_TL_BEGIN(p.tl);
     const int tid = threadIdx.x;
@@ -218,38 +248,17 @@ conv_umma_kernel(const __grid_constant__ UmmaConvParams p) {
     if (tid == 0) {
         for (int i = 0; i < SA; ++i) {
             mbar_init(&full[i], kProd + (p.b_resident ? 0 : 1));
-            mbar_init(&empty[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tfull[i], 1);
-            mbar_init(&tempty[i], EPI_WARPS);
+            mbar_init(&empty[i], kConsumerThreads / 32);
         }
         mbar_init(wbar, 1);
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&a2_full[i], EPI_WARPS);
-            mbar_init(&a2_empty[i], 1);
-            mbar_init(&tfull2[i], 1);
-            mbar_init(&tempty2[i], EPI_WARPS);
-        }
-        for (int i = 0; i < 8; ++i) mbar_init(&res_bar[i], 1);
+        mbar_init(&res_bar[0], 1);
+        mbar_init(&res_bar[1], 1);
         fence_mbar_init();
     }
-    if (warp == kMmaWarp) tmem_alloc(tmem_slot, p.tmem_cols);
-    // The per-channel shift (folded BatchNorm / bias) is added ON THE TENSOR CORE: one extra K=16 MMA per tile of a
-    // constant A operand (column 0 = 1) with a B operand whose k = 0 row holds the bf16 shift.  The epilogue is then just
-    // (+residual) ReLU + convert.
-    for (int i = tid; i < 256; i += kThreads)
-        reinterpret_cast<uint4*>(smem + kSmemOnesOff)[i] = i < 128 ? make_uint4(F16 ? 0x00003C00u : 0x00003F80u, 0u, 0u, 0u) : make_uint4(0u, 0u, 0u, 0u);
-    for (int i = tid; i < 2 * p.Cout; i += kThreads) {
-        const uint32_t b = (i < p.Cout && p.shift) ? bits16<F16>(p.shift[i]) : 0u;
-        reinterpret_cast<uint4*>(smem + p.smem_bias_off)[i] = make_uint4(b, 0u, 0u, 0u);
-    }
+    // per-channel shifts (folded BatchNorm / bias), rounded to the 16-bit type, added to the fp32 accumulators by the epilogue
+    for (int i = tid; i < p.Cout; i += kThreads) bias[i] = p.shift ? round16<F16>(p.shift[i]) : 0.f;
     const int cn2 = p.Cout2 + p.Cout3;      // second GEMM of the launch: fused 1x1 tail or fused 1x1/s2 shortcut (never both)
-    for (int i = tid; i < 2 * cn2; i += kThreads) {
-        const uint32_t b = (i < cn2 && p.shift2) ? bits16<F16>(p.shift2[i]) : 0u;
-        reinterpret_cast<uint4*>(smem + p.smem_bias2_off)[i] = make_uint4(b, 0u, 0u, 0u);
-    }
-    fence_proxy_async_smem();   // these operands are read by tcgen05.mma (async proxy)
+    for (int i = tid; i < cn2; i += kThreads) bias2[i] = p.shift2 ? round16<F16>(p.shift2[i]) : 0.f;
     // halo pixel table (tile independent)
     if (MODE != MODE_FLAT && MODE != MODE_STEM) {
         for (int i = tid; i < p.n_px; i += kThreads) {
@@ -278,278 +287,148 @@ conv_umma_kernel(const __grid_constant__ UmmaConvParams p) {
             delta[i] = d;
         }
     }
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
 
     const int HW = p.H * p.W;
     const int n_cc = p.Cin / p.Cc;
 
-    if (warp < EPI_WARPS) {
-        // ============================================================== EPILOGUE
-        // Every warp works on its own: TMEM lane quarter (warp % 4) x a 1/WPQ slice of the columns -> bf16 rows in its OWN
-        // staging region -> its own TMA tensor store (32 rows x cw channels).  No CTA-wide barrier is involved, and with two
-        // staging buffers the store of tile t is still being read by the TMA engine while tile t+1 is converted.
-        pdl_wait();                                   // residual reads, output stores and statistics depend on upstream kernels
-        constexpr int WPQ = EPI_WARPS / 4;
-        constexpr int MAXB = EPI_WARPS == 4 ? 32 : 64;   // the two-CTAs-per-SM kernels have 96 registers per thread
-        const int quarter = warp & 3, chalf = warp >> 2;
-        const uint32_t lane_base = (uint32_t)(quarter * 32) << 16;   // a warp may only touch TMEM lanes 32 * (warp % 4) ..
-        const int cw = p.Cf / WPQ;                    // stored channels handled by this warp (16, 32, 64 or 128)
-        const int cw1 = p.Cout / WPQ;                 // tail: channels of the intermediate handled by this warp
-        const int ch0 = chalf * cw;
-        // Staging rows are laid out the way the TMA engine expects for its swizzle modes: 128-byte panels
-        // [panel][32 rows][128 B] with the 16-byte chunk index XORed by (row & 7) (SWIZZLE_128B); 64 / 32-byte rows use the
-        // 64B / 32B patterns.  Row offsets are multiples of the row size, so "+" is "^" and chunk k of this lane's row is at
-        //   (pre ^ ((k & 7) << 4)) + (k >> 3) * 4096        with a per-thread constant `pre`.
-        const int row_bytes = cw >= 64 ? 128 : cw * 2;
-        const uint32_t warp_stg = 64u * cw;           // bytes of one staging buffer of this warp: 32 rows x cw x 2
-        const uint32_t stg0 = smem_u32(staging) + (uint32_t)warp * p.stg_nbuf * warp_stg;
-        const uint32_t swz = row_bytes == 128 ? (lane & 7) : (row_bytes == 64 ? ((lane >> 1) & 3) : ((lane >> 2) & 1));
-        const uint32_t pre = (uint32_t)(lane * row_bytes) ^ (swz << 4);
-        const int n_panels = cw >= 64 ? (cw >> 6) : 1;
-        const int HoWo = p.Ho * p.Wo;
-        const bool has_res = p.res != nullptr;
-        // code variant of the conversion loop: log2(cw / 16) | relu << 2 | residual << 3, or 16 + log2(cw / 16) with statistics
-        const int l2cw = cw == 16 ? 0 : (cw == 32 ? 1 : (cw == 64 ? 2 : 3));
-        const int l2cw1 = cw1 == 16 ? 0 : (cw1 == 32 ? 1 : (cw1 == 64 ? 2 : 3));
-        const int fin_relu = p.Cout2 ? p.relu2 : p.relu;
-        const int variant = p.stats ? 16 + l2cw : (l2cw | (fin_relu ? 4 : 0) | (has_res ? 8 : 0));
-        const int variant1 = l2cw1 | (p.relu ? 4 : 0);
-        if (lane == 0 && (stg0 & 1023u)) __trap();    // swizzle atoms need 1024-byte aligned staging regions
-
-        // ---- tail phase 1: main accumulator -> bf16 operand of the fused 1x1 conv (never leaves the SM)
-        auto mid_tile = [&](uint32_t tc) LFD_LAMBDA_INLINE {
-            const uint32_t a = tc & 1, aph = (tc >> 1) & 1;
-            const uint32_t b = p.n_a2 == 2 ? (tc & 1) : 0;
-            const uint32_t use = p.n_a2 == 2 ? (tc >> 1) : tc;       // how often this operand buffer has been filled before
-            mbar_wait(&tfull[a], aph);
-            mbar_wait(&a2_empty[b], (use & 1) ^ 1);                   // tail MMAs of the previous user of this buffer are done
-            tc_fence_after_sync();
-            const uint32_t trow = tmem_base + lane_base + a * p.Cout + chalf * cw1;
-            const uint32_t dst = smem_u32(smem + p.smem_a2_off) + b * p.a2_bytes + (uint32_t)(quarter * 32 + lane) * 16 + (uint32_t)((chalf * cw1) >> 3) * kA2Pitch;
-            switch (variant1) {
-                case 0: drain<16, false, false, false, true, MAXB, F16>(trow, dst, true, nullptr); break;
-                case 1: drain<32, false, false, false, true, MAXB, F16>(trow, dst, true, nullptr); break;
-                case 2: drain<64, false, false, false, true, MAXB, F16>(trow, dst, true, nullptr); break;
-                case 3: drain<128, false, false, false, true, MAXB, F16>(trow, dst, true, nullptr); break;
-                case 4: drain<16, true, false, false, true, MAXB, F16>(trow, dst, true, nullptr); break;
-                case 5: drain<32, true, false, false, true, MAXB, F16>(trow, dst, true, nullptr); break;
-                case 6: drain<64, true, false, false, true, MAXB, F16>(trow, dst, true, nullptr); break;
-                default: drain<128, true, false, false, true, MAXB, F16>(trow, dst, true, nullptr); break;
+    if (warp < kConsumerThreads / 32) {
+        // ============================================================== CONSUMERS (MMA + epilogue)
+        // registers move from the producer warpgroup to the accumulators: 2 x 128 x 224 + 128 x 56 = 64512 of 65536
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
+        const int wg = warp >> 2;
+        const uint32_t w2_bytes = p.Cout2 ? (uint32_t)(p.Cout * p.Cout2 * 2) : (p.Cout3 ? (uint32_t)(p.Cin * p.Cout3 * 2) : 0u);
+        if ((p.b_resident || w2_bytes) && tid == 0) {
+            const uint32_t w1_bytes = p.b_resident ? p.w_total_bytes : 0u;
+            mbar_arrive_expect_tx(wbar, w1_bytes + w2_bytes);
+            for (uint32_t off = 0; off < w1_bytes; off += 32768) {
+                uint32_t nb = w1_bytes - off < 32768 ? w1_bytes - off : 32768;
+                bulk_g2s(smem_u32(wres) + off, reinterpret_cast<const uint8_t*>(p.w) + off, nb, wbar);
             }
-            tc_fence_before_sync();
-            fence_proxy_async_smem();           // st.shared (generic proxy) -> tcgen05.mma (async proxy)
-            __syncwarp();
-            if (lane == 0) {
-                mbar_arrive(&a2_full[b]);
-                mbar_arrive(&tempty[a]);
-            }
-        };
-
-        // ---- final phase: accumulator (+residual) (+ReLU) -> bf16 staging rows -> TMA store (+ GroupNorm statistics)
-        uint32_t store_count = 0;   // staging buffers alternate per STORE (a launch with a fused shortcut stores twice per tile)
-        auto finish_tile = [&](int tile, uint32_t tc, uint64_t* bar_full, uint64_t* bar_empty, uint32_t col_base, const CUtensorMap* tmap,
-                               int var, bool first, bool last) LFD_LAMBDA_INLINE {
-            const int n = fast_div(tile, p.magic_tpi);
-            const int t = tile - n * p.tiles_per_img;
-            int c1, c2 = 0;      // coordinates of this warp's first row: pixel index (flat) or (x, y)
-            bool valid;          // this lane's row lies inside the feature map (statistics only; the TMA store clips)
-            if (MODE == MODE_FLAT) { c1 = t * 128 + quarter * 32; valid = c1 + lane < HoWo; }
-            else {
-                const int ty = fast_div(t, p.magic_tx);
-                c2 = ty * 16 + quarter * 4; c1 = (t - ty * p.tiles_x) * 8;
-                valid = (c2 + (lane >> 3) < p.Ho) && (c1 + (lane & 7) < p.Wo);
-            }
-            const uint32_t a = tc & 1, aph = (tc >> 1) & 1;
-            // (only the 3x3/s2 mode can store twice per tile; the other instantiations keep using the tile counter, which costs
-            //  them no extra live register -- the two-CTAs-per-SM kernels sit right at their 96-register budget)
-            const uint32_t sbuf = stg0 + (p.stg_nbuf == 2 ? ((MODE == MODE_3X3S2 ? store_count : tc) & 1) * warp_stg : 0u);
-            if (MODE == MODE_3X3S2) ++store_count;
-            if (lane == 0) {
-                // this staging buffer was the source of an earlier store: the TMA engine must be done reading it
-                if (p.stg_nbuf == 2) bulk_wait_read<1>(); else bulk_wait_read<0>();
-                if (has_res) {   // residual rows -> staging (out-of-map rows / columns arrive as zeros), added in place below
-                    mbar_arrive_expect_tx(&res_bar[warp], warp_stg);
-                    for (int pn = 0; pn < n_panels; ++pn) {
-                        if (MODE == MODE_FLAT) tma_load_3d(sbuf + pn * 4096, &p.tm_res, ch0 + pn * 64, c1, n, &res_bar[warp]);
-                        else tma_load_4d(sbuf + pn * 4096, &p.tm_res, ch0 + pn * 64, c1, c2, n, &res_bar[warp]);
-                    }
-                }
-            }
-            if (tid == 0) LFD_TRACE(2, tc, 0);
-            if (first) {
-                mbar_wait(&bar_full[a], aph);
-                tc_fence_after_sync();
-            }
-            if (tid == 0) LFD_TRACE(2, tc, 1);
-            if (has_res) mbar_wait(&res_bar[warp], tc & 1);
-            else __syncwarp();                    // lane 0 has seen the buffer free
-            const uint32_t trow = tmem_base + lane_base + col_base + a * p.Cf + ch0;
-            const uint32_t base = sbuf + pre;
-            auto publish = [&]() LFD_LAMBDA_INLINE {
-                tc_fence_before_sync();
-                fence_proxy_async_smem();             // st.shared (generic proxy) -> TMA store (async proxy)
-                __syncwarp();
-                if (lane == 0) {
-                    if (last) mbar_arrive(&bar_empty[a]);   // accumulator stage may be overwritten by the next-but-one tile
-                    for (int pn = 0; pn < n_panels; ++pn) {   // rows / columns outside the map are clipped by the TMA engine
-                        if (MODE == MODE_FLAT) tma_store_3d(tmap, sbuf + pn * 4096, ch0 + pn * 64, c1, n);
-                        else tma_store_4d(tmap, sbuf + pn * 4096, ch0 + pn * 64, c1, c2, n);
-                    }
-                    bulk_commit();
-                }
-            };
-            // GroupNorm partial sums are taken over the STORED (bf16) values; one group = one 16-byte chunk (8 channels)
-            double* sdst = p.stats ? p.stats + ((size_t)n * p.gn_groups + (ch0 >> 3)) * 2 : nullptr;
-            switch (var) {
-                case 0: drain<16, false, false, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 1: drain<32, false, false, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 2: drain<64, false, false, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 3: drain<128, false, false, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 4: drain<16, true, false, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 5: drain<32, true, false, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 6: drain<64, true, false, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 7: drain<128, true, false, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 8: drain<16, false, true, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 9: drain<32, false, true, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 10: drain<64, false, true, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 11: drain<128, false, true, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 12: drain<16, true, true, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 13: drain<32, true, true, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 14: drain<64, true, true, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 15: drain<128, true, true, false, false, MAXB, F16>(trow, base, valid, nullptr); break;
-                case 16: { float st[4]; drain<16, false, false, true, false, MAXB, F16>(trow, base, valid, st); publish(); stats_flush<16>(st, lane, sdst); } break;
-                case 17: { float st[8]; drain<32, false, false, true, false, MAXB, F16>(trow, base, valid, st); publish(); stats_flush<32>(st, lane, sdst); } break;
-                case 18: { float st[16]; drain<64, false, false, true, false, MAXB, F16>(trow, base, valid, st); publish(); stats_flush<64>(st, lane, sdst); } break;
-                default: { float st[32]; drain<128, false, false, true, false, MAXB, F16>(trow, base, valid, st); publish(); stats_flush<128>(st, lane, sdst); } break;
-            }
-            if (var < 16) publish();
-            if (tid == 0) LFD_TRACE(2, tc, 2);
-            if (tid == 0) LFD_TRACE(2, tc, 3);
-        };
-
-        if (!p.Cout2) {
-            uint32_t tcount = 0;
-            // fused shortcut (3x3/s2 only): a second pass drains the second accumulator of the same stage (same barriers) into
-            // its own tensor, without ReLU.  One call site, so that the lambda stays inlined in every instantiation.
-            const int n_pass = (MODE == MODE_3X3S2 && p.Cout3) ? 2 : 1;
-            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++tcount)
-                for (int ps = 0; ps < n_pass; ++ps)
-                    finish_tile(tile, tcount, tfull, tempty, ps ? 2 * p.Cout : 0, ps ? &p.tm_out3 : &p.tm_out, ps ? l2cw : variant, ps == 0,
-                                ps == n_pass - 1);
-        } else {
-            // software pipelined: intermediate of tile t, then the finished tail of tile t-1
-            uint32_t tcount = 0;
-            for (int tile = blockIdx.x;; tile += gridDim.x, ++tcount) {
-                const bool has = tile < p.num_tiles;
-                if (has) mid_tile(tcount);
-                if (tcount >= 1) finish_tile(tile - (int)gridDim.x, tcount - 1, tfull2, tempty2, 2 * p.Cout, &p.tm_out, variant, true, true);
-                if (!has) break;
-            }
+            if (w2_bytes) bulk_g2s(smem_u32(smem + p.smem_w2_off), p.w2, w2_bytes, wbar);
         }
-        if (lane == 0) bulk_wait_all();   // all tile stores have been performed before the CTA retires
-    } else if (warp == kMmaWarp) {
-        // ============================================================== MMA ISSUER
-        // The whole warp runs the (warp-uniform) control flow so that descriptors live in uniform registers; one elected
-        // lane issues the tcgen05 instructions.
-        const uint32_t idesc = umma_idesc_16(128, p.Cout, F16);
-        const uint32_t lbo_b = p.Cout * 16;
+        pdl_wait();                                   // residual reads, output stores and statistics depend on upstream kernels
+        if (p.b_resident || w2_bytes) mbar_wait(wbar, 0);
+
+        EpiCtx e;
+        e.stg_bytes = 64u * p.Cf * 2u;
+        e.nbuf = p.stg_nbuf;
+        e.stg = smem_u32(staging) + (uint32_t)wg * e.nbuf * e.stg_bytes;
+        e.r0 = (warp & 3) * 16 + (lane >> 2);
+        e.tq = lane & 3;
+        e.wtid = tid & 127;
+        e.wg = wg;
+        e.lane = lane;
+        if (e.wtid == 0 && (e.stg & 1023u)) __trap();    // swizzle atoms need 1024-byte aligned staging regions
+
+        const uint32_t lbo_b = COUT * 16;
         // descriptors differ only in the 14-bit start-address field (bytes >> 4): pre-compute everything else
-        const uint64_t adesc0 = umma_smem_desc(0, p.lbo_a, p.sbo_a);
-        const uint64_t bdesc0 = umma_smem_desc(0, lbo_b, 128);
+        const uint64_t adesc0 = wgmma_desc(0, p.lbo_a, p.sbo_a);
+        const uint64_t bdesc0 = wgmma_desc(0, lbo_b, 128);
         const uint32_t a_k16 = (2 * p.lbo_a) >> 4;      // address-field step per 16 input channels (A)
         const uint32_t b_k16 = (2 * lbo_b) >> 4;        //   (B)
         const uint32_t b_tap = (cpc * lbo_b) >> 4;      // address-field step per tap (B)
+        const uint32_t a_wg = (8u * p.sbo_a * wg) >> 4; // this warpgroup's 64 rows start 8 core-matrix rows further down
         const int nk16 = p.Cc >> 4;
-        const uint32_t w2_bytes = p.Cout2 ? (uint32_t)(p.Cout * p.Cout2 * 2) : (p.Cout3 ? (uint32_t)(p.Cin * p.Cout3 * 2) : 0u);
-        if (p.b_resident || w2_bytes) {
-            if (elect_one_sync()) {
-                const uint32_t w1_bytes = p.b_resident ? p.w_total_bytes : 0u;
-                mbar_arrive_expect_tx(wbar, w1_bytes + w2_bytes);
-                for (uint32_t off = 0; off < w1_bytes; off += 32768) {
-                    uint32_t nb = w1_bytes - off < 32768 ? w1_bytes - off : 32768;
-                    bulk_g2s(smem_u32(wres) + off, reinterpret_cast<const uint8_t*>(p.w) + off, nb, wbar);
-                }
-                if (w2_bytes) bulk_g2s(smem_u32(smem + p.smem_w2_off), p.w2, w2_bytes, wbar);
-            }
-            __syncwarp();
-            mbar_wait(wbar, 0);
-        }
-        // fused 1x1 tail: D2[128 x Cout2] = A2[128 x Cout] . W2, A2 written by the epilogue warps (mid_tile)
-        const uint32_t idesc2 = umma_idesc_16(128, cn2 ? cn2 : 16, F16);
-        const uint64_t ones_desc = umma_smem_desc(smem_u32(smem + kSmemOnesOff), 2048, 128);
-        const uint64_t bias_desc = umma_smem_desc(smem_u32(smem + p.smem_bias_off), lbo_b, 128);
-        const uint64_t bias2_desc = umma_smem_desc(smem_u32(smem + p.smem_bias2_off), cn2 * 16, 128);
-        const uint64_t a2desc0 = umma_smem_desc(0, kA2Pitch, 128);
-        const uint64_t b2desc0 = umma_smem_desc(smem_u32(smem + p.smem_w2_off), cn2 * 16, 128);
-        auto issue_tail = [&](uint32_t u) LFD_LAMBDA_INLINE {
-            const uint32_t b = p.n_a2 == 2 ? (u & 1) : 0, use = p.n_a2 == 2 ? (u >> 1) : u;
-            const uint32_t a2s = u & 1, a2ph = (u >> 1) & 1;
-            mbar_wait(&a2_full[b], use & 1);
-            mbar_wait(&tempty2[a2s], a2ph ^ 1);
-            tc_fence_after_sync();
-            fence_proxy_async_smem();
-            if (elect_one_sync()) {
-                const uint64_t ad2 = a2desc0 + ((smem_u32(smem + p.smem_a2_off) + b * p.a2_bytes) >> 4);
-                const uint32_t d2 = tmem_base + 2 * p.Cout + a2s * p.Cout2;
-                for (int k16 = 0; k16 < (p.Cout >> 4); ++k16)
-                    umma_bf16(d2, ad2 + (uint32_t)(k16 * ((2 * kA2Pitch) >> 4)), b2desc0 + (uint32_t)(k16 * ((2 * p.Cout2 * 16) >> 4)), idesc2, k16 != 0);
-                if (p.shift2) umma_bf16(d2, ones_desc, bias2_desc, idesc2, 1);
-                umma_commit(&tfull2[a2s]);
-                umma_commit(&a2_empty[b]);
-            }
-            __syncwarp();
-        };
-        uint32_t it = 0, tcount = 0;
-        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++tcount) {
-            const uint32_t a = tcount & 1, aph = (tcount >> 1) & 1;
-            if (lane == 0) LFD_TRACE(1, tcount, 0);
-            mbar_wait(&tempty[a], aph ^ 1);
-            tc_fence_after_sync();
-            if (lane == 0) LFD_TRACE(1, tcount, 1);
-            const uint32_t d_tmem = tmem_base + a * p.Cout;
+        const uint64_t b2desc0 = wgmma_desc(smem_u32(smem + p.smem_w2_off), cn2 * 16, 128);
+        const int HoWo = p.Ho * p.Wo;
+
+        float acc[COUT / 2];
+        float acc3[MODE == MODE_3X3S2 ? COUT / 2 : 1];
+        uint32_t it = 0, store_count = 0, res_count = 0;
+        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
             for (int cc = 0; cc < n_cc; ++cc, ++it) {
                 const uint32_t s = it % SA, ph = (it / SA) & 1;
                 mbar_wait(&full[s], ph);
-                tc_fence_after_sync();
-                fence_proxy_async_smem();   // cp.async (generic proxy) writes -> tcgen05.mma (async proxy) reads
-                if (cc == 0 && lane == 0) LFD_TRACE(1, tcount, 2);
+                fence_proxy_async_smem();   // cp.async / st.shared (generic proxy) writes -> wgmma (async proxy) reads
                 const uint32_t a_base = smem_u32(ring) + s * p.stage_bytes;
                 const uint32_t b_base = p.b_resident ? smem_u32(wres) + cc * p.b_slice_bytes : a_base + p.a_stage_bytes;
-                const uint64_t ad = adesc0 + (a_base >> 4), bd = bdesc0 + (b_base >> 4);
-                if (elect_one_sync()) {
-                    for (int k16 = 0; k16 < nk16; ++k16) {
-                        const uint64_t adk = ad + (uint32_t)(k16 * a_k16), bdk = bd + (uint32_t)(k16 * b_k16);
+                const uint64_t ad = adesc0 + ((a_base >> 4) + a_wg), bd = bdesc0 + (b_base >> 4);
+                wgmma_fence_regs<COUT / 2>(acc);
+                wgmma_fence();
+                for (int k16 = 0; k16 < nk16; ++k16) {
+                    const uint64_t adk = ad + (uint32_t)(k16 * a_k16), bdk = bd + (uint32_t)(k16 * b_k16);
 #pragma unroll
-                        for (int tap = 0; tap < TAPS; ++tap)
-                            umma_bf16(d_tmem, adk + (uint32_t)tap_view<MODE>(tap), bdk + (uint32_t)(tap * b_tap), idesc, (cc | k16 | tap) != 0);
-                    }
-                    if (MODE == MODE_3X3S2 && p.Cout3) {
-                        // fused 1x1/s2 shortcut conv of the residual block: its input pixel is this conv's centre tap, so it
-                        // is one more MMA per 16 channels on the operand that is already in shared memory
-                        const uint32_t d3 = tmem_base + 2 * p.Cout + a * p.Cout3;
-                        for (int k16 = 0; k16 < nk16; ++k16)
-                            umma_bf16(d3, ad + (uint32_t)(k16 * a_k16) + (uint32_t)tap_view<MODE>(4),
-                                      b2desc0 + (uint32_t)(((cc * cpc + 2 * k16) * p.Cout3 * 16) >> 4), idesc2, (cc | k16) != 0);
-                        if (cc == n_cc - 1 && p.shift2) umma_bf16(d3, ones_desc, bias2_desc, idesc2, 1);
-                    }
-                    umma_commit(&empty[s]);
-                    if (cc == n_cc - 1) {
-                        if (p.shift) umma_bf16(d_tmem, ones_desc, bias_desc, idesc, 1);
-                        umma_commit(&tfull[a]);
+                    for (int tap = 0; tap < TAPS; ++tap)
+                        wgmma_ss<COUT, F16>(acc, adk + (uint32_t)tap_view<MODE>(tap), bdk + (uint32_t)(tap * b_tap), (cc | k16 | tap) != 0);
+                }
+                if (MODE == MODE_3X3S2 && p.Cout3) {
+                    // fused 1x1/s2 shortcut conv of the residual block: its input pixel is this conv's centre tap, so it
+                    // is one more MMA per 16 channels on the operand that is already in shared memory
+                    wgmma_fence_regs<MODE == MODE_3X3S2 ? COUT / 2 : 1>(acc3);
+                    for (int k16 = 0; k16 < nk16; ++k16)
+                        wgmma_ss<COUT, F16>(acc3, ad + (uint32_t)(k16 * a_k16) + (uint32_t)tap_view<MODE>(4),
+                                            b2desc0 + (uint32_t)(((cc * cpc + 2 * k16) * COUT * 16) >> 4), (cc | k16) != 0);
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_regs<COUT / 2>(acc);
+                if (MODE == MODE_3X3S2) wgmma_fence_regs<MODE == MODE_3X3S2 ? COUT / 2 : 1>(acc3);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[s]);     // this warp's part of the stage has been consumed
+            }
+
+            // ---- epilogue of the tile: this warpgroup's 64 rows
+            const int n = fast_div(tile, p.magic_tpi);
+            const int t = tile - n * p.tiles_per_img;
+            int c0, c1 = 0;      // coordinates of the warpgroup's first row: pixel index (flat) or (x, y)
+            bool v0, v1;         // this thread's two rows lie inside the feature map (statistics only; the TMA store clips)
+            if (MODE == MODE_FLAT) {
+                c0 = t * 128 + wg * 64;
+                v0 = c0 + e.r0 < HoWo; v1 = c0 + e.r0 + 8 < HoWo;
+            } else {
+                const int ty = fast_div(t, p.magic_tx);
+                c1 = ty * 16 + wg * 8; c0 = (t - ty * p.tiles_x) * 8;
+                const bool xin = c0 + (e.r0 & 7) < p.Wo;
+                v0 = xin && c1 + (e.r0 >> 3) < p.Ho; v1 = xin && c1 + (e.r0 >> 3) + 1 < p.Ho;
+            }
+            const bool has_res = p.res != nullptr;
+            // GroupNorm partial sums are taken over the STORED (16-bit) values; one group = one 16-byte chunk (8 channels); a
+            // layer with statistics stores the raw (conv + shift) values
+            double* sdst = p.stats ? p.stats + (size_t)n * p.gn_groups * 2 : nullptr;
+            if (p.Cout2) {
+                // fused 1x1 tail: D2[64 x Cout2] = round16(act(D + shift)) . W2, the A operand straight from the accumulator registers
+                uint32_t a2[COUT / 4];
+#pragma unroll
+                for (int kk = 0; kk < COUT / 16; ++kk) {
+                    const int c = 16 * kk + 2 * e.tq;
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) {     // q: (row + 8 (q & 1), column + 8 (q >> 1))
+                        const float x0 = acc[8 * kk + 2 * q] + bias[c + 8 * (q >> 1)], x1 = acc[8 * kk + 2 * q + 1] + bias[c + 8 * (q >> 1) + 1];
+                        a2[4 * kk + q] = p.relu ? pack2_relu<F16>(x0, x1) : pack2<F16>(x0, x1);
                     }
                 }
-                __syncwarp();
-                if (cc == n_cc - 1 && lane == 0) LFD_TRACE(1, tcount, 3);
+                float acc2[64];
+                wgmma_fence_regs<64>(acc2);
+                wgmma_fence();
+#pragma unroll
+                for (int nb = 0; nb < 8; ++nb) {
+                    if (nb < p.Cout2 / 16) {
+#pragma unroll
+                        for (int kk = 0; kk < COUT / 16; ++kk)
+                            wgmma_rs_n16<F16>(acc2 + 8 * nb, a2 + 4 * kk, b2desc0 + (uint32_t)((kk * 2 * p.Cout2 * 16 + nb * 256) >> 4), kk != 0);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_regs<64>(acc2);
+                store_tile<MODE, 128, F16>(e, acc2, p.Cout2, bias2, p.stats ? false : (bool)p.relu2, p.stats ? false : has_res, sdst,
+                                           &p.tm_out, &p.tm_res, c0, c1, n, v0, v1, &res_bar[wg], store_count, res_count);
+            } else {
+                store_tile<MODE, COUT, F16>(e, acc, COUT, bias, p.stats ? false : (bool)p.relu, p.stats ? false : has_res, sdst,
+                                            &p.tm_out, &p.tm_res, c0, c1, n, v0, v1, &res_bar[wg], store_count, res_count);
+                if constexpr (MODE == MODE_3X3S2) {
+                    if (p.Cout3)
+                        store_tile<MODE, COUT, F16>(e, acc3, COUT, bias2, false, false, nullptr, &p.tm_out3, nullptr, c0, c1, n, v0, v1,
+                                                    &res_bar[wg], store_count, res_count);
+                }
             }
-            if (p.Cout2 && tcount >= 1) issue_tail(tcount - 1);
         }
-        if (p.Cout2 && tcount >= 1) issue_tail(tcount - 1);
+        if (e.wtid == 0) bulk_wait_all();   // all tile stores have been performed before the CTA retires
     } else {
         // ============================================================== PRODUCERS
-        const int ptid = tid - (kEpiThreads + 32);
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+        const int ptid = tid - kConsumerThreads;
         if (MODE == MODE_STEM) {
             // Raw image patch -> normalised bf16 [row][pixel][b g r 0] in the ring stage (see kStem* above).  Every thread owns
             // up to 5 patch pixels; the raw values of the NEXT tile are fetched into registers right after the current patch
@@ -628,7 +507,7 @@ conv_umma_kernel(const __grid_constant__ UmmaConvParams p) {
                     const uint32_t lo = pack2<F16>(f[0], f[1]), hi = pack2<F16>(f[2], 0.f);   // rounding point R0
                     asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(dst0 + j * (kProdThreads * 8)), "r"(lo), "r"(hi) : "memory");
                 }
-                fence_proxy_async_smem();       // generic-proxy st.shared -> tcgen05.mma reads
+                fence_proxy_async_smem();       // generic-proxy st.shared -> wgmma reads
                 mbar_arrive(&full[s]);
                 if (tile + (int)gridDim.x < p.num_tiles) fetch(tile + gridDim.x);
             }
@@ -714,22 +593,12 @@ conv_umma_kernel(const __grid_constant__ UmmaConvParams p) {
         cp_async_wait_all();
         }
     }
-
-    // ------------------------------------------------------------------ teardown
-    tc_fence_before_sync();
-    __syncthreads();
-    if (warp == kMmaWarp) {
-        tc_fence_after_sync();
-        tmem_dealloc(tmem_base, p.tmem_cols);
-    }
     LFD_TL_END(p.tl);
 }
 
 // ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
-static int epi_warps_of(int mode) { return (mode == MODE_3X3S1 || mode == MODE_3X3S2) ? 8 : 4; }
-
 static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvParams* out, size_t* smem_bytes, int* grid) {
     UmmaConvParams p;
     memset(&p, 0, sizeof(p));
@@ -743,8 +612,9 @@ static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvPara
     else if (g.ksize == 3 && g.stride == 2) mode = MODE_3X3S2;
     else if (g.ksize == 1 && g.stride == 2) mode = MODE_1X1S2;
     else return -1;
-    if (g.Cin % 16 || g.Cout % 16 || g.Cout > 128 || g.Cout < 16) return -1;
-    if (epi_warps_of(mode) == 8 && g.Cout < 32) return -1;   // two epilogue warps per lane quarter need >= 16 columns each
+    // instantiated output widths (conv_umma_launch): 16 / 32 / 64 / 128 channels, 3x3 convs from 32
+    if (g.Cin % 16 || (g.Cout != 16 && g.Cout != 32 && g.Cout != 64 && g.Cout != 128)) return -1;
+    if ((mode == MODE_3X3S1 || mode == MODE_3X3S2) && g.Cout < 32) return -1;
     p.mode = mode;
     p.N = g.N; p.H = g.H; p.W = g.W; p.Cin = g.Cin; p.Ho = g.Ho; p.Wo = g.Wo; p.Cout = g.Cout;
     const int taps = g.stem ? 3 : g.ksize * g.ksize;   // stem: one MMA group per filter row
@@ -769,31 +639,26 @@ static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvPara
     p.magic_tx = p.tiles_x ? ((1ull << 40) + p.tiles_x - 1) / p.tiles_x : 0;
     const int Cf = g.tail_cout > 0 ? g.tail_cout : g.Cout;
     if (g.ds_cout && (mode != MODE_3X3S2 || g.tail_cout || g.ds_cout != g.Cout)) return -6;
-    if (g.tail_cout) {
-        if (g.tail_cout % 16 || g.tail_cout > 128 || g.tail_cout < 16 || 2 * (g.Cout + g.tail_cout) > 512) return -4;
-        if (epi_warps_of(mode) == 8 && g.tail_cout < 32) return -4;
-    }
-    const size_t staging = (size_t)nbuf * 128 * Cf * 2;   // [epilogue warp][buffer][32 rows][Cf / (warps per quarter)]
-    // fixed head of the shared-memory map: barriers | ones operand | [halo table] | bias | [tail bias] | staging (1 KB aligned)
-    size_t hoff = kSmemOnesOff + 4096;
+    if (g.tail_cout && (g.tail_cout % 16 || g.tail_cout > 128 || g.tail_cout < 16)) return -4;
+    const size_t staging = (size_t)nbuf * 128 * Cf * 2;   // [warpgroup][buffer][64 rows][Cf]
+    // fixed head of the shared-memory map: barriers | [halo table] | shift | [tail shift] | staging (1 KB aligned)
+    size_t hoff = kSmemTableOff;
     p.smem_table_off = (uint32_t)hoff;
     if (mode != MODE_FLAT && mode != MODE_STEM) hoff += ((size_t)p.n_px * 10 + 127) & ~(size_t)127;   // PxEntry[n_px] | PxDelta[n_px]
-    p.smem_bias_off = (uint32_t)hoff; hoff += (size_t)g.Cout * 32;
-    p.smem_bias2_off = (uint32_t)hoff; hoff += (size_t)(g.tail_cout + g.ds_cout) * 32;
+    p.smem_bias_off = (uint32_t)hoff; hoff += ((size_t)g.Cout * 4 + 15) & ~(size_t)15;
+    p.smem_bias2_off = (uint32_t)hoff; hoff += ((size_t)(g.tail_cout + g.ds_cout) * 4 + 15) & ~(size_t)15;
     p.smem_staging_off = (uint32_t)((hoff + 1023) & ~(size_t)1023);
     const size_t fixed = p.smem_staging_off + staging;
-    // everything that lives behind the ring: fused-tail weights + two operand buffers
-    const size_t a2_bytes = g.tail_cout ? ((size_t)(g.Cout / 8) * 129 * 16 + 127) & ~(size_t)127 : 0;
+    // what lives behind the ring: the weights of the fused tail / shortcut conv
     const size_t w2_bytes = g.tail_cout ? ((size_t)g.Cout * g.tail_cout * 2 + 127) & ~(size_t)127
                                         : (g.ds_cout ? ((size_t)g.Cin * g.ds_cout * 2 + 127) & ~(size_t)127 : 0);
-    const size_t post = w2_bytes + 2 * a2_bytes;
+    const size_t post = w2_bytes;
     const size_t budget = 224 * 1024 - post;
     const size_t w_total = (size_t)taps * g.Cin * g.Cout * 2;
     // Choose the channel chunk Cc, weight residency and ring depth.  Preference order:
     //   1. resident weights (loaded once per CTA) with >= 3 A stages, the largest Cc first;
     //   2. otherwise streamed weights: the largest Cc that still gives >= 4 stages (deep ring hides the per-stage
     //      weight fetch), then >= 3, then >= 2.
-    // Memory-bound 1x1 layers additionally cap the ring so that two CTAs fit on one SM (latency hiding).
     const int cands[3] = {64, 32, 16};
     int best_cc = 0, best_res = 0, best_st = 0;
     auto a_bytes = [&](int cc) -> size_t {
@@ -810,8 +675,8 @@ static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvPara
         if (st > 4 && stage >= 8192) st = 4;
         return st;
     };
-    // (16-channel chunks mean 32-byte global segments per pixel and twice the barrier round trips per tile: measured
-    //  1600 cycles per 19 KB stage for the 3x3/s2 stem conv, so a 2-deep ring of 32-channel stages beats a 4-deep one of 16)
+    // (16-channel chunks mean 32-byte global segments per pixel and twice the barrier round trips per tile, so a 2-deep ring of
+    //  32-channel stages is preferred to a 4-deep one of 16)
     static const int force_cc = getenv("LFD_B200_FORCE_CC") ? atoi(getenv("LFD_B200_FORCE_CC")) : 0;   // experiments only
     if (force_cc && mode == MODE_3X3S2) {
         int st = stages_for(force_cc, 1);
@@ -825,8 +690,7 @@ static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvPara
             if (st >= want) { best_cc = cands[ci]; best_res = 1; best_st = st; }
         }
     // Streaming re-reads the whole filter bank from L2 for every tile, so it is taken only when the weights cannot be
-    // resident next to a ring of >= 2 stages of >= 32 channels (measured on the 3x3/s2 64->64 + tail layer at 180x320:
-    // resident / 32 / 2 stages beats streamed / 16 / 4 stages).
+    // resident next to a ring of >= 2 stages of >= 32 channels.
     if (!best_cc || (best_st < 3 && best_cc < 32)) {
         for (int want = 4; want >= 2; --want) {
             bool found = false;
@@ -845,17 +709,6 @@ static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvPara
     p.w_total_bytes = (uint32_t)w_total;
     p.smem_w_off = (uint32_t)fixed;
     p.smem_ring_off = (uint32_t)(fixed + (best_res ? w_total : 0));
-    // two CTAs per SM when a >= 2-deep ring fits in half of the shared memory (1x1 / stem layers; 4 epilogue warps each)
-    p.ctas_per_sm = 1;
-    if (epi_warps_of(mode) == 4) {
-        const size_t half = (227 * 1024) / 2 - 1024;
-        const size_t base = p.smem_ring_off + post;
-        if (base + 2 * (size_t)p.stage_bytes <= half) {
-            int st = (int)((half - base) / p.stage_bytes);
-            if (st > p.stages) st = p.stages;
-            if (st >= 2) { p.stages = st; p.ctas_per_sm = 2; }
-        }
-    }
     auto ilog2 = [](int v) { int l = 0; while ((1 << l) < v) ++l; return l; };
     p.log2_cpc = ilog2(p.Cc / 8);
     p.Cf = Cf;
@@ -863,36 +716,22 @@ static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvPara
     p.Cout3 = g.ds_cout;
     p.log2_cpr = ilog2(Cf / 8);
     if ((1 << p.log2_cpr) != Cf / 8) return -3;       // stored channel count must be 16/32/64/128
-    p.log2_rp128 = Cf * 2 >= 128 ? 0 : ilog2(128 / (Cf * 2));
-    {   // TMEM: two accumulator stages of the conv (+ two of the tail); power of two >= 32
-        int need = 2 * g.Cout + 2 * (g.tail_cout + g.ds_cout), cols = 32;
-        while (cols < need) cols <<= 1;
-        p.tmem_cols = cols;
-    }
     size_t off = p.smem_ring_off + (size_t)p.stages * p.stage_bytes;
-    if (g.tail_cout) {
-        p.smem_w2_off = (uint32_t)off; off += w2_bytes;
-        p.smem_a2_off = (uint32_t)off; off += 2 * a2_bytes;
-        p.a2_bytes = (uint32_t)a2_bytes; p.n_a2 = 2;
-    } else if (g.ds_cout) {
-        p.smem_w2_off = (uint32_t)off; off += w2_bytes;
-    }
+    p.smem_w2_off = (uint32_t)off; off += w2_bytes;
     *smem_bytes = off;
-    if (p.ctas_per_sm == 2 && 2 * p.tmem_cols > 512) p.ctas_per_sm = 1;
-    const int max_ctas = num_sms * p.ctas_per_sm;
-    *grid = p.num_tiles < max_ctas ? p.num_tiles : max_ctas;
+    *grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
     *out = p;
     return 0;
 }
 
 int umma_conv_configure(const ConvGeom& g, int num_sms, UmmaConvParams* out, size_t* smem_bytes, int* grid) {
-    // a second staging buffer per epilogue warp is taken when it costs neither occupancy, weight residency nor ring depth
+    // a second staging buffer per warpgroup is taken when it costs neither weight residency nor ring depth
     UmmaConvParams p1, p2;
     size_t s1 = 0, s2 = 0;
     int g1 = 0, g2 = 0;
     const int rc = configure_with(g, num_sms, 1, &p1, &s1, &g1);
     if (rc) return rc;
-    if (configure_with(g, num_sms, 2, &p2, &s2, &g2) == 0 && p2.ctas_per_sm == p1.ctas_per_sm && p2.b_resident == p1.b_resident &&
+    if (configure_with(g, num_sms, 2, &p2, &s2, &g2) == 0 && p2.b_resident == p1.b_resident &&
         p2.Cc == p1.Cc && p2.stages >= (p1.stages < 3 ? p1.stages : 3)) {
         *out = p2; *smem_bytes = s2; *grid = g2;
     } else {
@@ -917,14 +756,13 @@ static EncodeTiledFn encode_fn() {
     return fn;
 }
 
-// One tensor map per stored tensor; the box is what ONE epilogue warp moves: 32 tile rows (32 pixels of a flat tile, 8 x 4 of
-// a spatial one) x min(64, its channel slice) channels, shared-memory side in the matching swizzle mode.
+// One tensor map per stored tensor; the box is what ONE warpgroup moves: 64 tile rows (64 pixels of a flat tile, 8 x 8 of
+// a spatial one) x min(64, Cf) channels, shared-memory side in the matching swizzle mode.
 static int encode_one(const UmmaConvParams& p, const void* ptr, CUtensorMap* tm) {
     EncodeTiledFn fn = encode_fn();
     if (!fn) return -1;
     const cuuint64_t Cf = p.Cf, HoWo = (cuuint64_t)p.Ho * p.Wo;
-    const int cw = p.Cf / (epi_warps_of(p.mode) / 4);
-    const cuuint32_t inner = cw < 64 ? cw : 64;
+    const cuuint32_t inner = p.Cf < 64 ? p.Cf : 64;
     const CUtensorMapSwizzle swz = inner * 2 >= 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (inner * 2 == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
     cuuint64_t dims[4], strides[3];
     cuuint32_t box[4], estr[4] = {1, 1, 1, 1};
@@ -933,12 +771,12 @@ static int encode_one(const UmmaConvParams& p, const void* ptr, CUtensorMap* tm)
         rank = 3;
         dims[0] = Cf; dims[1] = HoWo; dims[2] = p.N;
         strides[0] = Cf * 2; strides[1] = HoWo * Cf * 2;
-        box[0] = inner; box[1] = 32; box[2] = 1;
+        box[0] = inner; box[1] = 64; box[2] = 1;
     } else {
         rank = 4;
         dims[0] = Cf; dims[1] = p.Wo; dims[2] = p.Ho; dims[3] = p.N;
         strides[0] = Cf * 2; strides[1] = (cuuint64_t)p.Wo * Cf * 2; strides[2] = HoWo * Cf * 2;
-        box[0] = inner; box[1] = 8; box[2] = 4; box[3] = 1;
+        box[0] = inner; box[1] = 8; box[2] = 8; box[3] = 1;
     }
     CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
                     CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -952,14 +790,14 @@ int umma_conv_encode_maps(UmmaConvParams* p) {
     return 0;
 }
 
-template <int MODE, int EPI_WARPS, bool F16>
+template <int MODE, int COUT, bool F16>
 static cudaError_t launch_mode_t(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
     // cudaFuncAttributeMaxDynamicSharedMemorySize is a PER-DEVICE attribute: one flag per device ordinal
     static bool configured[kMaxDevices] = {};
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
     if (!configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel<MODE, EPI_WARPS, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(224 * 1024));
+        cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel<MODE, COUT, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(224 * 1024));
         if (e != cudaSuccess) return e;
         configured[dev] = true;
     }
@@ -967,7 +805,7 @@ static cudaError_t launch_mode_t(const UmmaConvParams& p, size_t smem, int grid,
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(EPI_WARPS * 32 + 32 + ProdThreads<MODE>::value);
+    cfg.blockDim = dim3(kConvThreads);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
@@ -975,21 +813,33 @@ static cudaError_t launch_mode_t(const UmmaConvParams& p, size_t smem, int grid,
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = use_pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, conv_umma_kernel<MODE, EPI_WARPS, F16>, p);
+    return cudaLaunchKernelEx(&cfg, conv_umma_kernel<MODE, COUT, F16>, p);
 }
 
-template <int MODE, int EPI_WARPS>
+template <int MODE, int COUT>
 static cudaError_t launch_mode(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
-    return p.f16 ? launch_mode_t<MODE, EPI_WARPS, true>(p, smem, grid, st) : launch_mode_t<MODE, EPI_WARPS, false>(p, smem, grid, st);
+    return p.f16 ? launch_mode_t<MODE, COUT, true>(p, smem, grid, st) : launch_mode_t<MODE, COUT, false>(p, smem, grid, st);
+}
+
+// the output widths umma_conv_configure accepts per mode
+template <int MODE>
+static cudaError_t launch_cout(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
+    switch (p.Cout) {
+        case 16: if (MODE != MODE_3X3S1 && MODE != MODE_3X3S2) return launch_mode<MODE, 16>(p, smem, grid, st); break;
+        case 32: return launch_mode<MODE, 32>(p, smem, grid, st);
+        case 64: return launch_mode<MODE, 64>(p, smem, grid, st);
+        case 128: if (MODE != MODE_STEM) return launch_mode<MODE, 128>(p, smem, grid, st); break;
+    }
+    return cudaErrorInvalidValue;
 }
 
 cudaError_t umma_conv_launch(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
     switch (p.mode) {
-        case MODE_FLAT: return launch_mode<MODE_FLAT, 4>(p, smem, grid, st);
-        case MODE_3X3S1: return launch_mode<MODE_3X3S1, 8>(p, smem, grid, st);
-        case MODE_3X3S2: return launch_mode<MODE_3X3S2, 8>(p, smem, grid, st);
-        case MODE_1X1S2: return launch_mode<MODE_1X1S2, 4>(p, smem, grid, st);
-        case MODE_STEM: return launch_mode<MODE_STEM, 4>(p, smem, grid, st);
+        case MODE_FLAT: return launch_cout<MODE_FLAT>(p, smem, grid, st);
+        case MODE_3X3S1: return launch_cout<MODE_3X3S1>(p, smem, grid, st);
+        case MODE_3X3S2: return launch_cout<MODE_3X3S2>(p, smem, grid, st);
+        case MODE_1X1S2: return launch_cout<MODE_1X1S2>(p, smem, grid, st);
+        case MODE_STEM: return launch_cout<MODE_STEM>(p, smem, grid, st);
     }
     return cudaErrorInvalidValue;
 }

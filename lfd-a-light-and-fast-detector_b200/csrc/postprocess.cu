@@ -507,7 +507,7 @@ cudaError_t candidates_launch(const PostParams& p, int num_sms, cudaStream_t st)
     if (p.cls_mode == 0 && p.C > 1) {
         const long long total = (long long)p.P * p.cls_stride;
         long long blocks = (total + 255) / 256;
-        const long long cap = (long long)(num_sms > 0 ? num_sms : 148) * 8;     // grid-stride beyond 8 blocks per SM and image
+        const long long cap = (long long)(num_sms > 0 ? num_sms : 132) * 8;     // grid-stride beyond 8 blocks per SM and image
         if (blocks > cap) blocks = cap;
         candidates_flat_kernel<<<dim3((unsigned)blocks, p.N), 256, 0, st>>>(p);
     } else if (p.cls_stride > 1 && (size_t)kRowsPts * p.cls_stride * 4 <= 48 * 1024) {

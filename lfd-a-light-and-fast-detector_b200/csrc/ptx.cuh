@@ -1,11 +1,8 @@
-// ptx.cuh -- thin inline-PTX wrappers for sm_100a: mbarrier, cp.async, bulk copy (TMA 1-D), tcgen05
-// (alloc / mma / commit / ld / fences), plus UMMA descriptor builders.
+// ptx.cuh -- thin inline-PTX wrappers for sm_90a: mbarrier, cp.async, bulk copy (TMA 1-D), TMA tensor copies,
+// wgmma (warpgroup MMA) and its shared-memory descriptors.
 //
-// Descriptor bit layouts follow the sm_100 UMMA conventions (shared-memory matrix descriptor:
-// start>>4 @[0,14), LBO>>4 @[16,30), SBO>>4 @[32,46), version=1 @[46,48), layout type @[61,64);
-// instruction descriptor: c_format @[4,6), a/b_format @[7,10)/[10,13), a/b_major @15/@16,
-// N>>3 @[17,23), M>>4 @[24,29)).  All operands here are K-major, SWIZZLE_NONE ("interleaved" 8x16B
-// core matrices): element (row r, k) of an operand lives at
+// The convolution operands are K-major, SWIZZLE_NONE ("interleaved" 8x16B core matrices): element (row r, k) of an operand
+// lives at
 //     start + (r%8)*16 + (r/8)*SBO + (k/8)*LBO + (k%8)*2        (bf16)
 // which makes arbitrary 16-byte-aligned *shifted views* of a pixel plane legal operands -- the
 // property the implicit-GEMM convolution in conv_umma.cu is built on.
@@ -58,8 +55,6 @@ LFD_DEVINL void mbar_wait(uint64_t* bar, uint32_t parity) {
 
 // ---------------------------------------------------------------- proxies / fences
 LFD_DEVINL void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-LFD_DEVINL void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-LFD_DEVINL void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ---------------------------------------------------------------- programmatic dependent launch
 LFD_DEVINL void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -134,66 +129,120 @@ LFD_DEVINL void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" :::
 template <int N>
 LFD_DEVINL void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 
-// ---------------------------------------------------------------- tcgen05: TMEM alloc
-// cols: power of two in [32, 512]
-LFD_DEVINL void tmem_alloc(uint32_t* slot_in_smem, uint32_t cols) {  // whole warp, .sync.aligned
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)),
-                 "r"(cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-LFD_DEVINL void tmem_dealloc(uint32_t taddr, uint32_t cols) {  // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-
-// ---------------------------------------------------------------- tcgen05: descriptors
-// K-major, no swizzle.  lbo/sbo in bytes (multiples of 16).
-LFD_DEVINL uint64_t umma_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// ---------------------------------------------------------------- wgmma (warpgroup MMA, sm_90a)
+// Shared-memory matrix descriptor, SWIZZLE_NONE: start>>4 @[0,14), LBO>>4 @[16,30), SBO>>4 @[32,46), layout type 0 @[62,64).
+// lbo / sbo in bytes (multiples of 16).  K-major: LBO = stride between the 16-byte K chunks, SBO = between 8-row groups;
+// MN-major: LBO = stride between 8-row K groups, SBO = between 8-element MN chunks.
+LFD_DEVINL uint64_t wgmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-    return d;                // base_offset = 0, lbo_mode = 0, layout_type = SWIZZLE_NONE (0)
+    return d;
 }
-// bf16 x bf16 (or fp16 x fp16) -> fp32, both operands K-major, M = 128, N = n.
-LFD_DEVINL constexpr uint32_t umma_idesc_16(uint32_t m, uint32_t n, bool f16) {
-    return (1u << 4)                    // c_format  = F32
-           | ((f16 ? 0u : 1u) << 7)     // a_format  = F16 (0) / BF16 (1)
-           | ((f16 ? 0u : 1u) << 10)    // b_format
-           | ((n >> 3) << 17)           // N / 8
-           | ((m >> 4) << 24);          // M / 16
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-LFD_DEVINL void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// mbarrier arrives when all previously issued MMAs of this thread have completed.
-LFD_DEVINL void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// ---------------------------------------------------------------- tcgen05: TMEM -> registers
-// 32 lanes x 32-bit, 16 consecutive columns; thread t of warp w reads lane 32*(w%4)+t.
-LFD_DEVINL void tmem_ld16(uint32_t taddr, float* v) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
+LFD_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+LFD_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+LFD_DEVINL void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from touching accumulator registers across wgmma issue / wait
+template <int N>
+LFD_DEVINL void wgmma_fence_regs(float* d) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-LFD_DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], fp32 accumulators in registers of the issuing warpgroup (all 128 threads execute it).
+// Thread t of warp w holds rows 16w + t/4 (+8) and columns 8j + 2(t%4) (+1): d[4j + 2h + e] = (row 16w + t/4 + 8h, column 8j + 2(t%4) + e).
+// ss: both operands in shared memory (TA / TB = 1: MN-major); acc = 0 overwrites D.
+template <int N> struct Wgmma;
+template <> struct Wgmma<16> {
+    template <int TA, int TB>
+    static LFD_DEVINL void ss_bf16(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                     : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+    template <int TA, int TB>
+    static LFD_DEVINL void ss_f16(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                     : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+};
+template <> struct Wgmma<32> {
+    template <int TA, int TB>
+    static LFD_DEVINL void ss_bf16(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                     : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+    template <int TA, int TB>
+    static LFD_DEVINL void ss_f16(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                     : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+};
+template <> struct Wgmma<64> {
+    template <int TA, int TB>
+    static LFD_DEVINL void ss_bf16(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                     : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+    template <int TA, int TB>
+    static LFD_DEVINL void ss_f16(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                     : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+};
+template <> struct Wgmma<128> {
+    template <int TA, int TB>
+    static LFD_DEVINL void ss_bf16(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                     : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+    template <int TA, int TB>
+    static LFD_DEVINL void ss_f16(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                     : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+    }
+};
+LFD_DEVINL void wgmma_rs_n16_bf16(float* d, const uint32_t* a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
+}
+LFD_DEVINL void wgmma_rs_n16_f16(float* d, const uint32_t* a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
+}
+template <int N, bool F16, int TA = 0, int TB = 0>
+LFD_DEVINL void wgmma_ss(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    if (F16) Wgmma<N>::template ss_f16<TA, TB>(d, a, b, acc);
+    else Wgmma<N>::template ss_bf16<TA, TB>(d, a, b, acc);
+}
+// rs: A (64 x 16, K-major) from registers in the accumulator's row / column distribution, packed 16-bit pairs:
+// a[0] = (row, k 2(t%4) ..), a[1] = (row + 8, same k), a[2] = (row, k + 8), a[3] = (row + 8, k + 8)
+template <bool F16>
+LFD_DEVINL void wgmma_rs_n16(float* d, const uint32_t* a, uint64_t b, uint32_t acc) {
+    if (F16) wgmma_rs_n16_f16(d, a, b, acc);
+    else wgmma_rs_n16_bf16(d, a, b, acc);
+}
 
 // ---------------------------------------------------------------- misc
 // Kernel time-line for tests/debug_timeline.py (only with -DLFD_B200_TIMELINE): tl[0] = earliest CTA start, tl[1] = latest CTA end,

@@ -1,6 +1,6 @@
 // train.cu -- the SIMT (HBM-bound) kernels of the training step: parameter staging, BatchNorm batch statistics / apply,
 // BatchNorm / GroupNorm backward, the backward of the final head convs, the stem conv's weight gradient, gradient-norm
-// clipping + SGD.  The GEMM-shaped parts (forward convs, dgrad, wgrad) run on the tensor cores (conv_umma.cu, wgrad_umma.cu).
+// clipping + SGD.  The GEMM-shaped parts (forward convs, dgrad, wgrad) run on the tensor cores (wgmma: conv_umma.cu, wgrad_umma.cu).
 //
 // Reference semantics (what autograd computes for the reference's modules in train mode):
 //   BatchNorm2d      lfd/model/backbone/lfd_resnet.py:10-18 (nn.BatchNorm2d defaults: eps 1e-5, momentum 0.1, biased variance

@@ -103,7 +103,7 @@ cudaError_t head_final_bwd_launch(const HeadFinalBwdParams& p, int num_sms, cuda
 // weight gradients
 // ---------------------------------------------------------------------------------------------------
 struct WgradGeom { int N, H, W, Cin, Ho, Wo, Cout, ksize, stride; };
-// tcgen05 kernel (wgrad_umma.cu): dstage[tap][Cin][Cout] += sum over pixels x_tap[pixel][ci] * dz[pixel][co]
+// wgmma kernel (wgrad_umma.cu): dstage[tap][Cin][Cout] += sum over pixels x_tap[pixel][ci] * dz[pixel][co]
 int wgrad_umma_supported(const WgradGeom& g);
 cudaError_t wgrad_umma_launch(const WgradGeom& g, const __nv_bfloat16* x, const __nv_bfloat16* dz, float* dstage, int num_sms, cudaStream_t st);
 // SIMT cross-check (validation only)

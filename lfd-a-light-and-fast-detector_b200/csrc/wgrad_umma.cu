@@ -1,20 +1,21 @@
-// wgrad_umma.cu -- convolution weight gradient on 5th-gen tensor cores (tcgen05 / TMEM), sm_100a only.
+// wgrad_umma.cu -- convolution weight gradient on Hopper tensor cores (wgmma), sm_90a.
 //
 // Replaces what autograd's conv backward-weights (cuDNN) computes for every nn.Conv2d of the reference's backbone / neck /
 // head towers in training (lfd/model/backbone/lfd_resnet.py:96-154,354-473, neck/simple_neck.py:35-47, head/lfd_head.py:85-135):
 //     dW[tap][ci][co] = sum over (n, oy, ox)  x[n, s*oy + kh - pad, s*ox + kw - pad, ci] * dz[n, oy, ox, co]
 //
 // Formulation: a GEMM whose reduction (K) dimension is the PIXEL index.  With NHWC activations the pixel planes the forward
-// kernel already uses -- plane[8-channel chunk][pixel][16 B] -- are exactly the UMMA *MN-major* SWIZZLE_NONE canonical layout
+// kernel already uses -- plane[8-channel chunk][pixel][16 B] -- are exactly the wgmma *MN-major* SWIZZLE_NONE canonical layout
 // (core matrix = 8 pixels x 16 B, 8 consecutive channels per 16-byte row; LBO = stride between 8-pixel groups = halo row pitch,
 // SBO = stride between 8-channel chunks = plane pitch), so
 //   * the x halo of a 16x8 output tile is loaded ONCE (same producers / tables as conv_umma.cu) and the 9 taps are shifted views;
 //   * the dz tile is loaded as plane[8-channel chunk][128 pixels][16 B] (the N-major B operand);
 //   * one tile = 8 K-steps (16 pixels = two tile rows each) x taps MMAs of M = 64 input channels, N = Cout, K = 16;
-//   * the accumulators D[tap][64 x Cout] stay in TMEM for ALL tiles of the CTA (persistent split-K over pixels) and are
-//     flushed once with vector atomics into the fp32 staging tensor dstage[tap][Cin][Cout].
-// TMEM holds 512 columns: the taps of a 3x3 conv are split into groups of floor(512 / Cout) accumulators handled by different
-// CTAs, and Cin = 128 into two 64-channel chunks (grid = pixel slices x channel chunks x tap groups).
+//   * the accumulators D[tap][64 x Cout] stay in the registers of the two consumer warpgroups (each owns a subset of the taps)
+//     for ALL tiles of the CTA (persistent split-K over pixels) and are flushed once with vector atomics into the fp32
+//     staging tensor dstage[tap][Cin][Cout].
+// A warpgroup holds at most 128 accumulator registers per thread (256 / Cout taps): the taps of a 3x3 conv are split into groups
+// handled by different CTAs, and Cin = 128 into two 64-channel chunks (grid = pixel slices x channel chunks x tap groups).
 #include <stdlib.h>
 
 #include "conv_common.cuh"
@@ -26,7 +27,8 @@ namespace lfd {
 namespace {
 
 constexpr int kWgProd = 128;                       // producer threads
-constexpr int kWgThreads = 128 + 32 + kWgProd;     // 4 epilogue warps | MMA warp | 4 producer warps
+constexpr int kWgConsumers = 256;                  // two warpgroups
+constexpr int kWgThreads = kWgConsumers + kWgProd;
 constexpr int kWgMaxStages = 4;
 constexpr uint32_t kWgBPitch = 129 * 16;           // pitch between the 8-channel planes of the dz tile (odd multiple of 16 B)
 
@@ -42,23 +44,16 @@ struct alignas(16) WgradParams {
     unsigned long long magic_tpi, magic_tx;
     int n_px, Cc, log2_cpc, log2_cpo;
     int n_cich, n_tapg, taps_per_group, n_taps, grid_tiles;
-    int stages, tmem_cols, interleave;
-    int pair;                   // swizzled 3x3: TWO taps per accumulator -- an M = 128 operand whose second 64-row group (LBO) is the next tap's shifted view
-    int sw;                     // 1: operands in the 128-byte-swizzled MN-major layout ([pixel slot][64 channels = 128 B], 16-byte chunk ^ (slot & 7))
-    int sw_base_mode;           // descriptor base_offset of shifted (tap) views: 1 = 0 (measured correct: the tensor core swizzles on ABSOLUTE shared-memory
-                                // address bits, so a 128-byte-aligned shifted view of a 1024-byte-aligned swizzled buffer needs no phase), 0 = (start >> 7) & 7 (wrong, kept as the experiment)
-    int row_slots;              // pixel slots per halo row (3x3/s1: 16 in the swizzled layout so that every 8-pixel K group starts a swizzle period)
-    uint32_t b_group_bytes;     // swizzled dz tile: bytes between the 64-channel groups
+    int stages;
     uint32_t a_plane_pitch, a_row_pitch, a_stage_bytes, stage_bytes;
     uint32_t smem_table_off, smem_ring_off;
 };
 
-LFD_DEVINL int wg_fast_div(int x, uint64_t magic) { return (int)(((uint64_t)(uint32_t)x * magic) >> 40); }
+// taps one consumer warpgroup accumulates: 128 registers per thread of m64 x Cout accumulators
+template <int MODE, int COUT>
+struct WgTaps { static constexpr int value = (MODE == MODE_3X3S1 || MODE == MODE_3X3S2) ? (256 / COUT < 9 ? 256 / COUT : 9) : 1; };
 
-// MN-major operands on both sides: a_major (bit 15) = b_major (bit 16) = 1
-LFD_DEVINL constexpr uint32_t wg_idesc(uint32_t m, uint32_t n) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
+LFD_DEVINL int wg_fast_div(int x, uint64_t magic) { return (int)(((uint64_t)(uint32_t)x * magic) >> 40); }
 
 template <int MODE>
 LFD_DEVINL constexpr int wg_tap_view(int tap) {   // pixel-slot offset of tap's shifted view (same planes as conv_umma.cu)
@@ -70,30 +65,12 @@ LFD_DEVINL constexpr int wg_tap_view(int tap) {   // pixel-slot offset of tap's 
     return 0;
 }
 
-// 128-byte-swizzled MN-major operand: start>>4 | LBO (64-channel group stride) | SBO (8-pixel group stride) | version | base offset | SWIZZLE_128B
-LFD_DEVINL uint64_t wg_sw_desc(uint32_t start, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t base_off) {
-    uint64_t d = 0;
-    d |= (uint64_t)((start >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)(base_off & 7) << 49;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
-LFD_DEVINL void red_add_v4(float* addr, const float* v) {
-    atomicAdd(reinterpret_cast<float4*>(addr), make_float4(v[0], v[1], v[2], v[3]));
-}
-
-template <int MODE>
+template <int MODE, int COUT>
 __global__ void __launch_bounds__(kWgThreads, 1) wgrad_umma_kernel(const __grid_constant__ WgradParams p) {
-    constexpr int TAPS = (MODE == MODE_3X3S1 || MODE == MODE_3X3S2) ? 9 : 1;
-    extern __shared__ __align__(1024) uint8_t smem[];      // 1024 B = the period of the 128-byte swizzle
+    constexpr int TPW = WgTaps<MODE, COUT>::value;
+    extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t* full = reinterpret_cast<uint64_t*>(smem);
     uint64_t* empty = full + kWgMaxStages;
-    uint64_t* done = empty + kWgMaxStages;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done + 1);
     WgEntry* table = reinterpret_cast<WgEntry*>(smem + p.smem_table_off);
     WgDelta* delta = reinterpret_cast<WgDelta*>(smem + p.smem_table_off + (size_t)p.n_px * sizeof(WgEntry));
     uint8_t* ring = smem + p.smem_ring_off;
@@ -108,11 +85,9 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_umma_kernel(const __grid_
     const int SA = p.stages;
 
     if (tid == 0) {
-        for (int i = 0; i < SA; ++i) { mbar_init(&full[i], kWgProd); mbar_init(&empty[i], 1); }
-        mbar_init(done, 1);
+        for (int i = 0; i < SA; ++i) { mbar_init(&full[i], kWgProd); mbar_init(&empty[i], kWgConsumers / 32); }
         fence_mbar_init();
     }
-    if (warp == 4) tmem_alloc(tmem_slot, p.tmem_cols);
     if (MODE != MODE_FLAT) {
         for (int i = tid; i < p.n_px; i += kWgThreads) {
             int dy, dx, slot;
@@ -136,141 +111,81 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_umma_kernel(const __grid_
             delta[i] = d;
         }
     }
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
     const int HW = p.H * p.W, HoWo = p.Ho * p.Wo;
 
-    if (warp < 4) {
-        // ============================================================== EPILOGUE (once, after the last tile)
-        mbar_wait(done, 0);
-        tc_fence_after_sync();
-        // M = 64 accumulators occupy lanes 16q .. 16q+15 of every 32-lane quarter q (row r -> lane (r % 16) + 32 * (r / 16));
-        // with `interleave` the odd taps sit in the other half (lanes + 16) of the same columns.
-        const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-        if (p.pair) {
-            // M = 128 accumulators: lane = row; rows 0..63 = tap 2a, rows 64..127 = tap 2a + 1 (a trailing single tap uses the M = 64 layout)
-            const int nacc = (ntap + 1) / 2;
-            for (int a = 0; a < nacc; ++a) {
-                const bool single = 2 * a + 1 >= ntap;
-                int t, ci;
-                bool act;
-                if (single) { t = 2 * a; ci = cich * 64 + warp * 16 + (lane & 15); act = lane < 16; }
-                else { t = 2 * a + (warp >> 1); ci = cich * 64 + (warp & 1) * 32 + lane; act = true; }
-                act = act && ci < p.Cin;
-                float* dst = p.dstage + ((size_t)(tap0 + t) * p.Cin + ci) * p.Cout;
-                for (int c0 = 0; c0 < p.Cout; c0 += 16) {
-                    float v[16];
-                    tmem_ld16(tmem_base + lane_base + (uint32_t)(a * p.Cout + c0), v);
-                    tmem_ld_wait();
-                    if (act) {
-                        red_add_v4(dst + c0, v); red_add_v4(dst + c0 + 4, v + 4);
-                        red_add_v4(dst + c0 + 8, v + 8); red_add_v4(dst + c0 + 12, v + 12);
-                    }
-                }
-            }
-        } else {
-        const int row = warp * 16 + (lane & 15);
-        const int ci = cich * 64 + row;
-        const int nacc = p.interleave ? (ntap + 1) / 2 : ntap;
-        for (int a = 0; a < nacc; ++a) {
-            const int t = p.interleave ? 2 * a + (lane >> 4) : a;
-            const bool act = (p.interleave || lane < 16) && t < ntap && ci < p.Cin;
-            float* dst = p.dstage + ((size_t)(tap0 + t) * p.Cin + ci) * p.Cout;
-            for (int c0 = 0; c0 < p.Cout; c0 += 16) {
-                float v[16];
-                tmem_ld16(tmem_base + lane_base + (uint32_t)(a * p.Cout + c0), v);
-                tmem_ld_wait();
-                if (act) {
-                    red_add_v4(dst + c0, v); red_add_v4(dst + c0 + 4, v + 4);
-                    red_add_v4(dst + c0 + 8, v + 8); red_add_v4(dst + c0 + 12, v + 12);
-                }
-            }
-        }
-        }
-        tc_fence_before_sync();
-    } else if (warp == 4) {
-        // ============================================================== MMA ISSUER
-        const uint32_t idesc = wg_idesc(64, p.Cout);
+    if (warp < kWgConsumers / 32) {
+        // ============================================================== CONSUMERS: MMAs, then one flush of the accumulators
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
+        const int wg = warp >> 2;
+        // this warpgroup's taps: the first or the second half of the CTA's tap group
+        const int half = (ntap + 1) / 2;
+        const int t_lo = wg * half, t_n = min(ntap, t_lo + half) - t_lo;
         // MN-major SWIZZLE_NONE: LBO = byte stride between 8-element K groups (pixels), SBO = between 8-element MN chunks (channels)
-        const uint64_t adesc0 = umma_smem_desc(0, p.a_row_pitch, p.a_plane_pitch);
-        const uint64_t bdesc0 = umma_smem_desc(0, 128, kWgBPitch);
+        const uint64_t adesc0 = wgmma_desc(0, p.a_row_pitch, p.a_plane_pitch);
+        const uint64_t bdesc0 = wgmma_desc(0, 128, kWgBPitch);
         const uint32_t a_kstep = (2 * p.a_row_pitch) >> 4;    // one K = 16 step = two tile rows
+        float acc[TPW][COUT / 2];
+#pragma unroll
+        for (int t = 0; t < TPW; ++t)
+#pragma unroll
+            for (int i = 0; i < COUT / 2; ++i) acc[t][i] = 0.f;
         uint32_t it = 0;
-        bool first = true;
         for (int tile = slice; tile < p.num_tiles; tile += p.grid_tiles, ++it) {
             const uint32_t s = it % SA, ph = (it / SA) & 1;
             mbar_wait(&full[s], ph);
-            tc_fence_after_sync();
-            fence_proxy_async_smem();
+            fence_proxy_async_smem();   // cp.async (generic proxy) writes -> wgmma (async proxy) reads
             const uint32_t a_base = smem_u32(ring) + s * p.stage_bytes;
             const uint32_t b_base = a_base + p.a_stage_bytes;
             const uint64_t ad = adesc0 + (a_base >> 4), bd = bdesc0 + (b_base >> 4);
-            if (elect_one_sync()) {
-                if (p.sw) {
-                    const uint32_t sbo_a = (uint32_t)p.row_slots * 128u;
-                    for (int kg = 0; kg < 8; ++kg) {
-                        const uint32_t b_start = b_base + (uint32_t)kg * 2048u;
-                        const uint64_t bdesc = wg_sw_desc(b_start, p.b_group_bytes, 1024u, 0u);
-                        if (p.pair) {
-                            for (int q = 0; 2 * q < ntap; ++q) {
-                                const int t0 = tap0 + 2 * q, t1 = t0 + 1;
-                                const bool two = 2 * q + 1 < ntap;
-                                const uint32_t v0 = (uint32_t)((t0 / 3) * p.row_slots + t0 % 3), v1 = (uint32_t)((t1 / 3) * p.row_slots + t1 % 3);
-                                const uint32_t a_start = a_base + (v0 + (uint32_t)(kg * 2 * p.row_slots)) * 128u;
-                                // second 64-row group of the M = 128 operand = the next tap's view of the same halo: LBO = distance of the two views
-                                const uint64_t adesc = wg_sw_desc(a_start, two ? (v1 - v0) * 128u : 16u, sbo_a, 0u);
-                                umma_bf16(tmem_base + (uint32_t)(q * p.Cout), adesc, bdesc, two ? wg_idesc(128, p.Cout) : idesc, (first && kg == 0) ? 0u : 1u);
-                            }
-                            continue;
-                        }
 #pragma unroll
-                        for (int t = 0; t < TAPS; ++t) {
-                            if (t >= ntap) break;
-                            const int tap = tap0 + t;
-                            const uint32_t view = TAPS == 1 ? 0u : (uint32_t)((tap / 3) * p.row_slots + tap % 3);
-                            const uint32_t a_start = a_base + (view + (uint32_t)(kg * 2 * p.row_slots)) * 128u;
-                            const uint64_t adesc = wg_sw_desc(a_start, 16u, sbo_a, p.sw_base_mode ? 0u : (a_start >> 7));
-                            const uint32_t d = p.interleave ? tmem_base + (uint32_t)((t >> 1) * p.Cout) + ((uint32_t)((t & 1) * 16) << 16)
-                                                            : tmem_base + (uint32_t)(t * p.Cout);
-                            umma_bf16(d, adesc, bdesc, idesc, (first && kg == 0) ? 0u : 1u);
+            for (int t = 0; t < TPW; ++t) wgmma_fence_regs<COUT / 2>(acc[t]);
+            wgmma_fence();
+            for (int kg = 0; kg < 8; ++kg) {
+                const uint64_t adk = ad + (uint32_t)(kg * a_kstep), bdk = bd + (uint32_t)(kg * 16);
+#pragma unroll
+                for (int t = 0; t < TPW; ++t) {
+                    if (t >= t_n) break;
+                    // tap_view needs a compile-time tap for the 3x3/s2 formula: switch on the run-time tap
+                    uint32_t view;
+                    if (TPW == 1 && MODE != MODE_3X3S1 && MODE != MODE_3X3S2) view = 0;
+                    else {
+                        switch (tap0 + t_lo + t) {
+                            case 0: view = wg_tap_view<MODE>(0); break; case 1: view = wg_tap_view<MODE>(1); break;
+                            case 2: view = wg_tap_view<MODE>(2); break; case 3: view = wg_tap_view<MODE>(3); break;
+                            case 4: view = wg_tap_view<MODE>(4); break; case 5: view = wg_tap_view<MODE>(5); break;
+                            case 6: view = wg_tap_view<MODE>(6); break; case 7: view = wg_tap_view<MODE>(7); break;
+                            default: view = wg_tap_view<MODE>(8); break;
                         }
                     }
-                } else
-                for (int kg = 0; kg < 8; ++kg) {
-                    const uint64_t adk = ad + (uint32_t)(kg * a_kstep), bdk = bd + (uint32_t)(kg * 16);
-#pragma unroll
-                    for (int t = 0; t < TAPS; ++t) {
-                        if (t >= ntap) break;
-                        const uint32_t d = p.interleave ? tmem_base + (uint32_t)((t >> 1) * p.Cout) + ((uint32_t)((t & 1) * 16) << 16)
-                                                        : tmem_base + (uint32_t)(t * p.Cout);
-                        // tap_view needs a compile-time tap for the 3x3/s2 formula: tap0 is a multiple of taps_per_group, switch on it
-                        uint32_t view;
-                        if (TAPS == 1) view = 0;
-                        else {
-                            const int tap = tap0 + t;
-                            switch (tap) {
-                                case 0: view = wg_tap_view<MODE>(0); break; case 1: view = wg_tap_view<MODE>(1); break;
-                                case 2: view = wg_tap_view<MODE>(2); break; case 3: view = wg_tap_view<MODE>(3); break;
-                                case 4: view = wg_tap_view<MODE>(4); break; case 5: view = wg_tap_view<MODE>(5); break;
-                                case 6: view = wg_tap_view<MODE>(6); break; case 7: view = wg_tap_view<MODE>(7); break;
-                                default: view = wg_tap_view<MODE>(8); break;
-                            }
-                        }
-                        umma_bf16(d, adk + view, bdk, idesc, (first && kg == 0) ? 0u : 1u);
-                    }
+                    wgmma_ss<COUT, false, 1, 1>(acc[t], adk + view, bdk, 1u);
                 }
-                umma_commit(&empty[s]);
             }
+            wgmma_commit();
+            wgmma_wait<0>();
+#pragma unroll
+            for (int t = 0; t < TPW; ++t) wgmma_fence_regs<COUT / 2>(acc[t]);
             __syncwarp();
-            first = false;
+            if (lane == 0) mbar_arrive(&empty[s]);
         }
-        if (elect_one_sync()) umma_commit(done);
-        __syncwarp();
+        // flush: thread holds rows (input channels) r0, r0 + 8 and columns (output channels) 8j + 2 (lane % 4) (+1)
+        const int r0 = (warp & 3) * 16 + (lane >> 2), tq = lane & 3;
+#pragma unroll
+        for (int t = 0; t < TPW; ++t) {
+            if (t >= t_n) break;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int ci = cich * 64 + r0 + 8 * h;
+                if (ci >= p.Cin) continue;
+                float* dst = p.dstage + ((size_t)(tap0 + t_lo + t) * p.Cin + ci) * COUT + 2 * tq;
+#pragma unroll
+                for (int j = 0; j < COUT / 8; ++j) atomicAdd(reinterpret_cast<float2*>(dst + 8 * j), make_float2(acc[t][4 * j + 2 * h], acc[t][4 * j + 2 * h + 1]));
+            }
+        }
     } else {
         // ============================================================== PRODUCERS
-        const int ptid = tid - 160;
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+        const int ptid = tid - kWgConsumers;
         const int cpc = p.Cc >> 3;
         const int ch = ptid & (cpc - 1);
         const int px0 = ptid >> p.log2_cpc;
@@ -304,26 +219,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_umma_kernel(const __grid_
             const bool interior = MODE == MODE_FLAT ? (ix0 + 128 <= HW)
                                                     : (iy0 + kDyMin >= 0 && ix0 + kDxMin >= 0 && iy0 + kDyMax < p.H && ix0 + kDxMax < p.W);
             const uint32_t dst_cc = a_base + ch_dst;
-            // swizzled layout: slot s, chunk ch at a_base + s * 128 + ((ch ^ (s & 7)) << 4); halo rows of the 3x3/s1 mode are 16 slots apart
-            auto sw_dst = [&](uint32_t slot) -> uint32_t { return a_base + (slot << 7) + (((uint32_t)ch ^ (slot & 7u)) << 4); };
-            if (p.sw && MODE == MODE_FLAT) {
-#pragma unroll 4
-                for (int pxi = px0; pxi < 128; pxi += pstep) {
-                    const int q = ix0 + pxi;
-                    const bool ok = q < HW;
-                    cp_async16(sw_dst((uint32_t)pxi), img + (size_t)(ok ? q : 0) * p.Cin, ok);
-                }
-            } else if (p.sw) {
-#pragma unroll 2
-                for (int pxi = px0; pxi < p.n_px; pxi += pstep) {
-                    const WgDelta pd = delta[pxi];
-                    const int y = iy0 + pd.dy, x = ix0 + pd.dx;
-                    const bool ok = ((unsigned)y < (unsigned)p.H) && ((unsigned)x < (unsigned)p.W);
-                    uint32_t slot = table[pxi].dst_off >> 4;
-                    if (MODE == MODE_3X3S1) slot = (slot / 10u) * 16u + slot % 10u;      // row pitch 10 -> 16
-                    cp_async16(sw_dst(slot), img + (size_t)(ok ? (y * p.W + x) : 0) * p.Cin, ok);
-                }
-            } else if (MODE == MODE_FLAT) {
+            if (MODE == MODE_FLAT) {
 #pragma unroll 4
                 for (int pxi = px0; pxi < 128; pxi += pstep) {
                     const int q = ix0 + pxi;
@@ -360,21 +256,13 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_umma_kernel(const __grid_
                     ok = oy < p.Ho && ox < p.Wo;
                     q = oy * p.Wo + ox;
                 }
-                const uint32_t bd_ = p.sw ? a_base + p.a_stage_bytes + (uint32_t)(chb >> 3) * p.b_group_bytes + ((uint32_t)sl << 7) + ((((uint32_t)chb & 7u) ^ ((uint32_t)sl & 7u)) << 4)
-                                          : b_dst + sl * 16;
-                cp_async16(bd_, dzi + (size_t)(ok ? q : 0) * p.Cout, ok);
+                cp_async16(b_dst + sl * 16, dzi + (size_t)(ok ? q : 0) * p.Cout, ok);
             }
             cp_async_mbar_arrive(&full[s]);
         }
         cp_async_wait_all();
     }
 
-    tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 4) {
-        tc_fence_after_sync();
-        tmem_dealloc(tmem_base, p.tmem_cols);
-    }
 }
 
 int wg_mode_of(const WgradGeom& g) {
@@ -417,58 +305,19 @@ int wg_configure(const WgradGeom& g, int num_sms, WgradParams* out, size_t* smem
     if ((1 << p.log2_cpo) != g.Cout / 8) return -2;           // Cout in {16, 32, 64, 128}
     p.n_cich = (g.Cin + 63) / 64;
     p.n_taps = g.ksize * g.ksize;
-    static const int use_il = getenv("LFD_B200_WGRAD_INTERLEAVE") ? atoi(getenv("LFD_B200_WGRAD_INTERLEAVE")) : 0;
-    p.interleave = use_il && p.n_taps > 1;
-    const int acc_per_cta = (512 / g.Cout) * (p.interleave ? 2 : 1);
-    p.n_tapg = (p.n_taps + acc_per_cta - 1) / acc_per_cta;
+    // two warpgroups of (at most) 256 / Cout taps per CTA; the groups are balanced (e.g. Cout = 64: 5 + 4 taps, not 8 + 1)
+    const int per_wg = p.n_taps == 1 ? 1 : (256 / g.Cout < 9 ? 256 / g.Cout : 9);
+    const int max_group = 2 * per_wg;
+    p.n_tapg = (p.n_taps + max_group - 1) / max_group;
     p.taps_per_group = (p.n_taps + p.n_tapg - 1) / p.n_tapg;
-    if (p.interleave && (p.taps_per_group & 1) && p.n_tapg > 1) p.taps_per_group += 1;   // groups start on an even tap
-    p.n_tapg = (p.n_taps + p.taps_per_group - 1) / p.taps_per_group;
-    {
-        const int need = (p.interleave ? (p.taps_per_group + 1) / 2 : p.taps_per_group) * g.Cout;
-        int cols = 32;
-        while (cols < need) cols <<= 1;
-        if (cols > 512) return -6;
-        p.tmem_cols = cols;
-    }
     // the A stage always provides the 8 planes an M = 64 operand addresses (Cin = 32: the upper 4 are never written, their
     // accumulator rows are never read)
     p.a_stage_bytes = (uint32_t)((8 * (size_t)p.a_plane_pitch + 127) & ~(size_t)127);
-    uint32_t b_stage = (uint32_t)((((size_t)g.Cout / 8) * kWgBPitch + 127) & ~(size_t)127);
-    p.row_slots = row_slots;
-    // 128-byte-swizzled operands (the transposing read path of the tensor core is bank-conflict free only in the swizzled layouts: the
-    // SWIZZLE_NONE kernel measures ~225 clk per M64 N64 K16 MMA).  Needs 64-channel rows and 8-pixel K groups that start a swizzle period:
-    // flat tiles (8 slots per row) and 3x3/s1 halos re-pitched to 16 slots per row; the 3x3/s2 parity planes (pitch 9) keep SWIZZLE_NONE.
-    static const int use_sw = getenv("LFD_B200_WGRAD_SW") ? atoi(getenv("LFD_B200_WGRAD_SW")) : 1;
-    static const int sw_base = getenv("LFD_B200_WGRAD_SW_BASE") ? atoi(getenv("LFD_B200_WGRAD_SW_BASE")) : 1;
-    p.sw = use_sw && mode != MODE_3X3S2 && g.Cin % 64 == 0 && (g.Cout == 64 || g.Cout == 128);
-    p.sw_base_mode = sw_base;
-    static const int use_pair = getenv("LFD_B200_WGRAD_PAIR") ? atoi(getenv("LFD_B200_WGRAD_PAIR")) : 1;
-    p.pair = p.sw && use_pair && mode == MODE_3X3S1;
-    if (p.pair) {      // two taps per accumulator: regroup the taps (groups start on an even tap)
-        p.interleave = 0;
-        const int acc_cols = 512 / g.Cout;                      // accumulators per CTA
-        p.taps_per_group = 2 * acc_cols < p.n_taps ? 2 * acc_cols : p.n_taps;
-        p.n_tapg = (p.n_taps + p.taps_per_group - 1) / p.taps_per_group;
-        if (p.n_tapg > 1) {                                     // balance: e.g. Cout = 128: 4 accumulators -> groups of 6 + 3 taps
-            p.taps_per_group = ((p.n_taps + p.n_tapg - 1) / p.n_tapg + 1) & ~1;
-            p.n_tapg = (p.n_taps + p.taps_per_group - 1) / p.taps_per_group;
-        }
-        int cols = 32;
-        while (cols < ((p.taps_per_group + 1) / 2) * g.Cout) cols <<= 1;
-        p.tmem_cols = cols;
-    }
-    if (p.sw) {
-        if (mode == MODE_3X3S1) p.row_slots = 16;
-        const int slots = mode == MODE_3X3S1 ? 18 * 16 : 128;
-        p.a_stage_bytes = (uint32_t)(slots * 128);              // multiples of 1024
-        p.b_group_bytes = 128 * 128;
-        b_stage = (uint32_t)(g.Cout / 64) * p.b_group_bytes;
-    }
+    const uint32_t b_stage = (uint32_t)((((size_t)g.Cout / 8) * kWgBPitch + 127) & ~(size_t)127);
     p.stage_bytes = p.a_stage_bytes + b_stage;
     p.smem_table_off = 512;
     const size_t table_bytes = mode == MODE_FLAT ? 0 : (((size_t)p.n_px * 10 + 127) & ~(size_t)127);
-    p.smem_ring_off = (uint32_t)((512 + table_bytes + 1023) & ~(size_t)1023);      // 1024-aligned: the swizzle period
+    p.smem_ring_off = (uint32_t)((512 + table_bytes + 1023) & ~(size_t)1023);
     const size_t budget = 226 * 1024;
     int st = (int)((budget - p.smem_ring_off) / p.stage_bytes);
     if (st > kWgMaxStages) st = kWgMaxStages;
@@ -485,18 +334,29 @@ int wg_configure(const WgradGeom& g, int num_sms, WgradParams* out, size_t* smem
     return 0;
 }
 
-template <int MODE>
-cudaError_t wg_launch_mode(const WgradParams& p, size_t smem, int grid, cudaStream_t st) {
+template <int MODE, int COUT>
+cudaError_t wg_launch_t(const WgradParams& p, size_t smem, int grid, cudaStream_t st) {
     static bool configured[kMaxDevices] = {};
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
     if (!configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(wgrad_umma_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+        cudaError_t e = cudaFuncSetAttribute(wgrad_umma_kernel<MODE, COUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
         if (e != cudaSuccess) return e;
         configured[dev] = true;
     }
-    wgrad_umma_kernel<MODE><<<grid, kWgThreads, smem, st>>>(p);
+    wgrad_umma_kernel<MODE, COUT><<<grid, kWgThreads, smem, st>>>(p);
     return cudaGetLastError();
+}
+
+template <int MODE>
+cudaError_t wg_launch_mode(const WgradParams& p, size_t smem, int grid, cudaStream_t st) {
+    switch (p.Cout) {
+        case 16: return wg_launch_t<MODE, 16>(p, smem, grid, st);
+        case 32: return wg_launch_t<MODE, 32>(p, smem, grid, st);
+        case 64: return wg_launch_t<MODE, 64>(p, smem, grid, st);
+        case 128: return wg_launch_t<MODE, 128>(p, smem, grid, st);
+    }
+    return cudaErrorInvalidValue;
 }
 
 }  // namespace
@@ -505,14 +365,14 @@ int wgrad_umma_supported(const WgradGeom& g) {
     WgradParams p;
     size_t smem;
     int grid;
-    return wg_configure(g, 148, &p, &smem, &grid) == 0;
+    return wg_configure(g, 132, &p, &smem, &grid) == 0;
 }
 
 cudaError_t wgrad_umma_launch(const WgradGeom& g, const __nv_bfloat16* x, const __nv_bfloat16* dz, float* dstage, int num_sms, cudaStream_t st) {
     WgradParams p;
     size_t smem = 0;
     int grid = 0;
-    if (wg_configure(g, num_sms > 0 ? num_sms : 148, &p, &smem, &grid)) return cudaErrorInvalidValue;
+    if (wg_configure(g, num_sms > 0 ? num_sms : 132, &p, &smem, &grid)) return cudaErrorInvalidValue;
     p.x = x; p.dz = dz; p.dstage = dstage;
     switch (p.mode) {
         case MODE_FLAT: return wg_launch_mode<MODE_FLAT>(p, smem, grid, st);

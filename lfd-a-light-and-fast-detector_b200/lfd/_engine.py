@@ -1,6 +1,6 @@
 # -*- coding: utf-8 -*-
 """Layer-plan builder: walks an lfd.model.LFD module tree once per (batch, height, width), folds BatchNorm
-into per-channel scale/shift, packs conv weights into the tcgen05 kernel's operand order, lays the bf16 NHWC
+into per-channel scale/shift, packs conv weights into the wgmma kernel's operand order, lays the bf16 NHWC
 activations out in one workspace with liveness-based reuse, and hands the op list to liblfd_b200.so
 (lfd_plan_create / lfd_plan_forward).
 
@@ -189,7 +189,7 @@ class InferencePlan(object):
 
     def _emit_stem0(self, conv, norm, relu, out_name, h, w, tail=None):
         if conv.in_channels != 3 or conv.kernel_size != (3, 3) or conv.stride != (2, 2):
-            raise NotImplementedError('the B200 stem kernel handles the 3x3/s2 conv on a 3-channel image only')
+            raise NotImplementedError('the H100 stem kernel handles the 3x3/s2 conv on a 3-channel image only')
         ho, wo = _conv_out(h, 3, 2), _conv_out(w, 3, 2)
         scale, shift = self._fold(conv, norm)
         wt = pack_stem_weight(fold_scale(conv.weight, scale), self.tdtype)
@@ -205,7 +205,7 @@ class InferencePlan(object):
         k, s = conv.kernel_size[0], conv.stride[0]
         if conv.kernel_size[0] != conv.kernel_size[1] or k not in (1, 3) or s not in (1, 2) or conv.padding[0] != k // 2 \
                 or conv.groups != 1 or conv.dilation != (1, 1):
-            raise NotImplementedError('unsupported conv geometry for the B200 kernels: %r' % (conv,))
+            raise NotImplementedError('unsupported conv geometry for the H100 kernels: %r' % (conv,))
         cin, cout = conv.in_channels, conv.out_channels
         ho, wo = _conv_out(h, k, s), _conv_out(w, k, s)
         q = nat.conv_query(self.N, h, w, cin, ho, wo, cout, k, s, tail[0].out_channels if tail is not None else 0,
@@ -264,7 +264,7 @@ class InferencePlan(object):
         if len(taps) != head._num_heads:
             raise ValueError('backbone taps (%d) and head levels (%d) differ' % (len(taps), head._num_heads))
         if make_norm_probe(head) is not None and not isinstance(make_norm_probe(head), nn.GroupNorm):
-            raise NotImplementedError('the B200 head kernels implement GroupNorm towers and towers without norm layers (the shipped configs)')
+            raise NotImplementedError('the H100 head kernels implement GroupNorm towers and towers without norm layers (the shipped configs)')
         # point offsets need every level size up front: strides are fixed by the stage index
         sizes, hh, ww = {}, h, w
         for si, stage in enumerate(bb.stages()):

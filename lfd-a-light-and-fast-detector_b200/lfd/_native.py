@@ -1,7 +1,7 @@
 # -*- coding: utf-8 -*-
 """ctypes binding of liblfd_b200.so (C-ABI declared in include/lfd_b200.h).
 
-The library is built in-tree by ../build.py (nvcc, sm_100a).  Loading never falls back to anything else:
+The library is built in-tree by ../build.py (nvcc, sm_90a).  Loading never falls back to anything else:
 if the shared object is missing and cannot be built, importing a native entry point raises.
 """
 import ctypes as C

@@ -1,7 +1,7 @@
 # -*- coding: utf-8 -*-
 """Native training step of the LFD conv stack: forward in train mode (BatchNorm batch statistics), backward (data and weight
 gradients of every conv, BatchNorm / GroupNorm / ReLU / residual backward, final head convs + Scale) -- all hand-written
-sm_100a kernels behind liblfd_b200.so (lfd_train_plan_*), driven by two op lists built here from the module tree.
+sm_90a kernels behind liblfd_b200.so (lfd_train_plan_*), driven by two op lists built here from the module tree.
 
 Replaces what the reference gets from autograd over its nn.Module graph in `Executor.train` (lfd/execution/executor.py:185-214:
 `model(x)` ... `loss.backward()`), i.e. LFD.forward in train mode (lfd/model/lfd.py:511-542) and its backward.
@@ -10,7 +10,7 @@ Data layout: activations and their gradients bf16 NHWC in ONE workspace (every f
 parameters, gradients and BatchNorm running statistics are fp32 torch tensors -- all parameters are views into ONE flat
 buffer (`FlatParameters`), all gradients views into one flat gradient buffer, so that the gradient all-reduce and the fused
 clip + SGD step (lfd/execution/optim.py) are single calls.  Per step the fp32 master weights are re-staged as bf16 tensor-core
-operands (PACK), weight gradients are accumulated in fp32 staging tensors by the tcgen05 wgrad kernel and scattered into the
+operands (PACK), weight gradients are accumulated in fp32 staging tensors by the wgmma wgrad kernel and scattered into the
 OIHW gradient tensors at the end (UNPACK).
 
 Rounding points (bf16 training): conv output z (fp32 accumulate) -> bf16; BatchNorm statistics over the stored z (fp64 sums);
@@ -45,7 +45,7 @@ class FlatParameters(object):
             raise ValueError('module without parameters')
         dev = params[0].device
         if dev.type != 'cuda' and not allow_cpu:      # allow_cpu: host-side planning only (CPU tests of the planner)
-            raise RuntimeError('lfd_b200 has no CPU path: move the model to a CUDA (B200) device before training')
+            raise RuntimeError('lfd_b200 has no CPU path: move the model to a CUDA (H100) device before training')
         for p in params:
             if p.dtype != torch.float32 or p.device != dev:
                 raise TypeError('native training keeps fp32 master parameters on one device')
@@ -181,7 +181,7 @@ class TrainPlan(object):
         """conv (no bias) -> BatchNorm (batch statistics) -> (+res) -> ReLU.  x = None: the stem conv on the image."""
         k, s = conv.kernel_size[0], conv.stride[0]
         if conv.kernel_size[0] != conv.kernel_size[1] or k not in (1, 3) or s not in (1, 2) or conv.padding[0] != k // 2:
-            raise NotImplementedError('unsupported conv geometry for the B200 kernels: %r' % (conv,))
+            raise NotImplementedError('unsupported conv geometry for the H100 kernels: %r' % (conv,))
         if conv.bias is not None or not isinstance(norm, nn.BatchNorm2d):
             raise NotImplementedError('native training implements conv(bias=False) + BatchNorm2d for backbone / neck layers')
         cin, cout = conv.in_channels, conv.out_channels
@@ -392,7 +392,7 @@ class TrainPlan(object):
         conv, geo, x = L['conv'], L['geo'], L['x']
         gs = self._gstage_of(conv)
         if x is None:
-            x27 = self._act('stem_im2col', geo['Ho'], geo['Wo'], 32)      # scratch of the im2col + tcgen05 path
+            x27 = self._act('stem_im2col', geo['Ho'], geo['Wo'], 32)      # scratch of the im2col + wgmma path
             self._bwd.append(dict(kind=nat.TOP_WGRAD_STEM, impl=nat.WGRAD_UMMA, off={0: x27, 1: dz, 5: gs}, **geo))
             return
         self._bwd.append(dict(kind=nat.TOP_WGRAD, impl=nat.WGRAD_UMMA, off={0: x, 1: dz, 5: gs}, **geo))

@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""Data parallelism for the B200 build: one process per GPU (torch.distributed, NCCL over NVLink; gloo in the CPU tests)
+"""Data parallelism for the H100 build: one process per GPU (torch.distributed, NCCL over NVLink; gloo in the CPU tests)
 instead of the reference's single-process `nn.DataParallel` (lfd/execution/executor.py:39).
 
 Inference shards the batch across ranks with no collective.  Training reduces gradients with ONE all-reduce over a single

@@ -85,7 +85,7 @@ def set_random_seed(seed, deterministic=False):
 
 
 def set_cudnn_backend(benchmark=True, deterministic=False):
-    """Kept for config-script compatibility; the B200 path does not go through cuDNN."""
+    """Kept for config-script compatibility; the H100 path does not go through cuDNN."""
     torch.backends.cudnn.benchmark = bool(benchmark)
     torch.backends.cudnn.deterministic = bool(deterministic)
 

@@ -26,7 +26,7 @@ def make_activation(activation_cfg):
     cfg = dict(activation_cfg)
     kind = cfg.pop('type')
     if kind != 'ReLU':
-        raise NotImplementedError('only ReLU is fused into the B200 kernels (got %r)' % (kind,))
+        raise NotImplementedError('only ReLU is fused into the H100 kernels (got %r)' % (kind,))
     return nn.ReLU(**cfg)
 
 

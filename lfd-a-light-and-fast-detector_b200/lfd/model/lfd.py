@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""LFD -- drop-in for the reference detector class (lfd/model/lfd.py:15-655) on B200.
+"""LFD -- drop-in for the reference detector class (lfd/model/lfd.py:15-655) on H100.
 
 Same constructor kwargs, state_dict keys and public methods (`forward`, `get_loss`, `get_results`,
 `predict_for_single_image`, `generate_point_coordinates`, `annotation_to_target`, `distance2bbox`,
@@ -10,9 +10,9 @@ Same constructor kwargs, state_dict keys and public methods (`forward`, `get_los
     annotation_to_target      -> lfd_assign_targets    (label assignment on device)
     get_loss                  -> lfd_assign_targets + lfd_detection_loss (loss + gradients w.r.t. the outputs)
 
-There is no CPU path: modules and inputs must live on a CUDA (sm_100) device.
+There is no CPU path: modules and inputs must live on a CUDA (sm_90) device.
 `predict_for_single_image_with_tensorrt` (reference :657-800) is out of scope (TensorRT is not part of the
-B200 path) and raises.
+H100 path) and raises.
 """
 import ctypes as C
 
@@ -166,7 +166,7 @@ class LFD(nn.Module):
         """x: float32 [N,3,H,W] (reference contract) or uint8 [N,H,W,3] BGR (normalisation fused), on CUDA.
         -> (classification [N,P,C'], regression [N,P,4]) float32."""
         if not x.is_cuda:
-            raise RuntimeError('lfd_b200 has no CPU path: move the model and the input to a CUDA (B200) device')
+            raise RuntimeError('lfd_b200 has no CPU path: move the model and the input to a CUDA (H100) device')
         if self.training:
             # native training step (lfd/_train.py): forward with BatchNorm batch statistics, every intermediate kept for the backward,
             # which loss.backward() triggers through one autograd node

@@ -1,6 +1,6 @@
 # -*- coding: utf-8 -*-
 """FocalLoss -- API of lfd/model/losses/focal_loss.py:12-92; the element-wise forward / backward run in
-liblfd_b200.so (lfd_sigmoid_focal_loss_{forward,backward}), the sm_100a replacement of the reference's
+liblfd_b200.so (lfd_sigmoid_focal_loss_{forward,backward}), the sm_90a replacement of the reference's
 sigmoid_focal_loss_ext (which needs THC and no longer builds).  CUDA only, like the reference."""
 import torch
 import torch.nn as nn

@@ -53,7 +53,7 @@ class ForwardPostPipeline(object):
             # latency-bound; with a priority above the forward graph's nodes their CTAs are placed at the first kernel boundary of the
             # NEXT batch's forward instead of queueing behind its persistent CTAs
             self.post_stream = torch.cuda.Stream(device=dev, priority=-100)
-        self.n_slots = 2                # output pairs of the plan: 2 and 3 measured alike (profiles/r02_tuning_notes.md)
+        self.n_slots = 2                # output pairs of the plan: the forward of batch i+1 writes one while batch i is post-processed
         self.fwd_done = [torch.cuda.Event() for _ in range(self.n_slots)]
         self.post_done = [torch.cuda.Event() for _ in range(self.n_slots)]
         self.k = 0

@@ -12,7 +12,7 @@ for p in (ROOT, PKG, os.path.dirname(os.path.abspath(__file__))):
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA (B200) device; run with -m gpu on the GPU box')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA (H100) device; run with -m gpu on the GPU box')
 
 
 def pytest_collection_modifyitems(config, items):

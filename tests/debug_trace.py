@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""Debug aid: clock64() timeline of CTA 0 of one tcgen05 conv launch (producer / MMA issuer / epilogue per tile)."""
+"""Debug aid: clock64() timeline of CTA 0 of one wgmma conv launch (producer / MMA issuer / epilogue per tile)."""
 import os
 import sys
 

@@ -162,6 +162,27 @@ def forward_case(R, name, n, h, w, cls_bias, out_dir):
     print('forward %s: P=%d cls %s loss %s' % (name, cls.shape[1], tuple(cls.shape), ld['loss_values']))
 
 
+# inputs of tests/test_oracle_vs_golden.py::test_reference_cpu_nms_binary_agrees_with_oracle
+NMS_SIZES, NMS_THRS = (1, 7, 300), (0.3, 0.6)
+
+
+def nms_dets(n, rng):
+    d = np.concatenate([rng.uniform(0, 100, (n, 2)), rng.uniform(1, 40, (n, 2)), rng.uniform(0, 1, (n, 1))], 1).astype(np.float32)
+    d[:, 2:4] += d[:, 0:2]
+    return d
+
+
+def reference_nms_case(nms_ext, out_dir):
+    """The reference's compiled CPU NMS (nms_cpu.cpp) on seeded random boxes -> golden/reference_nms.pt."""
+    rng = np.random.RandomState(3)
+    cases = []
+    for n in NMS_SIZES:
+        d = nms_dets(n, rng)
+        cases.append(dict(dets=d, keep={thr: nms_ext.nms(torch.from_numpy(d), thr).numpy() for thr in NMS_THRS}))
+    torch.save(cases, os.path.join(out_dir, 'reference_nms.pt'))
+    print('reference nms: keep sizes', [{t: len(k) for t, k in c['keep'].items()} for c in cases])
+
+
 def main():
     R = import_reference()
     out_dir = os.path.join(HERE, 'golden')
@@ -184,6 +205,7 @@ def main():
     torch.save(dict(nms_doc_dets=dets, nms_doc_keep=keep, nms_rand_dets=rnd, nms_rand_keep=keep_rnd, nms_rand_thr=0.3,
                     overlaps_b1=b1, overlaps_b2=b2, overlaps=bbox_overlaps(b1, b2)), os.path.join(out_dir, 'known_answers.pt'))
     print('known answers: doc keep', keep.tolist(), 'random keep', len(keep_rnd))
+    reference_nms_case(R['nms_ext'], out_dir)
 
     for name, (n, h, w, cls_bias) in FORWARD_CASES.items():
         forward_case(R, name, n, h, w, cls_bias, out_dir)

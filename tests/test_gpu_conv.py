@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""GPU parity (Gate A): the tcgen05 implicit-GEMM convolution (and its SIMT cross-check) against an fp32 CPU
+"""GPU parity (Gate A): the wgmma implicit-GEMM convolution (and its SIMT cross-check) against an fp32 CPU
 convolution of the same bf16 operands, through the C-ABI (lfd_run_op)."""
 import pytest
 import torch

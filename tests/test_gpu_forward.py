@@ -73,7 +73,7 @@ def test_forward_fp16_meets_1e3_end_to_end(name, impl):
     ocls, oreg, sizes = orc.forward(cfg, sd, x, emulate='fp16')
     ec, er = rel_err(cls, ocls), rel_err(reg, oreg)
     print('fp16 vs fp16-emulated oracle %s: cls max/rms %.2e/%.2e reg %.2e/%.2e' % (name, ec[0], ec[1], er[0], er[1]))
-    # (the stated 1e-3 is the gate of the product path -- the tcgen05 kernels; the SIMT cross-check kernels sum in a different order and get 1.5x)
+    # (the stated 1e-3 is the gate of the product path -- the wgmma kernels; the SIMT cross-check kernels sum in a different order and get 1.5x)
     slack = 1.0 if impl == nat.CONV_UMMA else 2.0
     if name == 'TL_L':        # 33 conv layers deep (the BASELINE configs have 21-29): the rounding noise of the extra layers, stated not hidden
         slack *= 1.5

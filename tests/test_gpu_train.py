@@ -2,7 +2,7 @@
 """The native training step through the drop-in API on the GPU (SURVEY section 8 rows a19 / g1, section 8e).
 
 Everything in the step is hand-written CUDA: forward in train mode (BatchNorm batch statistics), label assignment, losses, the
-backward of the whole conv stack (tcgen05 dgrad / wgrad, norm backward), the flat-bucket gradient all-reduce, clip + SGD.
+backward of the whole conv stack (wgmma dgrad / wgrad, norm backward), the flat-bucket gradient all-reduce, clip + SGD.
 The checker is tests/aten_train_reference.py: the SAME module graph evaluated by ATen in fp32 and differentiated by autograd --
 the reference's arithmetic (lfd/model/lfd.py:511-542 through autograd)."""
 import os

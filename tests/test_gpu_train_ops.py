@@ -1,7 +1,7 @@
 # -*- coding: utf-8 -*-
 """Per-kernel parity of the native training ops against torch autograd (fp32, CPU) on the SAME 16-bit operands: parameter
 staging, BatchNorm batch statistics / apply, BatchNorm / GroupNorm backward, head-final backward, data gradients (the forward
-tcgen05 kernel on transposed / flipped weights, zero-inserted for stride 2), weight gradients (tcgen05 MN-major kernel, SIMT
+wgmma kernel on transposed / flipped weights, zero-inserted for stride 2), weight gradients (wgmma MN-major kernel, SIMT
 cross-check, stem), clip + SGD.  Reference semantics: torch.nn modules as the reference uses them (lfd_resnet.py:10-18,96-154,
 lfd_head.py:85-185, optimizer_hook.py:21-36)."""
 import pytest

@@ -8,7 +8,6 @@ import torch
 import synth
 from helpers import load_golden, build_model, rel_err
 from oracle import lfd_oracle as orc
-from oracle import build_ref
 
 FWD = ['WIDERFACE_XS', 'WIDERFACE_S', 'WIDERFACE_L', 'TT100K_L', 'TL_L', 'TEST_FAST', 'TEST_FASTEST']
 
@@ -112,16 +111,15 @@ def test_known_answers():
 
 
 def test_reference_cpu_nms_binary_agrees_with_oracle():
-    """oracle/_ref = the reference's own nms_cpu.cpp compiled here; skipped where it was not built."""
-    mod = build_ref.load_module()
-    if mod is None:
-        pytest.skip('oracle/_ref/nms_ext_ref.so not built')
+    """The reference's own nms_cpu.cpp (its kept indices on seeded random boxes, stored by tests/gen_golden.py) against the oracle's NMS."""
+    from gen_golden import NMS_THRS, nms_dets
+    cases = load_golden('reference_nms.pt')
     rng = np.random.RandomState(3)
-    for n in (1, 7, 300):
-        d = np.concatenate([rng.uniform(0, 100, (n, 2)), rng.uniform(1, 40, (n, 2)), rng.uniform(0, 1, (n, 1))], 1).astype(np.float32)
-        d[:, 2:4] += d[:, 0:2]
-        for thr in (0.3, 0.6):
-            assert mod.nms(torch.from_numpy(d), thr).tolist() == orc.nms(d, thr).tolist()
+    for c in cases:
+        d = nms_dets(len(c['dets']), rng)
+        assert np.array_equal(d, c['dets'])
+        for thr in NMS_THRS:
+            assert c['keep'][thr].tolist() == orc.nms(d, thr).tolist()
 
 
 def test_focal_restatement_pinned_against_torchvision():
