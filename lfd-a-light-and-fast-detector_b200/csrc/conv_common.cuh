@@ -47,7 +47,7 @@ struct alignas(64) UmmaConvParams {
     uint32_t smem_w2_off;
     double* stats;              // optional [N][groups][2] (sum, sumsq) of the stored output
     unsigned long long* tl;     // debugging: [start, end] of the launch in %globaltimer ns (LFD_B200_TIMELINE builds), normally null
-    long long* trace;           // debugging: clock64() timeline of CTA 0 ([role 0..2][tile < 32][4]), normally null
+    long long* trace;           // debugging: clock64() timeline of CTA 0 ([role 0..3][entry < 32][4], see conv_umma.cu), normally null
     int N, H, W, Cin, Ho, Wo, Cout;
     int relu, gn_groups, mode;
     int tiles_x, tiles_per_img, num_tiles;

@@ -34,6 +34,8 @@
 //   * programmatic dependent launch: the prologue (barriers, weight fetch) overlaps the previous layer.
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "conv_common.cuh"
 #include "ptx.cuh"
 
@@ -47,12 +49,20 @@ static constexpr int kConvThreads = kConsumerThreads + kProdThreads;
 // closure is materialised in local memory and the kernel runs 2-3x slower (a large stack frame in ptxas -v is the symptom).  Force it.
 #define LFD_LAMBDA_INLINE __attribute__((always_inline))
 
-// clock64() timeline of CTA 0 (tests/debug_trace.py); compiled in only with -DLFD_B200_TRACE (LFD_B200_TRACE=1 python build.py)
+// clock64() timeline of CTA 0 (tests/debug_trace_consumers.py); compiled in only with -DLFD_B200_TRACE (LFD_B200_TRACE=1 python build.py).
+// Buffer [4 roles][32 entries][4 slots]:
+//   role 0        producer, per stage                : wait_empty  got_empty  issued  arrived_full (stem: next tile's fetch issued)
+//   role 1 + wg   consumer warpgroup wg, per tile    : wait_full  got_full (last chunk)  main_mma_done  tail_mma_done
+//   role 3        epilogues, entry 2 * store + wg    : store_entry  after_bulk_wait_read  tma_issued  -
+// Only thread 0 of each role stamps.
 #ifdef LFD_B200_TRACE
 #define LFD_TRACE(role, idx, slot) \
     do { if (p.trace && blockIdx.x == 0 && (idx) < 32) p.trace[((role) * 32 + (idx)) * 4 + (slot)] = clock64(); } while (0)
+#define LFD_TRACE_EPI(tr, idx, slot) \
+    do { if ((tr) && blockIdx.x == 0 && (idx) < 16) (tr)[(idx) * 8 + (slot)] = clock64(); } while (0)
 #else
 #define LFD_TRACE(role, idx, slot) ((void)0)
+#define LFD_TRACE_EPI(tr, idx, slot) ((void)0)
 #endif
 
 // floor(x / d) for 0 <= x < 2^24 via one 32x32->64 multiply; m = ceil(2^40 / d), exact for d < 2^16
@@ -139,6 +149,14 @@ __device__ __forceinline__ constexpr int tap_view(int tap) {  // pixel offset of
 
 LFD_DEVINL void wg_bar_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }   // the 128 threads of warpgroup wg
 
+// fused 1x1 tail: acc2[64 x N] = A[64 x K] . W2[K x N], A from registers (K / 16 fragments of 4 packed pairs), W2 resident in shared
+// memory as [K / 8][N][8] (LBO = N * 16 B between 8-channel K chunks, SBO = 128 B between 8-column groups)
+template <int N, int K, bool F16>
+LFD_DEVINL void tail_mma(float* acc2, const uint32_t* a2, uint64_t b2desc0) {
+#pragma unroll
+    for (int kk = 0; kk < K / 16; ++kk) wgmma_rs<N, F16>(acc2, a2 + 4 * kk, b2desc0 + (uint32_t)((kk * 2 * N * 16) >> 4), kk != 0);
+}
+
 // Where the epilogue of one warpgroup writes and what it stores
 struct EpiCtx {
     uint32_t stg;          // this warpgroup's staging region: [buffer][64 rows x Cf x 2 B]
@@ -147,6 +165,9 @@ struct EpiCtx {
     int r0, tq;            // this thread's first row (second: r0 + 8) within the warpgroup's 64, column pair index (lane % 4)
     int wtid;              // thread index within the warpgroup
     int wg, lane;
+#ifdef LFD_B200_TRACE
+    long long* tr;         // this warpgroup's first epilogue entry of the trace buffer (null: no trace); its entries are 8 apart
+#endif
 };
 
 // Register accumulators (rows r0 / r0 + 8, NC <= NCMAX columns) (+shift) (+residual) (+ReLU) -> 16-bit staging rows in the TMA swizzle
@@ -158,12 +179,17 @@ LFD_DEVINL void store_tile(const EpiCtx& e, const float* acc, int nc, const floa
                            const CUtensorMap* tmap, const CUtensorMap* tmres, int c0, int c1, int n, bool v0, bool v1,
                            uint64_t* res_bar, uint32_t& store_count, uint32_t& res_count) {
     const uint32_t buf = e.stg + (e.nbuf == 2 ? (store_count & 1) * e.stg_bytes : 0u);
+#ifdef LFD_B200_TRACE
+    const uint32_t tidx = store_count;
+#endif
     ++store_count;
     const int row_bytes = nc >= 64 ? 128 : nc * 2;
     const int n_panels = nc >= 64 ? nc / 64 : 1;
     if (e.wtid == 0) {
+        LFD_TRACE_EPI(e.tr, tidx, 0);
         // this staging buffer was the source of an earlier store: the TMA engine must be done reading it
         if (e.nbuf == 2) bulk_wait_read<1>(); else bulk_wait_read<0>();
+        LFD_TRACE_EPI(e.tr, tidx, 1);
         if (res) {   // residual rows -> staging (out-of-map rows / columns arrive as zeros), added in place below
             mbar_arrive_expect_tx(res_bar, 64u * nc * 2u);
             for (int pn = 0; pn < n_panels; ++pn) {
@@ -172,6 +198,16 @@ LFD_DEVINL void store_tile(const EpiCtx& e, const float* acc, int nc, const floa
             }
         }
     }
+    // The shifts of this thread's columns are loaded ahead of the staging stores, up to 8 column pairs at a time (4 with 128 columns):
+    // the stores' "memory" clobber would otherwise order every load behind the previous store, one shared-memory round trip per pair.
+    constexpr int JB = NCMAX / 8 < 8 ? NCMAX / 8 : 4;
+    float2 bv[JB];
+    auto load_shifts = [&](int j0) LFD_LAMBDA_INLINE {
+#pragma unroll
+        for (int i = 0; i < JB; ++i)
+            if (j0 + i < nc / 8) bv[i] = *reinterpret_cast<const float2*>(bias + 8 * (j0 + i) + 2 * e.tq);
+    };
+    load_shifts(0);
     wg_bar_sync(e.wg);
     if (res) { mbar_wait(res_bar, res_count & 1); ++res_count; }
     float st[NCMAX == 128 ? 32 : 1];
@@ -179,8 +215,8 @@ LFD_DEVINL void store_tile(const EpiCtx& e, const float* acc, int nc, const floa
 #pragma unroll
     for (int j = 0; j < NCMAX / 8; ++j) {
         if (j < nc / 8) {
-            const int c = 8 * j + 2 * e.tq;
-            const float b0 = bias[c], b1 = bias[c + 1];
+            if (j > 0 && j % JB == 0) load_shifts(j);
+            const float b0 = bv[j % JB].x, b1 = bv[j % JB].y;
             float s1 = 0.f, s2 = 0.f;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
@@ -212,6 +248,7 @@ LFD_DEVINL void store_tile(const EpiCtx& e, const float* acc, int nc, const floa
             else tma_store_4d(tmap, buf + pn * 8192, pn * 64, c0, c1, n);
         }
         bulk_commit();
+        LFD_TRACE_EPI(e.tr, tidx, 2);
     }
     if (NCMAX == 128 && stat) stats_flush<128>(st, e.lane, stats);
 }
@@ -319,6 +356,9 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
         e.wtid = tid & 127;
         e.wg = wg;
         e.lane = lane;
+#ifdef LFD_B200_TRACE
+        e.tr = p.trace && e.wtid == 0 ? p.trace + (3 * 32 + wg) * 4 : nullptr;
+#endif
         if (e.wtid == 0 && (e.stg & 1023u)) __trap();    // swizzle atoms need 1024-byte aligned staging regions
 
         const uint32_t lbo_b = COUT * 16;
@@ -336,10 +376,12 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
         float acc[COUT / 2];
         float acc3[MODE == MODE_3X3S2 ? COUT / 2 : 1];
         uint32_t it = 0, store_count = 0, res_count = 0;
-        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        for (int tile = blockIdx.x, lt = 0; tile < p.num_tiles; tile += gridDim.x, ++lt) {
             for (int cc = 0; cc < n_cc; ++cc, ++it) {
                 const uint32_t s = it % SA, ph = (it / SA) & 1;
+                if (cc == 0 && e.wtid == 0) LFD_TRACE(1 + wg, lt, 0);
                 mbar_wait(&full[s], ph);
+                if (e.wtid == 0) LFD_TRACE(1 + wg, lt, 1);
                 fence_proxy_async_smem();   // cp.async / st.shared (generic proxy) writes -> wgmma (async proxy) reads
                 const uint32_t a_base = smem_u32(ring) + s * p.stage_bytes;
                 const uint32_t b_base = p.b_resident ? smem_u32(wres) + cc * p.b_slice_bytes : a_base + p.a_stage_bytes;
@@ -367,6 +409,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty[s]);     // this warp's part of the stage has been consumed
             }
+            if (e.wtid == 0) LFD_TRACE(1 + wg, lt, 2);
 
             // ---- epilogue of the tile: this warpgroup's 64 rows
             const int n = fast_div(tile, p.magic_tpi);
@@ -401,19 +444,23 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                 float acc2[64];
                 wgmma_fence_regs<64>(acc2);
                 wgmma_fence();
-#pragma unroll
-                for (int nb = 0; nb < 8; ++nb) {
-                    if (nb < p.Cout2 / 16) {
-#pragma unroll
-                        for (int kk = 0; kk < COUT / 16; ++kk)
-                            wgmma_rs_n16<F16>(acc2 + 8 * nb, a2 + 4 * kk, b2desc0 + (uint32_t)((kk * 2 * p.Cout2 * 16 + nb * 256) >> 4), kk != 0);
-                    }
+                // COUT / 16 MMAs of N = Cout2 and the store of Cout2 columns (the widths umma_conv_configure accepts for a stored tensor)
+                auto tail = [&](auto n2) LFD_LAMBDA_INLINE {
+                    constexpr int N2 = decltype(n2)::value;
+                    tail_mma<N2, COUT, F16>(acc2, a2, b2desc0);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_regs<N2 / 2>(acc2);
+                    if (e.wtid == 0) LFD_TRACE(1 + wg, lt, 3);
+                    store_tile<MODE, N2, F16>(e, acc2, N2, bias2, p.stats ? false : (bool)p.relu2, p.stats ? false : has_res, sdst,
+                                              &p.tm_out, &p.tm_res, c0, c1, n, v0, v1, &res_bar[wg], store_count, res_count);
+                };
+                switch (p.Cout2) {
+                    case 16: tail(std::integral_constant<int, 16>()); break;
+                    case 32: tail(std::integral_constant<int, 32>()); break;
+                    case 64: tail(std::integral_constant<int, 64>()); break;
+                    default: tail(std::integral_constant<int, 128>()); break;
                 }
-                wgmma_commit();
-                wgmma_wait<0>();
-                wgmma_fence_regs<64>(acc2);
-                store_tile<MODE, 128, F16>(e, acc2, p.Cout2, bias2, p.stats ? false : (bool)p.relu2, p.stats ? false : has_res, sdst,
-                                           &p.tm_out, &p.tm_res, c0, c1, n, v0, v1, &res_bar[wg], store_count, res_count);
             } else {
                 store_tile<MODE, COUT, F16>(e, acc, COUT, bias, p.stats ? false : (bool)p.relu, p.stats ? false : has_res, sdst,
                                             &p.tm_out, &p.tm_res, c0, c1, n, v0, v1, &res_bar[wg], store_count, res_count);
@@ -493,7 +540,9 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
             if ((int)blockIdx.x < p.num_tiles) fetch(blockIdx.x);
             for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
                 const uint32_t s = it % SA, ph = (it / SA) & 1;
+                if (ptid == 0) LFD_TRACE(0, it, 0);
                 mbar_wait(&empty[s], ph ^ 1);
+                if (ptid == 0) LFD_TRACE(0, it, 1);
                 const uint32_t dst0 = smem_u32(ring) + s * p.stage_bytes + ptid * 8;
 #pragma unroll
                 for (int j = 0; j < kStemPerThread; ++j) {
@@ -509,7 +558,9 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                 }
                 fence_proxy_async_smem();       // generic-proxy st.shared -> wgmma reads
                 mbar_arrive(&full[s]);
+                if (ptid == 0) LFD_TRACE(0, it, 2);
                 if (tile + (int)gridDim.x < p.num_tiles) fetch(tile + gridDim.x);
+                if (ptid == 0) LFD_TRACE(0, it, 3);
             }
         } else {
         // every thread owns ONE 16-byte channel chunk (cpc divides 128) and walks the halo pixels with a fixed stride
