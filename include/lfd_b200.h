@@ -57,7 +57,7 @@ const char* lfd_last_error(void);
 int lfd_device_sm_count(void);
 
 /* ------------------------------------------------------------------------------------------ forward plan */
-enum { LFD_OP_STEM0 = 0, LFD_OP_CONV = 1, LFD_OP_GN_APPLY = 2, LFD_OP_HEAD_FINAL = 3 };
+enum { LFD_OP_STEM0 = 0, LFD_OP_CONV = 1, LFD_OP_GN_APPLY = 2, LFD_OP_HEAD_FINAL = 3, LFD_OP_STEM4 = 4 };
 enum { LFD_INPUT_F32_NCHW = 0, LFD_INPUT_U8_NHWC = 1 };
 enum { LFD_CONV_UMMA = 0, LFD_CONV_SIMT = 1 }; /* SIMT = cross-check kernel, validation only */
 /* 16-bit storage type of activations and packed weights (fp32 accumulation either way; same bytes, same tensor-core rate):
@@ -70,6 +70,12 @@ enum { LFD_DTYPE_BF16 = 0, LFD_DTYPE_FP16 = 1 };
  *              weight = bf16 packed [kh][2][Cout][8]: element (kh, kc, n, j) = weight of output n, input channel j % 4, filter
  *              column kw = 2*kc + j/4 (zero for kw = 3 and for the padded 4th channel): the kernel keeps the image patch as
  *              4-channel bf16 pixels and lets the wgmma address generator do the im2col (K = 16 per filter row).
+ *   STEM4      the four convolutions of a 'faster' stem in one kernel: stem0 3x3/s2 3->64 (weight / shift / relu, packed as STEM0),
+ *              stem1 1x1 64->64 (tail_weight / tail_shift / tail_relu, tail_cout = 64), stem2 3x3/s2 64->64 (s2_weight = bf16 packed
+ *              [9][8][64][8], i.e. the CONV packing with cc = 64; s2_shift / s2_relu) and stem3 1x1 64->64 (s3_weight = bf16 packed
+ *              [8][64][8]; s3_shift / s3_relu).  Cin = 3, Cout = 64, ksize = 3, stride = 2; H x W = the image, Ho x Wo = the stem3
+ *              output (two stride-2 steps); in_off ignored.  Every intermediate is rounded to bf16 exactly as the STEM0 + CONV pair
+ *              path rounds it, so the output is bit-identical to it; the stem1 map never reaches HBM.  Sizes: lfd_stem4_query.
  *   CONV       ksize in {1,3}, stride in {1,2}, pad = ksize/2; y = conv(x) + shift (+res) (ReLU) -> bf16;
  *              weight = bf16 packed [Cin/cc][ksize^2][cc/8][Cout][8] with cc from lfd_conv_query, ALREADY MULTIPLIED by the
  *              per-output-channel scale (folded BatchNorm); `scale` must be NULL; `shift` (fp32 [Cout], may be NULL) is rounded
@@ -117,12 +123,21 @@ typedef struct lfd_op {
     int64_t ds_out_off;
     const void* ds_weight;
     const float* ds_shift;
+    /* STEM4 only: the third and fourth convolution of the fused stem (see STEM4 above) */
+    int32_t s2_relu, s3_relu;
+    const void* s2_weight;
+    const float* s2_shift;
+    const void* s3_weight;
+    const float* s3_shift;
 } lfd_op;
 
 /* Tile / pipeline configuration the wgmma kernel will use for a conv (host only, no launch).
  * cc = input-channel chunk the weights must be packed with. */
 int lfd_conv_query(int N, int H, int W, int Cin, int Ho, int Wo, int Cout, int ksize, int stride, int tail_cout, int ds_cout, int* cc,
                    int* stages, int* weights_resident, int* num_tiles, int64_t* smem_bytes);
+/* The same for a STEM4 op on N images of H x W (host only): its tiles (16 x 8 stem3 pixels each), dynamic shared memory per CTA
+ * and stem3 output size. */
+int lfd_stem4_query(int N, int H, int W, int* num_tiles, int64_t* smem_bytes, int* Ho, int* Wo);
 
 /* The plan copies the op list.  stats_off/stats_bytes: region of the workspace zeroed at the start of each forward. */
 int lfd_plan_create(const lfd_op* ops, int n_ops, int N, int P, int cls_channels, int64_t stats_off, int64_t stats_bytes,

@@ -44,8 +44,11 @@ def _check_stack_frames(ptxas_log, limit=64):
         if m:
             name = m.group(1)
         m = re.search(r'(\d+) bytes stack frame', line)
-        if m and name and 'conv_umma_kernel' in name and int(m.group(1)) > _STACK_EXEMPT.get(name, limit):
+        if m and name and ('conv_umma_kernel' in name or 'stem4_kernel' in name) and int(m.group(1)) > _STACK_EXEMPT.get(name, limit):
             raise RuntimeError('%s has a %s-byte stack frame (limit %d): registers went to local memory' % (name, m.group(1), _STACK_EXEMPT.get(name, limit)))
+        # ptxas warning C7520: it could not prove the wgmma pipeline safe and serialised every wgmma of the kernel
+        if 'C7520' in line and 'stem4_kernel' in line:
+            raise RuntimeError('ptxas serialised the wgmma instructions of the fused stem kernel:\n%s' % line)
 
 
 def build(force=False, verbose=False):

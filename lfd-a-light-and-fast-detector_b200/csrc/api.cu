@@ -113,6 +113,7 @@ static ConvGeom geom_of(const lfd_op& o) {
     ConvGeom g;
     g.N = o.N; g.H = o.H; g.W = o.W; g.Cin = o.Cin; g.Ho = o.Ho; g.Wo = o.Wo; g.Cout = o.Cout; g.ksize = o.ksize; g.stride = o.stride;
     g.stem = o.kind == LFD_OP_STEM0 ? 1 : 0;
+    g.stem4 = o.kind == LFD_OP_STEM4 ? 1 : 0;
     g.tail_cout = o.tail_cout;
     g.ds_cout = o.ds_cout;
     if (g.stem) g.Cin = 16;   // K of one filter row: 4 pixels x 4 (padded) channels
@@ -135,6 +136,20 @@ extern "C" int lfd_conv_query(int N, int H, int W, int Cin, int Ho, int Wo, int 
     return LFD_OK;
 }
 
+extern "C" int lfd_stem4_query(int N, int H, int W, int* num_tiles, int64_t* smem_bytes, int* Ho, int* Wo) {
+    const int h1 = (H - 1) / 2 + 1, w1 = (W - 1) / 2 + 1;
+    ConvGeom g = {N, H, W, 3, (h1 - 1) / 2 + 1, (w1 - 1) / 2 + 1, 64, 3, 2, 64, 0, 0, 1};
+    UmmaConvParams p;
+    size_t smem = 0;
+    int grid = 0;
+    if (N < 1 || H < 1 || W < 1 || umma_conv_configure(g, 132, &p, &smem, &grid)) return fail(LFD_ERR_UNSUPPORTED, "stem4: unsupported size N=%d H=%d W=%d", N, H, W);
+    if (num_tiles) *num_tiles = p.num_tiles;
+    if (smem_bytes) *smem_bytes = (int64_t)smem;
+    if (Ho) *Ho = p.Ho;
+    if (Wo) *Wo = p.Wo;
+    return LFD_OK;
+}
+
 static int check_op(const lfd_op& o) {
     const int eh = (o.H + 2 * (o.ksize / 2) - o.ksize) / (o.stride > 0 ? o.stride : 1) + 1;
     const int ew = (o.W + 2 * (o.ksize / 2) - o.ksize) / (o.stride > 0 ? o.stride : 1) + 1;
@@ -145,6 +160,13 @@ static int check_op(const lfd_op& o) {
             if (o.Cin != 3 || o.ksize != 3 || o.stride != 2) return fail(LFD_ERR_UNSUPPORTED, "stem0 supports 3x3/s2 on 3 input channels only (got Cin=%d k=%d s=%d)", o.Cin, o.ksize, o.stride);
             if (o.Cout != 16 && o.Cout != 32 && o.Cout != 64) return fail(LFD_ERR_UNSUPPORTED, "stem0 Cout must be 16/32/64 (got %d)", o.Cout);
             if (o.Ho != eh || o.Wo != ew) return fail(LFD_ERR_INVALID, "stem0 output size mismatch");
+            break;
+        case LFD_OP_STEM4:
+            if (o.scale || o.tail_scale) return fail(LFD_ERR_INVALID, "conv scale must be folded into the packed weights (pass scale = NULL)");
+            if (o.Cin != 3 || o.ksize != 3 || o.stride != 2 || o.Cout != 64 || o.tail_cout != 64 || o.ds_cout || o.res_off >= 0 || o.gn_groups)
+                return fail(LFD_ERR_UNSUPPORTED, "stem4 is 3x3/s2 3->64, 1x1 64->64, 3x3/s2 64->64, 1x1 64->64 without residual / statistics");
+            if (!o.weight || !o.tail_weight || !o.s2_weight || !o.s3_weight) return fail(LFD_ERR_INVALID, "stem4 needs the weights of all four convs");
+            if (o.Ho != (eh - 1) / 2 + 1 || o.Wo != (ew - 1) / 2 + 1) return fail(LFD_ERR_INVALID, "stem4 output size mismatch (expected the stem3 map)");
             break;
         case LFD_OP_CONV:
             if (o.scale || o.tail_scale) return fail(LFD_ERR_INVALID, "conv scale must be folded into the packed weights (pass scale = NULL)");
@@ -177,7 +199,7 @@ static int plan_op(const lfd_op& o, int conv_impl, PlannedOp* out) {
     out->op = o;
     out->smem = 0;
     out->grid = 0;
-    if (o.kind == LFD_OP_CONV || o.kind == LFD_OP_STEM0) {
+    if (o.kind == LFD_OP_CONV || o.kind == LFD_OP_STEM0 || o.kind == LFD_OP_STEM4) {
         rc = umma_conv_configure(geom_of(o), sm_count() > 0 ? sm_count() : 132, &out->cp, &out->smem, &out->grid);
         if (rc) return fail(LFD_ERR_UNSUPPORTED, "conv %dx%d s%d Cin=%d Cout=%d unsupported (rc=%d)", o.ksize, o.ksize, o.stride, o.Cin, o.Cout, rc);
         if (o.kind == LFD_OP_CONV && out->cp.Cc != o.cc) return fail(LFD_ERR_INVALID, "weights packed with cc=%d but the kernel needs cc=%d", o.cc, out->cp.Cc);
@@ -214,8 +236,23 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
             }
             break;
         }
+        case LFD_OP_STEM4: {
+            if (!input) return fail(LFD_ERR_INVALID, "stem4 needs the external input pointer");
+            if (conv_impl == LFD_CONV_SIMT) return fail(LFD_ERR_UNSUPPORTED, "the SIMT cross-check kernels do not implement the fused stem (plan its four convs)");
+            UmmaConvParams p = po.cp;
+            p.in_raw = input; p.input_format = input_format; p.in = nullptr;
+            p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off); p.res = nullptr; p.stats = nullptr;
+            p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift; p.relu = o.relu;
+            p.w2 = reinterpret_cast<const __nv_bfloat16*>(o.tail_weight); p.shift2 = o.tail_shift; p.relu2 = o.tail_relu;
+            p.w_s2 = reinterpret_cast<const __nv_bfloat16*>(o.s2_weight); p.shift_s2 = o.s2_shift; p.relu_s2 = o.s2_relu;
+            p.w_s3 = reinterpret_cast<const __nv_bfloat16*>(o.s3_weight); p.shift_s3 = o.s3_shift; p.relu_s3 = o.s3_relu;
+            p.gn_groups = 0; p.trace = g_trace; p.tl = tl; p.f16 = o.dtype;
+            if (umma_conv_encode_maps(&p)) return fail(LFD_ERR_CUDA, "cuTensorMapEncodeTiled failed for the fused stem");
+            CUDA_TRY(umma_conv_launch(p, po.smem, po.grid, st));
+            break;
+        }
         case LFD_OP_CONV: {
-            const __nv_bfloat16* in = reinterpret_cast<const __nv_bfloat16*>(ws + o.in_off);
+            const __nv_bfloat16* in =reinterpret_cast<const __nv_bfloat16*>(ws + o.in_off);
             __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off);
             const __nv_bfloat16* res = o.res_off >= 0 ? reinterpret_cast<const __nv_bfloat16*>(ws + o.res_off) : nullptr;
             double* stats = o.gn_groups ? reinterpret_cast<double*>(ws + o.stats_off) : nullptr;

@@ -8,7 +8,8 @@
 
 namespace lfd {
 
-enum { MODE_FLAT = 0, MODE_3X3S1 = 1, MODE_3X3S2 = 2, MODE_1X1S2 = 3, MODE_STEM = 4 };
+// MODE_STEM4: the four convolutions of the 'faster' stem (3x3/s2 3->64, 1x1, 3x3/s2 64->64, 1x1) in one kernel (stem4_kernel)
+enum { MODE_FLAT = 0, MODE_3X3S1 = 1, MODE_3X3S2 = 2, MODE_1X1S2 = 3, MODE_STEM = 4, MODE_STEM4 = 5 };
 
 static constexpr int kMaxStages = 8;
 static constexpr int kMaxDevices = 64;   // per-device state (function attributes, SM counts) is indexed by the device ordinal
@@ -23,6 +24,7 @@ struct ConvGeom {
     int tail_cout;   // > 0: a 1x1/s1 conv (Cout -> tail_cout) is fused behind this conv (second GEMM in the same kernel)
     int ds_cout;     // > 0 (3x3/s2 only): the residual block's 1x1/s2 shortcut conv (Cin -> ds_cout == Cout) is fused: second output tensor
     int stem;   // 1: 3x3/s2 conv on the raw 3-channel image (K = 27 padded to 32), operand built by the producers
+    int stem4;  // 1: the fused four-conv stem (MODE_STEM4); H x W = the image, Ho x Wo = the stem3 output, Cout = tail_cout = 64
 };
 
 struct alignas(64) UmmaConvParams {
@@ -61,6 +63,13 @@ struct alignas(64) UmmaConvParams {
     uint32_t smem_w_off, smem_ring_off;
     int input_format;
     int f16;                    // activation / weight type: 0 = bf16, 1 = IEEE fp16 (same bytes, same tensor-core rate)
+    // MODE_STEM4: stem0 = w / shift / relu, stem1 = w2 / shift2 / relu2 (the tail fields), stem2 = its 3x3/s2 weights packed
+    // [9][8][64][8] + shift + ReLU, stem3 = its 1x1 weights packed [8][64][8] + shift + ReLU; H1 x W1 = the stem1 map
+    const __nv_bfloat16* w_s2;
+    const float* shift_s2;
+    const __nv_bfloat16* w_s3;
+    const float* shift_s3;
+    int relu_s2, relu_s3, H1, W1;
 };
 
 // returns 0 when the geometry is supported by the wgmma kernel

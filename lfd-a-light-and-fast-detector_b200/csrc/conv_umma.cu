@@ -49,7 +49,8 @@ static constexpr int kConvThreads = kConsumerThreads + kProdThreads;
 // closure is materialised in local memory and the kernel runs 2-3x slower (a large stack frame in ptxas -v is the symptom).  Force it.
 #define LFD_LAMBDA_INLINE __attribute__((always_inline))
 
-// clock64() timeline of CTA 0 (tests/debug_trace_consumers.py); compiled in only with -DLFD_B200_TRACE (LFD_B200_TRACE=1 python build.py).
+// clock64() timeline of CTA 0 (tests/debug_trace_consumers.py; tests/debug_stem_fusion.py --trace for stem4_kernel); compiled in only with
+// -DLFD_B200_TRACE (LFD_B200_TRACE=1 python build.py).
 // Buffer [4 roles][32 entries][4 slots]:
 //   role 0        producer, per stage                : wait_empty  got_empty  issued  arrived_full (stem: next tile's fetch issued)
 //   role 1 + wg   consumer warpgroup wg, per tile    : wait_full  got_full (last chunk)  main_mma_done  tail_mma_done
@@ -648,6 +649,306 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
 }
 
 // ---------------------------------------------------------------------------------------------------
+// MODE_STEM4: the 'faster' stem -- stem0 3x3/s2 3->64, stem1 1x1 64->64, stem2 3x3/s2 64->64, stem3 1x1 64->64 -- as ONE kernel.
+// Tiles are 16 x 8 pixels of the final (stem3) map, as in MODE_3X3S2.  Per tile:
+//   producer   the raw-image patch (67 rows x 36 pixels from image (4 oy0 - 3, 4 ox0 - 3)) in the MODE_STEM format -> ring stage;
+//   consumers  stem0 + stem1 on the 33 x 17 stem1 pixels stem2's halo needs (rows 2 oy0 - 1 .., columns 2 ox0 - 1 ..), as 16
+//              MODE_STEM m64 blocks of 8 x 8 stem1 pixels (the 15 of the cover below plus a repeat of the last, 8 per warpgroup);
+//              each block's stem1 result (+shift, ReLU, 16-bit) goes straight into the MODE_3X3S2 parity planes, zeros where the
+//              pixel lies outside the stem1 map (stem2's padding); then stem2 as the MODE_3X3S2 main loop (same MMA order as the
+//              two-kernel path: k16-major, tap-minor), the stem3 tail and the TMA store of the two-kernel path.
+// The stem1 tensor never exists outside shared memory.  Every wgmma group is waited for before the next barrier / divergent code.
+// Trace (LFD_B200_TRACE builds, tests/debug_stem_fusion.py --trace), per tile lt:
+//   role 0        producer            : wait_empty  got_empty  patch_written(arrived_full)  -
+//   role 1 + wg   consumer warpgroup  : wait_full  got_full  stem01_done  plane_barrier_passed
+//   role 3        entry 2 * lt + wg   : store_entry (= tail done)  after_bulk_wait_read  tma_issued  stem2_mma_done
+static constexpr int kS4Rows = 67, kS4Cols = 36, kS4Pix = kS4Rows * kS4Cols;                      // 2412 patch pixels
+static constexpr int kS4RowBytes = kS4Cols * 8;                                                    // 288
+static constexpr int kS4PatchBytes = kS4Pix * 8;                                                   // 19296
+static constexpr int kS4PerThread = (kS4Pix + kProdThreads - 1) / kProdThreads;                   // 19
+static constexpr int kS4Batch = 5;                                                                 // patch pixels in flight per producer thread
+static constexpr int kS4Lbo = 595 * 16;                                                            // plane pitch (MODE_3X3S2, 64 channels)
+// shared-memory map (bytes)
+static constexpr int kS4Bar = 0;                    // full[2] | empty[2] | weights | res_bar[2] (unused: no residual)
+static constexpr int kS4Shift = 256;                // fp32 shifts of stem0 .. stem3, 64 each
+static constexpr int kS4Staging = 2048;             // [warpgroup][64 rows x 64 channels], 1024-byte aligned (TMA swizzle)
+static constexpr int kS4W0 = kS4Staging + 2 * 8192; // stem0 [3][2][64][8]
+static constexpr int kS4W1 = kS4W0 + 6144;          // stem1 [8][64][8]
+static constexpr int kS4W2 = kS4W1 + 8192;          // stem2 [9][8][64][8]
+static constexpr int kS4W3 = kS4W2 + 73728;         // stem3 [8][64][8]
+static constexpr int kS4Planes = kS4W3 + 8192;      // EE | EO | OE | OO x 8 channel chunks
+static constexpr int kS4Ring = kS4Planes + 8 * kS4Lbo;
+static constexpr int kS4Smem = kS4Ring + 2 * kS4PatchBytes;   // 229440 (<= 227 KB)
+static constexpr int kS4WBytes = kS4Planes - kS4W0;
+
+// origin (stem1 halo row a0, column b0) of m64 block i: rows {0, 8, 16, 24, 25} x columns {0, 8, 9}; block 15 repeats block 14
+LFD_DEVINL int s4_block_a0(int i) { const int r = (i < 15 ? i : 14) / 3; return r < 4 ? 8 * r : 25; }
+LFD_DEVINL int s4_block_b0(int i) { const int c = (i < 15 ? i : 14) % 3; return c == 0 ? 0 : 7 + c; }
+
+LFD_DEVINL void consumers_bar_sync() { asm volatile("bar.sync 3, 256;" ::: "memory"); }   // the two consumer warpgroups
+
+template <bool F16>
+__global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_constant__ UmmaConvParams p) {
+    extern __shared__ __align__(1024) uint8_t smem[];
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + kS4Bar);
+    uint64_t* empty = full + 2;
+    uint64_t* wbar = empty + 2;
+    uint64_t* res_bar = wbar + 1;
+    float* shifts = reinterpret_cast<float*>(smem + kS4Shift);
+    pdl_launch_dependents();
+    LFD_TL_BEGIN(p.tl);
+    const int tid = threadIdx.x;
+    const int warp = tid >> 5;
+    const int lane = tid & 31;
+    if (tid == 0) {
+        for (int i = 0; i < 2; ++i) {
+            mbar_init(&full[i], kProdThreads);
+            mbar_init(&empty[i], kConsumerThreads / 32);
+        }
+        mbar_init(wbar, 1);
+        mbar_init(&res_bar[0], 1);
+        mbar_init(&res_bar[1], 1);
+        fence_mbar_init();
+    }
+    if (tid < 256) {
+        const int k = tid >> 6;
+        const float* s = k == 0 ? p.shift : (k == 1 ? p.shift2 : (k == 2 ? p.shift_s2 : p.shift_s3));
+        shifts[tid] = s ? round16<F16>(s[tid & 63]) : 0.f;
+    }
+    __syncthreads();
+
+    if (warp < kConsumerThreads / 32) {
+        // ============================================================== CONSUMERS
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
+        const int wg = warp >> 2;
+        if (tid == 0) {
+            mbar_arrive_expect_tx(wbar, kS4WBytes);
+            auto load_w = [&](uint32_t dst, const __nv_bfloat16* src, uint32_t bytes) LFD_LAMBDA_INLINE {
+                for (uint32_t off = 0; off < bytes; off += 32768)
+                    bulk_g2s(smem_u32(smem) + dst + off, reinterpret_cast<const uint8_t*>(src) + off, bytes - off < 32768 ? bytes - off : 32768, wbar);
+            };
+            load_w(kS4W0, p.w, kS4W1 - kS4W0);
+            load_w(kS4W1, p.w2, kS4W2 - kS4W1);
+            load_w(kS4W2, p.w_s2, kS4W3 - kS4W2);
+            load_w(kS4W3, p.w_s3, kS4Planes - kS4W3);
+        }
+        pdl_wait();
+        mbar_wait(wbar, 0);
+
+        EpiCtx e;
+        e.stg_bytes = 8192u;
+        e.nbuf = 1;
+        e.stg = smem_u32(smem + kS4Staging) + (uint32_t)wg * 8192u;
+        e.r0 = (warp & 3) * 16 + (lane >> 2);
+        e.tq = lane & 3;
+        e.wtid = tid & 127;
+        e.wg = wg;
+        e.lane = lane;
+#ifdef LFD_B200_TRACE
+        e.tr = p.trace && e.wtid == 0 ? p.trace + (3 * 32 + wg) * 4 : nullptr;
+#endif
+        const float* sh0 = shifts;
+        const float* sh1 = shifts + 64;
+        const float* sh2 = shifts + 128;
+        const float* sh3 = shifts + 192;
+        const uint32_t planes = smem_u32(smem + kS4Planes);
+        // descriptors: stem0 A = the patch (MODE_STEM view: SBO = 2 patch rows, LBO = 16 B), B = [kh][2][64][8];
+        // stem1 / stem3 B = [8][64][8]; stem2 A = the planes (SBO = pitch-9 rows, LBO = plane pitch), B = [tap][8][64][8]
+        const uint64_t adesc_stem = wgmma_desc(0, 16, 2 * kS4RowBytes);
+        const uint64_t b0desc = wgmma_desc(smem_u32(smem + kS4W0), 64 * 16, 128);
+        const uint64_t b1desc = wgmma_desc(smem_u32(smem + kS4W1), 64 * 16, 128);
+        const uint64_t b2desc = wgmma_desc(smem_u32(smem + kS4W2), 64 * 16, 128);
+        const uint64_t b3desc = wgmma_desc(smem_u32(smem + kS4W3), 64 * 16, 128);
+        const uint64_t adesc_pl = wgmma_desc(planes + (uint32_t)wg * 8u * 144u, kS4Lbo, 144);
+        // this thread's stem1 pixels inside a block: (row 2 (warp & 3) + h, column lane / 4)
+        const int brow = 2 * (warp & 3), bcol = lane >> 2;
+
+        uint32_t store_count = 0, res_count = 0;
+        for (int tile = blockIdx.x, lt = 0; tile < p.num_tiles; tile += gridDim.x, ++lt) {
+            const uint32_t s = lt & 1, ph = (lt >> 1) & 1;
+            const int n = fast_div(tile, p.magic_tpi);
+            const int t = tile - n * p.tiles_per_img;
+            const int ty = fast_div(t, p.magic_tx);
+            const int oy0 = ty * 16, ox0 = (t - ty * p.tiles_x) * 8;
+            if (e.wtid == 0) LFD_TRACE(1 + wg, lt, 0);
+            mbar_wait(&full[s], ph);
+            if (e.wtid == 0) LFD_TRACE(1 + wg, lt, 1);
+            fence_proxy_async_smem();
+            const uint32_t patch = smem_u32(smem + kS4Ring) + s * kS4PatchBytes;
+
+            // ---- stem0 + stem1 on this warpgroup's 8 blocks, two per MMA group
+#pragma unroll
+            for (int kp = 0; kp < 4; ++kp) {
+                const int i0 = wg * 8 + 2 * kp;
+                float c0[2][32];
+                wgmma_fence_regs<32>(c0[0]);
+                wgmma_fence_regs<32>(c0[1]);
+                wgmma_fence();
+#pragma unroll
+                for (int q = 0; q < 2; ++q) {
+                    const uint32_t boff = (uint32_t)(s4_block_a0(i0 + q) * 2 * kS4RowBytes + s4_block_b0(i0 + q) * 16);
+                    const uint64_t ad = adesc_stem + ((patch + boff) >> 4);
+#pragma unroll
+                    for (int kh = 0; kh < 3; ++kh)
+                        wgmma_ss<64, F16>(c0[q], ad + (uint32_t)(kh * kS4RowBytes / 16), b0desc + (uint32_t)(kh * 2 * 64 * 16 / 16), kh != 0);
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_regs<32>(c0[0]);
+                wgmma_fence_regs<32>(c0[1]);
+                // stem0 (+shift, ReLU) -> 16 bits -> register A operand of stem1, exactly as the fused tail of the two-kernel path
+                uint32_t a1[2][16];
+#pragma unroll
+                for (int q = 0; q < 2; ++q)
+#pragma unroll
+                    for (int kk = 0; kk < 4; ++kk) {
+                        const int c = 16 * kk + 2 * e.tq;
+#pragma unroll
+                        for (int r = 0; r < 4; ++r) {
+                            const float x0 = c0[q][8 * kk + 2 * r] + sh0[c + 8 * (r >> 1)], x1 = c0[q][8 * kk + 2 * r + 1] + sh0[c + 8 * (r >> 1) + 1];
+                            a1[q][4 * kk + r] = p.relu ? pack2_relu<F16>(x0, x1) : pack2<F16>(x0, x1);
+                        }
+                    }
+                float c1[2][32];
+                wgmma_fence_regs<32>(c1[0]);
+                wgmma_fence_regs<32>(c1[1]);
+                wgmma_fence();
+                tail_mma<64, 64, F16>(c1[0], a1[0], b1desc);
+                tail_mma<64, 64, F16>(c1[1], a1[1], b1desc);
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_regs<32>(c1[0]);
+                wgmma_fence_regs<32>(c1[1]);
+                // stem1 (+shift, ReLU) -> 16 bits -> the stem2 parity planes; zeros outside the stem1 map (stem2's padding)
+                float2 bv[8];
+#pragma unroll
+                for (int j = 0; j < 8; ++j) bv[j] = *reinterpret_cast<const float2*>(sh1 + 8 * j + 2 * e.tq);
+#pragma unroll
+                for (int q = 0; q < 2; ++q) {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int a = s4_block_a0(i0 + q) + brow + h, b = s4_block_b0(i0 + q) + bcol;
+                        const int y1 = 2 * oy0 - 1 + a, x1 = 2 * ox0 - 1 + b;
+                        const bool in = (unsigned)y1 < (unsigned)p.H1 && (unsigned)x1 < (unsigned)p.W1;
+                        const uint32_t slot = ((a & 1) ? 0u : 288u) + ((b & 1) ? 0u : ((a & 1) ? 144u : 153u)) + (uint32_t)((a >> 1) * 9 + (b >> 1));
+                        const uint32_t addr = planes + slot * 16u + 4u * e.tq;
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            const float x0 = c1[q][4 * j + 2 * h] + bv[j].x, x1v = c1[q][4 * j + 2 * h + 1] + bv[j].y;
+                            uint32_t v = p.relu2 ? pack2_relu<F16>(x0, x1v) : pack2<F16>(x0, x1v);
+                            v = in ? v : 0u;
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr + (uint32_t)(j * kS4Lbo)), "r"(v) : "memory");
+                        }
+                    }
+                }
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[s]);      // this warp's stem0 MMAs have read the patch
+            if (e.wtid == 0) LFD_TRACE(1 + wg, lt, 2);
+            fence_proxy_async_smem();                   // st.shared (generic proxy) -> wgmma (async proxy) reads of the planes
+            consumers_bar_sync();
+            if (e.wtid == 0) LFD_TRACE(1 + wg, lt, 3);
+
+            // ---- stem2: the MODE_3X3S2 main loop over the planes
+            float acc[32];
+            wgmma_fence_regs<32>(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int k16 = 0; k16 < 4; ++k16)
+#pragma unroll
+                for (int tap = 0; tap < 9; ++tap)
+                    wgmma_ss<64, F16>(acc, adesc_pl + (uint32_t)(k16 * 2 * kS4Lbo / 16 + tap_view<MODE_3X3S2>(tap)),
+                                      b2desc + (uint32_t)((tap * 8 + 2 * k16) * 64 * 16 / 16), (k16 | tap) != 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs<32>(acc);
+            consumers_bar_sync();                       // both warpgroups are done reading the planes: the next tile may write them
+#ifdef LFD_B200_TRACE
+            if (e.wtid == 0 && p.trace && blockIdx.x == 0 && lt < 16) p.trace[(3 * 32 + wg + 2 * lt) * 4 + 3] = clock64();
+#endif
+
+            // ---- stem3: fused 1x1 tail and the tile store, as in the two-kernel path
+            uint32_t a2[16];
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                const int c = 16 * kk + 2 * e.tq;
+#pragma unroll
+                for (int r = 0; r < 4; ++r) {
+                    const float x0 = acc[8 * kk + 2 * r] + sh2[c + 8 * (r >> 1)], x1 = acc[8 * kk + 2 * r + 1] + sh2[c + 8 * (r >> 1) + 1];
+                    a2[4 * kk + r] = p.relu_s2 ? pack2_relu<F16>(x0, x1) : pack2<F16>(x0, x1);
+                }
+            }
+            float acc2[32];
+            wgmma_fence_regs<32>(acc2);
+            wgmma_fence();
+            tail_mma<64, 64, F16>(acc2, a2, b3desc);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs<32>(acc2);
+            store_tile<MODE_3X3S2, 64, F16>(e, acc2, 64, sh3, (bool)p.relu_s3, false, nullptr, &p.tm_out, &p.tm_res, ox0, oy0 + wg * 8, n,
+                                            true, true, &res_bar[wg], store_count, res_count);
+        }
+        if (e.wtid == 0) bulk_wait_all();
+    } else {
+        // ============================================================== PRODUCER: raw image patch -> normalised 16-bit [row][pixel][b g r 0]
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+        const int ptid = tid - kConsumerThreads;
+        const bool u8 = p.input_format == 1;
+        const int plane = p.H * p.W;
+        pdl_wait();
+        for (int tile = blockIdx.x, lt = 0; tile < p.num_tiles; tile += gridDim.x, ++lt) {
+            const uint32_t s = lt & 1, ph = (lt >> 1) & 1;
+            const int n = fast_div(tile, p.magic_tpi), t = tile - n * p.tiles_per_img;
+            const int ty = fast_div(t, p.magic_tx);
+            const int iy0 = 4 * 16 * ty - 3, ix0 = 4 * 8 * (t - ty * p.tiles_x) - 3;
+            const bool interior = iy0 >= 0 && ix0 >= 0 && iy0 + kS4Rows <= p.H && ix0 + kS4Cols <= p.W;
+            if (ptid == 0) LFD_TRACE(0, lt, 0);
+            mbar_wait(&empty[s], ph ^ 1);
+            if (ptid == 0) LFD_TRACE(0, lt, 1);
+            const uint32_t dst0 = smem_u32(smem + kS4Ring) + s * kS4PatchBytes;
+#pragma unroll 1
+            for (int j0 = 0; j0 < kS4PerThread; j0 += kS4Batch) {
+                uint32_t raw[kS4Batch][3];
+                bool ok[kS4Batch];
+#pragma unroll
+                for (int j = 0; j < kS4Batch; ++j) {
+                    const int q = ptid + (j0 + j) * kProdThreads;
+                    const int r = q / kS4Cols, c = q - r * kS4Cols;
+                    const int y = iy0 + r, x = ix0 + c;
+                    ok[j] = q < kS4Pix && (interior || ((unsigned)y < (unsigned)p.H && (unsigned)x < (unsigned)p.W));
+                    const ptrdiff_t pix = ok[j] ? (ptrdiff_t)n * plane + (ptrdiff_t)y * p.W + x : 0;
+                    if (u8) {
+                        const uint8_t* src = reinterpret_cast<const uint8_t*>(p.in_raw) + pix * 3;
+                        raw[j][0] = __ldg(src); raw[j][1] = __ldg(src + 1); raw[j][2] = __ldg(src + 2);
+                    } else {
+                        const float* src = reinterpret_cast<const float*>(p.in_raw) + (ok[j] ? (ptrdiff_t)n * 2 * plane + pix : 0);
+                        raw[j][0] = __float_as_uint(__ldg(src)); raw[j][1] = __float_as_uint(__ldg(src + plane));
+                        raw[j][2] = __float_as_uint(__ldg(src + 2 * plane));
+                    }
+                }
+#pragma unroll
+                for (int j = 0; j < kS4Batch; ++j) {
+                    const int q = ptid + (j0 + j) * kProdThreads;
+                    if (q >= kS4Pix) break;
+                    float f[3];
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) {
+                        f[k] = u8 ? ((float)raw[j][k] - 127.5f) * (1.0f / 127.5f) : __uint_as_float(raw[j][k]);
+                        if (!ok[j]) f[k] = 0.f;             // conv zero padding (of the normalised image)
+                    }
+                    const uint32_t lo = pack2<F16>(f[0], f[1]), hi = pack2<F16>(f[2], 0.f);   // rounding point R0
+                    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(dst0 + q * 8), "r"(lo), "r"(hi) : "memory");
+                }
+            }
+            fence_proxy_async_smem();
+            mbar_arrive(&full[s]);
+            if (ptid == 0) LFD_TRACE(0, lt, 2);
+        }
+    }
+    LFD_TL_END(p.tl);
+}
+
+// ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
 static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvParams* out, size_t* smem_bytes, int* grid) {
@@ -775,7 +1076,30 @@ static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvPara
     return 0;
 }
 
+static int configure_stem4(const ConvGeom& g, int num_sms, UmmaConvParams* out, size_t* smem_bytes, int* grid) {
+    if (g.Cin != 3 || g.ksize != 3 || g.stride != 2 || g.Cout != 64 || g.tail_cout != 64 || g.ds_cout) return -1;
+    UmmaConvParams p;
+    memset(&p, 0, sizeof(p));
+    p.mode = MODE_STEM4;
+    p.N = g.N; p.H = g.H; p.W = g.W; p.Cin = 3; p.Cout = 64; p.Cout2 = 64; p.Cf = 64;
+    p.H1 = (g.H - 1) / 2 + 1; p.W1 = (g.W - 1) / 2 + 1;           // stem0 / stem1 map
+    p.Ho = (p.H1 - 1) / 2 + 1; p.Wo = (p.W1 - 1) / 2 + 1;         // stem2 / stem3 map
+    if (g.H < 1 || g.W < 1 || g.Ho != p.Ho || g.Wo != p.Wo) return -1;
+    p.tiles_x = (p.Wo + 7) / 8;
+    p.tiles_per_img = p.tiles_x * ((p.Ho + 15) / 16);
+    p.num_tiles = p.tiles_per_img * g.N;
+    if (p.num_tiles >= (1 << 24) || p.tiles_per_img >= (1 << 16)) return -5;
+    p.magic_tpi = ((1ull << 40) + p.tiles_per_img - 1) / p.tiles_per_img;
+    p.magic_tx = ((1ull << 40) + p.tiles_x - 1) / p.tiles_x;
+    p.stg_nbuf = 1; p.stages = 2;
+    *smem_bytes = kS4Smem;
+    *grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
+    *out = p;
+    return 0;
+}
+
 int umma_conv_configure(const ConvGeom& g, int num_sms, UmmaConvParams* out, size_t* smem_bytes, int* grid) {
+    if (g.stem4) return configure_stem4(g, num_sms, out, smem_bytes, grid);
     // a second staging buffer per warpgroup is taken when it costs neither weight residency nor ring depth
     UmmaConvParams p1, p2;
     size_t s1 = 0, s2 = 0;
@@ -841,14 +1165,13 @@ int umma_conv_encode_maps(UmmaConvParams* p) {
     return 0;
 }
 
-template <int MODE, int COUT, bool F16>
-static cudaError_t launch_mode_t(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
-    // cudaFuncAttributeMaxDynamicSharedMemorySize is a PER-DEVICE attribute: one flag per device ordinal
-    static bool configured[kMaxDevices] = {};
+// configured: one flag per device ordinal of the kernel's own (cudaFuncAttributeMaxDynamicSharedMemorySize is a PER-DEVICE attribute)
+static cudaError_t launch_persistent(void (*kernel)(UmmaConvParams), bool* configured, int max_smem, const UmmaConvParams& p, size_t smem,
+                                     int grid, cudaStream_t st) {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
     if (!configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel<MODE, COUT, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(224 * 1024));
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
         if (e != cudaSuccess) return e;
         configured[dev] = true;
     }
@@ -864,7 +1187,19 @@ static cudaError_t launch_mode_t(const UmmaConvParams& p, size_t smem, int grid,
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = use_pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, conv_umma_kernel<MODE, COUT, F16>, p);
+    return cudaLaunchKernelEx(&cfg, kernel, p);
+}
+
+template <int MODE, int COUT, bool F16>
+static cudaError_t launch_mode_t(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
+    static bool configured[kMaxDevices] = {};
+    return launch_persistent(conv_umma_kernel<MODE, COUT, F16>, configured, 224 * 1024, p, smem, grid, st);
+}
+
+template <bool F16>
+static cudaError_t launch_stem4(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
+    static bool configured[kMaxDevices] = {};
+    return launch_persistent(stem4_kernel<F16>, configured, kS4Smem, p, smem, grid, st);
 }
 
 template <int MODE, int COUT>
@@ -891,6 +1226,7 @@ cudaError_t umma_conv_launch(const UmmaConvParams& p, size_t smem, int grid, cud
         case MODE_3X3S2: return launch_cout<MODE_3X3S2>(p, smem, grid, st);
         case MODE_1X1S2: return launch_cout<MODE_1X1S2>(p, smem, grid, st);
         case MODE_STEM: return launch_cout<MODE_STEM>(p, smem, grid, st);
+        case MODE_STEM4: return p.f16 ? launch_stem4<true>(p, smem, grid, st) : launch_stem4<false>(p, smem, grid, st);
     }
     return cudaErrorInvalidValue;
 }

@@ -98,7 +98,9 @@ class _Arena(object):
 class InferencePlan(object):
     """One native forward plan for a fixed input shape."""
 
-    def __init__(self, model, N, H, W, device, conv_impl=nat.CONV_UMMA, create_native=True, act_dtype='bf16'):
+    def __init__(self, model, N, H, W, device, conv_impl=nat.CONV_UMMA, create_native=True, act_dtype='bf16', fuse_stem=None):
+        """fuse_stem: run a four-conv 'faster' stem as one kernel (LFD_OP_STEM4) -- None: when its stem1 map would not stay in
+        L2 (see _use_stem4), True / False: always / never (tests).  LFD_B200_NO_STEM_FUSION=1 turns it off."""
         self.N, self.H, self.W = N, H, W
         if act_dtype not in ACT_DTYPES:
             raise ValueError("act_dtype must be 'bf16' or 'fp16' (got %r)" % (act_dtype,))
@@ -117,6 +119,7 @@ class InferencePlan(object):
         self.fuse_shortcuts = conv_impl == nat.CONV_UMMA and not os.environ.get('LFD_B200_NO_FUSED_SHORTCUT')
         # conv -> 1x1 conv pairs run as ONE kernel (tensor-core kernels only; the SIMT cross-check runs them unfused)
         self.fuse_tails = conv_impl == nat.CONV_UMMA and not os.environ.get('LFD_B200_NO_TAIL')
+        self.fuse_stem = fuse_stem
         self._build(model)
         self._finalize()
 
@@ -201,6 +204,49 @@ class InferencePlan(object):
         self._push(op)
         return ho, wo
 
+    def _l2_bytes(self):
+        dev = torch.device(self.device)
+        if dev.type == 'cuda' and torch.cuda.is_available():
+            return torch.cuda.get_device_properties(dev).L2_cache_size
+        return 50 << 20          # H100 SXM, as the 132-SM fallback assumes an H100
+
+    def _use_stem4(self, layers):
+        """A 'faster' stem (3x3/s2 3->64, 1x1, 3x3/s2 64->64, 1x1, all 64 channels) runs as one kernel when its stem1 map -- the
+        tensor the fusion keeps out of HBM -- would not stay in L2 between the two fused pairs (more than half of it).  Smaller
+        plans have no HBM round trip to remove and keep the two-kernel path."""
+        if not self.fuse_tails or self.fuse_stem is False or os.environ.get('LFD_B200_NO_STEM_FUSION') or len(layers) != 4:
+            return False
+        (c0, _, _), (c1, _, _), (c2, _, _), (c3, _, _) = layers
+
+        def conv3s2(c, cin):
+            return (c.in_channels == cin and c.out_channels == 64 and c.kernel_size == (3, 3) and c.stride == (2, 2)
+                    and c.padding == (1, 1) and c.groups == 1 and c.dilation == (1, 1))
+        if not (conv3s2(c0, 3) and conv3s2(c2, 64) and self._can_tail(c0, layers[1]) and self._can_tail(c2, layers[3])
+                and c1.out_channels == 64 and c3.out_channels == 64):
+            return False
+        if self.fuse_stem:
+            return True
+        stem1_bytes = self.N * _conv_out(self.H, 3, 2) * _conv_out(self.W, 3, 2) * 64 * 2
+        return stem1_bytes > self._l2_bytes() // 2
+
+    def _emit_stem4(self, layers, out_name, h, w):
+        (c0, n0, r0), tail1, (c2, n2, r2), (c3, n3, r3) = layers
+        h1, w1 = _conv_out(h, 3, 2), _conv_out(w, 3, 2)
+        ho, wo = _conv_out(h1, 3, 2), _conv_out(w1, 3, 2)
+        s0, b0 = self._fold(c0, n0)
+        s2, b2 = self._fold(c2, n2)
+        s3, b3 = self._fold(c3, n3)
+        op = dict(kind=nat.OP_STEM4, H=h, W=w, Cin=3, Ho=ho, Wo=wo, Cout=64, ksize=3, stride=2, relu=int(r0),
+                  w_bf16=self._add_bf16(pack_stem_weight(fold_scale(c0.weight, s0), self.tdtype)), shift=self._add_f32(b0), modules=(c0, n0),
+                  s2_w=self._add_bf16(pack_conv_weight(fold_scale(c2.weight, s2), 64, self.tdtype)), s2_shift=self._add_f32(b2), s2_relu=int(r2),
+                  s2_modules=(c2, n2),
+                  s3_w=self._add_bf16(pack_conv_weight(fold_scale(c3.weight, s3), 64, self.tdtype)), s3_shift=self._add_f32(b3), s3_relu=int(r3),
+                  s3_modules=(c3, n3))
+        op.update(self._tail_fields(tail1, 64))
+        op['out'] = self._tensor(out_name, self.N, ho, wo, 64)
+        self._push(op)
+        return ho, wo
+
     def _emit_conv(self, conv, norm, relu, in_name, out_name, h, w, res=None, gn_groups=0, cache=None, tail=None, shortcut=None):
         k, s = conv.kernel_size[0], conv.stride[0]
         if conv.kernel_size[0] != conv.kernel_size[1] or k not in (1, 3) or s not in (1, 2) or conv.padding[0] != k // 2 \
@@ -248,6 +294,9 @@ class InferencePlan(object):
         cur = None
         layers = bb.stem_layers()
         i = 0
+        if self._use_stem4(layers):
+            h, w = self._emit_stem4(layers, 'stem3', h, w)
+            cur, i = 'stem3', len(layers)
         while i < len(layers):
             conv, norm, relu = layers[i]
             tail = None
@@ -469,6 +518,9 @@ class InferencePlan(object):
                 o.ds_weight = bb + 2 * op['ds_w']
                 o.ds_shift = fb + 4 * op['ds_shift']
                 o.ds_out_off = offsets[op['out2']]
+            if op['kind'] == nat.OP_STEM4:
+                o.s2_weight, o.s2_shift, o.s2_relu = bb + 2 * op['s2_w'], fb + 4 * op['s2_shift'], op['s2_relu']
+                o.s3_weight, o.s3_shift, o.s3_relu = bb + 2 * op['s3_w'], fb + 4 * op['s3_shift'], op['s3_relu']
             o.in_off = offsets[op['inp']] if op.get('inp') is not None else -1
             o.out_off = offsets[op['out']] if op.get('out') is not None else -1
             o.res_off = offsets[op['res']] if op.get('res') is not None else -1
@@ -611,12 +663,15 @@ class InferencePlan(object):
         return raw.view(self.tdtype).view(self.N, op['Ho'], op['Wo'], c)
 
     def describe(self):
-        names = {nat.OP_STEM0: 'stem0', nat.OP_CONV: 'conv', nat.OP_GN_APPLY: 'gn_apply', nat.OP_HEAD_FINAL: 'head_final'}
+        """One row per launch.  The fused four-conv stem is reported as a 'stem0' row from the image to the stem3 map with
+        fused_stem=4: its bytes are then exactly the kernel's (image in, stem3 out, weights), its flops count stem0 at the
+        stem3 resolution + one 1x1 conv only (tests/debug_stem_fusion.py has the true count)."""
+        names = {nat.OP_STEM0: 'stem0', nat.OP_CONV: 'conv', nat.OP_GN_APPLY: 'gn_apply', nat.OP_HEAD_FINAL: 'head_final', nat.OP_STEM4: 'stem0'}
         rows = []
         for op in self._ops:
             rows.append(dict(kind=names[op['kind']], H=op['H'], W=op['W'], Cin=op['Cin'], Ho=op['Ho'], Wo=op['Wo'], Cout=op['Cout'],
                              ksize=op.get('ksize', 1), stride=op.get('stride', 1), res=op.get('res') is not None, tail_cout=op.get('tail_cout', 0), ds_cout=op.get('ds_cout', 0),
-                             out=op.get('out'), query=op.get('query')))
+                             out=op.get('out'), query=op.get('query'), fused_stem=4 if op['kind'] == nat.OP_STEM4 else 0))
         return rows
 
     def __del__(self):

@@ -13,7 +13,7 @@ _PKG = os.path.dirname(_HERE)
 LIB_PATH = os.environ.get('LFD_B200_LIB') or os.path.join(_PKG, 'liblfd_b200.so')   # LFD_B200_LIB: an alternative build of the SAME library (tuning experiments)
 MAX_LEVELS = 8
 
-OP_STEM0, OP_CONV, OP_GN_APPLY, OP_HEAD_FINAL = 0, 1, 2, 3
+OP_STEM0, OP_CONV, OP_GN_APPLY, OP_HEAD_FINAL, OP_STEM4 = 0, 1, 2, 3, 4
 INPUT_F32_NCHW, INPUT_U8_NHWC = 0, 1
 CONV_UMMA, CONV_SIMT = 0, 1
 DTYPE_BF16, DTYPE_FP16 = 0, 1
@@ -40,7 +40,9 @@ class Op(C.Structure):
                 ('tail_cout', C.c_int32), ('tail_relu', C.c_int32),
                 ('tail_weight', C.c_void_p), ('tail_scale', C.c_void_p), ('tail_shift', C.c_void_p),
                 ('ds_cout', C.c_int32), ('dtype', C.c_int32), ('max_ctas', C.c_int32), ('pad_', C.c_int32), ('ds_out_off', C.c_int64),
-                ('ds_weight', C.c_void_p), ('ds_shift', C.c_void_p)]
+                ('ds_weight', C.c_void_p), ('ds_shift', C.c_void_p),
+                ('s2_relu', C.c_int32), ('s3_relu', C.c_int32),
+                ('s2_weight', C.c_void_p), ('s2_shift', C.c_void_p), ('s3_weight', C.c_void_p), ('s3_shift', C.c_void_p)]
 
 
 class PostCfg(C.Structure):
@@ -105,6 +107,7 @@ SYMBOLS = {
     'lfd_last_error': (C.c_char_p, []),
     'lfd_device_sm_count': (_i, []),
     'lfd_conv_query': (_i, [_i] * 11 + [C.POINTER(_i)] * 4 + [C.POINTER(_i64)]),
+    'lfd_stem4_query': (_i, [_i] * 3 + [C.POINTER(_i), C.POINTER(_i64), C.POINTER(_i), C.POINTER(_i)]),
     'lfd_plan_create': (_i, [C.POINTER(Op), _i, _i, _i, _i, _i64, _i64, _i64, _i, C.POINTER(_vp)]),
     'lfd_plan_destroy': (_i, [_vp]),
     'lfd_plan_num_launches': (_i, [_vp]),
@@ -190,3 +193,11 @@ def conv_query(N, H, W, Cin, Ho, Wo, Cout, ksize, stride, tail_cout=0, ds_cout=0
     check(lib().lfd_conv_query(N, H, W, Cin, Ho, Wo, Cout, ksize, stride, tail_cout, ds_cout, C.byref(cc), C.byref(st), C.byref(res),
                                C.byref(nt), C.byref(smem)))
     return dict(cc=cc.value, stages=st.value, weights_resident=res.value, num_tiles=nt.value, smem_bytes=smem.value)
+
+
+def stem4_query(N, H, W):
+    """Tiles, shared memory and stem3 output size of the fused four-conv stem (LFD_OP_STEM4) on N images of H x W."""
+    nt, ho, wo = C.c_int(), C.c_int(), C.c_int()
+    smem = C.c_int64()
+    check(lib().lfd_stem4_query(N, H, W, C.byref(nt), C.byref(smem), C.byref(ho), C.byref(wo)))
+    return dict(num_tiles=nt.value, smem_bytes=smem.value, Ho=ho.value, Wo=wo.value)
