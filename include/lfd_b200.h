@@ -80,8 +80,8 @@ enum { LFD_DTYPE_BF16 = 0, LFD_DTYPE_FP16 = 1 };
  *              weight = bf16 packed [Cin/cc][ksize^2][cc/8][Cout][8] with cc from lfd_conv_query, ALREADY MULTIPLIED by the
  *              per-output-channel scale (folded BatchNorm); `scale` must be NULL; `shift` (fp32 [Cout], may be NULL) is rounded
  *              to bf16 and added on the tensor core;
- *              gn_groups > 0: also accumulates sum / sum-of-squares of the stored output per (image, group)
- *              into double[N][gn_groups][2] at stats_off (group size must be 8).
+ *              gn_groups > 0: also accumulates sum / sum-of-squares of the stored output (after residual and ReLU, as rounded
+ *              to bf16) per (image, group) into double[N][gn_groups][2] at stats_off (group size must be 8).
  *   GN_APPLY   y = relu(gamma * (x - mean) * rstd + beta) from the statistics at stats_off, bf16 -> bf16.
  *   HEAD_FINAL GN_APPLY (as above, rounded to bf16; gn_groups = 0: no normalisation, the input is an already activated tensor --
  *              heads built with norm_cfg=None) followed by the final 1x1 convs of one level: outputs

@@ -427,8 +427,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                 v0 = xin && c1 + (e.r0 >> 3) < p.Ho; v1 = xin && c1 + (e.r0 >> 3) + 1 < p.Ho;
             }
             const bool has_res = p.res != nullptr;
-            // GroupNorm partial sums are taken over the STORED (16-bit) values; one group = one 16-byte chunk (8 channels); a
-            // layer with statistics stores the raw (conv + shift) values
+            // GroupNorm partial sums are taken over the STORED (16-bit) values, after residual and ReLU; one group = one 16-byte
+            // chunk (8 channels)
             double* sdst = p.stats ? p.stats + (size_t)n * p.gn_groups * 2 : nullptr;
             if (p.Cout2) {
                 // fused 1x1 tail: D2[64 x Cout2] = round16(act(D + shift)) . W2, the A operand straight from the accumulator registers
@@ -453,7 +453,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                     wgmma_wait<0>();
                     wgmma_fence_regs<N2 / 2>(acc2);
                     if (e.wtid == 0) LFD_TRACE(1 + wg, lt, 3);
-                    store_tile<MODE, N2, F16>(e, acc2, N2, bias2, p.stats ? false : (bool)p.relu2, p.stats ? false : has_res, sdst,
+                    store_tile<MODE, N2, F16>(e, acc2, N2, bias2, (bool)p.relu2, has_res, sdst,
                                               &p.tm_out, &p.tm_res, c0, c1, n, v0, v1, &res_bar[wg], store_count, res_count);
                 };
                 switch (p.Cout2) {
@@ -463,7 +463,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                     default: tail(std::integral_constant<int, 128>()); break;
                 }
             } else {
-                store_tile<MODE, COUT, F16>(e, acc, COUT, bias, p.stats ? false : (bool)p.relu, p.stats ? false : has_res, sdst,
+                store_tile<MODE, COUT, F16>(e, acc, COUT, bias, (bool)p.relu, has_res, sdst,
                                             &p.tm_out, &p.tm_res, c0, c1, n, v0, v1, &res_bar[wg], store_count, res_count);
                 if constexpr (MODE == MODE_3X3S2) {
                     if (p.Cout3)
