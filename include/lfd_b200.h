@@ -305,7 +305,9 @@ typedef struct lfd_top {
                                   everything enqueued so far on branch w.  The per-level neck / head chains of the forward and of the
                                   backward are independent of the backbone's smaller stages: lfd/_train.py derives the masks from the
                                   read / write / accumulate role of every off[] entry. */
-    int32_t max_ctas;  /* CONV / WGRAD: upper bound on the persistent CTAs (0 = all), as in lfd_op */
+    int32_t max_ctas;  /* CONV / WGRAD: upper bound on the persistent CTAs (0 = all), as in lfd_op.  BN_* / GN_APPLY / HEAD_FINAL* /
+                          NORM_BWD_* / WGRAD_STEM size their grids from the SM count: max_ctas > 0 stands in for it (so a kernel with
+                          k blocks per SM gets k * max_ctas blocks) and every thread walks more of its grid-stride loop */
     float eps, momentum;
     int64_t off[8];
     const void* ptr[6];

@@ -187,7 +187,8 @@ static int check_op(const lfd_op& o) {
     return LFD_OK;
 }
 
-// GN_APPLY / HEAD_FINAL size their grids from the SM count: a max_ctas bound (side-branch layers, see lfd_op) scales them the same way
+// GN_APPLY / HEAD_FINAL and the SIMT training ops size their grids from the SM count: a max_ctas bound (side-branch layers, see lfd_op;
+// forced small grids in the tests) scales them the same way
 static int bounded_sms(int max_ctas) {
     const int sms = sm_count() > 0 ? sm_count() : 132;
     return max_ctas > 0 && max_ctas < sms ? max_ctas : sms;
@@ -758,7 +759,7 @@ static T* at(uint8_t* ws, int64_t off) { return off >= 0 ? reinterpret_cast<T*>(
 
 static int launch_top(const PlannedTop& pt, const void* input, int fmt, uint8_t* ws, cudaStream_t st) {
     const lfd_top& t = pt.op;
-    const int sms = sm_count();
+    const int sms = bounded_sms(t.max_ctas);   // the SIMT ops size their grids from it; CONV reads max_ctas itself (conv_op_of)
     switch (t.kind) {
         case LFD_TOP_PACK:
             CUDA_TRY(pack_launch(reinterpret_cast<const PackDesc*>(t.ptr[0]), t.n_desc, t.max_n, st));
@@ -813,7 +814,7 @@ static int launch_top(const PlannedTop& pt, const void* input, int fmt, uint8_t*
             p.N = t.N; p.HW = t.H * t.W; p.C = t.Cout; p.groups = t.groups; p.n_out = no; p.n_cls = t.n_cls;
             p.P = t.P; p.point_off = t.point_off; p.cls_stride = t.cls_stride; p.eps = t.eps; p.f16 = 0; p.tl = nullptr;
             if ((t.n_cls && !p.cls) || (t.n_reg && !p.reg)) return fail(LFD_ERR_INVALID, "head_final: output pointers missing");
-            CUDA_TRY(head_final_launch(p, sm_count(), st));
+            CUDA_TRY(head_final_launch(p, sms, st));
             break;
         }
         case LFD_TOP_HEAD_FINAL_BWD: {
@@ -856,7 +857,7 @@ static int launch_top(const PlannedTop& pt, const void* input, int fmt, uint8_t*
             float* ds = at<float>(ws, t.off[5]);
             if (!x || !dz || !ds) return fail(LFD_ERR_INVALID, "wgrad: missing tensor");
             if (t.impl == LFD_WGRAD_SIMT) CUDA_TRY(wgrad_simt_launch(g, x, dz, ds, st));
-            else CUDA_TRY(wgrad_umma_launch(g, x, dz, ds, t.max_ctas > 0 && t.max_ctas < sms ? t.max_ctas : sms, st));
+            else CUDA_TRY(wgrad_umma_launch(g, x, dz, ds, sms, st));
             break;
         }
         case LFD_TOP_WGRAD_STEM: {

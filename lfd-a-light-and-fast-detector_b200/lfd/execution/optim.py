@@ -8,6 +8,9 @@ It is a torch.optim.Optimizer: `param_groups` (and the dicts in it) are shared w
 lr schedulers and the warm-up hook that were built on the original optimizer keep driving the learning rate; `state_dict()` /
 `load_state_dict()` use torch.optim.SGD's format (per-parameter 'momentum_buffer'), i.e. checkpoints stay interchangeable
 with the reference's.
+
+Like torch.optim.SGD, a parameter's momentum buffer starts as its first (weight-decayed) gradient, undamped: the flat runs whose
+parameters have no buffer yet step with dampening 0 on their zeroed buffer slots, which gives exactly that.
 """
 import ctypes as C
 
@@ -30,6 +33,7 @@ class FusedSGD(torch.optim.Optimizer):
         self._flat, self._mom, self._runs = None, None, None
         self._sq = None
         self._pending = None      # momentum buffers loaded before the flat buffer exists
+        self._has_buf = set()     # id() of the parameters that have a momentum buffer (stepped, or loaded from a state)
         for g in param_groups:
             if g.get('maximize'):
                 raise NotImplementedError('FusedSGD implements minimisation only')
@@ -52,31 +56,39 @@ class FusedSGD(torch.optim.Optimizer):
             old = self._state_buffers() if self._flat is not None else (self._pending or {})
             self._flat = flat
             self._mom = torch.zeros_like(flat.data)
+            self._has_buf = set()
             for p, off in zip(flat.params, flat.offsets):
                 buf = old.get(id(p))
                 if buf is not None:
                     self._mom[off:off + p.numel()].copy_(buf.reshape(-1))
+                    self._has_buf.add(id(p))
             self._pending = None
             self._sq = torch.zeros(1, dtype=torch.float64, device=flat.data.device)
-            group_of = {}
-            for gi, g in enumerate(self.param_groups):
-                for p in g['params']:
-                    group_of[id(p)] = gi
-            runs = []          # (begin, end, group index): maximal runs of flat slots with the same hyper-parameters
-            for p, off in zip(flat.params, flat.offsets):
-                if id(p) not in group_of:
-                    raise ValueError('a model parameter is missing from the optimizer param_groups')
-                end = off + (p.numel() + 3) // 4 * 4
-                gi = group_of[id(p)]
-                if runs and runs[-1][2] == gi and runs[-1][1] == off:
-                    runs[-1][1] = end
-                else:
-                    runs.append([off, end, gi])
-            self._runs = runs
+            self._make_runs()
         return flat
 
+    def _make_runs(self):
+        """Maximal runs of flat slots with the same hyper-parameters and the same momentum-buffer state: (begin, end, group index,
+        every parameter of the run has a buffer)."""
+        group_of = {}
+        for gi, g in enumerate(self.param_groups):
+            for p in g['params']:
+                group_of[id(p)] = gi
+        runs = []
+        for p, off in zip(self._flat.params, self._flat.offsets):
+            if id(p) not in group_of:
+                raise ValueError('a model parameter is missing from the optimizer param_groups')
+            end = off + (p.numel() + 3) // 4 * 4
+            key = (group_of[id(p)], id(p) in self._has_buf)
+            if runs and runs[-1][2:] == list(key) and runs[-1][1] == off:
+                runs[-1][1] = end
+            else:
+                runs.append([off, end, key[0], key[1]])
+        self._runs = runs
+
     def _state_buffers(self):
-        return {id(p): self._mom[off:off + p.numel()].view(p.shape) for p, off in zip(self._flat.params, self._flat.offsets)}
+        return {id(p): self._mom[off:off + p.numel()].view(p.shape) for p, off in zip(self._flat.params, self._flat.offsets)
+                if id(p) in self._has_buf}
 
     # ------------------------------------------------------------------ torch.optim.Optimizer interface
     def zero_grad(self, set_to_none=False):
@@ -96,13 +108,21 @@ class FusedSGD(torch.optim.Optimizer):
         with torch.cuda.device(flat.data.device):
             if max_norm and max_norm > 0:
                 nat.check(L.lfd_grad_sqnorm(nat.ptr(flat.grad), flat.numel, nat.ptr(self._sq), st))
-            for b, e, gi in self._runs:
+            started = []
+            for b, e, gi, has_buf in self._runs:
                 g = self.param_groups[gi]
                 mom = float(g.get('momentum', 0.0))
+                # first step of a buffer: torch.optim.SGD sets buf = grad, i.e. momentum * 0 + (1 - 0) * grad on the zeroed slots
+                damp = float(g.get('dampening', 0.0)) if has_buf else 0.0
                 nat.check(L.lfd_sgd_step(C.c_void_p(flat.data.data_ptr() + 4 * b), C.c_void_p(flat.grad.data_ptr() + 4 * b),
-                                         C.c_void_p(self._mom.data_ptr() + 4 * b), e - b, float(g['lr']), mom, float(g.get('dampening', 0.0)),
+                                         C.c_void_p(self._mom.data_ptr() + 4 * b), e - b, float(g['lr']), mom, damp,
                                          float(g.get('weight_decay', 0.0)), int(bool(g.get('nesterov', False))), float(max_norm or 0.0),
                                          float(grad_scale), nat.ptr(self._sq), st))
+                if not has_buf and mom != 0.0:
+                    started.append((b, e))
+            if started:
+                self._has_buf |= {id(p) for p, off in zip(flat.params, flat.offsets) if any(b <= off < e for b, e in started)}
+                self._make_runs()
         if max_norm and max_norm > 0:
             return self._sq.sqrt() * abs(float(grad_scale))
         return None
@@ -111,8 +131,8 @@ class FusedSGD(torch.optim.Optimizer):
         """torch.optim.SGD format."""
         flat = self._sync()
         index = {id(p): i for i, p in enumerate(p for g in self.param_groups for p in g['params'])}
-        state = {index[id(p)]: {'momentum_buffer': buf.clone()} for p, buf in zip(flat.params, self._state_buffers().values())
-                 if any(float(g.get('momentum', 0.0)) != 0.0 for g in self.param_groups)}
+        bufs = self._state_buffers()          # (torch.optim.SGD has no entry for a parameter that never stepped with momentum)
+        state = {index[id(p)]: {'momentum_buffer': bufs[id(p)].clone()} for p in flat.params if id(p) in bufs}
         groups, n = [], 0
         for g in self.param_groups:
             d = {k: v for k, v in g.items() if k != 'params'}
@@ -129,6 +149,10 @@ class FusedSGD(torch.optim.Optimizer):
         if self._flat is None:
             self._pending = bufs
         else:
-            for p, off in zip(self._flat.params, self._flat.offsets):
+            for p, off in zip(self._flat.params, self._flat.offsets):     # the loaded state replaces the current one, as in torch
                 if id(p) in bufs:
                     self._mom[off:off + p.numel()].copy_(bufs[id(p)].reshape(-1).to(self._mom.device))
+                else:
+                    self._mom[off:off + p.numel()].zero_()
+            self._has_buf = {id(p) for p in self._flat.params if id(p) in bufs}
+            self._make_runs()
