@@ -205,7 +205,7 @@ static int plan_op(const lfd_op& o, int conv_impl, PlannedOp* out) {
         if (rc) return fail(LFD_ERR_UNSUPPORTED, "conv %dx%d s%d Cin=%d Cout=%d unsupported (rc=%d)", o.ksize, o.ksize, o.stride, o.Cin, o.Cout, rc);
         if (o.kind == LFD_OP_CONV && out->cp.Cc != o.cc) return fail(LFD_ERR_INVALID, "weights packed with cc=%d but the kernel needs cc=%d", o.cc, out->cp.Cc);
         if (o.max_ctas < 0) return fail(LFD_ERR_INVALID, "max_ctas = %d", o.max_ctas);
-        if (o.max_ctas > 0 && out->grid > o.max_ctas) out->grid = o.max_ctas;   // tiles are strided by gridDim: any grid size is valid
+        if (o.max_ctas > 0 && out->grid > o.max_ctas) out->grid = o.max_ctas;   // tiles are strided by gridDim (fused stem: contiguous runs): any grid size is valid
     }
     (void)conv_impl;
     return LFD_OK;
@@ -242,6 +242,7 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
             if (conv_impl == LFD_CONV_SIMT) return fail(LFD_ERR_UNSUPPORTED, "the SIMT cross-check kernels do not implement the fused stem (plan its four convs)");
             UmmaConvParams p = po.cp;
             p.in_raw = input; p.input_format = input_format; p.in = nullptr;
+            p.in_words = input_format == LFD_INPUT_U8_NHWC && o.W % 4 == 0 && (reinterpret_cast<uintptr_t>(input) & 3) == 0;
             p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off); p.res = nullptr; p.stats = nullptr;
             p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift; p.relu = o.relu;
             p.w2 = reinterpret_cast<const __nv_bfloat16*>(o.tail_weight); p.shift2 = o.tail_shift; p.relu2 = o.tail_relu;

@@ -70,6 +70,7 @@ struct alignas(64) UmmaConvParams {
     const __nv_bfloat16* w_s3;
     const float* shift_s3;
     int relu_s2, relu_s3, H1, W1;
+    int in_words;               // MODE_STEM4: u8 NHWC image with W % 4 == 0 at a 4-byte aligned address -> the producer loads aligned words
 };
 
 // returns 0 when the geometry is supported by the wgmma kernel

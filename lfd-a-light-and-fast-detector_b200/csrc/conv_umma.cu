@@ -650,13 +650,17 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
 
 // ---------------------------------------------------------------------------------------------------
 // MODE_STEM4: the 'faster' stem -- stem0 3x3/s2 3->64, stem1 1x1 64->64, stem2 3x3/s2 64->64, stem3 1x1 64->64 -- as ONE kernel.
-// Tiles are 16 x 8 pixels of the final (stem3) map, as in MODE_3X3S2.  Per tile:
+// Tiles are 16 x 8 pixels of the final (stem3) map, as in MODE_3X3S2.  Each CTA walks a contiguous run of tiles in row-major
+// order (floor or ceil of num_tiles / gridDim tiles).  Per tile:
 //   producer   the raw-image patch (67 rows x 36 pixels from image (4 oy0 - 3, 4 ox0 - 3)) in the MODE_STEM format -> ring stage;
-//   consumers  stem0 + stem1 on the 33 x 17 stem1 pixels stem2's halo needs (rows 2 oy0 - 1 .., columns 2 ox0 - 1 ..), as 16
-//              MODE_STEM m64 blocks of 8 x 8 stem1 pixels (the 15 of the cover below plus a repeat of the last, 8 per warpgroup);
-//              each block's stem1 result (+shift, ReLU, 16-bit) goes straight into the MODE_3X3S2 parity planes, zeros where the
-//              pixel lies outside the stem1 map (stem2's padding); then stem2 as the MODE_3X3S2 main loop (same MMA order as the
-//              two-kernel path: k16-major, tap-minor), the stem3 tail and the TMA store of the two-kernel path.
+//   consumers  stem0 + stem1 on the 33 x 17 stem1 pixels stem2's halo needs (rows 2 oy0 - 1 .., columns 2 ox0 - 1 ..), as
+//              MODE_STEM m64 blocks (s4_block), two per MMA group; each block's stem1 result (+shift, ReLU, 16-bit) goes into the
+//              stem2 parity planes by stmatrix, zeros where the pixel lies outside the stem1 map (stem2's padding); then stem2 as
+//              the MODE_3X3S2 main loop (same MMA order as the two-kernel path: k16-major, tap-minor), the stem3 tail and the TMA
+//              store of the two-kernel path.
+// Column 0 of tile (ty, tx + 1) is column 16 of tile (ty, tx).  So, within a run, a tile whose left neighbour came before it
+// inherits that column (copied inside the planes after stem2 of the neighbour, see s4_slot) and computes columns 1..16 only:
+// 9 blocks instead of 14.
 // The stem1 tensor never exists outside shared memory.  Every wgmma group is waited for before the next barrier / divergent code.
 // Trace (LFD_B200_TRACE builds, tests/debug_stem_fusion.py --trace), per tile lt:
 //   role 0        producer            : wait_empty  got_empty  patch_written(arrived_full)  -
@@ -667,7 +671,19 @@ static constexpr int kS4RowBytes = kS4Cols * 8;                                 
 static constexpr int kS4PatchBytes = kS4Pix * 8;                                                   // 19296
 static constexpr int kS4PerThread = (kS4Pix + kProdThreads - 1) / kProdThreads;                   // 19
 static constexpr int kS4Batch = 5;                                                                 // patch pixels in flight per producer thread
-static constexpr int kS4Lbo = 595 * 16;                                                            // plane pitch (MODE_3X3S2, 64 channels)
+// word loader: a patch row is 10 groups of 4 pixels = 3 aligned 32-bit words (see the producer)
+static constexpr int kS4Groups = kS4Rows * 10;                                                     // 670
+static constexpr int kS4GroupsPerThread = (kS4Groups + kProdThreads - 1) / kProdThreads;          // 6
+static constexpr int kS4GroupBatch = 3;                                                            // groups in flight per producer thread
+// The packed row-32 block reads up to 7 stem1 columns past the patch row (rows it discards); the last stage needs this tail.
+static constexpr int kS4PatchOverrun = 768;
+// Parity planes of the stem1 halo, per 8-channel chunk: [a odd, b odd] 16 x 9 | [a odd, b even] 16 x 9 | [a even, b odd] 17 x 9 |
+// [a even, b even] 17 x 9 slots of 16 B (rows of pitch 9).  The even-b plane starts 3 slots (mod 8) after the odd-b plane of the
+// same row parity: the 8 pixels b0 .. b0 + 7 (b0 odd) of one stmatrix then fill 8 distinct 16-byte bank groups.
+LFD_DEVINL constexpr int s4_slot(int a, int b) {
+    return ((a & 1) ? ((b & 1) ? 0 : 147) : ((b & 1) ? 291 : 446)) + (a >> 1) * 9 + (b >> 1);
+}
+static constexpr int kS4Lbo = 599 * 16;                                                            // plane pitch (odd in 16 B)
 // shared-memory map (bytes)
 static constexpr int kS4Bar = 0;                    // full[2] | empty[2] | weights | res_bar[2] (unused: no residual)
 static constexpr int kS4Shift = 256;                // fp32 shifts of stem0 .. stem3, 64 each
@@ -676,14 +692,28 @@ static constexpr int kS4W0 = kS4Staging + 2 * 8192; // stem0 [3][2][64][8]
 static constexpr int kS4W1 = kS4W0 + 6144;          // stem1 [8][64][8]
 static constexpr int kS4W2 = kS4W1 + 8192;          // stem2 [9][8][64][8]
 static constexpr int kS4W3 = kS4W2 + 73728;         // stem3 [8][64][8]
-static constexpr int kS4Planes = kS4W3 + 8192;      // EE | EO | OE | OO x 8 channel chunks
+static constexpr int kS4Planes = kS4W3 + 8192;      // the parity planes x 8 channel chunks
 static constexpr int kS4Ring = kS4Planes + 8 * kS4Lbo;
-static constexpr int kS4Smem = kS4Ring + 2 * kS4PatchBytes;   // 229440 (<= 227 KB)
+static constexpr int kS4Smem = kS4Ring + 2 * kS4PatchBytes + kS4PatchOverrun;   // 230720 (<= 227 KB)
 static constexpr int kS4WBytes = kS4Planes - kS4W0;
+static_assert(kS4Smem <= 227 * 1024, "stem4 shared memory");
 
-// origin (stem1 halo row a0, column b0) of m64 block i: rows {0, 8, 16, 24, 25} x columns {0, 8, 9}; block 15 repeats block 14
-LFD_DEVINL int s4_block_a0(int i) { const int r = (i < 15 ? i : 14) / 3; return r < 4 ? 8 * r : 25; }
-LFD_DEVINL int s4_block_b0(int i) { const int c = (i < 15 ? i : 14) % 3; return c == 0 ? 0 : 7 + c; }
+// m64 block i of a tile's stem1 cover, origin (halo row a0, column b0):
+//   i < 8     rows 8 (i / 2) .. + 7, columns 1 + 8 (i % 2) .. + 7     (every tile)
+//   i = 8     row 32 packed: its 8-row groups step along the row (SBO = 8 stem1 columns), columns 1 .. 16 kept
+//   9 .. 12   rows 8 (i - 9) .. + 7, columns 0 .. 7                   (tiles that do not inherit column 0)
+//   i = 13    row 32 packed, columns 0 .. 15 kept
+// Only the first two 8-row groups (warp 0 of the warpgroup) of a packed block are kept.
+LFD_DEVINL void s4_block(int i, int& a0, int& b0, bool& packed) {
+    packed = i == 8 || i == 13;
+    a0 = packed ? 32 : 8 * (i < 8 ? i >> 1 : i - 9);
+    b0 = i < 8 ? 1 + 8 * (i & 1) : (i == 8 ? 1 : 0);
+}
+// This CTA's run of tiles [t0, t1)
+LFD_DEVINL void s4_run(int num_tiles, int& t0, int& t1) {
+    t0 = (int)((uint64_t)blockIdx.x * (uint32_t)num_tiles / gridDim.x);
+    t1 = (int)((uint64_t)(blockIdx.x + 1) * (uint32_t)num_tiles / gridDim.x);
+}
 
 LFD_DEVINL void consumers_bar_sync() { asm volatile("bar.sync 3, 256;" ::: "memory"); }   // the two consumer warpgroups
 
@@ -755,39 +785,53 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
         // descriptors: stem0 A = the patch (MODE_STEM view: SBO = 2 patch rows, LBO = 16 B), B = [kh][2][64][8];
         // stem1 / stem3 B = [8][64][8]; stem2 A = the planes (SBO = pitch-9 rows, LBO = plane pitch), B = [tap][8][64][8]
         const uint64_t adesc_stem = wgmma_desc(0, 16, 2 * kS4RowBytes);
+        const uint64_t adesc_row = wgmma_desc(0, 16, 8 * 16);          // packed row 32: 8-row groups 8 stem1 columns apart
         const uint64_t b0desc = wgmma_desc(smem_u32(smem + kS4W0), 64 * 16, 128);
         const uint64_t b1desc = wgmma_desc(smem_u32(smem + kS4W1), 64 * 16, 128);
         const uint64_t b2desc = wgmma_desc(smem_u32(smem + kS4W2), 64 * 16, 128);
         const uint64_t b3desc = wgmma_desc(smem_u32(smem + kS4W3), 64 * 16, 128);
         const uint64_t adesc_pl = wgmma_desc(planes + (uint32_t)wg * 8u * 144u, kS4Lbo, 144);
-        // this thread's stem1 pixels inside a block: (row 2 (warp & 3) + h, column lane / 4)
+        // this thread's stem1 pixels inside a block: (row 2 (warp & 3) + h, column lane / 4); its stmatrix row address is the
+        // pixel (row 2 (warp & 3) + sh, column sc), channel chunk lane / 16 (+ 2 per stmatrix)
         const int brow = 2 * (warp & 3), bcol = lane >> 2;
+        const int sh = (lane >> 3) & 1, sc = lane & 7;
 
+        int tile0, tile1;
+        s4_run(p.num_tiles, tile0, tile1);
         uint32_t store_count = 0, res_count = 0;
-        for (int tile = blockIdx.x, lt = 0; tile < p.num_tiles; tile += gridDim.x, ++lt) {
+        for (int tile = tile0, lt = 0; tile < tile1; ++tile, ++lt) {
             const uint32_t s = lt & 1, ph = (lt >> 1) & 1;
             const int n = fast_div(tile, p.magic_tpi);
             const int t = tile - n * p.tiles_per_img;
             const int ty = fast_div(t, p.magic_tx);
-            const int oy0 = ty * 16, ox0 = (t - ty * p.tiles_x) * 8;
+            const int tx = t - ty * p.tiles_x;
+            const int oy0 = ty * 16, ox0 = tx * 8;
+            // column 0 was copied from the previous tile / column 16 goes to the next tile
+            const bool inherit = tile > tile0 && tx > 0, pass_on = tile + 1 < tile1 && tx + 1 < p.tiles_x;
             if (e.wtid == 0) LFD_TRACE(1 + wg, lt, 0);
             mbar_wait(&full[s], ph);
             if (e.wtid == 0) LFD_TRACE(1 + wg, lt, 1);
             fence_proxy_async_smem();
             const uint32_t patch = smem_u32(smem + kS4Ring) + s * kS4PatchBytes;
 
-            // ---- stem0 + stem1 on this warpgroup's 8 blocks, two per MMA group
-#pragma unroll
-            for (int kp = 0; kp < 4; ++kp) {
-                const int i0 = wg * 8 + 2 * kp;
+            // ---- stem0 + stem1, two blocks per MMA group: warpgroup 0 takes blocks 0 .. 4 (of 9) or 0 .. 6 (of 14), warpgroup 1
+            //      the rest; an odd count repeats its last block (same bits to the same slots)
+            const int nblk = inherit ? 9 : 14, half = (nblk + 1) >> 1;
+            const int first = wg ? half : 0, cnt = wg ? nblk - half : half;
+#pragma unroll 1
+            for (int kp = 0; kp < (cnt + 1) >> 1; ++kp) {
+                int blk[2] = {first + 2 * kp, first + min(2 * kp + 1, cnt - 1)};
                 float c0[2][32];
                 wgmma_fence_regs<32>(c0[0]);
                 wgmma_fence_regs<32>(c0[1]);
                 wgmma_fence();
 #pragma unroll
                 for (int q = 0; q < 2; ++q) {
-                    const uint32_t boff = (uint32_t)(s4_block_a0(i0 + q) * 2 * kS4RowBytes + s4_block_b0(i0 + q) * 16);
-                    const uint64_t ad = adesc_stem + ((patch + boff) >> 4);
+                    int a0, b0;
+                    bool packed;
+                    s4_block(blk[q], a0, b0, packed);
+                    const uint32_t boff = (uint32_t)(a0 * 2 * kS4RowBytes + b0 * 16);
+                    const uint64_t ad = (packed ? adesc_row : adesc_stem) + ((patch + boff) >> 4);
 #pragma unroll
                     for (int kh = 0; kh < 3; ++kh)
                         wgmma_ss<64, F16>(c0[q], ad + (uint32_t)(kh * kS4RowBytes / 16), b0desc + (uint32_t)(kh * 2 * 64 * 16 / 16), kh != 0);
@@ -819,27 +863,35 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                 wgmma_wait<0>();
                 wgmma_fence_regs<32>(c1[0]);
                 wgmma_fence_regs<32>(c1[1]);
-                // stem1 (+shift, ReLU) -> 16 bits -> the stem2 parity planes; zeros outside the stem1 map (stem2's padding)
+                // stem1 (+shift, ReLU) -> 16 bits -> the stem2 parity planes; zeros outside the stem1 map (stem2's padding).
+                // One 8x8 stmatrix = 8 channels (one plane chunk) of 8 pixels of one block row, each a 16-byte plane slot.
                 float2 bv[8];
 #pragma unroll
                 for (int j = 0; j < 8; ++j) bv[j] = *reinterpret_cast<const float2*>(sh1 + 8 * j + 2 * e.tq);
 #pragma unroll
                 for (int q = 0; q < 2; ++q) {
+                    int a0, b0;
+                    bool packed;
+                    s4_block(blk[q], a0, b0, packed);
+                    if (packed && (warp & 3)) continue;         // warp-uniform: the discarded groups of the packed row
+                    uint32_t v[8][2];
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
-                        const int a = s4_block_a0(i0 + q) + brow + h, b = s4_block_b0(i0 + q) + bcol;
+                        const int a = packed ? a0 : a0 + brow + h, b = b0 + bcol + (packed ? 8 * h : 0);
                         const int y1 = 2 * oy0 - 1 + a, x1 = 2 * ox0 - 1 + b;
                         const bool in = (unsigned)y1 < (unsigned)p.H1 && (unsigned)x1 < (unsigned)p.W1;
-                        const uint32_t slot = ((a & 1) ? 0u : 288u) + ((b & 1) ? 0u : ((a & 1) ? 144u : 153u)) + (uint32_t)((a >> 1) * 9 + (b >> 1));
-                        const uint32_t addr = planes + slot * 16u + 4u * e.tq;
 #pragma unroll
                         for (int j = 0; j < 8; ++j) {
                             const float x0 = c1[q][4 * j + 2 * h] + bv[j].x, x1v = c1[q][4 * j + 2 * h + 1] + bv[j].y;
-                            uint32_t v = p.relu2 ? pack2_relu<F16>(x0, x1v) : pack2<F16>(x0, x1v);
-                            v = in ? v : 0u;
-                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr + (uint32_t)(j * kS4Lbo)), "r"(v) : "memory");
+                            const uint32_t w = p.relu2 ? pack2_relu<F16>(x0, x1v) : pack2<F16>(x0, x1v);
+                            v[j][h] = in ? w : 0u;
                         }
                     }
+                    const int a = packed ? a0 : a0 + brow + sh, b = b0 + sc + (packed ? 8 * sh : 0);
+                    const uint32_t addr = planes + (uint32_t)s4_slot(a, b) * 16u + (uint32_t)(lane >> 4) * kS4Lbo;
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)
+                        stmatrix_x4(addr + (uint32_t)(2 * k * kS4Lbo), v[2 * k][0], v[2 * k][1], v[2 * k + 1][0], v[2 * k + 1][1]);
                 }
             }
             __syncwarp();
@@ -857,12 +909,25 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
             for (int k16 = 0; k16 < 4; ++k16)
 #pragma unroll
                 for (int tap = 0; tap < 9; ++tap)
-                    wgmma_ss<64, F16>(acc, adesc_pl + (uint32_t)(k16 * 2 * kS4Lbo / 16 + tap_view<MODE_3X3S2>(tap)),
+                    wgmma_ss<64, F16>(acc, adesc_pl + (uint32_t)(k16 * 2 * kS4Lbo / 16 + s4_slot(tap / 3, tap % 3)),
                                       b2desc + (uint32_t)((tap * 8 + 2 * k16) * 64 * 16 / 16), (k16 | tap) != 0);
             wgmma_commit();
             wgmma_wait<0>();
             wgmma_fence_regs<32>(acc);
             consumers_bar_sync();                       // both warpgroups are done reading the planes: the next tile may write them
+            if (pass_on) {
+                // column 16 -> column 0 (even-b slot 8 -> 0) for the next tile.  Each row is copied by the warp that writes its
+                // column 16 in the next tile (blocks 1, 3 | 5, 7 and the packed block 8 of warpgroup 0 | 1: warp w writes rows
+                // a0 + 2w, + 1), so program order alone keeps the copy ahead of that write; no barrier is needed.
+                const int rs = lane >> 3, a = 16 * wg + brow + (rs & 1) + 8 * (rs >> 1);
+                const uint32_t src = planes + (uint32_t)(lane & 7) * kS4Lbo + (uint32_t)s4_slot(a, 16) * 16u;
+                sts128(src - 8u * 16u, lds128(src));
+                if (wg == 1 && brow == 0 && lane < 8) {
+                    const uint32_t src32 = planes + (uint32_t)lane * kS4Lbo + (uint32_t)s4_slot(32, 16) * 16u;
+                    sts128(src32 - 8u * 16u, lds128(src32));
+                }
+                __syncwarp();
+            }
 #ifdef LFD_B200_TRACE
             if (e.wtid == 0 && p.trace && blockIdx.x == 0 && lt < 16) p.trace[(3 * 32 + wg + 2 * lt) * 4 + 3] = clock64();
 #endif
@@ -896,7 +961,9 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
         const bool u8 = p.input_format == 1;
         const int plane = p.H * p.W;
         pdl_wait();
-        for (int tile = blockIdx.x, lt = 0; tile < p.num_tiles; tile += gridDim.x, ++lt) {
+        int tile0, tile1;
+        s4_run(p.num_tiles, tile0, tile1);
+        for (int tile = tile0, lt = 0; tile < tile1; ++tile, ++lt) {
             const uint32_t s = lt & 1, ph = (lt >> 1) & 1;
             const int n = fast_div(tile, p.magic_tpi), t = tile - n * p.tiles_per_img;
             const int ty = fast_div(t, p.magic_tx);
@@ -906,38 +973,87 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
             mbar_wait(&empty[s], ph ^ 1);
             if (ptid == 0) LFD_TRACE(0, lt, 1);
             const uint32_t dst0 = smem_u32(smem + kS4Ring) + s * kS4PatchBytes;
+            if (p.in_words) {
+                // ix0 = 1 (mod 4): group g of a patch row = image columns ix0 - 1 + 4g .. + 3 = patch columns 4g - 1 .. 4g + 2,
+                // 12 bytes at a 4-byte aligned address (W % 4 == 0).  A group lies wholly inside or wholly outside the image, so
+                // no load touches a byte outside the tensor.  Two batches of 3 groups: all loads of a batch are issued before any
+                // is used (6 groups at once do not fit the producer's 56 registers).
 #pragma unroll 1
-            for (int j0 = 0; j0 < kS4PerThread; j0 += kS4Batch) {
-                uint32_t raw[kS4Batch][3];
-                bool ok[kS4Batch];
+                for (int j0 = 0; j0 < kS4GroupsPerThread; j0 += kS4GroupBatch) {
+                    uint32_t wd[kS4GroupBatch][3];
+                    bool ok[kS4GroupBatch];
 #pragma unroll
-                for (int j = 0; j < kS4Batch; ++j) {
-                    const int q = ptid + (j0 + j) * kProdThreads;
-                    const int r = q / kS4Cols, c = q - r * kS4Cols;
-                    const int y = iy0 + r, x = ix0 + c;
-                    ok[j] = q < kS4Pix && (interior || ((unsigned)y < (unsigned)p.H && (unsigned)x < (unsigned)p.W));
-                    const ptrdiff_t pix = ok[j] ? (ptrdiff_t)n * plane + (ptrdiff_t)y * p.W + x : 0;
-                    if (u8) {
-                        const uint8_t* src = reinterpret_cast<const uint8_t*>(p.in_raw) + pix * 3;
-                        raw[j][0] = __ldg(src); raw[j][1] = __ldg(src + 1); raw[j][2] = __ldg(src + 2);
-                    } else {
-                        const float* src = reinterpret_cast<const float*>(p.in_raw) + (ok[j] ? (ptrdiff_t)n * 2 * plane + pix : 0);
-                        raw[j][0] = __float_as_uint(__ldg(src)); raw[j][1] = __float_as_uint(__ldg(src + plane));
-                        raw[j][2] = __float_as_uint(__ldg(src + 2 * plane));
+                    for (int j = 0; j < kS4GroupBatch; ++j) {
+                        const int q = ptid + (j0 + j) * kProdThreads;
+                        const int r = q / 10, g = q - r * 10;
+                        const int y = iy0 + r, x = ix0 - 1 + 4 * g;
+                        ok[j] = q < kS4Groups && (unsigned)y < (unsigned)p.H && (unsigned)x < (unsigned)p.W;
+                        const uint32_t* src = reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint8_t*>(p.in_raw) +
+                                                                                ((ptrdiff_t)n * plane + (ptrdiff_t)y * p.W + x) * 3);
+#pragma unroll
+                        for (int k = 0; k < 3; ++k) wd[j][k] = ok[j] ? __ldg(src + k) : 0u;
+                    }
+#pragma unroll
+                    for (int j = 0; j < kS4GroupBatch; ++j) {
+                        const int q = ptid + (j0 + j) * kProdThreads;
+                        if (q >= kS4Groups) break;
+                        const int r = q / 10, g = q - r * 10;
+                        uint32_t px[4][2];
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) {
+                            float f[3];
+#pragma unroll
+                            for (int c = 0; c < 3; ++c) {
+                                const uint32_t byte = (wd[j][(3 * k + c) >> 2] >> (8 * ((3 * k + c) & 3))) & 0xffu;
+                                f[c] = ok[j] ? ((float)byte - 127.5f) * (1.0f / 127.5f) : 0.f;   // zero padding of the normalised image
+                            }
+                            px[k][0] = pack2<F16>(f[0], f[1]);                                       // rounding point R0
+                            px[k][1] = pack2<F16>(f[2], 0.f);
+                        }
+                        const uint32_t d = dst0 + (uint32_t)(r * kS4RowBytes + 32 * g);              // patch column 4g, 16-byte aligned
+                        if (g > 0) asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(d - 8u), "r"(px[0][0]), "r"(px[0][1]) : "memory");
+                        if (g < 9) {
+                            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(d), "r"(px[1][0]), "r"(px[1][1]), "r"(px[2][0]),
+                                         "r"(px[2][1]) : "memory");
+                            asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(d + 16u), "r"(px[3][0]), "r"(px[3][1]) : "memory");
+                        }
                     }
                 }
+            } else {
+                // per-pixel loader: fp32 NCHW, or u8 rows that are not whole aligned words
+#pragma unroll 1
+                for (int j0 = 0; j0 < kS4PerThread; j0 += kS4Batch) {
+                    uint32_t raw[kS4Batch][3];
+                    bool ok[kS4Batch];
 #pragma unroll
-                for (int j = 0; j < kS4Batch; ++j) {
-                    const int q = ptid + (j0 + j) * kProdThreads;
-                    if (q >= kS4Pix) break;
-                    float f[3];
-#pragma unroll
-                    for (int k = 0; k < 3; ++k) {
-                        f[k] = u8 ? ((float)raw[j][k] - 127.5f) * (1.0f / 127.5f) : __uint_as_float(raw[j][k]);
-                        if (!ok[j]) f[k] = 0.f;             // conv zero padding (of the normalised image)
+                    for (int j = 0; j < kS4Batch; ++j) {
+                        const int q = ptid + (j0 + j) * kProdThreads;
+                        const int r = q / kS4Cols, c = q - r * kS4Cols;
+                        const int y = iy0 + r, x = ix0 + c;
+                        ok[j] = q < kS4Pix && (interior || ((unsigned)y < (unsigned)p.H && (unsigned)x < (unsigned)p.W));
+                        const ptrdiff_t pix = ok[j] ? (ptrdiff_t)n * plane + (ptrdiff_t)y * p.W + x : 0;
+                        if (u8) {
+                            const uint8_t* src = reinterpret_cast<const uint8_t*>(p.in_raw) + pix * 3;
+                            raw[j][0] = __ldg(src); raw[j][1] = __ldg(src + 1); raw[j][2] = __ldg(src + 2);
+                        } else {
+                            const float* src = reinterpret_cast<const float*>(p.in_raw) + (ok[j] ? (ptrdiff_t)n * 2 * plane + pix : 0);
+                            raw[j][0] = __float_as_uint(__ldg(src)); raw[j][1] = __float_as_uint(__ldg(src + plane));
+                            raw[j][2] = __float_as_uint(__ldg(src + 2 * plane));
+                        }
                     }
-                    const uint32_t lo = pack2<F16>(f[0], f[1]), hi = pack2<F16>(f[2], 0.f);   // rounding point R0
-                    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(dst0 + q * 8), "r"(lo), "r"(hi) : "memory");
+#pragma unroll
+                    for (int j = 0; j < kS4Batch; ++j) {
+                        const int q = ptid + (j0 + j) * kProdThreads;
+                        if (q >= kS4Pix) break;
+                        float f[3];
+#pragma unroll
+                        for (int k = 0; k < 3; ++k) {
+                            f[k] = u8 ? ((float)raw[j][k] - 127.5f) * (1.0f / 127.5f) : __uint_as_float(raw[j][k]);
+                            if (!ok[j]) f[k] = 0.f;             // conv zero padding (of the normalised image)
+                        }
+                        const uint32_t lo = pack2<F16>(f[0], f[1]), hi = pack2<F16>(f[2], 0.f);   // rounding point R0
+                        asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(dst0 + q * 8), "r"(lo), "r"(hi) : "memory");
+                    }
                 }
             }
             fence_proxy_async_smem();

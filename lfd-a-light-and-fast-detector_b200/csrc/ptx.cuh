@@ -288,6 +288,12 @@ LFD_DEVINL void wgmma_rs(float* d, const uint32_t* a, uint64_t b, uint32_t acc) 
     if (F16) WgmmaRs<N>::rs_f16(d, a, b, acc);
     else WgmmaRs<N>::rs_bf16(d, a, b, acc);
 }
+// Four 8x8 matrices of 16-bit values to shared memory (warp-collective): lanes 8i .. 8i+7 give the 16-byte row addresses of
+// matrix i, and r_i holds this thread's pair (row t/4, columns 2(t%4), +1) of matrix i -- the layout of one 8-column slice of a
+// wgmma accumulator fragment packed to 16 bits.
+LFD_DEVINL void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
+}
 
 // ---------------------------------------------------------------- misc
 // Kernel time-line for tests/debug_timeline.py (only with -DLFD_B200_TIMELINE): tl[0] = earliest CTA start, tl[1] = latest CTA end,
