@@ -50,7 +50,7 @@ typedef struct lfd_plan lfd_plan;
 
 int lfd_abi_version(void);
 /* sizeof of the structs of this header as the library was compiled, for bindings that mirror them field by field (ctypes, cffi):
- * which = 0 lfd_op, 1 lfd_top, 2 lfd_pack_desc, 3 lfd_unpack_desc; -1 for anything else. */
+ * which = 0 lfd_op, 1 lfd_top, 2 lfd_pack_desc, 3 lfd_unpack_desc, 4 lfd_post_cfg, 5 lfd_loss_cfg, 6 lfd_levels; -1 for anything else. */
 int lfd_struct_bytes(int which);
 const char* lfd_last_error(void);
 /* number of SMs of the current device (0 + error when there is no usable device) */
@@ -176,6 +176,8 @@ typedef struct lfd_post_cfg {
     float level_hi[LFD_MAX_LEVELS]; /* upper end of the level's regression range */
     float score_thr, iou_thr;
     int32_t cap;                /* per-image capacity for candidates and outputs */
+    int32_t max_ctas;           /* 0 = default.  > 0: stands in for the SM count the sigmoid multi-class candidate launch is sized from
+                                   (at most 8 * max_ctas blocks per image), so its grid-stride loop runs more rounds (tests) */
 } lfd_post_cfg;
 
 size_t lfd_postprocess_workspace_bytes(const lfd_post_cfg* cfg);
@@ -232,6 +234,8 @@ typedef struct lfd_loss_cfg {
     float reg_eps;               /* IoU family eps */
     float smooth_l1_beta;
     float cls_weight, reg_weight;
+    int32_t max_ctas;            /* 0 = default.  > 0: stands in for the SM count the two loss launches are sized from (4 * max_ctas blocks
+                                    each), so every thread walks more of its grid-stride loop (tests) */
 } lfd_loss_cfg;
 /* loss_sums double[2] = {sum of element-wise cls loss over valid rows, sum of the regression loss over positives} (zeroed inside);
  * the reference's normalisation is loss = sums[0]/(n_pos+1) + sums[1]/n_pos.  grad_cls / grad_reg (optional) receive

@@ -99,6 +99,9 @@ extern "C" int lfd_struct_bytes(int which) {
         case 1: return (int)sizeof(lfd_top);
         case 2: return (int)sizeof(lfd_pack_desc);
         case 3: return (int)sizeof(lfd_unpack_desc);
+        case 4: return (int)sizeof(lfd_post_cfg);
+        case 5: return (int)sizeof(lfd_loss_cfg);
+        case 6: return (int)sizeof(lfd_levels);
     }
     return -1;
 }
@@ -520,7 +523,7 @@ extern "C" int lfd_postprocess(const lfd_post_cfg* c, const float* cls, const fl
     p.cand_src = reinterpret_cast<int*>(ws + L.src); p.cand_count = reinterpret_cast<int*>(ws + L.count);
     CUDA_TRY(cudaMemsetAsync(p.cand_count, 0, (size_t)c->N * 4, st));
     CUDA_TRY(cudaMemsetAsync(overflow, 0, 4, st));
-    CUDA_TRY(candidates_launch(p, sm_count(), st));
+    CUDA_TRY(candidates_launch(p, c->max_ctas > 0 ? c->max_ctas : sm_count(), st));
     NmsParams q;
     q.cand_box = p.cand_box; q.cand_score = p.cand_score; q.cand_src = p.cand_src; q.cand_count = p.cand_count;
     q.scratch = ws + L.scratch; q.scratch_stride = L.scratch_stride; q.cap = c->cap; q.cap_pow2 = L.cap_pow2; q.C = c->C;
@@ -658,17 +661,18 @@ extern "C" int lfd_detection_loss(const lfd_levels* lv, const lfd_loss_cfg* c, c
     if (c->reg_loss == LFD_REG_SMOOTH_L1 && !(c->smooth_l1_beta > 0.f)) return fail(LFD_ERR_INVALID, "lfd_detection_loss: SmoothL1 beta must be > 0");
     if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_detection_loss: no CUDA device (there is no CPU fallback)");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const int sms = c->max_ctas > 0 ? c->max_ctas : sm_count();
     CUDA_TRY(cudaMemsetAsync(loss_sums, 0, 16, st));
     ClsLossParams k;
     k.logits = cls_logits; k.cls_target = cls_target; k.label = label; k.counters = counters; k.grad = grad_cls; k.loss_sum = loss_sums;
     k.N = c->N; k.P = c->P; k.C = c->C; k.cls_mode = c->cls_mode; k.gamma = c->gamma; k.alpha = c->alpha; k.loss_weight = c->cls_weight;
-    CUDA_TRY(cls_loss_launch(k, sm_count(), st));
+    CUDA_TRY(cls_loss_launch(k, sms, st));
     RegLossParams r;
     fill_levels(lv, &r.lv);
     r.reg = reg; r.reg_target = reg_target; r.label = label; r.counters = counters; r.grad = grad_reg; r.loss_sum = loss_sums + 1;
     r.N = c->N; r.P = c->P; r.C = c->C; r.bbox_mode = c->bbox_mode; r.loss_kind = c->reg_loss; r.eps = c->reg_eps; r.loss_weight = c->reg_weight;
     r.beta = c->smooth_l1_beta;
-    CUDA_TRY(iou_loss_launch(r, sm_count(), st));
+    CUDA_TRY(iou_loss_launch(r, sms, st));
     return LFD_OK;
 }
 

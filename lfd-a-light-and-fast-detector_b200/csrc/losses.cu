@@ -297,7 +297,10 @@ __device__ __forceinline__ Dual iou_family_loss(int kind, const Dual* pr, const 
     const Dual w2 = tg[2] - tg[0], h2 = tg[3] - tg[1] + dc(eps);
     const Dual da = datan(w2 / h2) - datan(w1 / h1);
     const Dual v = dc(0.40528473456935109f) * da * da;          // 4 / pi^2
-    return dc(1.f) - (ious - (rho2 / c2 + (v * v) / (dc(1.f) - ious + v)));
+    // v = 0 (equal aspect ratios): the term and its derivatives are 0.  Evaluated, it is 0 / 0 when the fp32 IoU rounds to 1 (identical
+    // boxes whose area swamps eps), where the reference's value in exact arithmetic is 0 / (eps / (area + eps)) = 0.
+    const Dual vt = v.v == 0.f ? dc(0.f) : (v * v) / (dc(1.f) - ious + v);
+    return dc(1.f) - (ious - (rho2 / c2 + vt));
 }
 
 // regression loss of get_loss (lfd.py:343-387): positives, avg_factor = n_pos.  loss_kind 0: -log IoU (analytic gradient);
@@ -367,10 +370,11 @@ __global__ void __launch_bounds__(256) iou_loss_kernel(const RegLossParams p) {
                 const float g_ap = -g_iou * un_live * ov / (un * un);
                 const float g_w = rw > 0.f ? g_ov * h : 0.f, g_h = rh > 0.f ? g_ov * w : 0.f;
                 float g_px1 = -g_ap * ph, g_px2 = g_ap * ph, g_py1 = -g_ap * pw, g_py2 = g_ap * pw;
-                if (px2 < tx2) g_px2 += g_w;
-                if (px1 > tx1) g_px1 -= g_w;
-                if (py2 < ty2) g_py2 += g_h;
-                if (py1 > ty1) g_py1 -= g_h;
+                // torch.max / torch.min of the reference's bbox_overlaps: a predicted edge equal to the target edge gets half the gradient
+                if (px2 < tx2) g_px2 += g_w; else if (px2 == tx2) g_px2 += 0.5f * g_w;
+                if (px1 > tx1) g_px1 -= g_w; else if (px1 == tx1) g_px1 -= 0.5f * g_w;
+                if (py2 < ty2) g_py2 += g_h; else if (py2 == ty2) g_py2 += 0.5f * g_h;
+                if (py1 > ty1) g_py1 -= g_h; else if (py1 == ty1) g_py1 -= 0.5f * g_h;
                 const float sc = inv_avg * p.loss_weight;
                 g4 = make_float4(-g_px1 * dd[0] * sc, -g_py1 * dd[1] * sc, g_px2 * dd[2] * sc, g_py2 * dd[3] * sc);
             }

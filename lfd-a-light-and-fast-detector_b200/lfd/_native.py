@@ -51,7 +51,7 @@ class PostCfg(C.Structure):
                 ('num_levels', C.c_int32),
                 ('level_off', C.c_int32 * MAX_LEVELS), ('level_w', C.c_int32 * MAX_LEVELS),
                 ('level_stride', C.c_int32 * MAX_LEVELS), ('level_hi', C.c_float * MAX_LEVELS),
-                ('score_thr', C.c_float), ('iou_thr', C.c_float), ('cap', C.c_int32)]
+                ('score_thr', C.c_float), ('iou_thr', C.c_float), ('cap', C.c_int32), ('max_ctas', C.c_int32)]
 
 
 class Levels(C.Structure):
@@ -64,7 +64,7 @@ class Levels(C.Structure):
 class LossCfg(C.Structure):
     _fields_ = [('N', C.c_int32), ('P', C.c_int32), ('C', C.c_int32), ('cls_mode', C.c_int32), ('bbox_mode', C.c_int32), ('reg_loss', C.c_int32),
                 ('gamma', C.c_float), ('alpha', C.c_float), ('reg_eps', C.c_float), ('smooth_l1_beta', C.c_float),
-                ('cls_weight', C.c_float), ('reg_weight', C.c_float)]
+                ('cls_weight', C.c_float), ('reg_weight', C.c_float), ('max_ctas', C.c_int32)]
 
 
 # training plan ops (include/lfd_b200.h, lfd_top)
@@ -166,7 +166,7 @@ def lib():
         fn.argtypes = args
     if L.lfd_abi_version() != 5:
         raise LfdError('liblfd_b200.so ABI version mismatch')
-    for which, st in enumerate((Op, Top, PackDesc, UnpackDesc)):
+    for which, st in enumerate((Op, Top, PackDesc, UnpackDesc, PostCfg, LossCfg, Levels)):
         if L.lfd_struct_bytes(which) != C.sizeof(st):
             raise LfdError('liblfd_b200.so: %s is %d bytes in the library, %d in lfd/_native.py' % (st.__name__, L.lfd_struct_bytes(which), C.sizeof(st)))
     _lib = L
