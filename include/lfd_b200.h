@@ -50,7 +50,8 @@ typedef struct lfd_plan lfd_plan;
 
 int lfd_abi_version(void);
 /* sizeof of the structs of this header as the library was compiled, for bindings that mirror them field by field (ctypes, cffi):
- * which = 0 lfd_op, 1 lfd_top, 2 lfd_pack_desc, 3 lfd_unpack_desc, 4 lfd_post_cfg, 5 lfd_loss_cfg, 6 lfd_levels; -1 for anything else. */
+ * which = 0 lfd_op, 1 lfd_top, 2 lfd_pack_desc, 3 lfd_unpack_desc, 4 lfd_post_cfg, 5 lfd_loss_cfg, 6 lfd_levels, 7 lfd_input_desc;
+ * -1 for anything else. */
 int lfd_struct_bytes(int which);
 const char* lfd_last_error(void);
 /* number of SMs of the current device (0 + error when there is no usable device) */
@@ -359,6 +360,37 @@ int lfd_grad_sqnorm(const float* grads, int64_t n, double* sqnorm, lfd_stream st
  * buf = momentum * buf + (1 - dampening) * g; p -= lr * (nesterov ? g + momentum * buf : buf).  momentum_buf may be NULL. */
 int lfd_sgd_step(float* params, float* grads, float* momentum_buf, int64_t n, float lr, float momentum, float dampening,
                  float weight_decay, int nesterov, float max_norm, float grad_scale, const double* sqnorm, lfd_stream stream);
+
+/* ------------------------------------------------------------------------------------------ training input batch
+ * One launch builds a batch of training crops from uint8 source windows, the pixel work of the reference's data loader
+ * (RandomBBoxCropRegionSampler & co. lfd/data_pipeline/sampler/region_sampler.py, crop_from_image :280-300, the gray -> 3 channel
+ * tile data_loader.py:122-124, HorizontalFlip / BGR2RGB / Normalize, _image_batch_postprocess data_loader.py:68-83):
+ *   R = cv2.resize(S, (0, 0), fx = s, fy = s) (INTER_LINEAR on uint8, bit-exact; INTER_AREA when 1/s == 2; a copy when the size is kept),
+ *   crop[y][x] = R[crop_y + y][crop_x + x] inside R, 0 outside; out[y][x] = crop[y][out_w - 1 - x] when flipped.
+ * R is never materialised. */
+enum { LFD_RESIZE_COPY = 0, LFD_RESIZE_LINEAR = 1, LFD_RESIZE_AREA2 = 2 };
+enum { LFD_INPUT_OUT_U8_NHWC = 0, LFD_INPUT_OUT_F32_NCHW = 1 };
+typedef struct lfd_input_desc {
+    int64_t src_off;          /* byte offset in src of the window's first pixel */
+    double inv_scale;         /* 1 / s */
+    int32_t pitch;            /* bytes between window rows (>= win_w * channels) */
+    int32_t channels;         /* 1 (gray) or 3 (BGR) */
+    int32_t win_x, win_y;     /* window origin inside the full source image */
+    int32_t win_w, win_h;     /* window size; it holds every source pixel the crop reads (0 x 0 when the crop misses R) */
+    int32_t src_w, src_h;     /* full source image size */
+    int32_t dw, dh;           /* size of R: round-half-even(src_w * s), round-half-even(src_h * s) */
+    int32_t mode;             /* LFD_RESIZE_*: COPY when (dw, dh) == (src_w, src_h), AREA2 when 1/s == 2 exactly, else LINEAR */
+    int32_t crop_x, crop_y;   /* crop origin in R's coordinates (may be negative or beyond R) */
+    int32_t out_w, out_h;     /* crop size, <= W, H */
+    int32_t flip;             /* 1: horizontal flip of the crop */
+} lfd_input_desc;
+/* descs: device lfd_input_desc[n]; src: device bytes holding every window.
+ * out_mode LFD_INPUT_OUT_U8_NHWC: out uint8 [n, H, W, 3]; LFD_INPUT_OUT_F32_NCHW: out float32 [n, 3, H, W] with
+ * out = (v - mean[c]) * scale[c] (albumentations' Normalize: mean[c] = mean * max_pixel, scale[c] = float32(1 / (std * max_pixel))).
+ * Pixels outside an image's out_w x out_h are 0 in both modes (the zero padding of mixed-size batches).  swap_rb: BGR -> RGB; a
+ * 1-channel source is replicated to 3.  mean / scale: host float[3], unused in the uint8 mode.  W <= 6144. */
+int lfd_input_batch(const lfd_input_desc* descs, int n, const uint8_t* src, void* out, int out_mode, int swap_rb, int H, int W,
+                    const float* mean, const float* scale, lfd_stream stream);
 
 #ifdef __cplusplus
 }

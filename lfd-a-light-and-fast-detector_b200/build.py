@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 OUT = os.environ.get('LFD_B200_OUT') or os.path.join(HERE, 'liblfd_b200.so')      # LFD_B200_OUT / LFD_B200_EXTRA_FLAGS: tuning experiments only
-SOURCES = ['api.cu', 'conv_umma.cu', 'conv_simt.cu', 'postprocess.cu', 'losses.cu', 'train.cu', 'wgrad_umma.cu']
+SOURCES = ['api.cu', 'conv_umma.cu', 'conv_simt.cu', 'postprocess.cu', 'losses.cu', 'train.cu', 'wgrad_umma.cu', 'input.cu']
 HEADERS = ['ptx.cuh', 'conv_common.cuh', 'kernels.cuh', 'train.cuh', os.path.join('..', '..', 'include', 'lfd_b200.h')]
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']

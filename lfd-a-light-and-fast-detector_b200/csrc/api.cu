@@ -102,6 +102,7 @@ extern "C" int lfd_struct_bytes(int which) {
         case 4: return (int)sizeof(lfd_post_cfg);
         case 5: return (int)sizeof(lfd_loss_cfg);
         case 6: return (int)sizeof(lfd_levels);
+        case 7: return (int)sizeof(lfd_input_desc);
     }
     return -1;
 }
@@ -1060,5 +1061,18 @@ extern "C" int lfd_sgd_step(float* params, float* grads, float* momentum_buf, in
     p.max_norm = max_norm; p.sqnorm = sqnorm; p.grad_scale = grad_scale;
     if (momentum != 0.f && !momentum_buf) return fail(LFD_ERR_INVALID, "lfd_sgd_step: momentum buffer missing");
     CUDA_TRY(sgd_launch(p, sm_count(), st_of(stream)));
+    return LFD_OK;
+}
+
+extern "C" int lfd_input_batch(const lfd_input_desc* descs, int n, const uint8_t* src, void* out, int out_mode, int swap_rb, int H, int W,
+                               const float* mean, const float* scale, lfd_stream stream) {
+    if (n < 0 || H < 1 || W < 1 || (n > 0 && (!descs || !src || !out))) return fail(LFD_ERR_INVALID, "lfd_input_batch: bad arguments (n=%d H=%d W=%d)", n, H, W);
+    if (out_mode != LFD_INPUT_OUT_U8_NHWC && out_mode != LFD_INPUT_OUT_F32_NCHW) return fail(LFD_ERR_INVALID, "lfd_input_batch: out_mode %d", out_mode);
+    if (out_mode == LFD_INPUT_OUT_F32_NCHW && (!mean || !scale)) return fail(LFD_ERR_INVALID, "lfd_input_batch: the fp32 mode needs mean and scale");
+    if (W > 6144) return fail(LFD_ERR_UNSUPPORTED, "lfd_input_batch: W=%d > 6144 (the column table lives in 48 KB of shared memory)", W);
+    if (n > 65535) return fail(LFD_ERR_UNSUPPORTED, "lfd_input_batch: n=%d > 65535", n);
+    if (n == 0) return LFD_OK;
+    if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_input_batch: no CUDA device (there is no CPU fallback)");
+    CUDA_TRY(input_batch_launch(descs, n, src, out, out_mode, swap_rb, H, W, mean, scale, st_of(stream)));
     return LFD_OK;
 }

@@ -137,4 +137,8 @@ cudaError_t iou_loss_launch(const RegLossParams& p, int num_sms, cudaStream_t st
 // element-wise IoU-family loss (kind 0..3) + d loss / d pred on explicit box pairs
 cudaError_t box_loss_launch(int kind, const float* pred, const float* target, int n, float eps, float* loss, float* grad, cudaStream_t st);
 
+// input.cu: descs = device lfd_input_desc[n] (include/lfd_b200.h, lfd_input_batch)
+cudaError_t input_batch_launch(const void* descs, int n, const uint8_t* src, void* out, int out_mode, int swap_rb, int H, int W,
+                               const float* mean, const float* scale, cudaStream_t st);
+
 }  // namespace lfd

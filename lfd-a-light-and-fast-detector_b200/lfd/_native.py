@@ -77,6 +77,16 @@ UNPACK_CONV, UNPACK_ADD = 0, 1
 
 MAX_BRANCHES = 8          # LFD_MAX_BRANCHES
 
+RESIZE_COPY, RESIZE_LINEAR, RESIZE_AREA2 = 0, 1, 2
+INPUT_OUT_U8_NHWC, INPUT_OUT_F32_NCHW = 0, 1
+
+
+class InputDesc(C.Structure):
+    _fields_ = [('src_off', C.c_int64), ('inv_scale', C.c_double), ('pitch', C.c_int32), ('channels', C.c_int32),
+                ('win_x', C.c_int32), ('win_y', C.c_int32), ('win_w', C.c_int32), ('win_h', C.c_int32),
+                ('src_w', C.c_int32), ('src_h', C.c_int32), ('dw', C.c_int32), ('dh', C.c_int32), ('mode', C.c_int32),
+                ('crop_x', C.c_int32), ('crop_y', C.c_int32), ('out_w', C.c_int32), ('out_h', C.c_int32), ('flip', C.c_int32)]
+
 
 class Top(C.Structure):
     _fields_ = [('kind', C.c_int32),
@@ -135,6 +145,7 @@ SYMBOLS = {
     'lfd_run_top': (_i, [C.POINTER(Top), _vp, _i, _vp, _vp]),
     'lfd_grad_sqnorm': (_i, [_vp, _i64, _vp, _vp]),
     'lfd_sgd_step': (_i, [_vp, _vp, _vp, _i64, _f, _f, _f, _f, _i, _f, _f, _vp, _vp]),
+    'lfd_input_batch': (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, C.POINTER(_f), C.POINTER(_f), _vp]),
 }
 
 _lib = None
@@ -166,7 +177,7 @@ def lib():
         fn.argtypes = args
     if L.lfd_abi_version() != 5:
         raise LfdError('liblfd_b200.so ABI version mismatch')
-    for which, st in enumerate((Op, Top, PackDesc, UnpackDesc, PostCfg, LossCfg, Levels)):
+    for which, st in enumerate((Op, Top, PackDesc, UnpackDesc, PostCfg, LossCfg, Levels, InputDesc)):
         if L.lfd_struct_bytes(which) != C.sizeof(st):
             raise LfdError('liblfd_b200.so: %s is %d bytes in the library, %d in lfd/_native.py' % (st.__name__, L.lfd_struct_bytes(which), C.sizeof(st)))
     _lib = L

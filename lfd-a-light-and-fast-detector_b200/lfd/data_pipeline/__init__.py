@@ -1,5 +1,9 @@
 # -*- coding: utf-8 -*-
-"""Only the two pieces of the reference data pipeline that touch the hot path (SURVEY 2 #12): `Sample` and the
-`simple_normalize` contract.  Dataset packing, samplers, loaders and albumentations pipelines are out of scope."""
-from .dataset import Sample
-from .augmentation import simple_normalize_pipeline
+"""The reference's training input pipeline under its module paths: packed datasets (dataset.Dataset), batch index samplers and
+region samplers (sampler), declarative augmentation pipelines (augmentation) and the DataLoader, whose resize / crop / flip /
+normalisation runs in one CUDA kernel per batch (lfd_input_batch).  Dataset parsers and packing scripts are not included: files
+packed by the reference load as they are."""
+from .dataset import Sample, Dataset
+from .augmentation import *
+from .sampler import *
+from .data_loader import DataLoader, RankLocalBatch

@@ -1,4 +1,6 @@
 # -*- coding: utf-8 -*-
+import random
+
 import numpy
 
 __all__ = ['simple_normalize_pipeline']
@@ -10,3 +12,124 @@ def simple_normalize_pipeline(sample):
     img = sample['image'].astype(numpy.float32)
     sample['image'] = (img - numpy.float32(127.5)) * numpy.float32(1.0 / 127.5)
     return sample
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# Declarative stand-ins for the albumentations transforms the reference's pipelines use (augmentation_pipeline.py,
+# new_augmentations.py).  The data loader reads them (flip probability, channel order, mean, std, max_pixel) and runs them inside
+# the input kernel; called on a host sample they apply the same operation with numpy.  albumentations' own consumption of the
+# random stream (Compose and every transform draw for their `p`) is not reproduced: only HorizontalFlip draws, random.random() < p.
+
+__all__ += ['Compose', 'HorizontalFlip', 'Normalize', 'BboxParams', 'BGR2RGB',
+            'typical_coco_train_pipeline', 'typical_coco_val_pipeline', 'simple_widerface_train_pipeline',
+            'simple_widerface_val_pipeline', 'caffe_imagenet_normalize', 'standard_normalize', 'simple_normalize', 'bbox_param']
+
+
+class BboxParams(object):
+    def __init__(self, format='coco', label_fields=None, **kwargs):
+        assert format == 'coco', 'only coco boxes (x, y, w, h) are supported'
+        self.format, self.label_fields = format, label_fields
+
+
+class HorizontalFlip(object):
+    def __init__(self, always_apply=False, p=0.5):
+        self.p = 1.0 if always_apply else p
+
+    def apply(self, sample, flip):
+        if flip:
+            w = sample['image'].shape[1]
+            sample['image'] = numpy.ascontiguousarray(sample['image'][:, ::-1])
+            if 'bboxes' in sample:
+                sample['bboxes'] = [(w - b[0] - b[2], b[1], b[2], b[3]) for b in sample['bboxes']]
+        return sample
+
+
+class BGR2RGB(object):
+    def __init__(self, always_apply=False, p=1.):
+        self.p = 1.0 if always_apply else p
+
+    def apply(self, sample):
+        sample['image'] = numpy.ascontiguousarray(sample['image'][..., ::-1])
+        return sample
+
+
+class Normalize(object):
+    def __init__(self, mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225), max_pixel_value=255.0, always_apply=False, p=1.0):
+        self.mean, self.std, self.max_pixel_value, self.p = mean, std, max_pixel_value, 1.0 if always_apply else p
+
+    def constants(self):
+        """(mean * max_pixel, reciprocal(std * max_pixel)) in float32, as albumentations.normalize computes them."""
+        m = numpy.array(self.mean, numpy.float32) * numpy.float32(self.max_pixel_value)
+        d = numpy.reciprocal(numpy.array(self.std, numpy.float32) * numpy.float32(self.max_pixel_value), dtype=numpy.float32)
+        return m, d
+
+    def apply(self, sample):
+        m, d = self.constants()
+        sample['image'] = (sample['image'].astype(numpy.float32) - m) * d
+        return sample
+
+
+class _Probe(object):
+    """Stands in for the image when the data loader asks a pipeline which Compose it would run (see Compose.__call__)."""
+
+
+class Compose(object):
+    def __init__(self, transforms, bbox_params=None, p=1.0):
+        self.transforms, self.bbox_params, self.p = list(transforms), bbox_params, p
+
+    def __call__(self, sample=None, **kwargs):
+        sample = dict(sample if sample is not None else kwargs)
+        if isinstance(sample.get('image'), _Probe):
+            return {'image': self}
+        for t in self.transforms:
+            if isinstance(t, HorizontalFlip):
+                t.apply(sample, random.random() < t.p)
+            else:
+                t.apply(sample)
+        return sample
+
+    def device_spec(self):
+        """(flip_p or None, swap_rb, mean[3], scale[3]) when the input kernel can run this pipeline, else None: at most one flip,
+        BGR2RGB and Normalize with p = 1, Normalize (at most one) last."""
+        flip_p, swap, norm = None, False, None
+        for i, t in enumerate(self.transforms):
+            if isinstance(t, HorizontalFlip) and flip_p is None:
+                flip_p = t.p
+            elif isinstance(t, BGR2RGB) and t.p == 1:
+                swap = not swap
+            elif isinstance(t, Normalize) and t.p == 1 and i == len(self.transforms) - 1:
+                norm = t
+            else:
+                return None
+        mean, scale = norm.constants() if norm is not None else (numpy.zeros(3, numpy.float32), numpy.ones(3, numpy.float32))
+        return flip_p, swap, mean, scale
+
+
+def pipeline_device_spec(pipeline, with_bboxes):
+    """What the input kernel needs to run `pipeline` on a sample with / without boxes, or None when it has to run on the host:
+    the pipeline is None, a Compose of the stand-ins above, or a function that only picks such a Compose from the sample's keys."""
+    if pipeline is None:
+        return None, False, numpy.zeros(3, numpy.float32), numpy.ones(3, numpy.float32)
+    compose = pipeline
+    if not isinstance(pipeline, Compose):
+        probe = {'image': _Probe()}
+        if with_bboxes:
+            probe.update(bboxes=[], bbox_labels=[])
+        try:
+            compose = pipeline(probe)['image']
+        except Exception:
+            return None
+    return compose.device_spec() if isinstance(compose, Compose) else None
+
+
+random_horizon_flip = HorizontalFlip(p=0.5)
+caffe_imagenet_normalize = Normalize(mean=(102.9801, 115.9465, 122.7717), std=(1.0, 1.0, 1.0), max_pixel_value=1.0, p=1.0)
+standard_normalize = Normalize(mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225), max_pixel_value=255.0, p=1.0)
+simple_normalize = Normalize(mean=(0.5, 0.5, 0.5), std=(0.5, 0.5, 0.5), max_pixel_value=255.0, p=1.0)
+bbox_param = BboxParams(format='coco', label_fields=['bbox_labels'])
+
+# the reference picks a Compose with or without bbox_params by the sample's keys; the stand-in handles both with one
+typical_coco_train_pipeline = Compose([random_horizon_flip, caffe_imagenet_normalize], bbox_params=bbox_param, p=1.)
+typical_coco_val_pipeline = Compose([caffe_imagenet_normalize], bbox_params=bbox_param, p=1.)
+simple_widerface_train_pipeline = Compose([random_horizon_flip, simple_normalize], bbox_params=bbox_param, p=1.)
+simple_widerface_val_pipeline = Compose([simple_normalize], bbox_params=bbox_param, p=1.)

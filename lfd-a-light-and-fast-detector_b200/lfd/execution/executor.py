@@ -12,6 +12,7 @@ import torch
 
 from .hooks import CheckpointHook, EvaluationHook, LoggerHook, LrSchedulerHook, OptimizerHook, SpeedHook, get_priority
 from .parallel import broadcast_module_state, shard_batch, world
+from ..data_pipeline.data_loader import RankLocalBatch
 from .utils import AverageMeter, get_root_logger, load_checkpoint, save_checkpoint
 
 _RESUME_BLACKLIST = ('timestamp', 'work_dir', 'log_path', 'training_epochs', 'gpu_list', 'display_interval', 'save_interval',
@@ -117,6 +118,11 @@ class Executor(object):
         t = torch.from_numpy(image_batch) if not torch.is_tensor(image_batch) else image_batch
         return t.to(self.device, non_blocking=True)
 
+    @staticmethod
+    def _local(data_batch):
+        """This rank's share of a batch: a RankLocalBatch already is one (the loader built only this rank's images)."""
+        return tuple(data_batch) if isinstance(data_batch, RankLocalBatch) else shard_batch(data_batch)
+
     def train(self):
         cfg = self.config_dict
         cfg['mode'] = 'train'
@@ -125,7 +131,7 @@ class Executor(object):
         for i, data_batch in enumerate(cfg['train_data_loader']):
             cfg.update(inner_train_iter=i)
             self._call_hooks('before_train_iter')
-            image_batch, annotation_batch, meta_batch = shard_batch(data_batch)
+            image_batch, annotation_batch, meta_batch = self._local(data_batch)
             cfg.update(batch_size=len(annotation_batch))
             if len(annotation_batch) == 0:
                 # the last batch had fewer images than ranks: this rank has nothing to compute but must still take part in the
@@ -149,7 +155,7 @@ class Executor(object):
         for i, data_batch in enumerate(cfg['val_data_loader']):
             cfg.update(inner_val_iter=i)
             self._call_hooks('before_val_iter')
-            image_batch, annotation_batch, meta_batch = shard_batch(data_batch)
+            image_batch, annotation_batch, meta_batch = self._local(data_batch)
             cfg.update(batch_size=len(annotation_batch))
             with torch.no_grad():
                 predict_outputs = cfg['model'](self._to_device(image_batch))
