@@ -286,13 +286,21 @@ int lfd_sigmoid_focal_loss_backward(const float* logits, const int64_t* targets,
  *                                                                                                        x27 = -1 or impl = SIMT: the SIMT kernel, 27 rows)
  *   UNPACK           -        -       -       -        -          -        -       -        table (lfd_unpack_desc[n_desc], device)
  *   ZERO             begin    bytes   -       -        -          -        -       -        -          (cudaMemsetAsync of a workspace region)
+ *   INFER            in       out     res     ds_out   -          -        -       -        op (const lfd_op*, HOST memory, read by lfd_train_plan_create)
+ *                                                                                                        one inference op inside the training plan: STEM0 / CONV
+ *                                                                                                        (with tail and fused shortcut) / STEM4, bf16, no GroupNorm
+ *                                                                                                        statistics.  Its weight / shift pointers are the caller's
+ *                                                                                                        packed operands (lfd_op conventions); off[0..3] replace the
+ *                                                                                                        op's in_off / out_off / res_off / ds_out_off, max_ctas its
+ *                                                                                                        max_ctas.  The frozen backbone prefix of a fine-tuning step
+ *                                                                                                        (BatchNorm folded, no statistics, no backward) runs on it.
  *
  * head staging (fp32): w[n_out][C] (bf16-rounded values), scale[n_out], shift[n_out] = bias * scale, bias[n_out];
  * head dstage (fp32): dW[n_out][C], dbias[n_out]; dscale (fp32): the level's Scale gradient [1].  wgrad dstage (fp32): [ksize^2][Cin][Cout].
  * BatchNorm statistics are taken over the STORED bf16 conv output; GroupNorm ones come from the conv epilogue as in inference. */
 enum { LFD_TOP_PACK = 0, LFD_TOP_STEM0 = 1, LFD_TOP_CONV = 2, LFD_TOP_BN_STATS = 3, LFD_TOP_BN_APPLY = 4, LFD_TOP_GN_APPLY = 5,
        LFD_TOP_HEAD_FINAL = 6, LFD_TOP_HEAD_FINAL_BWD = 7, LFD_TOP_NORM_BWD_REDUCE = 8, LFD_TOP_NORM_BWD_APPLY = 9, LFD_TOP_WGRAD = 10,
-       LFD_TOP_WGRAD_STEM = 11, LFD_TOP_UNPACK = 12, LFD_TOP_ZERO = 13 };
+       LFD_TOP_WGRAD_STEM = 11, LFD_TOP_UNPACK = 12, LFD_TOP_ZERO = 13, LFD_TOP_INFER = 14 };
 enum { LFD_WGRAD_UMMA = 0, LFD_WGRAD_SIMT = 1 }; /* SIMT = cross-check kernel, validation only */
 
 typedef struct lfd_top {

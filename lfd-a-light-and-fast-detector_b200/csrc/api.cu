@@ -742,6 +742,17 @@ static int plan_top(const lfd_top& t, int64_t ws_bytes, PlannedTop* out) {
             o.weight = reinterpret_cast<const void*>(1);   // placeholder: resolved against the workspace at launch
             return plan_op(o, t.impl, &out->conv);
         }
+        case LFD_TOP_INFER: {
+            if (!t.ptr[0]) return fail(LFD_ERR_INVALID, "infer: missing op descriptor");
+            lfd_op o = *reinterpret_cast<const lfd_op*>(t.ptr[0]);
+            if (o.kind != LFD_OP_STEM0 && o.kind != LFD_OP_CONV && o.kind != LFD_OP_STEM4)
+                return fail(LFD_ERR_UNSUPPORTED, "infer: op kind %d (STEM0 / CONV / STEM4 only)", o.kind);
+            if (o.dtype != LFD_DTYPE_BF16 || o.gn_groups) return fail(LFD_ERR_UNSUPPORTED, "infer: bf16 ops without GroupNorm statistics only");
+            if (t.off[1] < 0 || (o.kind == LFD_OP_CONV && t.off[0] < 0)) return fail(LFD_ERR_INVALID, "infer: missing in / out offset");
+            o.in_off = t.off[0]; o.out_off = t.off[1]; o.res_off = t.off[2]; o.ds_out_off = t.off[3]; o.stats_off = -1;
+            o.branch = 0; o.wait_mask = 0; o.max_ctas = t.max_ctas;
+            return plan_op(o, LFD_CONV_UMMA, &out->conv);
+        }
         case LFD_TOP_WGRAD: {
             WgradGeom g = {t.N, t.H, t.W, t.Cin, t.Ho, t.Wo, t.Cout, t.ksize, t.stride};
             if (t.impl == LFD_WGRAD_UMMA && !wgrad_umma_supported(g))
@@ -782,6 +793,8 @@ static int launch_top(const PlannedTop& pt, const void* input, int fmt, uint8_t*
             po.op.weight = ws + t.off[4];
             return launch_op(po, 0, input, fmt, ws, nullptr, nullptr, 0, 0, t.impl, st);
         }
+        case LFD_TOP_INFER:
+            return launch_op(pt.conv, 0, input, fmt, ws, nullptr, nullptr, 0, 0, LFD_CONV_UMMA, st);
         case LFD_TOP_BN_STATS: {
             BnStatsParams p;
             p.z = at<const __nv_bfloat16>(ws, t.off[0]); p.sums = at<double>(ws, t.off[3]);

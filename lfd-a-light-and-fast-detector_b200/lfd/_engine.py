@@ -101,6 +101,11 @@ class InferencePlan(object):
     def __init__(self, model, N, H, W, device, conv_impl=nat.CONV_UMMA, create_native=True, act_dtype='bf16', fuse_stem=None):
         """fuse_stem: run a four-conv 'faster' stem as one kernel (LFD_OP_STEM4) -- None: when its stem1 map would not stay in
         L2 (see _use_stem4), True / False: always / never (tests).  LFD_B200_NO_STEM_FUSION=1 turns it off."""
+        self._configure(N, H, W, device, conv_impl, create_native, act_dtype, fuse_stem)
+        self._build(model)
+        self._finalize()
+
+    def _configure(self, N, H, W, device, conv_impl, create_native, act_dtype, fuse_stem):
         self.N, self.H, self.W = N, H, W
         if act_dtype not in ACT_DTYPES:
             raise ValueError("act_dtype must be 'bf16' or 'fp16' (got %r)" % (act_dtype,))
@@ -120,8 +125,6 @@ class InferencePlan(object):
         # conv -> 1x1 conv pairs run as ONE kernel (tensor-core kernels only; the SIMT cross-check runs them unfused)
         self.fuse_tails = conv_impl == nat.CONV_UMMA and not os.environ.get('LFD_B200_NO_TAIL')
         self.fuse_stem = fuse_stem
-        self._build(model)
-        self._finalize()
 
     # ------------------------------------------------------------------ parameter staging
     def _add_f32(self, t):
@@ -288,11 +291,9 @@ class InferencePlan(object):
         return ho, wo
 
     # ------------------------------------------------------------------ graph walk
-    def _build(self, model):
-        bb, neck, head = model._backbone, model._neck, model._head
-        h, w = self.H, self.W
+    def _emit_stem(self, layers, h, w):
+        """The stem on the image -> (name of its output, h, w)."""
         cur = None
-        layers = bb.stem_layers()
         i = 0
         if self._use_stem4(layers):
             h, w = self._emit_stem4(layers, 'stem3', h, w)
@@ -309,6 +310,44 @@ class InferencePlan(object):
                 h, w = self._emit_conv(conv, norm, relu, cur, name, h, w, tail=tail)
             cur = name
             i += 2 if tail is not None else 1
+        return cur, h, w
+
+    def _emit_block(self, block, base, cur, h, w, n_taps):
+        """One residual block on the tensor `cur` -> (name of its output, h, w)."""
+        identity = cur
+        aux = False
+        pairs = block.conv_norm_pairs()
+        fuse_sc = None
+        if block._downsample is not None and self.fuse_shortcuts and self._can_fuse_shortcut(block, pairs):
+            ds = list(block._downsample)
+            fuse_sc = (ds[0], ds[1] if len(ds) > 1 else None, base + '_id')
+            identity = base + '_id'
+        elif block._downsample is not None:
+            # the 1x1/s2 shortcut conv only depends on the block input: it runs on the auxiliary branch, next to the
+            # block's first conv, and the block's last conv (which adds it) waits for it
+            ds = list(block._downsample)
+            aux = self.concurrent_levels and self.aux_shortcut and n_taps + 1 <= _AUX_BRANCH
+            if aux:
+                self._branch = _AUX_BRANCH
+            self._emit_conv(ds[0], ds[1] if len(ds) > 1 else None, False, cur, base + '_id', h, w)
+            if aux:
+                self._ops[-1]['wait_mask'] = 1          # the block input comes from the main stream
+                self._branch = 0
+            identity = base + '_id'
+        x, hh, ww = cur, h, w
+        for li, (conv, norm) in enumerate(pairs):
+            last = li == len(pairs) - 1
+            name = base + ('_out' if last else '_c%d' % li)
+            hh, ww = self._emit_conv(conv, norm, True, x, name, hh, ww, res=identity if last else None,
+                                     shortcut=fuse_sc if li == 0 else None)
+            if last and aux:
+                self._ops[-1]['wait_mask'] = 1 << _AUX_BRANCH
+            x = name
+        return x, hh, ww
+
+    def _build(self, model):
+        bb, neck, head = model._backbone, model._neck, model._head
+        cur, h, w = self._emit_stem(bb.stem_layers(), self.H, self.W)
         taps = list(bb._out_indices)
         if len(taps) != head._num_heads:
             raise ValueError('backbone taps (%d) and head levels (%d) differ' % (len(taps), head._num_heads))
@@ -331,37 +370,7 @@ class InferencePlan(object):
         cache = {}
         for si, stage in enumerate(bb.stages()):
             for bi, block in enumerate(stage):
-                base = 's%db%d' % (si, bi)
-                identity = cur
-                aux = False
-                pairs = block.conv_norm_pairs()
-                fuse_sc = None
-                if block._downsample is not None and self.fuse_shortcuts and self._can_fuse_shortcut(block, pairs):
-                    ds = list(block._downsample)
-                    fuse_sc = (ds[0], ds[1] if len(ds) > 1 else None, base + '_id')
-                    identity = base + '_id'
-                elif block._downsample is not None:
-                    # the 1x1/s2 shortcut conv only depends on the block input: it runs on the auxiliary branch, next to the
-                    # block's first conv, and the block's last conv (which adds it) waits for it
-                    ds = list(block._downsample)
-                    aux = self.concurrent_levels and self.aux_shortcut and len(taps) + 1 <= _AUX_BRANCH
-                    if aux:
-                        self._branch = _AUX_BRANCH
-                    self._emit_conv(ds[0], ds[1] if len(ds) > 1 else None, False, cur, base + '_id', h, w)
-                    if aux:
-                        self._ops[-1]['wait_mask'] = 1          # the block input comes from the main stream
-                        self._branch = 0
-                    identity = base + '_id'
-                x, hh, ww = cur, h, w
-                for li, (conv, norm) in enumerate(pairs):
-                    last = li == len(pairs) - 1
-                    name = base + ('_out' if last else '_c%d' % li)
-                    hh, ww = self._emit_conv(conv, norm, True, x, name, hh, ww, res=identity if last else None,
-                                             shortcut=fuse_sc if li == 0 else None)
-                    if last and aux:
-                        self._ops[-1]['wait_mask'] = 1 << _AUX_BRANCH
-                    x = name
-                cur, h, w = x, hh, ww
+                cur, h, w = self._emit_block(block, 's%db%d' % (si, bi), cur, h, w, len(taps))
                 if (si, bi) in taps:
                     l = taps.index((si, bi))
                     assert (h, w) == self.level_sizes[l]
@@ -499,40 +508,7 @@ class InferencePlan(object):
         fb, bb = self.params_f32.data_ptr(), self.params_bf16.data_ptr()
         arr = (nat.Op * len(self._ops))()
         for i, op in enumerate(self._ops):
-            o = arr[i]
-            o.kind = op['kind']
-            o.dtype = self.dtype_code
-            o.N, o.H, o.W, o.Cin, o.Ho, o.Wo, o.Cout = self.N, op['H'], op['W'], op['Cin'], op['Ho'], op['Wo'], op['Cout']
-            o.ksize, o.stride, o.relu = op.get('ksize', 1), op.get('stride', 1), op.get('relu', 0)
-            o.gn_groups = op.get('gn_groups', 0)
-            o.n_cls, o.n_reg, o.point_off, o.cc = op.get('n_cls', 0), op.get('n_reg', 0), op.get('point_off', 0), op.get('cc', 0)
-            o.branch = op.get('branch', 0)
-            o.wait_mask = op.get('wait_mask', 0)
-            o.max_ctas = op.get('max_ctas', 0)
-            o.tail_cout, o.tail_relu = op.get('tail_cout', 0), op.get('tail_relu', 0)
-            if op.get('tail_cout'):
-                o.tail_weight = bb + 2 * op['tail_w']
-                o.tail_shift = fb + 4 * op['tail_shift']
-            o.ds_cout, o.ds_out_off = op.get('ds_cout', 0), -1
-            if op.get('ds_cout'):
-                o.ds_weight = bb + 2 * op['ds_w']
-                o.ds_shift = fb + 4 * op['ds_shift']
-                o.ds_out_off = offsets[op['out2']]
-            if op['kind'] == nat.OP_STEM4:
-                o.s2_weight, o.s2_shift, o.s2_relu = bb + 2 * op['s2_w'], fb + 4 * op['s2_shift'], op['s2_relu']
-                o.s3_weight, o.s3_shift, o.s3_relu = bb + 2 * op['s3_w'], fb + 4 * op['s3_shift'], op['s3_relu']
-            o.in_off = offsets[op['inp']] if op.get('inp') is not None else -1
-            o.out_off = offsets[op['out']] if op.get('out') is not None else -1
-            o.res_off = offsets[op['res']] if op.get('res') is not None else -1
-            o.stats_off = op['stats'] * stats_each if op.get('stats') is not None else -1
-            if 'w_bf16' in op:
-                o.weight = bb + 2 * op['w_bf16']
-            elif 'w_f32' in op:
-                o.weight = fb + 4 * op['w_f32']
-            o.scale = fb + 4 * op['scale'] if 'scale' in op else None
-            o.shift = fb + 4 * op['shift'] if 'shift' in op else None
-            o.gamma = fb + 4 * op['gamma'] if 'gamma' in op else None
-            o.beta = fb + 4 * op['beta'] if 'beta' in op else None
+            self._fill_op(arr[i], op, offsets, fb, bb, stats_each)
         self._op_array = arr
         self.cls_out = torch.empty((self.N, self.P, self.cls_channels), dtype=torch.float32, device=dev)
         self.reg_out = torch.empty((self.N, self.P, 4), dtype=torch.float32, device=dev)
@@ -544,6 +520,42 @@ class InferencePlan(object):
         self.handle = self._create_handle()
         self.num_launches = nat.lib().lfd_plan_num_launches(self.handle)
         self.side_ctas, self.autotuned = {}, False     # branch -> bound on the persistent CTAs of its convs (autotune)
+
+    def _fill_op(self, o, op, offsets, fb, bb, stats_each=0):
+        """op dict -> nat.Op: tensor names through `offsets`, staged parameters relative to the fp32 / 16-bit buffers at fb / bb."""
+        o.kind = op['kind']
+        o.dtype = self.dtype_code
+        o.N, o.H, o.W, o.Cin, o.Ho, o.Wo, o.Cout = self.N, op['H'], op['W'], op['Cin'], op['Ho'], op['Wo'], op['Cout']
+        o.ksize, o.stride, o.relu = op.get('ksize', 1), op.get('stride', 1), op.get('relu', 0)
+        o.gn_groups = op.get('gn_groups', 0)
+        o.n_cls, o.n_reg, o.point_off, o.cc = op.get('n_cls', 0), op.get('n_reg', 0), op.get('point_off', 0), op.get('cc', 0)
+        o.branch = op.get('branch', 0)
+        o.wait_mask = op.get('wait_mask', 0)
+        o.max_ctas = op.get('max_ctas', 0)
+        o.tail_cout, o.tail_relu = op.get('tail_cout', 0), op.get('tail_relu', 0)
+        if op.get('tail_cout'):
+            o.tail_weight = bb + 2 * op['tail_w']
+            o.tail_shift = fb + 4 * op['tail_shift']
+        o.ds_cout, o.ds_out_off = op.get('ds_cout', 0), -1
+        if op.get('ds_cout'):
+            o.ds_weight = bb + 2 * op['ds_w']
+            o.ds_shift = fb + 4 * op['ds_shift']
+            o.ds_out_off = offsets[op['out2']]
+        if op['kind'] == nat.OP_STEM4:
+            o.s2_weight, o.s2_shift, o.s2_relu = bb + 2 * op['s2_w'], fb + 4 * op['s2_shift'], op['s2_relu']
+            o.s3_weight, o.s3_shift, o.s3_relu = bb + 2 * op['s3_w'], fb + 4 * op['s3_shift'], op['s3_relu']
+        o.in_off = offsets[op['inp']] if op.get('inp') is not None else -1
+        o.out_off = offsets[op['out']] if op.get('out') is not None else -1
+        o.res_off = offsets[op['res']] if op.get('res') is not None else -1
+        o.stats_off = op['stats'] * stats_each if op.get('stats') is not None else -1
+        if 'w_bf16' in op:
+            o.weight = bb + 2 * op['w_bf16']
+        elif 'w_f32' in op:
+            o.weight = fb + 4 * op['w_f32']
+        o.scale = fb + 4 * op['scale'] if 'scale' in op else None
+        o.shift = fb + 4 * op['shift'] if 'shift' in op else None
+        o.gamma = fb + 4 * op['gamma'] if 'gamma' in op else None
+        o.beta = fb + 4 * op['beta'] if 'beta' in op else None
 
     def _create_handle(self):
         handle = C.c_void_p()
@@ -681,6 +693,22 @@ class InferencePlan(object):
                 self.handle = None
         except Exception:
             pass
+
+
+class PrefixEmitter(InferencePlan):
+    """The inference plan's stem and residual-block emitters, for a training plan's frozen backbone prefix (lfd/_train.py): the same
+    BatchNorm folding, weight packing and fusion decisions (STEM4 gate, fused tails and shortcuts), bf16, every op on the main stream.
+    The training plan places the ops in its own workspace and runs them as LFD_TOP_INFER ops."""
+
+    def __init__(self, N, H, W, device):
+        self._configure(N, H, W, device, nat.CONV_UMMA, False, 'bf16', None)
+        self.aux_shortcut = False
+
+    def staged(self):
+        """-> (fp32, int16) host tensors of the folded / packed parameters the ops' offsets point into."""
+        f32 = torch.cat(self._f32) if self._f32 else torch.zeros(4)
+        b16 = torch.cat(self._bf16) if self._bf16 else torch.zeros(8, dtype=torch.int16)
+        return f32, b16
 
 
 def make_norm_probe(head):

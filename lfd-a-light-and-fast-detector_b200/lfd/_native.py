@@ -67,9 +67,11 @@ class LossCfg(C.Structure):
                 ('cls_weight', C.c_float), ('reg_weight', C.c_float), ('max_ctas', C.c_int32)]
 
 
-# training plan ops (include/lfd_b200.h, lfd_top)
+# training plan ops (include/lfd_b200.h, lfd_top).  TOP_INFER runs one inference op (an Op: STEM0 / CONV with tail and shortcut /
+# STEM4, bf16) inside a training plan: ptr[0] = the host address of the Op, off[0..3] = its input / output / residual / shortcut
+# output, which replace the Op's own offsets (the frozen backbone prefix of a fine-tuning step, lfd/_train.py)
 (TOP_PACK, TOP_STEM0, TOP_CONV, TOP_BN_STATS, TOP_BN_APPLY, TOP_GN_APPLY, TOP_HEAD_FINAL, TOP_HEAD_FINAL_BWD, TOP_NORM_BWD_REDUCE,
- TOP_NORM_BWD_APPLY, TOP_WGRAD, TOP_WGRAD_STEM, TOP_UNPACK, TOP_ZERO) = range(14)
+ TOP_NORM_BWD_APPLY, TOP_WGRAD, TOP_WGRAD_STEM, TOP_UNPACK, TOP_ZERO, TOP_INFER) = range(15)
 WGRAD_UMMA, WGRAD_SIMT = 0, 1
 PACK_CONV_FWD, PACK_CONV_DGRAD, PACK_STEM, PACK_ROUND_F32, PACK_SCALE_SHIFT = range(5)
 UNPACK_CONV, UNPACK_ADD = 0, 1

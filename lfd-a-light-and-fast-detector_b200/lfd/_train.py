@@ -13,6 +13,9 @@ clip + SGD step (lfd/execution/optim.py) are single calls.  Per step the fp32 ma
 operands (PACK), weight gradients are accumulated in fp32 staging tensors by the wgmma wgrad kernel and scattered into the
 OIHW gradient tensors at the end (UNPACK).
 
+Fine-tuning (frozen parameters, LFDResNet(frozen_stages=k)): backward ops are emitted only for what reaches a trainable parameter, and the
+frozen backbone prefix runs on the inference plan's ops and packing (LFD_TOP_INFER), keeping only the tensors the trainable part reads.
+
 Rounding points (bf16 training): conv output z (fp32 accumulate) -> bf16; BatchNorm statistics over the stored z (fp64 sums);
 normalised + residual + ReLU output -> bf16; every activation gradient -> bf16; weight / norm-parameter gradients fp32.
 """
@@ -23,6 +26,7 @@ import torch
 import torch.nn as nn
 
 from . import _native as nat
+from ._engine import PrefixEmitter, _Arena
 
 __all__ = ['FlatParameters', 'TrainPlan', 'train_forward']
 
@@ -63,10 +67,14 @@ class FlatParameters(object):
         self.attach_grads()
 
     def attach_grads(self):
-        """(Re-)installs the .grad views (optimizer.zero_grad(set_to_none=True) drops them)."""
+        """(Re-)installs the .grad views (optimizer.zero_grad(set_to_none=True) drops them).  A frozen parameter (requires_grad False)
+        has no gradient, as after torch's backward: its slot of the flat gradient stays zero and its .grad None."""
         for p, off in zip(self.params, self.offsets):
             g = self.grad[off:off + p.numel()].view(p.shape)
-            if p.grad is None or p.grad.data_ptr() != g.data_ptr():
+            if not p.requires_grad:
+                if p.grad is not None and p.grad.data_ptr() == g.data_ptr():
+                    p.grad = None
+            elif p.grad is None or p.grad.data_ptr() != g.data_ptr():
                 p.grad = g
 
     def intact(self):
@@ -126,6 +134,9 @@ class TrainPlan(object):
         self._grad_written = set()
         self._zero_fwd, self._zero_bwd = [], []          # (name) regions cleared at the start of the forward / backward
         self._check_supported(model)
+        self._trainable = {id(p) for p in model.parameters() if p.requires_grad}
+        self._needs_grad = set()                         # forward tensors with a trainable parameter upstream: the only ones given a gradient
+        self._prefix = None                              # the frozen backbone prefix, run on the inference kernels (_emit_prefix)
         self._build(model)
         self._finalize()
 
@@ -138,9 +149,8 @@ class TrainPlan(object):
                     raise NotImplementedError('native training needs affine BatchNorm2d with running statistics and a fixed momentum')
             if isinstance(m, nn.Conv2d) and (m.groups != 1 or m.dilation != (1, 1)):
                 raise NotImplementedError('grouped / dilated convolutions are outside the LFD hot path')
-        for p in model.parameters():
-            if not p.requires_grad:
-                raise NotImplementedError('native training differentiates every parameter (no frozen parameters)')
+        if not any(p.requires_grad for p in model.parameters()):
+            raise ValueError('no parameter of the model is trainable (every requires_grad is False): nothing to train')
 
     # ------------------------------------------------------------------ workspace
     def _alloc(self, name, nbytes):
@@ -176,6 +186,14 @@ class TrainPlan(object):
                                            src=name, dst=conv.weight))
         return self._gstage[key]
 
+    def _tr(self, *params):
+        return any(p is not None and id(p) in self._trainable for p in params)
+
+    def _mark(self, outs, inputs, params):
+        """The tensors `outs` need a gradient when one of `inputs` does or one of `params` is trainable."""
+        if any(t is not None and t in self._needs_grad for t in inputs) or self._tr(*params):
+            self._needs_grad.update(outs)
+
     # ------------------------------------------------------------------ forward emitters
     def _conv_bn(self, name, conv, norm, relu, x, h, w, res=None):
         """conv (no bias) -> BatchNorm (batch statistics) -> (+res) -> ReLU.  x = None: the stem conv on the image."""
@@ -205,6 +223,7 @@ class TrainPlan(object):
         self._fwd.append(dict(kind=nat.TOP_BN_APPLY, relu=int(relu), momentum=float(norm.momentum), off={0: z, 1: y, 2: res, 3: sums},
                               ptr={0: norm.weight, 1: norm.bias, 2: norm.running_mean, 3: norm.running_var}, **bn_geo))
         self._layers.append(dict(type='bn', name=name, conv=conv, norm=norm, relu=relu, x=x, z=z, y=y, res=res, sums=sums, geo=geo, frozen=frozen))
+        self._mark([y], [x, res], [conv.weight, norm.weight, norm.bias])
         if not frozen:
             self._bn_modules.append(norm)
         return y, ho, wo
@@ -230,6 +249,7 @@ class TrainPlan(object):
             self._fwd.append(dict(kind=nat.TOP_GN_APPLY, N=self.N, H=h, W=w, Cout=cout, groups=16, eps=float(norm.eps), off={0: raw, 1: act, 3: stats},
                                   ptr={0: norm.weight, 1: norm.bias}))
         self._layers.append(dict(type='gn', name=name, conv=conv, norm=norm, x=x, raw=raw, act=act, stats=stats, geo=geo))
+        self._mark([raw, act], [x], [conv.weight, norm.weight, norm.bias])
         return raw, act, stats
 
     @staticmethod
@@ -262,7 +282,8 @@ class TrainPlan(object):
         import types
         fake = types.SimpleNamespace(weight=c['ones'], bias=conv.bias, running_mean=c['zeros'], running_var=c['var'], eps=1e-5)
         self._layers.append(dict(type='bn', name=name, conv=conv, norm=fake, relu=True, x=x, z=z, y=y, res=None, sums=None, geo=geo, frozen=1,
-                                 dgamma=c['sink'], dbeta=('grad', conv.bias)))
+                                 dgamma=c['sink'], dbeta=('grad', conv.bias) if self._tr(conv.bias) else None))
+        self._mark([y], [x], [conv.weight, conv.bias])
         return y
 
     def _head_final(self, name, l, raw, stats, norm, convs, n_cls, n_reg, h, w, point_off, scale_param):
@@ -276,8 +297,10 @@ class TrainPlan(object):
             row = 0
             for c in convs:
                 r = c.out_channels
-                self._unpack.items.append(dict(kind=nat.UNPACK_ADD, n=r * Cc, src=(ds, row * Cc * 4), dst=c.weight))
-                self._unpack.items.append(dict(kind=nat.UNPACK_ADD, n=r, src=(ds, (no * Cc + row) * 4), dst=c.bias))
+                if self._tr(c.weight):
+                    self._unpack.items.append(dict(kind=nat.UNPACK_ADD, n=r * Cc, src=(ds, row * Cc * 4), dst=c.weight))
+                if self._tr(c.bias):
+                    self._unpack.items.append(dict(kind=nat.UNPACK_ADD, n=r, src=(ds, (no * Cc + row) * 4), dst=c.bias))
                 row += r
         ds = self._hstage[key]
         # the weight rows are shared by the levels; scale / shift / bias depend on the level's Scale parameter, so every level
@@ -294,7 +317,7 @@ class TrainPlan(object):
                                          dst=(lst, (no * Cc + row) * 4), dst2=(lst, (no * Cc + no + row) * 4), dst3=(lst, (no * Cc + 2 * no + row) * 4)))
             row += r
         dscale = None
-        if scale_param is not None and n_reg:
+        if scale_param is not None and n_reg and self._tr(scale_param):
             dscale = self._alloc('%s_dscale' % name, 4)
             self._zero_bwd.append(dscale)
             self._unpack.items.append(dict(kind=nat.UNPACK_ADD, n=1, src=dscale, dst=scale_param))
@@ -307,13 +330,56 @@ class TrainPlan(object):
                                  dact='d_' + (raw + '_act' if gn else raw)))
 
     # ------------------------------------------------------------------ graph walk (same order as the inference plan)
+    @staticmethod
+    def _prefix_units(model):
+        """Modules of the frozen backbone prefix: the longest run of backbone units from the input (the stem, then whole residual
+        blocks) whose parameters are all frozen and whose BatchNorms are all in eval mode -- with BatchNorm folded, exactly the
+        inference network.  LFDResNet(frozen_stages=k >= 1) freezes the stem and stages 0..k-1 so."""
+        bb = model._backbone
+        units = [bb._stem] + [block for stage in bb.stages() for block in stage]
+        n = 0
+        for u in units:
+            if any(p.requires_grad for p in u.parameters()) or any(isinstance(m, nn.BatchNorm2d) and m.training for m in u.modules()):
+                break
+            n += 1
+        return units[:n]
+
+    def _emit_prefix(self, model, n_units):
+        """The first n_units backbone units on the inference plan's emitters -> (emitter, [(first op, end op, output, h, w) per unit])."""
+        bb = model._backbone
+        pre = PrefixEmitter(self.N, self.H, self.W, self.device)
+        cur, h, w = pre._emit_stem(bb.stem_layers(), self.H, self.W)
+        units = [(0, len(pre._ops), cur, h, w)]
+        blocks = [('s%db%d' % (si, bi), block) for si, stage in enumerate(bb.stages()) for bi, block in enumerate(stage)]
+        for base, block in blocks[:n_units - 1]:
+            b0 = len(pre._ops)
+            cur, h, w = pre._emit_block(block, base, cur, h, w, len(bb._out_indices))
+            units.append((b0, len(pre._ops), cur, h, w))
+        return pre, units
+
+    def _infer_unit(self, unit):
+        """LFD_TOP_INFER ops of one prefix unit (their Op descriptors are filled in by _stage_prefix once the workspace is laid out)."""
+        for op in self._prefix['emitter']._ops[unit[0]:unit[1]]:
+            self._fwd.append(dict(kind=nat.TOP_INFER, N=self.N, H=op['H'], W=op['W'], Cin=op['Cin'], Ho=op['Ho'], Wo=op['Wo'], Cout=op['Cout'],
+                                  ksize=op.get('ksize', 1), stride=op.get('stride', 1), relu=op.get('relu', 0),
+                                  off={0: op.get('inp'), 1: op['out'], 2: op.get('res'), 3: op.get('out2')}, ptr={0: None}))
+            self._prefix['ops'].append((self._fwd[-1], op))
+
     def _build(self, model):
         bb, neck, head = model._backbone, model._neck, model._head
         self._bn_modules = []
         h, w = self.H, self.W
         cur = None
-        for i, (conv, norm, relu) in enumerate(bb.stem_layers()):
-            cur, h, w = self._conv_bn('stem%d' % i, conv, norm, relu, cur, h, w)
+        modules = self._prefix_units(model)
+        units = []
+        if modules:
+            pre, units = self._emit_prefix(model, len(modules))
+            self._prefix = dict(emitter=pre, modules=modules, ops=[])
+            self._infer_unit(units[0])
+            cur, h, w = units[0][2:]
+        else:
+            for i, (conv, norm, relu) in enumerate(bb.stem_layers()):
+                cur, h, w = self._conv_bn('stem%d' % i, conv, norm, relu, cur, h, w)
         taps = list(bb._out_indices)
         if len(taps) != head._num_heads:
             raise ValueError('backbone taps (%d) and head levels (%d) differ' % (len(taps), head._num_heads))
@@ -330,19 +396,25 @@ class TrainPlan(object):
         for fh, fw in self.level_sizes:
             offs.append(acc)
             acc += fh * fw
+        ui = 0
         for si, stage in enumerate(bb.stages()):
             for bi, block in enumerate(stage):
                 base = 's%db%d' % (si, bi)
-                identity = cur
-                if block._downsample is not None:
-                    ds = list(block._downsample)
-                    identity, _, _ = self._conv_bn(base + '_id', ds[0], ds[1] if len(ds) > 1 else None, False, cur, h, w)
-                x, hh, ww = cur, h, w
-                pairs = block.conv_norm_pairs()
-                for li, (conv, norm) in enumerate(pairs):
-                    last = li == len(pairs) - 1
-                    x, hh, ww = self._conv_bn(base + ('_out' if last else '_c%d' % li), conv, norm, True, x, hh, ww, res=identity if last else None)
-                cur, h, w = x, hh, ww
+                ui += 1
+                if ui < len(units):                      # a block of the frozen prefix
+                    self._infer_unit(units[ui])
+                    cur, h, w = units[ui][2:]
+                else:
+                    identity = cur
+                    if block._downsample is not None:
+                        ds = list(block._downsample)
+                        identity, _, _ = self._conv_bn(base + '_id', ds[0], ds[1] if len(ds) > 1 else None, False, cur, h, w)
+                    x, hh, ww = cur, h, w
+                    pairs = block.conv_norm_pairs()
+                    for li, (conv, norm) in enumerate(pairs):
+                        last = li == len(pairs) - 1
+                        x, hh, ww = self._conv_bn(base + ('_out' if last else '_c%d' % li), conv, norm, True, x, hh, ww, res=identity if last else None)
+                    cur, h, w = x, hh, ww
                 if (si, bi) in taps:
                     l = taps.index((si, bi))
                     f0, l0 = len(self._fwd), len(self._layers)
@@ -388,14 +460,18 @@ class TrainPlan(object):
         return g
 
     def _emit_conv_backward(self, L, dz, dz_up):
-        """Weight gradient and data gradient of L['conv'] given the gradient of its output."""
+        """Weight gradient (trainable weight) and data gradient (input with a trainable parameter upstream) of L['conv'] given the
+        gradient of its output."""
         conv, geo, x = L['conv'], L['geo'], L['x']
-        gs = self._gstage_of(conv)
-        if x is None:
-            x27 = self._act('stem_im2col', geo['Ho'], geo['Wo'], 32)      # scratch of the im2col + wgmma path
-            self._bwd.append(dict(kind=nat.TOP_WGRAD_STEM, impl=nat.WGRAD_UMMA, off={0: x27, 1: dz, 5: gs}, **geo))
+        if self._tr(conv.weight):
+            gs = self._gstage_of(conv)
+            if x is None:
+                x27 = self._act('stem_im2col', geo['Ho'], geo['Wo'], 32)      # scratch of the im2col + wgmma path
+                self._bwd.append(dict(kind=nat.TOP_WGRAD_STEM, impl=nat.WGRAD_UMMA, off={0: x27, 1: dz, 5: gs}, **geo))
+                return
+            self._bwd.append(dict(kind=nat.TOP_WGRAD, impl=nat.WGRAD_UMMA, off={0: x, 1: dz, 5: gs}, **geo))
+        if x is None or x not in self._needs_grad:
             return
-        self._bwd.append(dict(kind=nat.TOP_WGRAD, impl=nat.WGRAD_UMMA, off={0: x, 1: dz, 5: gs}, **geo))
         # data gradient = the forward kernel on the transposed / tap-flipped weights (stride 2: on the zero-inserted dz)
         k, s, cin, cout, h, w = geo['ksize'], geo['stride'], geo['Cin'], geo['Cout'], geo['H'], geo['W']
         cc = self._query(self.N, h, w, cout, h, w, cin, k, 1)['cc']
@@ -416,8 +492,14 @@ class TrainPlan(object):
             for op in self._bwd[b0:]:
                 op['branch'] = L.get('branch', 0)
 
+    def _grad_ptr(self, p):
+        """Where a norm backward deposits d loss / d p: p's gradient slot, or nothing for a frozen parameter."""
+        return ('grad', p) if self._tr(p) else None
+
     def _backward_of(self, L):
         geo = L['geo']
+        if L['type'] != 'final' and L['raw' if L['type'] == 'gn' else 'y'] not in self._needs_grad:
+            return                                    # no trainable parameter at or upstream of this layer: no backward
         if L['type'] == 'final':
             dact = L['dact']
             acc = dact in self._grad_written          # (never: every tower has its own last tensor)
@@ -441,8 +523,8 @@ class TrainPlan(object):
             offs = {0: dact, 2: L['raw'], 3: L['stats'], 4: bs}
             self._bwd.append(dict(kind=nat.TOP_NORM_BWD_REDUCE, off=dict(offs), ptr={0: L['norm'].weight, 1: L['norm'].bias}, **n_geo))
             offs[5] = draw
-            self._bwd.append(dict(kind=nat.TOP_NORM_BWD_APPLY, off=offs, ptr={0: L['norm'].weight, 1: L['norm'].bias, 2: ('grad', L['norm'].weight),
-                                                                           3: ('grad', L['norm'].bias)}, **n_geo))
+            self._bwd.append(dict(kind=nat.TOP_NORM_BWD_APPLY, off=offs, ptr={0: L['norm'].weight, 1: L['norm'].bias, 2: self._grad_ptr(L['norm'].weight),
+                                                                           3: self._grad_ptr(L['norm'].bias)}, **n_geo))
             self._emit_conv_backward(L, draw, None)
         else:
             ho, wo, cout, s = geo['Ho'], geo['Wo'], geo['Cout'], geo['stride']
@@ -452,10 +534,10 @@ class TrainPlan(object):
             bs = self._alloc(L['name'] + '_bsums', cout * 16)
             self._zero_bwd.append(bs)
             dz = self._grad_of(L['z'], ho, wo, cout)
-            need_up = s == 2 and L['x'] is not None
+            need_up = s == 2 and L['x'] is not None and L['x'] in self._needs_grad
             dz_up = self._act('d_' + L['z'] + '_up', geo['H'], geo['W'], cout) if need_up else None
             dres, acc = None, 0
-            if L['res'] is not None:
+            if L['res'] is not None and L['res'] in self._needs_grad:
                 dres = self._grad_of(L['res'], ho, wo, cout)
                 acc = int(dres in self._grad_written)
                 self._grad_written.add(dres)
@@ -465,7 +547,9 @@ class TrainPlan(object):
             self._bwd.append(dict(kind=nat.TOP_NORM_BWD_REDUCE, off=dict(offs), ptr={0: L['norm'].weight, 1: L['norm'].bias, 4: rstats[4], 5: rstats[5]}, **n_geo))
             offs.update({5: dz, 6: dz_up, 7: dres})
             self._bwd.append(dict(kind=nat.TOP_NORM_BWD_APPLY, accumulate=acc, upH=geo['H'] if need_up else 0, upW=geo['W'] if need_up else 0, off=offs,
-                                  ptr={0: L['norm'].weight, 1: L['norm'].bias, 2: L.get('dgamma', ('grad', L['norm'].weight)), 3: L.get('dbeta', ('grad', L['norm'].bias)),
+                                  ptr={0: L['norm'].weight, 1: L['norm'].bias,
+                                       2: L['dgamma'] if 'dgamma' in L else self._grad_ptr(L['norm'].weight),
+                                       3: L['dbeta'] if 'dbeta' in L else self._grad_ptr(L['norm'].bias),
                                        4: rstats[4], 5: rstats[5]},
                                   **n_geo))
             self._emit_conv_backward(L, dz, dz_up)
@@ -476,7 +560,8 @@ class TrainPlan(object):
               nat.TOP_HEAD_FINAL: {0: 'R', 3: 'R', 4: 'R'}, nat.TOP_HEAD_FINAL_BWD: {0: 'R', 1: 'W', 3: 'R', 4: 'R', 5: 'A', 6: 'A'},
               nat.TOP_NORM_BWD_REDUCE: {0: 'R', 1: 'R', 2: 'R', 3: 'R', 4: 'A'},
               nat.TOP_NORM_BWD_APPLY: {0: 'R', 1: 'R', 2: 'R', 3: 'R', 4: 'R', 5: 'W', 6: 'W', 7: 'W'},
-              nat.TOP_WGRAD: {0: 'R', 1: 'R', 5: 'A'}, nat.TOP_WGRAD_STEM: {0: 'W', 1: 'R', 5: 'A'}}
+              nat.TOP_WGRAD: {0: 'R', 1: 'R', 5: 'A'}, nat.TOP_WGRAD_STEM: {0: 'W', 1: 'R', 5: 'A'},
+              nat.TOP_INFER: {0: 'R', 1: 'W', 2: 'R', 3: 'W'}}
 
     @classmethod
     def _assign_waits(cls, ops):
@@ -535,6 +620,65 @@ class TrainPlan(object):
                         st['r'][b] = me
             op['wait_mask'] = mask
 
+    # ------------------------------------------------------------------ frozen prefix
+    def _place_prefix(self):
+        """Workspace of the prefix: the tensors the trainable part reads (taps inside the prefix, the boundary tensor) get their own
+        regions; every other prefix tensor lives in one scratch region, reused by liveness as in the inference plan."""
+        pre, ops = self._prefix['emitter'], [op for _, op in self._prefix['ops']]
+        outs = {op[k] for op in ops for k in ('out', 'out2') if op.get(k) is not None}
+        read = {v for op in self._fwd if op['kind'] != nat.TOP_INFER for v in op.get('off', {}).values()}
+        keep = outs & read
+        shapes = {}
+        for op in ops:
+            shapes[op['out']] = (op['Ho'], op['Wo'], op.get('tail_cout') or op['Cout'])
+            if op.get('out2') is not None:
+                shapes[op['out2']] = (op['Ho'], op['Wo'], op['ds_cout'])
+        self.prefix_outputs = {n: shapes[n] for n in keep}          # name -> (h, w, channels), bf16 NHWC
+        for n in sorted(keep):
+            self._alloc(n, pre._tensors[n])
+        last = {op[k]: i for i, op in enumerate(ops) for k in ('inp', 'res') if op.get(k) is not None and op[k] not in keep}
+        arena, local = _Arena(), {}
+        for i, op in enumerate(ops):
+            for k in ('out', 'out2'):
+                if op.get(k) is not None and op[k] not in keep:
+                    local[op[k]] = arena.alloc(pre._tensors[op[k]])
+            for n, lu in last.items():
+                if lu == i:
+                    arena.release(local[n], pre._tensors[n])
+        if local:
+            self._alloc('prefix_scratch', arena.top)
+        self._prefix['scratch'] = local
+
+    def _prefix_fingerprint(self):
+        return tuple((t.data_ptr(), t._version) for m in self._prefix['modules'] for t in list(m.parameters()) + list(m.buffers()))
+
+    def _stage_prefix(self):
+        """Folded BatchNorm + packed weights of the prefix (host-built, as the inference plan builds them) and one Op descriptor per
+        LFD_TOP_INFER op pointing at them."""
+        pre = self._prefix['emitter']
+        for n, o in self._prefix['scratch'].items():
+            self._off[n] = self._off['prefix_scratch'] + o
+        f32, b16 = pre.staged()
+        self._prefix['f32'], self._prefix['b16'] = f32.to(self.device), b16.to(self.device)
+        self._prefix['fp'] = self._prefix_fingerprint()
+        fb, bb = self._prefix['f32'].data_ptr(), self._prefix['b16'].data_ptr()
+        arr = (nat.Op * len(self._prefix['ops']))()
+        for i, (top, op) in enumerate(self._prefix['ops']):
+            pre._fill_op(arr[i], op, self._off, fb, bb)
+            top['ptr'][0] = C.addressof(arr[i])
+        self._prefix['arr'] = arr
+
+    def _restage_prefix(self):
+        """A prefix parameter or buffer changed (load_state_dict, a checkpoint resume, a pretrained-weight load): fold and pack again
+        into the same device buffers, which the native plans and their CUDA graphs point at."""
+        pre, _ = self._emit_prefix(self.model, len(self._prefix['modules']))
+        f32, b16 = pre.staged()
+        if f32.shape != self._prefix['f32'].shape or b16.shape != self._prefix['b16'].shape:
+            raise RuntimeError('the frozen prefix changed its structure; build a new training plan')
+        self._prefix['f32'].copy_(f32)
+        self._prefix['b16'].copy_(b16)
+        self._prefix['fp'] = self._prefix_fingerprint()
+
     def _layout(self):
         """Byte offsets: [regions cleared before the forward][regions cleared before the backward][everything else]."""
         zf, zb = set(self._zero_fwd), set(self._zero_bwd)
@@ -547,7 +691,11 @@ class TrainPlan(object):
     def _finalize(self):
         dev = self.device
         self._build_backward()
+        if self._prefix is not None:
+            self._place_prefix()
         self._layout()
+        if self._prefix is not None:
+            self._stage_prefix()
         self.workspace_bytes = self._top + 256
         self.workspace = torch.zeros(self.workspace_bytes, dtype=torch.uint8, device=dev)
         base = self.workspace.data_ptr()
@@ -558,9 +706,11 @@ class TrainPlan(object):
         self.anchor = torch.zeros(1, dtype=torch.float32, device=dev, requires_grad=True)
         named = {'cls': self.cls_out, 'reg': self.reg_out, 'gcls': self.gcls, 'greg': self.greg}
 
-        def addr(v):      # workspace name | (name, byte offset) | tensor | ('grad', param) | None -> absolute device pointer
+        def addr(v):      # workspace name | (name, byte offset) | tensor | ('grad', param) | None | address -> absolute pointer
             if v is None:
                 return 0
+            if isinstance(v, int):
+                return v
             if isinstance(v, str):
                 return named[v].data_ptr() if v in named else base + self._off[v]
             if isinstance(v, tuple) and v[0] == 'grad':
@@ -643,6 +793,8 @@ class TrainPlan(object):
         if self._input is None or self._input.dtype != x.dtype:
             self._input = torch.empty_like(x, memory_format=torch.contiguous_format)
         self._input.copy_(x)
+        if self._prefix is not None and self._prefix_fingerprint() != self._prefix['fp']:
+            self._restage_prefix()
         self._fmt = fmt
         with torch.cuda.device(self.device):
             nat.check(nat.lib().lfd_train_plan_run(self.fwd_handle, nat.ptr(self._input), fmt, nat.ptr(self.workspace), int(bool(use_graph)), nat.stream_ptr()))

@@ -65,19 +65,25 @@ class FusedSGD(torch.optim.Optimizer):
             self._pending = None
             self._sq = torch.zeros(1, dtype=torch.float64, device=flat.data.device)
             self._make_runs()
+        elif tuple(p.requires_grad for p in flat.params) != self._requires_grad:      # parameters frozen / unfrozen since
+            self._make_runs()
         return flat
 
     def _make_runs(self):
         """Maximal runs of flat slots with the same hyper-parameters and the same momentum-buffer state: (begin, end, group index,
-        every parameter of the run has a buffer)."""
+        every parameter of the run has a buffer).  Frozen parameters (requires_grad False) have no gradient, and torch.optim.SGD
+        skips them -- no weight decay, no momentum, no buffer: they are in no run."""
         group_of = {}
         for gi, g in enumerate(self.param_groups):
             for p in g['params']:
                 group_of[id(p)] = gi
         runs = []
+        self._requires_grad = tuple(p.requires_grad for p in self._flat.params)
         for p, off in zip(self._flat.params, self._flat.offsets):
             if id(p) not in group_of:
                 raise ValueError('a model parameter is missing from the optimizer param_groups')
+            if not p.requires_grad:
+                continue
             end = off + (p.numel() + 3) // 4 * 4
             key = (group_of[id(p)], id(p) in self._has_buf)
             if runs and runs[-1][2:] == list(key) and runs[-1][1] == off:

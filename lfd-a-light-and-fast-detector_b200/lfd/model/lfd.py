@@ -142,8 +142,10 @@ class LFD(nn.Module):
         """The native training plan (forward + backward op lists) for one input shape (built on first use)."""
         from .._train import TrainPlan, flat_parameters
         flat_parameters(self)
-        # BatchNorm modules in eval mode (norm_eval, frozen stages) normalise with their running statistics: part of the plan
-        key = (n, h, w, str(device), tuple(m.training for m in self.modules() if isinstance(m, nn.BatchNorm2d)))
+        # BatchNorm modules in eval mode (norm_eval, frozen stages) normalise with their running statistics, and frozen parameters
+        # (requires_grad False) get no gradient ops and may form a prefix on the inference kernels: both are part of the plan
+        key = (n, h, w, str(device), tuple(m.training for m in self.modules() if isinstance(m, nn.BatchNorm2d)),
+               tuple(p.requires_grad for p in self.parameters()))
         if key not in self._train_plans:
             self._train_plans[key] = TrainPlan(self, n, h, w, device)
             self._train_plans[key].use_graph = bool(getattr(self, 'use_cuda_graph_training', False))
