@@ -47,28 +47,6 @@ struct PlannedOp {
     int grid;
 };
 
-struct lfd_plan {
-    std::vector<PlannedOp> ops;
-    int N, P, cls_channels, conv_impl;
-    int64_t stats_off, stats_bytes, workspace_bytes;
-    // CUDA graph cache: one instantiated graph per (input, workspace, cls, reg, format) pointer tuple
-    struct GraphEntry {
-        cudaGraphExec_t exec;
-        const void* input;
-        void* ws;
-        float* cls;
-        float* reg;
-        int fmt;
-    };
-    std::vector<GraphEntry> graphs;
-    // side streams for independent branches (the per-level neck + head chains)
-    cudaStream_t side[LFD_MAX_BRANCHES];
-    cudaEvent_t fork_ev[LFD_MAX_BRANCHES], join_ev[LFD_MAX_BRANCHES];
-    std::vector<cudaEvent_t> dep_ev;   // one per (op, wait_mask bit): mid-graph cross-branch dependencies
-    int n_branches;
-};
-static constexpr size_t kMaxGraphs = 32;
-
 // Stream the CUDA graphs are captured on: the main chain (the backbone: the critical path of the step) runs two priority levels above
 // the side streams of the per-level chains (created at the default = lowest level) -- captured kernel nodes inherit the level, so when
 // SMs free up the pending CTAs of the critical path are placed first.  The levels above are left to the caller's latency-critical
@@ -82,6 +60,172 @@ static cudaError_t create_capture_stream(cudaStream_t* cap) {
     }
     return cudaStreamCreateWithFlags(cap, cudaStreamNonBlocking);
 }
+
+// Runs the op list of either plan kind (lfd_plan, lfd_train_plan).  Op i runs on the caller's stream (branch 0) or on side stream b,
+// forked after the main-stream op that precedes the branch's first op; wait_mask bit w makes it wait for everything enqueued so far on
+// branch w; every started branch is joined back into the caller's stream at the end.  With use_graph the sequence is captured into a
+// CUDA graph on the first use of a pointer tuple and replayed afterwards.  launch(i, stream) enqueues op i and returns a status.
+struct BranchExecutor {
+    std::vector<int> branch, wait_mask;    // per op
+    int n_branches = 1;                    // side[b], fork_ev[b] and join_ev[b] exist for 1 <= b < n_branches
+    cudaStream_t side[LFD_MAX_BRANCHES];
+    cudaEvent_t fork_ev[LFD_MAX_BRANCHES], join_ev[LFD_MAX_BRANCHES];
+    std::vector<cudaEvent_t> dep_ev;       // one per (op, wait_mask bit): mid-graph cross-branch dependencies
+    int64_t clear_off = 0, clear_bytes = 0;   // workspace region zeroed on the caller's stream before the first op
+    size_t max_graphs = 0;
+    struct Graph {
+        cudaGraphExec_t exec;
+        const void* input;
+        void* ws;
+        float* cls;
+        float* reg;
+        int fmt;
+    };
+    std::vector<Graph> graphs;             // one instantiated graph per (input, workspace, cls, reg, format) tuple, oldest first
+
+    BranchExecutor() = default;
+    BranchExecutor(const BranchExecutor&) = delete;
+    BranchExecutor& operator=(const BranchExecutor&) = delete;
+    ~BranchExecutor() {
+        for (auto& g : graphs) cudaGraphExecDestroy(g.exec);
+        for (int b = 1; b < n_branches; ++b) {
+            cudaStreamDestroy(side[b]);
+            cudaEventDestroy(fork_ev[b]);
+            cudaEventDestroy(join_ev[b]);
+        }
+        for (auto ev : dep_ev) cudaEventDestroy(ev);
+    }
+
+    // Validates the schedule (branch_of(i), wait_of(i)) and creates the side streams and events.  On failure it keeps only what it
+    // created completely, which the destructor releases.
+    template <typename BranchOf, typename WaitOf>
+    int init(const char* who, int n_ops, BranchOf branch_of, WaitOf wait_of, size_t graph_cap) {
+        max_graphs = graph_cap;
+        int nb = 1;
+        size_t n_dep = 0;
+        for (int i = 0; i < n_ops; ++i) {
+            const int b = branch_of(i), w = wait_of(i);
+            if (b < 0 || b >= LFD_MAX_BRANCHES || w < 0 || w >= (1 << LFD_MAX_BRANCHES))
+                return fail(LFD_ERR_INVALID, "%s: op %d: branch %d / wait_mask 0x%x out of range", who, i, b, w);
+            branch.push_back(b);
+            wait_mask.push_back(w);
+            if (b + 1 > nb) nb = b + 1;
+            n_dep += (size_t)__builtin_popcount((unsigned)w);
+        }
+        for (int b = 1; b < nb; ++b) {
+            if (cudaStreamCreateWithFlags(&side[b], cudaStreamNonBlocking) != cudaSuccess) return fail(LFD_ERR_CUDA, "%s: cannot create side streams", who);
+            if (cudaEventCreateWithFlags(&fork_ev[b], cudaEventDisableTiming) != cudaSuccess) {
+                cudaStreamDestroy(side[b]);
+                return fail(LFD_ERR_CUDA, "%s: cannot create events", who);
+            }
+            if (cudaEventCreateWithFlags(&join_ev[b], cudaEventDisableTiming) != cudaSuccess) {
+                cudaStreamDestroy(side[b]);
+                cudaEventDestroy(fork_ev[b]);
+                return fail(LFD_ERR_CUDA, "%s: cannot create events", who);
+            }
+            n_branches = b + 1;
+        }
+        for (size_t i = 0; i < n_dep; ++i) {
+            cudaEvent_t ev;
+            if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) return fail(LFD_ERR_CUDA, "%s: cannot create dependency events", who);
+            dep_ev.push_back(ev);
+        }
+        return LFD_OK;
+    }
+
+    // Fork / wait / launch / join.  Every started branch is joined also on error paths, so that a stream capture can be closed.
+    template <typename Launch>
+    int enqueue(uint8_t* ws, cudaStream_t st, const Launch& launch) {
+        if (clear_bytes > 0) CUDA_TRY(cudaMemsetAsync(ws + clear_off, 0, (size_t)clear_bytes, st));
+        bool started[LFD_MAX_BRANCHES] = {false};
+        int rc = LFD_OK;
+        size_t dep = 0;
+        cudaError_t ce = cudaSuccess;
+        for (size_t i = 0; i < branch.size() && !rc && ce == cudaSuccess; ++i) {
+            const int b = branch[i];
+            cudaStream_t s = b > 0 ? side[b] : st;
+            if (b > 0 && !started[b]) {   // fork: everything enqueued on the main stream so far precedes this branch
+                if ((ce = cudaEventRecord(fork_ev[b], st)) != cudaSuccess || (ce = cudaStreamWaitEvent(s, fork_ev[b], 0)) != cudaSuccess) break;
+                started[b] = true;
+            }
+            for (int w = 0; w < LFD_MAX_BRANCHES && ce == cudaSuccess; ++w) {   // explicit cross-branch dependencies
+                if (!((wait_mask[i] >> w) & 1)) continue;
+                cudaEvent_t ev = dep_ev[dep++];
+                if (w == b || (w > 0 && (w >= n_branches || !started[w]))) continue;   // nothing to wait for
+                if ((ce = cudaEventRecord(ev, w == 0 ? st : side[w])) == cudaSuccess) ce = cudaStreamWaitEvent(s, ev, 0);
+            }
+            if (ce == cudaSuccess) rc = launch(i, s);
+        }
+        for (int b = 1; b < n_branches; ++b)
+            if (started[b]) {
+                cudaEventRecord(join_ev[b], side[b]);
+                cudaStreamWaitEvent(st, join_ev[b], 0);
+            }
+        if (!rc && ce != cudaSuccess) rc = fail(LFD_ERR_CUDA, "plan stream dependencies: %s", cudaGetErrorString(ce));
+        return rc;
+    }
+
+    template <typename Launch>
+    int run(const void* input, int fmt, void* workspace, float* cls, float* reg, int use_graph, cudaStream_t st, Launch launch) {
+        uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+        if (!use_graph) return enqueue(ws, st, launch);
+        for (auto& g : graphs)
+            if (g.input == input && g.ws == workspace && g.cls == cls && g.reg == reg && g.fmt == fmt) {
+                CUDA_TRY(cudaGraphLaunch(g.exec, st));
+                return LFD_OK;
+            }
+        // first use of this pointer tuple: one eager pass (sets function attributes outside of capture, surfaces launch errors directly
+        // and produces this call's results), then capture + instantiate for the following calls.  Capture executes nothing, so the
+        // state (statistics, staging) is untouched.
+        int rc = enqueue(ws, st, launch);
+        if (rc) return rc;
+        if (graphs.size() >= max_graphs) {
+            cudaGraphExecDestroy(graphs.front().exec);
+            graphs.erase(graphs.begin());
+        }
+        cudaStream_t cap;
+        CUDA_TRY(create_capture_stream(&cap));
+        cudaGraph_t graph = nullptr;
+        cudaError_t ce = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
+        if (ce != cudaSuccess) { cudaStreamDestroy(cap); return fail(LFD_ERR_CUDA, "cudaStreamBeginCapture: %s", cudaGetErrorString(ce)); }
+        rc = enqueue(ws, cap, launch);
+        ce = cudaStreamEndCapture(cap, &graph);
+        if (rc || ce != cudaSuccess) {
+            if (graph) cudaGraphDestroy(graph);
+            cudaStreamDestroy(cap);
+            return rc ? rc : fail(LFD_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(ce));
+        }
+        Graph e = {nullptr, input, workspace, cls, reg, fmt};
+        ce = cudaGraphInstantiate(&e.exec, graph, 0);
+        cudaGraphDestroy(graph);
+        cudaStreamDestroy(cap);
+        if (ce != cudaSuccess) return fail(LFD_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(ce));
+        graphs.push_back(e);
+        return LFD_OK;
+    }
+
+    // One eager pass with every op on the caller's stream and an event pair around each -> ms_per_op[i].
+    template <typename Launch>
+    int profile(const char* who, uint8_t* ws, float* ms_per_op, cudaStream_t st, Launch launch) {
+        const size_t n = branch.size();
+        std::vector<cudaEvent_t> ev(n + 1);
+        for (auto& e : ev) CUDA_TRY(cudaEventCreate(&e));
+        if (clear_bytes > 0) CUDA_TRY(cudaMemsetAsync(ws + clear_off, 0, (size_t)clear_bytes, st));
+        int rc = LFD_OK;
+        CUDA_TRY(cudaEventRecord(ev[0], st));
+        for (size_t i = 0; i < n && !rc; ++i) {
+            rc = launch(i, st);
+            cudaEventRecord(ev[i + 1], st);
+        }
+        cudaError_t ce = cudaStreamSynchronize(st);
+        if (!rc && ce == cudaSuccess)
+            for (size_t i = 0; i < n; ++i) cudaEventElapsedTime(&ms_per_op[i], ev[i], ev[i + 1]);
+        for (auto& e : ev) cudaEventDestroy(e);
+        if (rc) return rc;
+        if (ce != cudaSuccess) return fail(LFD_ERR_CUDA, "%s: %s", who, cudaGetErrorString(ce));
+        return LFD_OK;
+    }
+};
 
 
 extern "C" int lfd_debug_set_trace(void* device_buffer) {
@@ -198,7 +342,7 @@ static int bounded_sms(int max_ctas) {
     return max_ctas > 0 && max_ctas < sms ? max_ctas : sms;
 }
 
-static int plan_op(const lfd_op& o, int conv_impl, PlannedOp* out) {
+static int plan_op(const lfd_op& o, PlannedOp* out) {
     int rc = check_op(o);
     if (rc) return rc;
     out->op = o;
@@ -211,7 +355,6 @@ static int plan_op(const lfd_op& o, int conv_impl, PlannedOp* out) {
         if (o.max_ctas < 0) return fail(LFD_ERR_INVALID, "max_ctas = %d", o.max_ctas);
         if (o.max_ctas > 0 && out->grid > o.max_ctas) out->grid = o.max_ctas;   // tiles are strided by gridDim (fused stem: contiguous runs): any grid size is valid
     }
-    (void)conv_impl;
     return LFD_OK;
 }
 
@@ -306,157 +449,55 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
     return LFD_OK;
 }
 
+// graph-cache bounds: how many pointer tuples a plan keeps an instantiated graph for (callers rotate input buffers and output slots)
+static constexpr size_t kMaxInferenceGraphs = 32;
+static constexpr size_t kMaxTrainingGraphs = 8;
+
+struct lfd_plan {
+    std::vector<PlannedOp> ops;
+    int P, cls_channels, conv_impl;
+    BranchExecutor ex;   // the GroupNorm statistics region is its clear region
+};
+
 extern "C" int lfd_plan_create(const lfd_op* ops, int n_ops, int N, int P, int cls_channels, int64_t stats_off, int64_t stats_bytes,
                                int64_t workspace_bytes, int conv_impl, lfd_plan** out) {
     if (!ops || n_ops <= 0 || !out) return fail(LFD_ERR_INVALID, "lfd_plan_create: bad arguments");
     if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_plan_create: no CUDA device (there is no CPU fallback)");
     lfd_plan* pl = new lfd_plan();
-    pl->N = N; pl->P = P; pl->cls_channels = cls_channels; pl->conv_impl = conv_impl;
-    pl->stats_off = stats_off; pl->stats_bytes = stats_bytes; pl->workspace_bytes = workspace_bytes;
-    pl->n_branches = 1;
-    for (int i = 0; i < n_ops; ++i) {
-        PlannedOp po;
-        int rc = plan_op(ops[i], conv_impl, &po);
-        if (rc) { delete pl; return rc; }
-        if (ops[i].branch < 0 || ops[i].branch >= LFD_MAX_BRANCHES) { delete pl; return fail(LFD_ERR_INVALID, "op %d: branch %d out of range", i, ops[i].branch); }
-        if (ops[i].branch + 1 > pl->n_branches) pl->n_branches = ops[i].branch + 1;
-        if (ops[i].wait_mask < 0 || ops[i].wait_mask >= (1 << LFD_MAX_BRANCHES)) { delete pl; return fail(LFD_ERR_INVALID, "op %d: wait_mask 0x%x out of range", i, ops[i].wait_mask); }
-        pl->ops.push_back(po);
-    }
-    size_t n_dep = 0;
-    for (auto& po : pl->ops) n_dep += (size_t)__builtin_popcount((unsigned)po.op.wait_mask);
-    for (int b = 1; b < pl->n_branches; ++b) {
-        if (cudaStreamCreateWithFlags(&pl->side[b], cudaStreamNonBlocking) != cudaSuccess ||
-            cudaEventCreateWithFlags(&pl->fork_ev[b], cudaEventDisableTiming) != cudaSuccess ||
-            cudaEventCreateWithFlags(&pl->join_ev[b], cudaEventDisableTiming) != cudaSuccess) {
-            pl->n_branches = b;  // destroy what exists
-            lfd_plan_destroy(pl);
-            return fail(LFD_ERR_CUDA, "lfd_plan_create: cannot create side streams");
-        }
-    }
-    for (size_t i = 0; i < n_dep; ++i) {
-        cudaEvent_t ev;
-        if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) {
-            lfd_plan_destroy(pl);
-            return fail(LFD_ERR_CUDA, "lfd_plan_create: cannot create dependency events");
-        }
-        pl->dep_ev.push_back(ev);
-    }
+    pl->P = P; pl->cls_channels = cls_channels; pl->conv_impl = conv_impl;
+    pl->ex.clear_off = stats_off; pl->ex.clear_bytes = stats_bytes;
+    pl->ops.resize(n_ops);
+    int rc = LFD_OK;
+    for (int i = 0; i < n_ops && !rc; ++i) rc = plan_op(ops[i], &pl->ops[i]);
+    if (!rc) rc = pl->ex.init("lfd_plan_create", n_ops, [&](int i) { return ops[i].branch; }, [&](int i) { return ops[i].wait_mask; }, kMaxInferenceGraphs);
+    if (rc) { delete pl; return rc; }
     *out = pl;
     return LFD_OK;
 }
 
 extern "C" int lfd_plan_destroy(lfd_plan* plan) {
-    if (!plan) return LFD_OK;
-    for (auto& g : plan->graphs) cudaGraphExecDestroy(g.exec);
-    for (int b = 1; b < plan->n_branches; ++b) {
-        cudaStreamDestroy(plan->side[b]);
-        cudaEventDestroy(plan->fork_ev[b]);
-        cudaEventDestroy(plan->join_ev[b]);
-    }
-    for (auto ev : plan->dep_ev) cudaEventDestroy(ev);
     delete plan;
     return LFD_OK;
 }
 
 extern "C" int lfd_plan_num_launches(const lfd_plan* plan) { return plan ? (int)plan->ops.size() : 0; }
 
-static int enqueue_all(lfd_plan* pl, const void* input, int fmt, uint8_t* ws, float* cls, float* reg, cudaStream_t st) {
-    if (pl->stats_bytes > 0) CUDA_TRY(cudaMemsetAsync(ws + pl->stats_off, 0, (size_t)pl->stats_bytes, st));
-    bool started[LFD_MAX_BRANCHES] = {false};
-    int rc = LFD_OK;
-    size_t dep = 0;
-    for (size_t i = 0; i < pl->ops.size() && !rc; ++i) {
-        const int b = pl->ops[i].op.branch;
-        cudaStream_t s = st;
-        if (b > 0) {
-            s = pl->side[b];
-            if (!started[b]) {  // fork: everything enqueued on the main stream so far precedes this branch
-                CUDA_TRY(cudaEventRecord(pl->fork_ev[b], st));
-                CUDA_TRY(cudaStreamWaitEvent(s, pl->fork_ev[b], 0));
-                started[b] = true;
-            }
-        }
-        for (int w = 0; w < LFD_MAX_BRANCHES; ++w) {   // explicit cross-branch dependencies
-            if (!((pl->ops[i].op.wait_mask >> w) & 1)) continue;
-            cudaEvent_t ev = pl->dep_ev[dep++];
-            if (w == b || (w > 0 && (w >= pl->n_branches || !started[w]))) continue;   // nothing to wait for
-            CUDA_TRY(cudaEventRecord(ev, w == 0 ? st : pl->side[w]));
-            CUDA_TRY(cudaStreamWaitEvent(s, ev, 0));
-        }
-        rc = launch_op(pl->ops[i], i, input, fmt, ws, cls, reg, pl->P, pl->cls_channels, pl->conv_impl, s);
-    }
-    for (int b = 1; b < pl->n_branches; ++b)   // join (also on error paths, so that a stream capture can be closed)
-        if (started[b]) {
-            cudaEventRecord(pl->join_ev[b], pl->side[b]);
-            cudaStreamWaitEvent(st, pl->join_ev[b], 0);
-        }
-    return rc;
-}
-
 extern "C" int lfd_plan_forward(lfd_plan* pl, const void* input, int input_format, void* workspace, float* cls_out, float* reg_out,
                                 int use_graph, lfd_stream stream) {
     if (!pl || !input || !workspace || !cls_out || !reg_out) return fail(LFD_ERR_INVALID, "lfd_plan_forward: null argument");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    if (!use_graph) return enqueue_all(pl, input, input_format, ws, cls_out, reg_out, st);
-    for (auto& g : pl->graphs)
-        if (g.input == input && g.ws == workspace && g.cls == cls_out && g.reg == reg_out && g.fmt == input_format) {
-            CUDA_TRY(cudaGraphLaunch(g.exec, st));
-            return LFD_OK;
-        }
-    // first use of this pointer tuple: one eager pass (sets function attributes outside of capture, surfaces launch
-    // errors directly and produces this call's outputs), then capture + instantiate for the following calls
-    int rc = enqueue_all(pl, input, input_format, ws, cls_out, reg_out, st);
-    if (rc) return rc;
-    if (pl->graphs.size() >= kMaxGraphs) {
-        cudaGraphExecDestroy(pl->graphs.front().exec);
-        pl->graphs.erase(pl->graphs.begin());
-    }
-    cudaStream_t cap;
-    CUDA_TRY(create_capture_stream(&cap));
-    cudaGraph_t graph = nullptr;
-    cudaError_t ce = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
-    if (ce != cudaSuccess) { cudaStreamDestroy(cap); return fail(LFD_ERR_CUDA, "cudaStreamBeginCapture: %s", cudaGetErrorString(ce)); }
-    rc = enqueue_all(pl, input, input_format, ws, cls_out, reg_out, cap);
-    ce = cudaStreamEndCapture(cap, &graph);
-    if (rc || ce != cudaSuccess) {
-        if (graph) cudaGraphDestroy(graph);
-        cudaStreamDestroy(cap);
-        return rc ? rc : fail(LFD_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(ce));
-    }
-    lfd_plan::GraphEntry e;
-    e.exec = nullptr; e.input = input; e.ws = workspace; e.cls = cls_out; e.reg = reg_out; e.fmt = input_format;
-    ce = cudaGraphInstantiate(&e.exec, graph, 0);
-    cudaGraphDestroy(graph);
-    cudaStreamDestroy(cap);
-    if (ce != cudaSuccess) return fail(LFD_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(ce));
-    pl->graphs.push_back(e);
-    return LFD_OK;
+    return pl->ex.run(input, input_format, workspace, cls_out, reg_out, use_graph, st_of(stream), [&](size_t i, cudaStream_t s) {
+        return launch_op(pl->ops[i], i, input, input_format, ws, cls_out, reg_out, pl->P, pl->cls_channels, pl->conv_impl, s);
+    });
 }
 
 extern "C" int lfd_plan_profile(lfd_plan* pl, const void* input, int input_format, void* workspace, float* cls_out, float* reg_out,
                                 float* ms_per_op, lfd_stream stream) {
     if (!pl || !input || !workspace || !cls_out || !reg_out || !ms_per_op) return fail(LFD_ERR_INVALID, "lfd_plan_profile: null argument");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    const size_t n = pl->ops.size();
-    std::vector<cudaEvent_t> ev(n + 1);
-    for (auto& e : ev) CUDA_TRY(cudaEventCreate(&e));
-    if (pl->stats_bytes > 0) CUDA_TRY(cudaMemsetAsync(ws + pl->stats_off, 0, (size_t)pl->stats_bytes, st));
-    int rc = LFD_OK;
-    CUDA_TRY(cudaEventRecord(ev[0], st));
-    for (size_t i = 0; i < n && !rc; ++i) {
-        rc = launch_op(pl->ops[i], i, input, input_format, ws, cls_out, reg_out, pl->P, pl->cls_channels, pl->conv_impl, st);
-        cudaEventRecord(ev[i + 1], st);
-    }
-    cudaError_t ce = cudaStreamSynchronize(st);
-    if (!rc && ce == cudaSuccess)
-        for (size_t i = 0; i < n; ++i) cudaEventElapsedTime(&ms_per_op[i], ev[i], ev[i + 1]);
-    for (auto& e : ev) cudaEventDestroy(e);
-    if (rc) return rc;
-    if (ce != cudaSuccess) return fail(LFD_ERR_CUDA, "lfd_plan_profile: %s", cudaGetErrorString(ce));
-    return LFD_OK;
+    return pl->ex.profile("lfd_plan_profile", ws, ms_per_op, st_of(stream), [&](size_t i, cudaStream_t s) {
+        return launch_op(pl->ops[i], i, input, input_format, ws, cls_out, reg_out, pl->P, pl->cls_channels, pl->conv_impl, s);
+    });
 }
 
 
@@ -465,7 +506,7 @@ extern "C" int lfd_run_op(const lfd_op* op, const void* input, int input_format,
     if (!op || !workspace) return fail(LFD_ERR_INVALID, "lfd_run_op: null argument");
     if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_run_op: no CUDA device (there is no CPU fallback)");
     PlannedOp po;
-    int rc = plan_op(*op, conv_impl, &po);
+    int rc = plan_op(*op, &po);
     if (rc) return rc;
     return launch_op(po, 0, input, input_format, reinterpret_cast<uint8_t*>(workspace), cls_out, reg_out, P, cls_channels, conv_impl,
                      reinterpret_cast<cudaStream_t>(stream));
@@ -707,14 +748,7 @@ struct PlannedTop {
 
 struct lfd_train_plan {
     std::vector<PlannedTop> ops;
-    int64_t workspace_bytes;
-    struct GraphEntry { cudaGraphExec_t exec; const void* input; void* ws; int fmt; };
-    std::vector<GraphEntry> graphs;
-    // side streams of the independent per-level chains (same fork / wait / join protocol as lfd_plan)
-    cudaStream_t side[LFD_MAX_BRANCHES];
-    cudaEvent_t fork_ev[LFD_MAX_BRANCHES], join_ev[LFD_MAX_BRANCHES];
-    std::vector<cudaEvent_t> dep_ev;
-    int n_branches = 1;
+    BranchExecutor ex;
 };
 
 static lfd_op conv_op_of(const lfd_top& t) {
@@ -740,7 +774,7 @@ static int plan_top(const lfd_top& t, int64_t ws_bytes, PlannedTop* out) {
             if (t.off[1] < 0 || t.off[4] < 0 || (t.kind == LFD_TOP_CONV && t.off[0] < 0)) return fail(LFD_ERR_INVALID, "training conv: missing in / out / packed-weight offset");
             lfd_op o = conv_op_of(t);
             o.weight = reinterpret_cast<const void*>(1);   // placeholder: resolved against the workspace at launch
-            return plan_op(o, t.impl, &out->conv);
+            return plan_op(o, &out->conv);
         }
         case LFD_TOP_INFER: {
             if (!t.ptr[0]) return fail(LFD_ERR_INVALID, "infer: missing op descriptor");
@@ -751,7 +785,7 @@ static int plan_top(const lfd_top& t, int64_t ws_bytes, PlannedTop* out) {
             if (t.off[1] < 0 || (o.kind == LFD_OP_CONV && t.off[0] < 0)) return fail(LFD_ERR_INVALID, "infer: missing in / out offset");
             o.in_off = t.off[0]; o.out_off = t.off[1]; o.res_off = t.off[2]; o.ds_out_off = t.off[3]; o.stats_off = -1;
             o.branch = 0; o.wait_mask = 0; o.max_ctas = t.max_ctas;
-            return plan_op(o, LFD_CONV_UMMA, &out->conv);
+            return plan_op(o, &out->conv);
         }
         case LFD_TOP_WGRAD: {
             WgradGeom g = {t.N, t.H, t.W, t.Cin, t.Ho, t.Wo, t.Cout, t.ksize, t.stride};
@@ -904,145 +938,36 @@ extern "C" int lfd_train_plan_create(const lfd_top* ops, int n_ops, int64_t work
     if (!ops || n_ops <= 0 || !out || workspace_bytes <= 0) return fail(LFD_ERR_INVALID, "lfd_train_plan_create: bad arguments");
     if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_train_plan_create: no CUDA device (there is no CPU fallback)");
     lfd_train_plan* pl = new lfd_train_plan();
-    pl->workspace_bytes = workspace_bytes;
-    size_t n_dep = 0;
-    for (int i = 0; i < n_ops; ++i) {
-        PlannedTop pt;
-        int rc = plan_top(ops[i], workspace_bytes, &pt);
-        if (rc) { delete pl; return rc; }
-        if (ops[i].branch < 0 || ops[i].branch >= LFD_MAX_BRANCHES || ops[i].wait_mask < 0 || ops[i].wait_mask >= (1 << LFD_MAX_BRANCHES)) {
-            delete pl;
-            return fail(LFD_ERR_INVALID, "training op %d: branch %d / wait_mask 0x%x out of range", i, ops[i].branch, ops[i].wait_mask);
-        }
-        if (ops[i].branch + 1 > pl->n_branches) pl->n_branches = ops[i].branch + 1;
-        n_dep += (size_t)__builtin_popcount((unsigned)ops[i].wait_mask);
-        pl->ops.push_back(pt);
-    }
-    const int nb = pl->n_branches;
-    pl->n_branches = 1;
-    for (int b = 1; b < nb; ++b) {
-        if (cudaStreamCreateWithFlags(&pl->side[b], cudaStreamNonBlocking) != cudaSuccess) { lfd_train_plan_destroy(pl); return fail(LFD_ERR_CUDA, "lfd_train_plan_create: cannot create side streams"); }
-        if (cudaEventCreateWithFlags(&pl->fork_ev[b], cudaEventDisableTiming) != cudaSuccess) { cudaStreamDestroy(pl->side[b]); lfd_train_plan_destroy(pl); return fail(LFD_ERR_CUDA, "lfd_train_plan_create: cannot create events"); }
-        if (cudaEventCreateWithFlags(&pl->join_ev[b], cudaEventDisableTiming) != cudaSuccess) { cudaStreamDestroy(pl->side[b]); cudaEventDestroy(pl->fork_ev[b]); lfd_train_plan_destroy(pl); return fail(LFD_ERR_CUDA, "lfd_train_plan_create: cannot create events"); }
-        pl->n_branches = b + 1;
-    }
-    for (size_t i = 0; i < n_dep; ++i) {
-        cudaEvent_t ev;
-        if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) { lfd_train_plan_destroy(pl); return fail(LFD_ERR_CUDA, "lfd_train_plan_create: cannot create dependency events"); }
-        pl->dep_ev.push_back(ev);
-    }
+    pl->ops.resize(n_ops);
+    int rc = LFD_OK;
+    for (int i = 0; i < n_ops && !rc; ++i) rc = plan_top(ops[i], workspace_bytes, &pl->ops[i]);
+    if (!rc) rc = pl->ex.init("lfd_train_plan_create", n_ops, [&](int i) { return ops[i].branch; }, [&](int i) { return ops[i].wait_mask; }, kMaxTrainingGraphs);
+    if (rc) { delete pl; return rc; }
     *out = pl;
     return LFD_OK;
 }
 
 extern "C" int lfd_train_plan_destroy(lfd_train_plan* plan) {
-    if (!plan) return LFD_OK;
-    for (auto& g : plan->graphs) cudaGraphExecDestroy(g.exec);
-    for (int b = 1; b < plan->n_branches; ++b) {
-        cudaStreamDestroy(plan->side[b]);
-        cudaEventDestroy(plan->fork_ev[b]);
-        cudaEventDestroy(plan->join_ev[b]);
-    }
-    for (auto ev : plan->dep_ev) cudaEventDestroy(ev);
     delete plan;
     return LFD_OK;
 }
 
 extern "C" int lfd_train_plan_num_ops(const lfd_train_plan* plan) { return plan ? (int)plan->ops.size() : 0; }
 
-static int train_enqueue(lfd_train_plan* pl, const void* input, int fmt, uint8_t* ws, cudaStream_t st) {
-    bool started[LFD_MAX_BRANCHES] = {false};
-    int rc = LFD_OK;
-    size_t dep = 0;
-    cudaError_t ce = cudaSuccess;
-    for (size_t i = 0; i < pl->ops.size() && !rc && ce == cudaSuccess; ++i) {
-        const lfd_top& t = pl->ops[i].op;
-        const int b = t.branch;
-        cudaStream_t s = st;
-        if (b > 0) {
-            s = pl->side[b];
-            if (!started[b]) {   // fork: everything enqueued on the main stream so far precedes this branch
-                if ((ce = cudaEventRecord(pl->fork_ev[b], st)) != cudaSuccess || (ce = cudaStreamWaitEvent(s, pl->fork_ev[b], 0)) != cudaSuccess) break;
-                started[b] = true;
-            }
-        }
-        for (int w = 0; w < LFD_MAX_BRANCHES && ce == cudaSuccess; ++w) {
-            if (!((t.wait_mask >> w) & 1)) continue;
-            cudaEvent_t ev = pl->dep_ev[dep++];
-            if (w == b || (w > 0 && (w >= pl->n_branches || !started[w]))) continue;
-            if ((ce = cudaEventRecord(ev, w == 0 ? st : pl->side[w])) == cudaSuccess) ce = cudaStreamWaitEvent(s, ev, 0);
-        }
-        if (ce == cudaSuccess) rc = launch_top(pl->ops[i], input, fmt, ws, s);
-    }
-    for (int b = 1; b < pl->n_branches; ++b)   // join (also on error paths, so that a stream capture can be closed)
-        if (started[b]) {
-            cudaEventRecord(pl->join_ev[b], pl->side[b]);
-            cudaStreamWaitEvent(st, pl->join_ev[b], 0);
-        }
-    if (!rc && ce != cudaSuccess) rc = fail(LFD_ERR_CUDA, "training plan stream dependencies: %s", cudaGetErrorString(ce));
-    return rc;
-}
-
 extern "C" int lfd_train_plan_run(lfd_train_plan* pl, const void* input, int input_format, void* workspace, int use_graph, lfd_stream stream) {
     if (!pl || !workspace) return fail(LFD_ERR_INVALID, "lfd_train_plan_run: null argument");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    if (!use_graph) return train_enqueue(pl, input, input_format, ws, st);
-    for (auto& g : pl->graphs)
-        if (g.input == input && g.ws == workspace && g.fmt == input_format) {
-            CUDA_TRY(cudaGraphLaunch(g.exec, st));
-            return LFD_OK;
-        }
-    int rc = train_enqueue(pl, input, input_format, ws, st);   // eager first pass (function attributes, launch errors)
-    if (rc) return rc;
-    if (pl->graphs.size() >= 8) {
-        cudaGraphExecDestroy(pl->graphs.front().exec);
-        pl->graphs.erase(pl->graphs.begin());
-    }
-    // The first eager pass already produced this call's results; the graph is captured for the FOLLOWING calls.  Capture does
-    // not execute anything, so the state (statistics, staging) is untouched.
-    cudaStream_t cap;
-    CUDA_TRY(create_capture_stream(&cap));
-    cudaGraph_t graph = nullptr;
-    cudaError_t ce = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
-    if (ce != cudaSuccess) { cudaStreamDestroy(cap); return fail(LFD_ERR_CUDA, "cudaStreamBeginCapture: %s", cudaGetErrorString(ce)); }
-    rc = train_enqueue(pl, input, input_format, ws, cap);
-    ce = cudaStreamEndCapture(cap, &graph);
-    if (rc || ce != cudaSuccess) {
-        if (graph) cudaGraphDestroy(graph);
-        cudaStreamDestroy(cap);
-        return rc ? rc : fail(LFD_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(ce));
-    }
-    lfd_train_plan::GraphEntry e;
-    e.exec = nullptr; e.input = input; e.ws = workspace; e.fmt = input_format;
-    ce = cudaGraphInstantiate(&e.exec, graph, 0);
-    cudaGraphDestroy(graph);
-    cudaStreamDestroy(cap);
-    if (ce != cudaSuccess) return fail(LFD_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(ce));
-    pl->graphs.push_back(e);
-    return LFD_OK;
+    return pl->ex.run(input, input_format, workspace, nullptr, nullptr, use_graph, st_of(stream), [&](size_t i, cudaStream_t s) {
+        return launch_top(pl->ops[i], input, input_format, ws, s);
+    });
 }
 
 extern "C" int lfd_train_plan_profile(lfd_train_plan* pl, const void* input, int input_format, void* workspace, float* ms_per_op, lfd_stream stream) {
     if (!pl || !workspace || !ms_per_op) return fail(LFD_ERR_INVALID, "lfd_train_plan_profile: null argument");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    const size_t n = pl->ops.size();
-    std::vector<cudaEvent_t> ev(n + 1);
-    for (auto& e : ev) CUDA_TRY(cudaEventCreate(&e));
-    int rc = LFD_OK;
-    CUDA_TRY(cudaEventRecord(ev[0], st));
-    for (size_t i = 0; i < n && !rc; ++i) {
-        rc = launch_top(pl->ops[i], input, input_format, ws, st);
-        cudaEventRecord(ev[i + 1], st);
-    }
-    cudaError_t ce = cudaStreamSynchronize(st);
-    if (!rc && ce == cudaSuccess)
-        for (size_t i = 0; i < n; ++i) cudaEventElapsedTime(&ms_per_op[i], ev[i], ev[i + 1]);
-    for (auto& e : ev) cudaEventDestroy(e);
-    if (rc) return rc;
-    if (ce != cudaSuccess) return fail(LFD_ERR_CUDA, "lfd_train_plan_profile: %s", cudaGetErrorString(ce));
-    return LFD_OK;
+    return pl->ex.profile("lfd_train_plan_profile", ws, ms_per_op, st_of(stream), [&](size_t i, cudaStream_t s) {
+        return launch_top(pl->ops[i], input, input_format, ws, s);
+    });
 }
 
 extern "C" int lfd_run_top(const lfd_top* op, const void* input, int input_format, void* workspace, lfd_stream stream) {

@@ -17,6 +17,7 @@ Rounding points of the bf16 pipeline (mirrored by oracle/lfd_oracle.py forward(e
 """
 import ctypes as C
 import os
+import time
 
 import torch
 import torch.nn as nn
@@ -26,8 +27,64 @@ from . import _native as nat
 BN_TYPES = (nn.BatchNorm2d,)
 
 
-def _conv_out(size, k, s):
+def conv_out(size, k, s):
     return (size + 2 * (k // 2) - k) // s + 1
+
+
+def level_geometry(backbone, head, h, w):
+    """Sizes of the head levels for a stem output of h x w (every stage starts with a stride-2 block) -> (level_sizes, P, offset of
+    each level's first point)."""
+    taps = list(backbone._out_indices)
+    if len(taps) != head._num_heads:
+        raise ValueError('backbone taps (%d) and head levels (%d) differ' % (len(taps), head._num_heads))
+    sizes = {}
+    for si, stage in enumerate(backbone.stages()):
+        h, w = conv_out(h, 3, 2), conv_out(w, 3, 2)
+        for bi in range(len(stage)):
+            if (si, bi) in taps:
+                sizes[(si, bi)] = (h, w)
+    level_sizes = [sizes[t] for t in taps]
+    offs, acc = [], 0
+    for fh, fw in level_sizes:
+        offs.append(acc)
+        acc += fh * fw
+    return level_sizes, acc, offs
+
+
+def check_input(x, N, H, W, contiguous):
+    """x: float32 [N,3,H,W] or uint8 [N,H,W,3] on a CUDA device -> its nat.INPUT_* format."""
+    if x.dtype == torch.float32:
+        fmt, ok = nat.INPUT_F32_NCHW, tuple(x.shape) == (N, 3, H, W)
+    elif x.dtype == torch.uint8:
+        fmt, ok = nat.INPUT_U8_NHWC, tuple(x.shape) == (N, H, W, 3)
+    else:
+        raise TypeError('input must be float32 NCHW or uint8 NHWC, got %s' % (x.dtype,))
+    if not ok or not x.is_cuda or (contiguous and not x.is_contiguous()):
+        raise ValueError('input must be a%s CUDA tensor matching the plan shape N=%d H=%d W=%d (got %s)'
+                         % (' contiguous' if contiguous else '', N, H, W, tuple(x.shape)))
+    return fmt
+
+
+def tune_branch_bounds(work, measure, candidates, budget_s, max_branches=None):
+    """Coordinate descent over per-branch bounds on the persistent CTAs of side-branch kernels.  work: {branch: amount of work};
+    measure(caps) -> time of the plan with caps = {branch: bound} (0 = unbounded).  The branches with the most work come first (at most
+    max_branches of them); each candidate bound is tried on top of the best caps so far and kept only when it is measurably faster
+    (below 0.995x the best time).  No trial starts after budget_s seconds.  -> (caps, [(label, time), ...])."""
+    t_end = time.time() + budget_s
+    caps = {b: 0 for b in work}
+    best = measure(caps)
+    log = [('all SMs', best)]
+    for b in sorted(work, key=lambda k: -work[k])[:max_branches]:
+        for c in candidates:
+            if time.time() > t_end:
+                break
+            trial = dict(caps)
+            trial[b] = c
+            t = measure(trial)
+            log.append(('branch %d <= %d CTAs' % (b, c), t))
+            if t < best * 0.995:
+                best, caps = t, trial
+    return caps, log
 
 
 ACT_DTYPES = {'bf16': (torch.bfloat16, nat.DTYPE_BF16), 'fp16': (torch.float16, nat.DTYPE_FP16)}
@@ -93,6 +150,23 @@ class _Arena(object):
             else:
                 merged.append((o, s))
         self.free = merged
+
+
+def place_tensors(ops, sizes, arenas, hold=(), skip=()):
+    """Liveness placement: a tensor an op writes ('out', 'out2') is allocated in the arena of the op's branch when the op runs and
+    released after the last op that reads it ('inp', 'res').  Tensors in `hold` are never released, tensors in `skip` are placed
+    elsewhere by the caller.  -> {name: offset inside its arena}"""
+    last = {op[k]: i for i, op in enumerate(ops) for k in ('inp', 'res') if op.get(k) is not None and op[k] not in skip}
+    placed = {}                                  # name -> (arena, offset)
+    for i, op in enumerate(ops):
+        arena = arenas[op.get('branch', 0)]
+        for k in ('out', 'out2'):
+            if op.get(k) is not None and op[k] not in skip:
+                placed[op[k]] = (arena, arena.alloc(sizes[op[k]]))
+        for name, lu in last.items():
+            if lu == i and name not in hold:
+                placed[name][0].release(placed[name][1], sizes[name])
+    return {name: off for name, (_, off) in placed.items()}
 
 
 class InferencePlan(object):
@@ -196,7 +270,7 @@ class InferencePlan(object):
     def _emit_stem0(self, conv, norm, relu, out_name, h, w, tail=None):
         if conv.in_channels != 3 or conv.kernel_size != (3, 3) or conv.stride != (2, 2):
             raise NotImplementedError('the H100 stem kernel handles the 3x3/s2 conv on a 3-channel image only')
-        ho, wo = _conv_out(h, 3, 2), _conv_out(w, 3, 2)
+        ho, wo = conv_out(h, 3, 2), conv_out(w, 3, 2)
         scale, shift = self._fold(conv, norm)
         wt = pack_stem_weight(fold_scale(conv.weight, scale), self.tdtype)
         op = dict(kind=nat.OP_STEM0, H=h, W=w, Cin=3, Ho=ho, Wo=wo, Cout=conv.out_channels, ksize=3, stride=2, relu=int(relu),
@@ -229,13 +303,13 @@ class InferencePlan(object):
             return False
         if self.fuse_stem:
             return True
-        stem1_bytes = self.N * _conv_out(self.H, 3, 2) * _conv_out(self.W, 3, 2) * 64 * 2
+        stem1_bytes = self.N * conv_out(self.H, 3, 2) * conv_out(self.W, 3, 2) * 64 * 2
         return stem1_bytes > self._l2_bytes() // 2
 
     def _emit_stem4(self, layers, out_name, h, w):
         (c0, n0, r0), tail1, (c2, n2, r2), (c3, n3, r3) = layers
-        h1, w1 = _conv_out(h, 3, 2), _conv_out(w, 3, 2)
-        ho, wo = _conv_out(h1, 3, 2), _conv_out(w1, 3, 2)
+        h1, w1 = conv_out(h, 3, 2), conv_out(w, 3, 2)
+        ho, wo = conv_out(h1, 3, 2), conv_out(w1, 3, 2)
         s0, b0 = self._fold(c0, n0)
         s2, b2 = self._fold(c2, n2)
         s3, b3 = self._fold(c3, n3)
@@ -256,7 +330,7 @@ class InferencePlan(object):
                 or conv.groups != 1 or conv.dilation != (1, 1):
             raise NotImplementedError('unsupported conv geometry for the H100 kernels: %r' % (conv,))
         cin, cout = conv.in_channels, conv.out_channels
-        ho, wo = _conv_out(h, k, s), _conv_out(w, k, s)
+        ho, wo = conv_out(h, k, s), conv_out(w, k, s)
         q = nat.conv_query(self.N, h, w, cin, ho, wo, cout, k, s, tail[0].out_channels if tail is not None else 0,
                            shortcut[0].out_channels if shortcut is not None else 0)
         cc = q['cc']
@@ -348,25 +422,11 @@ class InferencePlan(object):
     def _build(self, model):
         bb, neck, head = model._backbone, model._neck, model._head
         cur, h, w = self._emit_stem(bb.stem_layers(), self.H, self.W)
+        self.level_sizes, self.P, offs = level_geometry(bb, head, h, w)
         taps = list(bb._out_indices)
-        if len(taps) != head._num_heads:
-            raise ValueError('backbone taps (%d) and head levels (%d) differ' % (len(taps), head._num_heads))
         if make_norm_probe(head) is not None and not isinstance(make_norm_probe(head), nn.GroupNorm):
             raise NotImplementedError('the H100 head kernels implement GroupNorm towers and towers without norm layers (the shipped configs)')
-        # point offsets need every level size up front: strides are fixed by the stage index
-        sizes, hh, ww = {}, h, w
-        for si, stage in enumerate(bb.stages()):
-            hh, ww = _conv_out(hh, 3, 2), _conv_out(ww, 3, 2)
-            for bi in range(len(stage)):
-                if (si, bi) in taps:
-                    sizes[(si, bi)] = (hh, ww)
-        self.level_sizes = [sizes[t] for t in taps]
-        self.P = sum(fh * fw for (fh, fw) in self.level_sizes)
         self.cls_channels = head.num_cls_channels
-        offs, acc = [], 0
-        for (fh, fw) in self.level_sizes:
-            offs.append(acc)
-            acc += fh * fw
         cache = {}
         for si, stage in enumerate(bb.stages()):
             for bi, block in enumerate(stage):
@@ -475,33 +535,17 @@ class InferencePlan(object):
         self.stats_bytes = (n_stats * stats_each + 255) & ~255
         producer = {op['out']: op['branch'] for op in self._ops if op.get('out') is not None}
         producer.update({op['out2']: op['branch'] for op in self._ops if op.get('out2') is not None})
-        last_use, shared = {}, set()
-        for i, op in enumerate(self._ops):
-            for k in ('inp', 'res'):
-                if op.get(k) is not None:
-                    last_use[op[k]] = i
-                    if producer[op[k]] != op['branch']:
-                        shared.add(op[k])      # read by another branch (a backbone tap): lives for the whole forward
-        n_br = 1 + max(op['branch'] for op in self._ops)
-        arenas = [_Arena(base=0) for _ in range(n_br)]
-        local = {}                              # name -> (branch, offset inside the branch's arena)
-        no_reuse = bool(os.environ.get('LFD_B200_NO_REUSE'))
-        for i, op in enumerate(self._ops):
-            for key in ('out', 'out2'):
-                if op.get(key) is not None:
-                    local[op[key]] = (op['branch'], arenas[op['branch']].alloc(self._tensors[op[key]]))
-            for name, lu in list(last_use.items()):
-                if lu == i:
-                    del last_use[name]
-                    if not no_reuse and name not in shared:
-                        arenas[local[name][0]].release(local[name][1], self._tensors[name])
+        # a tensor read by another branch (a backbone tap) lives for the whole forward
+        shared = {op[k] for op in self._ops for k in ('inp', 'res') if op.get(k) is not None and producer[op[k]] != op['branch']}
+        arenas = [_Arena() for _ in range(1 + max(op['branch'] for op in self._ops))]
+        local = place_tensors(self._ops, self._tensors, arenas, hold=set(self._tensors) if os.environ.get('LFD_B200_NO_REUSE') else shared)
         bases, top = [], self.stats_bytes
         for a in arenas:
             bases.append(top)
             top += (a.top + 255) & ~255
-        offsets = {name: bases[b] + off for name, (b, off) in local.items()}
+        offsets = {name: bases[producer[name]] + off for name, off in local.items()}
         self.workspace_bytes = max(top, 256)
-        self.tensor_branch = {name: b for name, (b, _) in local.items()}
+        self.tensor_branch = {name: producer[name] for name in local}
         self.shared_tensors = shared
         self.workspace = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=dev)
         self.activation_bytes = sum(self._tensors.values())
@@ -575,7 +619,6 @@ class InferencePlan(object):
         stages (the critical path of the step); when their persistent CTAs hold all SMs, every small layer queues behind a whole
         side-branch layer.  Coordinate descent over the branches (largest first), keeping a bound only when it is measurably faster.
         Results do not depend on the bound (tiles are independent).  Returns {branch: bound} (0 = unbounded)."""
-        import time
         if self.handle is None:
             raise nat.LfdError('this plan was built for host-side inspection only (create_native=False)')
         if x is None:
@@ -610,24 +653,11 @@ class InferencePlan(object):
                 self.handle = saved
                 lib.lfd_plan_destroy(h)
 
-        t_end = time.time() + budget_s
         work = {}
         for op in self._ops:
             if op['kind'] == nat.OP_CONV and op.get('branch', 0) > 0:
                 work[op['branch']] = work.get(op['branch'], 0) + self.N * op['Ho'] * op['Wo'] * (op['Cin'] + op['Cout'])
-        caps = {b: 0 for b in work}
-        base = measure(caps)
-        log = [('all SMs', base)]
-        for b in sorted(work, key=lambda k: -work[k]):
-            for c in candidates:
-                if time.time() > t_end:
-                    break
-                trial = dict(caps)
-                trial[b] = c
-                t = measure(trial)
-                log.append(('branch %d <= %d CTAs' % (b, c), t))
-                if t < base * 0.995:
-                    base, caps = t, trial
+        caps, log = tune_branch_bounds(work, measure, candidates, budget_s)
         self.apply_side_ctas(caps)
         self.autotune_log = log
         return caps
@@ -648,17 +678,9 @@ class InferencePlan(object):
     def forward(self, x, use_graph=True, slot=0):
         """x: cuda float32 [N,3,H,W] (contiguous) or uint8 [N,H,W,3].  Returns the plan-owned (cls, reg) buffers of output
         `slot` (a second slot lets the post-process of one batch overlap the forward of the next, lfd/pipeline.py)."""
-        if x.dtype == torch.float32:
-            fmt, ok = nat.INPUT_F32_NCHW, tuple(x.shape) == (self.N, 3, self.H, self.W)
-        elif x.dtype == torch.uint8:
-            fmt, ok = nat.INPUT_U8_NHWC, tuple(x.shape) == (self.N, self.H, self.W, 3)
-        else:
-            raise TypeError('input must be float32 NCHW or uint8 NHWC, got %s' % (x.dtype,))
         if self.handle is None:
             raise nat.LfdError('this plan was built for host-side inspection only (create_native=False)')
-        if not ok or not x.is_cuda or not x.is_contiguous():
-            raise ValueError('input must be a contiguous CUDA tensor matching the plan shape N=%d H=%d W=%d (got %s)'
-                             % (self.N, self.H, self.W, tuple(x.shape)))
+        fmt = check_input(x, self.N, self.H, self.W, contiguous=True)
         cls_out, reg_out = self.outputs(slot)
         with torch.cuda.device(self.device):
             nat.check(nat.lib().lfd_plan_forward(self.handle, nat.ptr(x), fmt, nat.ptr(self.workspace), nat.ptr(cls_out),

@@ -20,19 +20,16 @@ Rounding points (bf16 training): conv output z (fp32 accumulate) -> bf16; BatchN
 normalised + residual + ReLU output -> bf16; every activation gradient -> bf16; weight / norm-parameter gradients fp32.
 """
 import os
+import time
 import ctypes as C
 
 import torch
 import torch.nn as nn
 
 from . import _native as nat
-from ._engine import PrefixEmitter, _Arena
+from ._engine import PrefixEmitter, _Arena, check_input, conv_out, level_geometry, place_tensors, tune_branch_bounds
 
 __all__ = ['FlatParameters', 'TrainPlan', 'train_forward']
-
-
-def _conv_out(size, k, s):
-    return (size + 2 * (k // 2) - k) // s + 1
 
 
 class FlatParameters(object):
@@ -203,7 +200,7 @@ class TrainPlan(object):
         if conv.bias is not None or not isinstance(norm, nn.BatchNorm2d):
             raise NotImplementedError('native training implements conv(bias=False) + BatchNorm2d for backbone / neck layers')
         cin, cout = conv.in_channels, conv.out_channels
-        ho, wo = _conv_out(h, k, s), _conv_out(w, k, s)
+        ho, wo = conv_out(h, k, s), conv_out(w, k, s)
         z, y = self._act(name + '_z', ho, wo, cout), self._act(name, ho, wo, cout)
         sums = self._alloc(name + '_sums', cout * 16)
         self._zero_fwd.append(sums)
@@ -380,22 +377,9 @@ class TrainPlan(object):
         else:
             for i, (conv, norm, relu) in enumerate(bb.stem_layers()):
                 cur, h, w = self._conv_bn('stem%d' % i, conv, norm, relu, cur, h, w)
-        taps = list(bb._out_indices)
-        if len(taps) != head._num_heads:
-            raise ValueError('backbone taps (%d) and head levels (%d) differ' % (len(taps), head._num_heads))
-        sizes, hh, ww = {}, h, w
-        for si, stage in enumerate(bb.stages()):
-            hh, ww = _conv_out(hh, 3, 2), _conv_out(ww, 3, 2)
-            for bi in range(len(stage)):
-                if (si, bi) in taps:
-                    sizes[(si, bi)] = (hh, ww)
-        self.level_sizes = [sizes[t] for t in taps]
-        self.P = sum(fh * fw for fh, fw in self.level_sizes)
+        self.level_sizes, self.P, offs = level_geometry(bb, head, h, w)
         self.cls_channels = head.num_cls_channels
-        offs, acc = [], 0
-        for fh, fw in self.level_sizes:
-            offs.append(acc)
-            acc += fh * fw
+        taps = list(bb._out_indices)
         ui = 0
         for si, stage in enumerate(bb.stages()):
             for bi, block in enumerate(stage):
@@ -636,15 +620,8 @@ class TrainPlan(object):
         self.prefix_outputs = {n: shapes[n] for n in keep}          # name -> (h, w, channels), bf16 NHWC
         for n in sorted(keep):
             self._alloc(n, pre._tensors[n])
-        last = {op[k]: i for i, op in enumerate(ops) for k in ('inp', 'res') if op.get(k) is not None and op[k] not in keep}
-        arena, local = _Arena(), {}
-        for i, op in enumerate(ops):
-            for k in ('out', 'out2'):
-                if op.get(k) is not None and op[k] not in keep:
-                    local[op[k]] = arena.alloc(pre._tensors[op[k]])
-            for n, lu in last.items():
-                if lu == i:
-                    arena.release(local[n], pre._tensors[n])
+        arena = _Arena()
+        local = place_tensors(ops, pre._tensors, [arena], skip=keep)       # (every prefix op is on the main stream)
         if local:
             self._alloc('prefix_scratch', arena.top)
         self._prefix['scratch'] = local
@@ -781,14 +758,7 @@ class TrainPlan(object):
 
     # ------------------------------------------------------------------ execution
     def forward(self, x, use_graph=False):
-        if x.dtype == torch.float32:
-            fmt, ok = nat.INPUT_F32_NCHW, tuple(x.shape) == (self.N, 3, self.H, self.W)
-        elif x.dtype == torch.uint8:
-            fmt, ok = nat.INPUT_U8_NHWC, tuple(x.shape) == (self.N, self.H, self.W, 3)
-        else:
-            raise TypeError('input must be float32 NCHW or uint8 NHWC, got %s' % (x.dtype,))
-        if not ok or not x.is_cuda:
-            raise ValueError('input must be a CUDA tensor matching the plan shape N=%d H=%d W=%d (got %s)' % (self.N, self.H, self.W, tuple(x.shape)))
+        fmt = check_input(x, self.N, self.H, self.W, contiguous=False)
         # the backward reads the image again (stem weight gradient): keep it in a plan-owned buffer with a fixed address
         if self._input is None or self._input.dtype != x.dtype:
             self._input = torch.empty_like(x, memory_format=torch.contiguous_format)
@@ -814,7 +784,6 @@ class TrainPlan(object):
         """As InferencePlan.autotune: bounds on the persistent CTAs of the side-branch (per-level chain) convs / data-gradient convs /
         weight-gradient kernels, picked per branch by timing the replayed forward and backward graphs.  Model state touched by the timing
         runs (BatchNorm running statistics, the flat gradient buffer, the plan's outputs) is saved and restored."""
-        import time
         if not self.create_native or not self.branches:
             return {}
         dev, lib = self.device, nat.lib()
@@ -862,19 +831,7 @@ class TrainPlan(object):
                 for op in ops:
                     if op['kind'] in tuned and op.get('branch', 0) > 0:
                         work[op['branch']] = work.get(op['branch'], 0) + op['N'] * op['Ho'] * op['Wo'] * (op['Cin'] + op['Cout'])
-                caps = {b: 0 for b in work}
-                base = measure(caps)
-                log = [('all SMs', base)]
-                for b in sorted(work, key=lambda k: -work[k])[:3]:
-                    for c in candidates:
-                        if time.time() > t_end:
-                            break
-                        trial = dict(caps)
-                        trial[b] = c
-                        t = measure(trial)
-                        log.append(('branch %d <= %d CTAs' % (b, c), t))
-                        if t < base * 0.995:
-                            base, caps = t, trial
+                caps, log = tune_branch_bounds(work, measure, candidates, t_end - time.time(), max_branches=3)     # (fwd and bwd share the budget)
                 set_caps(caps)
                 name = which + '_handle'
                 old = getattr(self, name)

@@ -190,54 +190,16 @@ def test_training_plan_branches_order_every_conflict(name):
     read / write / accumulate role of each operand.  Replay the fork / wait protocol of lfd_train_plan_run with vector clocks and check
     that every pair of ops that conflict on a workspace tensor (write vs anything, accumulate vs read) is ordered."""
     from lfd._train import TrainPlan
+    from plan_order import check_every_conflict_ordered
     model, _ = synth_model(name)
     model.train()
     plan = TrainPlan(model, 2, 128, 160, torch.device('cpu'), create_native=False)
     assert plan.branches
-    for ops in (plan.fwd_ops, plan.bwd_ops):
+    for which, ops in (('fwd', plan.fwd_ops), ('bwd', plan.bwd_ops)):
         branches = sorted({op.get('branch', 0) for op in ops})
         assert branches[0] == 0 and len(branches) == 1 + len(plan.level_sizes) and branches[-1] < nat.MAX_BRANCHES
-        clock, last, seq, info = [], {}, {}, []
-        for i, op in enumerate(ops):
-            b = op.get('branch', 0)
-            if b in last:
-                vc = dict(clock[last[b]])
-            else:
-                vc = dict(clock[last[0]]) if 0 in last else {}       # fork after the preceding main-stream op
-            for w in range(nat.MAX_BRANCHES):
-                if (op['wait_mask'] >> w) & 1 and w in last:
-                    for k, v in clock[last[w]].items():
-                        vc[k] = max(vc.get(k, -1), v)
-            seq[b] = seq.get(b, -1) + 1
-            vc[b] = seq[b]
-            clock.append(vc)
-            last[b] = i
-            roles = TrainPlan._ROLES.get(op['kind'])
-            acc = {}
-            if roles is not None:
-                for j, nm in op.get('off', {}).items():
-                    if nm is not None:
-                        acc.setdefault(nm, set()).add(roles[j])
-            info.append((b, seq[b], acc, roles is None))
-        by_name = {}
-        n_pairs = 0
-        for j, (bj, sj, accj, barrier) in enumerate(info):
-            if barrier:                                              # PACK / ZERO / UNPACK: ordered against everything before
-                for i in range(j):
-                    bi, si = info[i][0], info[i][1]
-                    assert clock[j].get(bi, -1) >= si, (name, 'barrier', i, j)
-                continue
-            for nm, rj in accj.items():
-                for (i, ri) in by_name.get(nm, []):
-                    bi, si = info[i][0], info[i][1]
-                    if bi == bj:
-                        continue
-                    conflict = 'W' in ri or 'W' in rj or (('A' in ri) != ('A' in rj)) or (('A' in ri) and ('R' in ri or 'R' in rj))
-                    if conflict:
-                        n_pairs += 1
-                        assert clock[j].get(bi, -1) >= si, (name, nm, i, j, ops[i]['kind'], ops[j]['kind'])
-                by_name.setdefault(nm, []).append((j, rj))
-        if ops is plan.bwd_ops:
+        n_pairs = check_every_conflict_ordered(ops, (name, which))
+        if which == 'bwd':
             assert n_pairs >= len(plan.level_sizes)                  # at least the taps' gradients: level chain writes, backbone accumulates
     # the backward starts every level chain before the backbone
     first_main = next(i for i, op in enumerate(plan.bwd_ops) if op.get('branch', 0) == 0 and op['kind'] not in (nat.TOP_ZERO,))
@@ -261,3 +223,31 @@ def test_side_branch_cta_bounds_touch_only_side_branch_ops():
     assert seen == {nat.OP_CONV, nat.OP_GN_APPLY, nat.OP_HEAD_FINAL}
     plan._set_side_ctas({})
     assert all(o.max_ctas == 0 for o in plan._op_array)
+
+
+def test_tune_branch_bounds_descent(monkeypatch):
+    """The coordinate descent behind InferencePlan.autotune / TrainPlan.autotune, on a table of times and a fake clock (one second per
+    measurement): branches in decreasing work, a bound kept only below 0.995x the best time so far, at most max_branches branches, no
+    trial after the budget, and the log starts with the unbounded time."""
+    import types
+    import lfd._engine as eng
+    clock = [0.0]
+    monkeypatch.setattr(eng, 'time', types.SimpleNamespace(time=lambda: clock[0]))
+    # kept: 99.0 < 0.995 x 100, 97.0, 90.0; marginal gains below 0.995x the best are dropped: 98.7 vs 99.0, 89.8 vs 90.0
+    table = {(): 100.0, ((2, 64),): 99.0, ((2, 32),): 98.7, ((2, 64), (3, 64)): 97.0, ((2, 64), (3, 32)): 90.0,
+             ((1, 64), (2, 64), (3, 32)): 95.0, ((1, 32), (2, 64), (3, 32)): 89.8}
+
+    def measure(caps):
+        clock[0] += 1.0
+        return table.get(tuple(sorted((b, c) for b, c in caps.items() if c)), 1000.0)
+
+    work = {1: 10, 2: 30, 3: 20}
+    caps, log = eng.tune_branch_bounds(work, measure, (64, 32), 100.0)
+    assert caps == {1: 0, 2: 64, 3: 32} and log[0] == ('all SMs', 100.0)
+    assert log[1:] == [('branch %d <= %d CTAs' % (b, c), t) for b, c, t in [(2, 64, 99.0), (2, 32, 98.7), (3, 64, 97.0), (3, 32, 90.0),
+                                                                            (1, 64, 95.0), (1, 32, 89.8)]]
+    caps, log = eng.tune_branch_bounds(work, measure, (64, 32), 100.0, max_branches=2)
+    assert caps == {1: 0, 2: 64, 3: 32} and len(log) == 5 and not any(l.startswith('branch 1 ') for l, _ in log)
+    clock[0] = 0.0
+    caps, log = eng.tune_branch_bounds(work, measure, (64, 32), 2.5)       # trials start at t = 1 and 2 only
+    assert caps == {1: 0, 2: 64, 3: 0} and [l for l, _ in log] == ['all SMs', 'branch 2 <= 64 CTAs', 'branch 2 <= 32 CTAs']
