@@ -15,6 +15,8 @@
  *   lfd_postprocess                LFD._get_results_for_single_image   lfd/model/lfd.py:434-509, predict path :577-641,
  *                                  multiclass_nms / batched_nms        lfd/model/utils/nms.py:119-220
  *   lfd_multiclass_nms             multiclass_nms / batched_nms        lfd/model/utils/nms.py:119-220 (on explicit boxes)
+ *   lfd_postprocess_soft_nms,      soft_nms, nms_cfg type 'soft_nms'   lfd/model/utils/nms.py:62-158,
+ *   lfd_multiclass_soft_nms                                            build/nms/src/cpu/nms_cpu.cpp:76-217
  *   lfd_nms                        nms_ext.nms                         lfd/model/utils/build/nms/src/nms_ext.cpp:18-29,
  *                                                                      cpu/nms_cpu.cpp:8-75, cuda/nms_kernel.cu:71-138
  *   lfd_sigmoid_focal_loss_forward sigmoid_focal_loss_ext.forward      lfd/model/losses/build/sigmoid_focal_loss/src/sigmoid_focal_loss_ext.cpp:19-34
@@ -199,6 +201,25 @@ size_t lfd_multiclass_nms_workspace_bytes(int cap);
 int lfd_multiclass_nms(const float* boxes, int box_per_class, const float* scores, int score_stride, const int32_t* labels_in, int n, int C,
                        float score_thr, float iou_thr, int class_agnostic, int cap, void* workspace, float* dets, int32_t* labels, int32_t* src,
                        int32_t* count, int32_t* overflow, lfd_stream stream);
+
+/* Soft-NMS (soft_nms of lfd/model/utils/nms.py:62-116, nms_cfg type 'soft_nms' in batched_nms / multiclass_nms :119-220) in place of the
+ * greedy NMS of lfd_postprocess / lfd_multiclass_nms: the same arguments and candidates, plus
+ *   method    LFD_SOFT_NMS_LINEAR (score *= 1 - iou when iou > cfg->iou_thr / iou_thr) or LFD_SOFT_NMS_GAUSSIAN (score *= exp(-iou^2 / sigma));
+ *             any other value fails with LFD_ERR_INVALID
+ *   min_score a reweighted candidate whose score is < min_score is dropped (the selected one never is).
+ * One CTA per image runs the reference's loop (nms_cpu.cpp:76-206) over all classes in one array, starting from the candidates in source
+ * order (src ascending); the class offsets are those of the greedy path.  Outputs as there, except: rows in selection order and d[4] = the
+ * decayed score at selection.  Linear mode is bit-exact with the reference; gaussian mode rounds exp(double) to fp32.
+ * Up to 8192 candidates per image live in shared memory, more in the workspace.  No allocation, no host synchronisation. */
+enum { LFD_SOFT_NMS_LINEAR = 1, LFD_SOFT_NMS_GAUSSIAN = 2 };
+size_t lfd_postprocess_soft_nms_workspace_bytes(const lfd_post_cfg* cfg);
+int lfd_postprocess_soft_nms(const lfd_post_cfg* cfg, const float* cls, const float* reg, const float* img_w, const float* img_h,
+                             const float* resize_scale, void* workspace, float* dets, int32_t* labels, int32_t* src, int32_t* count,
+                             int32_t* overflow, int method, float sigma, float min_score, lfd_stream stream);
+size_t lfd_multiclass_soft_nms_workspace_bytes(int cap);
+int lfd_multiclass_soft_nms(const float* boxes, int box_per_class, const float* scores, int score_stride, const int32_t* labels_in, int n, int C,
+                            float score_thr, float iou_thr, int class_agnostic, int cap, void* workspace, float* dets, int32_t* labels, int32_t* src,
+                            int32_t* count, int32_t* overflow, int method, float sigma, float min_score, lfd_stream stream);
 
 size_t lfd_nms_workspace_bytes(int n);
 /* dets device float[n][5]; keep device int64[n] (first *n_keep valid, score-descending); n_keep device int32[1]. */

@@ -32,6 +32,9 @@ def _stale():
 
 # conv_umma_kernel<MODE_3X3S2, 128>: the only instantiation with two 128-column accumulators (conv + fused shortcut); it spills part of them
 _STACK_EXEMPT = {'_ZN3lfd16conv_umma_kernelILi2ELi128ELb0EEEvNS_14UmmaConvParamsE': 512, '_ZN3lfd16conv_umma_kernelILi2ELi128ELb1EEEvNS_14UmmaConvParamsE': 512}
+# kernels whose per-thread state must stay in registers (the soft-NMS kernel runs one iteration per candidate: a spill is paid K times)
+_STACK_GUARDED = ('conv_umma_kernel', 'stem4_kernel', 'soft_nms_kernel')
+_PTXAS_VERBOSE = ('conv_umma.cu', 'postprocess.cu')
 
 
 def _check_stack_frames(ptxas_log, limit=64):
@@ -44,7 +47,7 @@ def _check_stack_frames(ptxas_log, limit=64):
         if m:
             name = m.group(1)
         m = re.search(r'(\d+) bytes stack frame', line)
-        if m and name and ('conv_umma_kernel' in name or 'stem4_kernel' in name) and int(m.group(1)) > _STACK_EXEMPT.get(name, limit):
+        if m and name and any(k in name for k in _STACK_GUARDED) and int(m.group(1)) > _STACK_EXEMPT.get(name, limit):
             raise RuntimeError('%s has a %s-byte stack frame (limit %d): registers went to local memory' % (name, m.group(1), _STACK_EXEMPT.get(name, limit)))
         # ptxas warning C7520: it could not prove the wgmma pipeline safe and serialised every wgmma of the kernel
         if 'C7520' in line and 'stem4_kernel' in line:
@@ -58,15 +61,15 @@ def build(force=False, verbose=False):
     procs = []
     for s in SOURCES:
         o = os.path.join(CSRC, s.replace('.cu', '.o')) if not os.environ.get('LFD_B200_OUT') else os.path.join('/tmp', os.path.basename(OUT) + '.' + s.replace('.cu', '.o'))
-        # conv_umma.cu is always compiled with ptxas -v: see _check_stack_frames
-        cmd = [NVCC] + FLAGS + (['-Xptxas', '-v'] if (verbose or s == 'conv_umma.cu') else []) + ['-c', os.path.join(CSRC, s), '-o', o]
+        # conv_umma.cu and postprocess.cu are always compiled with ptxas -v: see _check_stack_frames
+        cmd = [NVCC] + FLAGS + (['-Xptxas', '-v'] if (verbose or s in _PTXAS_VERBOSE) else []) + ['-c', os.path.join(CSRC, s), '-o', o]
         procs.append((s, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)))
         objs.append(o)
     for s, p in procs:
         out = p.communicate()[0].decode()
         if p.returncode != 0:
             raise RuntimeError('nvcc failed on %s:\n%s' % (s, out))
-        if s == 'conv_umma.cu':
+        if s in _PTXAS_VERBOSE:
             _check_stack_frames(out)
             if not verbose:
                 out = '\n'.join(l for l in out.splitlines() if 'ptxas info' not in l and 'bytes stack frame' not in l)

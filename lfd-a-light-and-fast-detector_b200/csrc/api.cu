@@ -543,13 +543,14 @@ extern "C" size_t lfd_postprocess_workspace_bytes(const lfd_post_cfg* cfg) {
     return post_layout(cfg->N, cfg->cap).total;
 }
 
-extern "C" int lfd_postprocess(const lfd_post_cfg* c, const float* cls, const float* reg, const float* img_w, const float* img_h,
-                               const float* resize_scale, void* workspace, float* dets, int32_t* labels, int32_t* src, int32_t* count,
-                               int32_t* overflow, lfd_stream stream) {
+// soft == nullptr: greedy NMS (lfd_postprocess); else Soft-NMS with soft->method / sigma / min_score (lfd_postprocess_soft_nms)
+static int postprocess_impl(const char* fn, const lfd_post_cfg* c, const float* cls, const float* reg, const float* img_w, const float* img_h,
+                            const float* resize_scale, void* workspace, float* dets, int32_t* labels, int32_t* src, int32_t* count,
+                            int32_t* overflow, const SoftNmsParams* soft, lfd_stream stream) {
     if (!c || !cls || !reg || !img_w || !img_h || !resize_scale || !workspace || !dets || !labels || !src || !count || !overflow)
-        return fail(LFD_ERR_INVALID, "lfd_postprocess: null argument");
-    if (c->num_levels < 1 || c->num_levels > LFD_MAX_LEVELS || c->C < 1 || c->cap < 1) return fail(LFD_ERR_INVALID, "lfd_postprocess: bad config");
-    if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_postprocess: no CUDA device (there is no CPU fallback)");
+        return fail(LFD_ERR_INVALID, "%s: null argument", fn);
+    if (c->num_levels < 1 || c->num_levels > LFD_MAX_LEVELS || c->C < 1 || c->cap < 1) return fail(LFD_ERR_INVALID, "%s: bad config", fn);
+    if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "%s: no CUDA device (there is no CPU fallback)", fn);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
     const PostLayout L = post_layout(c->N, c->cap);
@@ -571,19 +572,50 @@ extern "C" int lfd_postprocess(const lfd_post_cfg* c, const float* cls, const fl
     q.scratch = ws + L.scratch; q.scratch_stride = L.scratch_stride; q.cap = c->cap; q.cap_pow2 = L.cap_pow2; q.C = c->C;
     q.class_agnostic = c->class_agnostic; q.iou_thr = c->iou_thr;
     q.out_dets = dets; q.out_label = labels; q.out_src = src; q.out_count = count; q.overflow = overflow;
-    CUDA_TRY(nms_launch(q, c->N, st));
+    if (soft) {
+        SoftNmsParams sq = *soft;
+        sq.nms = q;
+        CUDA_TRY(soft_nms_launch(sq, c->N, st));
+    } else {
+        CUDA_TRY(nms_launch(q, c->N, st));
+    }
     return LFD_OK;
+}
+
+extern "C" int lfd_postprocess(const lfd_post_cfg* c, const float* cls, const float* reg, const float* img_w, const float* img_h,
+                               const float* resize_scale, void* workspace, float* dets, int32_t* labels, int32_t* src, int32_t* count,
+                               int32_t* overflow, lfd_stream stream) {
+    return postprocess_impl("lfd_postprocess", c, cls, reg, img_w, img_h, resize_scale, workspace, dets, labels, src, count, overflow, nullptr, stream);
+}
+
+// the reference's soft_nms method codes (nms.py:101); method 0 of soft_nms_cpu (hard suppression) is not reachable from its Python
+static int soft_params(const char* fn, int method, float sigma, float min_score, SoftNmsParams* out) {
+    if (method != 1 && method != 2) return fail(LFD_ERR_INVALID, "%s: method must be 1 (linear) or 2 (gaussian)", fn);
+    out->method = method; out->sigma = sigma; out->min_score = min_score;
+    return LFD_OK;
+}
+
+extern "C" size_t lfd_postprocess_soft_nms_workspace_bytes(const lfd_post_cfg* cfg) { return lfd_postprocess_workspace_bytes(cfg); }
+
+extern "C" int lfd_postprocess_soft_nms(const lfd_post_cfg* c, const float* cls, const float* reg, const float* img_w, const float* img_h,
+                                        const float* resize_scale, void* workspace, float* dets, int32_t* labels, int32_t* src, int32_t* count,
+                                        int32_t* overflow, int method, float sigma, float min_score, lfd_stream stream) {
+    SoftNmsParams sq;
+    const int rc = soft_params("lfd_postprocess_soft_nms", method, sigma, min_score, &sq);
+    if (rc) return rc;
+    return postprocess_impl("lfd_postprocess_soft_nms", c, cls, reg, img_w, img_h, resize_scale, workspace, dets, labels, src, count, overflow, &sq,
+                            stream);
 }
 
 // multiclass_nms / batched_nms on explicit boxes (lfd/model/utils/nms.py:119-220): threshold + class-offset NMS, all on the device
 extern "C" size_t lfd_multiclass_nms_workspace_bytes(int cap) { return cap > 0 ? post_layout(1, cap).total : 256; }
 
-extern "C" int lfd_multiclass_nms(const float* boxes, int box_per_class, const float* scores, int score_stride, const int32_t* labels_in, int n, int C,
-                                  float score_thr, float iou_thr, int class_agnostic, int cap, void* workspace, float* dets, int32_t* labels, int32_t* src,
-                                  int32_t* count, int32_t* overflow, lfd_stream stream) {
+static int multiclass_impl(const char* fn, const float* boxes, int box_per_class, const float* scores, int score_stride, const int32_t* labels_in,
+                           int n, int C, float score_thr, float iou_thr, int class_agnostic, int cap, void* workspace, float* dets, int32_t* labels,
+                           int32_t* src, int32_t* count, int32_t* overflow, const SoftNmsParams* soft, lfd_stream stream) {
     if (n < 0 || C < 1 || cap < 1 || !workspace || !dets || !labels || !src || !count || !overflow || (n > 0 && (!boxes || !scores)))
-        return fail(LFD_ERR_INVALID, "lfd_multiclass_nms: bad arguments");
-    if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_multiclass_nms: no CUDA device (there is no CPU fallback)");
+        return fail(LFD_ERR_INVALID, "%s: bad arguments", fn);
+    if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "%s: no CUDA device (there is no CPU fallback)", fn);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
     const PostLayout L = post_layout(1, cap);
@@ -599,8 +631,33 @@ extern "C" int lfd_multiclass_nms(const float* boxes, int box_per_class, const f
     q.scratch = ws + L.scratch; q.scratch_stride = L.scratch_stride; q.cap = cap; q.cap_pow2 = L.cap_pow2; q.C = C;
     q.class_agnostic = class_agnostic; q.iou_thr = iou_thr;
     q.out_dets = dets; q.out_label = labels; q.out_src = src; q.out_count = count; q.overflow = overflow;
-    CUDA_TRY(nms_launch(q, 1, st));
+    if (soft) {
+        SoftNmsParams sq = *soft;
+        sq.nms = q;
+        CUDA_TRY(soft_nms_launch(sq, 1, st));
+    } else {
+        CUDA_TRY(nms_launch(q, 1, st));
+    }
     return LFD_OK;
+}
+
+extern "C" int lfd_multiclass_nms(const float* boxes, int box_per_class, const float* scores, int score_stride, const int32_t* labels_in, int n, int C,
+                                  float score_thr, float iou_thr, int class_agnostic, int cap, void* workspace, float* dets, int32_t* labels, int32_t* src,
+                                  int32_t* count, int32_t* overflow, lfd_stream stream) {
+    return multiclass_impl("lfd_multiclass_nms", boxes, box_per_class, scores, score_stride, labels_in, n, C, score_thr, iou_thr, class_agnostic, cap,
+                           workspace, dets, labels, src, count, overflow, nullptr, stream);
+}
+
+extern "C" size_t lfd_multiclass_soft_nms_workspace_bytes(int cap) { return lfd_multiclass_nms_workspace_bytes(cap); }
+
+extern "C" int lfd_multiclass_soft_nms(const float* boxes, int box_per_class, const float* scores, int score_stride, const int32_t* labels_in, int n,
+                                       int C, float score_thr, float iou_thr, int class_agnostic, int cap, void* workspace, float* dets, int32_t* labels,
+                                       int32_t* src, int32_t* count, int32_t* overflow, int method, float sigma, float min_score, lfd_stream stream) {
+    SoftNmsParams sq;
+    const int rc = soft_params("lfd_multiclass_soft_nms", method, sigma, min_score, &sq);
+    if (rc) return rc;
+    return multiclass_impl("lfd_multiclass_soft_nms", boxes, box_per_class, scores, score_stride, labels_in, n, C, score_thr, iou_thr, class_agnostic,
+                           cap, workspace, dets, labels, src, count, overflow, &sq, stream);
 }
 
 // standalone NMS on raw dets (mirror of nms_ext.nms)

@@ -90,6 +90,13 @@ size_t nms_scratch_stride(int cap, int cap_pow2);
 cudaError_t box_candidates_launch(const float* boxes, int box_per_class, const float* scores, int score_stride, const int* labels_in, int n, int C,
                                   float score_thr, int cap, float* cand_box, float* cand_score, int* cand_src, int* cand_count, cudaStream_t st);
 cudaError_t nms_launch(const NmsParams& p, int n_images, cudaStream_t st);
+// Soft-NMS on the same candidates, scratch and outputs (nms.iou_thr = the linear threshold; outputs in selection order, scores decayed)
+struct SoftNmsParams {
+    NmsParams nms;
+    int method;                // 1 linear, 2 gaussian (the reference's codes)
+    float sigma, min_score;
+};
+cudaError_t soft_nms_launch(const SoftNmsParams& p, int n_images, cudaStream_t st);
 
 struct AssignParams {
     LevelTable lv;

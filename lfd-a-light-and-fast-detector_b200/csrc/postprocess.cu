@@ -214,6 +214,81 @@ __device__ __forceinline__ float iou_ref(const float4 a, const float aa, const f
     const float inter = __fmul_rn(w, h);
     return __fdiv_rn(inter, __fsub_rn(__fadd_rn(aa, ab), inter));  // nms_cpu.cpp:57-61
 }
+__device__ __forceinline__ float box_area(const float4 b) { return __fmul_rn(__fsub_rn(b.z, b.x), __fsub_rn(b.w, b.y)); }
+
+// largest and smallest coordinate over the K candidate boxes (nms.py:148 `bboxes.max()`), every thread gets both
+__device__ __forceinline__ void block_box_extent(const float4* cbox, int K, float* s_red, float* s_red2, float& mx, float& mn) {
+    const int tid = threadIdx.x;
+    mx = -3.4e38f; mn = 3.4e38f;
+    for (int i = tid; i < K; i += kNmsThreads) {
+        const float4 b = cbox[i];
+        mx = fmaxf(mx, fmaxf(fmaxf(b.x, b.y), fmaxf(b.z, b.w)));
+        mn = fminf(mn, fminf(fminf(b.x, b.y), fminf(b.z, b.w)));
+    }
+    for (int o = 16; o; o >>= 1) {
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+    }
+    if ((tid & 31) == 0) { s_red[tid >> 5] = mx; s_red2[tid >> 5] = mn; }
+    __syncthreads();
+    mx = s_red[0];
+    mn = s_red2[0];
+    for (int i = 1; i < kNmsThreads / 32; ++i) { mx = fmaxf(mx, s_red[i]); mn = fminf(mn, s_red2[i]); }
+}
+
+// ascending bitonic sort of Kp (a power of two) 64-bit keys, with an optional 32-bit payload
+__device__ __forceinline__ void block_bitonic_sort(unsigned long long* keys, uint32_t* pay, int Kp) {
+    const int tid = threadIdx.x;
+    for (int size = 2; size <= Kp; size <<= 1)
+        for (int stride = size >> 1; stride > 0; stride >>= 1) {
+            for (int i = tid; i < (Kp >> 1); i += kNmsThreads) {
+                const int lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
+                const bool up = (lo & size) == 0;
+                const unsigned long long a = keys[lo], b = keys[hi];
+                if ((a > b) == up) {
+                    keys[lo] = b; keys[hi] = a;
+                    if (pay) { const uint32_t t = pay[lo]; pay[lo] = pay[hi]; pay[hi] = t; }
+                }
+            }
+            __syncthreads();
+        }
+}
+
+// exclusive prefix of v over the block's threads; the total lands in s_scan[32]
+__device__ __forceinline__ int block_exclusive_scan(int v, int* s_scan) {
+    const int tid = threadIdx.x;
+    int incl = v;
+    for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, o);
+        if ((tid & 31) >= o) incl += t;
+    }
+    __syncthreads();
+    if ((tid & 31) == 31) s_scan[tid >> 5] = incl;
+    __syncthreads();
+    if (tid < 32) {
+        int w = s_scan[tid], wi = w;
+        for (int o = 1; o < 32; o <<= 1) {
+            const int t = __shfl_up_sync(0xffffffffu, wi, o);
+            if (tid >= o) wi += t;
+        }
+        s_scan[tid] = wi - w;
+        if (tid == 31) s_scan[32] = wi;
+    }
+    __syncthreads();
+    return s_scan[tid >> 5] + incl - v;
+}
+
+// output row k of image n: the box with its class offset taken off again (nms.py:155, the fp32 round trip kept), score, label, source
+__device__ __forceinline__ void write_det(const NmsParams& p, int n, int k, float4 ob, float score, int src, float offmul) {
+    if (!p.class_agnostic) {
+        const float off = __fmul_rn((float)(src % p.C), offmul);
+        ob.x = __fsub_rn(ob.x, off); ob.y = __fsub_rn(ob.y, off); ob.z = __fsub_rn(ob.z, off); ob.w = __fsub_rn(ob.w, off);
+    }
+    float* d = p.out_dets + ((size_t)n * p.cap + k) * 5;
+    d[0] = ob.x; d[1] = ob.y; d[2] = ob.z; d[3] = ob.w; d[4] = score;
+    p.out_label[(size_t)n * p.cap + k] = src % p.C;
+    p.out_src[(size_t)n * p.cap + k] = src;
+}
 
 __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsParams p) {
     extern __shared__ __align__(16) uint8_t nsm[];
@@ -249,22 +324,7 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsParams p) {
 
     // 1. max coordinate over the candidate boxes (nms.py:148 `bboxes.max()`)
     float mx = -3.4e38f, mn = 3.4e38f;
-    if (!p.class_agnostic) {
-        for (int i = tid; i < K; i += kNmsThreads) {
-            const float4 b = cbox[i];
-            mx = fmaxf(mx, fmaxf(fmaxf(b.x, b.y), fmaxf(b.z, b.w)));
-            mn = fminf(mn, fminf(fminf(b.x, b.y), fminf(b.z, b.w)));
-        }
-        for (int o = 16; o; o >>= 1) {
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-            mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
-        }
-        if ((tid & 31) == 0) { s_red[tid >> 5] = mx; s_red2[tid >> 5] = mn; }
-        __syncthreads();
-        mx = s_red[0];
-        mn = s_red2[0];
-        for (int i = 1; i < kNmsThreads / 32; ++i) { mx = fmaxf(mx, s_red[i]); mn = fminf(mn, s_red2[i]); }
-    }
+    if (!p.class_agnostic) block_box_extent(cbox, K, s_red, s_red2, mx, mn);
     const float offmul = __fadd_rn(mx, 1.0f);
 
     // 2. sort keys: score descending, source index ascending (deterministic total order)
@@ -275,19 +335,7 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsParams p) {
         pay[i] = (uint32_t)i;
     }
     __syncthreads();
-    for (int size = 2; size <= Kp; size <<= 1)
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            for (int i = tid; i < (Kp >> 1); i += kNmsThreads) {
-                const int lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
-                const bool up = (lo & size) == 0;
-                const unsigned long long a = keys[lo], b = keys[hi];
-                if ((a > b) == up) {
-                    keys[lo] = b; keys[hi] = a;
-                    const uint32_t t = pay[lo]; pay[lo] = pay[hi]; pay[hi] = t;
-                }
-            }
-            __syncthreads();
-        }
+    block_bitonic_sort(keys, pay, Kp);
 
     // 3. sorted, class-offset boxes
     for (int i = tid; i < K; i += kNmsThreads) {
@@ -346,16 +394,7 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsParams p) {
         for (int k = tid; k < nkeep; k += kNmsThreads) {
             const int i = keep_list[k];
             const int s = (int)pay[i];
-            const int src = csrc[s];
-            float4 ob = sbox[i];
-            if (!p.class_agnostic) {  // nms.py:155 subtracts the offsets again (fp32 round trip kept)
-                const float off = __fmul_rn((float)(src % p.C), offmul);
-                ob.x = __fsub_rn(ob.x, off); ob.y = __fsub_rn(ob.y, off); ob.z = __fsub_rn(ob.z, off); ob.w = __fsub_rn(ob.w, off);
-            }
-            float* d = p.out_dets + ((size_t)n * p.cap + k) * 5;
-            d[0] = ob.x; d[1] = ob.y; d[2] = ob.z; d[3] = ob.w; d[4] = cscore[s];
-            p.out_label[(size_t)n * p.cap + k] = src % p.C;
-            p.out_src[(size_t)n * p.cap + k] = src;
+            write_det(p, n, k, sbox[i], cscore[s], csrc[s], offmul);
         }
         if (tid == 0) p.out_count[n] = nkeep;
         return;
@@ -372,43 +411,13 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsParams p) {
         for (int i = tid; i < Kp; i += kNmsThreads)
             keys[i] = i < K ? (((unsigned long long)(unsigned)(csrc[pay[i]] % p.C) << 32) | (unsigned)i) : ~0ull;
         __syncthreads();
-        for (int size = 2; size <= Kp; size <<= 1)
-            for (int stride = size >> 1; stride > 0; stride >>= 1) {
-                for (int i = tid; i < (Kp >> 1); i += kNmsThreads) {
-                    const int lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
-                    const bool up = (lo & size) == 0;
-                    const unsigned long long a = keys[lo], b = keys[hi];
-                    if ((a > b) == up) { keys[lo] = b; keys[hi] = a; }
-                }
-                __syncthreads();
-            }
+        block_bitonic_sort(keys, nullptr, Kp);
         // segment starts, in order (block-wide exclusive scan of the boundary flags; each thread owns a run of consecutive positions)
         const int per = (K + kNmsThreads - 1) / kNmsThreads;
         const int i0 = min(tid * per, K), i1 = min(i0 + per, K);
-        auto block_offset = [&](int v) -> int {          // exclusive prefix of v over the threads; total in s_scan[32]
-            int incl = v;
-            for (int o = 1; o < 32; o <<= 1) {
-                const int t = __shfl_up_sync(0xffffffffu, incl, o);
-                if ((tid & 31) >= o) incl += t;
-            }
-            __syncthreads();
-            if ((tid & 31) == 31) s_scan[tid >> 5] = incl;
-            __syncthreads();
-            if (tid < 32) {
-                int w = s_scan[tid], wi = w;
-                for (int o = 1; o < 32; o <<= 1) {
-                    const int t = __shfl_up_sync(0xffffffffu, wi, o);
-                    if (tid >= o) wi += t;
-                }
-                s_scan[tid] = wi - w;
-                if (tid == 31) s_scan[32] = wi;
-            }
-            __syncthreads();
-            return s_scan[tid >> 5] + incl - v;
-        };
         int cnt = 0;
         for (int i = i0; i < i1; ++i) cnt += (i == 0 || (keys[i] >> 32) != (keys[i - 1] >> 32)) ? 1 : 0;
-        int pos = block_offset(cnt);
+        int pos = block_exclusive_scan(cnt, s_scan);
         const int nseg = s_scan[32];
         for (int i = i0; i < i1; ++i)
             if (i == 0 || (keys[i] >> 32) != (keys[i - 1] >> 32)) seg[pos++] = i;
@@ -455,18 +464,11 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsParams p) {
         // kept boxes in global rank (score) order
         cnt = 0;
         for (int i = i0; i < i1; ++i) cnt += removed[i] ? 0 : 1;
-        int k = block_offset(cnt);
+        int k = block_exclusive_scan(cnt, s_scan);
         for (int i = i0; i < i1; ++i) {
             if (removed[i]) continue;
             const int sidx = (int)pay[i];
-            const int src = csrc[sidx];
-            float4 ob = sbox[i];
-            const float off = __fmul_rn((float)(src % p.C), offmul);      // nms.py:155 subtracts the offsets again (fp32 round trip kept)
-            ob.x = __fsub_rn(ob.x, off); ob.y = __fsub_rn(ob.y, off); ob.z = __fsub_rn(ob.z, off); ob.w = __fsub_rn(ob.w, off);
-            float* d = p.out_dets + ((size_t)n * p.cap + k) * 5;
-            d[0] = ob.x; d[1] = ob.y; d[2] = ob.z; d[3] = ob.w; d[4] = cscore[sidx];
-            p.out_label[(size_t)n * p.cap + k] = src % p.C;
-            p.out_src[(size_t)n * p.cap + k] = src;
+            write_det(p, n, k, sbox[i], cscore[sidx], csrc[sidx], offmul);
             ++k;
         }
         if (tid == 0) p.out_count[n] = s_scan[32];
@@ -479,18 +481,8 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsParams p) {
         const float4 bi = sbox[i];
         const float ai = __fmul_rn(__fsub_rn(bi.z, bi.x), __fsub_rn(bi.w, bi.y));
         if (tid == 0) {
-            const int k = s_keep++;
             const int s = (int)pay[i];
-            const int src = csrc[s];
-            float4 ob = bi;
-            if (!p.class_agnostic) {  // nms.py:155 subtracts the offsets again (fp32 round trip kept)
-                const float off = __fmul_rn((float)(src % p.C), offmul);
-                ob.x = __fsub_rn(ob.x, off); ob.y = __fsub_rn(ob.y, off); ob.z = __fsub_rn(ob.z, off); ob.w = __fsub_rn(ob.w, off);
-            }
-            float* d = p.out_dets + ((size_t)n * p.cap + k) * 5;
-            d[0] = ob.x; d[1] = ob.y; d[2] = ob.z; d[3] = ob.w; d[4] = cscore[s];
-            p.out_label[(size_t)n * p.cap + k] = src % p.C;
-            p.out_src[(size_t)n * p.cap + k] = src;
+            write_det(p, n, s_keep++, bi, cscore[s], csrc[s], offmul);
         }
         for (int j = i + 1 + tid; j < K; j += kNmsThreads) {
             if (removed[j]) continue;
@@ -501,6 +493,173 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsParams p) {
         __syncthreads();
     }
     if (tid == 0) p.out_count[n] = s_keep;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Soft-NMS (nms_cpu.cpp:76-206 behind utils/nms.py:62-158): one CTA per image runs the reference's in-place loop over ONE array
+// holding every class (per-class CTAs would differ: the swaps of one class move positions that decide the ties of another).
+//   0. the candidates are sorted by source index, which is the reference's initial order (input rows, or nonzero() of the
+//      thresholded (point, class) grid); class-aware mode adds label * (max coordinate + 1) in fp32 as the hard path does
+//   per iteration i over the n live positions:
+//   1. select: one block reduction of key = desc_key(score) << 32 | position over [i, n) -- the FIRST position of the maximum
+//      (the reference scans with `max < s[pos]`, so -0 ties +0, a NaN at i is selected, a NaN behind i never is)
+//   2. swap the selected element m with i (only the element at i has to move: position i is never read again) and emit row i
+//   3. reweight (i, n): linear w = ovr > thr ? 1 - ovr : 1, gaussian w = (float)exp((double)(-(ovr * ovr) / sigma)); an element
+//      whose new score is < min_score is removed
+//   4. only when the block votes a removal: reproduce the reference's swap-with-last compaction as a permutation -- the j-th lowest
+//      removed position below the new count receives the j-th highest surviving position at or above it (the weights do not depend
+//      on the position, so reweighting everything first and permuting afterwards gives the same array)
+// Layout (shared memory up to kSoftSmem entries, else the image's global scratch): box float4 [L] (class-offset boxes; areas are
+// recomputed) | (score, src) float2 [Lp] (the u64 sort keys before step 0 ends) | hole table int [L / 2 + 1] | removed flags u8 [L].
+// Arithmetic that decides the results uses _rn intrinsics: linear mode is bit-exact against the reference's fp32 loop.
+static constexpr int kSoftSmem = 8192;
+static constexpr size_t kSoftSmemBytes = (size_t)kSoftSmem * 24 + ((size_t)kSoftSmem / 2 + 1) * 4 + kSoftSmem;   // 216 KB
+
+__global__ void __launch_bounds__(kNmsThreads) soft_nms_kernel(const SoftNmsParams sp) {
+    extern __shared__ __align__(16) uint8_t ssm[];
+    __shared__ float s_red[32], s_red2[32];
+    __shared__ unsigned long long s_min[32];
+    __shared__ int s_scan[33];
+    const NmsParams& p = sp.nms;
+    const int n = blockIdx.x;
+    const int tid = threadIdx.x, lane = tid & 31;
+    int K = p.cand_count[n];
+    if (K > p.cap) {  // capacity overflow: report, process the first cap (host turns this into an error)
+        if (tid == 0) atomicExch(p.overflow, 1);
+        K = p.cap;
+    }
+    if (K == 0) {
+        if (tid == 0) p.out_count[n] = 0;
+        return;
+    }
+    int Kp = 1;
+    while (Kp < K) Kp <<= 1;
+    const bool in_smem = K <= kSoftSmem;
+    const size_t L = in_smem ? kSoftSmem : p.cap, Lp = in_smem ? kSoftSmem : p.cap_pow2;
+    uint8_t* base = in_smem ? ssm : p.scratch + (size_t)n * p.scratch_stride;
+    float4* box = reinterpret_cast<float4*>(base);
+    unsigned long long* keys = reinterpret_cast<unsigned long long*>(base + L * 16);
+    float2* ss = reinterpret_cast<float2*>(keys);
+    int* holes = reinterpret_cast<int*>(base + L * 16 + Lp * 8);
+    uint8_t* gone = reinterpret_cast<uint8_t*>(holes + L / 2 + 1);
+    const float4* cbox = reinterpret_cast<const float4*>(p.cand_box) + (size_t)n * p.cap;
+    const float* cscore = p.cand_score + (size_t)n * p.cap;
+    const int* csrc = p.cand_src + (size_t)n * p.cap;
+
+    float mx = -3.4e38f, mn = 3.4e38f;
+    if (!p.class_agnostic) block_box_extent(cbox, K, s_red, s_red2, mx, mn);
+    const float offmul = __fadd_rn(mx, 1.0f);
+
+    // 0. reference order: sort by source index (unique per image), candidate slot in the low word
+    for (int i = tid; i < Kp; i += kNmsThreads)
+        keys[i] = i < K ? (((unsigned long long)(unsigned)csrc[i] << 32) | (unsigned)i) : ~0ull;
+    __syncthreads();
+    block_bitonic_sort(keys, nullptr, Kp);
+    for (int i = tid; i < K; i += kNmsThreads) {
+        const int c = (int)(unsigned)keys[i];     // ss[i] overwrites keys[i]: same thread, same address
+        const int src = csrc[c];
+        float4 b = cbox[c];
+        if (!p.class_agnostic) {
+            const float off = __fmul_rn((float)(src % p.C), offmul);
+            b.x = __fadd_rn(b.x, off); b.y = __fadd_rn(b.y, off); b.z = __fadd_rn(b.z, off); b.w = __fadd_rn(b.w, off);
+        }
+        box[i] = b;
+        ss[i] = make_float2(cscore[c], __int_as_float(src));
+    }
+    __syncthreads();
+
+    const float thr = p.iou_thr, sigma = sp.sigma, min_score = sp.min_score;
+    const bool linear = sp.method == 1;
+    int cnt = K;   // live positions (block-uniform)
+    for (int i = 0; i < cnt; ++i) {
+        // 1. selection
+        unsigned long long best = ~0ull;
+        for (int q = i + tid; q < cnt; q += kNmsThreads) {
+            const float s = ss[q].x;
+            unsigned long long k;
+            if (s != s) k = q == i ? (unsigned long long)(unsigned)i : ~0ull;   // desc_key never yields 0 for a number
+            else k = ((unsigned long long)desc_key(s == 0.f ? 0.f : s) << 32) | (unsigned)q;
+            best = k < best ? k : best;
+        }
+        for (int o = 16; o; o >>= 1) {
+            const unsigned long long t = __shfl_xor_sync(0xffffffffu, best, o);
+            best = t < best ? t : best;
+        }
+        if (lane == 0) s_min[tid >> 5] = best;
+        __syncthreads();
+        best = s_min[0];
+        for (int w = 1; w < kNmsThreads / 32; ++w) best = s_min[w] < best ? s_min[w] : best;
+        const int m = (int)(unsigned)best;
+        const float4 bm = box[m];
+        const float2 em = ss[m];
+        const float am = box_area(bm);
+        if (tid == 0) write_det(p, n, i, bm, em.x, __float_as_int(em.y), offmul);
+        __syncthreads();   // position m is rewritten below
+
+        // 2 + 3. the element at i moves to m; reweight (i, cnt)
+        bool any_gone = false;
+        for (int q = i + 1 + tid; q < cnt; q += kNmsThreads) {
+            const int from = q == m ? i : q;
+            const float4 b = box[from];
+            float2 e = ss[from];
+            const float ovr = iou_ref(bm, am, b, box_area(b));
+            float w = 1.f;
+            if (linear) {
+                if (ovr > thr) w = __fsub_rn(1.f, ovr);
+            } else {
+                w = (float)exp((double)__fdiv_rn(-__fmul_rn(ovr, ovr), sigma));
+            }
+            e.x = __fmul_rn(w, e.x);
+            const bool g = e.x < min_score;
+            if (q == m) box[q] = b;
+            ss[q] = e;
+            gone[q] = g;
+            any_gone |= g;
+        }
+        if (!__syncthreads_or(any_gone)) continue;
+
+        // 4. compaction (each thread owns a run of consecutive positions of (i, cnt))
+        const int a = i + 1, len = cnt - a;
+        const int per = (len + kNmsThreads - 1) / kNmsThreads;
+        const int q0 = min(a + tid * per, cnt), q1 = min(q0 + per, cnt);
+        int c = 0;
+        for (int q = q0; q < q1; ++q) c += gone[q];
+        const int before = block_exclusive_scan(c, s_scan);   // removed positions in [a, q0)
+        const int removed = s_scan[32];
+        const int n2 = cnt - removed, survivors = len - removed;
+        int r = before;
+        for (int q = q0; q < q1; ++q)
+            if (gone[q]) {
+                if (q < n2) holes[r] = q;                      // removed positions below n2 come first: rank among the holes = r
+                ++r;
+            }
+        __syncthreads();
+        r = before;
+        for (int q = q0; q < q1; ++q) {
+            if (gone[q]) { ++r; continue; }
+            if (q >= n2) {
+                const int h = holes[survivors - ((q - a + 1) - r)];   // rank from the top = survivors in (q, cnt)
+                box[h] = box[q];
+                ss[h] = ss[q];
+            }
+        }
+        __syncthreads();
+        cnt = n2;
+    }
+    if (tid == 0) p.out_count[n] = cnt;
+}
+
+cudaError_t soft_nms_launch(const SoftNmsParams& p, int n_images, cudaStream_t st) {
+    static bool attr[kMaxDevices] = {};   // per-device function attribute
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
+    if (!attr[dev]) {
+        cudaError_t e = cudaFuncSetAttribute(soft_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSoftSmemBytes);
+        if (e != cudaSuccess) return e;
+        attr[dev] = true;
+    }
+    soft_nms_kernel<<<n_images, kNmsThreads, kSoftSmemBytes, st>>>(p);
+    return cudaGetLastError();
 }
 
 cudaError_t candidates_launch(const PostParams& p, int num_sms, cudaStream_t st) {

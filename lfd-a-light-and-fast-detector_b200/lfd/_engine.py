@@ -740,10 +740,11 @@ def make_norm_probe(head):
 
 
 class PostPlan(object):
-    """Pre-allocated device post-process (lfd_postprocess) for a fixed batch size / level geometry."""
+    """Pre-allocated device post-process (lfd_postprocess, or lfd_postprocess_soft_nms when soft = (method code, sigma, min_score)) for a
+    fixed batch size / level geometry."""
 
-    def __init__(self, cfg, device):
-        self.cfg, self.device = cfg, device
+    def __init__(self, cfg, device, soft=None):
+        self.cfg, self.device, self.soft = cfg, device, soft
         N, cap = cfg.N, cfg.cap
         self.ws = torch.empty(max(nat.lib().lfd_postprocess_workspace_bytes(C.byref(cfg)), 256), dtype=torch.uint8, device=device)
         self.dets = torch.empty((N, cap, 5), dtype=torch.float32, device=device)
@@ -766,7 +767,12 @@ class PostPlan(object):
         if iou_thr is not None:
             self.cfg.iou_thr = float(iou_thr)
         with torch.cuda.device(self.device):
-            nat.check(nat.lib().lfd_postprocess(C.byref(self.cfg), nat.ptr(cls), nat.ptr(reg), nat.ptr(self.meta[0]), nat.ptr(self.meta[1]),
-                                                nat.ptr(self.meta[2]), nat.ptr(self.ws), nat.ptr(self.dets), nat.ptr(self.labels),
-                                                nat.ptr(self.src), nat.ptr(self.count), nat.ptr(self.count[self.cfg.N:]), nat.stream_ptr()))
+            args = (C.byref(self.cfg), nat.ptr(cls), nat.ptr(reg), nat.ptr(self.meta[0]), nat.ptr(self.meta[1]), nat.ptr(self.meta[2]),
+                    nat.ptr(self.ws), nat.ptr(self.dets), nat.ptr(self.labels), nat.ptr(self.src), nat.ptr(self.count),
+                    nat.ptr(self.count[self.cfg.N:]))
+            if self.soft is None:
+                nat.check(nat.lib().lfd_postprocess(*args, nat.stream_ptr()))
+            else:
+                method, sigma, min_score = self.soft
+                nat.check(nat.lib().lfd_postprocess_soft_nms(*args, int(method), float(sigma), float(min_score), nat.stream_ptr()))
         return self.dets, self.labels, self.src, self.count

@@ -20,6 +20,7 @@ DTYPE_BF16, DTYPE_FP16 = 0, 1
 CLS_SIGMOID, CLS_SOFTMAX, CLS_BCE, CLS_QFL = 0, 1, 2, 3
 REG_IOU, REG_GIOU, REG_DIOU, REG_CIOU, REG_SMOOTH_L1, REG_MSE = range(6)
 BBOX_SIGMOID, BBOX_EXP, BBOX_INDEPENDENT = 0, 1, 2
+SOFT_NMS_METHODS = {'linear': 1, 'gaussian': 2}   # the reference's soft_nms method codes (utils/nms.py:101)
 ASSIGN_DIST, ASSIGN_LONGER, ASSIGN_SHORTER = 0, 1, 2
 
 
@@ -132,6 +133,10 @@ SYMBOLS = {
     'lfd_postprocess': (_i, [C.POINTER(PostCfg)] + [_vp] * 11),
     'lfd_multiclass_nms_workspace_bytes': (C.c_size_t, [_i]),
     'lfd_multiclass_nms': (_i, [_vp, _i, _vp, _i, _vp, _i, _i, _f, _f, _i, _i] + [_vp] * 7),
+    'lfd_postprocess_soft_nms_workspace_bytes': (C.c_size_t, [C.POINTER(PostCfg)]),
+    'lfd_postprocess_soft_nms': (_i, [C.POINTER(PostCfg)] + [_vp] * 11 + [_i, _f, _f, _vp]),
+    'lfd_multiclass_soft_nms_workspace_bytes': (C.c_size_t, [_i]),
+    'lfd_multiclass_soft_nms': (_i, [_vp, _i, _vp, _i, _vp, _i, _i, _f, _f, _i, _i] + [_vp] * 6 + [_i, _f, _f, _vp]),
     'lfd_nms_workspace_bytes': (C.c_size_t, [_i]),
     'lfd_nms': (_i, [_vp, _i, _f, _vp, _vp, _vp, _vp]),
     'lfd_assign_targets': (_i, [C.POINTER(Levels), _i, _i, _i, _i, _i, _i] + [_vp] * 8),

@@ -6,7 +6,8 @@ Same constructor kwargs, state_dict keys and public methods (`forward`, `get_los
 `head_indexes_to_feature_map_sizes`); all device work is done by liblfd_b200.so:
 
     forward                   -> lfd_plan_forward      (whole net = one layer plan, CUDA-graph replayed)
-    get_results / predict_*   -> lfd_postprocess       (sigmoid|softmax + decode + class-aware NMS on device)
+    get_results / predict_*   -> lfd_postprocess       (sigmoid|softmax + decode + class-aware NMS on device), or
+                                 lfd_postprocess_soft_nms when _nms_cfg['type'] is 'soft_nms'
     annotation_to_target      -> lfd_assign_targets    (label assignment on device)
     get_loss                  -> lfd_assign_targets + lfd_detection_loss (loss + gradients w.r.t. the outputs)
 
@@ -24,6 +25,7 @@ import torch.nn as nn
 
 from .. import _native as nat
 from .._engine import InferencePlan, PostPlan
+from .utils.nms import _nms_args
 
 __all__ = ['LFD']
 
@@ -402,17 +404,33 @@ class LFD(nn.Module):
         cfg.cap = int(self.max_detections_per_image)
         return cfg
 
+    def _soft_nms_cfg(self):
+        """_nms_cfg['type'] 'nms' -> None; 'soft_nms' -> (method code, sigma, min_score); anything else raises (the reference would fail
+        in its batched_nms; running greedy NMS instead would return other detections without a word)."""
+        nms_type = self._nms_cfg.get('type', 'nms')
+        if nms_type == 'nms':
+            return None
+        if nms_type != 'soft_nms':
+            raise ValueError('unknown nms_cfg type %r: expected "nms" or "soft_nms"' % (nms_type,))
+        return _nms_args(self._nms_cfg)[2]
+
     def post_plan(self, n, sizes, device, class_agnostic=False):
+        """The cached device post-process for this batch geometry and the current _nms_cfg type (greedy NMS or Soft-NMS with its method,
+        sigma and min_score)."""
+        soft = self._soft_nms_cfg()
         key = (n, tuple(map(tuple, sizes)), int(self.max_detections_per_image), str(device), bool(class_agnostic),
                type(self._classification_loss_func).__name__, self._distance_to_bbox_mode, self._regression_loss_type)
+        if soft is not None:
+            key = key + ('soft_nms',) + soft
         if key not in self._post_plans:
             self._post_plans[key] = PostPlan(self._post_cfg(n, sizes, self._classification_threshold, self._nms_cfg['iou_thr'],
-                                                            class_agnostic), device)
+                                                            class_agnostic), device, soft)
         return self._post_plans[key]
 
     def detect(self, predict_outputs, heights, widths, scales, score_thr, iou_thr, class_agnostic=False):
-        """Device post-process.  -> (dets [N,cap,5] x1,y1,x2,y2,score ; labels [N,cap] ; src [N,cap] ; count [N] ; overflow [1])
-        on the device (buffers owned by the cached post-process plan)."""
+        """Device post-process with the NMS of _nms_cfg['type'] (iou_thr: the greedy threshold, or Soft-NMS's linear one).
+        -> (dets [N,cap,5] x1,y1,x2,y2,score ; labels [N,cap] ; src [N,cap] ; count [N] ; overflow [1]) on the device (buffers owned by
+        the cached post-process plan); Soft-NMS rows are in selection order with their decayed scores."""
         cls, reg = predict_outputs
         if not cls.is_cuda:
             raise RuntimeError('lfd_b200 has no CPU path')

@@ -99,7 +99,7 @@ class StreamingDetector(object):
             self.plan.autotune()
         for i, hw in enumerate(self.plan.level_sizes):
             model._head_indexes_to_feature_map_sizes[i] = hw
-        self.post = model.post_plan(batch, self.plan.level_sizes, dev)
+        self.post = model.post_plan(batch, self.plan.level_sizes, dev)   # greedy NMS or Soft-NMS: model._nms_cfg as of now
         self.post.set_meta([width] * batch, [height] * batch, [1.0] * batch)
         self.pipe = ForwardPostPipeline(model, self.plan, self.post, self.score_thr, self.iou_thr)
         self.slots = []
