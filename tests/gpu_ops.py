@@ -158,24 +158,24 @@ def stem_input(img, fmt, dtype='bf16'):
     16-bit type."""
     rnd = DTYPES[dtype][1]
     if fmt == 'u8':
-        return rnd((img.cpu().float() - 127.5) * (1.0 / 127.5))
-    return rnd(img.cpu().float().permute(0, 2, 3, 1))
+        return rnd((img.float() - 127.5) * (1.0 / 127.5))
+    return rnd(img.float().permute(0, 2, 3, 1))
 
 
-def ref_conv64(x_nhwc, weight, scale, shift, stride, relu, res=None, dtype='bf16'):
-    """float64 CPU evaluation of the fused layer on exactly the operands the kernel sees: round16(weight * scale), round16(shift),
-    the 16-bit input and residual.  -> (y [N,Ho,Wo,Cout] float64, not rounded; S = the same sum over |terms| per output;
-    K = the number of terms the kernel adds in fp32 per output)."""
+def ref_conv64(x_nhwc, weight, scale, shift, stride, relu, res=None, dtype='bf16', device='cpu'):
+    """float64 evaluation of the fused layer on exactly the operands the kernel sees: round16(weight * scale), round16(shift),
+    the 16-bit input and residual, on `device` (the CPU, or the GPU for whole-network sizes).  -> (y [N,Ho,Wo,Cout] float64, not
+    rounded; S = the same sum over |terms| per output; K = the number of terms the kernel adds in fp32 per output)."""
     rnd = DTYPES[dtype][1]
-    x = x_nhwc.cpu().double().permute(0, 3, 1, 2)
-    w = rnd(fold_scale(weight, scale)).double()
-    b = rnd(shift.float().cpu()).double()[None, :, None, None]
+    x = x_nhwc.to(device).double().permute(0, 3, 1, 2)
+    w = rnd(fold_scale(weight, scale)).double().to(device)
+    b = rnd(shift.float().cpu()).double().to(device)[None, :, None, None]
     k = weight.shape[-1]
     y = F.conv2d(x, w, None, stride=stride, padding=k // 2) + b
     S = F.conv2d(x.abs(), w.abs(), None, stride=stride, padding=k // 2) + b.abs()
     K = weight.shape[1] * k * k + 1
     if res is not None:
-        r = res.cpu().double().permute(0, 3, 1, 2)
+        r = res.to(device).double().permute(0, 3, 1, 2)
         y, S, K = y + r, S + r.abs(), K + 1
     if relu:
         y = F.relu(y)
@@ -209,13 +209,14 @@ def assert_faithful(out, ref64, S, K, dtype='bf16', what=''):
 def assert_tail_close(out, ref, dtype='bf16', what=''):
     """Bound for the output of a fused tail: its 16-bit intermediate may differ from the CPU one by 1 ulp on isolated elements
     (fp32 summation order), which moves isolated outputs by more than one output ulp, so 2e-3 of the output range is allowed on
-    top of the 1-ulp bound, and the RMS error must stay small."""
+    top of the 1-ulp bound, and the RMS error must stay small.  Compared on ref's device.  -> max err / tol."""
     ulp = DTYPES[dtype][2]
-    o, r = out.cpu().double(), ref.cpu().double()
+    o, r = out.to(ref.device).double(), ref.double()
     tol = r.abs() * ulp + 2e-3 * float(r.abs().max()) * (ulp / 2.0 ** -7)
     err = (o - r).abs()
     assert bool((err <= tol).all()), '%s: %d elements off, max err %g (ref max %g)' % (what, int((err > tol).sum()), float(err.max()), float(r.abs().max()))
     assert float(torch.sqrt((err ** 2).mean()) / torch.sqrt((r ** 2).mean()).clamp(min=1e-30)) < 3e-3 * (ulp / 2.0 ** -7), what
+    return float((err / tol.clamp(min=1e-300)).max())
 
 
 def assert_gn_stats(stats, out, groups, what=''):

@@ -112,35 +112,6 @@ def stem_wgrad_grid(N, Ho, Wo, sms):          # wgrad_stem (SIMT): (blocks, 64-p
     return min(4 * sms, n_seg), n_seg
 
 
-# ------------------------------------------------------------------------------------------------ float emulation
-def f32(x):
-    """float64 tensor -> the nearest float32 values, as float64."""
-    return x.float().double()
-
-
-def mean_rstd_f32(s1, s2, count, eps):
-    """The kernels' per-channel / per-group mean and rstd (train.cu mean_rstd_from_sums, conv_simt.cu gn_mean_rstd): float64 sums
-    -> (float)mean, (float)(1 / sqrt(var + (double)eps)).  The var line `s2 / count - m * m` may be compiled as one fma; both
-    roundings are evaluated and must give the same float32 results on the test's data, so the emulation is exact either way."""
-    from fractions import Fraction
-    s1, s2 = s1.double().reshape(-1), s2.double().reshape(-1)
-    m = s1 / count
-    q = s2 / count
-    var_sep = (q - m * m).clamp(min=0)
-    var_fma = torch.tensor([float(Fraction(a) - Fraction(b) ** 2) for a, b in zip(q.tolist(), m.tolist())], dtype=torch.float64).clamp(min=0)
-    epsd = float(torch.tensor(eps, dtype=torch.float32))
-    r_sep, r_fma = f32(1.0 / torch.sqrt(var_sep + epsd)), f32(1.0 / torch.sqrt(var_fma + epsd))
-    assert torch.equal(r_sep, r_fma), 'test data: the float rstd depends on fma contraction; pick other data'
-    return f32(m), r_sep
-
-
-def fma_f32(a, b, c):
-    """fmaf(a, b, c) on float32 operands (float64 tensors): the float64 product is exact, the sum is rounded to float64 and then to
-    float32.  Only the sign and the rounded value are used; a double rounding that differs from fmaf needs the exact sum within
-    2^-53 of a float32 rounding boundary."""
-    return f32(a * b + c)
-
-
 def assert_within(got, ref, S, K, what=''):
     """Per element |got - ref| <= K * 2^-24 * S: an fp32 (or fp64) result of an accumulation of terms whose magnitudes sum to S,
     each term passing through at most K fp32 roundings."""

@@ -9,13 +9,13 @@ import os
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 import synth
 from helpers import synth_model
 from lfd._engine import InferencePlan
 from lfd.execution.executor import Executor
 from lfd.execution.optim import FusedSGD
+from test_gpu_train_step_per_op import Replay
 
 pytestmark = pytest.mark.gpu
 
@@ -65,178 +65,6 @@ def test_prefix_tensors_equal_the_inference_plans(cfg, frozen_stages, shape, ste
         assert (4 in kinds) == stem4, kinds                 # lfd._native.OP_STEM4, chosen by the inference plan's L2 gate
     plan.forward(x)
     _prefix_matches_inference(model, plan, x, monkeypatch)
-
-
-def _teacher_forced_trainable(model, x_img, ann):
-    """test_gpu_train.py's teacher-forced layer check, restricted to what the plan differentiates: each layer with a backward, fed the
-    tensors the native path stored, reproduces torch autograd of that layer (same tolerances); layers of the frozen part have no
-    gradient tensor; frozen parameters have no .grad."""
-    n = x_img.shape[0]
-    out = model(x_img)
-    ld = model.get_loss(out, ann)
-    ld['loss'].backward()
-    torch.cuda.synchronize()
-    h, w = x_img.shape[2], x_img.shape[3]
-    plan = model.train_plan_for(n, h, w, x_img.device)
-    bf = lambda t: t.to(torch.bfloat16).float()
-
-    def nhwc(name, hh, ww, c):
-        return plan.tensor(name, hh, ww, c).float().permute(0, 3, 1, 2).contiguous()
-
-    def rel(a, b):
-        return float((a.double() - b.double()).norm() / b.double().norm().clamp(min=1e-20))
-
-    exp_grad, exp_param, shapes = {}, {}, {}
-
-    def note(kind, name, e, tol):
-        assert e < tol, (kind, name, e)
-
-    def add_param(p, g):
-        if p.requires_grad:
-            exp_param[id(p)] = exp_param.get(id(p), 0) + g
-
-    def conv_backward(L, dz_native):
-        conv, geo = L['conv'], L['geo']
-        k, s = geo['ksize'], geo['stride']
-        xin = bf(x_img) if L['x'] is None else nhwc(L['x'], geo['H'], geo['W'], geo['Cin'])
-        add_param(conv.weight, torch.nn.grad.conv2d_weight(xin, conv.weight.shape, dz_native, stride=s, padding=k // 2))
-        if L['x'] is not None and L['x'] in plan._needs_grad:
-            dx = torch.nn.grad.conv2d_input(xin.shape, bf(conv.weight.detach()), dz_native, stride=s, padding=k // 2)
-            exp_grad[L['x']] = exp_grad.get(L['x'], 0) + dx
-            shapes[L['x']] = (geo['H'], geo['W'], geo['Cin'])
-        zname = L['z'] if L['type'] == 'bn' else L['raw']
-        z_exp = F.conv2d(xin, bf(conv.weight.detach()), None, stride=s, padding=k // 2)
-        z_nat = nhwc(zname, geo['Ho'], geo['Wo'], geo['Cout'])
-        note('forward conv', L['name'], float((z_nat - z_exp).abs().max() / z_exp.abs().max().clamp(min=1e-20)), 2.0 ** -7)
-
-    n_checked = 0
-    for L in reversed(plan._layers):
-        geo = L['geo']
-        if L['type'] == 'final':
-            hh, ww = geo['H'], geo['W']
-            raw = nhwc(L['raw'], hh, ww, 128)
-            norm = L['norm']
-            if norm is None:
-                t = raw.clone().requires_grad_(True)
-            else:
-                t = bf(F.relu(F.group_norm(raw, 16, norm.weight.detach(), norm.bias.detach(), norm.eps))).requires_grad_(True)
-            no = geo['n_cls'] + geo['n_reg']
-            off = plan._off[L['stage']]
-            stg = plan.workspace[off:off + (no * 128 + 3 * no) * 4].view(torch.float32)
-            Wm = stg[:no * 128].view(no, 128).clone().requires_grad_(True)
-            sc = stg[no * 128:no * 128 + no].clone()
-            bias = stg[no * 128 + 2 * no:no * 128 + 3 * no].clone().requires_grad_(True)
-            scale_leaf = torch.ones((), device='cuda', requires_grad=True)
-            pre = torch.einsum('nchw,oc->nohw', t, Wm) + bias[None, :, None, None]
-            mult = torch.cat([sc[:geo['n_cls']], scale_leaf * sc[geo['n_cls']:]])
-            o = pre * mult[None, :, None, None]
-            po, HW = geo['point_off'], hh * ww
-            up = torch.cat([plan.gcls[:, po:po + HW, :geo['n_cls']], plan.greg[:, po:po + HW, :geo['n_reg']]], -1)
-            o.backward(up.permute(0, 2, 1).reshape(n, no, hh, ww))
-            note('head dact', L['name'], rel(nhwc(L['dact'], hh, ww, 128), t.grad), 1e-2)
-            L['_exp'] = (Wm.grad, bias.grad, scale_leaf.grad, sc)
-            continue
-        if L['type'] == 'gn':
-            if L['raw'] not in plan._needs_grad:
-                assert 'd_' + L['raw'] not in plan._sizes
-                continue
-            hh, ww, c = geo['H'], geo['W'], geo['Cout']
-            raw = nhwc(L['raw'], hh, ww, c).requires_grad_(True)
-            norm = L['norm']
-            g, b = norm.weight.detach().clone().requires_grad_(True), norm.bias.detach().clone().requires_grad_(True)
-            dact = nhwc('d_' + (L['act'] if L['act'] is not None else L['raw'] + '_act'), hh, ww, c)
-            F.relu(F.group_norm(raw, 16, g, b, norm.eps)).backward(dact)
-            note('gn dz', L['name'], rel(nhwc('d_' + L['raw'], hh, ww, c), raw.grad), 1.2e-2)
-            add_param(norm.weight, g.grad)
-            add_param(norm.bias, b.grad)
-            conv_backward(L, nhwc('d_' + L['raw'], hh, ww, c))
-            n_checked += 1
-            continue
-        if L['y'] not in plan._needs_grad:                  # a train-mode layer with nothing trainable at or upstream of it
-            assert 'd_' + L['y'] not in plan._sizes and 'd_' + L['z'] not in plan._sizes
-            continue
-        ho, wo, c = geo['Ho'], geo['Wo'], geo['Cout']
-        norm = L['norm']
-        z = nhwc(L['z'], ho, wo, c).requires_grad_(True)
-        g, b = norm.weight.detach().clone().requires_grad_(True), norm.bias.detach().clone().requires_grad_(True)
-        if L.get('frozen'):
-            yt = F.batch_norm(z, norm.running_mean[:c], norm.running_var[:c], g[:c], b, training=False, eps=norm.eps)
-        else:
-            yt = F.batch_norm(z, None, None, g, b, training=True, eps=norm.eps)
-        res = None
-        if L['res'] is not None:
-            res = nhwc(L['res'], ho, wo, c).requires_grad_(True)
-            yt = yt + res
-        if L['relu']:
-            yt = F.relu(yt)
-        note('forward bn', L['name'], float((nhwc(L['y'], ho, wo, c) - yt.detach()).abs().max() / yt.detach().abs().max()), 2.0 ** -7)
-        yt.backward(nhwc('d_' + L['y'], ho, wo, c))
-        note('bn dz', L['name'], rel(nhwc('d_' + L['z'], ho, wo, c), z.grad), 1.2e-2)
-        if not L.get('frozen'):
-            add_param(norm.weight, g.grad)
-        add_param(norm.bias, b.grad)
-        if res is not None and L['res'] in plan._needs_grad:
-            exp_grad[L['res']] = exp_grad.get(L['res'], 0) + res.grad
-            shapes[L['res']] = (ho, wo, c)
-        conv_backward(L, nhwc('d_' + L['z'], ho, wo, c))
-        n_checked += 1
-    assert n_checked > 0
-    for name, gexp in exp_grad.items():
-        hh, ww, c = shapes[name]
-        note('dx', name, rel(nhwc('d_' + name, hh, ww, c), gexp), 1.5e-2)
-    head = model._head
-    for L in plan._layers:
-        if L['type'] != 'final':
-            continue
-        Wg, bg, sg, sc = L.pop('_exp')
-        lvl = int(''.join(ch for ch in L['name'].split('fin')[0] if ch.isdigit()))
-        _, _, fin_cls, fin_reg = head.level_paths(lvl)
-        ncls = L['geo']['n_cls']
-        if ncls:
-            add_param(fin_cls.weight, Wg[:ncls].reshape(fin_cls.weight.shape))
-            add_param(fin_cls.bias, bg[:ncls])
-        if L['geo']['n_reg']:
-            add_param(fin_reg.weight, Wg[ncls:].reshape(fin_reg.weight.shape))
-            add_param(fin_reg.bias, bg[ncls:])
-            if head.uses_scale:
-                add_param(head._scales[lvl]._scale, sg / float(sc[ncls]))
-    for name, p in model.named_parameters():
-        if not p.requires_grad:
-            assert p.grad is None, name
-            continue
-        assert id(p) in exp_param, name                     # every trainable parameter is differentiated
-        if float(exp_param[id(p)].norm()) > 1e-12:
-            note('parameter gradient', name, rel(p.grad, exp_param[id(p)].reshape(p.shape)), 5e-3 if p.dim() != 0 else 2e-2)
-    if plan._prefix is not None:
-        pre = {op[k] for _, op in plan._prefix['ops'] for k in ('out', 'out2') if op.get(k) is not None}
-        assert not [s for s in plan._sizes if s.startswith('d_') and any(s.startswith('d_' + q) for q in pre)]
-    return plan
-
-
-@pytest.mark.parametrize('cfg,frozen_stages,shape', [('WIDERFACE_L', 1, (2, 128, 160)), ('WIDERFACE_S', 2, (2, 160, 192)),
-                                                     ('TT100K_L', 'all', (1, 128, 128)), ('TL_L', 2, (2, 128, 160))])
-def test_backward_of_the_trainable_part_teacher_forced(cfg, frozen_stages, shape):
-    model = finetune_model(cfg, frozen_stages)
-    n, h, w = shape
-    x = synth.synth_input(n, h, w).cuda()
-    ann = synth.synth_annotations(n, h, w, model._num_classes, seed=3)
-    plan = _teacher_forced_trainable(model, x, ann)
-    assert plan._prefix is not None
-
-
-def test_backward_with_a_hand_frozen_head_branch_teacher_forced():
-    model, _ = synth_model('TT100K_L', cls_bias=-2.0)
-    model.cuda().train()
-    cls_tower, _, fin_cls, _ = model._head.level_paths(0)
-    for conv, norm in cls_tower:
-        for p in list(conv.parameters()) + list(norm.parameters()):
-            p.requires_grad = False
-    for p in fin_cls.parameters():
-        p.requires_grad = False
-    x = synth.synth_input(1, 128, 128).cuda()
-    ann = synth.synth_annotations(1, 128, 128, model._num_classes, seed=3)
-    plan = _teacher_forced_trainable(model, x, ann)
-    assert plan._prefix is None
 
 
 def _sgd(model, lr=0.02):
@@ -387,7 +215,9 @@ def test_new_prefix_weights_are_repacked_and_unfreezing_differentiates(monkeypat
         p.requires_grad = True
     model.train()
     model._flat_parameters.grad.zero_()
-    plan2 = _teacher_forced_trainable(model, x, ann)
+    replay = Replay(model, x, ann)          # the unfrozen step, every op checked per element (test_gpu_train_step_per_op.py)
+    replay.replay()
+    plan2 = replay.plan
     assert plan2 is not plan and plan2._prefix is None
     stem = model._backbone.stem_layers()[0][0]
     assert stem.weight.grad is not None and float(stem.weight.grad.abs().sum()) > 0

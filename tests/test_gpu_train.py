@@ -73,161 +73,6 @@ def test_native_train_forward_matches_aten(cfg, frozen):
     assert worst < 2.0 * max(worst_emu, 1e-2), (worst, worst_emu)
 
 
-def _teacher_forced_backward_check(cfg, n, h, w):
-    """Gate A/B of the backward: every layer of the native backward plan, fed the tensors the native path itself stored
-    (teacher forced: x, z, y and the incoming gradient dy come from the workspace), must reproduce torch autograd of THAT layer --
-    dz (normalisation + ReLU (+residual) backward), its share of dx (data gradient), its weight gradient, the norm-parameter
-    gradients, and for the head the final-conv / Scale gradients.  ReLU masks are the native ones, so the comparison is free of the
-    mask-flip chaos that dominates any end-to-end gradient comparison of two 16-bit pipelines (see the e2e test below)."""
-    import torch.nn.functional as F
-    model, _ = synth_model(cfg, cls_bias=-2.0)
-    model.cuda().train()
-    x_img = synth.synth_input(n, h, w).cuda()
-    ann = synth.synth_annotations(n, h, w, model._num_classes, seed=3)
-    out = model(x_img)
-    ld = model.get_loss(out, ann)
-    ld['loss'].backward()
-    torch.cuda.synchronize()
-    plan = list(model._train_plans.values())[0]
-    flat = model._flat_parameters
-    bf = lambda t: t.to(torch.bfloat16).float()
-
-    def nhwc(name, hh, ww, c):               # native tensor -> fp32 NCHW
-        return plan.tensor(name, hh, ww, c).float().permute(0, 3, 1, 2).contiguous()
-
-    def rel(a, b):
-        return float((a.double() - b.double()).norm() / b.double().norm().clamp(min=1e-20))
-
-    exp_grad, exp_param, shapes, worst = {}, {}, {}, {}
-
-    def note(kind, name, e, tol):
-        worst[kind] = max(worst.get(kind, (0.0, ''))[0], e), name if e >= worst.get(kind, (0.0, ''))[0] else worst[kind][1]
-        assert e < tol, (cfg, kind, name, e)
-
-    def add_param(p, g):
-        exp_param[id(p)] = exp_param.get(id(p), 0) + g
-
-    def conv_backward(L, dz_native):
-        conv, geo = L['conv'], L['geo']
-        k, s = geo['ksize'], geo['stride']
-        if L['x'] is None:
-            xin = bf(x_img)
-        else:
-            xin = nhwc(L['x'], geo['H'], geo['W'], geo['Cin'])
-        add_param(conv.weight, torch.nn.grad.conv2d_weight(xin, conv.weight.shape, dz_native, stride=s, padding=k // 2))
-        if L['x'] is not None:
-            dx = torch.nn.grad.conv2d_input(xin.shape, bf(conv.weight.detach()), dz_native, stride=s, padding=k // 2)
-            exp_grad[L['x']] = exp_grad.get(L['x'], 0) + dx
-            shapes[L['x']] = (geo['H'], geo['W'], geo['Cin'])
-        # forward of this layer, teacher forced: z = conv(x) on the bf16 operands
-        zname = L['z'] if L['type'] == 'bn' else L['raw']
-        z_exp = F.conv2d(xin, bf(conv.weight.detach()), None, stride=s, padding=k // 2)
-        z_nat = nhwc(zname, geo['Ho'], geo['Wo'], geo['Cout'])
-        note('forward conv', L['name'], float((z_nat - z_exp).abs().max() / z_exp.abs().max().clamp(min=1e-20)), 2.0 ** -7)
-
-    for L in reversed(plan._layers):
-        geo = L['geo']
-        if L['type'] == 'final':
-            hh, ww = geo['H'], geo['W']
-            raw = nhwc(L['raw'], hh, ww, 128)
-            norm = L['norm']
-            if norm is None:               # tower without norm layers: raw is the activated tensor
-                t = raw.clone().requires_grad_(True)
-            else:
-                t = bf(F.relu(F.group_norm(raw, 16, norm.weight.detach(), norm.bias.detach(), norm.eps))).requires_grad_(True)
-            # the convs / Scale of this level, from the staging the native kernel read (bf16-rounded weights)
-            no = geo['n_cls'] + geo['n_reg']
-            off = plan._off[L['stage']]
-            stg = plan.workspace[off:off + (no * 128 + 3 * no) * 4].view(torch.float32)
-            Wm = stg[:no * 128].view(no, 128).clone().requires_grad_(True)
-            sc = stg[no * 128:no * 128 + no].clone()
-            bias = stg[no * 128 + 2 * no:no * 128 + 3 * no].clone().requires_grad_(True)
-            scale_leaf = torch.ones((), device='cuda', requires_grad=True)
-            pre = torch.einsum('nchw,oc->nohw', t, Wm) + bias[None, :, None, None]
-            mult = torch.cat([sc[:geo['n_cls']], scale_leaf * sc[geo['n_cls']:]])      # d/d(Scale) goes through the regression rows
-            o = pre * mult[None, :, None, None]
-            po, HW = geo['point_off'], hh * ww
-            up = torch.cat([plan.gcls[:, po:po + HW, :geo['n_cls']], plan.greg[:, po:po + HW, :geo['n_reg']]], -1)
-            o.backward(up.permute(0, 2, 1).reshape(n, no, hh, ww))
-            dact = nhwc(L['dact'], hh, ww, 128)
-            note('head dact', L['name'], rel(dact, t.grad), 1e-2)
-            L['_exp'] = (Wm.grad, bias.grad, scale_leaf.grad, sc)
-            continue
-        if L['type'] == 'gn':
-            hh, ww, c = geo['H'], geo['W'], geo['Cout']
-            raw = nhwc(L['raw'], hh, ww, c).requires_grad_(True)
-            norm = L['norm']
-            g, b = norm.weight.detach().clone().requires_grad_(True), norm.bias.detach().clone().requires_grad_(True)
-            dact = nhwc('d_' + (L['act'] if L['act'] is not None else L['raw'] + '_act'), hh, ww, c)
-            F.relu(F.group_norm(raw, 16, g, b, norm.eps)).backward(dact)
-            draw = nhwc('d_' + L['raw'], hh, ww, c)
-            note('gn dz', L['name'], rel(draw, raw.grad), 1.2e-2)
-            add_param(norm.weight, g.grad)
-            add_param(norm.bias, b.grad)
-            conv_backward(L, draw)
-            continue
-        ho, wo, c = geo['Ho'], geo['Wo'], geo['Cout']
-        norm = L['norm']
-        z = nhwc(L['z'], ho, wo, c).requires_grad_(True)
-        g, b = norm.weight.detach().clone().requires_grad_(True), norm.bias.detach().clone().requires_grad_(True)
-        if L.get('frozen'):                # conv + bias + ReLU of a no-norm tower, planned as a frozen BatchNorm with constant statistics
-            yt = F.batch_norm(z, norm.running_mean[:c], norm.running_var[:c], g[:c], b, training=False, eps=norm.eps)
-        else:
-            yt = F.batch_norm(z, None, None, g, b, training=True, eps=norm.eps)
-        res = None
-        if L['res'] is not None:
-            res = nhwc(L['res'], ho, wo, c).requires_grad_(True)
-            yt = yt + res
-        if L['relu']:
-            yt = F.relu(yt)
-        y_nat = nhwc(L['y'], ho, wo, c)
-        note('forward bn', L['name'], float((y_nat - yt.detach()).abs().max() / yt.detach().abs().max()), 2.0 ** -7)
-        yt.backward(nhwc('d_' + L['y'], ho, wo, c))
-        dz = nhwc('d_' + L['z'], ho, wo, c)
-        note('bn dz', L['name'], rel(dz, z.grad), 1.2e-2)
-        if not L.get('frozen'):
-            add_param(norm.weight, g.grad)
-        add_param(norm.bias, b.grad)
-        if res is not None:
-            exp_grad[L['res']] = exp_grad.get(L['res'], 0) + res.grad
-            shapes[L['res']] = (ho, wo, c)
-        conv_backward(L, dz)
-    # accumulated data gradients: every consumer's contribution, each computed from the NATIVE dz of that consumer
-    for name, gexp in exp_grad.items():
-        hh, ww, c = shapes[name]
-        note('dx', name, rel(nhwc('d_' + name, hh, ww, c), gexp), 1.5e-2)
-    # head final convs / Scale (the rows of a shared head add up over the levels)
-    head = model._head
-    for L in plan._layers:
-        if L['type'] != 'final':
-            continue
-        Wg, bg, sg, sc = L.pop('_exp')
-        lvl = int(''.join(ch for ch in L['name'].split('fin')[0] if ch.isdigit()))
-        cls_tower, reg_tower, fin_cls, fin_reg = head.level_paths(lvl)
-        ncls = L['geo']['n_cls']
-        if ncls:
-            add_param(fin_cls.weight, Wg[:ncls].reshape(fin_cls.weight.shape))
-            add_param(fin_cls.bias, bg[:ncls])
-        if L['geo']['n_reg']:
-            add_param(fin_reg.weight, Wg[ncls:].reshape(fin_reg.weight.shape))
-            add_param(fin_reg.bias, bg[ncls:])
-            if head.uses_scale:
-                add_param(head._scales[lvl]._scale, sg / float(sc[ncls]))      # d/dScale = d/d(scale_leaf) / Scale
-    for name, p in model.named_parameters():
-        if id(p) not in exp_param:
-            continue
-        e = rel(p.grad, exp_param[id(p)].reshape(p.shape))
-        if float(exp_param[id(p)].norm()) > 1e-12:
-            note('parameter gradient', name, e, 5e-3 if p.dim() != 0 else 2e-2)
-    print('%s teacher-forced backward: %s' % (cfg, {k: '%.1e (%s)' % v for k, v in worst.items()}))
-
-
-@pytest.mark.parametrize('cfg,shape', [('WIDERFACE_XS', (2, 160, 192)), ('WIDERFACE_L', (2, 128, 160)), ('TT100K_S', (2, 160, 160)), ('TT100K_L', (1, 128, 128)),
-                                       ('TL_L', (2, 128, 160)), ('TEST_FAST', (2, 128, 128))])
-def test_native_backward_teacher_forced(cfg, shape):
-    _teacher_forced_backward_check(cfg, *shape)
-
-
 @pytest.mark.parametrize('cfg', ['WIDERFACE_XS', 'WIDERFACE_L'])
 def test_native_parameter_gradients_end_to_end(cfg):
     """loss.backward() through the native backward plan vs autograd over the ATen evaluation, END TO END.  Two 16-bit pipelines whose
@@ -235,7 +80,7 @@ def test_native_parameter_gradients_end_to_end(cfg):
     the gradients of deep layers decorrelate at the 30-50 % level -- for ANY pair of bf16 pipelines: the ATen graph with the native
     rounding points (emulated) differs from ATen fp32 by as much as the native path does.  What is asserted end to end is therefore
     (a) losses agree, (b) the native gradients are as close to the fp32 ones as the emulation is (within 1.5x), (c) the layers next to
-    the loss (final head convs) agree tightly.  The tight, per-layer statement is test_native_backward_teacher_forced."""
+    the loss (final head convs) agree tightly.  The tight, per-element statement is test_gpu_train_step_per_op.py."""
     models = [synth_model(cfg, cls_bias=-2.0)[0].cuda().train() for _ in range(3)]
     n, h, w = 4, 192, 256
     x = synth.synth_input(n, h, w).cuda()

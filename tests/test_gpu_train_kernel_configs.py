@@ -3,8 +3,9 @@
 operands, across their configuration space and under forced small grids (lfd_top.max_ctas 1 and 3) that make every thread walk its
 batched grid-stride loops many times and every head-final-backward block run its cp.async ring through several refills.
 
-Bounds are per element: a 16-bit output must be a faithful rounding of the float64 value widened by K * 2^-24 * S (gpu_ops
-assert_faithful), an fp32 / fp64 result must lie within K * 2^-24 * S (gpu_train_ops assert_within).  S is the sum of the magnitudes
+Bounds are per element: a 16-bit output must be a faithful rounding of the float64 value widened by K * 2^-24 * S (train_op_ref
+check_faithful), an fp32 / fp64 result must lie within K * 2^-24 * S (check_within).  The references and bounds live in train_op_ref.py,
+shared with the op-by-op replay of whole training steps (test_gpu_train_step_per_op.py).  S is the sum of the magnitudes
 of the terms, K the number of fp32 roundings a term can pass through, written next to each assert from the kernel's accumulation:
 passes per thread, warp-shuffle levels, the 8 warp partials of a block, and fp32 atomics."""
 import functools
@@ -13,9 +14,11 @@ import math
 import pytest
 import torch
 
-from gpu_ops import DTYPES, assert_faithful, conv_out, stem_input
-from gpu_train_ops import (Workspace, bf16r, cdiv, desc_table, elementwise_blocks, f32, fma_f32, gn_bwd_blocks, grid_sms, head_bwd_grid,
-                           make_top, mean_rstd_f32, reduce_blocks, run_top, stem_wgrad_grid, assert_within)
+from gpu_ops import DTYPES, conv_out, stem_input
+from gpu_train_ops import (Workspace, bf16r, cdiv, desc_table, elementwise_blocks, gn_bwd_blocks, grid_sms, head_bwd_grid, make_top,
+                           reduce_blocks, run_top, stem_wgrad_grid, assert_within)
+from train_op_ref import (bn_apply_ref, bn_bwd_ref, bn_running_ref, bn_stats_ref, check_amb, check_faithful, check_within, conv_pack_ref,
+                          gn_bwd_ref, head_activation, head_backward_ref, head_forward_ref)
 from lfd import _native as nat
 
 DEV = 'cuda'
@@ -42,15 +45,6 @@ def _bn_grids(C, max_ctas, sms=H100_SMS):
     s = grid_sms(max_ctas, sms)
     return chunks, [('bn_stats', reduce_blocks(chunks, s), 4), ('bn_apply', elementwise_blocks(chunks, s), 4),
                     ('norm_bwd_reduce', reduce_blocks(chunks, s), 2), ('norm_bwd_apply', elementwise_blocks(chunks, s), 2)]
-
-
-def _passes(chunks, blocks):
-    """Most passes any thread makes over a grid-stride loop of `chunks` items."""
-    return cdiv(chunks, blocks * 256)
-
-
-def _shuffle_levels(C):
-    return 5 - int(math.log2(C // 8))      # block_reduce_groups: xor offsets cpr .. 16
 
 
 # (C, relu, res, frozen, cancel): cancel = every other channel has |mean| = 16 std, where E[x^2] - E[x]^2 cancels
@@ -209,44 +203,22 @@ def test_bn_stats_and_apply_match_fp64(case, max_ctas):
     sums, y, rm_got, rv_got = _run_bn(case, max_ctas)
     what = 'BN %s max_ctas=%d' % (_bn_id(case), max_ctas)
     zd = z.double().reshape(M, C)
-    s1, s2, a1 = zd.sum(0), (zd * zd).sum(0), zd.abs().sum(0)
-    # per-thread fp32 chain over its passes, the shuffle levels, the 8 warp partials; the fp64 atomics add no fp32 rounding
-    K_s = _passes(chunks, grids[0][1]) + _shuffle_levels(C) + 8 + 1
-    if frozen:
-        mean, var = rm.double(), rv.double()
-        K_y = 6         # rstd, gamma * rstd, fma shift, fma, + residual, plus one for the float32 running statistics
-    else:
-        assert_within(sums[:, 0], s1, a1, K_s, what + ' sum x')
-        assert_within(sums[:, 1], s2, s2, K_s, what + ' sum x^2')
-        mean = s1 / M
-        var = ((zd - mean) ** 2).sum(0) / M
-        K_y = 2 * K_s + 6      # the statistics' error, moved into rstd at most (E[x^2] + 2 |mean| E|x|) / (2 var) < 2 times (std >= 1, |mean| <= 0.5)
-    sc = gamma.double() / torch.sqrt(var + EPS)
-    ref = (zd - mean) * sc + beta.double()
-    S = (zd.abs() + mean.abs()) * sc.abs() + beta.double().abs()
-    if res:
-        ref, S = ref + r.double().reshape(M, C), S + r.double().abs().reshape(M, C)
-    if relu:
-        ref = ref.clamp(min=0)
+    sums_ref, sums_S, K_s = bn_stats_ref(zd, grids[0][1])
+    if not frozen:
+        check_within(sums, sums_ref, sums_S, K_s, what + ' sums')
+    ref, S, K_y = bn_apply_ref(zd, r.double().reshape(M, C) if res else None, gamma, beta, EPS, relu, frozen, rm, rv, K_s)
     yg = y.reshape(M, C)
-    if cancel:      # the channels with |mean| = 16 std: the bound holds with no allowance for the cancellation; report its margin
+    if cancel:      # the channels with |mean| = 16 std: report the margin of the bound there
         odd = torch.arange(C) % 2 == 1
-        err = (yg.double()[:, odd] - ref[:, odd]).abs()
-        from gpu_ops import ulp16
-        tol = ulp16(ref[:, odd]) + K_y * 2.0 ** -24 * S[:, odd]
-        print('%s: |mean| = 16 std channels: max |err| %.3g, max err / tol %.3g' % (what, float(err.max()), float((err / tol).max())))
-    assert_faithful(yg, ref, S, K_y, 'bf16', what + ' y')
+        m = check_faithful(yg[:, odd], ref[:, odd], S[:, odd], K_y, what + ' y (|mean| = 16 std)')
+        print('%s: |mean| = 16 std channels: max err / tol %.3g' % (what, m))
+    check_faithful(yg, ref, S, K_y, what + ' y')
     if frozen:      # eval-mode BatchNorm: the running statistics are read, never written
         assert torch.equal(rm_got, rm) and torch.equal(rv_got, rv), what
         return
-    # running statistics: (1 - m) r + m stat in float, the unbiased variance for the running estimate
-    var_u = var * M / (M - 1)
-    d_mean = K_s * 2.0 ** -24 * a1 / M
-    d_var = K_s * 2.0 ** -24 * (s2 + 2 * mean.abs() * a1) / M * M / (M - 1)
-    want_m = (1 - MOM) * rm.double() + MOM * mean
-    want_v = (1 - MOM) * rv.double() + MOM * var_u
-    assert_within(rm_got, want_m, (1 - MOM) * rm.double().abs() + MOM * mean.abs() + MOM * d_mean / 2.0 ** -24 / 4, 4, what + ' running_mean')
-    assert_within(rv_got, want_v, (1 - MOM) * rv.double() + MOM * var_u + MOM * d_var / 2.0 ** -24 / 4, 4, what + ' running_var')
+    (want_m, S_m, K_m), (want_v, S_v, K_v) = bn_running_ref(zd, rm, rv, 0.1, K_s)
+    check_within(rm_got, want_m, S_m, K_m, what + ' running_mean')
+    check_within(rv_got, want_v, S_v, K_v, what + ' running_var')
 
 
 # ================================================================================================ norm backward, BatchNorm
@@ -312,33 +284,18 @@ def test_bn_backward_matches_fp64(case, max_ctas):
             5: ws.off('dz'), 6: ws.off('dzu') if up else -1, 7: ws.off('dres') if res else -1}
     _run_norm_bwd(ws, geo, offs, {0: g_d.data_ptr(), 1: b_d.data_ptr(), 2: dg_d.data_ptr(), 3: db_d.data_ptr(), 4: rm_d.data_ptr(), 5: rv_d.data_ptr()})
     what = 'BN backward %s max_ctas=%d' % (_nb_id(case), max_ctas)
-    # the kernel's zhat: float mean / rstd from the statistics, (z - mean) * rstd in fp32
-    if frozen:
-        mean = f32(rm.double())
-        rstd = f32(1.0 / torch.sqrt(rv.double() + float(torch.tensor(EPS, dtype=torch.float32))))
-    else:
-        mean, rstd = mean_rstd_f32(fs[:, 0], fs[:, 1], float(M), EPS)
-    zh = f32(f32(zd.reshape(M, C) - mean) * rstd)
-    gm = dy.double().reshape(M, C) * ((y.reshape(M, C) > 0).double() if relu else 1.0)
-    S1, S2 = gm.sum(0), (gm * zh).sum(0)
-    A1, A2 = gm.abs().sum(0), (gm * zh).abs().sum(0)
-    ga = gamma.double()
-    K_r = _passes(chunks, grids[2][1]) + _shuffle_levels(C) + 8 + 1
-    if frozen:
-        ref, S = ga * rstd * gm, (ga * rstd * gm).abs()
-    else:
-        ref = ga * rstd * (gm - (S1 / M + zh * S2 / M))
-        S = (ga * rstd).abs() * (gm.abs() + (A1 + zh.abs() * A2) / M)
+    r = bn_bwd_ref(zd.reshape(M, C), dy.double().reshape(M, C), y.double().reshape(M, C), fs, gamma, EPS, relu, frozen, rm, rv, grids[2][1])
+    gm = r['g']
     dz = ws.get('dz').cpu()
-    assert_faithful(dz.reshape(M, C), ref, S, K_r + 6, 'bf16', what + ' dz')     # sums (K_r), S / M, zh * S2 / M + S1 / M, g - ., gamma * rstd, *
-    # parameter gradients: the reduce's sums, cast to float and added by one block (+1), zhat within 2 fp32 roundings of ours (+2)
-    assert_within(dg_d, S2, A2, K_r + 3, what + ' dgamma')
-    assert_within(db_d, S1, A1, K_r + 1, what + ' dbeta')
+    check_faithful(dz.reshape(M, C), *r['dz'], what=what + ' dz')
+    check_within(ws.get('bsums').cpu(), *r['bsums'], what=what + ' sums')
+    check_within(dg_d, *r['dgamma'], what=what + ' dgamma')
+    check_within(db_d, *r['dbeta'], what=what + ' dbeta')
     if res:
         got = ws.get('dres').cpu().reshape(M, C)
         if acc:
             want = gm + prev.double().reshape(M, C)
-            assert_faithful(got, want, gm.abs() + prev.double().abs().reshape(M, C), 1, 'bf16', what + ' dres')    # prev + g, one fp32 add
+            check_faithful(got, want, gm.abs() + prev.double().abs().reshape(M, C), 1, what + ' dres')    # prev + g, one fp32 add
         else:
             assert torch.equal(got.double(), gm), what + ' dres'
     if up:
@@ -388,22 +345,14 @@ def test_gn_backward_matches_fp64(case, max_ctas):
     offs = {0: ws.off('dy'), 2: ws.off('z'), 3: ws.off('fsums'), 4: ws.off('bsums'), 5: ws.off('dz')}
     _run_norm_bwd(ws, geo, offs, {0: g_d.data_ptr(), 1: b_d.data_ptr(), 2: dg_d.data_ptr(), 3: db_d.data_ptr()})
     what = 'GN backward %s max_ctas=%d' % ('g%d_N%d_%dx%d' % case, max_ctas)
-    Mg = HW * 8
-    mean, rstd = mean_rstd_f32(fs[..., 0], fs[..., 1], float(Mg), EPS)
-    mean, rstd = mean.reshape(N, 1, G, 1), rstd.reshape(N, 1, G, 1)
-    zh = f32(f32(zd - mean) * rstd)
-    ga, be = gamma.double().reshape(G, 8), beta.double().reshape(G, 8)
-    on = fma_f32(zh, ga, be) > 0                                           # the kernel's ReLU mask, recomputed exactly
-    gm = dy.double().reshape(N, HW, G, 8) * on.double()
-    T1, T2 = (gm * ga).sum((1, 3), keepdim=True), (gm * ga * zh).sum((1, 3), keepdim=True)
-    A1, A2 = (gm * ga).abs().sum((1, 3), keepdim=True), (gm * ga * zh).abs().sum((1, 3), keepdim=True)
-    ref = rstd * (gm * ga - (T1 / Mg + zh * T2 / Mg))
-    S = rstd * ((gm * ga).abs() + (A1 + zh.abs() * A2) / Mg)
-    K_r = _passes(HW * G, blocks) + _shuffle_levels(C) + 8 + 2        # + the g * gamma product
-    assert_faithful(ws.get('dz').cpu().reshape(N, HW, G, 8), ref, S, K_r + 6, 'bf16', what + ' dz')
-    dgam, dbet = (gm * zh).sum((0, 1)).reshape(C), gm.sum((0, 1)).reshape(C)
-    assert_within(dg_d, dgam, (gm * zh).abs().sum((0, 1)).reshape(C), K_r + 1, what + ' dgamma')
-    assert_within(db_d, dbet, gm.abs().sum((0, 1)).reshape(C), K_r + 1, what + ' dbeta')
+    r = gn_bwd_ref(zd, dy.double().reshape(N, HW, G, 8), fs, gamma, beta, EPS, blocks)
+    check_amb(r['amb'], what)
+    check_faithful(ws.get('dz').cpu().reshape(N, HW, G, 8), *r['dz'], what=what + ' dz')
+    bs = ws.get('bsums').cpu()
+    check_within(bs[:C * 2].view(C, 2), *r['bsums'][0], what=what + ' channel sums')
+    check_within(bs[C * 2:].view(N, G, 2), *r['bsums'][1], what=what + ' group sums')
+    check_within(dg_d, *r['dgamma'], what=what + ' dgamma')
+    check_within(db_d, *r['dbeta'], what=what + ' dbeta')
 
 
 # ================================================================================================ head final, forward and backward
@@ -432,34 +381,18 @@ def _head_operands(case, dtype='bf16'):
 
 
 def _head_activation(raw, gamma, beta, stats, groups, dtype='bf16'):
-    """a = round16(relu(fmaf((x - mean) * rstd, gamma, beta))) exactly as the kernels form it (rounding point Rg), float64."""
-    N, HW, C = raw.shape
-    rnd = DTYPES[dtype][1]
-    x = raw.double().reshape(N, HW, 16, 8)
-    if not groups:
-        return rnd(x.clamp(min=0).float()).double().reshape(N, HW, C)
-    mean, rstd = mean_rstd_f32(stats[..., 0], stats[..., 1], float(HW * 8), EPS)
-    zh = f32(f32(x - mean.reshape(N, 1, 16, 1)) * rstd.reshape(N, 1, 16, 1))
-    y = fma_f32(zh, gamma.double().reshape(16, 8), beta.double().reshape(16, 8)).clamp(min=0)
-    return rnd(y.float()).double().reshape(N, HW, C)
-
-
-def _head_forward_ref(a, w, scale, shift):
-    """out = scale * (W . a) + shift: float64 and the sum of |terms|.  K = 16 fp32 fmas per channel slice + 3 shuffle adds + 1 fma."""
-    wd = w.double()
-    ref = (a @ wd.t()) * scale.double() + shift.double()
-    S = (a.abs() @ wd.abs().t()) * scale.double().abs() + shift.double().abs()
-    return ref, S, 20
+    """-> (a, a_other, amb) of train_op_ref.head_activation on the case's GroupNorm(16, 128)."""
+    return head_activation(raw, gamma, beta, stats, 16 if groups else 0, EPS, dtype)
 
 
 def _check_head_outputs(cls_o, reg_o, ref, S, K, nc, point_off, HW, what):
     sl = slice(point_off, point_off + HW)
     if nc:
-        assert_within(cls_o[:, sl, :nc], ref[..., :nc], S[..., :nc], K, what + ' cls')
+        check_within(cls_o[:, sl, :nc], ref[..., :nc], S[..., :nc], K, what + ' cls')
         assert bool(torch.isnan(cls_o[:, sl, nc:]).all()), what + ': cls channels past n_cls written'
         assert bool(torch.isnan(cls_o[:, :point_off]).all() and torch.isnan(cls_o[:, point_off + HW:]).all()), what + ': cls rows outside the level written'
     if ref.shape[-1] > nc:
-        assert_within(reg_o[:, sl], ref[..., nc:], S[..., nc:], K, what + ' reg')
+        check_within(reg_o[:, sl], ref[..., nc:], S[..., nc:], K, what + ' reg')
         assert bool(torch.isnan(reg_o[:, :point_off]).all() and torch.isnan(reg_o[:, point_off + HW:]).all()), what + ': reg rows outside the level written'
 
 
@@ -493,33 +426,19 @@ def test_head_final_forward_and_backward_match_fp64(case, max_ctas):
                                                  5: ws.off('dstage'), 6: ws.off('dscale')},
                      ptr={**nptr, 2: gcls_d.data_ptr(), 3: greg_d.data_ptr()}, **geo), ws)
     what = 'head final %s max_ctas=%d' % (_head_id(case), max_ctas)
-    a = _head_activation(raw, gamma, beta, stats, groups)
-    ref, S, K = _head_forward_ref(a, w, scale, shift)
+    a, a_b, amb = _head_activation(raw, gamma, beta, stats, groups)
+    check_amb(amb, what)
+    ref, S, K = head_forward_ref(a, a_b, w, scale, shift)
     _check_head_outputs(cls_o.cpu(), reg_o.cpu(), ref, S, K, nc, point_off, HW, what)
     # backward: h_o = g_o * scale_o (one rounding); dact = sum_o h_o W_o; dW = sum_pix h a; db = sum_pix h; dScale = sum g (W . a + b)
     up = torch.cat([gcls[:, point_off:point_off + HW, :nc], greg[:, point_off:point_off + HW, :nr]], -1).double()     # [N][HW][no]
-    h = up * scale.double()
-    wd = w.double()
-    assert_faithful(ws.get('dact').cpu(), h @ wd, h.abs() @ wd.abs(), no + 1, 'bf16', what + ' dact')
-    small = no <= 5
-    ppt = 2 if small else 4                  # pixels per thread per tile
-    n_atom = bx * N                          # fp32 atomics onto the staging, one per block
-    if small:       # registers over all tiles, 2 shuffles, 8 warp partials through shared memory
-        K_w, K_b = 1 + (ppt + 1) * T + 2 + 8 + n_atom, 1 + ppt + T + 2 + 8 + n_atom
-        K_sc = 16 + 3 + 2 + 2 * ppt * T * 2 + 2 + 8 + n_atom
-    else:           # per tile: 4-pixel sums, 2 shuffles, one shared-memory atomic per warp (8 per tile)
-        K_w = K_b = 1 + ppt + 2 + 8 * T + n_atom
-        K_sc = 16 + 3 + 2 + nr * ppt * T + 32 + n_atom       # 32 slice-0 threads add into one shared float
+    r = head_backward_ref(a, a_b, up, w, scale, bias, nc, bx, tiles, N)
+    check_faithful(ws.get('dact').cpu(), *r['dact'], what=what + ' dact')
     ds = ws.get('dstage').cpu()
-    hf = h.reshape(-1, no)
-    af = a.reshape(-1, C)
-    assert_within(ds[:no * C].view(no, C), hf.t() @ af, hf.abs().t() @ af.abs(), K_w, what + ' dW')
-    assert_within(ds[no * C:], hf.sum(0), hf.abs().sum(0), K_b, what + ' dbias')
+    check_within(ds[:no * C].view(no, C), *r['dW'], what=what + ' dW')
+    check_within(ds[no * C:], *r['dbias'], what=what + ' dbias')
     if nr:
-        u = (af @ wd[nc:].t() + bias.double()[nc:])                        # [pix][n_reg]: W . a + b
-        ur = up.reshape(-1, no)[:, nc:]
-        Su = af.abs() @ wd[nc:].abs().t() + bias.double()[nc:].abs()
-        assert_within(ws.get('dscale').cpu(), (ur * u).sum().reshape(1), (ur.abs() * Su).sum().reshape(1), K_sc, what + ' dScale')
+        check_within(ws.get('dscale').cpu(), *r['dscale'], what=what + ' dScale')
     else:
         assert float(ws.get('dscale').cpu()[0]) == 0.0
 
@@ -549,9 +468,10 @@ def test_inference_gn_apply_matches_fp64(dtype):
     op.in_off, op.out_off, op.stats_off, op.res_off, op.ds_out_off = ws.off('in'), ws.off('out'), ws.off('stats'), -1, -1
     op.gamma, op.beta, op.max_ctas = g_d.data_ptr(), b_d.data_ptr(), 1
     _run_op(op, ws)
-    a = _head_activation(x, gamma, beta, stats, 16, dtype)
+    a, a_b, amb = _head_activation(x, gamma, beta, stats, 16, dtype)
     got = ws.get('out').cpu().double()
-    assert torch.equal(got, a), '%s GN apply: %d elements differ from the exact emulation' % (dtype, int((got != a).sum()))
+    bad = (got != a) & (got != a_b)
+    assert not bool(bad.any()), '%s GN apply: %d elements differ from the exact emulation' % (dtype, int(bad.sum()))
 
 
 def _run_op(op, ws, cls=None, reg=None, P=0, cls_channels=0):
@@ -586,8 +506,8 @@ def test_inference_head_final_matches_fp64(case, dtype):
     if groups:
         op.gamma, op.beta = g_d.data_ptr(), b_d.data_ptr()
     _run_op(op, ws, cls_o, reg_o, P, cls_stride)
-    a = _head_activation(raw, gamma, beta, stats, groups, dtype)
-    ref, S, K = _head_forward_ref(a, w, scale, shift)
+    a, a_b, _ = _head_activation(raw, gamma, beta, stats, groups, dtype)
+    ref, S, K = head_forward_ref(a, a_b, w, scale, shift)
     _check_head_outputs(cls_o.cpu(), reg_o.cpu(), ref, S, K, nc, point_off, HW, 'inference head final %s %s' % (_head_id(case), dtype))
 
 
@@ -623,23 +543,6 @@ def _shipped_pack_configs():
     return fwd, dgrad
 
 
-def _conv_pack_ref(w, cc, dgrad):
-    """Index formula of the packed operand [Kin/cc][k*k][cc/8][Nout][8]: forward Kin = Cin, Nout = Cout, W[n][kch][tap]; data
-    gradient Kin = Cout, Nout = Cin, W[kch][n][k*k - 1 - tap]."""
-    Cout, Cin, k, _ = w.shape
-    kk = k * k
-    nout = Cin if dgrad else Cout
-    idx = torch.arange(w.numel())
-    j, r = idx % 8, idx // 8
-    n, r = r % nout, r // nout
-    kc, r = r % (cc // 8), r // (cc // 8)
-    tap, c = r % kk, r // kk
-    kch = c * cc + kc * 8 + j
-    wf = w.reshape(-1)
-    v = wf[(kch * Cin + n) * kk + (kk - 1 - tap)] if dgrad else wf[(n * Cin + kch) * kk + tap]
-    return v.to(torch.bfloat16)
-
-
 @pytest.mark.gpu
 def test_pack_table_matches_index_formulas():
     """One PACK table with every kind and entries of very different n: each entry writes exactly its n elements."""
@@ -659,7 +562,7 @@ def test_pack_table_matches_index_formulas():
             keep.append(wd)
             descs.append(nat.PackDesc(kind=nat.PACK_CONV_DGRAD if dgrad else nat.PACK_CONV_FWD, Cout=co, Cin=ci, k=k, cc=cc, n=w.numel(),
                                       src=wd.data_ptr(), dst=o.data_ptr()))
-            want = _conv_pack_ref(w, cc, dgrad)
+            want = conv_pack_ref(w, cc, dgrad)
             if not dgrad:
                 assert torch.equal(want, pack_conv_weight(w, cc).reshape(-1))
             checks.append(('%s %s' % ('dgrad' if dgrad else 'fwd', (ci, co, k, cc)), o, want))
