@@ -52,7 +52,8 @@ typedef struct lfd_plan lfd_plan;
 
 int lfd_abi_version(void);
 /* sizeof of the structs of this header as the library was compiled, for bindings that mirror them field by field (ctypes, cffi):
- * which = 0 lfd_op, 1 lfd_top, 2 lfd_pack_desc, 3 lfd_unpack_desc, 4 lfd_post_cfg, 5 lfd_loss_cfg, 6 lfd_levels, 7 lfd_input_desc;
+ * which = 0 lfd_op, 1 lfd_top, 2 lfd_pack_desc, 3 lfd_unpack_desc, 4 lfd_post_cfg, 5 lfd_loss_cfg, 6 lfd_levels, 7 lfd_input_desc,
+ * 8 lfd_extent;
  * -1 for anything else. */
 int lfd_struct_bytes(int which);
 const char* lfd_last_error(void);
@@ -151,6 +152,25 @@ int lfd_plan_num_launches(const lfd_plan* plan); /* kernels launched per forward
  * CUDA graph on first use for this (input, workspace, cls_out, reg_out) tuple and replayed afterwards. */
 int lfd_plan_forward(lfd_plan* plan, const void* input, int input_format, void* workspace, float* cls_out, float* reg_out,
                      int use_graph, lfd_stream stream);
+/* Frames smaller than the plan: the plan's (N, H, W) is its capacity, and a frame of h <= H rows and w <= W columns runs on the same
+ * kernels, workspace and CUDA graph.  Every tensor keeps the plan's layout (row pitch = the plan's width of that tensor) with the valid
+ * h x w region, and its successors, in the top-left corner; nothing outside it is read.  ext[n_ops] (host) gives per op the valid
+ * input H x W and output Ho x Wo, and for HEAD_FINAL the level's first point and the frame's point count P (0 for the other ops), exactly
+ * the fields of a plan built for the frame.  The table is copied, stream-ordered, into a device table that the kernels read when they
+ * start.  `input` holds the frame in the capacity layout: uint8 [N][H][W][3] or float32 [N][3][H][W] with the frame in the top-left
+ * corner.  cls_out / reg_out receive the frame's outputs as a plan built for it lays them out: float[N][P][cls_channels] and
+ * float[N][P][4] at the start of the buffers.  h == H and w == W is lfd_plan_forward (ext is not read).  A frame outside the capacity
+ * or an inconsistent table fails with LFD_ERR_INVALID before anything is enqueued; the SIMT cross-check path runs full-size frames only
+ * (LFD_ERR_UNSUPPORTED).  use_graph: one graph per pointer tuple as in lfd_plan_forward, shared by every frame size. */
+typedef struct lfd_extent {
+    int32_t H, W, Ho, Wo;
+    int32_t point_off, P;
+    int32_t pad_[2];
+} lfd_extent;
+int lfd_plan_forward_extent(lfd_plan* plan, const void* input, int input_format, int h, int w, const lfd_extent* ext, void* workspace,
+                            float* cls_out, float* reg_out, int use_graph, lfd_stream stream);
+/* CUDA graphs the plan holds instantiated (tests) */
+int lfd_plan_num_graphs(const lfd_plan* plan);
 /* One eager forward with a CUDA event pair around every op: ms_per_op float[lfd_plan_num_launches()] (host).
  * Synchronises the stream.  Used by bench.py for the live per-kernel roofline. */
 int lfd_plan_profile(lfd_plan* plan, const void* input, int input_format, void* workspace, float* cls_out, float* reg_out,

@@ -31,7 +31,8 @@ def _stale():
 
 
 # conv_umma_kernel<MODE_3X3S2, 128>: the only instantiation with two 128-column accumulators (conv + fused shortcut); it spills part of them
-_STACK_EXEMPT = {'_ZN3lfd16conv_umma_kernelILi2ELi128ELb0EEEvNS_14UmmaConvParamsE': 512, '_ZN3lfd16conv_umma_kernelILi2ELi128ELb1EEEvNS_14UmmaConvParamsE': 512}
+# (the last template argument: the launch reads a geometry table, lfd_plan_forward_extent)
+_STACK_EXEMPT = {'_ZN3lfd16conv_umma_kernelILi2ELi128ELb%dELb%dEEEvNS_14UmmaConvParamsE' % (f16, ext): 512 for f16 in (0, 1) for ext in (0, 1)}
 # kernels whose per-thread state must stay in registers (the soft-NMS kernel runs one iteration per candidate: a spill is paid K times)
 _STACK_GUARDED = ('conv_umma_kernel', 'stem4_kernel', 'soft_nms_kernel')
 _PTXAS_VERBOSE = ('conv_umma.cu', 'postprocess.cu')

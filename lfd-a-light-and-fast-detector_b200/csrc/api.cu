@@ -80,8 +80,9 @@ struct BranchExecutor {
         float* cls;
         float* reg;
         int fmt;
+        const void* ext;
     };
-    std::vector<Graph> graphs;             // one instantiated graph per (input, workspace, cls, reg, format) tuple, oldest first
+    std::vector<Graph> graphs;             // one instantiated graph per (input, workspace, cls, reg, format, geometry table) tuple, oldest first
 
     BranchExecutor() = default;
     BranchExecutor(const BranchExecutor&) = delete;
@@ -166,11 +167,11 @@ struct BranchExecutor {
     }
 
     template <typename Launch>
-    int run(const void* input, int fmt, void* workspace, float* cls, float* reg, int use_graph, cudaStream_t st, Launch launch) {
+    int run(const void* input, int fmt, void* workspace, float* cls, float* reg, const void* ext, int use_graph, cudaStream_t st, Launch launch) {
         uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
         if (!use_graph) return enqueue(ws, st, launch);
         for (auto& g : graphs)
-            if (g.input == input && g.ws == workspace && g.cls == cls && g.reg == reg && g.fmt == fmt) {
+            if (g.input == input && g.ws == workspace && g.cls == cls && g.reg == reg && g.fmt == fmt && g.ext == ext) {
                 CUDA_TRY(cudaGraphLaunch(g.exec, st));
                 return LFD_OK;
             }
@@ -195,7 +196,7 @@ struct BranchExecutor {
             cudaStreamDestroy(cap);
             return rc ? rc : fail(LFD_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(ce));
         }
-        Graph e = {nullptr, input, workspace, cls, reg, fmt};
+        Graph e = {nullptr, input, workspace, cls, reg, fmt, ext};
         ce = cudaGraphInstantiate(&e.exec, graph, 0);
         cudaGraphDestroy(graph);
         cudaStreamDestroy(cap);
@@ -247,6 +248,7 @@ extern "C" int lfd_struct_bytes(int which) {
         case 5: return (int)sizeof(lfd_loss_cfg);
         case 6: return (int)sizeof(lfd_levels);
         case 7: return (int)sizeof(lfd_input_desc);
+        case 8: return (int)sizeof(lfd_extent);
     }
     return -1;
 }
@@ -358,10 +360,13 @@ static int plan_op(const lfd_op& o, PlannedOp* out) {
     return LFD_OK;
 }
 
+// ext: null, or this op's row of a plan's device geometry table (lfd_plan_forward_extent), which the kernel reads when it starts
 static int launch_op(const PlannedOp& po, size_t index, const void* input, int input_format, uint8_t* ws, float* cls, float* reg, int P,
-                     int cls_channels, int conv_impl, cudaStream_t st) {
+                     int cls_channels, int conv_impl, cudaStream_t st, const lfd_extent* ext = nullptr) {
     const lfd_op& o = po.op;
     unsigned long long* tl = g_timeline ? g_timeline + 2 * index : nullptr;
+    const int* ext_row = ext ? &ext->H : nullptr;
+    if (ext && conv_impl == LFD_CONV_SIMT) return fail(LFD_ERR_UNSUPPORTED, "the SIMT cross-check kernels run full-size frames only");
     switch (o.kind) {
         case LFD_OP_STEM0: {
             if (!input) return fail(LFD_ERR_INVALID, "stem0 needs the external input pointer");
@@ -379,6 +384,7 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
                 p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift; p.stats = nullptr;
                 p.relu = o.relu; p.gn_groups = 0; p.trace = g_trace; p.tl = tl; p.f16 = o.dtype;
                 p.w2 = reinterpret_cast<const __nv_bfloat16*>(o.tail_weight); p.shift2 = o.tail_shift; p.relu2 = o.tail_relu;
+                p.ext = ext_row;
                 if (umma_conv_encode_maps(&p)) return fail(LFD_ERR_CUDA, "cuTensorMapEncodeTiled failed for the stem conv");
                 CUDA_TRY(umma_conv_launch(p, po.smem, po.grid, st));
             }
@@ -395,7 +401,7 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
             p.w2 = reinterpret_cast<const __nv_bfloat16*>(o.tail_weight); p.shift2 = o.tail_shift; p.relu2 = o.tail_relu;
             p.w_s2 = reinterpret_cast<const __nv_bfloat16*>(o.s2_weight); p.shift_s2 = o.s2_shift; p.relu_s2 = o.s2_relu;
             p.w_s3 = reinterpret_cast<const __nv_bfloat16*>(o.s3_weight); p.shift_s3 = o.s3_shift; p.relu_s3 = o.s3_relu;
-            p.gn_groups = 0; p.trace = g_trace; p.tl = tl; p.f16 = o.dtype;
+            p.gn_groups = 0; p.trace = g_trace; p.tl = tl; p.f16 = o.dtype; p.ext = ext_row;
             if (umma_conv_encode_maps(&p)) return fail(LFD_ERR_CUDA, "cuTensorMapEncodeTiled failed for the fused stem");
             CUDA_TRY(umma_conv_launch(p, po.smem, po.grid, st));
             break;
@@ -418,7 +424,7 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
                     p.w2 = reinterpret_cast<const __nv_bfloat16*>(o.ds_weight); p.shift2 = o.ds_shift; p.relu2 = 0;
                     p.out3 = reinterpret_cast<__nv_bfloat16*>(ws + o.ds_out_off);
                 }
-                p.trace = g_trace; p.tl = tl;
+                p.trace = g_trace; p.tl = tl; p.ext = ext_row;
                 if (umma_conv_encode_maps(&p)) return fail(LFD_ERR_CUDA, "cuTensorMapEncodeTiled failed for conv %dx%d Cf=%d", o.ksize, o.ksize, p.Cf);
                 CUDA_TRY(umma_conv_launch(p, po.smem, po.grid, st));
             }
@@ -429,6 +435,7 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
             p.in = reinterpret_cast<const __nv_bfloat16*>(ws + o.in_off); p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off);
             p.stats = reinterpret_cast<const double*>(ws + o.stats_off); p.gamma = o.gamma; p.beta = o.beta;
             p.N = o.N; p.HW = o.H * o.W; p.C = o.Cin; p.groups = o.gn_groups; p.eps = 1e-5f; p.tl = tl; p.f16 = o.dtype;
+            p.ext = ext_row; p.W = o.W;
             CUDA_TRY(gn_apply_launch(p, bounded_sms(o.max_ctas), st));
             break;
         }
@@ -440,6 +447,7 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
             p.cls = o.n_cls ? cls : nullptr; p.reg = o.n_reg ? reg : nullptr;
             p.N = o.N; p.HW = o.H * o.W; p.C = o.Cin; p.groups = o.gn_groups; p.n_out = o.n_cls + o.n_reg; p.n_cls = o.n_cls;
             p.P = P; p.point_off = o.point_off; p.cls_stride = cls_channels; p.eps = 1e-5f; p.tl = tl; p.f16 = o.dtype;
+            p.ext = ext_row; p.W = o.W;
             if ((o.n_cls && !cls) || (o.n_reg && !reg)) return fail(LFD_ERR_INVALID, "head_final needs cls/reg output pointers");
             if (o.n_reg && o.n_reg != 4) return fail(LFD_ERR_INVALID, "head_final n_reg must be 0 or 4");
             CUDA_TRY(head_final_launch(p, bounded_sms(o.max_ctas), st));
@@ -453,10 +461,25 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
 static constexpr size_t kMaxInferenceGraphs = 32;
 static constexpr size_t kMaxTrainingGraphs = 8;
 
+// Host staging of the geometry table: a frame's table is written into the next slot of a ring of pinned buffers and copied to the device
+// table on the caller's stream; a slot is rewritten only after the event recorded behind its last copy has completed.
+static constexpr int kExtentRing = 4;
+
 struct lfd_plan {
     std::vector<PlannedOp> ops;
     int P, cls_channels, conv_impl;
     BranchExecutor ex;   // the GroupNorm statistics region is its clear region
+    // lfd_plan_forward_extent, allocated on its first call: the device geometry table (one lfd_extent per op), its pinned staging ring
+    lfd_extent* ext_dev = nullptr;
+    lfd_extent* ext_host = nullptr;      // [kExtentRing][ops]
+    cudaEvent_t ext_ev[kExtentRing] = {};
+    int ext_slot = 0;
+    ~lfd_plan() {
+        for (auto ev : ext_ev)
+            if (ev) cudaEventDestroy(ev);
+        if (ext_dev) cudaFree(ext_dev);
+        if (ext_host) cudaFreeHost(ext_host);
+    }
 };
 
 extern "C" int lfd_plan_create(const lfd_op* ops, int n_ops, int N, int P, int cls_channels, int64_t stats_off, int64_t stats_bytes,
@@ -486,10 +509,68 @@ extern "C" int lfd_plan_forward(lfd_plan* pl, const void* input, int input_forma
                                 int use_graph, lfd_stream stream) {
     if (!pl || !input || !workspace || !cls_out || !reg_out) return fail(LFD_ERR_INVALID, "lfd_plan_forward: null argument");
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    return pl->ex.run(input, input_format, workspace, cls_out, reg_out, use_graph, st_of(stream), [&](size_t i, cudaStream_t s) {
+    return pl->ex.run(input, input_format, workspace, cls_out, reg_out, nullptr, use_graph, st_of(stream), [&](size_t i, cudaStream_t s) {
         return launch_op(pl->ops[i], i, input, input_format, ws, cls_out, reg_out, pl->P, pl->cls_channels, pl->conv_impl, s);
     });
 }
+
+// A frame's table must describe the plan's own op list at no more than its capacity: every extent within the op's, the image op at h x w, and
+// the head outputs inside the frame's P <= the plan's P
+static int check_extent(const lfd_plan* pl, int h, int w, const lfd_extent* ext) {
+    const int n = (int)pl->ops.size();
+    int P = -1;
+    for (int i = 0; i < n; ++i) {
+        const lfd_op& o = pl->ops[i].op;
+        const lfd_extent& e = ext[i];
+        if (e.H < 1 || e.W < 1 || e.Ho < 1 || e.Wo < 1 || e.H > o.H || e.W > o.W || e.Ho > o.Ho || e.Wo > o.Wo)
+            return fail(LFD_ERR_INVALID, "lfd_plan_forward_extent: op %d: extent %dx%d -> %dx%d outside the plan's %dx%d -> %dx%d", i, e.H, e.W, e.Ho,
+                        e.Wo, o.H, o.W, o.Ho, o.Wo);
+        if ((o.kind == LFD_OP_STEM0 || o.kind == LFD_OP_STEM4) && (e.H != h || e.W != w))
+            return fail(LFD_ERR_INVALID, "lfd_plan_forward_extent: the image op's extent %dx%d is not the frame's %dx%d", e.H, e.W, h, w);
+        if (o.kind == LFD_OP_HEAD_FINAL) {
+            if (P < 0) P = e.P;
+            if (e.P != P || P > pl->P || e.point_off < 0 || (int64_t)e.point_off + (int64_t)e.H * e.W > P)
+                return fail(LFD_ERR_INVALID, "lfd_plan_forward_extent: op %d: points [%d, %d + %d x %d) outside the frame's %d (plan: %d)", i, e.point_off,
+                            e.point_off, e.H, e.W, e.P, pl->P);
+        }
+    }
+    return LFD_OK;
+}
+
+extern "C" int lfd_plan_forward_extent(lfd_plan* pl, const void* input, int input_format, int h, int w, const lfd_extent* ext, void* workspace,
+                                       float* cls_out, float* reg_out, int use_graph, lfd_stream stream) {
+    if (!pl || !input || !workspace || !cls_out || !reg_out) return fail(LFD_ERR_INVALID, "lfd_plan_forward_extent: null argument");
+    const lfd_op& img = pl->ops[0].op;
+    if (img.kind != LFD_OP_STEM0 && img.kind != LFD_OP_STEM4) return fail(LFD_ERR_INVALID, "lfd_plan_forward_extent: the plan does not start on the image");
+    if (h < 1 || w < 1 || h > img.H || w > img.W)
+        return fail(LFD_ERR_INVALID, "lfd_plan_forward_extent: frame %dx%d outside the plan's capacity %dx%d", h, w, img.H, img.W);
+    if (h == img.H && w == img.W) return lfd_plan_forward(pl, input, input_format, workspace, cls_out, reg_out, use_graph, stream);
+    if (pl->conv_impl == LFD_CONV_SIMT) return fail(LFD_ERR_UNSUPPORTED, "lfd_plan_forward_extent: the SIMT cross-check kernels run full-size frames only");
+    if (!ext) return fail(LFD_ERR_INVALID, "lfd_plan_forward_extent: a frame below the capacity needs its geometry table");
+    int rc = check_extent(pl, h, w, ext);
+    if (rc) return rc;
+    const size_t n = pl->ops.size(), bytes = n * sizeof(lfd_extent);
+    if (!pl->ext_ev[kExtentRing - 1]) {
+        if (!pl->ext_dev) CUDA_TRY(cudaMalloc(&pl->ext_dev, bytes));
+        if (!pl->ext_host) CUDA_TRY(cudaHostAlloc(&pl->ext_host, kExtentRing * bytes, cudaHostAllocDefault));
+        for (auto& ev : pl->ext_ev)
+            if (!ev) CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    }
+    cudaStream_t st = st_of(stream);
+    const int slot = pl->ext_slot;
+    pl->ext_slot = (slot + 1) % kExtentRing;
+    CUDA_TRY(cudaEventSynchronize(pl->ext_ev[slot]));   // the copy that last read this slot has been performed
+    lfd_extent* host = pl->ext_host + slot * n;
+    memcpy(host, ext, bytes);
+    CUDA_TRY(cudaMemcpyAsync(pl->ext_dev, host, bytes, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaEventRecord(pl->ext_ev[slot], st));
+    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+    return pl->ex.run(input, input_format, workspace, cls_out, reg_out, pl->ext_dev, use_graph, st, [&](size_t i, cudaStream_t s) {
+        return launch_op(pl->ops[i], i, input, input_format, ws, cls_out, reg_out, pl->P, pl->cls_channels, pl->conv_impl, s, pl->ext_dev + i);
+    });
+}
+
+extern "C" int lfd_plan_num_graphs(const lfd_plan* plan) { return plan ? (int)plan->ex.graphs.size() : 0; }
 
 extern "C" int lfd_plan_profile(lfd_plan* pl, const void* input, int input_format, void* workspace, float* cls_out, float* reg_out,
                                 float* ms_per_op, lfd_stream stream) {
@@ -1014,7 +1095,7 @@ extern "C" int lfd_train_plan_num_ops(const lfd_train_plan* plan) { return plan 
 extern "C" int lfd_train_plan_run(lfd_train_plan* pl, const void* input, int input_format, void* workspace, int use_graph, lfd_stream stream) {
     if (!pl || !workspace) return fail(LFD_ERR_INVALID, "lfd_train_plan_run: null argument");
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    return pl->ex.run(input, input_format, workspace, nullptr, nullptr, use_graph, st_of(stream), [&](size_t i, cudaStream_t s) {
+    return pl->ex.run(input, input_format, workspace, nullptr, nullptr, nullptr, use_graph, st_of(stream), [&](size_t i, cudaStream_t s) {
         return launch_top(pl->ops[i], input, input_format, ws, s);
     });
 }

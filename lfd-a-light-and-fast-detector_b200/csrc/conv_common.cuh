@@ -71,6 +71,10 @@ struct alignas(64) UmmaConvParams {
     const float* shift_s3;
     int relu_s2, relu_s3, H1, W1;
     int in_words;               // MODE_STEM4: u8 NHWC image with W % 4 == 0 at a 4-byte aligned address -> the producer loads aligned words
+    // null: the launch covers the whole tensors (H .. Wo).  Otherwise int4 (H, W, Ho, Wo) in device memory, read when the kernel starts: the
+    // valid extent of a smaller frame in the top-left corner of the same tensors (the pitches, the tensor maps and the grid stay those of
+    // H .. Wo; bounds, zero padding, statistics and the tile walk follow the valid extent)
+    const int* ext;
 };
 
 // returns 0 when the geometry is supported by the wgmma kernel

@@ -140,11 +140,16 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const GnApplyParams p) {
     __shared__ float s_mean[32], s_rstd[32];
     LFD_TL_BEGIN(p.tl);
     const int n = blockIdx.y;
-    if (threadIdx.x < p.groups)
-        gn_mean_rstd(p.stats, n, threadIdx.x, p.groups, (double)p.HW * 8.0, p.eps, &s_mean[threadIdx.x], &s_rstd[threadIdx.x]);
-    __syncthreads();
     const int cpr = p.C >> 3;
-    const size_t total = (size_t)p.HW * cpr;
+    int count = p.HW;
+    size_t total = (size_t)p.HW * cpr;
+    if (p.ext) {
+        count = p.ext[0] * p.ext[1];
+        total = (size_t)p.ext[0] * p.W * cpr;
+    }
+    if (threadIdx.x < p.groups)
+        gn_mean_rstd(p.stats, n, threadIdx.x, p.groups, (double)count * 8.0, p.eps, &s_mean[threadIdx.x], &s_rstd[threadIdx.x]);
+    __syncthreads();
     const uint4* in = reinterpret_cast<const uint4*>(p.in + (size_t)n * p.HW * p.C);
     uint4* out = reinterpret_cast<uint4*>(p.out + (size_t)n * p.HW * p.C);
 #pragma unroll 4
@@ -196,10 +201,14 @@ __global__ void __launch_bounds__(kHfThreads) head_final_kernel(const HeadFinalP
     float* s_rstd = s_mean + 32;
     LFD_TL_BEGIN(p.tl);
     const int n = blockIdx.y;
+    int HW = p.HW, vw = p.W, P = p.P, point_off = p.point_off;      // valid pixels, valid width, output geometry
+    if (p.ext) {
+        vw = p.ext[1]; HW = p.ext[0] * vw; point_off = p.ext[4]; P = p.ext[5];
+    }
     for (int i = threadIdx.x; i < p.n_out * p.C; i += kHfThreads) wsm[i] = p.w[i];
     const bool gn = p.groups > 0;      // groups == 0: the tower has no norm layers, the input is the already activated tensor
     if (gn && threadIdx.x < p.groups)
-        gn_mean_rstd(p.stats, n, threadIdx.x, p.groups, (double)p.HW * 8.0, p.eps, &s_mean[threadIdx.x], &s_rstd[threadIdx.x]);
+        gn_mean_rstd(p.stats, n, threadIdx.x, p.groups, (double)HW * 8.0, p.eps, &s_mean[threadIdx.x], &s_rstd[threadIdx.x]);
     __syncthreads();
     const int sl = threadIdx.x & 7;                       // channel slice: channels [16 sl, 16 sl + 16)
     float ga[16], be[16];
@@ -216,10 +225,13 @@ __global__ void __launch_bounds__(kHfThreads) head_final_kernel(const HeadFinalP
         for (int k = 0; k < kHfPpt; ++k) {
             const int pix = tile * kHfPixPerBlock + (threadIdx.x >> 3) + k * (kHfThreads / 8);
             nxt[k][0] = make_uint4(0, 0, 0, 0); nxt[k][1] = nxt[k][0];
-            if (pix < p.HW) { nxt[k][0] = rows[(size_t)pix * row_u4]; nxt[k][1] = rows[(size_t)pix * row_u4 + 1]; }
+            if (pix < HW) {
+                const size_t row = vw == p.W ? (size_t)pix : (size_t)(pix / vw) * p.W + pix % vw;   // valid pixel -> row of the map
+                nxt[k][0] = rows[row * row_u4]; nxt[k][1] = rows[row * row_u4 + 1];
+            }
         }
     };
-    const int n_tiles = (p.HW + kHfPixPerBlock - 1) / kHfPixPerBlock;
+    const int n_tiles = (HW + kHfPixPerBlock - 1) / kHfPixPerBlock;
     if ((int)blockIdx.x < n_tiles) fetch(blockIdx.x);
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const int pix0 = tile * kHfPixPerBlock + (threadIdx.x >> 3);
@@ -275,13 +287,13 @@ __global__ void __launch_bounds__(kHfThreads) head_final_kernel(const HeadFinalP
 #pragma unroll
             for (int k = 0; k < kHfPpt; ++k) {
                 const int pix = pix0 + k * (kHfThreads / 8);
-                if (pix >= p.HW) continue;
+                if (pix >= HW) continue;
                 float v = 0.f;
 #pragma unroll
                 for (int oo = 0; oo < 8; ++oo) v = (oo == sl) ? acc[oo][k] : v;   // select without dynamic register indexing
                 v = fmaf(v, sc, sh);
-                if (o < p.n_cls) p.cls[((size_t)n * p.P + p.point_off + pix) * p.cls_stride + o] = v;
-                else p.reg[((size_t)n * p.P + p.point_off + pix) * 4 + (o - p.n_cls)] = v;
+                if (o < p.n_cls) p.cls[((size_t)n * P + point_off + pix) * p.cls_stride + o] = v;
+                else p.reg[((size_t)n * P + point_off + pix) * 4 + (o - p.n_cls)] = v;
             }
         }
     }

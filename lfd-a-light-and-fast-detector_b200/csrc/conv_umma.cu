@@ -69,6 +69,41 @@ static constexpr int kConvThreads = kConsumerThreads + kProdThreads;
 // floor(x / d) for 0 <= x < 2^24 via one 32x32->64 multiply; m = ceil(2^40 / d), exact for d < 2^16
 LFD_DEVINL int fast_div(int x, uint64_t magic) { return (int)(((uint64_t)(uint32_t)x * magic) >> 40); }
 
+// What one launch covers: the valid extent (input H x W, output Ho x Wo) and the tile grid over it.  Without p.ext that is the host's
+// configuration; with it, the extent comes from the plan's geometry table and the grid is recomputed over it exactly as
+// configure_with / configure_stem4 compute it for a tensor of that size, so the tiles (and the fused stem's runs) are those of a plan
+// built for the frame.  MODE_FLAT tiles walk the first Ho rows of the tensor at its full pitch p.Wo.
+struct LaunchGrid {
+    int H, W, Ho, Wo;
+    int tiles_x, tiles_per_img, num_tiles;
+    uint64_t magic_tpi, magic_tx;
+};
+// EXT is false exactly when p.ext is null: the kernels are instantiated for both, so a launch over the whole tensors keeps the grid
+// in the constant bank and runs the code it ran before geometry tables existed
+template <int MODE, bool EXT>
+LFD_DEVINL LaunchGrid launch_grid(const UmmaConvParams& p) {
+    LaunchGrid g;
+    if constexpr (!EXT) {
+        g.H = p.H; g.W = p.W; g.Ho = p.Ho; g.Wo = p.Wo;
+        g.tiles_x = p.tiles_x; g.tiles_per_img = p.tiles_per_img; g.num_tiles = p.num_tiles;
+        g.magic_tpi = p.magic_tpi; g.magic_tx = p.magic_tx;
+        return g;
+    }
+    const int4 e = *reinterpret_cast<const int4*>(p.ext);
+    g.H = e.x; g.W = e.y; g.Ho = e.z; g.Wo = e.w;
+    if (MODE == MODE_FLAT) {
+        g.tiles_x = 0; g.magic_tx = 0;
+        g.tiles_per_img = (g.Ho * p.Wo + 127) / 128;
+    } else {
+        g.tiles_x = (g.Wo + 7) / 8;
+        g.magic_tx = ((1ull << 40) + (uint64_t)g.tiles_x - 1) / (uint64_t)g.tiles_x;
+        g.tiles_per_img = g.tiles_x * ((g.Ho + 15) / 16);
+    }
+    g.num_tiles = g.tiles_per_img * p.N;
+    g.magic_tpi = ((1ull << 40) + (uint64_t)g.tiles_per_img - 1) / (uint64_t)g.tiles_per_img;
+    return g;
+}
+
 struct PxEntry {  // one halo pixel: where it comes from and where it goes
     uint32_t src_off;  // byte offset of the pixel relative to the halo's top-left pixel (tile origin + (dy_min, dx_min))
     uint32_t dst_off;  // byte offset of its 16-byte slot inside a plane
@@ -254,7 +289,7 @@ LFD_DEVINL void store_tile(const EpiCtx& e, const float* acc, int nc, const floa
     if (NCMAX == 128 && stat) stats_flush<128>(st, e.lane, stats);
 }
 
-template <int MODE, int COUT, bool F16>
+template <int MODE, int COUT, bool F16, bool EXT>
 __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid_constant__ UmmaConvParams p) {
     constexpr int kProd = kProdThreads;
     constexpr int kThreads = kConvThreads;
@@ -327,8 +362,9 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
     }
     __syncthreads();
 
-    const int HW = p.H * p.W;
+    const int HW = p.H * p.W;              // image stride of the input (its full size; lg.H x lg.W of it is valid)
     const int n_cc = p.Cin / p.Cc;
+    const LaunchGrid lg = launch_grid<MODE, EXT>(p);
 
     if (warp < kConsumerThreads / 32) {
         // ============================================================== CONSUMERS (MMA + epilogue)
@@ -372,12 +408,12 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
         const uint32_t a_wg = (8u * p.sbo_a * wg) >> 4; // this warpgroup's 64 rows start 8 core-matrix rows further down
         const int nk16 = p.Cc >> 4;
         const uint64_t b2desc0 = wgmma_desc(smem_u32(smem + p.smem_w2_off), cn2 * 16, 128);
-        const int HoWo = p.Ho * p.Wo;
+        const int flat_valid = lg.Ho * p.Wo;      // MODE_FLAT: the rows of the valid extent, at the full pitch
 
         float acc[COUT / 2];
         float acc3[MODE == MODE_3X3S2 ? COUT / 2 : 1];
         uint32_t it = 0, store_count = 0, res_count = 0;
-        for (int tile = blockIdx.x, lt = 0; tile < p.num_tiles; tile += gridDim.x, ++lt) {
+        for (int tile = blockIdx.x, lt = 0; tile < lg.num_tiles; tile += gridDim.x, ++lt) {
             for (int cc = 0; cc < n_cc; ++cc, ++it) {
                 const uint32_t s = it % SA, ph = (it / SA) & 1;
                 if (cc == 0 && e.wtid == 0) LFD_TRACE(1 + wg, lt, 0);
@@ -413,18 +449,19 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
             if (e.wtid == 0) LFD_TRACE(1 + wg, lt, 2);
 
             // ---- epilogue of the tile: this warpgroup's 64 rows
-            const int n = fast_div(tile, p.magic_tpi);
-            const int t = tile - n * p.tiles_per_img;
+            const int n = fast_div(tile, lg.magic_tpi);
+            const int t = tile - n * lg.tiles_per_img;
             int c0, c1 = 0;      // coordinates of the warpgroup's first row: pixel index (flat) or (x, y)
-            bool v0, v1;         // this thread's two rows lie inside the feature map (statistics only; the TMA store clips)
+            bool v0, v1;         // this thread's two rows lie inside the valid extent (statistics only; the TMA store clips at the tensor)
             if (MODE == MODE_FLAT) {
                 c0 = t * 128 + wg * 64;
-                v0 = c0 + e.r0 < HoWo; v1 = c0 + e.r0 + 8 < HoWo;
+                const int q0 = c0 + e.r0, q1 = q0 + 8;
+                v0 = q0 < flat_valid && (!EXT || q0 % p.Wo < lg.Wo); v1 = q1 < flat_valid && (!EXT || q1 % p.Wo < lg.Wo);
             } else {
-                const int ty = fast_div(t, p.magic_tx);
-                c1 = ty * 16 + wg * 8; c0 = (t - ty * p.tiles_x) * 8;
-                const bool xin = c0 + (e.r0 & 7) < p.Wo;
-                v0 = xin && c1 + (e.r0 >> 3) < p.Ho; v1 = xin && c1 + (e.r0 >> 3) + 1 < p.Ho;
+                const int ty = fast_div(t, lg.magic_tx);
+                c1 = ty * 16 + wg * 8; c0 = (t - ty * lg.tiles_x) * 8;
+                const bool xin = c0 + (e.r0 & 7) < lg.Wo;
+                v0 = xin && c1 + (e.r0 >> 3) < lg.Ho; v1 = xin && c1 + (e.r0 >> 3) + 1 < lg.Ho;
             }
             const bool has_res = p.res != nullptr;
             // GroupNorm partial sums are taken over the STORED (16-bit) values, after residual and ReLU; one group = one 16-byte
@@ -496,10 +533,10 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
             uint32_t raw[kStemPerThread][3];
             uint32_t okmask = 0;
             auto fetch = [&](int tile) LFD_LAMBDA_INLINE {
-                const int n = fast_div(tile, p.magic_tpi), t = tile - n * p.tiles_per_img;
-                const int ty = fast_div(t, p.magic_tx);
-                const int iy0 = 2 * ty * 16 - 1, ix0 = 2 * (t - ty * p.tiles_x) * 8 - 1;
-                const bool interior = iy0 >= 0 && ix0 >= 0 && iy0 + kStemRows <= p.H && ix0 + kStemCols <= p.W;
+                const int n = fast_div(tile, lg.magic_tpi), t = tile - n * lg.tiles_per_img;
+                const int ty = fast_div(t, lg.magic_tx);
+                const int iy0 = 2 * ty * 16 - 1, ix0 = 2 * (t - ty * lg.tiles_x) * 8 - 1;
+                const bool interior = iy0 >= 0 && ix0 >= 0 && iy0 + kStemRows <= lg.H && ix0 + kStemCols <= lg.W;
                 okmask = 0;
                 if (u8) {
                     const uint8_t* img = reinterpret_cast<const uint8_t*>(p.in_raw) + (size_t)n * plane * 3;
@@ -511,7 +548,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                         bool ok = true;
                         if (!interior) {
                             const int y = iy0 + (prc[j] >> 8), x = ix0 + (prc[j] & 255);
-                            ok = (unsigned)y < (unsigned)p.H && (unsigned)x < (unsigned)p.W;
+                            ok = (unsigned)y < (unsigned)lg.H && (unsigned)x < (unsigned)lg.W;
                             if (!ok) src = img;
                         }
                         okmask |= (ok ? 1u : 0u) << j;
@@ -527,7 +564,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                         bool ok = true;
                         if (!interior) {
                             const int y = iy0 + (prc[j] >> 8), x = ix0 + (prc[j] & 255);
-                            ok = (unsigned)y < (unsigned)p.H && (unsigned)x < (unsigned)p.W;
+                            ok = (unsigned)y < (unsigned)lg.H && (unsigned)x < (unsigned)lg.W;
                             if (!ok) src = img;
                         }
                         okmask |= (ok ? 1u : 0u) << j;
@@ -538,8 +575,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
             };
             uint32_t it = 0;
             pdl_wait();
-            if ((int)blockIdx.x < p.num_tiles) fetch(blockIdx.x);
-            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
+            if ((int)blockIdx.x < lg.num_tiles) fetch(blockIdx.x);
+            for (int tile = blockIdx.x; tile < lg.num_tiles; tile += gridDim.x, ++it) {
                 const uint32_t s = it % SA, ph = (it / SA) & 1;
                 if (ptid == 0) LFD_TRACE(0, it, 0);
                 mbar_wait(&empty[s], ph ^ 1);
@@ -560,7 +597,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                 fence_proxy_async_smem();       // generic-proxy st.shared -> wgmma reads
                 mbar_arrive(&full[s]);
                 if (ptid == 0) LFD_TRACE(0, it, 2);
-                if (tile + (int)gridDim.x < p.num_tiles) fetch(tile + gridDim.x);
+                if (tile + (int)gridDim.x < lg.num_tiles) fetch(tile + gridDim.x);
                 if (ptid == 0) LFD_TRACE(0, it, 3);
             }
         } else {
@@ -572,25 +609,26 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
         const int my_cnt = (p.n_px - px0 + pstep - 1) / pstep;   // halo pixels this thread copies per stage
         uint32_t it = 0;
         pdl_wait();                                   // the input activations are produced by the previous kernel
-        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-            const int n = fast_div(tile, p.magic_tpi);
-            const int t = tile - n * p.tiles_per_img;
+        for (int tile = blockIdx.x; tile < lg.num_tiles; tile += gridDim.x) {
+            const int n = fast_div(tile, lg.magic_tpi);
+            const int t = tile - n * lg.tiles_per_img;
             int iy0 = 0, ix0 = 0;
             if (MODE == MODE_FLAT) ix0 = t * 128;
             else {
-                const int ty = fast_div(t, p.magic_tx);
-                int oy0 = ty * 16, ox0 = (t - ty * p.tiles_x) * 8;
+                const int ty = fast_div(t, lg.magic_tx);
+                int oy0 = ty * 16, ox0 = (t - ty * lg.tiles_x) * 8;
                 iy0 = (MODE == MODE_3X3S1) ? oy0 : 2 * oy0;
                 ix0 = (MODE == MODE_3X3S1) ? ox0 : 2 * ox0;
             }
             const __nv_bfloat16* img = p.in + (size_t)n * HW * p.Cin + ch * 8;
-            // tiles whose halo lies inside the image (the vast majority) copy without bounds checks: source = tile origin +
-            // a per-pixel offset from the table
+            // tiles whose halo lies inside the valid extent (the vast majority) copy without bounds checks: source = tile origin +
+            // a per-pixel offset from the table.  (Flat tiles are pixel-local: they may read the rest of the tensor, whose results
+            // land outside the valid extent.)
             constexpr int kDyMin = (MODE == MODE_1X1S2) ? 0 : -1, kDxMin = kDyMin;
             constexpr int kDyMax = (MODE == MODE_3X3S1) ? 16 : ((MODE == MODE_3X3S2) ? 31 : 30);
             constexpr int kDxMax = (MODE == MODE_3X3S1) ? 8 : ((MODE == MODE_3X3S2) ? 15 : 14);
             const bool interior = MODE == MODE_FLAT ? (ix0 + 128 <= HW)
-                                                    : (iy0 + kDyMin >= 0 && ix0 + kDxMin >= 0 && iy0 + kDyMax < p.H && ix0 + kDxMax < p.W);
+                                                    : (iy0 + kDyMin >= 0 && ix0 + kDxMin >= 0 && iy0 + kDyMax < lg.H && ix0 + kDxMax < lg.W);
             // flat: first pixel of the tile; otherwise the halo's top-left pixel (in range for interior tiles)
             const __nv_bfloat16* org = img + (ptrdiff_t)(MODE == MODE_FLAT ? ix0 : (iy0 + kDyMin) * p.W + ix0 + kDxMin) * p.Cin;
             for (int cc = 0; cc < n_cc; ++cc, ++it) {
@@ -634,7 +672,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                     for (int pxi = px0; pxi < p.n_px; pxi += pstep) {
                         const PxDelta pd = delta[pxi];
                         const int y = iy0 + pd.dy, x = ix0 + pd.dx;
-                        const bool ok = ((unsigned)y < (unsigned)p.H) && ((unsigned)x < (unsigned)p.W);
+                        const bool ok = ((unsigned)y < (unsigned)lg.H) && ((unsigned)x < (unsigned)lg.W);
                         cp_async16(dst_cc + table[pxi].dst_off, src_cc + (ok ? (y * p.W + x) : 0) * p.Cin, ok);
                     }
                 }
@@ -717,7 +755,7 @@ LFD_DEVINL void s4_run(int num_tiles, int& t0, int& t1) {
 
 LFD_DEVINL void consumers_bar_sync() { asm volatile("bar.sync 3, 256;" ::: "memory"); }   // the two consumer warpgroups
 
-template <bool F16>
+template <bool F16, bool EXT>
 __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_constant__ UmmaConvParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + kS4Bar);
@@ -746,6 +784,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
         shifts[tid] = s ? round16<F16>(s[tid & 63]) : 0.f;
     }
     __syncthreads();
+    // the valid image, stem3 map and tile grid; the runs and the inherited column below are defined over this grid
+    const LaunchGrid lg = launch_grid<MODE_STEM4, EXT>(p);
 
     if (warp < kConsumerThreads / 32) {
         // ============================================================== CONSUMERS
@@ -796,18 +836,19 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
         const int brow = 2 * (warp & 3), bcol = lane >> 2;
         const int sh = (lane >> 3) & 1, sc = lane & 7;
 
+        const int H1 = EXT ? (lg.H - 1) / 2 + 1 : p.H1, W1 = EXT ? (lg.W - 1) / 2 + 1 : p.W1;   // the valid stem1 map
         int tile0, tile1;
-        s4_run(p.num_tiles, tile0, tile1);
+        s4_run(lg.num_tiles, tile0, tile1);
         uint32_t store_count = 0, res_count = 0;
         for (int tile = tile0, lt = 0; tile < tile1; ++tile, ++lt) {
             const uint32_t s = lt & 1, ph = (lt >> 1) & 1;
-            const int n = fast_div(tile, p.magic_tpi);
-            const int t = tile - n * p.tiles_per_img;
-            const int ty = fast_div(t, p.magic_tx);
-            const int tx = t - ty * p.tiles_x;
+            const int n = fast_div(tile, lg.magic_tpi);
+            const int t = tile - n * lg.tiles_per_img;
+            const int ty = fast_div(t, lg.magic_tx);
+            const int tx = t - ty * lg.tiles_x;
             const int oy0 = ty * 16, ox0 = tx * 8;
             // column 0 was copied from the previous tile / column 16 goes to the next tile
-            const bool inherit = tile > tile0 && tx > 0, pass_on = tile + 1 < tile1 && tx + 1 < p.tiles_x;
+            const bool inherit = tile > tile0 && tx > 0, pass_on = tile + 1 < tile1 && tx + 1 < lg.tiles_x;
             if (e.wtid == 0) LFD_TRACE(1 + wg, lt, 0);
             mbar_wait(&full[s], ph);
             if (e.wtid == 0) LFD_TRACE(1 + wg, lt, 1);
@@ -879,7 +920,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                     for (int h = 0; h < 2; ++h) {
                         const int a = packed ? a0 : a0 + brow + h, b = b0 + bcol + (packed ? 8 * h : 0);
                         const int y1 = 2 * oy0 - 1 + a, x1 = 2 * ox0 - 1 + b;
-                        const bool in = (unsigned)y1 < (unsigned)p.H1 && (unsigned)x1 < (unsigned)p.W1;
+                        const bool in = (unsigned)y1 < (unsigned)H1 && (unsigned)x1 < (unsigned)W1;
 #pragma unroll
                         for (int j = 0; j < 8; ++j) {
                             const float x0 = c1[q][4 * j + 2 * h] + bv[j].x, x1v = c1[q][4 * j + 2 * h + 1] + bv[j].y;
@@ -962,22 +1003,23 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
         const int plane = p.H * p.W;
         pdl_wait();
         int tile0, tile1;
-        s4_run(p.num_tiles, tile0, tile1);
+        s4_run(lg.num_tiles, tile0, tile1);
         for (int tile = tile0, lt = 0; tile < tile1; ++tile, ++lt) {
             const uint32_t s = lt & 1, ph = (lt >> 1) & 1;
-            const int n = fast_div(tile, p.magic_tpi), t = tile - n * p.tiles_per_img;
-            const int ty = fast_div(t, p.magic_tx);
-            const int iy0 = 4 * 16 * ty - 3, ix0 = 4 * 8 * (t - ty * p.tiles_x) - 3;
-            const bool interior = iy0 >= 0 && ix0 >= 0 && iy0 + kS4Rows <= p.H && ix0 + kS4Cols <= p.W;
+            const int n = fast_div(tile, lg.magic_tpi), t = tile - n * lg.tiles_per_img;
+            const int ty = fast_div(t, lg.magic_tx);
+            const int iy0 = 4 * 16 * ty - 3, ix0 = 4 * 8 * (t - ty * lg.tiles_x) - 3;
+            const bool interior = iy0 >= 0 && ix0 >= 0 && iy0 + kS4Rows <= lg.H && ix0 + kS4Cols <= lg.W;
             if (ptid == 0) LFD_TRACE(0, lt, 0);
             mbar_wait(&empty[s], ph ^ 1);
             if (ptid == 0) LFD_TRACE(0, lt, 1);
             const uint32_t dst0 = smem_u32(smem + kS4Ring) + s * kS4PatchBytes;
             if (p.in_words) {
                 // ix0 = 1 (mod 4): group g of a patch row = image columns ix0 - 1 + 4g .. + 3 = patch columns 4g - 1 .. 4g + 2,
-                // 12 bytes at a 4-byte aligned address (W % 4 == 0).  A group lies wholly inside or wholly outside the image, so
-                // no load touches a byte outside the tensor.  Two batches of 3 groups: all loads of a batch are issued before any
-                // is used (6 groups at once do not fit the producer's 56 registers).
+                // 12 bytes at a 4-byte aligned address (W % 4 == 0).  A group lies wholly inside or wholly outside the tensor, so
+                // no load touches a byte outside it; a valid width that is not a multiple of 4 ends inside a group, whose pixels
+                // past it are zeroed one by one.  Two batches of 3 groups: all loads of a batch are issued before any is used
+                // (6 groups at once do not fit the producer's 56 registers).
 #pragma unroll 1
                 for (int j0 = 0; j0 < kS4GroupsPerThread; j0 += kS4GroupBatch) {
                     uint32_t wd[kS4GroupBatch][3];
@@ -987,7 +1029,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                         const int q = ptid + (j0 + j) * kProdThreads;
                         const int r = q / 10, g = q - r * 10;
                         const int y = iy0 + r, x = ix0 - 1 + 4 * g;
-                        ok[j] = q < kS4Groups && (unsigned)y < (unsigned)p.H && (unsigned)x < (unsigned)p.W;
+                        ok[j] = q < kS4Groups && (unsigned)y < (unsigned)lg.H && (unsigned)x < (unsigned)lg.W;
                         const uint32_t* src = reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint8_t*>(p.in_raw) +
                                                                                 ((ptrdiff_t)n * plane + (ptrdiff_t)y * p.W + x) * 3);
 #pragma unroll
@@ -998,14 +1040,16 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                         const int q = ptid + (j0 + j) * kProdThreads;
                         if (q >= kS4Groups) break;
                         const int r = q / 10, g = q - r * 10;
+                        const int in_cols = lg.W - (ix0 - 1 + 4 * g);    // pixels k < in_cols of the group lie inside the valid width
                         uint32_t px[4][2];
 #pragma unroll
                         for (int k = 0; k < 4; ++k) {
                             float f[3];
+                            const bool okk = ok[j] && (!EXT || k < in_cols);
 #pragma unroll
                             for (int c = 0; c < 3; ++c) {
                                 const uint32_t byte = (wd[j][(3 * k + c) >> 2] >> (8 * ((3 * k + c) & 3))) & 0xffu;
-                                f[c] = ok[j] ? ((float)byte - 127.5f) * (1.0f / 127.5f) : 0.f;   // zero padding of the normalised image
+                                f[c] = okk ? ((float)byte - 127.5f) * (1.0f / 127.5f) : 0.f;     // zero padding of the normalised image
                             }
                             px[k][0] = pack2<F16>(f[0], f[1]);                                       // rounding point R0
                             px[k][1] = pack2<F16>(f[2], 0.f);
@@ -1030,7 +1074,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                         const int q = ptid + (j0 + j) * kProdThreads;
                         const int r = q / kS4Cols, c = q - r * kS4Cols;
                         const int y = iy0 + r, x = ix0 + c;
-                        ok[j] = q < kS4Pix && (interior || ((unsigned)y < (unsigned)p.H && (unsigned)x < (unsigned)p.W));
+                        ok[j] = q < kS4Pix && (interior || ((unsigned)y < (unsigned)lg.H && (unsigned)x < (unsigned)lg.W));
                         const ptrdiff_t pix = ok[j] ? (ptrdiff_t)n * plane + (ptrdiff_t)y * p.W + x : 0;
                         if (u8) {
                             const uint8_t* src = reinterpret_cast<const uint8_t*>(p.in_raw) + pix * 3;
@@ -1306,21 +1350,31 @@ static cudaError_t launch_persistent(void (*kernel)(UmmaConvParams), bool* confi
     return cudaLaunchKernelEx(&cfg, kernel, p);
 }
 
-template <int MODE, int COUT, bool F16>
+template <int MODE, int COUT, bool F16, bool EXT>
 static cudaError_t launch_mode_t(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
     static bool configured[kMaxDevices] = {};
-    return launch_persistent(conv_umma_kernel<MODE, COUT, F16>, configured, 224 * 1024, p, smem, grid, st);
+    return launch_persistent(conv_umma_kernel<MODE, COUT, F16, EXT>, configured, 224 * 1024, p, smem, grid, st);
+}
+
+template <bool F16, bool EXT>
+static cudaError_t launch_stem4_t(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
+    static bool configured[kMaxDevices] = {};
+    return launch_persistent(stem4_kernel<F16, EXT>, configured, kS4Smem, p, smem, grid, st);
 }
 
 template <bool F16>
 static cudaError_t launch_stem4(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
-    static bool configured[kMaxDevices] = {};
-    return launch_persistent(stem4_kernel<F16>, configured, kS4Smem, p, smem, grid, st);
+    return p.ext ? launch_stem4_t<F16, true>(p, smem, grid, st) : launch_stem4_t<F16, false>(p, smem, grid, st);
+}
+
+template <int MODE, int COUT, bool F16>
+static cudaError_t launch_mode_e(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
+    return p.ext ? launch_mode_t<MODE, COUT, F16, true>(p, smem, grid, st) : launch_mode_t<MODE, COUT, F16, false>(p, smem, grid, st);
 }
 
 template <int MODE, int COUT>
 static cudaError_t launch_mode(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
-    return p.f16 ? launch_mode_t<MODE, COUT, true>(p, smem, grid, st) : launch_mode_t<MODE, COUT, false>(p, smem, grid, st);
+    return p.f16 ? launch_mode_e<MODE, COUT, true>(p, smem, grid, st) : launch_mode_e<MODE, COUT, false>(p, smem, grid, st);
 }
 
 // the output widths umma_conv_configure accepts per mode

@@ -28,6 +28,10 @@ struct GnApplyParams {
     float eps;
     int f16;
     unsigned long long* tl;    // debugging time-line slot or null
+    // null: all HW pixels.  Otherwise device int2 (h, w), read when the kernel starts: only the top-left h x w of the map (row pitch W) is
+    // valid -- the GroupNorm count is h * w; the first h rows are written (the pixels right of w are outside the valid extent)
+    const int* ext = nullptr;
+    int W = 0;
 };
 cudaError_t gn_apply_launch(const GnApplyParams& p, int num_sms, cudaStream_t st);
 
@@ -45,6 +49,10 @@ struct HeadFinalParams {
     float eps;
     int f16;
     unsigned long long* tl;    // debugging time-line slot or null
+    // null: all HW pixels.  Otherwise device int[6] (h, w, -, -, point_off, P), read when the kernel starts: the top-left h x w of the map
+    // (row pitch W) is valid; pixel (y, x) goes to point point_off + y * w + x of a (N, P, .) output -- the layout of a plan built for the frame
+    const int* ext = nullptr;
+    int W = 0;
 };
 cudaError_t head_final_launch(const HeadFinalParams& p, int num_sms, cudaStream_t st);
 

@@ -65,6 +65,22 @@ def check_input(x, N, H, W, contiguous):
     return fmt
 
 
+def check_frame(x, N, H, W):
+    """x: float32 [N,3,h,w] or uint8 [N,h,w,3], contiguous, on a CUDA device, with h <= H and w <= W -> (its nat.INPUT_* format, h, w)."""
+    if x.dtype == torch.float32:
+        fmt, ok = nat.INPUT_F32_NCHW, x.dim() == 4 and x.shape[1] == 3
+        h, w = (x.shape[2], x.shape[3]) if ok else (0, 0)
+    elif x.dtype == torch.uint8:
+        fmt, ok = nat.INPUT_U8_NHWC, x.dim() == 4 and x.shape[3] == 3
+        h, w = (x.shape[1], x.shape[2]) if ok else (0, 0)
+    else:
+        raise TypeError('input must be float32 NCHW or uint8 NHWC, got %s' % (x.dtype,))
+    if not ok or not x.is_cuda or not x.is_contiguous() or x.shape[0] != N or not (1 <= h <= H and 1 <= w <= W):
+        raise ValueError('input must be a contiguous CUDA tensor of N=%d frames of at most H=%d x W=%d (the plan\'s capacity), got %s'
+                         % (N, H, W, tuple(x.shape)))
+    return fmt, int(h), int(w)
+
+
 def tune_branch_bounds(work, measure, candidates, budget_s, max_branches=None):
     """Coordinate descent over per-branch bounds on the persistent CTAs of side-branch kernels.  work: {branch: amount of work};
     measure(caps) -> time of the plan with caps = {branch: bound} (0 = unbounded).  The branches with the most work come first (at most
@@ -499,7 +515,7 @@ class InferencePlan(object):
                 shs.append(b * sc)
             op = dict(kind=nat.OP_HEAD_FINAL, H=fh, W=fw, Cin=ws[0].shape[1], Ho=fh, Wo=fw, Cout=n_cls + n_reg,
                       gn_groups=tnorm.num_groups if tnorm is not None else 0, inp=raw, stats=stats_id, n_cls=n_cls, n_reg=n_reg,
-                      point_off=point_off, w_f32=self._add_f32(torch.cat(ws, 0)),
+                      point_off=point_off, level=l, w_f32=self._add_f32(torch.cat(ws, 0)),
                       scale=self._add_f32(torch.cat(scs)), shift=self._add_f32(torch.cat(shs)),
                       modules=(tnorm, [c for c, _ in convs], [sc for _, sc in convs]))
             if tnorm is not None:
@@ -558,6 +574,9 @@ class InferencePlan(object):
         self.reg_out = torch.empty((self.N, self.P, 4), dtype=torch.float32, device=dev)
         self._outputs = [(self.cls_out, self.reg_out)]      # slot 1 (second output pair) is allocated on first use
         self.offsets = offsets
+        self.frame_level_sizes, self.frame_P = self.level_sizes, self.P   # of the last forward's frame
+        self._extents = {}                  # (h, w) -> (lfd_extent table, level sizes, P) of a frame below the capacity
+        self._stage = None                  # frames below the capacity are copied into its top-left corner (allocated on first use)
         self.handle = None
         if not self.create_native:
             return
@@ -675,17 +694,87 @@ class InferencePlan(object):
             self._outputs.append((torch.empty_like(self.cls_out), torch.empty_like(self.reg_out)))
         return self._outputs[slot]
 
+    def extent_table(self, h, w):
+        """The geometry of an h x w frame on this plan -> (rows, level sizes, P): per op [H, W, Ho, Wo, point_off, P], the fields a plan built
+        for h x w has (point_off and P on HEAD_FINAL ops only, 0 elsewhere).  Every tensor's valid size follows from the frame through the
+        op list, exactly as _build derives the sizes of a plan."""
+        size, rows = {}, []
+        for op in self._ops:
+            H, W = (h, w) if op['kind'] in (nat.OP_STEM0, nat.OP_STEM4) else size[op['inp']]
+            if op['kind'] in (nat.OP_STEM0, nat.OP_CONV):
+                Ho, Wo = conv_out(H, op['ksize'], op['stride']), conv_out(W, op['ksize'], op['stride'])
+            elif op['kind'] == nat.OP_STEM4:
+                Ho, Wo = conv_out(conv_out(H, 3, 2), 3, 2), conv_out(conv_out(W, 3, 2), 3, 2)
+            else:
+                Ho, Wo = H, W
+            for k in ('out', 'out2'):
+                if op.get(k) is not None:
+                    size[op[k]] = (Ho, Wo)
+            rows.append([H, W, Ho, Wo, 0, 0])
+        level_sizes = [None] * len(self.level_sizes)
+        for op, r in zip(self._ops, rows):
+            if op['kind'] == nat.OP_HEAD_FINAL:
+                level_sizes[op['level']] = (r[0], r[1])
+        offs, P = [], 0
+        for fh, fw in level_sizes:
+            offs.append(P)
+            P += fh * fw
+        for op, r in zip(self._ops, rows):
+            if op['kind'] == nat.OP_HEAD_FINAL:
+                r[4], r[5] = offs[op['level']], P
+        return rows, level_sizes, P
+
+    def _extent(self, h, w):
+        if (h, w) not in self._extents:
+            rows, level_sizes, P = self.extent_table(h, w)
+            arr = (nat.Extent * len(rows))()
+            for e, r in zip(arr, rows):
+                e.H, e.W, e.Ho, e.Wo, e.point_off, e.P = r
+            self._extents[(h, w)] = (arr, level_sizes, P)
+        return self._extents[(h, w)]
+
+    def staging(self, fmt):
+        """The plan-owned input of frames below the capacity, in the capacity layout of format fmt (uint8 [N,H,W,3] or float32 [N,3,H,W])."""
+        if self._stage is None:
+            self._stage = torch.empty(self.N * 3 * self.H * self.W * 4, dtype=torch.uint8, device=self.device)
+        if fmt == nat.INPUT_U8_NHWC:
+            return self._stage[:self.N * self.H * self.W * 3].view(self.N, self.H, self.W, 3)
+        return self._stage.view(torch.float32).view(self.N, 3, self.H, self.W)
+
+    def num_graphs(self):
+        return nat.lib().lfd_plan_num_graphs(self.handle)
+
     def forward(self, x, use_graph=True, slot=0):
-        """x: cuda float32 [N,3,H,W] (contiguous) or uint8 [N,H,W,3].  Returns the plan-owned (cls, reg) buffers of output
-        `slot` (a second slot lets the post-process of one batch overlap the forward of the next, lfd/pipeline.py)."""
+        """x: cuda float32 [N,3,h,w] (contiguous) or uint8 [N,h,w,3] with h <= H and w <= W.  Returns the frame's (cls, reg) in the
+        plan-owned buffers of output `slot` (a second slot lets the post-process of one batch overlap the forward of the next,
+        lfd/pipeline.py): (N, P, C') and (N, P, 4) for the frame's P points, laid out as a plan built for h x w lays them out;
+        frame_level_sizes / frame_P describe them.  A frame of the full size is read in place; a smaller one is first copied into the
+        top-left corner of a plan-owned input, so that every frame size replays the same CUDA graph."""
         if self.handle is None:
             raise nat.LfdError('this plan was built for host-side inspection only (create_native=False)')
-        fmt = check_input(x, self.N, self.H, self.W, contiguous=True)
+        fmt, h, w = check_frame(x, self.N, self.H, self.W)
         cls_out, reg_out = self.outputs(slot)
+        lib = nat.lib()
+        if (h, w) == (self.H, self.W):
+            with torch.cuda.device(self.device):
+                nat.check(lib.lfd_plan_forward(self.handle, nat.ptr(x), fmt, nat.ptr(self.workspace), nat.ptr(cls_out),
+                                               nat.ptr(reg_out), int(bool(use_graph)), nat.stream_ptr()))
+            self.frame_level_sizes, self.frame_P = self.level_sizes, self.P
+            return cls_out, reg_out
+        if self.conv_impl != nat.CONV_UMMA:
+            raise nat.LfdError('the SIMT cross-check plan runs frames of its full size %dx%d only (got %dx%d)' % (self.H, self.W, h, w))
+        table, level_sizes, P = self._extent(h, w)
         with torch.cuda.device(self.device):
-            nat.check(nat.lib().lfd_plan_forward(self.handle, nat.ptr(x), fmt, nat.ptr(self.workspace), nat.ptr(cls_out),
-                                                 nat.ptr(reg_out), int(bool(use_graph)), nat.stream_ptr()))
-        return cls_out, reg_out
+            stage = self.staging(fmt)
+            if fmt == nat.INPUT_U8_NHWC:
+                stage[:, :h, :w].copy_(x)
+            else:
+                stage[:, :, :h, :w].copy_(x)
+            nat.check(lib.lfd_plan_forward_extent(self.handle, nat.ptr(stage), fmt, h, w, table, nat.ptr(self.workspace), nat.ptr(cls_out),
+                                                  nat.ptr(reg_out), int(bool(use_graph)), nat.stream_ptr()))
+        self.frame_level_sizes, self.frame_P = level_sizes, P
+        n, c = self.N, self.cls_channels
+        return cls_out.view(-1)[:n * P * c].view(n, P, c), reg_out.view(-1)[:n * P * 4].view(n, P, 4)
 
     def tensor(self, name):
         """Debug view of an intermediate activation as NHWC bf16 / fp16 (valid right after an eager forward only if

@@ -102,6 +102,12 @@ class Top(C.Structure):
                 ('off', C.c_int64 * 8), ('ptr', C.c_void_p * 6)]
 
 
+class Extent(C.Structure):
+    """lfd_extent: the valid geometry of one op for a frame below the plan's capacity (lfd_plan_forward_extent)."""
+    _fields_ = [('H', C.c_int32), ('W', C.c_int32), ('Ho', C.c_int32), ('Wo', C.c_int32), ('point_off', C.c_int32), ('P', C.c_int32),
+                ('pad_', C.c_int32 * 2)]
+
+
 class PackDesc(C.Structure):
     _fields_ = [('kind', C.c_int32), ('Cout', C.c_int32), ('Cin', C.c_int32), ('k', C.c_int32), ('cc', C.c_int32), ('n', C.c_int32),
                 ('src', C.c_void_p), ('src2', C.c_void_p), ('dst', C.c_void_p), ('dst2', C.c_void_p), ('dst3', C.c_void_p)]
@@ -126,6 +132,8 @@ SYMBOLS = {
     'lfd_plan_num_launches': (_i, [_vp]),
     'lfd_plan_forward': (_i, [_vp, _vp, _i, _vp, _vp, _vp, _i, _vp]),
     'lfd_plan_profile': (_i, [_vp, _vp, _i, _vp, _vp, _vp, C.POINTER(C.c_float), _vp]),
+    'lfd_plan_forward_extent': (_i, [_vp, _vp, _i, _i, _i, C.POINTER(Extent), _vp, _vp, _vp, _i, _vp]),
+    'lfd_plan_num_graphs': (_i, [_vp]),
     'lfd_debug_set_trace': (_i, [_vp]),
     'lfd_debug_set_timeline': (_i, [_vp]),
     'lfd_run_op': (_i, [C.POINTER(Op), _vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
@@ -184,7 +192,7 @@ def lib():
         fn.argtypes = args
     if L.lfd_abi_version() != 5:
         raise LfdError('liblfd_b200.so ABI version mismatch')
-    for which, st in enumerate((Op, Top, PackDesc, UnpackDesc, PostCfg, LossCfg, Levels, InputDesc)):
+    for which, st in enumerate((Op, Top, PackDesc, UnpackDesc, PostCfg, LossCfg, Levels, InputDesc, Extent)):
         if L.lfd_struct_bytes(which) != C.sizeof(st):
             raise LfdError('liblfd_b200.so: %s is %d bytes in the library, %d in lfd/_native.py' % (st.__name__, L.lfd_struct_bytes(which), C.sizeof(st)))
     _lib = L

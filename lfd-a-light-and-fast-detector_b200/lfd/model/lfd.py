@@ -157,13 +157,27 @@ class LFD(nn.Module):
         self._plans = {}
         self._plan_fingerprint = None
 
-    def inference_plan(self, n, h, w, device):
+    def inference_plan(self, n, h, w, device, exact=False):
+        """The native forward plan for n frames of h x w: a cached plan of exactly that size, else the smallest cached plan (same n,
+        device, conv_impl and act_dtype) that covers h x w -- its forward runs any frame up to its size with the results of a plan built
+        for the frame -- else a new plan of h x w, which replaces the cached plans it covers.  So a stream of varying sizes holds one plan
+        and builds a new one only at a new maximum.  exact=True: only a plan of exactly h x w (callers that need its full-size buffers)."""
         fp = self._fingerprint()
         if fp != self._plan_fingerprint:
             self._plans, self._plan_fingerprint = {}, fp
-        key = (n, h, w, str(device), self.conv_impl, self.act_dtype)
-        if key not in self._plans:
-            self._plans[key] = InferencePlan(self, n, h, w, device, self.conv_impl, act_dtype=self.act_dtype)
+        rest = (str(device), self.conv_impl, self.act_dtype)
+        key = (n, h, w) + rest
+        if key in self._plans:
+            return self._plans[key]
+        same = [k for k in self._plans if k[0] == n and k[3:] == rest]
+        if not exact and self.conv_impl == nat.CONV_UMMA:        # (the SIMT cross-check runs full-size frames only)
+            cover = [k for k in same if k[1] >= h and k[2] >= w]
+            if cover:
+                return self._plans[min(cover, key=lambda k: (k[1] * k[2], k[1], k[2]))]
+            for k in same:
+                if k[1] <= h and k[2] <= w:
+                    del self._plans[k]
+        self._plans[key] = InferencePlan(self, n, h, w, device, self.conv_impl, act_dtype=self.act_dtype)
         return self._plans[key]
 
     def forward(self, x):
@@ -185,7 +199,7 @@ class LFD(nn.Module):
             n, h, w = x.shape[0], x.shape[2], x.shape[3]
         plan = self.inference_plan(n, h, w, x.device)
         cls, reg = plan.forward(x.contiguous(), use_graph=self.use_cuda_graph)
-        for i, hw in enumerate(plan.level_sizes):
+        for i, hw in enumerate(plan.frame_level_sizes):
             self._head_indexes_to_feature_map_sizes[i] = hw
         return cls.clone(), reg.clone()
 
@@ -393,6 +407,13 @@ class LFD(nn.Module):
         else:
             cfg.bbox_mode = nat.BBOX_SIGMOID if self._distance_to_bbox_mode == 'sigmoid' else nat.BBOX_EXP
         cfg.class_agnostic = int(bool(class_agnostic))
+        self._post_levels(cfg, sizes)
+        cfg.score_thr, cfg.iou_thr = float(score_thr), float(iou_thr)
+        cfg.cap = int(self.max_detections_per_image)
+        return cfg
+
+    def _post_levels(self, cfg, sizes):
+        """The level geometry of lfd_post_cfg (read by every lfd_postprocess call; the workspace does not depend on it)."""
         cfg.num_levels = len(sizes)
         off = 0
         for i, (h, w) in enumerate(sizes):
@@ -400,9 +421,6 @@ class LFD(nn.Module):
             cfg.level_hi[i] = float(max(self._regression_ranges[i]))
             off += h * w
         cfg.P = off
-        cfg.score_thr, cfg.iou_thr = float(score_thr), float(iou_thr)
-        cfg.cap = int(self.max_detections_per_image)
-        return cfg
 
     def _soft_nms_cfg(self):
         """_nms_cfg['type'] 'nms' -> None; 'soft_nms' -> (method code, sigma, min_score); anything else raises (the reference would fail
@@ -416,14 +434,15 @@ class LFD(nn.Module):
 
     def post_plan(self, n, sizes, device, class_agnostic=False):
         """The cached device post-process for this batch geometry and the current _nms_cfg type (greedy NMS or Soft-NMS with its method,
-        sigma and min_score)."""
+        sigma and min_score).  sizes=None: one plan for every geometry of n images, whose level geometry the caller sets per call
+        (_post_levels), as detect does."""
         soft = self._soft_nms_cfg()
-        key = (n, tuple(map(tuple, sizes)), int(self.max_detections_per_image), str(device), bool(class_agnostic),
+        key = (n, tuple(map(tuple, sizes)) if sizes is not None else None, int(self.max_detections_per_image), str(device), bool(class_agnostic),
                type(self._classification_loss_func).__name__, self._distance_to_bbox_mode, self._regression_loss_type)
         if soft is not None:
             key = key + ('soft_nms',) + soft
         if key not in self._post_plans:
-            self._post_plans[key] = PostPlan(self._post_cfg(n, sizes, self._classification_threshold, self._nms_cfg['iou_thr'],
+            self._post_plans[key] = PostPlan(self._post_cfg(n, sizes or [], self._classification_threshold, self._nms_cfg['iou_thr'],
                                                             class_agnostic), device, soft)
         return self._post_plans[key]
 
@@ -436,7 +455,8 @@ class LFD(nn.Module):
             raise RuntimeError('lfd_b200 has no CPU path')
         N = cls.shape[0]
         sizes = self._sizes()
-        pp = self.post_plan(N, sizes, cls.device, class_agnostic)
+        pp = self.post_plan(N, None, cls.device, class_agnostic)    # one plan serves every frame size
+        self._post_levels(pp.cfg, sizes)
         if pp.cfg.P != cls.shape[1]:
             raise ValueError('prediction has %d points but the recorded feature maps give %d' % (cls.shape[1], pp.cfg.P))
         pp.set_meta(widths, heights, scales)

@@ -94,7 +94,7 @@ class StreamingDetector(object):
             # The copy itself costs the forward ~8 %: 0.561 ms per step with the input copy left out, tests/debug_e2e_timeline.py)
             self.copy_streams = [torch.cuda.Stream(device=dev) for _ in range(max(1, min(int(copy_streams), batch)))]
             self.copy_stream = self.copy_streams[0]
-        self.plan = model.inference_plan(batch, height, width, dev)
+        self.plan = model.inference_plan(batch, height, width, dev, exact=True)
         if getattr(model, 'use_cuda_graph', True) and not self.plan.autotuned:
             self.plan.autotune()
         for i, hw in enumerate(self.plan.level_sizes):
