@@ -30,17 +30,20 @@ def _stale():
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-# conv_umma_kernel<MODE_3X3S2, 128>: the only instantiation with two 128-column accumulators (conv + fused shortcut); it spills part of them
-# (the last template argument: the launch reads a geometry table, lfd_plan_forward_extent)
-_STACK_EXEMPT = {'_ZN3lfd16conv_umma_kernelILi2ELi128ELb%dELb%dEEEvNS_14UmmaConvParamsE' % (f16, ext): 512 for f16 in (0, 1) for ext in (0, 1)}
 # kernels whose per-thread state must stay in registers (the soft-NMS kernel runs one iteration per candidate: a spill is paid K times)
 _STACK_GUARDED = ('conv_umma_kernel', 'stem4_kernel', 'soft_nms_kernel')
+# kernels whose wgmmas must be pipelined: every instantiation, no exemptions
+_WGMMA_GUARDED = ('conv_umma_kernel', 'stem4_kernel')
 _PTXAS_VERBOSE = ('conv_umma.cu', 'postprocess.cu')
 
 
 def _check_stack_frames(ptxas_log, limit=64):
     """The warp-specialised conv kernel keeps its accumulators and role state in registers; a large stack frame means a lambda
-    was not inlined or an array went to local memory, which slows the kernel severalfold.  Fail the build instead."""
+    was not inlined or an array went to local memory, which slows the kernel severalfold.  Fail the build instead.
+
+    Also fail it when ptxas serialised the wgmmas of a conv kernel (C7511 / C7512: too few registers for the wgmma pipeline; C7520:
+    a compiler-inserted warpgroup.arrive on a divergent path): every MMA then waits for the previous one to finish, and which
+    instantiations it hits changes with unrelated edits."""
     import re
     name = None
     for line in ptxas_log.splitlines():
@@ -48,11 +51,11 @@ def _check_stack_frames(ptxas_log, limit=64):
         if m:
             name = m.group(1)
         m = re.search(r'(\d+) bytes stack frame', line)
-        if m and name and any(k in name for k in _STACK_GUARDED) and int(m.group(1)) > _STACK_EXEMPT.get(name, limit):
-            raise RuntimeError('%s has a %s-byte stack frame (limit %d): registers went to local memory' % (name, m.group(1), _STACK_EXEMPT.get(name, limit)))
-        # ptxas warning C7520: it could not prove the wgmma pipeline safe and serialised every wgmma of the kernel
-        if 'C7520' in line and 'stem4_kernel' in line:
-            raise RuntimeError('ptxas serialised the wgmma instructions of the fused stem kernel:\n%s' % line)
+        if m and name and any(k in name for k in _STACK_GUARDED) and int(m.group(1)) > limit:
+            raise RuntimeError('%s has a %s-byte stack frame (limit %d): registers went to local memory' % (name, m.group(1), limit))
+        m = re.search(r'\((C75\d\d)\).*wgmma\.mma_async instructions are serialized.*\'(\S+)\'', line)
+        if m and any(k in m.group(2) for k in _WGMMA_GUARDED):
+            raise RuntimeError('ptxas serialised the wgmma instructions of %s (%s):\n%s' % (m.group(2), m.group(1), line))
 
 
 def build(force=False, verbose=False):

@@ -289,8 +289,11 @@ LFD_DEVINL void store_tile(const EpiCtx& e, const float* acc, int nc, const floa
     if (NCMAX == 128 && stat) stats_flush<128>(st, e.lane, stats);
 }
 
-template <int MODE, int COUT, bool F16, bool EXT>
+// DS: the launch carries the fused 1x1/s2 shortcut (MODE_3X3S2, p.Cout3 > 0).  The shortcut and the fused tail never meet in one launch;
+// with COUT = 128 a kernel that holds the code of both needs more registers than its 168: it spills and ptxas serialises its wgmmas.
+template <int MODE, int COUT, bool F16, bool EXT, bool DS>
 __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid_constant__ UmmaConvParams p) {
+    static_assert(!DS || MODE == MODE_3X3S2, "the fused shortcut belongs to a 3x3/s2 conv");
     constexpr int kProd = kProdThreads;
     constexpr int kThreads = kConvThreads;
     constexpr int TAPS = (MODE == MODE_3X3S1 || MODE == MODE_3X3S2) ? 9 : (MODE == MODE_STEM ? 3 : 1);
@@ -411,7 +414,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
         const int flat_valid = lg.Ho * p.Wo;      // MODE_FLAT: the rows of the valid extent, at the full pitch
 
         float acc[COUT / 2];
-        float acc3[MODE == MODE_3X3S2 ? COUT / 2 : 1];
+        float acc3[DS ? COUT / 2 : 1];
         uint32_t it = 0, store_count = 0, res_count = 0;
         for (int tile = blockIdx.x, lt = 0; tile < lg.num_tiles; tile += gridDim.x, ++lt) {
             for (int cc = 0; cc < n_cc; ++cc, ++it) {
@@ -431,10 +434,10 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                     for (int tap = 0; tap < TAPS; ++tap)
                         wgmma_ss<COUT, F16>(acc, adk + (uint32_t)tap_view<MODE>(tap), bdk + (uint32_t)(tap * b_tap), (cc | k16 | tap) != 0);
                 }
-                if (MODE == MODE_3X3S2 && p.Cout3) {
+                if constexpr (DS) {
                     // fused 1x1/s2 shortcut conv of the residual block: its input pixel is this conv's centre tap, so it
                     // is one more MMA per 16 channels on the operand that is already in shared memory
-                    wgmma_fence_regs<MODE == MODE_3X3S2 ? COUT / 2 : 1>(acc3);
+                    wgmma_fence_regs<COUT / 2>(acc3);
                     for (int k16 = 0; k16 < nk16; ++k16)
                         wgmma_ss<COUT, F16>(acc3, ad + (uint32_t)(k16 * a_k16) + (uint32_t)tap_view<MODE>(4),
                                             b2desc0 + (uint32_t)(((cc * cpc + 2 * k16) * COUT * 16) >> 4), (cc | k16) != 0);
@@ -442,7 +445,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                 wgmma_commit();
                 wgmma_wait<0>();
                 wgmma_fence_regs<COUT / 2>(acc);
-                if (MODE == MODE_3X3S2) wgmma_fence_regs<MODE == MODE_3X3S2 ? COUT / 2 : 1>(acc3);
+                if constexpr (DS) wgmma_fence_regs<COUT / 2>(acc3);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty[s]);     // this warp's part of the stage has been consumed
             }
@@ -467,7 +470,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
             // GroupNorm partial sums are taken over the STORED (16-bit) values, after residual and ReLU; one group = one 16-byte
             // chunk (8 channels)
             double* sdst = p.stats ? p.stats + (size_t)n * p.gn_groups * 2 : nullptr;
-            if (p.Cout2) {
+            if (!DS && p.Cout2) {
                 // fused 1x1 tail: D2[64 x Cout2] = round16(act(D + shift)) . W2, the A operand straight from the accumulator registers
                 uint32_t a2[COUT / 4];
 #pragma unroll
@@ -479,12 +482,14 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                         a2[4 * kk + q] = p.relu ? pack2_relu<F16>(x0, x1) : pack2<F16>(x0, x1);
                     }
                 }
-                float acc2[64];
-                wgmma_fence_regs<64>(acc2);
-                wgmma_fence();
-                // COUT / 16 MMAs of N = Cout2 and the store of Cout2 columns (the widths umma_conv_configure accepts for a stored tensor)
+                // COUT / 16 MMAs of N = Cout2 and the store of Cout2 columns (the widths umma_conv_configure accepts for a stored tensor).
+                // Each width has its own accumulator array: with one array shared by MMAs of different N, ptxas runs out of registers
+                // for the wgmma pipeline and serialises every wgmma of the kernel (warning C7511), the main loop's included.
                 auto tail = [&](auto n2) LFD_LAMBDA_INLINE {
                     constexpr int N2 = decltype(n2)::value;
+                    float acc2[N2 / 2];
+                    wgmma_fence_regs<N2 / 2>(acc2);
+                    wgmma_fence();
                     tail_mma<N2, COUT, F16>(acc2, a2, b2desc0);
                     wgmma_commit();
                     wgmma_wait<0>();
@@ -502,11 +507,9 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
             } else {
                 store_tile<MODE, COUT, F16>(e, acc, COUT, bias, (bool)p.relu, has_res, sdst,
                                             &p.tm_out, &p.tm_res, c0, c1, n, v0, v1, &res_bar[wg], store_count, res_count);
-                if constexpr (MODE == MODE_3X3S2) {
-                    if (p.Cout3)
-                        store_tile<MODE, COUT, F16>(e, acc3, COUT, bias2, false, false, nullptr, &p.tm_out3, nullptr, c0, c1, n, v0, v1,
-                                                    &res_bar[wg], store_count, res_count);
-                }
+                if constexpr (DS)
+                    store_tile<MODE, COUT, F16>(e, acc3, COUT, bias2, false, false, nullptr, &p.tm_out3, nullptr, c0, c1, n, v0, v1,
+                                                &res_bar[wg], store_count, res_count);
             }
         }
         if (e.wtid == 0) bulk_wait_all();   // all tile stores have been performed before the CTA retires
@@ -1350,10 +1353,17 @@ static cudaError_t launch_persistent(void (*kernel)(UmmaConvParams), bool* confi
     return cudaLaunchKernelEx(&cfg, kernel, p);
 }
 
-template <int MODE, int COUT, bool F16, bool EXT>
+template <int MODE, int COUT, bool F16, bool EXT, bool DS>
 static cudaError_t launch_mode_t(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
     static bool configured[kMaxDevices] = {};
-    return launch_persistent(conv_umma_kernel<MODE, COUT, F16, EXT>, configured, 224 * 1024, p, smem, grid, st);
+    return launch_persistent(conv_umma_kernel<MODE, COUT, F16, EXT, DS>, configured, 224 * 1024, p, smem, grid, st);
+}
+
+template <int MODE, int COUT, bool F16, bool EXT>
+static cudaError_t launch_mode_ds(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
+    if constexpr (MODE == MODE_3X3S2)
+        if (p.Cout3) return launch_mode_t<MODE, COUT, F16, EXT, true>(p, smem, grid, st);
+    return launch_mode_t<MODE, COUT, F16, EXT, false>(p, smem, grid, st);
 }
 
 template <bool F16, bool EXT>
@@ -1369,7 +1379,7 @@ static cudaError_t launch_stem4(const UmmaConvParams& p, size_t smem, int grid, 
 
 template <int MODE, int COUT, bool F16>
 static cudaError_t launch_mode_e(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
-    return p.ext ? launch_mode_t<MODE, COUT, F16, true>(p, smem, grid, st) : launch_mode_t<MODE, COUT, F16, false>(p, smem, grid, st);
+    return p.ext ? launch_mode_ds<MODE, COUT, F16, true>(p, smem, grid, st) : launch_mode_ds<MODE, COUT, F16, false>(p, smem, grid, st);
 }
 
 template <int MODE, int COUT>
@@ -1377,14 +1387,14 @@ static cudaError_t launch_mode(const UmmaConvParams& p, size_t smem, int grid, c
     return p.f16 ? launch_mode_e<MODE, COUT, true>(p, smem, grid, st) : launch_mode_e<MODE, COUT, false>(p, smem, grid, st);
 }
 
-// the output widths umma_conv_configure accepts per mode
+// the output widths umma_conv_configure accepts per mode (and only those are instantiated)
 template <int MODE>
 static cudaError_t launch_cout(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
     switch (p.Cout) {
-        case 16: if (MODE != MODE_3X3S1 && MODE != MODE_3X3S2) return launch_mode<MODE, 16>(p, smem, grid, st); break;
+        case 16: if constexpr (MODE != MODE_3X3S1 && MODE != MODE_3X3S2) return launch_mode<MODE, 16>(p, smem, grid, st); break;
         case 32: return launch_mode<MODE, 32>(p, smem, grid, st);
         case 64: return launch_mode<MODE, 64>(p, smem, grid, st);
-        case 128: if (MODE != MODE_STEM) return launch_mode<MODE, 128>(p, smem, grid, st); break;
+        case 128: if constexpr (MODE != MODE_STEM) return launch_mode<MODE, 128>(p, smem, grid, st); break;
     }
     return cudaErrorInvalidValue;
 }
