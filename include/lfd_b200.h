@@ -80,7 +80,8 @@ enum { LFD_DTYPE_BF16 = 0, LFD_DTYPE_FP16 = 1 };
  *              [8][64][8]; s3_shift / s3_relu).  Cin = 3, Cout = 64, ksize = 3, stride = 2; H x W = the image, Ho x Wo = the stem3
  *              output (two stride-2 steps); in_off ignored.  Every intermediate is rounded to bf16 exactly as the STEM0 + CONV pair
  *              path rounds it, so the output is bit-identical to it; the stem1 map never reaches HBM.  Sizes: lfd_stem4_query.
- *   CONV       ksize in {1,3}, stride in {1,2}, pad = ksize/2; y = conv(x) + shift (+res) (ReLU) -> bf16;
+ *   CONV       ksize in {1,3}, stride in {1,2}, pad = ksize/2; y = conv(x) + shift (+res) (ReLU) -> bf16; Cout in {16, 32, 48, 64, 128}
+ *              (3x3: from 32), Cin a multiple of 16; STEM0 Cout in {16, 32, 48, 64};
  *              weight = bf16 packed [Cin/cc][ksize^2][cc/8][Cout][8] with cc from lfd_conv_query, ALREADY MULTIPLIED by the
  *              per-output-channel scale (folded BatchNorm); `scale` must be NULL; `shift` (fp32 [Cout], may be NULL) is rounded
  *              to bf16 and added on the tensor core;
@@ -109,7 +110,8 @@ typedef struct lfd_op {
     const float* gamma;
     const float* beta;
     /* STEM0 / CONV only: a 1x1/s1 conv (Cout -> tail_cout) + scale/shift (+ReLU) fused behind this layer inside the same
-     * kernel; tail_weight = bf16 packed [Cout/8][tail_cout][8] (scale folded in, tail_scale must be NULL).  The stored tensor then has tail_cout channels and
+     * kernel; tail_weight = bf16 packed [Cout/8][tail_cout][8] (scale folded in, tail_scale must be NULL); tail_cout = 48 goes with Cout = 48
+     * only, and the other tail widths (16 / 32 / 64 / 128) with the other Cout.  The stored tensor then has tail_cout channels and
      * res_off / gn_groups / stats_off refer to it; the Cout-channel intermediate never reaches HBM.  0 = no tail. */
     int32_t tail_cout, tail_relu;
     const void* tail_weight;
@@ -135,7 +137,8 @@ typedef struct lfd_op {
     const float* s3_shift;
 } lfd_op;
 
-/* Tile / pipeline configuration the wgmma kernel will use for a conv (host only, no launch).
+/* Tile / pipeline configuration the wgmma kernel will use for a conv (host only, no launch).  Output widths: 16 / 32 / 48 / 64 / 128
+ * (3x3 from 32; tail_cout as for lfd_op); fails with LFD_ERR_UNSUPPORTED otherwise.
  * cc = input-channel chunk the weights must be packed with. */
 int lfd_conv_query(int N, int H, int W, int Cin, int Ho, int Wo, int Cout, int ksize, int stride, int tail_cout, int ds_cout, int* cc,
                    int* stages, int* weights_resident, int* num_tiles, int64_t* smem_bytes);

@@ -31,9 +31,9 @@ def _stale():
 
 
 # kernels whose per-thread state must stay in registers (the soft-NMS kernel runs one iteration per candidate: a spill is paid K times)
-_STACK_GUARDED = ('conv_umma_kernel', 'stem4_kernel', 'soft_nms_kernel')
+_STACK_GUARDED = ('conv_umma_kernel', 'conv_umma_c48_kernel', 'stem4_kernel', 'soft_nms_kernel')
 # kernels whose wgmmas must be pipelined: every instantiation, no exemptions
-_WGMMA_GUARDED = ('conv_umma_kernel', 'stem4_kernel')
+_WGMMA_GUARDED = ('conv_umma_kernel', 'conv_umma_c48_kernel', 'stem4_kernel')
 _PTXAS_VERBOSE = ('conv_umma.cu', 'postprocess.cu')
 
 

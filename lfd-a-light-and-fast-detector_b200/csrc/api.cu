@@ -308,7 +308,7 @@ static int check_op(const lfd_op& o) {
         case LFD_OP_STEM0:
             if (o.scale || o.tail_scale) return fail(LFD_ERR_INVALID, "conv scale must be folded into the packed weights (pass scale = NULL)");
             if (o.Cin != 3 || o.ksize != 3 || o.stride != 2) return fail(LFD_ERR_UNSUPPORTED, "stem0 supports 3x3/s2 on 3 input channels only (got Cin=%d k=%d s=%d)", o.Cin, o.ksize, o.stride);
-            if (o.Cout != 16 && o.Cout != 32 && o.Cout != 64) return fail(LFD_ERR_UNSUPPORTED, "stem0 Cout must be 16/32/64 (got %d)", o.Cout);
+            if (o.Cout != 16 && o.Cout != 32 && o.Cout != 48 && o.Cout != 64) return fail(LFD_ERR_UNSUPPORTED, "stem0 Cout must be 16/32/48/64 (got %d)", o.Cout);
             if (o.Ho != eh || o.Wo != ew) return fail(LFD_ERR_INVALID, "stem0 output size mismatch");
             break;
         case LFD_OP_STEM4:

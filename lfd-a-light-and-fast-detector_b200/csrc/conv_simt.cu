@@ -30,7 +30,9 @@ static constexpr int kS0PatchPitch = 66;
 template <int NG>  // NG = Cout / 8 channel groups
 __global__ void __launch_bounds__(kS0Threads) stem0_kernel(const Stem0Params p) {
     constexpr int PXP = kS0Threads / NG;   // pixels per pass
-    constexpr int PASSES = 128 / PXP;
+    constexpr int PASSES = (128 + PXP - 1) / PXP;
+    // NG = 6 (48 channels): 42 pixels per pass, 4 passes, and the last 4 threads idle; the power-of-two widths tile 128 exactly
+    constexpr bool kRagged = PXP * PASSES != 128 || PXP * NG != kS0Threads;
     __shared__ float patch[3 * kS0PatchH * kS0PatchPitch];
     __shared__ __align__(16) float wsm[27 * 64];
     const int tid = threadIdx.x;
@@ -81,6 +83,7 @@ __global__ void __launch_bounds__(kS0Threads) stem0_kernel(const Stem0Params p) 
 #pragma unroll
             for (int ps = 0; ps < PASSES; ++ps) {
                 const int lp = ps * PXP + lp0;
+                if (kRagged && (lp0 >= PXP || lp >= 128)) continue;
                 const int ly = lp / kS0TileW, lx = lp % kS0TileW;
                 const float x = patch[(ci * kS0PatchH + 2 * ly + kh) * kS0PatchPitch + 2 * lx + kw];
                 acc[ps][0] = fmaf(x, w0.x, acc[ps][0]); acc[ps][1] = fmaf(x, w0.y, acc[ps][1]);
@@ -96,6 +99,7 @@ __global__ void __launch_bounds__(kS0Threads) stem0_kernel(const Stem0Params p) 
 #pragma unroll
     for (int ps = 0; ps < PASSES; ++ps) {
         const int lp = ps * PXP + lp0;
+        if (kRagged && (lp0 >= PXP || lp >= 128)) continue;
         const int oy = oy0 + lp / kS0TileW, ox = ox0 + lp % kS0TileW;
         if (oy >= p.Ho || ox >= p.Wo) continue;
         float o[8];
@@ -115,6 +119,7 @@ cudaError_t stem0_launch(const Stem0Params& p, cudaStream_t st) {
     dim3 grid((p.Wo + kS0TileW - 1) / kS0TileW, (p.Ho + kS0TileH - 1) / kS0TileH, p.N);
     switch (p.Cout) {
         case 64: stem0_kernel<8><<<grid, kS0Threads, 0, st>>>(p); break;
+        case 48: stem0_kernel<6><<<grid, kS0Threads, 0, st>>>(p); break;
         case 32: stem0_kernel<4><<<grid, kS0Threads, 0, st>>>(p); break;
         case 16: stem0_kernel<2><<<grid, kS0Threads, 0, st>>>(p); break;
         default: return cudaErrorInvalidValue;

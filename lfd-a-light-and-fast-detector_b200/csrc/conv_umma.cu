@@ -209,7 +209,8 @@ struct EpiCtx {
 // Register accumulators (rows r0 / r0 + 8, NC <= NCMAX columns) (+shift) (+residual) (+ReLU) -> 16-bit staging rows in the TMA swizzle
 // layout -> one TMA tensor store per 64-channel panel (+ GroupNorm partial statistics of the stored values, NC == 128 only).
 // Staging rows are laid out the way the TMA engine expects for its swizzle modes: 128-byte panels [panel][64 rows][128 B] with the
-// 16-byte chunk index XORed by (row & 7) (SWIZZLE_128B); 64 / 32-byte rows use the 64B / 32B patterns.
+// 16-byte chunk index XORed by (row & 7) (SWIZZLE_128B); 64 / 32-byte rows use the 64B / 32B patterns.  The 96-byte rows of a
+// 48-channel tensor have no swizzle mode of their width: they are stored plainly, [64 rows][96 B] (SWIZZLE_NONE, see encode_one).
 template <int MODE, int NCMAX, bool F16>
 LFD_DEVINL void store_tile(const EpiCtx& e, const float* acc, int nc, const float* bias, bool relu, bool res, double* stats,
                            const CUtensorMap* tmap, const CUtensorMap* tmres, int c0, int c1, int n, bool v0, bool v1,
@@ -257,7 +258,7 @@ LFD_DEVINL void store_tile(const EpiCtx& e, const float* acc, int nc, const floa
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int row = e.r0 + 8 * h;
-                const uint32_t swz = row_bytes == 128 ? (row & 7) : (row_bytes == 64 ? ((row >> 1) & 3) : ((row >> 2) & 1));
+                const uint32_t swz = NCMAX == 48 ? 0u : (row_bytes == 128 ? (row & 7) : (row_bytes == 64 ? ((row >> 1) & 3) : ((row >> 2) & 1)));
                 const uint32_t addr = buf + (uint32_t)(j >> 3) * 8192u + (uint32_t)(row * row_bytes) + ((((uint32_t)j & 7u) ^ swz) << 4) + 4u * e.tq;
                 float x0 = acc[4 * j + 2 * h] + b0, x1 = acc[4 * j + 2 * h + 1] + b1;
                 if (res) {
@@ -291,8 +292,9 @@ LFD_DEVINL void store_tile(const EpiCtx& e, const float* acc, int nc, const floa
 
 // DS: the launch carries the fused 1x1/s2 shortcut (MODE_3X3S2, p.Cout3 > 0).  The shortcut and the fused tail never meet in one launch;
 // with COUT = 128 a kernel that holds the code of both needs more registers than its 168: it spills and ptxas serialises its wgmmas.
+// The body of conv_umma_kernel (COUT = 16 / 32 / 64 / 128) and of conv_umma_c48_kernel (COUT = 48); p is the kernel's parameter.
 template <int MODE, int COUT, bool F16, bool EXT, bool DS>
-__global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid_constant__ UmmaConvParams p) {
+LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
     static_assert(!DS || MODE == MODE_3X3S2, "the fused shortcut belongs to a 3x3/s2 conv");
     constexpr int kProd = kProdThreads;
     constexpr int kThreads = kConvThreads;
@@ -485,6 +487,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                 // COUT / 16 MMAs of N = Cout2 and the store of Cout2 columns (the widths umma_conv_configure accepts for a stored tensor).
                 // Each width has its own accumulator array: with one array shared by MMAs of different N, ptxas runs out of registers
                 // for the wgmma pipeline and serialises every wgmma of the kernel (warning C7511), the main loop's included.
+                // A 48-channel conv has the 48-channel tail only (the 'fast' stem's 1x1 48->48), the other widths never a 48-channel one.
                 auto tail = [&](auto n2) LFD_LAMBDA_INLINE {
                     constexpr int N2 = decltype(n2)::value;
                     float acc2[N2 / 2];
@@ -498,11 +501,15 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
                     store_tile<MODE, N2, F16>(e, acc2, N2, bias2, (bool)p.relu2, has_res, sdst,
                                               &p.tm_out, &p.tm_res, c0, c1, n, v0, v1, &res_bar[wg], store_count, res_count);
                 };
-                switch (p.Cout2) {
-                    case 16: tail(std::integral_constant<int, 16>()); break;
-                    case 32: tail(std::integral_constant<int, 32>()); break;
-                    case 64: tail(std::integral_constant<int, 64>()); break;
-                    default: tail(std::integral_constant<int, 128>()); break;
+                if constexpr (COUT == 48) {
+                    tail(std::integral_constant<int, 48>());
+                } else {
+                    switch (p.Cout2) {
+                        case 16: tail(std::integral_constant<int, 16>()); break;
+                        case 32: tail(std::integral_constant<int, 32>()); break;
+                        case 64: tail(std::integral_constant<int, 64>()); break;
+                        default: tail(std::integral_constant<int, 128>()); break;
+                    }
                 }
             } else {
                 store_tile<MODE, COUT, F16>(e, acc, COUT, bias, (bool)p.relu, has_res, sdst,
@@ -687,6 +694,19 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
         }
     }
     LFD_TL_END(p.tl);
+}
+
+template <int MODE, int COUT, bool F16, bool EXT, bool DS>
+__global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid_constant__ UmmaConvParams p) {
+    static_assert(COUT != 48, "48-channel outputs run in conv_umma_c48_kernel");
+    conv_umma_body<MODE, COUT, F16, EXT, DS>(p);
+}
+
+// The 48-channel layers (TrafficLight LFD-S: its stem and stage 0): m64n48k16 MMAs into 24 accumulators per thread, the 48-channel
+// tail only, and 96-byte output rows.  A symbol of its own, so that the set of conv_umma_kernel instantiations stays what it was.
+template <int MODE, bool F16, bool EXT, bool DS>
+__global__ void __launch_bounds__(kConvThreads, 1) conv_umma_c48_kernel(const __grid_constant__ UmmaConvParams p) {
+    conv_umma_body<MODE, 48, F16, EXT, DS>(p);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1127,8 +1147,8 @@ static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvPara
     else if (g.ksize == 3 && g.stride == 2) mode = MODE_3X3S2;
     else if (g.ksize == 1 && g.stride == 2) mode = MODE_1X1S2;
     else return -1;
-    // instantiated output widths (conv_umma_launch): 16 / 32 / 64 / 128 channels, 3x3 convs from 32
-    if (g.Cin % 16 || (g.Cout != 16 && g.Cout != 32 && g.Cout != 64 && g.Cout != 128)) return -1;
+    // instantiated output widths (conv_umma_launch): 16 / 32 / 48 / 64 / 128 channels, 3x3 convs from 32
+    if (g.Cin % 16 || (g.Cout != 16 && g.Cout != 32 && g.Cout != 48 && g.Cout != 64 && g.Cout != 128)) return -1;
     if ((mode == MODE_3X3S1 || mode == MODE_3X3S2) && g.Cout < 32) return -1;
     p.mode = mode;
     p.N = g.N; p.H = g.H; p.W = g.W; p.Cin = g.Cin; p.Ho = g.Ho; p.Wo = g.Wo; p.Cout = g.Cout;
@@ -1155,6 +1175,7 @@ static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvPara
     const int Cf = g.tail_cout > 0 ? g.tail_cout : g.Cout;
     if (g.ds_cout && (mode != MODE_3X3S2 || g.tail_cout || g.ds_cout != g.Cout)) return -6;
     if (g.tail_cout && (g.tail_cout % 16 || g.tail_cout > 128 || g.tail_cout < 16)) return -4;
+    if (g.tail_cout && (g.tail_cout == 48) != (g.Cout == 48)) return -4;   // a 48-channel conv has the 48-channel tail only
     const size_t staging = (size_t)nbuf * 128 * Cf * 2;   // [warpgroup][buffer][64 rows][Cf]
     // fixed head of the shared-memory map: barriers | [halo table] | shift | [tail shift] | staging (1 KB aligned)
     size_t hoff = kSmemTableOff;
@@ -1230,7 +1251,7 @@ static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvPara
     p.Cout2 = g.tail_cout;
     p.Cout3 = g.ds_cout;
     p.log2_cpr = ilog2(Cf / 8);
-    if ((1 << p.log2_cpr) != Cf / 8) return -3;       // stored channel count must be 16/32/64/128
+    if ((1 << p.log2_cpr) != Cf / 8 && Cf != 48) return -3;       // stored channel count must be 16/32/48/64/128
     size_t off = p.smem_ring_off + (size_t)p.stages * p.stage_bytes;
     p.smem_w2_off = (uint32_t)off; off += w2_bytes;
     *smem_bytes = off;
@@ -1295,13 +1316,17 @@ static EncodeTiledFn encode_fn() {
 }
 
 // One tensor map per stored tensor; the box is what ONE warpgroup moves: 64 tile rows (64 pixels of a flat tile, 8 x 8 of
-// a spatial one) x min(64, Cf) channels, shared-memory side in the matching swizzle mode.
+// a spatial one) x min(64, Cf) channels, shared-memory side in the matching swizzle mode.  A 48-channel tensor has 96-byte rows, which
+// no swizzle mode spans: its box is the whole row, unswizzled, so a store or a residual load covers channels 0-47 of its pixels and
+// nothing of the next pixel.
 static int encode_one(const UmmaConvParams& p, const void* ptr, CUtensorMap* tm) {
     EncodeTiledFn fn = encode_fn();
     if (!fn) return -1;
     const cuuint64_t Cf = p.Cf, HoWo = (cuuint64_t)p.Ho * p.Wo;
     const cuuint32_t inner = p.Cf < 64 ? p.Cf : 64;
-    const CUtensorMapSwizzle swz = inner * 2 >= 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (inner * 2 == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+    const CUtensorMapSwizzle swz = inner * 2 >= 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                 : (inner * 2 == 96 ? CU_TENSOR_MAP_SWIZZLE_NONE
+                                                    : (inner * 2 == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B));
     cuuint64_t dims[4], strides[3];
     cuuint32_t box[4], estr[4] = {1, 1, 1, 1};
     cuuint32_t rank;
@@ -1356,7 +1381,8 @@ static cudaError_t launch_persistent(void (*kernel)(UmmaConvParams), bool* confi
 template <int MODE, int COUT, bool F16, bool EXT, bool DS>
 static cudaError_t launch_mode_t(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
     static bool configured[kMaxDevices] = {};
-    return launch_persistent(conv_umma_kernel<MODE, COUT, F16, EXT, DS>, configured, 224 * 1024, p, smem, grid, st);
+    if constexpr (COUT == 48) return launch_persistent(conv_umma_c48_kernel<MODE, F16, EXT, DS>, configured, 224 * 1024, p, smem, grid, st);
+    else return launch_persistent(conv_umma_kernel<MODE, COUT, F16, EXT, DS>, configured, 224 * 1024, p, smem, grid, st);
 }
 
 template <int MODE, int COUT, bool F16, bool EXT>
@@ -1393,6 +1419,7 @@ static cudaError_t launch_cout(const UmmaConvParams& p, size_t smem, int grid, c
     switch (p.Cout) {
         case 16: if constexpr (MODE != MODE_3X3S1 && MODE != MODE_3X3S2) return launch_mode<MODE, 16>(p, smem, grid, st); break;
         case 32: return launch_mode<MODE, 32>(p, smem, grid, st);
+        case 48: return launch_mode<MODE, 48>(p, smem, grid, st);
         case 64: return launch_mode<MODE, 64>(p, smem, grid, st);
         case 128: if constexpr (MODE != MODE_STEM) return launch_mode<MODE, 128>(p, smem, grid, st); break;
     }

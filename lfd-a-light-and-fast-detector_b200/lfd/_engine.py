@@ -273,15 +273,16 @@ class InferencePlan(object):
         ds = list(block._downsample)
         c0, sc = pairs[0][0], ds[0]
         return (len(pairs) >= 2 and c0.kernel_size == (3, 3) and c0.stride == (2, 2) and sc.kernel_size == (1, 1) and sc.stride == (2, 2)
-                and sc.in_channels == c0.in_channels and sc.out_channels == c0.out_channels and c0.out_channels in (32, 64, 128)
+                and sc.in_channels == c0.in_channels and sc.out_channels == c0.out_channels and c0.out_channels in (32, 48, 64, 128)
                 and sc.groups == 1 and c0.groups == 1)
 
     @staticmethod
     def _can_tail(conv, nxt):
-        """nxt = (conv, norm, relu): a bias-free-or-not 1x1/s1 conv directly consuming `conv`'s output."""
+        """nxt = (conv, norm, relu): a bias-free-or-not 1x1/s1 conv directly consuming `conv`'s output.  A 48-channel conv takes a
+        48-channel tail only (the 'fast' stem of TrafficLight LFD-S)."""
         c2 = nxt[0]
         return (c2.kernel_size == (1, 1) and c2.stride == (1, 1) and c2.groups == 1 and c2.in_channels == conv.out_channels
-                and conv.out_channels in (32, 64) and c2.out_channels in (32, 64, 128))
+                and ((conv.out_channels in (32, 64) and c2.out_channels in (32, 64, 128)) or (conv.out_channels == 48 and c2.out_channels == 48)))
 
     def _emit_stem0(self, conv, norm, relu, out_name, h, w, tail=None):
         if conv.in_channels != 3 or conv.kernel_size != (3, 3) or conv.stride != (2, 2):

@@ -116,6 +116,7 @@ class TrainPlan(object):
     """Forward (train mode) + backward op lists for a fixed input shape."""
 
     def __init__(self, model, N, H, W, device, create_native=True):
+        self._check_widths(model)
         self.N, self.H, self.W, self.device = N, H, W, device
         self.model = model
         self.create_native = create_native               # False: host-side planning only (CPU tests of the planner)
@@ -138,6 +139,15 @@ class TrainPlan(object):
         self._finalize()
 
     # ------------------------------------------------------------------ checks
+    @staticmethod
+    def _check_widths(model):
+        """48-channel layers (TrafficLight LFD-S) run for inference only.  Training them needs a weight gradient with 48 input
+        channels, which even a fully frozen backbone's level-0 neck conv needs, a 48-channel BatchNorm backward and a data gradient
+        into 48 channels; none of them exists yet."""
+        for m in model.modules():
+            if isinstance(m, nn.Conv2d) and 48 in (m.in_channels, m.out_channels):
+                raise NotImplementedError('native training of 48-channel layers is not implemented (%r); the model runs for inference only' % (m,))
+
     @staticmethod
     def _check_supported(model):
         for m in model.modules():
