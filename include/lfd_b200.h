@@ -69,6 +69,16 @@ enum { LFD_CONV_UMMA = 0, LFD_CONV_SIMT = 1 }; /* SIMT = cross-check kernel, val
  * dtype of BASELINE config 5 (WIDERFACE-XS fp16 4K sweep).  "bf16" in the op descriptions below reads "the plan's 16-bit type". */
 enum { LFD_DTYPE_BF16 = 0, LFD_DTYPE_FP16 = 1 };
 
+/* The input transform of the ops that read the uint8 image (lfd_op: STEM0, STEM4; lfd_top: STEM0, WGRAD_STEM; an INFER op carries its
+ * lfd_op's): in_swap_rb (0 / 1), in_mean[3], in_scale[3] in float32, indexed by NETWORK input channel:
+ *     input channel c of a pixel = ((float) byte[in_swap_rb ? 2 - c : c] - in_mean[c]) * in_scale[c]     (fp32: a subtract, then a multiply)
+ * which is albumentations' Normalize (mean[c] = mean * max_pixel_value, scale[c] = float32(1 / (std * max_pixel_value))) after an optional
+ * BGR -> RGB, so the 16-bit value a stem kernel builds for a pixel is the rounding of the fp32 number the host pipeline would have uploaded.
+ * Pixels outside the image (conv padding, beyond a smaller frame's extent) are 0 after the transform.  ALL SEVEN FIELDS ZERO selects
+ * simple_normalize on BGR, mean 127.5 and scale float32(1 / 127.5): a zero-filled struct behaves as the library always did.  Anything else
+ * must be complete: in_swap_rb 0 or 1, every mean finite, every scale finite and non-zero; otherwise the op fails with LFD_ERR_INVALID when
+ * it is planned, before anything is enqueued.  The LFD_INPUT_F32_NCHW input is taken as it is and ignores these fields. */
+
 /* One fused layer.  Activations are bf16 NHWC at byte offsets into the caller's workspace.
  *   STEM0      3x3/s2 conv on the 3-channel image + shift (+ReLU), scale folded into the weights like CONV; in_off ignored (reads the external input);
  *              weight = bf16 packed [kh][2][Cout][8]: element (kh, kc, n, j) = weight of output n, input channel j % 4, filter
@@ -135,6 +145,11 @@ typedef struct lfd_op {
     const float* s2_shift;
     const void* s3_weight;
     const float* s3_shift;
+    /* STEM0 / STEM4 on a LFD_INPUT_U8_NHWC image: the input transform (see below).  All zero = simple_normalize on BGR. */
+    int32_t in_swap_rb;
+    float in_mean[3];
+    float in_scale[3];
+    int32_t pad2_;
 } lfd_op;
 
 /* Tile / pipeline configuration the wgmma kernel will use for a conv (host only, no launch).  Output widths: 16 / 32 / 48 / 64 / 128
@@ -368,6 +383,12 @@ typedef struct lfd_top {
     float eps, momentum;
     int64_t off[8];
     const void* ptr[6];
+    /* STEM0 / WGRAD_STEM on a LFD_INPUT_U8_NHWC image: the input transform, as in lfd_op (all zero = simple_normalize on BGR).  The forward's
+     * STEM0 and the backward's WGRAD_STEM of one step must carry the same one. */
+    int32_t in_swap_rb;
+    float in_mean[3];
+    float in_scale[3];
+    int32_t pad2_;
 } lfd_top;
 
 /* entries of the PACK / UNPACK tables (device memory, absolute pointers) */

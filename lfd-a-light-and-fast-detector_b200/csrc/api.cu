@@ -1,5 +1,6 @@
 // api.cu -- the extern "C" boundary of liblfd_b200.so (declared in include/lfd_b200.h).
 #include <stdarg.h>
+#include <cmath>
 #include <stdio.h>
 
 #include <vector>
@@ -45,6 +46,7 @@ struct PlannedOp {
     UmmaConvParams cp;  // CONV via wgmma
     size_t smem;
     int grid;
+    InputTransform xf;  // STEM0 / STEM4 (and a training plan's WGRAD_STEM): the op's input transform with the all-zero default resolved
 };
 
 // Stream the CUDA graphs are captured on: the main chain (the backbone: the critical path of the step) runs two priority levels above
@@ -300,6 +302,27 @@ extern "C" int lfd_stem4_query(int N, int H, int W, int* num_tiles, int64_t* sme
     return LFD_OK;
 }
 
+// The input transform of an op as the kernels take it (constants by byte position, kernels.cuh) from the C-ABI's fields (by network
+// channel, see lfd_op): all seven fields zero = simple_normalize on BGR; anything else has to be a complete transform.  One place for
+// lfd_op and lfd_top.
+static int input_transform_of(int32_t swap, const float* mean, const float* scale, InputTransform* out) {
+    bool zero = swap == 0;
+    for (int c = 0; c < 3; ++c) zero = zero && mean[c] == 0.f && scale[c] == 0.f;
+    if (zero) {
+        out->swap = 0;
+        for (int c = 0; c < 3; ++c) { out->mean[c] = 127.5f; out->scale[c] = 1.0f / 127.5f; }
+        return LFD_OK;
+    }
+    if (swap != 0 && swap != 1) return fail(LFD_ERR_INVALID, "input transform: in_swap_rb = %d (0 or 1)", swap);
+    for (int c = 0; c < 3; ++c)
+        if (!std::isfinite(mean[c]) || !std::isfinite(scale[c]) || scale[c] == 0.f)
+            return fail(LFD_ERR_INVALID, "input transform: channel %d has mean %g, scale %g (set all of in_swap_rb / in_mean / in_scale with finite means and "
+                        "finite non-zero scales, or none of them)", c, (double)mean[c], (double)scale[c]);
+    out->swap = swap;
+    for (int m = 0; m < 3; ++m) { out->mean[m] = mean[swap ? 2 - m : m]; out->scale[m] = scale[swap ? 2 - m : m]; }   // by byte position
+    return LFD_OK;
+}
+
 static int check_op(const lfd_op& o) {
     const int eh = (o.H + 2 * (o.ksize / 2) - o.ksize) / (o.stride > 0 ? o.stride : 1) + 1;
     const int ew = (o.W + 2 * (o.ksize / 2) - o.ksize) / (o.stride > 0 ? o.stride : 1) + 1;
@@ -350,6 +373,10 @@ static int plan_op(const lfd_op& o, PlannedOp* out) {
     out->op = o;
     out->smem = 0;
     out->grid = 0;
+    if (o.kind == LFD_OP_STEM0 || o.kind == LFD_OP_STEM4) {
+        rc = input_transform_of(o.in_swap_rb, o.in_mean, o.in_scale, &out->xf);
+        if (rc) return rc;
+    }
     if (o.kind == LFD_OP_CONV || o.kind == LFD_OP_STEM0 || o.kind == LFD_OP_STEM4) {
         rc = umma_conv_configure(geom_of(o), sm_count() > 0 ? sm_count() : 132, &out->cp, &out->smem, &out->grid);
         if (rc) return fail(LFD_ERR_UNSUPPORTED, "conv %dx%d s%d Cin=%d Cout=%d unsupported (rc=%d)", o.ksize, o.ksize, o.stride, o.Cin, o.Cout, rc);
@@ -376,10 +403,13 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
                 p.in = input; p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off);
                 p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift;
                 p.input_format = input_format; p.N = o.N; p.H = o.H; p.W = o.W; p.Ho = o.Ho; p.Wo = o.Wo; p.Cout = o.Cout; p.relu = o.relu; p.f16 = o.dtype;
+                p.xf = po.xf;
                 CUDA_TRY(stem0_launch(p, st));
             } else {
                 UmmaConvParams p = po.cp;
                 p.in_raw = input; p.input_format = input_format; p.in = nullptr;
+                p.xf = po.xf;
+                if (input_format != LFD_INPUT_U8_NHWC) p.xf.swap = 0;   // the loaders order the channels at the load: fp32 planes are taken as they are
                 p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off); p.res = nullptr;
                 p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift; p.stats = nullptr;
                 p.relu = o.relu; p.gn_groups = 0; p.trace = g_trace; p.tl = tl; p.f16 = o.dtype;
@@ -395,6 +425,8 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
             if (conv_impl == LFD_CONV_SIMT) return fail(LFD_ERR_UNSUPPORTED, "the SIMT cross-check kernels do not implement the fused stem (plan its four convs)");
             UmmaConvParams p = po.cp;
             p.in_raw = input; p.input_format = input_format; p.in = nullptr;
+            p.xf = po.xf;
+            if (input_format != LFD_INPUT_U8_NHWC) p.xf.swap = 0;
             p.in_words = input_format == LFD_INPUT_U8_NHWC && o.W % 4 == 0 && (reinterpret_cast<uintptr_t>(input) & 3) == 0;
             p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off); p.res = nullptr; p.stats = nullptr;
             p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift; p.relu = o.relu;
@@ -899,6 +931,9 @@ static lfd_op conv_op_of(const lfd_top& t) {
     o.ds_out_off = -1;
     o.dtype = LFD_DTYPE_BF16;
     o.max_ctas = t.max_ctas;
+    o.in_swap_rb = t.in_swap_rb;
+    memcpy(o.in_mean, t.in_mean, sizeof(o.in_mean));
+    memcpy(o.in_scale, t.in_scale, sizeof(o.in_scale));
     return o;
 }
 
@@ -935,8 +970,10 @@ static int plan_top(const lfd_top& t, int64_t ws_bytes, PlannedTop* out) {
             if (!t.ptr[0] || t.n_desc < 0 || t.max_n < 0) return fail(LFD_ERR_INVALID, "pack / unpack: missing table");
             break;
         case LFD_TOP_BN_STATS: case LFD_TOP_BN_APPLY: case LFD_TOP_GN_APPLY: case LFD_TOP_HEAD_FINAL: case LFD_TOP_HEAD_FINAL_BWD:
-        case LFD_TOP_NORM_BWD_REDUCE: case LFD_TOP_NORM_BWD_APPLY: case LFD_TOP_WGRAD_STEM: case LFD_TOP_ZERO:
+        case LFD_TOP_NORM_BWD_REDUCE: case LFD_TOP_NORM_BWD_APPLY: case LFD_TOP_ZERO:
             break;
+        case LFD_TOP_WGRAD_STEM:
+            return input_transform_of(t.in_swap_rb, t.in_mean, t.in_scale, &out->conv.xf);
         default:
             return fail(LFD_ERR_INVALID, "unknown training op kind %d", t.kind);
     }
@@ -1058,11 +1095,11 @@ static int launch_top(const PlannedTop& pt, const void* input, int fmt, uint8_t*
                 // tensor-core path: im2col into the scratch tensor X27 [N][Ho][Wo][32] at off[0], then the 1x1 wgrad (32 -> Cout) over it;
                 // the staging at off[5] must hold 32 rows of Cout floats (rows 27..31 stay zero)
                 __nv_bfloat16* x27 = at<__nv_bfloat16>(ws, t.off[0]);
-                CUDA_TRY(stem_im2col_launch(g, input, fmt, x27, sms, st));
+                CUDA_TRY(stem_im2col_launch(g, input, fmt, pt.conv.xf, x27, sms, st));
                 WgradGeom g1 = {t.N, t.Ho, t.Wo, 32, t.Ho, t.Wo, t.Cout, 1, 1};
                 CUDA_TRY(wgrad_umma_launch(g1, x27, at<const __nv_bfloat16>(ws, t.off[1]), at<float>(ws, t.off[5]), sms, st));
             } else {
-                CUDA_TRY(wgrad_stem_launch(g, input, fmt, at<const __nv_bfloat16>(ws, t.off[1]), at<float>(ws, t.off[5]), sms, st));
+                CUDA_TRY(wgrad_stem_launch(g, input, fmt, pt.conv.xf, at<const __nv_bfloat16>(ws, t.off[1]), at<float>(ws, t.off[5]), sms, st));
             }
             break;
         }

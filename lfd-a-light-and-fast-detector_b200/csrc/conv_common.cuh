@@ -5,6 +5,7 @@
 #include <cuda_bf16.h>
 #include <stdint.h>
 #include <string.h>
+#include "kernels.cuh"
 
 namespace lfd {
 
@@ -62,6 +63,7 @@ struct alignas(64) UmmaConvParams {
     uint32_t smem_table_off, smem_bias_off, smem_bias2_off, smem_staging_off;
     uint32_t smem_w_off, smem_ring_off;
     int input_format;
+    InputTransform xf;          // MODE_STEM / MODE_STEM4, u8 NHWC image: byte -> network input (constant bank; xf.swap is 0 for fp32 input)
     int f16;                    // activation / weight type: 0 = bf16, 1 = IEEE fp16 (same bytes, same tensor-core rate)
     // MODE_STEM4: stem0 = w / shift / relu, stem1 = w2 / shift2 / relu2 (the tail fields), stem2 = its 3x3/s2 weights packed
     // [9][8][64][8] + shift + ReLU, stem3 = its 1x1 weights packed [8][64][8] + shift + ReLU; H1 x W1 = the stem1 map

@@ -28,7 +28,7 @@ static constexpr int kS0PatchW = 2 * kS0TileW + 1;       // 65
 static constexpr int kS0PatchPitch = 66;
 
 template <int NG>  // NG = Cout / 8 channel groups
-__global__ void __launch_bounds__(kS0Threads) stem0_kernel(const Stem0Params p) {
+__global__ void __launch_bounds__(kS0Threads) stem0_kernel(const __grid_constant__ Stem0Params p) {
     constexpr int PXP = kS0Threads / NG;   // pixels per pass
     constexpr int PASSES = (128 + PXP - 1) / PXP;
     // NG = 6 (48 channels): 42 pixels per pass, 4 passes, and the last 4 threads idle; the power-of-two widths tile 128 exactly
@@ -59,8 +59,8 @@ __global__ void __launch_bounds__(kS0Threads) stem0_kernel(const Stem0Params p) 
             if (p.input_format == 0) {
                 v = reinterpret_cast<const float*>(p.in)[(((size_t)n * 3 + ci) * p.H + y) * p.W + x];
             } else {
-                float u = (float)reinterpret_cast<const uint8_t*>(p.in)[(((size_t)n * p.H + y) * p.W + x) * 3 + ci];
-                v = (u - 127.5f) * (1.0f / 127.5f);
+                const int m = p.xf.swap ? 2 - ci : ci;
+                v = p.xf.apply(m, reinterpret_cast<const uint8_t*>(p.in)[(((size_t)n * p.H + y) * p.W + x) * 3 + m]);
             }
             v = round16_rt(v, p.f16);
         }

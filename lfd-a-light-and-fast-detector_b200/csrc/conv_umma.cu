@@ -598,10 +598,11 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
                     float f[3];
 #pragma unroll
                     for (int k = 0; k < 3; ++k) {
-                        f[k] = u8 ? ((float)raw[j][k] - 127.5f) * (1.0f / 127.5f) : __uint_as_float(raw[j][k]);
+                        f[k] = u8 ? p.xf.apply(k, raw[j][k]) : __uint_as_float(raw[j][k]);
                         if (!((okmask >> j) & 1u)) f[k] = 0.f;        // conv zero padding (of the normalised image)
                     }
-                    const uint32_t lo = pack2<F16>(f[0], f[1]), hi = pack2<F16>(f[2], 0.f);   // rounding point R0
+                    const bool sw = p.xf.swap;           // u8 BGR -> RGB: the normalised bytes 0 and 2 change places
+                    const uint32_t lo = pack2<F16>(sw ? f[2] : f[0], f[1]), hi = pack2<F16>(sw ? f[0] : f[2], 0.f);   // rounding point R0
                     asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(dst0 + j * (kProdThreads * 8)), "r"(lo), "r"(hi) : "memory");
                 }
                 fence_proxy_async_smem();       // generic-proxy st.shared -> wgmma reads
@@ -1023,6 +1024,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
         asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
         const int ptid = tid - kConsumerThreads;
         const bool u8 = p.input_format == 1;
+        const bool sw = p.xf.swap;       // u8 BGR -> RGB: the normalised bytes 0 and 2 of a pixel change places
         const int plane = p.H * p.W;
         pdl_wait();
         int tile0, tile1;
@@ -1072,10 +1074,10 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
 #pragma unroll
                             for (int c = 0; c < 3; ++c) {
                                 const uint32_t byte = (wd[j][(3 * k + c) >> 2] >> (8 * ((3 * k + c) & 3))) & 0xffu;
-                                f[c] = okk ? ((float)byte - 127.5f) * (1.0f / 127.5f) : 0.f;     // zero padding of the normalised image
+                                f[c] = okk ? p.xf.apply(c, byte) : 0.f;                              // zero padding of the normalised image
                             }
-                            px[k][0] = pack2<F16>(f[0], f[1]);                                       // rounding point R0
-                            px[k][1] = pack2<F16>(f[2], 0.f);
+                            px[k][0] = pack2<F16>(sw ? f[2] : f[0], f[1]);                           // rounding point R0
+                            px[k][1] = pack2<F16>(sw ? f[0] : f[2], 0.f);
                         }
                         const uint32_t d = dst0 + (uint32_t)(r * kS4RowBytes + 32 * g);              // patch column 4g, 16-byte aligned
                         if (g > 0) asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(d - 8u), "r"(px[0][0]), "r"(px[0][1]) : "memory");
@@ -1115,10 +1117,10 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                         float f[3];
 #pragma unroll
                         for (int k = 0; k < 3; ++k) {
-                            f[k] = u8 ? ((float)raw[j][k] - 127.5f) * (1.0f / 127.5f) : __uint_as_float(raw[j][k]);
+                            f[k] = u8 ? p.xf.apply(k, raw[j][k]) : __uint_as_float(raw[j][k]);
                             if (!ok[j]) f[k] = 0.f;             // conv zero padding (of the normalised image)
                         }
-                        const uint32_t lo = pack2<F16>(f[0], f[1]), hi = pack2<F16>(f[2], 0.f);   // rounding point R0
+                        const uint32_t lo = pack2<F16>(sw ? f[2] : f[0], f[1]), hi = pack2<F16>(sw ? f[0] : f[2], 0.f);   // rounding point R0
                         asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(dst0 + q * 8), "r"(lo), "r"(hi) : "memory");
                     }
                 }

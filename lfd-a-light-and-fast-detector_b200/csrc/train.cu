@@ -721,7 +721,7 @@ cudaError_t head_final_bwd_launch(const HeadFinalBwdParams& p, int num_sms, cuda
 // ===================================================================================================
 static constexpr int kWsSeg = 64, kWsCols = 2 * kWsSeg + 1;
 
-__global__ void __launch_bounds__(256) wgrad_stem_kernel(WgradGeom g, const void* __restrict__ image, int input_format,
+__global__ void __launch_bounds__(256) wgrad_stem_kernel(WgradGeom g, const void* __restrict__ image, int input_format, const __grid_constant__ InputTransform xf,
                                                          const __nv_bfloat16* __restrict__ dz, float* __restrict__ dstage) {
     __shared__ float patch[3][3][kWsCols + 3];   // [ci][kh][column]
     const int Cout = g.Cout;
@@ -742,7 +742,7 @@ __global__ void __launch_bounds__(256) wgrad_stem_kernel(WgradGeom g, const void
             const int y = iy0 + kh, x = ix0 + c;
             float v = 0.f;
             if ((unsigned)y < (unsigned)g.H && (unsigned)x < (unsigned)g.W) {
-                if (input_format == 1) v = ((float)reinterpret_cast<const uint8_t*>(image)[((size_t)n * plane + (size_t)y * g.W + x) * 3 + ci] - 127.5f) * (1.0f / 127.5f);
+                if (input_format == 1) { const int m = xf.swap ? 2 - ci : ci; v = xf.apply(m, reinterpret_cast<const uint8_t*>(image)[((size_t)n * plane + (size_t)y * g.W + x) * 3 + m]); }
                 else v = reinterpret_cast<const float*>(image)[((size_t)n * 3 + ci) * plane + (size_t)y * g.W + x];
                 v = bf16_round(v);
             }
@@ -770,19 +770,20 @@ __global__ void __launch_bounds__(256) wgrad_stem_kernel(WgradGeom g, const void
     }
 }
 
-cudaError_t wgrad_stem_launch(const WgradGeom& g, const void* image, int input_format, const __nv_bfloat16* dz, float* dstage, int num_sms, cudaStream_t st) {
+cudaError_t wgrad_stem_launch(const WgradGeom& g, const void* image, int input_format, const InputTransform& xf, const __nv_bfloat16* dz, float* dstage, int num_sms, cudaStream_t st) {
     if (g.Cin != 3 || g.ksize != 3 || g.stride != 2 || 256 % g.Cout || g.Cout < 16 || g.Cout > 64) return cudaErrorInvalidValue;
     const int n_seg = g.N * g.Ho * ((g.Wo + kWsSeg - 1) / kWsSeg);
     int blocks = 4 * num_sms;
     if (blocks > n_seg) blocks = n_seg;
-    wgrad_stem_kernel<<<blocks, 256, 0, st>>>(g, image, input_format, dz, dstage);
+    wgrad_stem_kernel<<<blocks, 256, 0, st>>>(g, image, input_format, xf, dz, dstage);
     return cudaGetLastError();
 }
 
 // im2col of the 3-channel stem conv for its weight gradient: X27[n][oy][ox][q] with q = (kh*3 + kw)*3 + ci (q >= 27: zero) as bf16, the
 // image normalised + rounded like the forward does (R0).  The weight gradient of the stem conv is then the weight gradient of a 1x1 conv
 // with 32 input channels over X27, i.e. one launch of the tensor-core wgrad kernel; its staging rows [q][co] ARE the [tap][ci][co] layout.
-__global__ void __launch_bounds__(256) stem_im2col_kernel(WgradGeom g, const void* __restrict__ image, int input_format, __nv_bfloat16* __restrict__ x27) {
+__global__ void __launch_bounds__(256) stem_im2col_kernel(WgradGeom g, const void* __restrict__ image, int input_format, const __grid_constant__ InputTransform xf,
+                                                          __nv_bfloat16* __restrict__ x27) {
     const size_t total = (size_t)g.N * g.Ho * g.Wo * 4;          // one thread per (output pixel, 8-value chunk)
     const size_t plane = (size_t)g.H * g.W;
     for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (size_t)gridDim.x * 256) {
@@ -798,7 +799,7 @@ __global__ void __launch_bounds__(256) stem_im2col_kernel(WgradGeom g, const voi
                 const int ci = q % 3, t = q / 3;
                 const int y = 2 * oy + t / 3 - 1, x = 2 * ox + t % 3 - 1;
                 if ((unsigned)y < (unsigned)g.H && (unsigned)x < (unsigned)g.W) {
-                    if (input_format == 1) f = ((float)reinterpret_cast<const uint8_t*>(image)[((size_t)n * plane + (size_t)y * g.W + x) * 3 + ci] - 127.5f) * (1.0f / 127.5f);
+                    if (input_format == 1) { const int m = xf.swap ? 2 - ci : ci; f = xf.apply(m, reinterpret_cast<const uint8_t*>(image)[((size_t)n * plane + (size_t)y * g.W + x) * 3 + m]); }
                     else f = reinterpret_cast<const float*>(image)[((size_t)n * 3 + ci) * plane + (size_t)y * g.W + x];
                 }
             }
@@ -808,12 +809,12 @@ __global__ void __launch_bounds__(256) stem_im2col_kernel(WgradGeom g, const voi
     }
 }
 
-cudaError_t stem_im2col_launch(const WgradGeom& g, const void* image, int input_format, __nv_bfloat16* x27, int num_sms, cudaStream_t st) {
+cudaError_t stem_im2col_launch(const WgradGeom& g, const void* image, int input_format, const InputTransform& xf, __nv_bfloat16* x27, int num_sms, cudaStream_t st) {
     if (g.Cin != 3 || g.ksize != 3 || g.stride != 2) return cudaErrorInvalidValue;
     const size_t total = (size_t)g.N * g.Ho * g.Wo * 4;
     size_t blocks = (total + 255) / 256;
     if (blocks > (size_t)num_sms * 16) blocks = (size_t)num_sms * 16;
-    stem_im2col_kernel<<<(int)blocks, 256, 0, st>>>(g, image, input_format, x27);
+    stem_im2col_kernel<<<(int)blocks, 256, 0, st>>>(g, image, input_format, xf, x27);
     return cudaGetLastError();
 }
 

@@ -11,6 +11,7 @@
 #include <stdint.h>
 
 #include "../../include/lfd_b200.h"
+#include "kernels.cuh"
 
 namespace lfd {
 
@@ -110,8 +111,8 @@ cudaError_t wgrad_umma_launch(const WgradGeom& g, const __nv_bfloat16* x, const 
 cudaError_t wgrad_simt_launch(const WgradGeom& g, const __nv_bfloat16* x, const __nv_bfloat16* dz, float* dstage, cudaStream_t st);
 // the 3-channel stem conv: x is the raw image (fp32 NCHW or u8 NHWC, normalised + rounded to bf16 like the forward does)
 // im2col of the stem conv's input for the tensor-core path: X27 bf16 [N][Ho][Wo][32] (27 (tap, ci) values + 5 zeros per output pixel)
-cudaError_t stem_im2col_launch(const WgradGeom& g, const void* image, int input_format, __nv_bfloat16* x27, int num_sms, cudaStream_t st);
-cudaError_t wgrad_stem_launch(const WgradGeom& g, const void* image, int input_format, const __nv_bfloat16* dz, float* dstage, int num_sms, cudaStream_t st);
+cudaError_t stem_im2col_launch(const WgradGeom& g, const void* image, int input_format, const InputTransform& xf, __nv_bfloat16* x27, int num_sms, cudaStream_t st);
+cudaError_t wgrad_stem_launch(const WgradGeom& g, const void* image, int input_format, const InputTransform& xf, const __nv_bfloat16* dz, float* dstage, int num_sms, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------------
 // optimizer: clip_grad_norm_ + SGD(momentum, weight decay) over flat fp32 buffers

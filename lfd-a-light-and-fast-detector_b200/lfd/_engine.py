@@ -188,10 +188,14 @@ def place_tensors(ops, sizes, arenas, hold=(), skip=()):
 class InferencePlan(object):
     """One native forward plan for a fixed input shape."""
 
-    def __init__(self, model, N, H, W, device, conv_impl=nat.CONV_UMMA, create_native=True, act_dtype='bf16', fuse_stem=None):
+    def __init__(self, model, N, H, W, device, conv_impl=nat.CONV_UMMA, create_native=True, act_dtype='bf16', fuse_stem=None,
+                 input_transform=None):
         """fuse_stem: run a four-conv 'faster' stem as one kernel (LFD_OP_STEM4) -- None: when its stem1 map would not stay in
-        L2 (see _use_stem4), True / False: always / never (tests).  LFD_B200_NO_STEM_FUSION=1 turns it off."""
+        L2 (see _use_stem4), True / False: always / never (tests).  LFD_B200_NO_STEM_FUSION=1 turns it off.
+        input_transform: what the stem op makes of uint8 frames -- None: simple_normalize on BGR, else an InputTransform
+        (lfd/data_pipeline/augmentation.py).  float32 NCHW input is taken as it is."""
         self._configure(N, H, W, device, conv_impl, create_native, act_dtype, fuse_stem)
+        self.input_transform = input_transform
         self._build(model)
         self._finalize()
 
@@ -215,6 +219,7 @@ class InferencePlan(object):
         # conv -> 1x1 conv pairs run as ONE kernel (tensor-core kernels only; the SIMT cross-check runs them unfused)
         self.fuse_tails = conv_impl == nat.CONV_UMMA and not os.environ.get('LFD_B200_NO_TAIL')
         self.fuse_stem = fuse_stem
+        self.input_transform = None
 
     # ------------------------------------------------------------------ parameter staging
     def _add_f32(self, t):
@@ -605,6 +610,8 @@ class InferencePlan(object):
             o.ds_weight = bb + 2 * op['ds_w']
             o.ds_shift = fb + 4 * op['ds_shift']
             o.ds_out_off = offsets[op['out2']]
+        if op['kind'] in (nat.OP_STEM0, nat.OP_STEM4):
+            nat.set_input_transform(o, self.input_transform)
         if op['kind'] == nat.OP_STEM4:
             o.s2_weight, o.s2_shift, o.s2_relu = bb + 2 * op['s2_w'], fb + 4 * op['s2_shift'], op['s2_relu']
             o.s3_weight, o.s3_shift, o.s3_relu = bb + 2 * op['s3_w'], fb + 4 * op['s3_shift'], op['s3_relu']
@@ -812,8 +819,9 @@ class PrefixEmitter(InferencePlan):
     BatchNorm folding, weight packing and fusion decisions (STEM4 gate, fused tails and shortcuts), bf16, every op on the main stream.
     The training plan places the ops in its own workspace and runs them as LFD_TOP_INFER ops."""
 
-    def __init__(self, N, H, W, device):
+    def __init__(self, N, H, W, device, input_transform=None):
         self._configure(N, H, W, device, nat.CONV_UMMA, False, 'bf16', None)
+        self.input_transform = input_transform
         self.aux_shortcut = False
 
     def staged(self):

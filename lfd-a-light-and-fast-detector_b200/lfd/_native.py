@@ -43,7 +43,8 @@ class Op(C.Structure):
                 ('ds_cout', C.c_int32), ('dtype', C.c_int32), ('max_ctas', C.c_int32), ('pad_', C.c_int32), ('ds_out_off', C.c_int64),
                 ('ds_weight', C.c_void_p), ('ds_shift', C.c_void_p),
                 ('s2_relu', C.c_int32), ('s3_relu', C.c_int32),
-                ('s2_weight', C.c_void_p), ('s2_shift', C.c_void_p), ('s3_weight', C.c_void_p), ('s3_shift', C.c_void_p)]
+                ('s2_weight', C.c_void_p), ('s2_shift', C.c_void_p), ('s3_weight', C.c_void_p), ('s3_shift', C.c_void_p),
+                ('in_swap_rb', C.c_int32), ('in_mean', C.c_float * 3), ('in_scale', C.c_float * 3), ('pad2_', C.c_int32)]
 
 
 class PostCfg(C.Structure):
@@ -99,7 +100,19 @@ class Top(C.Structure):
                 ('point_off', C.c_int32), ('P', C.c_int32), ('cls_stride', C.c_int32),
                 ('accumulate', C.c_int32), ('upH', C.c_int32), ('upW', C.c_int32), ('n_desc', C.c_int32), ('max_n', C.c_int32),
                 ('impl', C.c_int32), ('frozen', C.c_int32), ('branch', C.c_int32), ('wait_mask', C.c_int32), ('max_ctas', C.c_int32), ('eps', C.c_float), ('momentum', C.c_float),
-                ('off', C.c_int64 * 8), ('ptr', C.c_void_p * 6)]
+                ('off', C.c_int64 * 8), ('ptr', C.c_void_p * 6),
+                ('in_swap_rb', C.c_int32), ('in_mean', C.c_float * 3), ('in_scale', C.c_float * 3), ('pad2_', C.c_int32)]
+
+
+def set_input_transform(o, transform):
+    """The input transform fields of an Op (STEM0 / STEM4) or a Top (STEM0 / WGRAD_STEM): transform = None leaves them zero, which the
+    library reads as simple_normalize on BGR; else an InputTransform (lfd/data_pipeline/augmentation.py): swap_rb and the float32 mean
+    and scale of each network input channel."""
+    if transform is None:
+        return
+    o.in_swap_rb = int(transform.swap_rb)
+    o.in_mean[:] = transform.mean
+    o.in_scale[:] = transform.scale
 
 
 class Extent(C.Structure):

@@ -119,6 +119,7 @@ class TrainPlan(object):
         self._check_widths(model)
         self.N, self.H, self.W, self.device = N, H, W, device
         self.model = model
+        self.input_transform = getattr(model, 'input_transform', None)    # of uint8 batches: the stem conv, its weight gradient, the frozen prefix's stem
         self.create_native = create_native               # False: host-side planning only (CPU tests of the planner)
         self.branches = os.environ.get('LFD_B200_TRAIN_BRANCHES', '1') != '0'      # per-level chains on side streams (0: one stream, A/B runs)
         self.flat = flat_parameters(model, allow_cpu=not create_native)
@@ -354,7 +355,7 @@ class TrainPlan(object):
     def _emit_prefix(self, model, n_units):
         """The first n_units backbone units on the inference plan's emitters -> (emitter, [(first op, end op, output, h, w) per unit])."""
         bb = model._backbone
-        pre = PrefixEmitter(self.N, self.H, self.W, self.device)
+        pre = PrefixEmitter(self.N, self.H, self.W, self.device, self.input_transform)
         cur, h, w = pre._emit_stem(bb.stem_layers(), self.H, self.W)
         units = [(0, len(pre._ops), cur, h, w)]
         blocks = [('s%db%d' % (si, bi), block) for si, stage in enumerate(bb.stages()) for bi, block in enumerate(stage)]
@@ -739,6 +740,8 @@ class TrainPlan(object):
                 t = arr[i]
                 for j in range(8):
                     t.off[j] = -1
+                if op['kind'] in (nat.TOP_STEM0, nat.TOP_WGRAD_STEM):
+                    nat.set_input_transform(t, self.input_transform)
                 for key, v in op.items():
                     if key == 'off':
                         for j, o in v.items():

@@ -1,4 +1,5 @@
 # -*- coding: utf-8 -*-
+import collections
 import random
 
 import numpy
@@ -120,6 +121,29 @@ def pipeline_device_spec(pipeline, with_bboxes):
         except Exception:
             return None
     return compose.device_spec() if isinstance(compose, Compose) else None
+
+
+# What the stem kernels can do to a uint8 BGR frame while they read it: network input channel c of a pixel =
+# (float32(byte[2 - c if swap_rb else c]) - mean[c]) * scale[c], i.e. BGR2RGB.apply (optional) then Normalize.apply.  mean / scale: 3-tuples
+# of floats holding float32 values (Normalize.constants()); hashable, so a transform can be part of a plan's cache key.
+InputTransform = collections.namedtuple('InputTransform', 'swap_rb mean scale')
+__all__ += ['InputTransform', 'input_transform_of']
+
+
+def input_transform_of(pipeline, allow_flip=False):
+    """pipeline -> the InputTransform the stem kernels run in its place; None -> None (the kernels' default, simple_normalize on BGR); an
+    InputTransform is returned as it is.  Raises ValueError for a pipeline Compose.device_spec() cannot express, and for one with a
+    HorizontalFlip unless allow_flip (the training loader, whose input kernel does the flip before the stem sees the batch)."""
+    if pipeline is None or isinstance(pipeline, InputTransform):
+        return pipeline
+    spec = pipeline_device_spec(pipeline, False)
+    if spec is None:
+        raise ValueError('the stem kernels cannot run this pipeline on uint8 frames: it must be a Compose (or a function that picks one by the '
+                         "sample's keys) of BGR2RGB and one final Normalize, each with p = 1 (got %r)" % (pipeline,))
+    flip_p, swap, mean, scale = spec
+    if flip_p is not None and not allow_flip:
+        raise ValueError('the stem kernels cannot run a HorizontalFlip (p = %g): the input transform is a channel swap and a normalisation' % flip_p)
+    return InputTransform(bool(swap), tuple(float(v) for v in mean), tuple(float(v) for v in scale))
 
 
 random_horizon_flip = HorizontalFlip(p=0.5)

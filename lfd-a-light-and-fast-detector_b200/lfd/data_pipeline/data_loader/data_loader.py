@@ -28,7 +28,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy
 import torch
 
-from ..augmentation import pipeline_device_spec
+from ..augmentation import input_transform_of, pipeline_device_spec
 from ..dataset import reserved_keys
 from ..sampler.region_sampler import apply_draw, resize_plan, RESIZE_AREA2, RESIZE_LINEAR
 
@@ -165,7 +165,12 @@ class _Slot(object):
 
 class DataLoader(object):
 
-    def __init__(self, dataset, dataset_sampler, region_sampler, augmentation_pipeline=None, num_workers=1):
+    def __init__(self, dataset, dataset_sampler, region_sampler, augmentation_pipeline=None, num_workers=1, model_normalizes=False):
+        """model_normalizes: the model's stem kernels run the pipeline's channel swap and normalisation (LFD.set_input_transform with
+        this loader's `input_transform`; Executor.train does that): batches of equal-size crops are then raw uint8 BGR NHWC, a quarter of
+        the bytes, for every pipeline the input kernel can run.  The flip stays in the input kernel.  A batch with crops of different
+        sizes is float32 NCHW, normalised here, as without the argument (its zero padding is zero AFTER normalisation, which no byte
+        expresses); the model takes float32 batches as they are."""
         self._dataset = dataset
         self._dataset_sampler = dataset_sampler
         self._loops = len(dataset_sampler)
@@ -180,6 +185,11 @@ class DataLoader(object):
             (_, sw0, m0, s0), (_, sw1, m1, s1) = specs[False], specs[True]
             native = sw0 == sw1 and numpy.array_equal(m0, m1) and numpy.array_equal(s0, s1)
         self._specs = specs if native else None
+        if model_normalizes and not native:
+            raise ValueError('model_normalizes needs a region sampler with draw() and a pipeline the input kernel can run (flip, BGR2RGB, a final Normalize)')
+        # what the model has to do to this loader's uint8 batches; None: simple_normalize on BGR, the only pipeline that gives uint8 batches
+        # without model_normalizes
+        self.input_transform = input_transform_of(augmentation_pipeline, allow_flip=True) if model_normalizes else None
         self._slots = [_Slot(), _Slot()]
         self._stream = None
         self.last_stats = None   # host timings / bytes of the last native batch (tests/debug_input_timing.py)
@@ -294,9 +304,11 @@ class DataLoader(object):
         if self._stream is None:
             self._stream = torch.cuda.Stream(device)
         self._stream.wait_stream(torch.cuda.current_stream(device))
-        u8 = (not swap and all(d.crop[2] == W and d.crop[3] == H for _, d, _ in items) and
-              numpy.array_equal(mean, numpy.full(3, 127.5, numpy.float32)) and
-              numpy.array_equal(scale, numpy.full(3, numpy.float32(1.0) / numpy.float32(127.5), numpy.float32)))
+        u8 = all(d.crop[2] == W and d.crop[3] == H for _, d, _ in items) and (self.input_transform is not None or (
+            not swap and numpy.array_equal(mean, numpy.full(3, 127.5, numpy.float32)) and
+            numpy.array_equal(scale, numpy.full(3, numpy.float32(1.0) / numpy.float32(127.5), numpy.float32))))
+        if u8:
+            swap = False     # raw BGR bytes: with model_normalizes the swap happens in the stem kernel
         with torch.cuda.stream(self._stream):
             staged = torch.empty(off, dtype=torch.uint8, device=device)
             staged.copy_(buf[:off], non_blocking=True)

@@ -123,10 +123,17 @@ class Executor(object):
         """This rank's share of a batch: a RankLocalBatch already is one (the loader built only this rank's images)."""
         return tuple(data_batch) if isinstance(data_batch, RankLocalBatch) else shard_batch(data_batch)
 
+    def _set_input_transform(self, loader):
+        """A loader that leaves channel order and normalisation to the model (DataLoader(model_normalizes=True)) says which: its uint8
+        batches mean nothing without it.  A DataLoader without the argument resets the model to the default its uint8 batches assume."""
+        if hasattr(loader, 'input_transform') and hasattr(self.config_dict['model'], 'set_input_transform'):
+            self.config_dict['model'].set_input_transform(loader.input_transform)
+
     def train(self):
         cfg = self.config_dict
         cfg['mode'] = 'train'
         cfg['model'].train()
+        self._set_input_transform(cfg['train_data_loader'])
         self._call_hooks('before_train_epoch')
         for i, data_batch in enumerate(cfg['train_data_loader']):
             cfg.update(inner_train_iter=i)
@@ -151,6 +158,7 @@ class Executor(object):
         cfg = self.config_dict
         cfg['mode'] = 'val'
         cfg['model'].eval()
+        self._set_input_transform(cfg['val_data_loader'])
         self._call_hooks('before_val_epoch')
         for i, data_batch in enumerate(cfg['val_data_loader']):
             cfg.update(inner_val_iter=i)

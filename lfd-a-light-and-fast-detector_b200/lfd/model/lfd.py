@@ -128,6 +128,7 @@ class LFD(nn.Module):
         self._train_plans = {}
         self._plan_fingerprint = None
         self.conv_impl = nat.CONV_UMMA
+        self.input_transform = None            # what the stem kernels make of uint8 frames (set_input_transform); None: simple_normalize on BGR
         self.act_dtype = 'bf16'                # 16-bit storage type of the inference plan: 'bf16' or 'fp16' (lfd/_engine.py)
         self.use_cuda_graph = True
         self.max_detections_per_image = 8192   # candidate / output capacity of the device post-process
@@ -140,6 +141,16 @@ class LFD(nn.Module):
     def _fingerprint(self):
         return tuple((t.data_ptr(), t._version) for t in list(self.parameters()) + list(self.buffers()))
 
+    def set_input_transform(self, pipeline):
+        """How uint8 NHWC (BGR) input is normalised inside the stem kernels, in eval and in train mode: None = simple_normalize
+        ((x/255 - 0.5)/0.5 on BGR), or a pipeline of the declarative stand-ins (lfd/data_pipeline/augmentation.py: BGR2RGB and a final
+        Normalize, or a function that picks such a Compose by the sample's keys), e.g. the TrafficLight val_pipeline or
+        typical_coco_val_pipeline.  The kernels then build, per pixel, the 16-bit rounding of the very fp32 number the pipeline produces
+        on the host, so uint8 frames give the results of the float32 NCHW batch the pipeline makes of them.  Raises ValueError for a
+        pipeline the kernels cannot run (a flip, another transform, an opaque function).  float32 input is unaffected."""
+        from ..data_pipeline.augmentation import input_transform_of
+        self.input_transform = input_transform_of(pipeline)
+
     def train_plan_for(self, n, h, w, device):
         """The native training plan (forward + backward op lists) for one input shape (built on first use)."""
         from .._train import TrainPlan, flat_parameters
@@ -147,7 +158,7 @@ class LFD(nn.Module):
         # BatchNorm modules in eval mode (norm_eval, frozen stages) normalise with their running statistics, and frozen parameters
         # (requires_grad False) get no gradient ops and may form a prefix on the inference kernels: both are part of the plan
         key = (n, h, w, str(device), tuple(m.training for m in self.modules() if isinstance(m, nn.BatchNorm2d)),
-               tuple(p.requires_grad for p in self.parameters()))
+               tuple(p.requires_grad for p in self.parameters()), self.input_transform)
         if key not in self._train_plans:
             self._train_plans[key] = TrainPlan(self, n, h, w, device)
             self._train_plans[key].use_graph = bool(getattr(self, 'use_cuda_graph_training', False))
@@ -165,7 +176,7 @@ class LFD(nn.Module):
         fp = self._fingerprint()
         if fp != self._plan_fingerprint:
             self._plans, self._plan_fingerprint = {}, fp
-        rest = (str(device), self.conv_impl, self.act_dtype)
+        rest = (str(device), self.conv_impl, self.act_dtype, self.input_transform)
         key = (n, h, w) + rest
         if key in self._plans:
             return self._plans[key]
@@ -177,11 +188,12 @@ class LFD(nn.Module):
             for k in same:
                 if k[1] <= h and k[2] <= w:
                     del self._plans[k]
-        self._plans[key] = InferencePlan(self, n, h, w, device, self.conv_impl, act_dtype=self.act_dtype)
+        self._plans[key] = InferencePlan(self, n, h, w, device, self.conv_impl, act_dtype=self.act_dtype, input_transform=self.input_transform)
         return self._plans[key]
 
     def forward(self, x):
-        """x: float32 [N,3,H,W] (reference contract) or uint8 [N,H,W,3] BGR (normalisation fused), on CUDA.
+        """x: float32 [N,3,H,W] (reference contract) or uint8 [N,H,W,3] BGR (channel order and normalisation fused into the stem kernel:
+        set_input_transform), on CUDA.
         -> (classification [N,P,C'], regression [N,P,4]) float32."""
         if not x.is_cuda:
             raise RuntimeError('lfd_b200 has no CPU path: move the model and the input to a CUDA (H100) device')
@@ -493,17 +505,27 @@ class LFD(nn.Module):
 
     def predict_for_single_image(self, image, aug_pipeline, classification_threshold=None, nms_threshold=None,
                                  class_agnostic=False, cuda_device_index=0):
-        """reference :544-655.  `aug_pipeline=None` takes the fused path: the uint8 BGR image goes to the device as is and
-        `simple_normalize` ((x/255-0.5)/0.5, augmentation_pipeline.py:31-36) happens inside the stem kernel; a callable
-        pipeline is applied on the host exactly like the reference does."""
+        """reference :544-655.  A uint8 HxWx3 image takes the fused path when the stem kernels can run `aug_pipeline`: None (the model's
+        own set_input_transform setting, by default simple_normalize, augmentation_pipeline.py:31-36), or BGR2RGB / a final Normalize of
+        the declarative stand-ins.  The image then goes to the device as it is, 3 bytes per pixel, and is normalised inside the stem
+        kernel to the same 16-bit values, so the rows are those of the host path.  Any other pipeline or image is processed on the host
+        exactly like the reference does."""
         assert isinstance(image, str) or isinstance(image, numpy.ndarray)
         if isinstance(image, str):
             import cv2
             image = cv2.imread(image, cv2.IMREAD_UNCHANGED)
             assert image is not None, 'image is None, confirm that the path is valid!'
         device = torch.device('cuda', cuda_device_index)
-        if aug_pipeline is None:
-            if image.dtype != numpy.uint8 or image.ndim != 3 or image.shape[2] != 3:
+        from ..data_pipeline.augmentation import input_transform_of
+        fusable = image.dtype == numpy.uint8 and image.ndim == 3 and image.shape[2] == 3
+        transform = self.input_transform
+        if aug_pipeline is not None and fusable:
+            try:
+                transform = input_transform_of(aug_pipeline)
+            except ValueError:
+                fusable = False
+        if aug_pipeline is None or fusable:
+            if not fusable:
                 raise ValueError('the fused input path expects a uint8 HxWx3 (BGR) image')
             data = torch.from_numpy(numpy.ascontiguousarray(image))[None].to(device)
             height, width = image.shape[0], image.shape[1]
@@ -517,8 +539,12 @@ class LFD(nn.Module):
             height, width = data.size(2), data.size(3)
         self.cuda(cuda_device_index)
         self.eval()
-        with torch.no_grad():
-            outputs = self.forward(data)
+        own, self.input_transform = self.input_transform, transform      # for this call only
+        try:
+            with torch.no_grad():
+                outputs = self.forward(data)
+        finally:
+            self.input_transform = own
         thr = classification_threshold if classification_threshold is not None else self._classification_threshold
         if nms_threshold:
             self._nms_cfg.update({'iou_thr': nms_threshold})

@@ -80,7 +80,13 @@ class ForwardPostPipeline(object):
 
 class StreamingDetector(object):
 
-    def __init__(self, model, batch, height, width, score_thr, iou_thr, max_out=1024, device=None, depth=3, copy_streams=4):
+    def __init__(self, model, batch, height, width, score_thr, iou_thr, max_out=1024, device=None, depth=3, copy_streams=4,
+                 input_pipeline=None):
+        """input_pipeline: the model's val pipeline, run on the uint8 frames inside the stem kernel -- None: simple_normalize on BGR;
+        else BGR2RGB / a final Normalize of the declarative stand-ins (lfd/data_pipeline/augmentation.py), e.g. the TrafficLight
+        val_pipeline.  A pipeline the kernels cannot run raises ValueError here: frames are never normalised other than asked."""
+        from .data_pipeline.augmentation import input_transform_of
+        self.input_transform = input_transform_of(input_pipeline)
         self.model = model
         self.depth = max(2, int(depth))     # batches in flight: copy of i+2 | forward of i+1 | post-process + read-back of i
         self.device = device if device is not None else next(model.parameters()).device
@@ -94,7 +100,11 @@ class StreamingDetector(object):
             # The copy itself costs the forward ~8 %: 0.561 ms per step with the input copy left out, tests/debug_e2e_timeline.py)
             self.copy_streams = [torch.cuda.Stream(device=dev) for _ in range(max(1, min(int(copy_streams), batch)))]
             self.copy_stream = self.copy_streams[0]
-        self.plan = model.inference_plan(batch, height, width, dev, exact=True)
+        own, model.input_transform = getattr(model, 'input_transform', None), self.input_transform
+        try:
+            self.plan = model.inference_plan(batch, height, width, dev, exact=True)
+        finally:
+            model.input_transform = own
         if getattr(model, 'use_cuda_graph', True) and not self.plan.autotuned:
             self.plan.autotune()
         for i, hw in enumerate(self.plan.level_sizes):
