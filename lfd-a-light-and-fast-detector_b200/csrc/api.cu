@@ -52,11 +52,11 @@ struct PlannedOp {
 // Stream the CUDA graphs are captured on: the main chain (the backbone: the critical path of the step) runs two priority levels above
 // the side streams of the per-level chains (created at the default = lowest level) -- captured kernel nodes inherit the level, so when
 // SMs free up the pending CTAs of the critical path are placed first.  The levels above are left to the caller's latency-critical
-// streams (lfd/pipeline.py runs the post-process of the previous batch there).  LFD_B200_GRAPH_PRIO=0 disables it (A/B runs).
+// streams (lfd/pipeline.py runs the post-process of the previous batch there).  A device that reports no priority range gets a
+// stream at the default level.
 static cudaError_t create_capture_stream(cudaStream_t* cap) {
-    static const bool prio = !(getenv("LFD_B200_GRAPH_PRIO") && atoi(getenv("LFD_B200_GRAPH_PRIO")) == 0);
     int least = 0, greatest = 0;
-    if (prio && cudaDeviceGetStreamPriorityRange(&least, &greatest) == cudaSuccess && greatest < least) {
+    if (cudaDeviceGetStreamPriorityRange(&least, &greatest) == cudaSuccess && greatest < least) {
         const int level = least - 2 < greatest ? greatest : least - 2;     // numerically lower = higher priority
         return cudaStreamCreateWithPriority(cap, cudaStreamNonBlocking, level);
     }

@@ -11,7 +11,7 @@
 //                      reg 4 channels, bias, per-level Scale; lfd_head.py:137-143,164-185) writing fp32 straight
 //                      into the (N, P, C') / (N, P, 4) layout of lfd/model/lfd.py:526-540.
 //   simt_conv_kernel   direct convolution with the same packed weights and epilogue semantics as conv_umma.cu;
-//                      used only to cross-check the tensor-core kernel (tests, LFD_B200_CONV_IMPL=simt).
+//                      used only to cross-check the tensor-core kernel (tests, conv_impl = LFD_CONV_SIMT).
 #include "conv_common.cuh"
 #include "kernels.cuh"
 #include "ptx.cuh"

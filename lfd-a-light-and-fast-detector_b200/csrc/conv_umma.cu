@@ -1215,11 +1215,6 @@ static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvPara
     };
     // (16-channel chunks mean 32-byte global segments per pixel and twice the barrier round trips per tile, so a 2-deep ring of
     //  32-channel stages is preferred to a 4-deep one of 16)
-    static const int force_cc = getenv("LFD_B200_FORCE_CC") ? atoi(getenv("LFD_B200_FORCE_CC")) : 0;   // experiments only
-    if (force_cc && mode == MODE_3X3S2) {
-        int st = stages_for(force_cc, 1);
-        if (st >= 2) { best_cc = force_cc; best_res = 1; best_st = st; }
-    }
     for (int pass = 0; pass < 3 && !best_cc; ++pass)
         for (int ci = 0; ci < 3 && !best_cc; ++ci) {
             const int want = pass == 0 ? 3 : 2;
@@ -1365,7 +1360,6 @@ static cudaError_t launch_persistent(void (*kernel)(UmmaConvParams), bool* confi
         if (e != cudaSuccess) return e;
         configured[dev] = true;
     }
-    static const bool use_pdl = getenv("LFD_B200_NO_PDL") == nullptr;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(grid);
@@ -1376,7 +1370,7 @@ static cudaError_t launch_persistent(void (*kernel)(UmmaConvParams), bool* confi
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = use_pdl ? 1 : 0;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, p);
 }
 

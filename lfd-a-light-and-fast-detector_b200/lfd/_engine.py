@@ -16,7 +16,6 @@ Rounding points of the bf16 pipeline (mirrored by oracle/lfd_oracle.py forward(e
       to bf16 again; the final cls / reg outputs are fp32.
 """
 import ctypes as C
-import os
 import time
 
 import torch
@@ -188,16 +187,20 @@ def place_tensors(ops, sizes, arenas, hold=(), skip=()):
 class InferencePlan(object):
     """One native forward plan for a fixed input shape."""
 
+    # the per-level neck + head chains and the unfused residual shortcut convs run on side branches (graph branches / side streams)
+    side_branches = True
+
     def __init__(self, model, N, H, W, device, conv_impl=nat.CONV_UMMA, create_native=True, act_dtype='bf16', fuse_stem=None,
-                 input_transform=None):
+                 input_transform=None, reuse=True):
         """fuse_stem: run a four-conv 'faster' stem as one kernel (LFD_OP_STEM4) -- None: when its stem1 map would not stay in
-        L2 (see _use_stem4), True / False: always / never (tests).  LFD_B200_NO_STEM_FUSION=1 turns it off.
+        L2 (see _use_stem4), True / False: always / never (tests).
         input_transform: what the stem op makes of uint8 frames -- None: simple_normalize on BGR, else an InputTransform
-        (lfd/data_pipeline/augmentation.py).  float32 NCHW input is taken as it is."""
+        (lfd/data_pipeline/augmentation.py).  float32 NCHW input is taken as it is.
+        reuse: False gives every tensor its own workspace region, so that tensor() can read any intermediate after a forward (tests)."""
         self._configure(N, H, W, device, conv_impl, create_native, act_dtype, fuse_stem)
         self.input_transform = input_transform
         self._build(model)
-        self._finalize()
+        self._finalize(reuse)
 
     def _configure(self, N, H, W, device, conv_impl, create_native, act_dtype, fuse_stem):
         self.N, self.H, self.W = N, H, W
@@ -213,11 +216,9 @@ class InferencePlan(object):
         self._ops = []                       # dicts; tensors referenced by name
         self._tensors = {}                   # name -> bytes
         self._branch = 0                     # branch id given to the ops being emitted (0 = main stream)
-        self.concurrent_levels = not os.environ.get('LFD_B200_NO_BRANCHES')
-        self.aux_shortcut = not os.environ.get('LFD_B200_NO_AUX')
-        self.fuse_shortcuts = conv_impl == nat.CONV_UMMA and not os.environ.get('LFD_B200_NO_FUSED_SHORTCUT')
-        # conv -> 1x1 conv pairs run as ONE kernel (tensor-core kernels only; the SIMT cross-check runs them unfused)
-        self.fuse_tails = conv_impl == nat.CONV_UMMA and not os.environ.get('LFD_B200_NO_TAIL')
+        # conv -> 1x1 conv pairs and 1x1/s2 shortcuts run inside the conv they follow / share their input with (tensor-core kernels
+        # only; the SIMT cross-check runs them unfused)
+        self.fuse = conv_impl == nat.CONV_UMMA
         self.fuse_stem = fuse_stem
         self.input_transform = None
 
@@ -313,7 +314,7 @@ class InferencePlan(object):
         """A 'faster' stem (3x3/s2 3->64, 1x1, 3x3/s2 64->64, 1x1, all 64 channels) runs as one kernel when its stem1 map -- the
         tensor the fusion keeps out of HBM -- would not stay in L2 between the two fused pairs (more than half of it).  Smaller
         plans have no HBM round trip to remove and keep the two-kernel path."""
-        if not self.fuse_tails or self.fuse_stem is False or os.environ.get('LFD_B200_NO_STEM_FUSION') or len(layers) != 4:
+        if not self.fuse or self.fuse_stem is False or len(layers) != 4:
             return False
         (c0, _, _), (c1, _, _), (c2, _, _), (c3, _, _) = layers
 
@@ -397,7 +398,7 @@ class InferencePlan(object):
         while i < len(layers):
             conv, norm, relu = layers[i]
             tail = None
-            if self.fuse_tails and i + 1 < len(layers) and self._can_tail(conv, layers[i + 1]):
+            if self.fuse and i + 1 < len(layers) and self._can_tail(conv, layers[i + 1]):
                 tail = layers[i + 1]
             name = 'stem%d' % (i + (1 if tail is not None else 0))      # a fused pair is named after its last layer
             if i == 0:
@@ -414,7 +415,7 @@ class InferencePlan(object):
         aux = False
         pairs = block.conv_norm_pairs()
         fuse_sc = None
-        if block._downsample is not None and self.fuse_shortcuts and self._can_fuse_shortcut(block, pairs):
+        if block._downsample is not None and self.fuse and self._can_fuse_shortcut(block, pairs):
             ds = list(block._downsample)
             fuse_sc = (ds[0], ds[1] if len(ds) > 1 else None, base + '_id')
             identity = base + '_id'
@@ -422,7 +423,7 @@ class InferencePlan(object):
             # the 1x1/s2 shortcut conv only depends on the block input: it runs on the auxiliary branch, next to the
             # block's first conv, and the block's last conv (which adds it) waits for it
             ds = list(block._downsample)
-            aux = self.concurrent_levels and self.aux_shortcut and n_taps + 1 <= _AUX_BRANCH
+            aux = self.side_branches and n_taps + 1 <= _AUX_BRANCH
             if aux:
                 self._branch = _AUX_BRANCH
             self._emit_conv(ds[0], ds[1] if len(ds) > 1 else None, False, cur, base + '_id', h, w)
@@ -458,7 +459,7 @@ class InferencePlan(object):
                     assert (h, w) == self.level_sizes[l]
                     # the level's neck + head chain only depends on this tap: run it on its own stream / graph branch,
                     # concurrently with the rest of the backbone and with the other levels
-                    self._branch = 1 + l if (self.concurrent_levels and 1 + l < 8) else 0
+                    self._branch = 1 + l if (self.side_branches and 1 + l < 8) else 0
                     self._emit_level(neck, head, l, cur, h, w, offs[l], cache)
                     self._branch = 0
 
@@ -469,7 +470,7 @@ class InferencePlan(object):
         # merged heads: the neck's 1x1 conv (+BN+ReLU) has ONE consumer, the tower's first 1x1 conv -- run the pair as one kernel (the
         # 128-channel neck output never reaches HBM; the GroupNorm statistics are taken on the fused kernel's output as usual)
         t0 = cls_tower[0] if len(cls_tower) else None
-        fuse_neck = (self.fuse_tails and not os.environ.get('LFD_B200_NO_NECK_TAIL') and cls_tower is reg_tower and t0 is not None
+        fuse_neck = (self.fuse and cls_tower is reg_tower and t0 is not None
                      and conv.kernel_size == (1, 1) and conv.stride == (1, 1) and conv.groups == 1 and conv.out_channels == 128
                      and t0[0].kernel_size == (1, 1) and t0[0].stride == (1, 1) and t0[0].groups == 1 and t0[0].bias is None
                      and t0[0].in_channels == 128 and t0[0].out_channels == 128
@@ -547,7 +548,7 @@ class InferencePlan(object):
         return cache[key]
 
     # ------------------------------------------------------------------ memory plan + native plan
-    def _finalize(self):
+    def _finalize(self, reuse):
         dev = self.device
         self.params_f32 = torch.cat(self._f32).to(dev) if self._f32 else torch.zeros(4, device=dev)
         self.params_bf16 = torch.cat(self._bf16).to(dev) if self._bf16 else torch.zeros(8, dtype=torch.int16, device=dev)
@@ -560,7 +561,7 @@ class InferencePlan(object):
         # a tensor read by another branch (a backbone tap) lives for the whole forward
         shared = {op[k] for op in self._ops for k in ('inp', 'res') if op.get(k) is not None and producer[op[k]] != op['branch']}
         arenas = [_Arena() for _ in range(1 + max(op['branch'] for op in self._ops))]
-        local = place_tensors(self._ops, self._tensors, arenas, hold=set(self._tensors) if os.environ.get('LFD_B200_NO_REUSE') else shared)
+        local = place_tensors(self._ops, self._tensors, arenas, hold=shared if reuse else set(self._tensors))
         bases, top = [], self.stats_bytes
         for a in arenas:
             bases.append(top)
@@ -819,10 +820,11 @@ class PrefixEmitter(InferencePlan):
     BatchNorm folding, weight packing and fusion decisions (STEM4 gate, fused tails and shortcuts), bf16, every op on the main stream.
     The training plan places the ops in its own workspace and runs them as LFD_TOP_INFER ops."""
 
+    side_branches = False
+
     def __init__(self, N, H, W, device, input_transform=None):
         self._configure(N, H, W, device, nat.CONV_UMMA, False, 'bf16', None)
         self.input_transform = input_transform
-        self.aux_shortcut = False
 
     def staged(self):
         """-> (fp32, int16) host tensors of the folded / packed parameters the ops' offsets point into."""

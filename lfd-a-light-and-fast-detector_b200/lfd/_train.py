@@ -19,7 +19,6 @@ frozen backbone prefix runs on the inference plan's ops and packing (LFD_TOP_INF
 Rounding points (bf16 training): conv output z (fp32 accumulate) -> bf16; BatchNorm statistics over the stored z (fp64 sums);
 normalised + residual + ReLU output -> bf16; every activation gradient -> bf16; weight / norm-parameter gradients fp32.
 """
-import os
 import time
 import ctypes as C
 
@@ -121,7 +120,6 @@ class TrainPlan(object):
         self.model = model
         self.input_transform = getattr(model, 'input_transform', None)    # of uint8 batches: the stem conv, its weight gradient, the frozen prefix's stem
         self.create_native = create_native               # False: host-side planning only (CPU tests of the planner)
-        self.branches = os.environ.get('LFD_B200_TRAIN_BRANCHES', '1') != '0'      # per-level chains on side streams (0: one stream, A/B runs)
         self.flat = flat_parameters(model, allow_cpu=not create_native)
         self._off, self._top = {}, 256                  # workspace regions: name -> byte offset
         self._sizes = {}
@@ -415,7 +413,7 @@ class TrainPlan(object):
                     f0, l0 = len(self._fwd), len(self._layers)
                     self._level(neck, head, l, cur, h, w, offs[l])
                     # the level's neck + head chain depends on the tap only: its own branch (side stream), in the forward and in the backward
-                    br = (1 + l % (nat.MAX_BRANCHES - 1)) if self.branches else 0
+                    br = 1 + l % (nat.MAX_BRANCHES - 1)
                     for op in self._fwd[f0:]:
                         op['branch'] = br
                     for L in self._layers[l0:]:
@@ -797,7 +795,7 @@ class TrainPlan(object):
         """As InferencePlan.autotune: bounds on the persistent CTAs of the side-branch (per-level chain) convs / data-gradient convs /
         weight-gradient kernels, picked per branch by timing the replayed forward and backward graphs.  Model state touched by the timing
         runs (BatchNorm running statistics, the flat gradient buffer, the plan's outputs) is saved and restored."""
-        if not self.create_native or not self.branches:
+        if not self.create_native:
             return {}
         dev, lib = self.device, nat.lib()
         saved = [t.clone() for m in self._bn_modules for t in (m.running_mean, m.running_var)]

@@ -1,4 +1,4 @@
-"""Timing aid for A/B runs of environment knobs: graph-replayed forward plan of one workload, CUDA events over many replays."""
+"""Timing aid for A/B runs of two library builds (LFD_B200_LIB): graph-replayed forward plan of one workload, CUDA events over many replays."""
 import sys, os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, 'lfd-a-light-and-fast-detector_b200'), os.path.join(ROOT, 'tests')]

@@ -1,12 +1,11 @@
 # -*- coding: utf-8 -*-
 """Debug aid (not a test): per-layer comparison of the native plan against the bf16-emulated oracle.
 
-    LFD_B200_NO_REUSE=1 python tests/debug_layers.py WIDERFACE_S [simt|umma]
+    python tests/debug_layers.py WIDERFACE_S [simt|umma]
 """
 import os
 import sys
 
-os.environ['LFD_B200_NO_REUSE'] = '1'
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path[:0] = [HERE, os.path.dirname(HERE), os.path.join(os.path.dirname(HERE), 'lfd-a-light-and-fast-detector_b200')]
 import torch  # noqa: E402
@@ -14,6 +13,7 @@ import torch  # noqa: E402
 import synth  # noqa: E402
 from helpers import load_golden, synth_model, rel_err  # noqa: E402
 from lfd import _native as nat  # noqa: E402
+from lfd._engine import InferencePlan  # noqa: E402
 from oracle import lfd_oracle as orc  # noqa: E402
 
 
@@ -42,14 +42,12 @@ def main():
     g = load_golden('forward_%s.pt' % name)
     model, sd = synth_model(name, cls_bias=g['cls_bias'], seed=g['seed'])
     model.cuda()
-    model.conv_impl, model.use_cuda_graph = impl, False
     x = synth.synth_input(g['N'], g['H'], g['W'])
-    with torch.no_grad():
-        cls, reg = model(x.cuda())
-    torch.cuda.synchronize()
+    # reuse=False: every intermediate stays readable after the forward
+    plan = InferencePlan(model, g['N'], g['H'], g['W'], torch.device('cuda'), impl, reuse=False)
+    cls, reg = plan.forward(x.cuda(), use_graph=False)
     trace = {}
     ocls, oreg, _ = orc.forward(orc.CONFIGS[name], sd, x, emulate_bf16=True, trace=trace)
-    plan = list(model._plans.values())[0]
     for row in plan.describe():
         if row['out'] is None:
             continue

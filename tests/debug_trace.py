@@ -16,12 +16,13 @@ CASES = {'3x3s1': (8, 90, 160, 64, 64, 3, 1, True, False, 0), '3x3s1res': (8, 90
 
 
 def trace_plan_op(index):
-    """Timeline of op `index` of the WIDERFACE-S 720p b8 plan (0 = fused stem0+stem1, 1 = fused stem2+stem3)."""
+    """Timeline of op `index` of the WIDERFACE-S 720p b8 plan with the two-launch stem (0 = fused stem0+stem1, 1 = fused stem2+stem3)."""
     import ctypes as C
     from helpers import synth_model
+    from lfd._engine import InferencePlan
     model, _ = synth_model('WIDERFACE_S')
     model.cuda()
-    plan = model.inference_plan(8, 720, 1280, torch.device('cuda', 0))
+    plan = InferencePlan(model, 8, 720, 1280, torch.device('cuda', 0), fuse_stem=False)
     x = torch.randint(0, 256, (8, 720, 1280, 3), dtype=torch.uint8, device='cuda')
     plan.forward(x, use_graph=False)
     torch.cuda.synchronize()

@@ -4,7 +4,7 @@ the producer per stage, each consumer warpgroup's MMA phase per tile and the epi
 
     python tests/debug_trace_consumers.py op0 op1 3x3s2 ...
 
-opN = op N of the WIDERFACE-S 720p b8 plan (0 = fused stem0+stem1, 1 = fused stem2+stem3); other names are the stand-alone convs of
+opN = op N of the WIDERFACE-S 720p b8 plan with the two-launch stem (0 = fused stem0+stem1, 1 = fused stem2+stem3); other names are the stand-alone convs of
 debug_trace.CASES.  The buffer layout is the one in conv_umma.cu (LFD_TRACE): [4 roles][32 entries][4 slots]."""
 import os
 import sys

@@ -34,14 +34,13 @@ def _input(fmt, n, h, w, seed=0):
     return torch.randint(0, 256, (n, h, w, 3), generator=g, dtype=torch.uint8).cuda()
 
 
-def _prefix_matches_inference(model, plan, x, monkeypatch):
+def _prefix_matches_inference(model, plan, x):
     """Every tensor the prefix hands over == the same tensor of an InferencePlan for the same model, input and shape (bit for bit)."""
-    monkeypatch.setenv('LFD_B200_NO_REUSE', '1')          # keep every inference tensor readable after the forward
     n = x.shape[0]
     h, w = (x.shape[1], x.shape[2]) if x.dtype == torch.uint8 else (x.shape[2], x.shape[3])
     was_training = model.training
     model.eval()
-    ref = InferencePlan(model, n, h, w, x.device)
+    ref = InferencePlan(model, n, h, w, x.device, reuse=False)          # keep every inference tensor readable after the forward
     ref.forward(x, use_graph=False)
     model.train(was_training)
     torch.cuda.synchronize()
@@ -56,7 +55,7 @@ def _prefix_matches_inference(model, plan, x, monkeypatch):
 @pytest.mark.parametrize('cfg,frozen_stages,shape,stem4', [('WIDERFACE_S', 1, (2, 656, 640), True), ('WIDERFACE_S', 2, (2, 128, 160), False),
                                                            ('WIDERFACE_L', 'all', (2, 186, 252), None), ('TT100K_L', 2, (1, 186, 252), None)])
 @pytest.mark.parametrize('fmt', ['f32', 'u8'])
-def test_prefix_tensors_equal_the_inference_plans(cfg, frozen_stages, shape, stem4, fmt, monkeypatch):
+def test_prefix_tensors_equal_the_inference_plans(cfg, frozen_stages, shape, stem4, fmt):
     model = finetune_model(cfg, frozen_stages)
     x = _input(fmt, *shape)
     plan = model.train_plan_for(*shape, x.device)
@@ -64,7 +63,7 @@ def test_prefix_tensors_equal_the_inference_plans(cfg, frozen_stages, shape, ste
     if stem4 is not None:
         assert (4 in kinds) == stem4, kinds                 # lfd._native.OP_STEM4, chosen by the inference plan's L2 gate
     plan.forward(x)
-    _prefix_matches_inference(model, plan, x, monkeypatch)
+    _prefix_matches_inference(model, plan, x)
 
 
 def _sgd(model, lr=0.02):
@@ -193,7 +192,7 @@ def test_fine_tuning_reduces_the_loss():
     assert all(np.isfinite(losses)) and losses[-1] < 0.8 * losses[0], losses
 
 
-def test_new_prefix_weights_are_repacked_and_unfreezing_differentiates(monkeypatch):
+def test_new_prefix_weights_are_repacked_and_unfreezing_differentiates():
     """load_state_dict between two steps: the next step's prefix tensors equal a fresh InferencePlan's.  Unfreezing (frozen_stages -1 and
     train() again) gives a plan that differentiates the newly trainable layers, checked layer by layer."""
     model = finetune_model('WIDERFACE_S', 2)
@@ -207,7 +206,7 @@ def test_new_prefix_weights_are_repacked_and_unfreezing_differentiates(monkeypat
     model.train()
     out = model(x)
     assert model.train_plan_for(n, h, w, x.device) is plan
-    _prefix_matches_inference(model, plan, x, monkeypatch)
+    _prefix_matches_inference(model, plan, x)
     model.get_loss(out, ann)['loss'].backward()
     # unfreeze
     model._backbone._frozen_stages = -1

@@ -201,23 +201,20 @@ def test_predict_for_single_image_runs_end_to_end():
 
 
 @pytest.mark.parametrize('name', FWD)
-def test_every_layer_within_one_bf16_ulp_teacher_forced(name, monkeypatch):
+def test_every_layer_within_one_bf16_ulp_teacher_forced_without_reuse(name):
     """Gate A/B: each fused layer of the real network, evaluated in fp32 on the CPU from the inputs the CUDA path itself
     produced, matches the stored CUDA output to 1 bf16 ulp (final fp32 cls / reg: 2e-4 rms, 2e-3 max relative)."""
     import torch.nn.functional as F
     from gpu_ops import ref_conv, assert_bf16_close, bf16r
     from lfd._engine import InferencePlan
-    monkeypatch.setenv('LFD_B200_NO_REUSE', '1')     # keep every intermediate alive for inspection
     g = load_golden('forward_%s.pt' % name)
     model, sd = synth_model(name, cls_bias=g['cls_bias'], seed=g['seed'])
     model.cuda()
-    model.use_cuda_graph = False
     x = synth.synth_input(g['N'], g['H'], g['W'])
-    with torch.no_grad():
-        cls, reg = model(x.cuda())
-    torch.cuda.synchronize()
-    plan = list(model._plans.values())[0]
-    cls, reg = cls.cpu(), reg.cpu()
+    # the plan model(x) builds, with reuse=False: every intermediate stays alive for inspection
+    plan = InferencePlan(model, g['N'], g['H'], g['W'], torch.device('cuda'), model.conv_impl, act_dtype=model.act_dtype,
+                         input_transform=model.input_transform, reuse=False)
+    cls, reg = (t.cpu() for t in plan.forward(x.cuda(), use_graph=False))
     checked = 0
     for op in plan._ops:
         kind = op['kind']

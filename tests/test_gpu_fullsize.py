@@ -135,23 +135,20 @@ def test_one_720p_frame_against_the_oracle():
 def test_fp16_activation_range_is_safe():
     """max-abs trace of every stored tensor of the fp16 plan (WIDERFACE-S 720p, TT100K-L 1080p crops): orders of magnitude inside
     the fp16 range (65504) -- the values are post-BatchNorm / ReLU activations; the conversion saturates instead of overflowing."""
-    import os
-    os.environ['LFD_B200_NO_REUSE'] = '1'
-    try:
-        for name, h, w in (('WIDERFACE_S', 720, 1280), ('TT100K_L', 544, 960)):
-            model, _ = synth_model(name, cls_bias=-2.0)
-            model.cuda()
-            model.act_dtype, model.use_cuda_graph = 'fp16', False
-            x = torch.from_numpy(synth.synth_image_u8(h, w, seed=7))[None].cuda()
-            with torch.no_grad():
-                cls, reg = model(x)
-            plan = list(model._plans.values())[0]
-            worst = 0.0
-            for op in plan._ops:
-                for key in ('out', 'out2'):
-                    if op.get(key) is not None:
-                        worst = max(worst, float(plan.tensor(op[key]).float().abs().max()))
-            print('%s fp16 plan: largest stored activation %.1f' % (name, worst))
-            assert worst < 2048.0 and torch.isfinite(cls).all() and torch.isfinite(reg).all()
-    finally:
-        del os.environ['LFD_B200_NO_REUSE']
+    from lfd._engine import InferencePlan
+    for name, h, w in (('WIDERFACE_S', 720, 1280), ('TT100K_L', 544, 960)):
+        model, _ = synth_model(name, cls_bias=-2.0)
+        model.cuda()
+        model.act_dtype = 'fp16'
+        x = torch.from_numpy(synth.synth_image_u8(h, w, seed=7))[None].cuda()
+        # the plan model(x) builds, with reuse=False: every stored tensor stays readable after the forward
+        plan = InferencePlan(model, 1, h, w, torch.device('cuda'), model.conv_impl, act_dtype=model.act_dtype,
+                             input_transform=model.input_transform, reuse=False)
+        cls, reg = plan.forward(x, use_graph=False)
+        worst = 0.0
+        for op in plan._ops:
+            for key in ('out', 'out2'):
+                if op.get(key) is not None:
+                    worst = max(worst, float(plan.tensor(op[key]).float().abs().max()))
+        print('%s fp16 plan: largest stored activation %.1f' % (name, worst))
+        assert worst < 2048.0 and torch.isfinite(cls).all() and torch.isfinite(reg).all()

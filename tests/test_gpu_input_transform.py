@@ -164,14 +164,14 @@ def assert_heads(a, b, exact, what):
 
 @pytest.mark.parametrize('name', sorted(TRANSFORMS))
 @pytest.mark.parametrize('dtype', ['bf16', 'fp16'])
-def test_fused_stem_on_both_loaders(dtype, name, monkeypatch):
+def test_fused_stem_on_both_loaders(dtype, name):
     """STEM4 (WIDERFACE_S, forced): the word loader (W % 4 == 0, aligned base), the per-pixel loader (other widths, or a base address =
     1 mod 4): the stem3 map bit for bit, the head outputs up to the GroupNorm atomics."""
-    monkeypatch.setenv('LFD_B200_NO_REUSE', '1')
     kernel_pipe, host_pipe = TRANSFORMS[name]
     model = model_of('WIDERFACE_S')
     for h, w in ((186, 252), (185, 253), (187, 254), (184, 255)):
-        plan = InferencePlan(model, 2, h, w, torch.device('cuda'), act_dtype=dtype, fuse_stem=True, input_transform=input_transform_of(kernel_pipe))
+        plan = InferencePlan(model, 2, h, w, torch.device('cuda'), act_dtype=dtype, fuse_stem=True, input_transform=input_transform_of(kernel_pipe),
+                             reuse=False)
         assert plan._ops[0]['kind'] == nat.OP_STEM4
         x8 = frames(2, h, w)
         ref = run_plan(plan, host_f32(host_pipe, x8).cuda())

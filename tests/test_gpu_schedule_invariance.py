@@ -52,11 +52,10 @@ def _ulps(a, b):
 
 @pytest.mark.parametrize('name,fuse_stem', [('WIDERFACE_S', None), ('WIDERFACE_S', True), ('WIDERFACE_L', None), ('TT100K_L', None),
                                             ('TL_L', None), ('TEST_FAST', None)])
-def test_plan_outputs_do_not_depend_on_the_grid(name, fuse_stem, monkeypatch):
-    monkeypatch.setenv('LFD_B200_NO_REUSE', '1')          # every intermediate stays readable after the forward
+def test_plan_outputs_do_not_depend_on_the_grid(name, fuse_stem):
     model, _ = synth_model(name)
     model.cuda()
-    plan = InferencePlan(model, N, H, W, torch.device('cuda'), fuse_stem=fuse_stem)
+    plan = InferencePlan(model, N, H, W, torch.device('cuda'), fuse_stem=fuse_stem, reuse=False)   # every intermediate stays readable after the forward
     if fuse_stem:
         assert plan._ops[0]['kind'] == nat.OP_STEM4
     has_gn = any(op['kind'] == nat.OP_GN_APPLY or (op['kind'] == nat.OP_HEAD_FINAL and op.get('gn_groups')) for op in plan._ops)

@@ -53,12 +53,12 @@ def _run(plan, x, stem_ctas=None):
 
 
 def _check(shape, dtype, fmt, misaligned=False, grids=GRIDS):
-    """Needs LFD_B200_NO_REUSE=1 (set by the tests): the stem3 map must outlive the forward."""
+    """Both plans are built with reuse=False: the stem3 map must outlive the forward."""
     n, h, w = shape
     model = _model()
     dev = torch.device('cuda')
-    fused = InferencePlan(model, n, h, w, dev, act_dtype=dtype, fuse_stem=True)
-    pair = InferencePlan(model, n, h, w, dev, act_dtype=dtype, fuse_stem=False)
+    fused = InferencePlan(model, n, h, w, dev, act_dtype=dtype, fuse_stem=True, reuse=False)
+    pair = InferencePlan(model, n, h, w, dev, act_dtype=dtype, fuse_stem=False, reuse=False)
     assert fused._ops[0]['kind'] == nat.OP_STEM4 and pair._ops[0]['kind'] == nat.OP_STEM0
     x = _input(fmt, n, h, w, misaligned)
     s_p, c_p, r_p = _run(pair, x)
@@ -78,14 +78,12 @@ def _check(shape, dtype, fmt, misaligned=False, grids=GRIDS):
 @pytest.mark.parametrize('fmt', ['u8', 'f32'])
 @pytest.mark.parametrize('dtype', ['bf16', 'fp16'])
 @pytest.mark.parametrize('shape', [BENCH, RAGGED_W4, RAGGED], ids=['720p-b8', 'ragged-w4', 'ragged'])
-def test_fused_stem_runs_are_bit_identical_to_the_two_kernel_path(shape, dtype, fmt, monkeypatch):
-    monkeypatch.setenv('LFD_B200_NO_REUSE', '1')
+def test_fused_stem_runs_are_bit_identical_to_the_two_launch_stem(shape, dtype, fmt):
     _check(shape, dtype, fmt)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('shape', [BENCH, RAGGED_W4], ids=['720p-b8', 'ragged-w4'])
-def test_fused_stem_misaligned_u8_input_is_bit_identical(shape, monkeypatch):
+def test_fused_stem_on_misaligned_u8_input_is_bit_identical(shape):
     """A u8 image at an address that is not a multiple of 4 takes the per-pixel loader."""
-    monkeypatch.setenv('LFD_B200_NO_REUSE', '1')
     _check(shape, 'bf16', 'u8', misaligned=True, grids=(2, 7, 131))

@@ -15,8 +15,7 @@ def _conv_count(plan):
     return [r['kind'] for r in plan.describe()].count('conv')
 
 
-def test_planner_fuses_the_faster_stem_only_above_the_l2_gate(monkeypatch):
-    monkeypatch.delenv('LFD_B200_NO_STEM_FUSION', raising=False)
+def test_stem_fusion_follows_the_l2_gate_and_the_fuse_stem_argument():
     model, _ = synth_model('WIDERFACE_S')
     big = InferencePlan(model, 8, 720, 1280, CPU, create_native=False)
     small = InferencePlan(model, 2, 184, 248, CPU, create_native=False)
@@ -27,12 +26,10 @@ def test_planner_fuses_the_faster_stem_only_above_the_l2_gate(monkeypatch):
     # 2.9 MB of stem1 stays in L2: the small plan keeps the two fused pairs
     assert [o['kind'] for o in small._ops[:2]] == [nat.OP_STEM0, nat.OP_CONV] and small._ops[0]['tail_cout'] == 64
     assert all(o['kind'] != nat.OP_STEM4 for o in small._ops)
-    # the switch restores the two launches; the fused plan needs no stem1 buffer
-    monkeypatch.setenv('LFD_B200_NO_STEM_FUSION', '1')
-    unfused = InferencePlan(model, 8, 720, 1280, CPU, create_native=False)
+    # fuse_stem=False restores the two launches; the fused plan needs no stem1 buffer
+    unfused = InferencePlan(model, 8, 720, 1280, CPU, create_native=False, fuse_stem=False)
     assert unfused._ops[0]['kind'] == nat.OP_STEM0 and _conv_count(unfused) == _conv_count(small)
     assert big.workspace_bytes < unfused.workspace_bytes
-    monkeypatch.delenv('LFD_B200_NO_STEM_FUSION')
     forced = InferencePlan(model, 2, 184, 248, CPU, create_native=False, fuse_stem=True)
     assert forced._ops[0]['kind'] == nat.OP_STEM4
 
@@ -55,15 +52,14 @@ def _input(fmt, n, h, w):
 @pytest.mark.parametrize('fmt', ['u8', 'f32'])
 @pytest.mark.parametrize('dtype', ['bf16', 'fp16'])
 @pytest.mark.parametrize('n,h,w', [(8, 720, 1280), (2, 186, 250), (1, 722, 1270)])
-def test_fused_stem_is_bit_identical_to_the_two_kernel_path(n, h, w, dtype, fmt, monkeypatch):
+def test_fused_stem_is_bit_identical_to_the_two_launch_stem(n, h, w, dtype, fmt):
     """Same MMAs in the same order on the same 16-bit values: the stem3 map and the network outputs are bit-identical.
     186 x 250 and 722 x 1270 give stem3 maps that are not multiples of the 16 x 8 tile (border zeros on all four edges)."""
-    monkeypatch.setenv('LFD_B200_NO_REUSE', '1')      # keep the stem3 map alive after the forward
     model, _ = synth_model('WIDERFACE_S')
     model.cuda()
     dev = torch.device('cuda')
-    fused = InferencePlan(model, n, h, w, dev, act_dtype=dtype, fuse_stem=True)
-    pair = InferencePlan(model, n, h, w, dev, act_dtype=dtype, fuse_stem=False)
+    fused = InferencePlan(model, n, h, w, dev, act_dtype=dtype, fuse_stem=True, reuse=False)     # the stem3 map outlives the forward
+    pair = InferencePlan(model, n, h, w, dev, act_dtype=dtype, fuse_stem=False, reuse=False)
     assert fused._ops[0]['kind'] == nat.OP_STEM4 and pair._ops[0]['kind'] == nat.OP_STEM0
     x = _input(fmt, n, h, w)
     outs = []
@@ -79,13 +75,12 @@ def test_fused_stem_is_bit_identical_to_the_two_kernel_path(n, h, w, dtype, fmt,
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('dtype', ['bf16', 'fp16'])
-def test_fused_stem_matches_the_cpu_chain_of_four_convs(dtype, monkeypatch):
+def test_fused_stem3_map_matches_the_cpu_chain_of_four_convs(dtype):
     from gpu_ops import ref_conv, DTYPES
-    monkeypatch.setenv('LFD_B200_NO_REUSE', '1')
     model, _ = synth_model('WIDERFACE_S')
     model.cuda()
     n, h, w = 1, 186, 250
-    plan = InferencePlan(model, n, h, w, torch.device('cuda'), act_dtype=dtype, fuse_stem=True)
+    plan = InferencePlan(model, n, h, w, torch.device('cuda'), act_dtype=dtype, fuse_stem=True, reuse=False)
     x = synth.synth_input(n, h, w, seed=5)
     with torch.no_grad():
         plan.forward(x.cuda(), use_graph=False)

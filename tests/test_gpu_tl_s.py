@@ -1,7 +1,7 @@
 # -*- coding: utf-8 -*-
 """TrafficLight LFD-S, the shipped config with 48-channel layers (its stem and stage 0), end to end on the GPU: the wgmma path and the
 SIMT cross-check against the emulated oracle with the bounds of test_gpu_forward.py, the post-process against the oracle and the
-reference, the input formats, CUDA graphs, batches, capacity plans, the planner switches, and an independent cross-check against the
+reference, the input formats, CUDA graphs, batches, capacity plans, and an independent cross-check against the
 same weights zero-padded to a 64-channel model that runs on the 64-wide kernels."""
 import numpy as np
 import pytest
@@ -205,23 +205,6 @@ def test_tl_s_predict_for_single_image():
     assert len(soft) >= len(rows) > 0
 
 
-@pytest.mark.parametrize('switch', ['LFD_B200_NO_TAIL', 'LFD_B200_NO_FUSED_SHORTCUT'])
-def test_tl_s_planner_switches(switch, monkeypatch):
-    """Without the fused stem tail the stem's 1x1 48 -> 48 runs as FLAT 48; without the fused shortcut stage 0's runs as 1x1/s2 48."""
-    monkeypatch.setenv(switch, '1')
-    g, model, sd = _model('bf16')
-    x = synth.synth_input(g['N'], g['H'], g['W'])
-    cls, reg = _forward(model, x)
-    convs = _plan_convs(model)
-    if switch == 'LFD_B200_NO_TAIL':
-        assert any(op['Cout'] == 48 and op['ksize'] == 1 and op['stride'] == 1 for op in convs)
-    else:
-        assert any(op['Cout'] == 48 and op['ksize'] == 1 and op['stride'] == 2 for op in convs)
-    ocls, oreg, _ = orc.forward(CFG, sd, x, emulate_bf16=True)
-    ec, er = rel_err(cls, ocls), rel_err(reg, oreg)
-    assert ec[1] < TOL_E2E_RMS and er[1] < TOL_E2E_RMS and ec[0] < TOL_E2E_MAX and er[0] < TOL_E2E_MAX, (ec, er)
-
-
 def _padded_model(sd48):
     """The same function as a 64-channel model: the 48-channel layers zero-padded to 64 (conv weights and BatchNorm gamma / beta /
     running mean 0, running variance 1 in the padded channels, and 0 weights on the padded inputs of the next layer)."""
@@ -267,17 +250,18 @@ def test_tl_s_training_is_not_implemented():
 
 
 @pytest.mark.parametrize('impl', [nat.CONV_UMMA, nat.CONV_SIMT], ids=['umma', 'simt'])
-def test_tl_s_every_layer_within_one_bf16_ulp_teacher_forced(impl, monkeypatch):
+def test_tl_s_every_layer_within_one_bf16_ulp_teacher_forced_without_reuse(impl):
     """Gate A/B of test_gpu_forward.py for TL_S: each fused layer of the real network (the 3 -> 48 stem with its fused 48 tail, the
     stage-0 3x3/s2 conv with its fused 48 shortcut, the 48-channel blocks, the neck conv from 48 channels, ...), evaluated in fp32 on
     the CPU from the inputs the CUDA path itself produced, matches the stored CUDA output to 1 bf16 ulp; the head outputs to 2e-4 rms."""
     from gpu_ops import ref_conv, assert_bf16_close, bf16r
     from lfd._engine import InferencePlan
-    monkeypatch.setenv('LFD_B200_NO_REUSE', '1')     # keep every intermediate alive for inspection
     g, model, sd = _model('bf16', impl)
     x = synth.synth_input(g['N'], g['H'], g['W'])
-    cls, reg = _forward(model, x)
-    plan = list(model._plans.values())[0]
+    # the plan model(x) builds, with reuse=False: every intermediate stays alive for inspection
+    plan = InferencePlan(model, g['N'], g['H'], g['W'], torch.device('cuda'), model.conv_impl, act_dtype=model.act_dtype,
+                         input_transform=model.input_transform, reuse=False)
+    cls, reg = (t.cpu() for t in plan.forward(x.cuda(), use_graph=False))
     seen = set()
     for op in plan._ops:
         kind = op['kind']

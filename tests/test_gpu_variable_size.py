@@ -71,7 +71,7 @@ class _Exact(object):
     def get(self, h, w, fmt, x):
         key = (h, w, fmt)
         if key not in self.cache:
-            plan = InferencePlan(self.model, N, h, w, torch.device('cuda'), act_dtype=self.act_dtype, fuse_stem=self.fuse_stem)
+            plan = InferencePlan(self.model, N, h, w, torch.device('cuda'), act_dtype=self.act_dtype, fuse_stem=self.fuse_stem, reuse=False)
             with torch.no_grad():
                 cls, reg = plan.forward(x, use_graph=False)
             torch.cuda.synchronize()
@@ -131,11 +131,10 @@ CASES = [('WIDERFACE_S', None, 'bf16'), ('WIDERFACE_S', True, 'bf16'), ('WIDERFA
 
 
 @pytest.mark.parametrize('name,fuse_stem,act_dtype', CASES)
-def test_capacity_plan_matches_exact_plans(name, fuse_stem, act_dtype, monkeypatch):
-    monkeypatch.setenv('LFD_B200_NO_REUSE', '1')          # every intermediate stays readable after the forward
+def test_capacity_plan_matches_exact_plans_tensor_by_tensor(name, fuse_stem, act_dtype):
     model, _ = synth_model(name)
     model.cuda()
-    plan = InferencePlan(model, N, H, W, torch.device('cuda'), act_dtype=act_dtype, fuse_stem=fuse_stem)
+    plan = InferencePlan(model, N, H, W, torch.device('cuda'), act_dtype=act_dtype, fuse_stem=fuse_stem, reuse=False)   # intermediates stay readable
     stem4 = plan._ops[0]['kind'] == nat.OP_STEM4
     assert stem4 == bool(fuse_stem)
     # the exact plans are forced to the capacity plan's stem: a small frame alone would not take STEM4 (its stem1 map stays in L2), and

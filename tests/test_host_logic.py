@@ -185,7 +185,7 @@ def test_build_guard_rejects_large_stack_frames():
 
 
 @pytest.mark.parametrize('name', ['WIDERFACE_L', 'TT100K_S', 'TL_L', 'TEST_FAST'])
-def test_training_plan_branches_order_every_conflict(name):
+def test_training_plan_level_chains_order_every_conflict(name):
     """The training planner puts every level's neck + head chain on its own branch (side stream) and derives the wait masks from the
     read / write / accumulate role of each operand.  Replay the fork / wait protocol of lfd_train_plan_run with vector clocks and check
     that every pair of ops that conflict on a workspace tensor (write vs anything, accumulate vs read) is ordered."""
@@ -194,7 +194,6 @@ def test_training_plan_branches_order_every_conflict(name):
     model, _ = synth_model(name)
     model.train()
     plan = TrainPlan(model, 2, 128, 160, torch.device('cpu'), create_native=False)
-    assert plan.branches
     for which, ops in (('fwd', plan.fwd_ops), ('bwd', plan.bwd_ops)):
         branches = sorted({op.get('branch', 0) for op in ops})
         assert branches[0] == 0 and len(branches) == 1 + len(plan.level_sizes) and branches[-1] < nat.MAX_BRANCHES
@@ -204,6 +203,36 @@ def test_training_plan_branches_order_every_conflict(name):
     # the backward starts every level chain before the backbone
     first_main = next(i for i, op in enumerate(plan.bwd_ops) if op.get('branch', 0) == 0 and op['kind'] not in (nat.TOP_ZERO,))
     assert all(op.get('branch', 0) == 0 for op in plan.bwd_ops[first_main:])
+
+
+def test_plans_do_not_depend_on_the_environment(monkeypatch):
+    """The planners and the library read no environment variable that picks a path inside a plan: with every former A/B switch set,
+    the inference and training plans are the ones a clean environment gives (op fields, branches, wait masks, offsets, workspace size)."""
+    import tl_s
+    from lfd._train import TrainPlan
+    cpu = torch.device('cpu')
+    wf_s, tl = synth_model('WIDERFACE_S')[0], tl_s.synth_model()[0]
+    wf_l, wf_l_frozen = synth_model('WIDERFACE_L')[0], synth_model('WIDERFACE_L')[0]
+    wf_l_frozen._backbone._frozen_stages = 1
+    wf_l.train(), wf_l_frozen.train()
+
+    def plans():        # everything but pointers: the op dicts, the tensor offsets and the workspace size of each plan
+        out =[InferencePlan(m, n, h, w, cpu, create_native=False) for m, n, h, w in
+               ((wf_s, 2, 184, 248), (wf_s, 8, 720, 1280), (tl, 2, 184, 248))]       # WIDERFACE_S below and above the STEM4 gate
+        out = [(p._ops, p.offsets, p.workspace_bytes) for p in out]
+        for m in (wf_l, wf_l_frozen):
+            p = TrainPlan(m, 2, 128, 160, cpu, create_native=False)
+            out.append(([{k: v for k, v in op.items() if k != 'ptr'} for op in p.fwd_ops + p.bwd_ops], p._off, p.workspace_bytes))
+        return out
+
+    clean = plans()
+    assert clean[0][0][0]['kind'] == nat.OP_STEM0 and clean[1][0][0]['kind'] == nat.OP_STEM4
+    for name in ('NO_BRANCHES', 'NO_AUX', 'NO_TAIL', 'NO_FUSED_SHORTCUT', 'NO_STEM_FUSION', 'NO_NECK_TAIL', 'NO_REUSE', 'NO_PDL'):
+        monkeypatch.setenv('LFD_B200_' + name, '1')
+    monkeypatch.setenv('LFD_B200_TRAIN_BRANCHES', '0')
+    monkeypatch.setenv('LFD_B200_GRAPH_PRIO', '0')
+    monkeypatch.setenv('LFD_B200_FORCE_CC', '16')
+    assert plans() == clean
 
 
 def test_side_branch_cta_bounds_touch_only_side_branch_ops():
