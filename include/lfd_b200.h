@@ -62,7 +62,23 @@ int lfd_device_sm_count(void);
 
 /* ------------------------------------------------------------------------------------------ forward plan */
 enum { LFD_OP_STEM0 = 0, LFD_OP_CONV = 1, LFD_OP_GN_APPLY = 2, LFD_OP_HEAD_FINAL = 3, LFD_OP_STEM4 = 4 };
-enum { LFD_INPUT_F32_NCHW = 0, LFD_INPUT_U8_NHWC = 1 };
+enum { LFD_INPUT_F32_NCHW = 0, LFD_INPUT_U8_NHWC = 1, LFD_INPUT_U8_NV12 = 2 };
+/* LFD_INPUT_U8_NV12 (inference only): YUV 4:2:0 video frames, one contiguous uint8 buffer without row padding.  Image n starts at byte
+ * n * H * W * 3 / 2 and holds a Y plane of H rows x W bytes, then an interleaved UV plane of H / 2 rows x W bytes (U at even bytes, V at
+ * odd bytes): the bytes of a uint8 [N][3H/2][W] tensor.  H and W are even.  A pixel (y, x) is turned into the three bytes (B, G, R) from
+ * its Y byte and the (U, V) pair at UV row y / 2, UV column x & ~1, by BT.601 limited range in 20-bit fixed point:
+ *     y' = max(0, Y - 16) * 1220542,  u = U - 128,  v = V - 128,  h = 1 << 19
+ *     B = sat8((y' + h + 2116026 * u) >> 20)
+ *     G = sat8((y' + h - 852492 * v - 409993 * u) >> 20)
+ *     R = sat8((y' + h + 1673527 * v) >> 20)          (arithmetic shifts; sat8 clamps to 0..255)
+ * which is, bit for bit, cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12).  From there the frame is a uint8 BGR frame: the input transform
+ * below applies to the three bytes by their position (B = 0, G = 1, R = 2), and every op and plan gives on an NV12 frame exactly what it
+ * gives on the converted BGR frame.  A frame below a plan's capacity (lfd_plan_forward_extent) lies in the capacity layout: its h x w
+ * Y rows in the top-left corner of the H x W Y plane, its h / 2 UV rows in the top-left corner of the H / 2 x W UV plane.
+ * lfd_plan_forward, lfd_plan_forward_extent, lfd_plan_profile and lfd_run_op check before anything is enqueued: an odd frame height or
+ * width is LFD_ERR_INVALID, an NV12 frame on a plan (an image op) of odd capacity H or W is LFD_ERR_UNSUPPORTED.  lfd_train_plan_run,
+ * lfd_train_plan_profile and lfd_run_top refuse NV12 with LFD_ERR_UNSUPPORTED.  Every entry point refuses a format other than these three
+ * with LFD_ERR_INVALID. */
 enum { LFD_CONV_UMMA = 0, LFD_CONV_SIMT = 1 }; /* SIMT = cross-check kernel, validation only */
 /* 16-bit storage type of activations and packed weights (fp32 accumulation either way; same bytes, same tensor-core rate):
  * bf16 = the north-star dtype; fp16 = 3 more mantissa bits, the variant that meets 1e-3 END TO END (DESIGN.md "Parity") and the
@@ -145,7 +161,7 @@ typedef struct lfd_op {
     const float* s2_shift;
     const void* s3_weight;
     const float* s3_shift;
-    /* STEM0 / STEM4 on a LFD_INPUT_U8_NHWC image: the input transform (see below).  All zero = simple_normalize on BGR. */
+    /* STEM0 / STEM4 on a LFD_INPUT_U8_NHWC or LFD_INPUT_U8_NV12 image: the input transform (see below).  All zero = simple_normalize on BGR. */
     int32_t in_swap_rb;
     float in_mean[3];
     float in_scale[3];
@@ -175,8 +191,8 @@ int lfd_plan_forward(lfd_plan* plan, const void* input, int input_format, void* 
  * h x w region, and its successors, in the top-left corner; nothing outside it is read.  ext[n_ops] (host) gives per op the valid
  * input H x W and output Ho x Wo, and for HEAD_FINAL the level's first point and the frame's point count P (0 for the other ops), exactly
  * the fields of a plan built for the frame.  The table is copied, stream-ordered, into a device table that the kernels read when they
- * start.  `input` holds the frame in the capacity layout: uint8 [N][H][W][3] or float32 [N][3][H][W] with the frame in the top-left
- * corner.  cls_out / reg_out receive the frame's outputs as a plan built for it lays them out: float[N][P][cls_channels] and
+ * start.  `input` holds the frame in the capacity layout: uint8 [N][H][W][3], float32 [N][3][H][W] or NV12 uint8 [N][3H/2][W] (see
+ * LFD_INPUT_U8_NV12) with the frame in the top-left corner.  cls_out / reg_out receive the frame's outputs as a plan built for it lays them out: float[N][P][cls_channels] and
  * float[N][P][4] at the start of the buffers.  h == H and w == W is lfd_plan_forward (ext is not read).  A frame outside the capacity
  * or an inconsistent table fails with LFD_ERR_INVALID before anything is enqueued; the SIMT cross-check path runs full-size frames only
  * (LFD_ERR_UNSUPPORTED).  use_graph: one graph per pointer tuple as in lfd_plan_forward, shared by every frame size. */

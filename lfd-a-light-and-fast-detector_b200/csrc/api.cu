@@ -409,7 +409,7 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
                 UmmaConvParams p = po.cp;
                 p.in_raw = input; p.input_format = input_format; p.in = nullptr;
                 p.xf = po.xf;
-                if (input_format != LFD_INPUT_U8_NHWC) p.xf.swap = 0;   // the loaders order the channels at the load: fp32 planes are taken as they are
+                if (input_format == LFD_INPUT_F32_NCHW) p.xf.swap = 0;   // the loaders order the channels at the load: fp32 planes are taken as they are
                 p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off); p.res = nullptr;
                 p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift; p.stats = nullptr;
                 p.relu = o.relu; p.gn_groups = 0; p.trace = g_trace; p.tl = tl; p.f16 = o.dtype;
@@ -426,8 +426,10 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
             UmmaConvParams p = po.cp;
             p.in_raw = input; p.input_format = input_format; p.in = nullptr;
             p.xf = po.xf;
-            if (input_format != LFD_INPUT_U8_NHWC) p.xf.swap = 0;
-            p.in_words = input_format == LFD_INPUT_U8_NHWC && o.W % 4 == 0 && (reinterpret_cast<uintptr_t>(input) & 3) == 0;
+            if (input_format == LFD_INPUT_F32_NCHW) p.xf.swap = 0;
+            // the word loader: rows of whole aligned words (BGR: 3 words per 4 pixels; NV12: a Y word and a UV word, its image pitch
+            // H * W * 3 / 2 then being a multiple of 4 as well, since H is even)
+            p.in_words = input_format != LFD_INPUT_F32_NCHW && o.W % 4 == 0 && (reinterpret_cast<uintptr_t>(input) & 3) == 0;
             p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off); p.res = nullptr; p.stats = nullptr;
             p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift; p.relu = o.relu;
             p.w2 = reinterpret_cast<const __nv_bfloat16*>(o.tail_weight); p.shift2 = o.tail_shift; p.relu2 = o.tail_relu;
@@ -537,9 +539,38 @@ extern "C" int lfd_plan_destroy(lfd_plan* plan) {
 
 extern "C" int lfd_plan_num_launches(const lfd_plan* plan) { return plan ? (int)plan->ops.size() : 0; }
 
+// The input format of an inference entry point, before anything is enqueued: 0, 1 or 2.  An NV12 frame (h x w) has an even height and
+// width, on an image op whose capacity (H x W: the UV plane's pitch and twice its rows) is even too.
+static int check_input_format(const char* fn, int fmt, const lfd_op* img, int h, int w) {
+    if (fmt != LFD_INPUT_F32_NCHW && fmt != LFD_INPUT_U8_NHWC && fmt != LFD_INPUT_U8_NV12)
+        return fail(LFD_ERR_INVALID, "%s: input format %d (0 = float32 NCHW, 1 = uint8 NHWC, 2 = uint8 NV12)", fn, fmt);
+    if (fmt == LFD_INPUT_U8_NV12 && img) {
+        if ((img->H | img->W) & 1) return fail(LFD_ERR_UNSUPPORTED, "%s: NV12 frames need an even capacity, the plan's is %dx%d", fn, img->H, img->W);
+        if ((h | w) & 1) return fail(LFD_ERR_INVALID, "%s: an NV12 frame has an even height and width, got %dx%d", fn, h, w);
+    }
+    return LFD_OK;
+}
+
+// the op that reads the image (a plan's first op), or null
+static const lfd_op* image_op(const lfd_plan* pl) {
+    const lfd_op& o = pl->ops[0].op;
+    return o.kind == LFD_OP_STEM0 || o.kind == LFD_OP_STEM4 ? &o : nullptr;
+}
+
+// Training reads float32 NCHW or uint8 NHWC only
+static int check_train_format(const char* fn, int fmt) {
+    if (fmt == LFD_INPUT_U8_NV12) return fail(LFD_ERR_UNSUPPORTED, "%s: NV12 input is for inference plans only", fn);
+    if (fmt != LFD_INPUT_F32_NCHW && fmt != LFD_INPUT_U8_NHWC)
+        return fail(LFD_ERR_INVALID, "%s: input format %d (0 = float32 NCHW, 1 = uint8 NHWC)", fn, fmt);
+    return LFD_OK;
+}
+
 extern "C" int lfd_plan_forward(lfd_plan* pl, const void* input, int input_format, void* workspace, float* cls_out, float* reg_out,
                                 int use_graph, lfd_stream stream) {
     if (!pl || !input || !workspace || !cls_out || !reg_out) return fail(LFD_ERR_INVALID, "lfd_plan_forward: null argument");
+    const lfd_op* img = image_op(pl);
+    int rc = check_input_format("lfd_plan_forward", input_format, img, img ? img->H : 0, img ? img->W : 0);
+    if (rc) return rc;
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
     return pl->ex.run(input, input_format, workspace, cls_out, reg_out, nullptr, use_graph, st_of(stream), [&](size_t i, cudaStream_t s) {
         return launch_op(pl->ops[i], i, input, input_format, ws, cls_out, reg_out, pl->P, pl->cls_channels, pl->conv_impl, s);
@@ -576,10 +607,12 @@ extern "C" int lfd_plan_forward_extent(lfd_plan* pl, const void* input, int inpu
     if (img.kind != LFD_OP_STEM0 && img.kind != LFD_OP_STEM4) return fail(LFD_ERR_INVALID, "lfd_plan_forward_extent: the plan does not start on the image");
     if (h < 1 || w < 1 || h > img.H || w > img.W)
         return fail(LFD_ERR_INVALID, "lfd_plan_forward_extent: frame %dx%d outside the plan's capacity %dx%d", h, w, img.H, img.W);
+    int rc = check_input_format("lfd_plan_forward_extent", input_format, &img, h, w);
+    if (rc) return rc;
     if (h == img.H && w == img.W) return lfd_plan_forward(pl, input, input_format, workspace, cls_out, reg_out, use_graph, stream);
     if (pl->conv_impl == LFD_CONV_SIMT) return fail(LFD_ERR_UNSUPPORTED, "lfd_plan_forward_extent: the SIMT cross-check kernels run full-size frames only");
     if (!ext) return fail(LFD_ERR_INVALID, "lfd_plan_forward_extent: a frame below the capacity needs its geometry table");
-    int rc = check_extent(pl, h, w, ext);
+    rc = check_extent(pl, h, w, ext);
     if (rc) return rc;
     const size_t n = pl->ops.size(), bytes = n * sizeof(lfd_extent);
     if (!pl->ext_ev[kExtentRing - 1]) {
@@ -607,6 +640,9 @@ extern "C" int lfd_plan_num_graphs(const lfd_plan* plan) { return plan ? (int)pl
 extern "C" int lfd_plan_profile(lfd_plan* pl, const void* input, int input_format, void* workspace, float* cls_out, float* reg_out,
                                 float* ms_per_op, lfd_stream stream) {
     if (!pl || !input || !workspace || !cls_out || !reg_out || !ms_per_op) return fail(LFD_ERR_INVALID, "lfd_plan_profile: null argument");
+    const lfd_op* img = image_op(pl);
+    int rc = check_input_format("lfd_plan_profile", input_format, img, img ? img->H : 0, img ? img->W : 0);
+    if (rc) return rc;
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
     return pl->ex.profile("lfd_plan_profile", ws, ms_per_op, st_of(stream), [&](size_t i, cudaStream_t s) {
         return launch_op(pl->ops[i], i, input, input_format, ws, cls_out, reg_out, pl->P, pl->cls_channels, pl->conv_impl, s);
@@ -620,6 +656,9 @@ extern "C" int lfd_run_op(const lfd_op* op, const void* input, int input_format,
     if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_run_op: no CUDA device (there is no CPU fallback)");
     PlannedOp po;
     int rc = plan_op(*op, &po);
+    if (rc) return rc;
+    const bool reads_image = op->kind == LFD_OP_STEM0 || op->kind == LFD_OP_STEM4;
+    rc = check_input_format("lfd_run_op", input_format, reads_image ? op : nullptr, op->H, op->W);
     if (rc) return rc;
     return launch_op(po, 0, input, input_format, reinterpret_cast<uint8_t*>(workspace), cls_out, reg_out, P, cls_channels, conv_impl,
                      reinterpret_cast<cudaStream_t>(stream));
@@ -1131,6 +1170,8 @@ extern "C" int lfd_train_plan_num_ops(const lfd_train_plan* plan) { return plan 
 
 extern "C" int lfd_train_plan_run(lfd_train_plan* pl, const void* input, int input_format, void* workspace, int use_graph, lfd_stream stream) {
     if (!pl || !workspace) return fail(LFD_ERR_INVALID, "lfd_train_plan_run: null argument");
+    int rc = check_train_format("lfd_train_plan_run", input_format);
+    if (rc) return rc;
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
     return pl->ex.run(input, input_format, workspace, nullptr, nullptr, nullptr, use_graph, st_of(stream), [&](size_t i, cudaStream_t s) {
         return launch_top(pl->ops[i], input, input_format, ws, s);
@@ -1139,6 +1180,8 @@ extern "C" int lfd_train_plan_run(lfd_train_plan* pl, const void* input, int inp
 
 extern "C" int lfd_train_plan_profile(lfd_train_plan* pl, const void* input, int input_format, void* workspace, float* ms_per_op, lfd_stream stream) {
     if (!pl || !workspace || !ms_per_op) return fail(LFD_ERR_INVALID, "lfd_train_plan_profile: null argument");
+    int rc = check_train_format("lfd_train_plan_profile", input_format);
+    if (rc) return rc;
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
     return pl->ex.profile("lfd_train_plan_profile", ws, ms_per_op, st_of(stream), [&](size_t i, cudaStream_t s) {
         return launch_top(pl->ops[i], input, input_format, ws, s);
@@ -1150,6 +1193,8 @@ extern "C" int lfd_run_top(const lfd_top* op, const void* input, int input_forma
     if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_run_top: no CUDA device (there is no CPU fallback)");
     PlannedTop pt;
     int rc = plan_top(*op, INT64_MAX, &pt);
+    if (rc) return rc;
+    rc = check_train_format("lfd_run_top", input_format);
     if (rc) return rc;
     return launch_top(pt, input, input_format, reinterpret_cast<uint8_t*>(workspace), reinterpret_cast<cudaStream_t>(stream));
 }

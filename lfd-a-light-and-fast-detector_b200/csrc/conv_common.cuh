@@ -20,6 +20,18 @@ static constexpr int kSmemTableOff = 512;    // first per-layer region
 // from there, at offsets chosen per layer (UmmaConvParams::smem_*_off): halo pixel table (modes that need it), the fp32 shifts
 // of the conv and of the fused tail, then the 1024-byte aligned staging regions [warpgroup][buffer]
 
+// LFD_INPUT_U8_NV12: the three bytes (B, G, R) of a pixel from its Y byte and the (U, V) pair of its 2x2 block -- BT.601 limited
+// range in 20-bit fixed point, bit for bit what cv2.cvtColor(f, COLOR_YUV2BGR_NV12) gives.  The only code that knows the constants:
+// every loader of an NV12 frame calls it, then applies the input transform to the bytes as it does to BGR bytes.
+__host__ __device__ __forceinline__ uint32_t nv12_sat8(int v) { return (uint32_t)(v < 0 ? 0 : v > 255 ? 255 : v); }
+__host__ __device__ __forceinline__ void nv12_to_bgr(uint32_t Y, uint32_t U, uint32_t V, uint32_t bgr[3]) {
+    const int y = ((int)Y > 16 ? (int)Y - 16 : 0) * 1220542 + (1 << 19);     // max(0, Y - 16) * 1220542 + the rounding half
+    const int u = (int)U - 128, v = (int)V - 128;
+    bgr[0] = nv12_sat8((y + 2116026 * u) >> 20);                           // arithmetic shifts
+    bgr[1] = nv12_sat8((y - 852492 * v - 409993 * u) >> 20);
+    bgr[2] = nv12_sat8((y + 1673527 * v) >> 20);
+}
+
 struct ConvGeom {
     int N, H, W, Cin, Ho, Wo, Cout, ksize, stride;
     int tail_cout;   // > 0: a 1x1/s1 conv (Cout -> tail_cout) is fused behind this conv (second GEMM in the same kernel)

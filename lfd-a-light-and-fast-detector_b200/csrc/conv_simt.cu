@@ -58,6 +58,14 @@ __global__ void __launch_bounds__(kS0Threads) stem0_kernel(const __grid_constant
         if (y >= 0 && y < p.H && x >= 0 && x < p.W) {
             if (p.input_format == 0) {
                 v = reinterpret_cast<const float*>(p.in)[(((size_t)n * 3 + ci) * p.H + y) * p.W + x];
+            } else if (p.input_format == 2) {   // NV12: Y plane, then the interleaved UV plane at the same pitch
+                const int m = p.xf.swap ? 2 - ci : ci;
+                const size_t plane = (size_t)p.H * p.W;
+                const uint8_t* img = reinterpret_cast<const uint8_t*>(p.in) + (size_t)n * (plane + plane / 2);
+                const uint8_t* uv = img + plane + (size_t)(y >> 1) * p.W + (x & ~1);
+                uint32_t bgr[3];
+                nv12_to_bgr(img[(size_t)y * p.W + x], uv[0], uv[1], bgr);
+                v = p.xf.apply(m, bgr[m]);
             } else {
                 const int m = p.xf.swap ? 2 - ci : ci;
                 v = p.xf.apply(m, reinterpret_cast<const uint8_t*>(p.in)[(((size_t)n * p.H + y) * p.W + x) * 3 + m]);

@@ -528,16 +528,17 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
             // Raw image patch -> normalised bf16 [row][pixel][b g r 0] in the ring stage (see kStem* above).  Every thread owns
             // up to 5 patch pixels; the raw values of the NEXT tile are fetched into registers right after the current patch
             // has been written, so the loads fly while the thread waits for the next free stage.
-            const bool u8 = p.input_format == 1;
+            const bool u8 = p.input_format != 0;        // uint8 BGR (1) or NV12 (2): bytes, normalised by p.xf
+            const bool nv12 = p.input_format == 2;
             const int plane = p.H * p.W;
-            int rel[kStemPerThread];          // source offset of pixel j relative to the patch origin (bytes for u8, elements for fp32)
+            int rel[kStemPerThread];          // source offset of pixel j relative to the patch origin (bytes for BGR, elements for fp32 / NV12's Y)
             int prc[kStemPerThread];          // (row << 8) | col
 #pragma unroll
             for (int j = 0; j < kStemPerThread; ++j) {
                 const int q = min(ptid + j * kProdThreads, kStemPix - 1);
                 const int r = q / kStemCols, c = q - r * kStemCols;
                 prc[j] = (r << 8) | c;
-                rel[j] = u8 ? (r * p.W + c) * 3 : r * p.W + c;
+                rel[j] = p.input_format == 1 ? (r * p.W + c) * 3 : r * p.W + c;
             }
             const bool last_ok = ptid + (kStemPerThread - 1) * kProdThreads < kStemPix;   // this thread owns a pixel in the last round
             uint32_t raw[kStemPerThread][3];
@@ -548,7 +549,23 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
                 const int iy0 = 2 * ty * 16 - 1, ix0 = 2 * (t - ty * lg.tiles_x) * 8 - 1;
                 const bool interior = iy0 >= 0 && ix0 >= 0 && iy0 + kStemRows <= lg.H && ix0 + kStemCols <= lg.W;
                 okmask = 0;
-                if (u8) {
+                if (nv12) {
+                    // raw = (Y, U, V): the Y plane, then the interleaved UV plane at the same pitch, UV row = absolute row / 2 (the patch
+                    // starts at an odd row), UV column = x & ~1
+                    const uint8_t* img = reinterpret_cast<const uint8_t*>(p.in_raw) + (size_t)n * (plane + (plane >> 1));
+                    const uint8_t* org = img + (ptrdiff_t)iy0 * p.W + ix0;
+#pragma unroll
+                    for (int j = 0; j < kStemPerThread; ++j) {
+                        if (j == kStemPerThread - 1 && !last_ok) break;
+                        const int y = iy0 + (prc[j] >> 8), x = ix0 + (prc[j] & 255);
+                        const uint8_t* src = org + rel[j];
+                        const uint8_t* uv = img + plane + (ptrdiff_t)(y >> 1) * p.W + (x & ~1);
+                        const bool ok = interior || ((unsigned)y < (unsigned)lg.H && (unsigned)x < (unsigned)lg.W);
+                        if (!ok) { src = img; uv = img + plane; }
+                        okmask |= (ok ? 1u : 0u) << j;
+                        raw[j][0] = __ldg(src); raw[j][1] = __ldg(uv); raw[j][2] = __ldg(uv + 1);
+                    }
+                } else if (u8) {
                     const uint8_t* img = reinterpret_cast<const uint8_t*>(p.in_raw) + (size_t)n * plane * 3;
                     const uint8_t* org = img + ((ptrdiff_t)iy0 * p.W + ix0) * 3;
 #pragma unroll
@@ -595,6 +612,7 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
 #pragma unroll
                 for (int j = 0; j < kStemPerThread; ++j) {
                     if (j == kStemPerThread - 1 && !last_ok) break;
+                    if (nv12) nv12_to_bgr(raw[j][0], raw[j][1], raw[j][2], raw[j]);   // (Y, U, V) -> the bytes (B, G, R)
                     float f[3];
 #pragma unroll
                     for (int k = 0; k < 3; ++k) {
@@ -1023,7 +1041,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
         // ============================================================== PRODUCER: raw image patch -> normalised 16-bit [row][pixel][b g r 0]
         asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
         const int ptid = tid - kConsumerThreads;
-        const bool u8 = p.input_format == 1;
+        const bool u8 = p.input_format != 0;    // uint8 BGR (1) or NV12 (2): bytes, normalised by p.xf
+        const bool nv12 = p.input_format == 2;
         const bool sw = p.xf.swap;       // u8 BGR -> RGB: the normalised bytes 0 and 2 of a pixel change places
         const int plane = p.H * p.W;
         pdl_wait();
@@ -1041,7 +1060,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
             const uint32_t dst0 = smem_u32(smem + kS4Ring) + s * kS4PatchBytes;
             if (p.in_words) {
                 // ix0 = 1 (mod 4): group g of a patch row = image columns ix0 - 1 + 4g .. + 3 = patch columns 4g - 1 .. 4g + 2,
-                // 12 bytes at a 4-byte aligned address (W % 4 == 0).  A group lies wholly inside or wholly outside the tensor, so
+                // 12 bytes at a 4-byte aligned address (W % 4 == 0; NV12: the Y word and the UV word, both aligned since the image
+                // pitch H * W * 3 / 2 is then a multiple of 4 too).  A group lies wholly inside or wholly outside the tensor, so
                 // no load touches a byte outside it; a valid width that is not a multiple of 4 ends inside a group, whose pixels
                 // past it are zeroed one by one.  Two batches of 3 groups: all loads of a batch are issued before any is used
                 // (6 groups at once do not fit the producer's 56 registers).
@@ -1055,10 +1075,20 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                         const int r = q / 10, g = q - r * 10;
                         const int y = iy0 + r, x = ix0 - 1 + 4 * g;
                         ok[j] = q < kS4Groups && (unsigned)y < (unsigned)lg.H && (unsigned)x < (unsigned)lg.W;
-                        const uint32_t* src = reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint8_t*>(p.in_raw) +
-                                                                                ((ptrdiff_t)n * plane + (ptrdiff_t)y * p.W + x) * 3);
+                        if (nv12) {
+                            // two words: Y of pixels x .. x + 3 at (y, x), and U0 V0 U1 V1 of their two 2x2 blocks at UV row y / 2, column x
+                            const uint8_t* img = reinterpret_cast<const uint8_t*>(p.in_raw) + (ptrdiff_t)n * (plane + (plane >> 1));
+                            const uint32_t* ys = reinterpret_cast<const uint32_t*>(img + (ptrdiff_t)y * p.W + x);
+                            const uint32_t* uvs = reinterpret_cast<const uint32_t*>(img + plane + (ptrdiff_t)(y >> 1) * p.W + x);
+                            wd[j][0] = ok[j] ? __ldg(ys) : 0u;
+                            wd[j][1] = ok[j] ? __ldg(uvs) : 0u;
+                            wd[j][2] = 0u;
+                        } else {
+                            const uint32_t* src = reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint8_t*>(p.in_raw) +
+                                                                                    ((ptrdiff_t)n * plane + (ptrdiff_t)y * p.W + x) * 3);
 #pragma unroll
-                        for (int k = 0; k < 3; ++k) wd[j][k] = ok[j] ? __ldg(src + k) : 0u;
+                            for (int k = 0; k < 3; ++k) wd[j][k] = ok[j] ? __ldg(src + k) : 0u;
+                        }
                     }
 #pragma unroll
                     for (int j = 0; j < kS4GroupBatch; ++j) {
@@ -1071,11 +1101,16 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                         for (int k = 0; k < 4; ++k) {
                             float f[3];
                             const bool okk = ok[j] && (!EXT || k < in_cols);
+                            uint32_t bytes[3];
+                            if (nv12) {
+                                nv12_to_bgr((wd[j][0] >> (8 * k)) & 0xffu, (wd[j][1] >> (8 * (k & 2))) & 0xffu,
+                                            (wd[j][1] >> (8 * (k & 2) + 8)) & 0xffu, bytes);
+                            } else {
 #pragma unroll
-                            for (int c = 0; c < 3; ++c) {
-                                const uint32_t byte = (wd[j][(3 * k + c) >> 2] >> (8 * ((3 * k + c) & 3))) & 0xffu;
-                                f[c] = okk ? p.xf.apply(c, byte) : 0.f;                              // zero padding of the normalised image
+                                for (int c = 0; c < 3; ++c) bytes[c] = (wd[j][(3 * k + c) >> 2] >> (8 * ((3 * k + c) & 3))) & 0xffu;
                             }
+#pragma unroll
+                            for (int c = 0; c < 3; ++c) f[c] = okk ? p.xf.apply(c, bytes[c]) : 0.f;     // zero padding of the normalised image
                             px[k][0] = pack2<F16>(sw ? f[2] : f[0], f[1]);                           // rounding point R0
                             px[k][1] = pack2<F16>(sw ? f[0] : f[2], 0.f);
                         }
@@ -1089,7 +1124,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                     }
                 }
             } else {
-                // per-pixel loader: fp32 NCHW, or u8 rows that are not whole aligned words
+                // per-pixel loader: fp32 NCHW, or uint8 (BGR / NV12) rows that are not whole aligned words
 #pragma unroll 1
                 for (int j0 = 0; j0 < kS4PerThread; j0 += kS4Batch) {
                     uint32_t raw[kS4Batch][3];
@@ -1101,7 +1136,11 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                         const int y = iy0 + r, x = ix0 + c;
                         ok[j] = q < kS4Pix && (interior || ((unsigned)y < (unsigned)lg.H && (unsigned)x < (unsigned)lg.W));
                         const ptrdiff_t pix = ok[j] ? (ptrdiff_t)n * plane + (ptrdiff_t)y * p.W + x : 0;
-                        if (u8) {
+                        if (nv12) {      // (Y, U, V); UV row = absolute row / 2, UV column = x & ~1
+                            const uint8_t* img = reinterpret_cast<const uint8_t*>(p.in_raw) + (ok[j] ? (ptrdiff_t)n * (plane + (plane >> 1)) : 0);
+                            const uint8_t* uv = img + plane + (ok[j] ? (ptrdiff_t)(y >> 1) * p.W + (x & ~1) : 0);
+                            raw[j][0] = __ldg(img + (ok[j] ? (ptrdiff_t)y * p.W + x : 0)); raw[j][1] = __ldg(uv); raw[j][2] = __ldg(uv + 1);
+                        } else if (u8) {
                             const uint8_t* src = reinterpret_cast<const uint8_t*>(p.in_raw) + pix * 3;
                             raw[j][0] = __ldg(src); raw[j][1] = __ldg(src + 1); raw[j][2] = __ldg(src + 2);
                         } else {
@@ -1114,6 +1153,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                     for (int j = 0; j < kS4Batch; ++j) {
                         const int q = ptid + (j0 + j) * kProdThreads;
                         if (q >= kS4Pix) break;
+                        if (nv12) nv12_to_bgr(raw[j][0], raw[j][1], raw[j][2], raw[j]);   // (Y, U, V) -> the bytes (B, G, R)
                         float f[3];
 #pragma unroll
                         for (int k = 0; k < 3; ++k) {

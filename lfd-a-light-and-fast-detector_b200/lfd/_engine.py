@@ -80,6 +80,32 @@ def check_frame(x, N, H, W):
     return fmt, int(h), int(w)
 
 
+def check_nv12_frame(x, N, H, W):
+    """x: NV12 frames, uint8 [N, 3h/2, w] (each image a Y plane of h rows x w bytes, then an interleaved UV plane of h/2 rows x w bytes),
+    contiguous, on a CUDA device, h and w even, h <= H and w <= W, on a capacity H x W that is even too -> (h, w)."""
+    if H % 2 or W % 2:
+        raise ValueError('NV12 frames need a plan of even height and width, this plan\'s capacity is %dx%d' % (H, W))
+    if x.dtype != torch.uint8 or x.dim() != 3:
+        raise ValueError('NV12 frames are a uint8 [N, 3h/2, w] tensor, got %s %s' % (x.dtype, tuple(x.shape)))
+    n, rows, w = (int(s) for s in x.shape)
+    if rows % 3 or w % 2:
+        raise ValueError('NV12 frames have an even height and width: %d rows x %d columns is not [3h/2, w] of an even h and w' % (rows, w))
+    h = rows // 3 * 2
+    if n != N or not (1 <= h <= H and 1 <= w <= W):
+        raise ValueError('input must be N=%d NV12 frames of at most H=%d x W=%d (the plan\'s capacity), got %d frames of %dx%d' % (N, H, W, n, h, w))
+    if not x.is_cuda or not x.is_contiguous():
+        raise ValueError('NV12 frames must be a contiguous CUDA tensor')
+    return h, w
+
+
+def stage_nv12(stage, x, h, w):
+    """Copies NV12 frames x [N, 3h/2, w] into the capacity layout stage [N, 3H/2, W]: the Y rows into the top-left corner of the H x W Y
+    plane, the UV rows into the top-left corner of the H/2 x W UV plane."""
+    H = stage.shape[1] // 3 * 2
+    stage[:, :h, :w].copy_(x[:, :h])
+    stage[:, H:H + h // 2, :w].copy_(x[:, h:])
+
+
 def tune_branch_bounds(work, measure, candidates, budget_s, max_branches=None):
     """Coordinate descent over per-branch bounds on the persistent CTAs of side-branch kernels.  work: {branch: amount of work};
     measure(caps) -> time of the plan with caps = {branch: bound} (0 = unbounded).  The branches with the most work come first (at most
@@ -743,25 +769,35 @@ class InferencePlan(object):
         return self._extents[(h, w)]
 
     def staging(self, fmt):
-        """The plan-owned input of frames below the capacity, in the capacity layout of format fmt (uint8 [N,H,W,3] or float32 [N,3,H,W])."""
+        """The plan-owned input of frames below the capacity, in the capacity layout of format fmt (uint8 [N,H,W,3], float32 [N,3,H,W] or
+        NV12 uint8 [N,3H/2,W])."""
         if self._stage is None:
             self._stage = torch.empty(self.N * 3 * self.H * self.W * 4, dtype=torch.uint8, device=self.device)
         if fmt == nat.INPUT_U8_NHWC:
             return self._stage[:self.N * self.H * self.W * 3].view(self.N, self.H, self.W, 3)
+        if fmt == nat.INPUT_U8_NV12:
+            return self._stage[:self.N * self.H * self.W * 3 // 2].view(self.N, self.H * 3 // 2, self.W)
         return self._stage.view(torch.float32).view(self.N, 3, self.H, self.W)
 
     def num_graphs(self):
         return nat.lib().lfd_plan_num_graphs(self.handle)
 
-    def forward(self, x, use_graph=True, slot=0):
-        """x: cuda float32 [N,3,h,w] (contiguous) or uint8 [N,h,w,3] with h <= H and w <= W.  Returns the frame's (cls, reg) in the
+    def forward(self, x, use_graph=True, slot=0, frame_format=None):
+        """x: cuda float32 [N,3,h,w] (contiguous) or uint8 [N,h,w,3] with h <= H and w <= W; with frame_format='nv12', NV12 video frames
+        uint8 [N,3h/2,w] of even h and w (include/lfd_b200.h, LFD_INPUT_U8_NV12), which give bit for bit what the uint8 path gives on
+        cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12).  Returns the frame's (cls, reg) in the
         plan-owned buffers of output `slot` (a second slot lets the post-process of one batch overlap the forward of the next,
         lfd/pipeline.py): (N, P, C') and (N, P, 4) for the frame's P points, laid out as a plan built for h x w lays them out;
         frame_level_sizes / frame_P describe them.  A frame of the full size is read in place; a smaller one is first copied into the
-        top-left corner of a plan-owned input, so that every frame size replays the same CUDA graph."""
+        top-left corner of a plan-owned input, so that every frame size replays the same CUDA graph (one per input format)."""
         if self.handle is None:
             raise nat.LfdError('this plan was built for host-side inspection only (create_native=False)')
-        fmt, h, w = check_frame(x, self.N, self.H, self.W)
+        if frame_format is None:
+            fmt, h, w = check_frame(x, self.N, self.H, self.W)
+        elif frame_format == 'nv12':
+            fmt, (h, w) = nat.INPUT_U8_NV12, check_nv12_frame(x, self.N, self.H, self.W)
+        else:
+            raise ValueError("frame_format must be None (float32 NCHW or uint8 BGR, by dtype) or 'nv12', got %r" % (frame_format,))
         cls_out, reg_out = self.outputs(slot)
         lib = nat.lib()
         if (h, w) == (self.H, self.W):
@@ -775,7 +811,9 @@ class InferencePlan(object):
         table, level_sizes, P = self._extent(h, w)
         with torch.cuda.device(self.device):
             stage = self.staging(fmt)
-            if fmt == nat.INPUT_U8_NHWC:
+            if fmt == nat.INPUT_U8_NV12:
+                stage_nv12(stage, x, h, w)
+            elif fmt == nat.INPUT_U8_NHWC:
                 stage[:, :h, :w].copy_(x)
             else:
                 stage[:, :, :h, :w].copy_(x)

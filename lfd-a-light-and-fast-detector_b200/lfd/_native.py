@@ -14,7 +14,7 @@ LIB_PATH = os.environ.get('LFD_B200_LIB') or os.path.join(_PKG, 'liblfd_b200.so'
 MAX_LEVELS = 8
 
 OP_STEM0, OP_CONV, OP_GN_APPLY, OP_HEAD_FINAL, OP_STEM4 = 0, 1, 2, 3, 4
-INPUT_F32_NCHW, INPUT_U8_NHWC = 0, 1
+INPUT_F32_NCHW, INPUT_U8_NHWC, INPUT_U8_NV12 = 0, 1, 2     # NV12: inference only, uint8 [N, 3H/2, W] (include/lfd_b200.h)
 CONV_UMMA, CONV_SIMT = 0, 1
 DTYPE_BF16, DTYPE_FP16 = 0, 1
 CLS_SIGMOID, CLS_SOFTMAX, CLS_BCE, CLS_QFL = 0, 1, 2, 3

@@ -43,8 +43,10 @@ class ForwardPostPipeline(object):
     slot is rewritten only after its post-process has finished.  The post-process buffers are single: `consume(results)`
     is called with the post stream current, enqueue device->host copies (or anything else that reads them) there."""
 
-    def __init__(self, model, plan, post, score_thr, iou_thr):
+    def __init__(self, model, plan, post, score_thr, iou_thr, frame_format=None):
+        """frame_format: of the device inputs, passed to plan.forward (None: float32 NCHW or uint8 BGR by dtype, 'nv12': NV12 frames)."""
         self.model, self.plan, self.post = model, plan, post
+        self.frame_format = frame_format
         self.score_thr, self.iou_thr = float(score_thr), float(iou_thr)
         dev = plan.device
         with torch.cuda.device(dev):
@@ -66,7 +68,7 @@ class ForwardPostPipeline(object):
                 self.fwd_stream.wait_event(wait_for)
             if self.k >= self.n_slots:
                 self.fwd_stream.wait_event(self.post_done[slot])
-            cls, reg = self.plan.forward(x, use_graph=self.model.use_cuda_graph, slot=slot)
+            cls, reg = self.plan.forward(x, use_graph=self.model.use_cuda_graph, slot=slot, frame_format=self.frame_format)
             self.fwd_done[slot].record(self.fwd_stream)
         with torch.cuda.stream(self.post_stream):
             self.post_stream.wait_event(self.fwd_done[slot])
@@ -81,10 +83,18 @@ class ForwardPostPipeline(object):
 class StreamingDetector(object):
 
     def __init__(self, model, batch, height, width, score_thr, iou_thr, max_out=1024, device=None, depth=3, copy_streams=4,
-                 input_pipeline=None):
+                 input_pipeline=None, frame_format='bgr'):
         """input_pipeline: the model's val pipeline, run on the uint8 frames inside the stem kernel -- None: simple_normalize on BGR;
         else BGR2RGB / a final Normalize of the declarative stand-ins (lfd/data_pipeline/augmentation.py), e.g. the TrafficLight
-        val_pipeline.  A pipeline the kernels cannot run raises ValueError here: frames are never normalised other than asked."""
+        val_pipeline.  A pipeline the kernels cannot run raises ValueError here: frames are never normalised other than asked.
+        frame_format: 'bgr' -- host frames uint8 [N,H,W,3]; 'nv12' -- NV12 video frames uint8 [N,3H/2,W] (H and W even), half the bytes
+        to copy, converted to BGR inside the stem kernel bit for bit as cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12) would, after which
+        input_pipeline applies as it does to BGR frames."""
+        if frame_format not in ('bgr', 'nv12'):
+            raise ValueError("frame_format must be 'bgr' or 'nv12', got %r" % (frame_format,))
+        if frame_format == 'nv12' and (height % 2 or width % 2):
+            raise ValueError('NV12 frames have an even height and width, got %dx%d' % (height, width))
+        self.frame_format = frame_format
         from .data_pipeline.augmentation import input_transform_of
         self.input_transform = input_transform_of(input_pipeline)
         self.model = model
@@ -111,21 +121,24 @@ class StreamingDetector(object):
             model._head_indexes_to_feature_map_sizes[i] = hw
         self.post = model.post_plan(batch, self.plan.level_sizes, dev)   # greedy NMS or Soft-NMS: model._nms_cfg as of now
         self.post.set_meta([width] * batch, [height] * batch, [1.0] * batch)
-        self.pipe = ForwardPostPipeline(model, self.plan, self.post, self.score_thr, self.iou_thr)
+        nv12 = frame_format == 'nv12'
+        self.pipe = ForwardPostPipeline(model, self.plan, self.post, self.score_thr, self.iou_thr, frame_format='nv12' if nv12 else None)
+        frame_shape = (batch, height * 3 // 2, width) if nv12 else (batch, height, width, 3)
         self.slots = []
         for _ in range(self.depth):
             self.slots.append(dict(
-                x=torch.empty((batch, height, width, 3), dtype=torch.uint8, device=dev),
+                x=torch.empty(frame_shape, dtype=torch.uint8, device=dev),
                 out_dets=torch.empty((batch, self.max_out, 5), dtype=torch.float32).pin_memory(),
                 out_labels=torch.empty((batch, self.max_out), dtype=torch.int32).pin_memory(),
                 out_count=torch.empty((batch + 1,), dtype=torch.int32).pin_memory(),
                 h2d=torch.cuda.Event(), h2d_aux=[torch.cuda.Event() for _ in self.copy_streams[1:]], done=torch.cuda.Event(), busy=False))
         self.step = 0
-        self.h2d_bytes = batch * height * width * 3
+        self.h2d_bytes = batch * height * width * 3 // (2 if nv12 else 1)
         self.d2h_bytes = batch * self.max_out * (5 * 4 + 4) + (batch + 1) * 4
 
     def submit(self, frames_u8):
-        """frames_u8: pinned (or pageable) host uint8 [N,H,W,3].  Enqueues copy + compute; returns the slot index."""
+        """frames_u8: pinned (or pageable) host uint8 [N,H,W,3] (frame_format 'nv12': [N,3H/2,W]).  Enqueues copy + compute; returns the
+        slot index."""
         s = self.slots[self.step % self.depth]
         if s['busy']:
             s['done'].synchronize()
