@@ -24,6 +24,8 @@
  *   lfd_assign_targets             LFD.annotation_to_target            lfd/model/lfd.py:109-259
  *   lfd_detection_loss             LFD.get_loss (loss + d loss/d outputs) lfd/model/lfd.py:284-395 with
  *                                  FocalLoss / CrossEntropyLoss / IoULoss lfd/model/losses/{focal_loss,cross_entropy_loss,iou_loss}.py
+ *   lfd_loss_weight_sum,           the same with enable_classification_weight / enable_regression_weight (lfd/model/lfd.py:322-384,
+ *   lfd_detection_loss_weighted    weight_reduce_loss lfd/model/losses/utils.py:28-53)
  */
 #ifndef LFD_B200_H_
 #define LFD_B200_H_
@@ -320,6 +322,28 @@ typedef struct lfd_loss_cfg {
 int lfd_detection_loss(const lfd_levels* lv, const lfd_loss_cfg* cfg, const float* cls_logits, const float* reg, const float* cls_target,
                        const float* reg_target, const int32_t* label, const int32_t* counters, float* grad_cls, float* grad_reg,
                        double* loss_sums, lfd_stream stream);
+
+/* enable_classification_weight / enable_regression_weight of the reference's LFD (lfd/model/lfd.py:322-384).  The weight of a positive
+ * row is its maximal classification target (the row maximum of cls_target, >= 0.001), and weight_sum is their sum over the batch.
+ *   lfd_loss_weight_sum: *weight_sum (device double[1]) = that sum over the rows with 0 <= label < C, in a fixed order (per-block
+ *       partials in `workspace`, of lfd_loss_weight_sum_workspace_bytes(cfg) bytes, then one block adds them up; no atomics), so
+ *       repeated calls give the same bits.  Reads cfg->N, P, C and max_ctas.  Data-parallel callers sum *weight_sum over their ranks
+ *       before the loss, as they do the counters.
+ *   lfd_detection_loss_weighted: lfd_detection_loss with the two switches (0 or 1 each; anything else is LFD_ERR_INVALID):
+ *       cls_weighted: classification avg_factor = *weight_sum instead of n_pos + 1 (no per-element weight, every cls_mode);
+ *       reg_weighted: each positive's regression loss times its weight (loss_sums[1] is then sum w_i * loss_i), avg_factor =
+ *       *weight_sum instead of n_pos; without positives the regression loss and its gradient are 0, as unweighted.
+ *       reg_weighted needs cls_target and is LFD_ERR_INVALID with SmoothL1 / MSE: there the reference multiplies the (n, 4) element
+ *       loss by the (n,) weight, which does not broadcast.
+ *   With both switches 0 it is lfd_detection_loss, bit for bit, and weight_sum may be NULL.  A zero *weight_sum (no positives) with
+ *   cls_weighted divides by zero, as the reference does: the classification gradients are +-inf (NaN where the element's own is 0). */
+size_t lfd_loss_weight_sum_workspace_bytes(const lfd_loss_cfg* cfg);
+int lfd_loss_weight_sum(const lfd_loss_cfg* cfg, const float* cls_target, const int32_t* label, void* workspace, double* weight_sum,
+                        lfd_stream stream);
+int lfd_detection_loss_weighted(const lfd_levels* lv, const lfd_loss_cfg* cfg, const float* cls_logits, const float* reg,
+                                const float* cls_target, const float* reg_target, const int32_t* label, const int32_t* counters,
+                                float* grad_cls, float* grad_reg, double* loss_sums, int cls_weighted, int reg_weighted,
+                                const double* weight_sum, lfd_stream stream);
 
 /* Element-wise box losses of the stand-alone IoULoss / GIoULoss / DIoULoss / CIoULoss modules (lfd/model/losses/iou_loss.py:105-283,
  * before the reduction): pred / target float[n][4] xyxy, kind = LFD_REG_IOU .. LFD_REG_CIOU; loss float[n], grad_pred float[n][4]

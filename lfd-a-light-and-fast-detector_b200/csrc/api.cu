@@ -900,30 +900,72 @@ extern "C" int lfd_assign_targets(const lfd_levels* lv, int N, int P, int C, int
     return LFD_OK;
 }
 
-extern "C" int lfd_detection_loss(const lfd_levels* lv, const lfd_loss_cfg* c, const float* cls_logits, const float* reg, const float* cls_target,
-                                  const float* reg_target, const int32_t* label, const int32_t* counters, float* grad_cls, float* grad_reg,
-                                  double* loss_sums, lfd_stream stream) {
-    if (!lv || !c || !cls_logits || !reg || !reg_target || !label || !counters || !loss_sums) return fail(LFD_ERR_INVALID, "lfd_detection_loss: null argument");
-    if (c->cls_mode < LFD_CLS_SIGMOID || c->cls_mode > LFD_CLS_QFL) return fail(LFD_ERR_INVALID, "lfd_detection_loss: unknown classification loss %d", c->cls_mode);
-    if ((c->cls_mode == LFD_CLS_BCE || c->cls_mode == LFD_CLS_QFL) && !cls_target) return fail(LFD_ERR_INVALID, "lfd_detection_loss: BCE / QFL need the soft classification targets");
-    if (c->reg_loss < LFD_REG_IOU || c->reg_loss > LFD_REG_MSE) return fail(LFD_ERR_INVALID, "lfd_detection_loss: unknown regression loss %d", c->reg_loss);
+static int detection_loss(const char* fn, const lfd_levels* lv, const lfd_loss_cfg* c, const float* cls_logits, const float* reg,
+                          const float* cls_target, const float* reg_target, const int32_t* label, const int32_t* counters, float* grad_cls,
+                          float* grad_reg, double* loss_sums, int cls_weighted, int reg_weighted, const double* weight_sum, lfd_stream stream) {
+    if (!lv || !c || !cls_logits || !reg || !reg_target || !label || !counters || !loss_sums) return fail(LFD_ERR_INVALID, "%s: null argument", fn);
+    if (c->cls_mode < LFD_CLS_SIGMOID || c->cls_mode > LFD_CLS_QFL) return fail(LFD_ERR_INVALID, "%s: unknown classification loss %d", fn, c->cls_mode);
+    if ((c->cls_mode == LFD_CLS_BCE || c->cls_mode == LFD_CLS_QFL) && !cls_target) return fail(LFD_ERR_INVALID, "%s: BCE / QFL need the soft classification targets", fn);
+    if (c->reg_loss < LFD_REG_IOU || c->reg_loss > LFD_REG_MSE) return fail(LFD_ERR_INVALID, "%s: unknown regression loss %d", fn, c->reg_loss);
     const bool indep = c->reg_loss == LFD_REG_SMOOTH_L1 || c->reg_loss == LFD_REG_MSE;
-    if (indep != (c->bbox_mode == LFD_BBOX_INDEPENDENT)) return fail(LFD_ERR_INVALID, "lfd_detection_loss: SmoothL1 / MSE go with the 'independent' targets, the IoU family with sigmoid / exp");
-    if (c->reg_loss == LFD_REG_SMOOTH_L1 && !(c->smooth_l1_beta > 0.f)) return fail(LFD_ERR_INVALID, "lfd_detection_loss: SmoothL1 beta must be > 0");
-    if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_detection_loss: no CUDA device (there is no CPU fallback)");
+    if (indep != (c->bbox_mode == LFD_BBOX_INDEPENDENT)) return fail(LFD_ERR_INVALID, "%s: SmoothL1 / MSE go with the 'independent' targets, the IoU family with sigmoid / exp", fn);
+    if (c->reg_loss == LFD_REG_SMOOTH_L1 && !(c->smooth_l1_beta > 0.f)) return fail(LFD_ERR_INVALID, "%s: SmoothL1 beta must be > 0", fn);
+    if ((cls_weighted != 0 && cls_weighted != 1) || (reg_weighted != 0 && reg_weighted != 1))
+        return fail(LFD_ERR_INVALID, "%s: cls_weighted / reg_weighted must be 0 or 1 (got %d, %d)", fn, cls_weighted, reg_weighted);
+    if ((cls_weighted || reg_weighted) && !weight_sum) return fail(LFD_ERR_INVALID, "%s: weighting needs weight_sum (lfd_loss_weight_sum)", fn);
+    if (reg_weighted && !cls_target) return fail(LFD_ERR_INVALID, "%s: regression weighting reads the weights from cls_target", fn);
+    if (reg_weighted && indep)
+        return fail(LFD_ERR_INVALID, "%s: regression weighting with SmoothL1 / MSE: the reference multiplies the (n, 4) element loss by the (n,) "
+                                     "weight, which does not broadcast", fn);
+    if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "%s: no CUDA device (there is no CPU fallback)", fn);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int sms = c->max_ctas > 0 ? c->max_ctas : sm_count();
     CUDA_TRY(cudaMemsetAsync(loss_sums, 0, 16, st));
     ClsLossParams k;
     k.logits = cls_logits; k.cls_target = cls_target; k.label = label; k.counters = counters; k.grad = grad_cls; k.loss_sum = loss_sums;
     k.N = c->N; k.P = c->P; k.C = c->C; k.cls_mode = c->cls_mode; k.gamma = c->gamma; k.alpha = c->alpha; k.loss_weight = c->cls_weight;
+    k.weighted = cls_weighted; k.weight_sum = weight_sum;
     CUDA_TRY(cls_loss_launch(k, sms, st));
     RegLossParams r;
     fill_levels(lv, &r.lv);
     r.reg = reg; r.reg_target = reg_target; r.label = label; r.counters = counters; r.grad = grad_reg; r.loss_sum = loss_sums + 1;
     r.N = c->N; r.P = c->P; r.C = c->C; r.bbox_mode = c->bbox_mode; r.loss_kind = c->reg_loss; r.eps = c->reg_eps; r.loss_weight = c->reg_weight;
     r.beta = c->smooth_l1_beta;
+    r.weighted = reg_weighted; r.weight_sum = weight_sum; r.cls_target = cls_target;
     CUDA_TRY(iou_loss_launch(r, sms, st));
+    return LFD_OK;
+}
+
+extern "C" int lfd_detection_loss(const lfd_levels* lv, const lfd_loss_cfg* c, const float* cls_logits, const float* reg, const float* cls_target,
+                                  const float* reg_target, const int32_t* label, const int32_t* counters, float* grad_cls, float* grad_reg,
+                                  double* loss_sums, lfd_stream stream) {
+    return detection_loss("lfd_detection_loss", lv, c, cls_logits, reg, cls_target, reg_target, label, counters, grad_cls, grad_reg, loss_sums,
+                          0, 0, nullptr, stream);
+}
+
+extern "C" int lfd_detection_loss_weighted(const lfd_levels* lv, const lfd_loss_cfg* c, const float* cls_logits, const float* reg,
+                                           const float* cls_target, const float* reg_target, const int32_t* label, const int32_t* counters,
+                                           float* grad_cls, float* grad_reg, double* loss_sums, int cls_weighted, int reg_weighted,
+                                           const double* weight_sum, lfd_stream stream) {
+    return detection_loss("lfd_detection_loss_weighted", lv, c, cls_logits, reg, cls_target, reg_target, label, counters, grad_cls, grad_reg,
+                          loss_sums, cls_weighted, reg_weighted, weight_sum, stream);
+}
+
+extern "C" size_t lfd_loss_weight_sum_workspace_bytes(const lfd_loss_cfg* c) {
+    if (!c) { fail(LFD_ERR_INVALID, "lfd_loss_weight_sum_workspace_bytes: null argument"); return 0; }
+    const int sms = c->max_ctas > 0 ? c->max_ctas : sm_count();
+    if (sms <= 0) { fail(LFD_ERR_CUDA, "lfd_loss_weight_sum_workspace_bytes: no CUDA device"); return 0; }
+    return (size_t)loss_weight_blocks(sms) * sizeof(double);
+}
+
+extern "C" int lfd_loss_weight_sum(const lfd_loss_cfg* c, const float* cls_target, const int32_t* label, void* workspace, double* weight_sum,
+                                   lfd_stream stream) {
+    if (!c || !cls_target || !label || !workspace || !weight_sum) return fail(LFD_ERR_INVALID, "lfd_loss_weight_sum: null argument");
+    if (c->N < 1 || c->P < 1 || c->C < 1) return fail(LFD_ERR_INVALID, "lfd_loss_weight_sum: bad shape");
+    if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_loss_weight_sum: no CUDA device (there is no CPU fallback)");
+    const int sms = c->max_ctas > 0 ? c->max_ctas : sm_count();
+    CUDA_TRY(loss_weight_sum_launch(cls_target, label, (size_t)c->N * c->P, c->C, sms, reinterpret_cast<double*>(workspace), weight_sum,
+                                    reinterpret_cast<cudaStream_t>(stream)));
     return LFD_OK;
 }
 

@@ -145,8 +145,15 @@ struct ClsLossParams {
     double* loss_sum;          // zeroed by the caller
     int N, P, C, cls_mode;     // 0 sigmoid focal, 1 cross entropy (C+1 logits), 2 BCE-with-logits on the soft targets, 3 quality focal (beta = gamma)
     float gamma, alpha, loss_weight;
+    int weighted;              // 1: avg_factor = *weight_sum (the sum of the positives' weights) instead of n_pos + 1
+    const double* weight_sum;
 };
 cudaError_t cls_loss_launch(const ClsLossParams& p, int num_sms, cudaStream_t st);
+// sum over the positive rows (0 <= label < C) of the row maximum of cls_target, in a fixed order: one partial per block of
+// loss_weight_partials_kernel (blocks of them, into `partials`), then one block adds the partials in index order into *weight_sum
+int loss_weight_blocks(int num_sms);
+cudaError_t loss_weight_sum_launch(const float* cls_target, const int* label, size_t rows, int C, int num_sms, double* partials,
+                                   double* weight_sum, cudaStream_t st);
 
 struct RegLossParams {
     LevelTable lv;
@@ -159,6 +166,9 @@ struct RegLossParams {
     int N, P, C, bbox_mode;    // 0 sigmoid * range, 1 exp, 2 independent (raw outputs against targets / range)
     int loss_kind;             // 0 IoU (-log), 1 GIoU, 2 DIoU, 3 CIoU, 4 SmoothL1, 5 MSE (4, 5: bbox_mode 2 only)
     float eps, loss_weight, beta;
+    int weighted;              // 1: each positive's loss times its weight (row maximum of cls_target), avg_factor = *weight_sum
+    const double* weight_sum;
+    const float* cls_target;   // (N, P, C), read when weighted
 };
 cudaError_t iou_loss_launch(const RegLossParams& p, int num_sms, cudaStream_t st);
 // element-wise IoU-family loss (kind 0..3) + d loss / d pred on explicit box pairs

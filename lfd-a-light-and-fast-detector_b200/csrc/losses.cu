@@ -12,6 +12,8 @@
 //   ce_loss_kernel          F.cross_entropy(reduction='none') + gradient (losses/cross_entropy_loss.py:12-22).
 //   iou_loss_kernel         decode (lfd.py:261-282,353-378) + -log(IoU) (losses/iou_loss.py:66-80,98-123) + analytic
 //                           gradient w.r.t. the raw regression outputs.
+//   loss_weight_*_kernel    weight.sum() of enable_classification_weight / enable_regression_weight (lfd.py:322-324), the
+//                           avg_factor of the weighted losses, summed in a fixed order.
 // All label-assignment arithmetic uses _rn intrinsics (no FMA contraction) so that scores / deltas are
 // bit-identical to the reference's separately rounded fp32 tensor ops.
 #include <cfloat>
@@ -177,12 +179,44 @@ __device__ __forceinline__ double block_sum(double v, double* sh) {
     return r;  // valid on thread 0
 }
 
-// classification loss of get_loss (lfd.py:326-341): rows with label -1 are dropped, avg_factor = n_pos + 1.
-// cls_mode 0: sigmoid focal over C logits; 1: cross entropy over C+1 logits.  Writes d loss / d logit.
+// weight of a positive row (lfd.py:322-324): its maximal classification target, the centre score of its best green gt.  Read from
+// the soft targets rather than stored by assign_targets_kernel, so the assignment and its callers stay as they are; the loss
+// kernels read the row only for the few positive points.
+__device__ __forceinline__ float row_weight(const float* cls_target, size_t r, int C) {
+    const float* row = cls_target + r * C;
+    float w = row[0];
+    for (int c = 1; c < C; ++c) w = fmaxf(w, row[c]);
+    return w;
+}
+
+// sum of the positives' weights (the reference's weight.sum()): per-block partials in a fixed order, then one block adds them up in
+// index order -- no floating-point atomics, so repeated steps give the same bits
+__global__ void __launch_bounds__(256) loss_weight_partials_kernel(const float* __restrict__ cls_target, const int* __restrict__ label, size_t rows,
+                                                                   int C, double* __restrict__ partials) {
+    __shared__ double sh[8];
+    double acc = 0.0;
+    for (size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (size_t)gridDim.x * blockDim.x) {
+        const int t = label[r];
+        if (t >= 0 && t < C) acc += (double)row_weight(cls_target, r, C);
+    }
+    const double s = block_sum(acc, sh);
+    if (threadIdx.x == 0) partials[blockIdx.x] = s;
+}
+__global__ void __launch_bounds__(256) loss_weight_final_kernel(const double* __restrict__ partials, int n, double* __restrict__ weight_sum) {
+    __shared__ double sh[8];
+    double acc = 0.0;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) acc += partials[i];
+    const double s = block_sum(acc, sh);
+    if (threadIdx.x == 0) *weight_sum = s;
+}
+
+// classification loss of get_loss (lfd.py:326-341): rows with label -1 are dropped, avg_factor = n_pos + 1 (weighted: the sum of the
+// positives' weights, enable_classification_weight).  cls_mode 0: sigmoid focal over C logits; 1: cross entropy over C+1 logits.
+// Writes d loss / d logit.
 __global__ void __launch_bounds__(256) cls_loss_kernel(const ClsLossParams p) {
     __shared__ double sh[8];
     const int Cp = p.cls_mode == 1 ? p.C + 1 : p.C;
-    const float inv_avg = 1.0f / (float)(p.counters[0] + 1);
+    const float inv_avg = p.weighted ? 1.0f / (float)*p.weight_sum : 1.0f / (float)(p.counters[0] + 1);
     double acc = 0.0;
     const size_t rows = (size_t)p.N * p.P;
     if (p.cls_mode != 1) {
@@ -238,7 +272,14 @@ __global__ void __launch_bounds__(256) cls_loss_kernel(const ClsLossParams p) {
             for (int c = 0; c < Cp; ++c) den += expf(x[c] - mx);
             const float lden = logf(den);
             acc += (double)(-(x[t] - mx - lden));
-            if (g) for (int c = 0; c < Cp; ++c) g[c] = (expf(x[c] - mx) / den - (c == t ? 1.f : 0.f)) * inv_avg * p.loss_weight;
+            if (g && p.weighted) {
+                // as autograd's log_softmax backward, softmax * s - onehot * s: without positives s = inf and the target logit's
+                // gradient is NaN, the others +inf, exactly as the reference's
+                const float s = inv_avg * p.loss_weight;
+                for (int c = 0; c < Cp; ++c) g[c] = expf(x[c] - mx) / den * s - (c == t ? s : 0.f);
+            } else if (g) {
+                for (int c = 0; c < Cp; ++c) g[c] = (expf(x[c] - mx) / den - (c == t ? 1.f : 0.f)) * inv_avg * p.loss_weight;
+            }
         }
     }
     const double s = block_sum(acc, sh);
@@ -305,16 +346,23 @@ __device__ __forceinline__ Dual iou_family_loss(int kind, const Dual* pr, const 
 
 // regression loss of get_loss (lfd.py:343-387): positives, avg_factor = n_pos.  loss_kind 0: -log IoU (analytic gradient);
 // 1..3: GIoU / DIoU / CIoU through forward-mode derivatives; 4, 5: SmoothL1 / MSE on the raw outputs ('independent' targets).
+// weighted (enable_regression_weight, weight_reduce_loss of losses/utils.py:28-53): the row loss times the row's weight, avg_factor =
+// the sum of the weights; no positives: loss and gradients 0 either way (lfd.py:386-387).
 __global__ void __launch_bounds__(256) iou_loss_kernel(const RegLossParams p) {
     __shared__ double sh[8];
     const size_t rows = (size_t)p.N * p.P;
     const int npos = p.counters[0];
-    const float inv_avg = npos > 0 ? 1.0f / (float)npos : 0.f;
+    const float inv_avg = npos > 0 ? (p.weighted ? 1.0f / (float)*p.weight_sum : 1.0f / (float)npos) : 0.f;
     double acc = 0.0;
     for (size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (size_t)gridDim.x * blockDim.x) {
         const int t = p.label[r];
         float4 g4 = make_float4(0.f, 0.f, 0.f, 0.f);
         if (t >= 0 && t < p.C) {
+            float sc = inv_avg * p.loss_weight, wt = 1.0f;   // wt = 1: the product below is exact, the unweighted sums keep their bits
+            if (p.weighted) {
+                wt = row_weight(p.cls_target, r, p.C);
+                sc *= wt;
+            }
             const int pt = (int)(r % p.P);
             const PointGeom pg = point_geom(p.lv, pt);
             const float4 rv = reinterpret_cast<const float4*>(p.reg)[r];
@@ -331,8 +379,7 @@ __global__ void __launch_bounds__(256) iou_loss_kernel(const RegLossParams p) {
                         else { ls += ad - 0.5f * p.beta; gk[k] = df > 0.f ? 1.f : -1.f; }
                     } else { ls += df * df; gk[k] = 2.f * df; }  // F.mse_loss(reduction='none')
                 }
-                acc += (double)ls;
-                const float sc = inv_avg * p.loss_weight;
+                acc += (double)(ls * wt);
                 if (p.grad) reinterpret_cast<float4*>(p.grad)[r] = make_float4(gk[0] * sc, gk[1] * sc, gk[2] * sc, gk[3] * sc);
                 continue;
             }
@@ -347,8 +394,7 @@ __global__ void __launch_bounds__(256) iou_loss_kernel(const RegLossParams p) {
                 const Dual pr[4] = {dvar(px1, 0), dvar(py1, 1), dvar(px2, 2), dvar(py2, 3)};
                 const float tg[4] = {tx1, ty1, tx2, ty2};
                 const Dual ls = iou_family_loss(p.loss_kind, pr, tg, p.eps);
-                acc += (double)ls.v;
-                const float sc = inv_avg * p.loss_weight;
+                acc += (double)(ls.v * wt);
                 if (p.grad) reinterpret_cast<float4*>(p.grad)[r] = make_float4(-ls.d[0] * dd[0] * sc, -ls.d[1] * dd[1] * sc, ls.d[2] * dd[2] * sc, ls.d[3] * dd[3] * sc);
                 continue;
             }
@@ -362,7 +408,7 @@ __global__ void __launch_bounds__(256) iou_loss_kernel(const RegLossParams p) {
             const float un = fmaxf(ur, 1e-6f);
             const float iou = ov / un;
             const float iouc = fmaxf(iou, p.eps);
-            acc += (double)(-logf(iouc));
+            acc += (double)(-logf(iouc) * wt);
             if (p.grad) {
                 const float g_iou = iou >= p.eps ? -1.0f / iouc : 0.f;
                 const float un_live = ur > 1e-6f ? 1.f : 0.f;
@@ -375,7 +421,6 @@ __global__ void __launch_bounds__(256) iou_loss_kernel(const RegLossParams p) {
                 if (px1 > tx1) g_px1 -= g_w; else if (px1 == tx1) g_px1 -= 0.5f * g_w;
                 if (py2 < ty2) g_py2 += g_h; else if (py2 == ty2) g_py2 += 0.5f * g_h;
                 if (py1 > ty1) g_py1 -= g_h; else if (py1 == ty1) g_py1 -= 0.5f * g_h;
-                const float sc = inv_avg * p.loss_weight;
                 g4 = make_float4(-g_px1 * dd[0] * sc, -g_py1 * dd[1] * sc, g_px2 * dd[2] * sc, g_py2 * dd[3] * sc);
             }
         }
@@ -429,6 +474,16 @@ cudaError_t cls_loss_launch(const ClsLossParams& p, int num_sms, cudaStream_t st
 }
 cudaError_t iou_loss_launch(const RegLossParams& p, int num_sms, cudaStream_t st) {
     iou_loss_kernel<<<num_sms * 4, 256, 0, st>>>(p);
+    return cudaGetLastError();
+}
+int loss_weight_blocks(int num_sms) { return num_sms * 4; }
+cudaError_t loss_weight_sum_launch(const float* cls_target, const int* label, size_t rows, int C, int num_sms, double* partials,
+                                   double* weight_sum, cudaStream_t st) {
+    const int blocks = loss_weight_blocks(num_sms);
+    loss_weight_partials_kernel<<<blocks, 256, 0, st>>>(cls_target, label, rows, C, partials);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    loss_weight_final_kernel<<<1, 256, 0, st>>>(partials, blocks, weight_sum);
     return cudaGetLastError();
 }
 

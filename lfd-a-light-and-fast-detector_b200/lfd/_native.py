@@ -162,6 +162,9 @@ SYMBOLS = {
     'lfd_nms': (_i, [_vp, _i, _f, _vp, _vp, _vp, _vp]),
     'lfd_assign_targets': (_i, [C.POINTER(Levels), _i, _i, _i, _i, _i, _i] + [_vp] * 8),
     'lfd_detection_loss': (_i, [C.POINTER(Levels), C.POINTER(LossCfg)] + [_vp] * 10),
+    'lfd_loss_weight_sum_workspace_bytes': (C.c_size_t, [C.POINTER(LossCfg)]),
+    'lfd_loss_weight_sum': (_i, [C.POINTER(LossCfg)] + [_vp] * 5),
+    'lfd_detection_loss_weighted': (_i, [C.POINTER(Levels), C.POINTER(LossCfg)] + [_vp] * 9 + [_i, _i, _vp, _vp]),
     'lfd_box_loss': (_i, [_i, _vp, _vp, _i, _f, _vp, _vp, _vp]),
     'lfd_sigmoid_focal_loss_forward': (_i, [_vp, _vp, _i, _i, _f, _f, _vp, _vp]),
     'lfd_sigmoid_focal_loss_backward': (_i, [_vp, _vp, _vp, _i, _i, _f, _f, _vp, _vp]),

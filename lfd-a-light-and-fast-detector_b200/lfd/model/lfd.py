@@ -9,7 +9,8 @@ Same constructor kwargs, state_dict keys and public methods (`forward`, `get_los
     get_results / predict_*   -> lfd_postprocess       (sigmoid|softmax + decode + class-aware NMS on device), or
                                  lfd_postprocess_soft_nms when _nms_cfg['type'] is 'soft_nms'
     annotation_to_target      -> lfd_assign_targets    (label assignment on device)
-    get_loss                  -> lfd_assign_targets + lfd_detection_loss (loss + gradients w.r.t. the outputs)
+    get_loss                  -> lfd_assign_targets + lfd_detection_loss (loss + gradients w.r.t. the outputs); with classification /
+                                 regression weighting lfd_loss_weight_sum + lfd_detection_loss_weighted
 
 There is no CPU path: modules and inputs must live on a CUDA (sm_90) device.
 `predict_for_single_image_with_tensorrt` (reference :657-800) is out of scope (TensorRT is not part of the
@@ -337,8 +338,10 @@ class LFD(nn.Module):
                          MSELoss=nat.REG_MSE)
         if cname not in cls_codes or rname not in reg_codes:
             raise NotImplementedError('native get_loss: unknown loss pair %s + %s' % (cname, rname))
-        if self._enable_classification_weight or self._enable_regression_weight:
-            raise NotImplementedError('classification / regression weighting is disabled in every shipped config and not implemented')
+        cls_w, reg_w = bool(self._enable_classification_weight), bool(self._enable_regression_weight)
+        if reg_w and self._regression_loss_type == 'independent':
+            raise ValueError('enable_regression_weight with %s: the reference multiplies the (n, 4) element loss of the positives by their (n,) '
+                             'weights, which does not broadcast (it raises for every batch whose positive count is not 0, 1 or 4)' % rname)
         device = cls_pred.device
         if not cls_pred.is_cuda:
             raise RuntimeError('lfd_b200 has no CPU path')
@@ -349,12 +352,18 @@ class LFD(nn.Module):
         # Data-parallel training: the reference normalises by the positives of the WHOLE (gathered) batch
         # (reference :323,340,383 run after the DataParallel gather), so the per-rank counters are summed over the process
         # group before the loss kernels use them; per-rank losses / gradients then ADD up to the global-batch values and the
-        # gradient all-reduce must sum, not average (`loss_globally_normalised`, read by OptimizerHook).
+        # gradient all-reduce must sum, not average (`loss_globally_normalised`, read by OptimizerHook).  With weighting the sum of the
+        # positives' weights is the normaliser (the reference's weight.sum() over the gathered batch), summed the same way.
+        N, P = cls_pred.shape[0], cls_pred.shape[1]
+        lc = nat.LossCfg()
+        lc.N, lc.P, lc.C = N, P, self._num_classes
+        weight_sum = self._loss_weight_sum(lc, cls_t, label, device) if cls_w or reg_w else None
         self.loss_globally_normalised = False
         if self._data_parallel():
             torch.distributed.all_reduce(counters, op=torch.distributed.ReduceOp.SUM)
+            if weight_sum is not None:
+                torch.distributed.all_reduce(weight_sum, op=torch.distributed.ReduceOp.SUM)
             self.loss_globally_normalised = True
-        N, P = cls_pred.shape[0], cls_pred.shape[1]
         cls_c = cls_pred.detach().float().contiguous()
         reg_c = reg_pred.detach().float().contiguous()
         need_grad = cls_pred.requires_grad or reg_pred.requires_grad
@@ -362,8 +371,6 @@ class LFD(nn.Module):
         grad_reg = torch.empty_like(reg_c) if need_grad else None
         sums = torch.empty((2,), dtype=torch.float64, device=device)
         lf, rf = self._classification_loss_func, self._regression_loss_func
-        lc = nat.LossCfg()
-        lc.N, lc.P, lc.C = N, P, self._num_classes
         lc.cls_mode, lc.reg_loss = cls_codes[cname], reg_codes[rname]
         if self._regression_loss_type == 'independent':
             lc.bbox_mode = nat.BBOX_INDEPENDENT
@@ -375,11 +382,20 @@ class LFD(nn.Module):
         lc.smooth_l1_beta = float(getattr(rf, 'beta', 1.0))
         lc.cls_weight, lc.reg_weight = float(lf.loss_weight), float(rf.loss_weight)
         with torch.cuda.device(device):
-            nat.check(nat.lib().lfd_detection_loss(C.byref(lv), C.byref(lc), nat.ptr(cls_c), nat.ptr(reg_c), nat.ptr(cls_t), nat.ptr(reg_t), nat.ptr(label),
-                                                   nat.ptr(counters), nat.ptr(grad_cls), nat.ptr(grad_reg), nat.ptr(sums), nat.stream_ptr()))
+            if weight_sum is None:
+                nat.check(nat.lib().lfd_detection_loss(C.byref(lv), C.byref(lc), nat.ptr(cls_c), nat.ptr(reg_c), nat.ptr(cls_t), nat.ptr(reg_t),
+                                                       nat.ptr(label), nat.ptr(counters), nat.ptr(grad_cls), nat.ptr(grad_reg), nat.ptr(sums),
+                                                       nat.stream_ptr()))
+            else:
+                nat.check(nat.lib().lfd_detection_loss_weighted(C.byref(lv), C.byref(lc), nat.ptr(cls_c), nat.ptr(reg_c), nat.ptr(cls_t), nat.ptr(reg_t),
+                                                                nat.ptr(label), nat.ptr(counters), nat.ptr(grad_cls), nat.ptr(grad_reg), nat.ptr(sums),
+                                                                int(cls_w), int(reg_w), nat.ptr(weight_sum), nat.stream_ptr()))
         n_pos = counters[0].to(torch.float64)
-        cls_loss = (lf.loss_weight * sums[0] / (n_pos + 1.0)).float()
-        reg_loss = torch.where(n_pos > 0, rf.loss_weight * sums[1] / torch.clamp(n_pos, min=1.0), torch.zeros_like(sums[1])).float()
+        # weighted: avg_factor = weight.sum() (lfd.py:334-384); without positives it is 0 and the classification loss is inf / NaN, as in the
+        # reference, while the regression loss stays 0 (lfd.py:386-387)
+        cls_loss = (lf.loss_weight * sums[0] / (weight_sum[0] if cls_w else n_pos + 1.0)).float()
+        reg_den = weight_sum[0] if reg_w else torch.clamp(n_pos, min=1.0)
+        reg_loss = torch.where(n_pos > 0, rf.loss_weight * sums[1] / reg_den, torch.zeros_like(sums[1])).float()
         total = cls_loss + reg_loss
         if need_grad:
             loss = _DetectionLossFn.apply(cls_pred, reg_pred, total, grad_cls, grad_reg)
@@ -390,19 +406,29 @@ class LFD(nn.Module):
             torch.distributed.all_reduce(vals, op=torch.distributed.ReduceOp.SUM)
         return dict(loss=loss, loss_values=LossValues(vals))      # floats on first access (asynchronous D2H), see LossValues
 
+    def _loss_weight_sum(self, lc, cls_t, label, device):
+        """The sum of the positives' weights (their maximal classification targets) on the device, float64 [1], in a fixed order."""
+        weight_sum = torch.empty((1,), dtype=torch.float64, device=device)
+        with torch.cuda.device(device):
+            ws = torch.empty((max(int(nat.lib().lfd_loss_weight_sum_workspace_bytes(C.byref(lc))), 8) + 7) // 8, dtype=torch.float64, device=device)
+            nat.check(nat.lib().lfd_loss_weight_sum(C.byref(lc), nat.ptr(cls_t), nat.ptr(label), nat.ptr(ws), nat.ptr(weight_sum), nat.stream_ptr()))
+        return weight_sum
+
     def _data_parallel(self):
         return self.training and torch.distributed.is_available() and torch.distributed.is_initialized() \
             and torch.distributed.get_world_size() > 1
 
     def empty_shard_loss(self):
-        """A rank whose shard of the batch is empty: joins the two collectives of get_loss (positive counters, logged loss values)
-        with zeros and returns loss=None (OptimizerHook then reduces zero gradients)."""
+        """A rank whose shard of the batch is empty: joins the collectives of get_loss (positive counters, the weight sum when weighting is
+        on, logged loss values) with zeros and returns loss=None (OptimizerHook then reduces zero gradients)."""
         device = self._device()
         self.loss_globally_normalised = False
         vals = torch.zeros(3, dtype=torch.float32, device=device)
         if self._data_parallel():
             counters = torch.zeros((2,), dtype=torch.int32, device=device)
             torch.distributed.all_reduce(counters, op=torch.distributed.ReduceOp.SUM)
+            if self._enable_classification_weight or self._enable_regression_weight:
+                torch.distributed.all_reduce(torch.zeros((1,), dtype=torch.float64, device=device), op=torch.distributed.ReduceOp.SUM)
             self.loss_globally_normalised = True
             torch.distributed.all_reduce(vals, op=torch.distributed.ReduceOp.SUM)
         return dict(loss=None, loss_values=LossValues(vals))
