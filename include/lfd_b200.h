@@ -55,7 +55,7 @@ typedef struct lfd_plan lfd_plan;
 int lfd_abi_version(void);
 /* sizeof of the structs of this header as the library was compiled, for bindings that mirror them field by field (ctypes, cffi):
  * which = 0 lfd_op, 1 lfd_top, 2 lfd_pack_desc, 3 lfd_unpack_desc, 4 lfd_post_cfg, 5 lfd_loss_cfg, 6 lfd_levels, 7 lfd_input_desc,
- * 8 lfd_extent;
+ * 8 lfd_extent, 9 lfd_engine_desc;
  * -1 for anything else. */
 int lfd_struct_bytes(int which);
 const char* lfd_last_error(void);
@@ -504,6 +504,60 @@ typedef struct lfd_input_desc {
  * 1-channel source is replicated to 3.  mean / scale: host float[3], unused in the uint8 mode.  W <= 6144. */
 int lfd_input_batch(const lfd_input_desc* descs, int n, const uint8_t* src, void* out, int out_mode, int swap_rb, int H, int W,
                     const float* mean, const float* scale, lfd_stream stream);
+
+/* ------------------------------------------------------------------------------------------ model files
+ * A model file (written by lfd/_engine.py InferencePlan.export, lfd.deployment.export_model) is one inference plan with its weights and
+ * its post-process, so that a program that links only this library and cudart runs a trained model: the same kernels, launches and
+ * results as the Python plan it was exported from.  Little-endian; DESIGN.md "Model files" has the layout:
+ *   header   48 bytes: "LFDMODEL", format version (LFD_MODEL_FORMAT_VERSION), lfd_abi_version(), target "sm_90a", sizeof(lfd_op),
+ *            sizeof(lfd_post_cfg), payload bytes, CRC-32 of the payload (zlib's), a zero word
+ *   payload  the plan (capacity, P, cls_channels, dtype, conv_impl, op count, statistics region, workspace bytes, input transform,
+ *            NMS type and Soft-NMS arguments, blob sizes; 120 bytes), the lfd_post_cfg, the lfd_op records, per op (index of the op that
+ *            produces its input or -1, head level or -1), the fp32 blob, the 16-bit blob.
+ * In an lfd_op record every pointer field holds ((blob + 1) << 56) | byte offset into the blob (blob 0 = fp32, 1 = 16-bit), or 0 for NULL.
+ *
+ * lfd_engine_open validates the whole file before keeping it (host only, no device needed): header fields, struct sizes, checksum, sizes
+ * and bounds of the plan, every op (kind, geometry as lfd_plan_create and the wgmma kernel's configuration take it, the image op at the
+ * capacity, the input transform on the image op only and equal to the plan's, branch, every workspace range against the workspace, every
+ * (blob, offset) range against its blob, the producer / level table with each op reading an output of its producer of matching size and
+ * channels) and the post-process configuration.  A file it refuses gives LFD_ERR_INVALID (or
+ * LFD_ERR_UNSUPPORTED: another format version, ABI or target, a SIMT plan) and an lfd_last_error() that names the field. */
+#define LFD_MODEL_FORMAT_VERSION 1
+typedef struct lfd_engine lfd_engine;
+typedef struct lfd_engine_desc {
+    int32_t N, H, W;              /* capacity: frames of up to H x W, N per call */
+    int32_t P, cls_channels;      /* points and classification channels at the capacity */
+    int32_t num_classes, dtype, n_ops;
+    int32_t cap;                  /* detections per image (dets / labels rows) */
+    int32_t soft_nms;             /* 0 greedy NMS, 1 Soft-NMS */
+    int64_t weights_bytes;        /* device buffer for lfd_engine_bind's weights */
+    int64_t workspace_bytes;      /* forward workspace, including the engine's own cls / reg region */
+    int64_t post_workspace_bytes; /* post-process workspace */
+} lfd_engine_desc;
+int lfd_engine_open(const void* bytes, size_t n, lfd_engine** out);
+int lfd_engine_close(lfd_engine* engine);
+int lfd_engine_info(const lfd_engine* engine, lfd_engine_desc* out);
+/* op i of the file as stored (pointer fields in the (blob, offset) encoding above); src_op / level may be NULL */
+int lfd_engine_op(const lfd_engine* engine, int i, lfd_op* op, int32_t* src_op, int32_t* level);
+/* Copies the weights into `weights` (asynchronously on `stream`: the caller's later work on `stream` sees them), resolves the ops'
+ * pointers and creates the plan (lfd_plan_create: needs the device).  The buffers stay the caller's and must outlive the engine or the
+ * next bind; a buffer smaller than lfd_engine_info reports fails with LFD_ERR_CAPACITY, one not aligned to 256 bytes (what cudaMalloc
+ * returns; the weights are bulk-copied and the activations reached through TMA) with LFD_ERR_INVALID, before anything is copied.  Like
+ * lfd_plan_*, the engine's plan keeps its side streams, events and CUDA graphs, and on the first frame below the capacity a device
+ * geometry table and a pinned staging ring for it (lfd_plan_forward_extent); everything sized by the model is in the caller's buffers. */
+int lfd_engine_bind(lfd_engine* engine, void* weights, size_t weights_bytes, void* workspace, size_t workspace_bytes, void* post_workspace,
+                    size_t post_workspace_bytes, lfd_stream stream);
+/* One batch: lfd_plan_forward_extent on N frames of h x w (<= the capacity) in the capacity layout of input_format (see
+ * lfd_plan_forward_extent), then lfd_postprocess / lfd_postprocess_soft_nms with image size w x h and resize scale 1.  The geometry table
+ * of a smaller frame is derived from the file.  Outputs (device): dets float[N][cap][5] = x1, y1, x2, y2, score; labels int32[N][cap];
+ * count int32[N + 1] (count[N] = 1: an image had more than cap candidates).  cls_out float[N][P][cls_channels] / reg_out float[N][P][4]
+ * receive the frame's network outputs (laid out as lfd_plan_forward_extent lays them out), or are NULL: the engine's region of the
+ * workspace holds them then.  use_graph: the forward is replayed as a CUDA graph (lfd_plan_forward).  No host synchronisation; every
+ * argument is checked before anything is enqueued.  The calls of one engine share its workspaces: the caller orders them (one stream,
+ * or events between streams), as for one lfd_plan. */
+int lfd_engine_detect(lfd_engine* engine, const void* input, int input_format, int h, int w, float* dets, int32_t* labels, int32_t* count,
+                      float* cls_out, float* reg_out, int use_graph, lfd_stream stream);
+int lfd_engine_num_launches(const lfd_engine* engine); /* lfd_plan_num_launches of the bound plan (0 before lfd_engine_bind) */
 
 #ifdef __cplusplus
 }

@@ -15,6 +15,10 @@ CSRC = os.path.join(HERE, 'csrc')
 OUT = os.environ.get('LFD_B200_OUT') or os.path.join(HERE, 'liblfd_b200.so')      # LFD_B200_OUT / LFD_B200_EXTRA_FLAGS: tuning experiments only
 SOURCES = ['api.cu', 'conv_umma.cu', 'conv_simt.cu', 'postprocess.cu', 'losses.cu', 'train.cu', 'wgrad_umma.cu', 'input.cu']
 HEADERS = ['ptx.cuh', 'conv_common.cuh', 'kernels.cuh', 'train.cuh', os.path.join('..', '..', 'include', 'lfd_b200.h')]
+INCLUDE = os.path.join(os.path.dirname(HERE), 'include')
+# the C program that runs a model file through the library and cudart alone (include/lfd_b200.h, lfd_engine_*), built next to the library
+EXAMPLE = os.path.join(os.path.dirname(HERE), 'examples', 'lfd_detect.c')
+EXAMPLE_OUT = os.path.join(os.path.dirname(OUT), 'lfd_detect')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 FLAGS = ARCH + ['-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
@@ -22,12 +26,8 @@ FLAGS = ARCH + ['-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
         (['-DLFD_B200_TIMELINE'] if os.environ.get('LFD_B200_TIMELINE') else []) + os.environ.get('LFD_B200_EXTRA_FLAGS', '').split()
 
 
-def _stale():
-    if not os.path.exists(OUT):
-        return True
-    t = os.path.getmtime(OUT)
-    deps = [os.path.join(CSRC, s) for s in SOURCES + HEADERS] + [os.path.abspath(__file__)]
-    return any(os.path.getmtime(d) > t for d in deps)
+def _stale(out, deps):
+    return not os.path.exists(out) or any(os.path.getmtime(d) > os.path.getmtime(out) for d in deps)
 
 
 # kernels whose per-thread state must stay in registers (the soft-NMS kernel runs one iteration per candidate: a spill is paid K times)
@@ -59,7 +59,14 @@ def _check_stack_frames(ptxas_log, limit=64):
 
 
 def build(force=False, verbose=False):
-    if not force and not _stale():
+    """The library, then the example program; each is rebuilt only when its own inputs changed."""
+    build_library(force, verbose)
+    build_example(force)
+    return OUT
+
+
+def build_library(force=False, verbose=False):
+    if not force and not _stale(OUT, [os.path.join(CSRC, s) for s in SOURCES + HEADERS] + [os.path.abspath(__file__)]):
         return OUT
     objs = []
     procs = []
@@ -81,6 +88,16 @@ def build(force=False, verbose=False):
             sys.stderr.write(out)
     subprocess.check_call([NVCC, '-shared', '-o', OUT] + objs + ARCH + ['-lcudart'])
     return OUT
+
+
+def build_example(force=False):
+    """examples/lfd_detect.c, host code only: linked against the library by its file name (found next to the program at run time) and
+    the shared cudart the library uses."""
+    if not force and not _stale(EXAMPLE_OUT, [EXAMPLE, OUT, os.path.join(INCLUDE, 'lfd_b200.h'), os.path.abspath(__file__)]):
+        return EXAMPLE_OUT
+    subprocess.check_call([NVCC] + ARCH + ['-O2', '-I', INCLUDE, EXAMPLE, '-o', EXAMPLE_OUT, '-L', os.path.dirname(OUT), '-l:' + os.path.basename(OUT),
+                           '-cudart', 'shared', '-Xlinker', '-rpath,$ORIGIN'])
+    return EXAMPLE_OUT
 
 
 if __name__ == '__main__':

@@ -2,6 +2,7 @@
 #include <stdarg.h>
 #include <cmath>
 #include <stdio.h>
+#include <string.h>
 
 #include <vector>
 
@@ -251,6 +252,7 @@ extern "C" int lfd_struct_bytes(int which) {
         case 6: return (int)sizeof(lfd_levels);
         case 7: return (int)sizeof(lfd_input_desc);
         case 8: return (int)sizeof(lfd_extent);
+        case 9: return (int)sizeof(lfd_engine_desc);
     }
     return -1;
 }
@@ -1275,4 +1277,436 @@ extern "C" int lfd_input_batch(const lfd_input_desc* descs, int n, const uint8_t
     if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_input_batch: no CUDA device (there is no CPU fallback)");
     CUDA_TRY(input_batch_launch(descs, n, src, out, out_mode, swap_rb, H, W, mean, scale, st_of(stream)));
     return LFD_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ model files (lfd_engine_*)
+// The layout is documented in include/lfd_b200.h and DESIGN.md "Model files"; lfd/_engine.py InferencePlan.export is the writer.
+static constexpr size_t kModelHeaderBytes = 48, kModelPlanBytes = 120;
+static constexpr int kModelMaxOps = 4096, kModelMaxN = 1024, kModelMaxSide = 16384, kModelMaxChannels = 4096, kModelMaxCap = 1 << 20;
+static constexpr int64_t kModelMaxWorkspace = (int64_t)1 << 40, kModelMaxBlob = (int64_t)1 << 34;
+static constexpr uint64_t kBlobOffsetMask = ((uint64_t)1 << 56) - 1;
+
+struct lfd_engine {
+    int32_t N = 0, H = 0, W = 0, P = 0, cls_channels = 0, dtype = 0, conv_impl = 0;
+    int64_t stats_off = 0, stats_bytes = 0, ws_bytes = 0;
+    int32_t soft = 0, soft_method = 0;
+    float soft_sigma = 0.f, soft_min_score = 0.f;
+    int32_t in_swap_rb = 0;                   // the plan's input transform, which op 0 carries
+    float in_mean[3] = {0.f, 0.f, 0.f}, in_scale[3] = {0.f, 0.f, 0.f};
+    lfd_post_cfg post{};
+    std::vector<lfd_op> ops;                  // as stored: pointer fields in the (blob, offset) encoding
+    std::vector<int32_t> src, level;
+    std::vector<uint8_t> blob[2];
+    // lfd_engine_bind
+    lfd_plan* plan = nullptr;
+    uint8_t *weights = nullptr, *ws = nullptr, *post_ws = nullptr;
+    std::vector<lfd_extent> ext;              // the geometry table of the last frame below the capacity
+    int meta_h = 0, meta_w = 0;               // the frame size the post-process workspace holds (0: none yet), written on meta_stream
+    cudaStream_t meta_stream = nullptr;
+    ~lfd_engine() { lfd_plan_destroy(plan); }
+};
+
+static size_t blob1_base(const lfd_engine* e) { return align256(e->blob[0].size()); }
+static size_t engine_weights_bytes(const lfd_engine* e) { return blob1_base(e) + align256(e->blob[1].size()); }
+// forward workspace: the plan's, then the engine's own cls and reg outputs
+static size_t engine_cls_off(const lfd_engine* e) { return align256((size_t)e->ws_bytes); }
+static size_t engine_reg_off(const lfd_engine* e) { return engine_cls_off(e) + align256((size_t)e->N * e->P * e->cls_channels * 4); }
+static size_t engine_ws_bytes(const lfd_engine* e) { return engine_reg_off(e) + align256((size_t)e->N * e->P * 16); }
+// post-process workspace: lfd_postprocess's, then img_w / img_h / resize_scale float[N] each, then src int32[N][cap]
+static size_t engine_meta_off(const lfd_engine* e) { return align256(post_layout(e->N, e->post.cap).total); }
+static size_t engine_src_off(const lfd_engine* e) { return engine_meta_off(e) + align256((size_t)e->N * 12); }
+static size_t engine_post_bytes(const lfd_engine* e) { return engine_src_off(e) + align256((size_t)e->N * e->post.cap * 4); }
+
+// CRC-32 (IEEE 802.3, reflected 0xEDB88320: zlib.crc32)
+struct Crc32Table {
+    uint32_t t[256];
+    Crc32Table() {
+        for (uint32_t i = 0; i < 256; ++i) {
+            uint32_t c = i;
+            for (int k = 0; k < 8; ++k) c = c & 1 ? 0xEDB88320u ^ (c >> 1) : c >> 1;
+            t[i] = c;
+        }
+    }
+};
+static uint32_t crc32_of(const uint8_t* p, size_t n) {
+    static const Crc32Table tab;   // initialised once, thread-safe (a function-local static)
+    const uint32_t* table = tab.t;
+    uint32_t c = 0xFFFFFFFFu;
+    for (size_t i = 0; i < n; ++i) c = table[(c ^ p[i]) & 0xFF] ^ (c >> 8);
+    return c ^ 0xFFFFFFFFu;
+}
+
+template <typename T> static T rd(const uint8_t* p) {
+    T v;
+    memcpy(&v, p, sizeof(T));
+    return v;
+}
+
+static int bad_file(const char* fmt, ...) {
+    char msg[400];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(msg, sizeof(msg), fmt, ap);
+    va_end(ap);
+    return fail(LFD_ERR_INVALID, "lfd_engine_open: %s", msg);
+}
+
+static bool in_range(int64_t v, int64_t lo, int64_t hi) { return v >= lo && v <= hi; }
+
+// a workspace range [off, off + bytes): off = -1 only where the op does not use it
+static int check_ws(int i, const char* field, int64_t off, int64_t bytes, bool used, int64_t ws_bytes) {
+    if (!used) return off == -1 ? LFD_OK : bad_file("op %d: %s = %lld on an op that does not use it (expected -1)", i, field, (long long)off);
+    if (off < 0 || off % 16 || bytes > ws_bytes || off > ws_bytes - bytes)
+        return bad_file("op %d: %s = %lld (+ %lld bytes) outside the workspace of workspace_bytes = %lld", i, field, (long long)off, (long long)bytes,
+                        (long long)ws_bytes);
+    return LFD_OK;
+}
+
+// a pointer field: 0 = NULL, else ((blob + 1) << 56) | offset, in the blob of its type, aligned to its element, with `bytes` inside the blob
+static int check_ptr(const lfd_engine* e, int i, const char* field, const void* p, int blob, int64_t bytes, bool used, bool required) {
+    const uint64_t v = (uint64_t)(uintptr_t)p;
+    if (v == 0) return used && required ? bad_file("op %d: %s is missing", i, field) : LFD_OK;
+    if (!used) return bad_file("op %d: %s is set on an op that does not read it", i, field);
+    const uint64_t tag = v >> 56, off = v & kBlobOffsetMask;
+    if (tag != (uint64_t)blob + 1) return bad_file("op %d: %s refers to blob %lld, expected blob %d", i, field, (long long)tag - 1, blob);
+    const uint64_t size = e->blob[blob].size(), align = blob == 0 ? 4 : 16;
+    if (off % align || (uint64_t)bytes > size || off > size - (uint64_t)bytes)
+        return bad_file("op %d: %s = blob %d offset %llu (+ %lld bytes) outside the blob of %llu bytes", i, field, blob, (unsigned long long)off,
+                        (long long)bytes, (unsigned long long)size);
+    return LFD_OK;
+}
+
+static int check_model_op(const lfd_engine* e, int i) {
+    const lfd_op& o = e->ops[i];
+    if (o.kind < LFD_OP_STEM0 || o.kind > LFD_OP_STEM4) return bad_file("op %d: unknown op kind %d", i, o.kind);
+    const bool image = o.kind == LFD_OP_STEM0 || o.kind == LFD_OP_STEM4;
+    if (image != (i == 0)) return bad_file("op %d: kind %d, but the image op (STEM0 / STEM4) is op 0 and only op 0", i, o.kind);
+    if (o.N != e->N) return bad_file("op %d: N = %d, the plan's is %d", i, o.N, e->N);
+    if (o.dtype != e->dtype) return bad_file("op %d: dtype %d, the plan's is %d", i, o.dtype, e->dtype);
+    // the image op reads the caller's frames: its geometry is the capacity lfd_engine_info reports and lfd_engine_detect checks against
+    if (image && (o.H != e->H || o.W != e->W))
+        return bad_file("op 0: the image op reads %dx%d frames, the plan's capacity H x W is %dx%d", o.H, o.W, e->H, e->W);
+    // the input transform that runs is op 0's: it is the plan's, and no other op carries one
+    const bool same_xf = image ? o.in_swap_rb == e->in_swap_rb && !memcmp(o.in_mean, e->in_mean, sizeof(o.in_mean)) &&
+                                     !memcmp(o.in_scale, e->in_scale, sizeof(o.in_scale))
+                               : o.in_swap_rb == 0 && !memcmp(o.in_mean, "\0\0\0\0\0\0\0\0\0\0\0\0", 12) &&
+                                     !memcmp(o.in_scale, "\0\0\0\0\0\0\0\0\0\0\0\0", 12);
+    if (!same_xf) return bad_file("op %d: input transform (in_swap_rb / in_mean / in_scale) %s", i, image ? "differs from the plan's" : "set on an op that does not read the image");
+    const int32_t dims[] = {o.H, o.W, o.Ho, o.Wo};
+    for (int32_t d : dims)
+        if (!in_range(d, 1, kModelMaxSide)) return bad_file("op %d: H / W / Ho / Wo = %d / %d / %d / %d outside [1, %d]", i, o.H, o.W, o.Ho, o.Wo, kModelMaxSide);
+    const int32_t chans[] = {o.Cin, o.Cout, o.tail_cout, o.ds_cout, o.gn_groups, o.n_cls, o.n_reg, o.cc, o.ksize, o.stride};
+    for (int32_t c : chans)
+        if (!in_range(c, 0, kModelMaxChannels))
+            return bad_file("op %d: a channel count, group count, ksize or stride is outside [0, %d] (Cin %d Cout %d)", i, kModelMaxChannels, o.Cin, o.Cout);
+    if (o.branch < 0 || o.branch >= LFD_MAX_BRANCHES || o.wait_mask < 0 || o.wait_mask >= (1 << LFD_MAX_BRANCHES))
+        return bad_file("op %d: branch %d / wait_mask 0x%x out of range", i, o.branch, o.wait_mask);
+    if (o.max_ctas < 0) return bad_file("op %d: max_ctas = %d", i, o.max_ctas);
+    if (o.point_off < 0) return bad_file("op %d: point_off = %d", i, o.point_off);
+    const int64_t N = o.N, in_px = N * o.H * o.W, out_px = N * o.Ho * o.Wo;
+    const int64_t cf = o.tail_cout ? o.tail_cout : o.Cout, stats = N * o.gn_groups * 16, wsb = e->ws_bytes;
+    const bool conv = o.kind == LFD_OP_CONV, gn = o.kind == LFD_OP_GN_APPLY, head = o.kind == LFD_OP_HEAD_FINAL;
+    int rc = LFD_OK;
+    if (!rc) rc = check_ws(i, "in_off", o.in_off, in_px * o.Cin * 2, conv || gn || head, wsb);
+    if (!rc) rc = check_ws(i, "out_off", o.out_off, (gn ? in_px * o.Cin : out_px * cf) * 2, !head, wsb);
+    if (!rc) rc = check_ws(i, "res_off", o.res_off, out_px * cf * 2, conv && o.res_off != -1, wsb);
+    if (!rc) rc = check_ws(i, "stats_off", o.stats_off, stats, o.gn_groups > 0, wsb);
+    if (!rc) rc = check_ws(i, "ds_out_off", o.ds_out_off, out_px * o.ds_cout * 2, o.ds_cout > 0, wsb);
+    const bool stem4 = o.kind == LFD_OP_STEM4, conv_like = conv || o.kind == LFD_OP_STEM0 || stem4;
+    const int64_t k2 = (int64_t)o.ksize * o.ksize, n_out = o.n_cls + o.n_reg;
+    const int64_t w_bytes = conv ? o.Cin * k2 * o.Cout * 2 : conv_like ? 96 * (int64_t)o.Cout : head ? n_out * o.Cin * 4 : 0;
+    if (!rc) rc = check_ptr(e, i, "weight", o.weight, head ? 0 : 1, w_bytes, conv_like || head, true);
+    if (!rc) rc = check_ptr(e, i, "scale", o.scale, 0, n_out * 4, head, true);
+    if (!rc) rc = check_ptr(e, i, "shift", o.shift, 0, (head ? n_out : o.Cout) * 4, conv_like || head, head);
+    if (!rc) rc = check_ptr(e, i, "gamma", o.gamma, 0, o.Cin * 4, gn || (head && o.gn_groups), true);
+    if (!rc) rc = check_ptr(e, i, "beta", o.beta, 0, o.Cin * 4, gn || (head && o.gn_groups), true);
+    if (!rc) rc = check_ptr(e, i, "tail_weight", o.tail_weight, 1, (int64_t)o.Cout * o.tail_cout * 2, conv_like && o.tail_cout, true);
+    if (!rc) rc = check_ptr(e, i, "tail_scale", o.tail_scale, 0, 0, false, false);
+    if (!rc) rc = check_ptr(e, i, "tail_shift", o.tail_shift, 0, (int64_t)o.tail_cout * 4, conv_like && o.tail_cout, false);
+    if (!rc) rc = check_ptr(e, i, "ds_weight", o.ds_weight, 1, (int64_t)o.Cin * o.ds_cout * 2, conv && o.ds_cout, true);
+    if (!rc) rc = check_ptr(e, i, "ds_shift", o.ds_shift, 0, (int64_t)o.ds_cout * 4, conv && o.ds_cout, false);
+    if (!rc) rc = check_ptr(e, i, "s2_weight", o.s2_weight, 1, 9 * 64 * 64 * 2, stem4, true);
+    if (!rc) rc = check_ptr(e, i, "s2_shift", o.s2_shift, 0, 64 * 4, stem4, false);
+    if (!rc) rc = check_ptr(e, i, "s3_weight", o.s3_weight, 1, 64 * 64 * 2, stem4, true);
+    if (!rc) rc = check_ptr(e, i, "s3_shift", o.s3_shift, 0, 64 * 4, stem4, false);
+    if (rc) return rc;
+    if (conv && ((o.ksize != 1 && o.ksize != 3) || (o.stride != 1 && o.stride != 2)))
+        return bad_file("op %d: conv ksize %d / stride %d (1 or 3 / 1 or 2)", i, o.ksize, o.stride);
+    if (check_op(o)) {   // the same geometry rules lfd_plan_create applies
+        char msg[sizeof(g_err)];
+        snprintf(msg, sizeof(msg), "%s", g_err);
+        return bad_file("op %d: %s", i, msg);
+    }
+    if (conv_like) {   // the wgmma kernel's configuration, as lfd_plan_create derives it (host only)
+        UmmaConvParams cp;
+        size_t smem = 0;
+        int grid = 0;
+        if (umma_conv_configure(geom_of(o), 132, &cp, &smem, &grid))
+            return bad_file("op %d: conv %dx%d s%d Cin=%d Cout=%d tail_cout=%d ds_cout=%d is not supported by the wgmma kernel", i, o.ksize, o.ksize,
+                            o.stride, o.Cin, o.Cout, o.tail_cout, o.ds_cout);
+        if (conv && cp.Cc != o.cc) return bad_file("op %d: cc = %d, the wgmma kernel packs this conv with cc = %d", i, o.cc, cp.Cc);
+    }
+    if (head && o.n_reg != 0 && o.n_reg != 4) return bad_file("op %d: n_reg = %d (0 or 4)", i, o.n_reg);
+    if (head && o.n_cls + o.n_reg == 0) return bad_file("op %d: a head op without outputs (n_cls = n_reg = 0)", i);
+    // the producer / level table: what lfd_engine_detect derives a smaller frame's geometry from
+    const int32_t s = e->src[i], l = e->level[i];
+    if (image ? s != -1 : (s < 0 || s >= i)) return bad_file("op %d: src_op = %d (the image op has -1, every other op an earlier op)", i, s);
+    if (!image) {   // the op reads one of its producer's outputs, of its size and channel count
+        const lfd_op& p = e->ops[s];
+        if (p.Ho != o.H || p.Wo != o.W) return bad_file("op %d: src_op = %d makes %dx%d, this op reads %dx%d", i, s, p.Ho, p.Wo, o.H, o.W);
+        const int32_t main_c = p.kind == LFD_OP_GN_APPLY ? p.Cin : (p.tail_cout ? p.tail_cout : p.Cout);
+        const int32_t c = o.in_off == p.out_off ? main_c : (p.ds_cout && o.in_off == p.ds_out_off) ? p.ds_cout : -1;
+        if (p.kind == LFD_OP_HEAD_FINAL || c < 0)
+            return bad_file("op %d: in_off = %lld is not an output of src_op = %d", i, (long long)o.in_off, s);
+        if (c != o.Cin) return bad_file("op %d: Cin = %d, but src_op = %d stores %d channels", i, o.Cin, s, c);
+    }
+    if (head ? !in_range(l, 0, e->post.num_levels - 1) : l != -1) return bad_file("op %d: level = %d (head ops: 0 .. num_levels - 1, others -1)", i, l);
+    if (head && (o.point_off != e->post.level_off[l] || o.W != e->post.level_w[l]))
+        return bad_file("op %d: head of level %d at point_off %d, width %d; the post-process has level_off %d, level_w %d", i, l, o.point_off, o.W,
+                        e->post.level_off[l], e->post.level_w[l]);
+    if (head && (int64_t)o.point_off + (int64_t)o.H * o.W > e->P) return bad_file("op %d: points [%d, %d + %dx%d) beyond P = %d", i, o.point_off, o.point_off, o.H, o.W, e->P);
+    if (head && (o.n_cls > e->cls_channels || (o.n_cls && o.n_cls != e->cls_channels))) return bad_file("op %d: n_cls = %d, cls_channels = %d", i, o.n_cls, e->cls_channels);
+    return LFD_OK;
+}
+
+static int parse_model(const uint8_t* b, size_t n, lfd_engine* e) {
+    if (n < kModelHeaderBytes) return bad_file("the file has %zu bytes, less than the %zu-byte header", n, kModelHeaderBytes);
+    if (memcmp(b, "LFDMODEL", 8)) return bad_file("magic: not an LFD model file");
+    const uint32_t version = rd<uint32_t>(b + 8), abi = rd<uint32_t>(b + 12);
+    if (version != LFD_MODEL_FORMAT_VERSION)
+        return fail(LFD_ERR_UNSUPPORTED, "lfd_engine_open: format version %u, this library reads version %d", version, LFD_MODEL_FORMAT_VERSION);
+    if (abi != LFD_B200_ABI_VERSION) return fail(LFD_ERR_UNSUPPORTED, "lfd_engine_open: abi version %u, this library is version %d", abi, LFD_B200_ABI_VERSION);
+    if (memcmp(b + 16, "sm_90a\0\0", 8)) return fail(LFD_ERR_UNSUPPORTED, "lfd_engine_open: target \"%.8s\", this library runs sm_90a", (const char*)(b + 16));
+    const uint32_t op_bytes = rd<uint32_t>(b + 24), post_bytes = rd<uint32_t>(b + 28);
+    if (op_bytes != sizeof(lfd_op)) return bad_file("lfd_op struct bytes %u, this library's lfd_op has %zu", op_bytes, sizeof(lfd_op));
+    if (post_bytes != sizeof(lfd_post_cfg)) return bad_file("lfd_post_cfg struct bytes %u, this library's lfd_post_cfg has %zu", post_bytes, sizeof(lfd_post_cfg));
+    const uint64_t payload = rd<uint64_t>(b + 32);
+    const uint32_t checksum = rd<uint32_t>(b + 40), reserved = rd<uint32_t>(b + 44);
+    if (reserved) return bad_file("reserved header word = %u (expected 0)", reserved);
+    if (payload != n - kModelHeaderBytes)
+        return bad_file("payload_bytes = %llu, but the file holds %zu bytes after the header (truncated or trailing bytes)", (unsigned long long)payload,
+                        n - kModelHeaderBytes);
+    const uint8_t* p = b + kModelHeaderBytes;
+    if (crc32_of(p, payload) != checksum) return bad_file("checksum: the payload's CRC-32 is 0x%08x, the header says 0x%08x", crc32_of(p, payload), checksum);
+    if (payload < kModelPlanBytes + sizeof(lfd_post_cfg)) return bad_file("payload_bytes = %llu, too short for the plan section", (unsigned long long)payload);
+    e->N = rd<int32_t>(p + 0); e->H = rd<int32_t>(p + 4); e->W = rd<int32_t>(p + 8); e->P = rd<int32_t>(p + 12);
+    e->cls_channels = rd<int32_t>(p + 16); e->dtype = rd<int32_t>(p + 20); e->conv_impl = rd<int32_t>(p + 24);
+    const int32_t n_ops = rd<int32_t>(p + 28);
+    e->stats_off = rd<int64_t>(p + 32); e->stats_bytes = rd<int64_t>(p + 40); e->ws_bytes = rd<int64_t>(p + 48);
+    const int32_t swap = rd<int32_t>(p + 56);
+    float* mean = e->in_mean;
+    float* scale = e->in_scale;
+    e->in_swap_rb = swap;
+    for (int c = 0; c < 3; ++c) { mean[c] = rd<float>(p + 60 + 4 * c); scale[c] = rd<float>(p + 72 + 4 * c); }
+    if (rd<int32_t>(p + 100) != 0) return bad_file("reserved plan word at byte 100 = %d (expected 0)", rd<int32_t>(p + 100));
+    e->soft = rd<int32_t>(p + 84); e->soft_method = rd<int32_t>(p + 88);
+    e->soft_sigma = rd<float>(p + 92); e->soft_min_score = rd<float>(p + 96);
+    const int64_t blob_bytes[2] = {rd<int64_t>(p + 104), rd<int64_t>(p + 112)};
+    memcpy(&e->post, p + kModelPlanBytes, sizeof(lfd_post_cfg));
+    if (n_ops < 1 || n_ops > kModelMaxOps) return bad_file("n_ops = %d outside [1, %d]", n_ops, kModelMaxOps);
+    if (!in_range(e->N, 1, kModelMaxN) || !in_range(e->H, 1, kModelMaxSide) || !in_range(e->W, 1, kModelMaxSide))
+        return bad_file("capacity N x H x W = %d x %d x %d outside [1, %d] x [1, %d] x [1, %d]", e->N, e->H, e->W, kModelMaxN, kModelMaxSide, kModelMaxSide);
+    if (!in_range(e->P, 1, (int64_t)e->H * e->W) || !in_range(e->cls_channels, 1, kModelMaxChannels))
+        return bad_file("P = %d / cls_channels = %d out of range", e->P, e->cls_channels);
+    if (e->dtype != LFD_DTYPE_BF16 && e->dtype != LFD_DTYPE_FP16) return bad_file("dtype = %d", e->dtype);
+    if (e->conv_impl != LFD_CONV_UMMA) return fail(LFD_ERR_UNSUPPORTED, "lfd_engine_open: conv_impl = %d, model files hold wgmma (LFD_CONV_UMMA) plans", e->conv_impl);
+    if (!in_range(e->ws_bytes, 256, kModelMaxWorkspace)) return bad_file("workspace_bytes = %lld outside [256, 2^40]", (long long)e->ws_bytes);
+    if (e->stats_off < 0 || e->stats_bytes < 0 || e->stats_bytes > e->ws_bytes || e->stats_off > e->ws_bytes - e->stats_bytes)
+        return bad_file("stats_off / stats_bytes = %lld / %lld outside the workspace", (long long)e->stats_off, (long long)e->stats_bytes);
+    InputTransform xf;
+    if (input_transform_of(swap, mean, scale, &xf)) return bad_file("input transform: %s", g_err);
+    if (e->soft != 0 && e->soft != 1) return bad_file("nms_type = %d (0 greedy, 1 soft_nms)", e->soft);
+    if (e->soft && ((e->soft_method != LFD_SOFT_NMS_LINEAR && e->soft_method != LFD_SOFT_NMS_GAUSSIAN) || !std::isfinite(e->soft_sigma) ||
+                    !std::isfinite(e->soft_min_score)))
+        return bad_file("soft_nms method %d / sigma %g / min_score %g", e->soft_method, (double)e->soft_sigma, (double)e->soft_min_score);
+    for (int b = 0; b < 2; ++b)
+        if (!in_range(blob_bytes[b], 0, kModelMaxBlob) || blob_bytes[b] % 16) return bad_file("blob %d bytes = %lld", b, (long long)blob_bytes[b]);
+    const lfd_post_cfg& c = e->post;
+    if (c.N != e->N || c.P != e->P || c.cls_channels != e->cls_channels)
+        return bad_file("post-process N / P / cls_channels = %d / %d / %d, the plan's are %d / %d / %d", c.N, c.P, c.cls_channels, e->N, e->P, e->cls_channels);
+    if (!in_range(c.C, 1, c.cls_channels) || (c.cls_mode == LFD_CLS_SIGMOID ? c.C != c.cls_channels : c.cls_mode == LFD_CLS_SOFTMAX ? c.C + 1 != c.cls_channels : true))
+        return bad_file("post-process C = %d / cls_mode = %d do not fit cls_channels = %d", c.C, c.cls_mode, c.cls_channels);
+    if (!in_range(c.bbox_mode, LFD_BBOX_SIGMOID, LFD_BBOX_INDEPENDENT) || (c.class_agnostic != 0 && c.class_agnostic != 1) || c.max_ctas != 0)
+        return bad_file("post-process bbox_mode %d / class_agnostic %d / max_ctas %d", c.bbox_mode, c.class_agnostic, c.max_ctas);
+    if (!in_range(c.num_levels, 1, LFD_MAX_LEVELS) || !in_range(c.cap, 1, kModelMaxCap)) return bad_file("post-process num_levels %d / cap %d", c.num_levels, c.cap);
+    if (!std::isfinite(c.score_thr) || !std::isfinite(c.iou_thr)) return bad_file("post-process score_thr %g / iou_thr %g", (double)c.score_thr, (double)c.iou_thr);
+    for (int l = 0; l < c.num_levels; ++l)
+        if (!in_range(c.level_stride[l], 1, 1 << 16) || !std::isfinite(c.level_hi[l])) return bad_file("post-process level %d: stride %d", l, c.level_stride[l]);
+    const size_t ops_at = kModelPlanBytes + sizeof(lfd_post_cfg), aux_at = ops_at + (size_t)n_ops * sizeof(lfd_op), blob_at = aux_at + (size_t)n_ops * 8;
+    if (payload != blob_at + (uint64_t)blob_bytes[0] + (uint64_t)blob_bytes[1])
+        return bad_file("payload_bytes = %llu, the sections need %llu (n_ops = %d, blob bytes %lld + %lld)", (unsigned long long)payload,
+                        (unsigned long long)(blob_at + blob_bytes[0] + blob_bytes[1]), n_ops, (long long)blob_bytes[0], (long long)blob_bytes[1]);
+    e->ops.resize(n_ops);
+    memcpy(e->ops.data(), p + ops_at, (size_t)n_ops * sizeof(lfd_op));
+    e->src.resize(n_ops);
+    e->level.resize(n_ops);
+    for (int i = 0; i < n_ops; ++i) { e->src[i] = rd<int32_t>(p + aux_at + 8 * i); e->level[i] = rd<int32_t>(p + aux_at + 8 * i + 4); }
+    e->blob[0].assign(p + blob_at, p + blob_at + blob_bytes[0]);
+    e->blob[1].assign(p + blob_at + blob_bytes[0], p + blob_at + blob_bytes[0] + blob_bytes[1]);
+    int64_t points = 0;
+    int heads = 0;
+    for (int i = 0; i < n_ops; ++i) {
+        const int rc = check_model_op(e, i);
+        if (rc) return rc;
+        if (e->ops[i].kind == LFD_OP_HEAD_FINAL && e->ops[i].n_reg) { points += (int64_t)e->ops[i].H * e->ops[i].W; ++heads; }
+    }
+    if (heads != c.num_levels || points != e->P) return bad_file("the head ops cover %d levels and %lld points, the plan has %d levels and P = %d", heads, (long long)points, c.num_levels, e->P);
+    return LFD_OK;
+}
+
+extern "C" int lfd_engine_open(const void* bytes, size_t n, lfd_engine** out) {
+    if (!bytes || !out) return fail(LFD_ERR_INVALID, "lfd_engine_open: null argument");
+    lfd_engine* e = new lfd_engine();
+    const int rc = parse_model(reinterpret_cast<const uint8_t*>(bytes), n, e);
+    if (rc) { delete e; return rc; }
+    *out = e;
+    return LFD_OK;
+}
+
+extern "C" int lfd_engine_close(lfd_engine* engine) {
+    delete engine;
+    return LFD_OK;
+}
+
+extern "C" int lfd_engine_info(const lfd_engine* e, lfd_engine_desc* out) {
+    if (!e || !out) return fail(LFD_ERR_INVALID, "lfd_engine_info: null argument");
+    lfd_engine_desc d{};
+    d.N = e->N; d.H = e->H; d.W = e->W; d.P = e->P; d.cls_channels = e->cls_channels; d.num_classes = e->post.C; d.dtype = e->dtype;
+    d.n_ops = (int32_t)e->ops.size(); d.cap = e->post.cap; d.soft_nms = e->soft;
+    d.weights_bytes = (int64_t)engine_weights_bytes(e);
+    d.workspace_bytes = (int64_t)engine_ws_bytes(e);
+    d.post_workspace_bytes = (int64_t)engine_post_bytes(e);
+    *out = d;
+    return LFD_OK;
+}
+
+extern "C" int lfd_engine_op(const lfd_engine* e, int i, lfd_op* op, int32_t* src_op, int32_t* level) {
+    if (!e || !op || i < 0 || i >= (int)e->ops.size()) return fail(LFD_ERR_INVALID, "lfd_engine_op: bad arguments (op %d)", i);
+    *op = e->ops[i];
+    if (src_op) *src_op = e->src[i];
+    if (level) *level = e->level[i];
+    return LFD_OK;
+}
+
+extern "C" int lfd_engine_num_launches(const lfd_engine* e) { return e ? lfd_plan_num_launches(e->plan) : 0; }
+
+extern "C" int lfd_engine_bind(lfd_engine* e, void* weights, size_t weights_bytes, void* workspace, size_t workspace_bytes, void* post_workspace,
+                               size_t post_workspace_bytes, lfd_stream stream) {
+    if (!e || !weights || !workspace || !post_workspace) return fail(LFD_ERR_INVALID, "lfd_engine_bind: null argument");
+    if (weights_bytes < engine_weights_bytes(e) || workspace_bytes < engine_ws_bytes(e) || post_workspace_bytes < engine_post_bytes(e))
+        return fail(LFD_ERR_CAPACITY, "lfd_engine_bind: buffers of %zu / %zu / %zu bytes, the model needs weights %zu, workspace %zu, post workspace %zu",
+                    weights_bytes, workspace_bytes, post_workspace_bytes, engine_weights_bytes(e), engine_ws_bytes(e), engine_post_bytes(e));
+    if (((uintptr_t)weights | (uintptr_t)workspace | (uintptr_t)post_workspace) & 255)
+        return fail(LFD_ERR_INVALID, "lfd_engine_bind: weights %p / workspace %p / post workspace %p must be 256-byte aligned (as cudaMalloc returns)",
+                    weights, workspace, post_workspace);
+    if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_engine_bind: no CUDA device (there is no CPU fallback)");
+    uint8_t* wb = reinterpret_cast<uint8_t*>(weights);
+    const uint8_t* base[2] = {wb, wb + blob1_base(e)};
+    std::vector<lfd_op> ops = e->ops;
+    for (auto& o : ops) {
+        const void** fields[] = {&o.weight, (const void**)&o.scale, (const void**)&o.shift, (const void**)&o.gamma, (const void**)&o.beta,
+                                 &o.tail_weight, (const void**)&o.tail_scale, (const void**)&o.tail_shift, &o.ds_weight, (const void**)&o.ds_shift,
+                                 &o.s2_weight, (const void**)&o.s2_shift, &o.s3_weight, (const void**)&o.s3_shift};
+        for (const void** f : fields) {
+            const uint64_t v = (uint64_t)(uintptr_t)*f;
+            if (v) *f = base[(v >> 56) - 1] + (v & kBlobOffsetMask);
+        }
+    }
+    lfd_plan* plan = nullptr;
+    int rc = lfd_plan_create(ops.data(), (int)ops.size(), e->N, e->P, e->cls_channels, e->stats_off, e->stats_bytes, e->ws_bytes, e->conv_impl, &plan);
+    if (rc) return rc;
+    cudaStream_t st = st_of(stream);
+    for (int b = 0; b < 2; ++b) {
+        cudaError_t ce = e->blob[b].empty() ? cudaSuccess : cudaMemcpyAsync(const_cast<uint8_t*>(base[b]), e->blob[b].data(), e->blob[b].size(),
+                                                                            cudaMemcpyHostToDevice, st);
+        if (ce != cudaSuccess) { lfd_plan_destroy(plan); return fail(LFD_ERR_CUDA, "lfd_engine_bind: weight copy: %s", cudaGetErrorString(ce)); }
+    }
+    lfd_plan_destroy(e->plan);
+    e->plan = plan;
+    e->weights = wb;
+    e->ws = reinterpret_cast<uint8_t*>(workspace);
+    e->post_ws = reinterpret_cast<uint8_t*>(post_workspace);
+    e->meta_h = e->meta_w = 0;
+    return LFD_OK;
+}
+
+// cuMemsetD32Async: the post-process's per-image width / height / scale, as 32-bit patterns, without a host buffer
+typedef int (*MemsetD32Fn)(unsigned long long, unsigned int, size_t, cudaStream_t);
+static MemsetD32Fn memset_d32_fn() {
+    static const MemsetD32Fn fn = []() -> MemsetD32Fn {   // looked up once, thread-safe (a function-local static)
+        void* ptr = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        if (cudaGetDriverEntryPoint("cuMemsetD32Async", &ptr, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
+            return reinterpret_cast<MemsetD32Fn>(ptr);
+        return nullptr;
+    }();
+    return fn;
+}
+
+static int fill_f32(float* dst, float v, size_t n, cudaStream_t st) {
+    MemsetD32Fn fn = memset_d32_fn();
+    if (!fn) return fail(LFD_ERR_CUDA, "lfd_engine_detect: cuMemsetD32Async is not available");
+    unsigned int bits;
+    memcpy(&bits, &v, 4);
+    if (fn((unsigned long long)(uintptr_t)dst, bits, n, st) != 0) return fail(LFD_ERR_CUDA, "lfd_engine_detect: cuMemsetD32Async failed");
+    return LFD_OK;
+}
+
+extern "C" int lfd_engine_detect(lfd_engine* e, const void* input, int input_format, int h, int w, float* dets, int32_t* labels, int32_t* count,
+                                 float* cls_out, float* reg_out, int use_graph, lfd_stream stream) {
+    if (!e || !input || !dets || !labels || !count) return fail(LFD_ERR_INVALID, "lfd_engine_detect: null argument");
+    if (!e->plan) return fail(LFD_ERR_INVALID, "lfd_engine_detect: the engine is not bound (lfd_engine_bind)");
+    if (h < 1 || w < 1 || h > e->H || w > e->W) return fail(LFD_ERR_INVALID, "lfd_engine_detect: frame %dx%d outside the capacity %dx%d", h, w, e->H, e->W);
+    int rc = check_input_format("lfd_engine_detect", input_format, &e->ops[0], h, w);
+    if (rc) return rc;
+    const int n_ops = (int)e->ops.size();
+    // the frame's geometry: every op's extent follows from its producer's, as a plan built for h x w has it (lfd/_engine.py extent_table)
+    e->ext.assign(n_ops, lfd_extent{});
+    int level_h[LFD_MAX_LEVELS] = {0}, level_w[LFD_MAX_LEVELS] = {0};
+    for (int i = 0; i < n_ops; ++i) {
+        const lfd_op& o = e->ops[i];
+        lfd_extent& x = e->ext[i];
+        x.H = i == 0 ? h : e->ext[e->src[i]].Ho;
+        x.W = i == 0 ? w : e->ext[e->src[i]].Wo;
+        x.Ho = x.H; x.Wo = x.W;
+        if (o.kind == LFD_OP_STEM0 || o.kind == LFD_OP_CONV) {
+            x.Ho = (x.H + 2 * (o.ksize / 2) - o.ksize) / o.stride + 1;
+            x.Wo = (x.W + 2 * (o.ksize / 2) - o.ksize) / o.stride + 1;
+        } else if (o.kind == LFD_OP_STEM4) {
+            x.Ho = ((x.H - 1) / 2) / 2 + 1;
+            x.Wo = ((x.W - 1) / 2) / 2 + 1;
+        }
+        if (o.kind == LFD_OP_HEAD_FINAL) { level_h[e->level[i]] = x.H; level_w[e->level[i]] = x.W; }
+    }
+    lfd_post_cfg cfg = e->post;
+    int P = 0;
+    for (int l = 0; l < cfg.num_levels; ++l) {
+        cfg.level_off[l] = P;
+        cfg.level_w[l] = level_w[l];
+        P += level_h[l] * level_w[l];
+    }
+    cfg.P = P;
+    for (int i = 0; i < n_ops; ++i)
+        if (e->ops[i].kind == LFD_OP_HEAD_FINAL) { e->ext[i].point_off = cfg.level_off[e->level[i]]; e->ext[i].P = P; }
+    float* cls = cls_out ? cls_out : reinterpret_cast<float*>(e->ws + engine_cls_off(e));
+    float* reg = reg_out ? reg_out : reinterpret_cast<float*>(e->ws + engine_reg_off(e));
+    cudaStream_t st = st_of(stream);
+    rc = lfd_plan_forward_extent(e->plan, input, input_format, h, w, e->ext.data(), e->ws, cls, reg, use_graph, stream);
+    if (rc) return rc;
+    float* meta = reinterpret_cast<float*>(e->post_ws + engine_meta_off(e));
+    const size_t N = (size_t)e->N;
+    // written once per frame size and stream: the post-process workspace is the engine's alone, and a call on another stream writes it
+    // again so that its post-process is ordered after the values it reads
+    if (h != e->meta_h || w != e->meta_w || st != e->meta_stream) {
+        e->meta_h = e->meta_w = 0;
+        if ((rc = fill_f32(meta, (float)w, N, st)) || (rc = fill_f32(meta + N, (float)h, N, st)) || (rc = fill_f32(meta + 2 * N, 1.0f, N, st))) return rc;
+        e->meta_h = h;
+        e->meta_w = w;
+        e->meta_stream = st;
+    }
+    int32_t* src = reinterpret_cast<int32_t*>(e->post_ws + engine_src_off(e));
+    if (e->soft)
+        return lfd_postprocess_soft_nms(&cfg, cls, reg, meta, meta + N, meta + 2 * N, e->post_ws, dets, labels, src, count, count + N, e->soft_method,
+                                        e->soft_sigma, e->soft_min_score, stream);
+    return lfd_postprocess(&cfg, cls, reg, meta, meta + N, meta + 2 * N, e->post_ws, dets, labels, src, count, count + N, stream);
 }

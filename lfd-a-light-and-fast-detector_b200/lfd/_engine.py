@@ -16,7 +16,9 @@ Rounding points of the bf16 pipeline (mirrored by oracle/lfd_oracle.py forward(e
       to bf16 again; the final cls / reg outputs are fp32.
 """
 import ctypes as C
+import struct
 import time
+import zlib
 
 import torch
 import torch.nn as nn
@@ -156,6 +158,11 @@ def pack_stem_weight(weight, dtype=torch.bfloat16):
 
 
 _AUX_BRANCH = 7      # graph branch of the residual blocks' shortcut convs (LFD_MAX_BRANCHES - 1)
+
+# model files (include/lfd_b200.h): a pointer field of an op record holds ((blob + 1) << 56) | byte offset, blob 0 = fp32, 1 = 16-bit
+MODEL_MAGIC = b'LFDMODEL'
+MODEL_FORMAT_VERSION = 1
+MODEL_BLOB_F32, MODEL_BLOB_16 = 1 << 56, 2 << 56
 
 
 class _Arena(object):
@@ -472,6 +479,7 @@ class InferencePlan(object):
         bb, neck, head = model._backbone, model._neck, model._head
         cur, h, w = self._emit_stem(bb.stem_layers(), self.H, self.W)
         self.level_sizes, self.P, offs = level_geometry(bb, head, h, w)
+        self.level_offsets = offs
         taps = list(bb._out_indices)
         if make_norm_probe(head) is not None and not isinstance(make_norm_probe(head), nn.GroupNorm):
             raise NotImplementedError('the H100 head kernels implement GroupNorm towers and towers without norm layers (the shipped configs)')
@@ -843,6 +851,48 @@ class InferencePlan(object):
                              ksize=op.get('ksize', 1), stride=op.get('stride', 1), res=op.get('res') is not None, tail_cout=op.get('tail_cout', 0), ds_cout=op.get('ds_cout', 0),
                              out=op.get('out'), query=op.get('query'), fused_stem=4 if op['kind'] == nat.OP_STEM4 else 0))
         return rows
+
+    def export(self, path, post):
+        """Writes this plan and the post-process `post` (a PostPlan for N images of this plan's level geometry) to the model file `path`
+        (include/lfd_b200.h "model files", DESIGN.md "Model files"), which lfd_engine_open reads without Python or torch.  The ops are
+        the records this plan hands to lfd_plan_create, with the current CTA bounds (autotune), their pointers as (blob, offset) into the
+        two staging buffers.  The same plan gives the same bytes.  -> the file's size."""
+        data = self.model_file_bytes(post)
+        with open(path, 'wb') as f:
+            f.write(data)
+        return len(data)
+
+    def model_file_bytes(self, post):
+        """The bytes export writes."""
+        if self.conv_impl != nat.CONV_UMMA:
+            raise ValueError('model files hold wgmma plans (conv_impl=CONV_UMMA), not the SIMT cross-check')
+        c = post.cfg
+        if (c.N, c.P, c.cls_channels, c.num_levels) != (self.N, self.P, self.cls_channels, len(self.level_sizes)) or \
+                [(c.level_off[l], c.level_w[l]) for l in range(c.num_levels)] != [(self.level_offsets[l], s[1]) for l, s in enumerate(self.level_sizes)]:
+            raise ValueError('the post-process was not made for this plan (N, P, cls_channels or level geometry differ)')
+        producer = {}
+        records, aux = [], []
+        for i, op in enumerate(self._ops):
+            o = nat.Op()
+            self._fill_op(o, op, self.offsets, MODEL_BLOB_F32, MODEL_BLOB_16, self.N * 16 * 2 * 8)
+            o.max_ctas = self._op_array[i].max_ctas         # the autotuned CTA bounds live in the op array
+            records.append(C.string_at(C.addressof(o), C.sizeof(o)))
+            aux.append(struct.pack('<ii', producer[op['inp']] if op.get('inp') is not None else -1,
+                                   op['level'] if op['kind'] == nat.OP_HEAD_FINAL else -1))
+            for k in ('out', 'out2'):
+                if op.get(k) is not None:
+                    producer[op[k]] = i
+        blob_f32 = self.params_f32.detach().cpu().contiguous().numpy().tobytes()
+        blob_16 = self.params_bf16.detach().cpu().contiguous().numpy().tobytes()
+        xf = self.input_transform
+        swap, mean, scale = (0, (0.0,) * 3, (0.0,) * 3) if xf is None else (int(xf.swap_rb), tuple(xf.mean), tuple(xf.scale))
+        soft = (1,) + tuple(post.soft) if post.soft is not None else (0, 0, 0.0, 0.0)
+        plan = struct.pack('<8i3qi3f3f2i2fi2q', self.N, self.H, self.W, self.P, self.cls_channels, self.dtype_code, self.conv_impl, len(records),
+                           0, self.stats_bytes, self.workspace_bytes, swap, *mean, *scale, *soft, 0, len(blob_f32), len(blob_16))
+        payload = b''.join([plan, C.string_at(C.addressof(c), C.sizeof(c))] + records + aux + [blob_f32, blob_16])
+        header = MODEL_MAGIC + struct.pack('<II8sIIQII', MODEL_FORMAT_VERSION, nat.ABI_VERSION, b'sm_90a', C.sizeof(nat.Op), C.sizeof(nat.PostCfg),
+                                           len(payload), zlib.crc32(payload), 0)
+        return header + payload
 
     def __del__(self):
         try:

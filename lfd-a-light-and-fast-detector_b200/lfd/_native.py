@@ -12,6 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _PKG = os.path.dirname(_HERE)
 LIB_PATH = os.environ.get('LFD_B200_LIB') or os.path.join(_PKG, 'liblfd_b200.so')   # LFD_B200_LIB: an alternative build of the SAME library (tuning experiments)
 MAX_LEVELS = 8
+ABI_VERSION = 5           # LFD_B200_ABI_VERSION
 
 OP_STEM0, OP_CONV, OP_GN_APPLY, OP_HEAD_FINAL, OP_STEM4 = 0, 1, 2, 3, 4
 INPUT_F32_NCHW, INPUT_U8_NHWC, INPUT_U8_NV12 = 0, 1, 2     # NV12: inference only, uint8 [N, 3H/2, W] (include/lfd_b200.h)
@@ -121,6 +122,13 @@ class Extent(C.Structure):
                 ('pad_', C.c_int32 * 2)]
 
 
+class EngineDesc(C.Structure):
+    """lfd_engine_desc: what a model file needs (lfd_engine_info)."""
+    _fields_ = [('N', C.c_int32), ('H', C.c_int32), ('W', C.c_int32), ('P', C.c_int32), ('cls_channels', C.c_int32),
+                ('num_classes', C.c_int32), ('dtype', C.c_int32), ('n_ops', C.c_int32), ('cap', C.c_int32), ('soft_nms', C.c_int32),
+                ('weights_bytes', C.c_int64), ('workspace_bytes', C.c_int64), ('post_workspace_bytes', C.c_int64)]
+
+
 class PackDesc(C.Structure):
     _fields_ = [('kind', C.c_int32), ('Cout', C.c_int32), ('Cin', C.c_int32), ('k', C.c_int32), ('cc', C.c_int32), ('n', C.c_int32),
                 ('src', C.c_void_p), ('src2', C.c_void_p), ('dst', C.c_void_p), ('dst2', C.c_void_p), ('dst3', C.c_void_p)]
@@ -177,6 +185,13 @@ SYMBOLS = {
     'lfd_grad_sqnorm': (_i, [_vp, _i64, _vp, _vp]),
     'lfd_sgd_step': (_i, [_vp, _vp, _vp, _i64, _f, _f, _f, _f, _i, _f, _f, _vp, _vp]),
     'lfd_input_batch': (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, C.POINTER(_f), C.POINTER(_f), _vp]),
+    'lfd_engine_open': (_i, [_vp, C.c_size_t, C.POINTER(_vp)]),
+    'lfd_engine_close': (_i, [_vp]),
+    'lfd_engine_info': (_i, [_vp, C.POINTER(EngineDesc)]),
+    'lfd_engine_op': (_i, [_vp, _i, C.POINTER(Op), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    'lfd_engine_bind': (_i, [_vp, _vp, C.c_size_t, _vp, C.c_size_t, _vp, C.c_size_t, _vp]),
+    'lfd_engine_detect': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
+    'lfd_engine_num_launches': (_i, [_vp]),
 }
 
 _lib = None
@@ -206,9 +221,9 @@ def lib():
         fn = getattr(L, name)
         fn.restype = res
         fn.argtypes = args
-    if L.lfd_abi_version() != 5:
+    if L.lfd_abi_version() != ABI_VERSION:
         raise LfdError('liblfd_b200.so ABI version mismatch')
-    for which, st in enumerate((Op, Top, PackDesc, UnpackDesc, PostCfg, LossCfg, Levels, InputDesc, Extent)):
+    for which, st in enumerate((Op, Top, PackDesc, UnpackDesc, PostCfg, LossCfg, Levels, InputDesc, Extent, EngineDesc)):
         if L.lfd_struct_bytes(which) != C.sizeof(st):
             raise LfdError('liblfd_b200.so: %s is %d bytes in the library, %d in lfd/_native.py' % (st.__name__, L.lfd_struct_bytes(which), C.sizeof(st)))
     _lib = L
