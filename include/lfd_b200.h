@@ -175,6 +175,10 @@ typedef struct lfd_op {
  * cc = input-channel chunk the weights must be packed with. */
 int lfd_conv_query(int N, int H, int W, int Cin, int Ho, int Wo, int Cout, int ksize, int stride, int tail_cout, int ds_cout, int* cc,
                    int* stages, int* weights_resident, int* num_tiles, int64_t* smem_bytes);
+/* The consumer schedule the wgmma kernel runs for that conv on this device (host only): *solo = 1 when each of its two consumer
+ * warpgroups computes whole tiles and the two alternate on the tensor cores (64 -> 64 channel 3x3/s1 convs without tail with at least
+ * two tiles per CTA), 0 when both work on every tile. */
+int lfd_conv_schedule(int N, int H, int W, int Cin, int Ho, int Wo, int Cout, int ksize, int stride, int tail_cout, int ds_cout, int* solo);
 /* The same for a STEM4 op on N images of H x W (host only): its tiles (16 x 8 stem3 pixels each), dynamic shared memory per CTA
  * and stem3 output size. */
 int lfd_stem4_query(int N, int H, int W, int* num_tiles, int64_t* smem_bytes, int* Ho, int* Wo);

@@ -31,9 +31,10 @@ def _stale(out, deps):
 
 
 # kernels whose per-thread state must stay in registers (the soft-NMS kernel runs one iteration per candidate: a spill is paid K times)
-_STACK_GUARDED = ('conv_umma_kernel', 'conv_umma_c48_kernel', 'stem4_kernel', 'soft_nms_kernel')
+# (kernel names are matched by substring: conv_umma_solo_kernel is not covered by conv_umma_kernel and is listed on its own)
+_STACK_GUARDED = ('conv_umma_kernel', 'conv_umma_c48_kernel', 'conv_umma_solo_kernel', 'stem4_kernel', 'soft_nms_kernel')
 # kernels whose wgmmas must be pipelined: every instantiation, no exemptions
-_WGMMA_GUARDED = ('conv_umma_kernel', 'conv_umma_c48_kernel', 'stem4_kernel')
+_WGMMA_GUARDED = ('conv_umma_kernel', 'conv_umma_c48_kernel', 'conv_umma_solo_kernel', 'stem4_kernel')
 _PTXAS_VERBOSE = ('conv_umma.cu', 'postprocess.cu')
 
 

@@ -290,6 +290,18 @@ extern "C" int lfd_conv_query(int N, int H, int W, int Cin, int Ho, int Wo, int 
     return LFD_OK;
 }
 
+extern "C" int lfd_conv_schedule(int N, int H, int W, int Cin, int Ho, int Wo, int Cout, int ksize, int stride, int tail_cout, int ds_cout,
+                                 int* solo) {
+    ConvGeom g = {N, H, W, Cin, Ho, Wo, Cout, ksize, stride, tail_cout, ds_cout, 0};
+    UmmaConvParams p;
+    size_t smem = 0;
+    int grid = 0;
+    int rc = umma_conv_configure(g, sm_count() > 0 ? sm_count() : 132, &p, &smem, &grid);
+    if (rc) return fail(LFD_ERR_UNSUPPORTED, "conv %dx%d s%d Cin=%d Cout=%d not supported by the wgmma kernel (rc=%d)", ksize, ksize, stride, Cin, Cout, rc);
+    if (solo) *solo = p.solo;
+    return LFD_OK;
+}
+
 extern "C" int lfd_stem4_query(int N, int H, int W, int* num_tiles, int64_t* smem_bytes, int* Ho, int* Wo) {
     const int h1 = (H - 1) / 2 + 1, w1 = (W - 1) / 2 + 1;
     ConvGeom g = {N, H, W, 3, (h1 - 1) / 2 + 1, (w1 - 1) / 2 + 1, 64, 3, 2, 64, 0, 0, 1};

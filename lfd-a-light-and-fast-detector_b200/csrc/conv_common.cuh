@@ -45,6 +45,7 @@ struct alignas(64) UmmaConvParams {
     CUtensorMap tm_res;         // TMA descriptor of the residual tensor (same geometry)
     CUtensorMap tm_out3;        // TMA descriptor of the fused shortcut conv's output (same geometry)
     int stg_nbuf;               // staging buffers per warpgroup (2: the store of tile t overlaps the conversion of tile t+1)
+    int solo;                   // 1: conv_umma_solo_kernel (one consumer warpgroup per tile, see umma_conv_configure)
     const __nv_bfloat16* in;
     __nv_bfloat16* out;
     const void* in_raw;         // MODE_STEM: the image, fp32 NCHW (input_format 0) or uint8 NHWC (1)

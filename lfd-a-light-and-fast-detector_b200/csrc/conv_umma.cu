@@ -54,7 +54,8 @@ static constexpr int kConvThreads = kConsumerThreads + kProdThreads;
 // Buffer [4 roles][32 entries][4 slots]:
 //   role 0        producer, per stage                : wait_empty  got_empty  issued  arrived_full (stem: next tile's fetch issued)
 //   role 1 + wg   consumer warpgroup wg, per tile    : wait_full  got_full (last chunk)  main_mma_done  tail_mma_done
-//   role 3        epilogues, entry 2 * store + wg    : store_entry  after_bulk_wait_read  tma_issued  -
+//   role 3        epilogues, entry 2 * store + wg    : store_entry  after_bulk_wait_read  tma_issued  residual_landed (after the shift loads
+//                                                    and the warpgroup barrier; without a residual, after the barrier)
 // Only thread 0 of each role stamps.
 #ifdef LFD_B200_TRACE
 #define LFD_TRACE(role, idx, slot) \
@@ -247,6 +248,7 @@ LFD_DEVINL void store_tile(const EpiCtx& e, const float* acc, int nc, const floa
     load_shifts(0);
     wg_bar_sync(e.wg);
     if (res) { mbar_wait(res_bar, res_count & 1); ++res_count; }
+    if (e.wtid == 0) LFD_TRACE_EPI(e.tr, tidx, 3);
     float st[NCMAX == 128 ? 32 : 1];
     const bool stat = NCMAX == 128 && stats != nullptr;
 #pragma unroll
@@ -290,12 +292,140 @@ LFD_DEVINL void store_tile(const EpiCtx& e, const float* acc, int nc, const floa
     if (NCMAX == 128 && stat) stats_flush<128>(st, e.lane, stats);
 }
 
+// The consumers of conv_umma_solo_kernel: MODE_3X3S1, 64 -> 64 channels, resident weights, Cc = 64 (one ring stage per tile), no tail,
+// shortcut or statistics.  Consumer warpgroup wg takes the tiles lt = wg, wg + 2, ... of the CTA's sequence and computes all 128 rows
+// of each as two m64n64 blocks that share every B descriptor (64 fp32 accumulators per thread), in the k16-outer / tap-inner order of
+// conv_umma_body, so every output gets the same sums.  The two warpgroups take turns on the tensor pipe: a warpgroup waits on
+// turn[wg] before its first wgmma of a tile and arrives on the other's turn barrier once its MMAs have been waited for, so its epilogue
+// runs under the other warpgroup's MMAs.  Warpgroup 0 starts; the alternation follows the tile order, so it never waits for a tile the
+// other warpgroup does not have.  The residual rows of a tile are requested at the start of the tile and land under its MMAs.  Each
+// warpgroup stages its tile in its own 16 KB region ([box: rows 0-63 | 64-127][64 rows x 128 B], SWIZZLE_128B) and stores it as two
+// TMA boxes.
+// Trace (LFD_B200_TRACE): role 1 + wg per tile of the warpgroup (k = 0, 1, ...): wait_full  got_full  main_mma_done  got_turn;
+// role 3 entry 2 k + wg: epilogue entry  -  tma_issued  residual_landed (after the shift loads and the warpgroup barrier).
+template <bool F16, bool EXT>
+LFD_DEVINL void solo_consumers(const UmmaConvParams& p, const LaunchGrid& lg, uint64_t* full, uint64_t* empty, uint64_t* wbar,
+                               uint64_t* res_bar, uint64_t* turn, const float* bias, uint8_t* staging, uint8_t* wres, uint8_t* ring) {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int wg = warp >> 2, wtid = tid & 127;
+    if (tid == 0) {
+        mbar_arrive_expect_tx(wbar, p.w_total_bytes);
+        for (uint32_t off = 0; off < p.w_total_bytes; off += 32768) {
+            const uint32_t nb = p.w_total_bytes - off < 32768 ? p.w_total_bytes - off : 32768;
+            bulk_g2s(smem_u32(wres) + off, reinterpret_cast<const uint8_t*>(p.w) + off, nb, wbar);
+        }
+    }
+    pdl_wait();                                   // residual reads and output stores depend on upstream kernels
+    mbar_wait(wbar, 0);
+
+    constexpr uint32_t kBox = 64u * 64u * 2u;     // one 64-row box of 64 channels
+    const uint32_t stg = smem_u32(staging) + (uint32_t)wg * 2u * kBox;
+    if (wtid == 0 && (stg & 1023u)) __trap();    // swizzle atoms need 1024-byte aligned staging regions
+    const int r0 = (warp & 3) * 16 + (lane >> 2), tq = lane & 3;
+    const uint64_t adesc0 = wgmma_desc(0, p.lbo_a, p.sbo_a);
+    const uint64_t bd = wgmma_desc(0, 64 * 16, 128) + (smem_u32(wres) >> 4);
+    const uint32_t a_k16 = (2 * p.lbo_a) >> 4, b_k16 = (2 * 64 * 16) >> 4, b_tap = (8 * 64 * 16) >> 4;
+    const uint32_t a_blk = (8u * p.sbo_a) >> 4;  // rows 64..127 start 8 core-matrix rows further down
+    const bool has_res = p.res != nullptr, relu = p.relu != 0;
+#ifdef LFD_B200_TRACE
+    long long* tr = p.trace && wtid == 0 ? p.trace + (3 * 32 + wg) * 4 : nullptr;
+#endif
+
+    float acc0[32], acc1[32];
+    uint32_t k = 0;                               // tiles of this warpgroup so far
+    for (int lt = wg, tile = blockIdx.x + wg * gridDim.x; tile < lg.num_tiles; lt += 2, tile += 2 * gridDim.x, ++k) {
+        const int n = fast_div(tile, lg.magic_tpi), t = tile - n * lg.tiles_per_img;
+        const int ty = fast_div(t, lg.magic_tx);
+        const int c0 = (t - ty * lg.tiles_x) * 8, c1 = ty * 16;
+        if (wtid == 0) {
+            bulk_wait_read<0>();                  // the previous tile's stores have read the staging region
+            if (has_res) {
+                mbar_arrive_expect_tx(&res_bar[wg], 2u * kBox);
+                tma_load_4d(stg, &p.tm_res, 0, c0, c1, n, &res_bar[wg]);
+                tma_load_4d(stg + kBox, &p.tm_res, 0, c0, c1 + 8, n, &res_bar[wg]);
+            }
+            LFD_TRACE(1 + wg, k, 0);
+        }
+        const uint32_t s = (uint32_t)lt % p.stages, ph = ((uint32_t)lt / p.stages) & 1;
+        mbar_wait(&full[s], ph);
+        if (wtid == 0) LFD_TRACE(1 + wg, k, 1);
+        if (lt > 0) mbar_wait(&turn[wg], (k - (wg == 0 ? 1u : 0u)) & 1);
+        if (wtid == 0) LFD_TRACE(1 + wg, k, 3);
+        fence_proxy_async_smem();   // cp.async (generic proxy) writes -> wgmma (async proxy) reads
+        const uint64_t ad = adesc0 + ((smem_u32(ring) + s * p.stage_bytes) >> 4);
+        wgmma_fence_regs<32>(acc0);
+        wgmma_fence_regs<32>(acc1);
+        wgmma_fence();
+#pragma unroll
+        for (int k16 = 0; k16 < 4; ++k16) {
+            const uint64_t adk = ad + (uint32_t)(k16 * a_k16), bdk = bd + (uint32_t)(k16 * b_k16);
+#pragma unroll
+            for (int tap = 0; tap < 9; ++tap) {
+                const uint64_t b = bdk + (uint32_t)(tap * b_tap);
+                wgmma_ss<64, F16>(acc0, adk + (uint32_t)tap_view<MODE_3X3S1>(tap), b, (k16 | tap) != 0);
+                wgmma_ss<64, F16>(acc1, adk + a_blk + (uint32_t)tap_view<MODE_3X3S1>(tap), b, (k16 | tap) != 0);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs<32>(acc0);
+        wgmma_fence_regs<32>(acc1);
+        __syncwarp();
+        if (lane == 0) {
+            mbar_arrive(&empty[s]);               // this warp's part of the stage has been consumed
+            mbar_arrive(&turn[wg ^ 1]);           // the tensor pipe is the other warpgroup's
+        }
+        if (wtid == 0) LFD_TRACE(1 + wg, k, 2);
+
+        // ---- epilogue: (+shift) (+residual) (+ReLU) -> 16-bit staging rows -> two TMA stores
+        if (wtid == 0) LFD_TRACE_EPI(tr, k, 0);
+        float2 bv[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) bv[j] = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * tq);
+        wg_bar_sync(wg);                          // orders thread 0's wait for the staging region before every thread's stores
+        if (has_res) mbar_wait(&res_bar[wg], k & 1);
+        if (wtid == 0) LFD_TRACE_EPI(tr, k, 3);
+        auto stage_box = [&](const float* acc, uint32_t box) LFD_LAMBDA_INLINE {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = r0 + 8 * h;
+                    const uint32_t addr = box + (uint32_t)(row * 128) + (((uint32_t)j ^ (uint32_t)(row & 7)) << 4) + 4u * tq;
+                    float x0 = acc[4 * j + 2 * h] + bv[j].x, x1 = acc[4 * j + 2 * h + 1] + bv[j].y;
+                    if (has_res) {
+                        uint32_t rv;
+                        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(rv) : "r"(addr) : "memory");
+                        x0 += up_lo<F16>(rv); x1 += up_hi<F16>(rv);
+                    }
+                    const uint32_t o = relu ? pack2_relu<F16>(x0, x1) : pack2<F16>(x0, x1);
+                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(o) : "memory");
+                }
+            }
+        };
+        stage_box(acc0, stg);
+        stage_box(acc1, stg + kBox);
+        fence_proxy_async_smem();                 // st.shared (generic proxy) -> TMA store (async proxy)
+        wg_bar_sync(wg);
+        if (wtid == 0) {                          // rows / columns outside the map are clipped by the TMA engine
+            tma_store_4d(&p.tm_out, stg, 0, c0, c1, n);
+            tma_store_4d(&p.tm_out, stg + kBox, 0, c0, c1 + 8, n);
+            bulk_commit();
+            LFD_TRACE_EPI(tr, k, 2);
+        }
+    }
+    if (wtid == 0) bulk_wait_all();   // all tile stores have been performed before the CTA retires
+}
+
 // DS: the launch carries the fused 1x1/s2 shortcut (MODE_3X3S2, p.Cout3 > 0).  The shortcut and the fused tail never meet in one launch;
 // with COUT = 128 a kernel that holds the code of both needs more registers than its 168: it spills and ptxas serialises its wgmmas.
-// The body of conv_umma_kernel (COUT = 16 / 32 / 64 / 128) and of conv_umma_c48_kernel (COUT = 48); p is the kernel's parameter.
-template <int MODE, int COUT, bool F16, bool EXT, bool DS>
+// The body of conv_umma_kernel (COUT = 16 / 32 / 64 / 128), of conv_umma_c48_kernel (COUT = 48) and of conv_umma_solo_kernel (SOLO: the
+// consumers are solo_consumers); p is the kernel's parameter.
+template <int MODE, int COUT, bool F16, bool EXT, bool DS, bool SOLO = false>
 LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
     static_assert(!DS || MODE == MODE_3X3S2, "the fused shortcut belongs to a 3x3/s2 conv");
+    static_assert(!SOLO || (MODE == MODE_3X3S1 && COUT == 64 && !DS), "the solo schedule is the 64-channel 3x3/s1 conv's");
     constexpr int kProd = kProdThreads;
     constexpr int kThreads = kConvThreads;
     constexpr int TAPS = (MODE == MODE_3X3S1 || MODE == MODE_3X3S2) ? 9 : (MODE == MODE_STEM ? 3 : 1);
@@ -304,6 +434,7 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
     uint64_t* empty = full + kMaxStages;
     uint64_t* wbar = empty + kMaxStages;
     uint64_t* res_bar = wbar + 1;     // [2] residual rows of one warpgroup landed (TMA load)
+    uint64_t* turn = res_bar + 2;     // [2] SOLO: warpgroup wg may issue its MMAs
     PxEntry* table = reinterpret_cast<PxEntry*>(smem + p.smem_table_off);
     PxDelta* delta = reinterpret_cast<PxDelta*>(smem + p.smem_table_off + (size_t)p.n_px * sizeof(PxEntry));
     float* bias = reinterpret_cast<float*>(smem + p.smem_bias_off);
@@ -326,11 +457,15 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
     if (tid == 0) {
         for (int i = 0; i < SA; ++i) {
             mbar_init(&full[i], kProd + (p.b_resident ? 0 : 1));
-            mbar_init(&empty[i], kConsumerThreads / 32);
+            mbar_init(&empty[i], SOLO ? 4 : kConsumerThreads / 32);   // SOLO: a stage is consumed by the 4 warps of one warpgroup
         }
         mbar_init(wbar, 1);
         mbar_init(&res_bar[0], 1);
         mbar_init(&res_bar[1], 1);
+        if (SOLO) {
+            mbar_init(&turn[0], 4);
+            mbar_init(&turn[1], 4);
+        }
         fence_mbar_init();
     }
     // per-channel shifts (folded BatchNorm / bias), rounded to the 16-bit type, added to the fp32 accumulators by the epilogue
@@ -371,7 +506,9 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
     const int n_cc = p.Cin / p.Cc;
     const LaunchGrid lg = launch_grid<MODE, EXT>(p);
 
-    if (warp < kConsumerThreads / 32) {
+    if (SOLO && warp < kConsumerThreads / 32) {
+        if constexpr (SOLO) solo_consumers<F16, EXT>(p, lg, full, empty, wbar, res_bar, turn, bias, staging, wres, ring);
+    } else if (warp < kConsumerThreads / 32) {
         // ============================================================== CONSUMERS (MMA + epilogue)
         // registers move from the producer warpgroup to the accumulators: 2 x 128 x 224 + 128 x 56 = 64512 of 65536
         asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
@@ -726,6 +863,13 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_kernel(const __grid
 template <int MODE, bool F16, bool EXT, bool DS>
 __global__ void __launch_bounds__(kConvThreads, 1) conv_umma_c48_kernel(const __grid_constant__ UmmaConvParams p) {
     conv_umma_body<MODE, 48, F16, EXT, DS>(p);
+}
+
+// The 64-channel 3x3/s1 convs with one ring stage per tile and more tiles than CTAs: one consumer warpgroup per tile, the two
+// warpgroups' MMA phases alternating (solo_consumers).  umma_conv_configure sets p.solo from the geometry.
+template <bool F16, bool EXT>
+__global__ void __launch_bounds__(kConvThreads, 1) conv_umma_solo_kernel(const __grid_constant__ UmmaConvParams p) {
+    conv_umma_body<MODE_3X3S1, 64, F16, EXT, false, true>(p);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1176,10 +1320,12 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
 // ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
-static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvParams* out, size_t* smem_bytes, int* grid) {
+// solo: the layout of conv_umma_solo_kernel, whose warpgroups stage all 128 rows of a tile
+static int configure_with(const ConvGeom& g, int num_sms, int nbuf, bool solo, UmmaConvParams* out, size_t* smem_bytes, int* grid) {
     UmmaConvParams p;
     memset(&p, 0, sizeof(p));
     p.stg_nbuf = nbuf;
+    p.solo = solo ? 1 : 0;
     int mode;
     if (g.stem) {
         if (g.ksize != 3 || g.stride != 2 || g.Cin != 16) return -1;   // "Cin" = K of one filter row: 4 pixels x 4 padded channels
@@ -1218,7 +1364,7 @@ static int configure_with(const ConvGeom& g, int num_sms, int nbuf, UmmaConvPara
     if (g.ds_cout && (mode != MODE_3X3S2 || g.tail_cout || g.ds_cout != g.Cout)) return -6;
     if (g.tail_cout && (g.tail_cout % 16 || g.tail_cout > 128 || g.tail_cout < 16)) return -4;
     if (g.tail_cout && (g.tail_cout == 48) != (g.Cout == 48)) return -4;   // a 48-channel conv has the 48-channel tail only
-    const size_t staging = (size_t)nbuf * 128 * Cf * 2;   // [warpgroup][buffer][64 rows][Cf]
+    const size_t staging = (size_t)nbuf * (solo ? 256 : 128) * Cf * 2;   // [warpgroup][buffer][64 rows (solo: 128)][Cf]
     // fixed head of the shared-memory map: barriers | [halo table] | shift | [tail shift] | staging (1 KB aligned)
     size_t hoff = kSmemTableOff;
     p.smem_table_off = (uint32_t)hoff;
@@ -1325,12 +1471,22 @@ int umma_conv_configure(const ConvGeom& g, int num_sms, UmmaConvParams* out, siz
     UmmaConvParams p1, p2;
     size_t s1 = 0, s2 = 0;
     int g1 = 0, g2 = 0;
-    const int rc = configure_with(g, num_sms, 1, &p1, &s1, &g1);
+    const int rc = configure_with(g, num_sms, 1, false, &p1, &s1, &g1);
     if (rc) return rc;
-    if (configure_with(g, num_sms, 2, &p2, &s2, &g2) == 0 && p2.b_resident == p1.b_resident &&
+    if (configure_with(g, num_sms, 2, false, &p2, &s2, &g2) == 0 && p2.b_resident == p1.b_resident &&
         p2.Cc == p1.Cc && p2.stages >= (p1.stages < 3 ? p1.stages : 3)) {
         *out = p2; *smem_bytes = s2; *grid = g2;
     } else {
+        *out = p1; *smem_bytes = s1; *grid = g1;
+    }
+    // conv_umma_solo_kernel for the 64-channel 3x3/s1 convs with one resident-weight ring stage per tile (a 64-channel conv never has
+    // GroupNorm statistics, a 3x3/s1 conv never a shortcut) and more tiles than CTAs, so that the warpgroups have tiles to alternate
+    // on (measured on WIDERFACE-S 720p b8: the 45x80 layers, 240 tiles, gain from it; the 23x40 ones, 80 tiles, gain nothing).  One
+    // staging region per warpgroup (its stores have drained by the time its next tile, two tiles later, is staged) and a ring of at
+    // least 3 stages: two tiles are consumed while the next one fills.
+    const bool solo_geom = !g.stem && g.ksize == 3 && g.stride == 1 && g.Cin == 64 && g.Cout == 64 && !g.tail_cout && !g.ds_cout;
+    if (solo_geom && out->Cc == 64 && out->b_resident && out->num_tiles > *grid &&
+        configure_with(g, num_sms, 1, true, &p1, &s1, &g1) == 0 && p1.b_resident && p1.Cc == 64 && p1.stages >= 3) {
         *out = p1; *smem_bytes = s1; *grid = g1;
     }
     return 0;
@@ -1425,6 +1581,11 @@ template <int MODE, int COUT, bool F16, bool EXT>
 static cudaError_t launch_mode_ds(const UmmaConvParams& p, size_t smem, int grid, cudaStream_t st) {
     if constexpr (MODE == MODE_3X3S2)
         if (p.Cout3) return launch_mode_t<MODE, COUT, F16, EXT, true>(p, smem, grid, st);
+    if constexpr (MODE == MODE_3X3S1 && COUT == 64)
+        if (p.solo) {
+            static bool configured[kMaxDevices] = {};
+            return launch_persistent(conv_umma_solo_kernel<F16, EXT>, configured, 224 * 1024, p, smem, grid, st);
+        }
     return launch_mode_t<MODE, COUT, F16, EXT, false>(p, smem, grid, st);
 }
 

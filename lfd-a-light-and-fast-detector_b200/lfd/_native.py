@@ -147,6 +147,7 @@ SYMBOLS = {
     'lfd_last_error': (C.c_char_p, []),
     'lfd_device_sm_count': (_i, []),
     'lfd_conv_query': (_i, [_i] * 11 + [C.POINTER(_i)] * 4 + [C.POINTER(_i64)]),
+    'lfd_conv_schedule': (_i, [_i] * 11 + [C.POINTER(_i)]),
     'lfd_stem4_query': (_i, [_i] * 3 + [C.POINTER(_i), C.POINTER(_i64), C.POINTER(_i), C.POINTER(_i)]),
     'lfd_plan_create': (_i, [C.POINTER(Op), _i, _i, _i, _i, _i64, _i64, _i64, _i, C.POINTER(_vp)]),
     'lfd_plan_destroy': (_i, [_vp]),
@@ -249,7 +250,11 @@ def conv_query(N, H, W, Cin, Ho, Wo, Cout, ksize, stride, tail_cout=0, ds_cout=0
     smem = C.c_int64()
     check(lib().lfd_conv_query(N, H, W, Cin, Ho, Wo, Cout, ksize, stride, tail_cout, ds_cout, C.byref(cc), C.byref(st), C.byref(res),
                                C.byref(nt), C.byref(smem)))
-    return dict(cc=cc.value, stages=st.value, weights_resident=res.value, num_tiles=nt.value, smem_bytes=smem.value)
+    solo = C.c_int()
+    check(lib().lfd_conv_schedule(N, H, W, Cin, Ho, Wo, Cout, ksize, stride, tail_cout, ds_cout, C.byref(solo)))
+    # schedule: 'solo' = one consumer warpgroup per tile (conv_umma_solo_kernel), 'shared' = both consumer warpgroups on every tile
+    return dict(cc=cc.value, stages=st.value, weights_resident=res.value, num_tiles=nt.value, smem_bytes=smem.value,
+                schedule='solo' if solo.value else 'shared')
 
 
 def stem4_query(N, H, W):
