@@ -1,10 +1,12 @@
 /* lfd_detect -- runs a model file on raw video frames with liblfd_b200.so and cudart alone (no Python, no torch).
  *
- *     lfd_detect MODEL FRAMES HEIGHT WIDTH [bgr|nv12]
+ *     lfd_detect MODEL FRAMES HEIGHT WIDTH [bgr|gray|nv12]
  *
  * MODEL   a model file written by lfd.deployment.export_model (include/lfd_b200.h, "model files")
- * FRAMES  raw uint8 frames of HEIGHT x WIDTH back to back: BGR (HEIGHT * WIDTH * 3 bytes each, the default) or NV12 (a Y plane of
- *         HEIGHT x WIDTH bytes, then the interleaved UV plane of HEIGHT / 2 x WIDTH bytes); HEIGHT and WIDTH at most the model's capacity
+ * FRAMES  raw uint8 frames of HEIGHT x WIDTH back to back: the model's own kind by default -- BGR (HEIGHT * WIDTH * 3 bytes each) for a
+ *         model whose image op (op 0) has Cin = 3, gray (HEIGHT * WIDTH bytes each) for one with Cin = 1 -- or NV12 (a Y plane of
+ *         HEIGHT x WIDTH bytes, then the interleaved UV plane of HEIGHT / 2 x WIDTH bytes; a gray model reads the Y plane only);
+ *         HEIGHT and WIDTH at most the model's capacity
  *
  * The frames run in batches of the model's N (a last partial batch is padded with black frames, whose rows are not printed).  For every
  * frame it prints "frame INDEX COUNT" and then COUNT rows "label score x y w h" -- the rows of LFD.predict_for_single_image, with
@@ -53,13 +55,13 @@ static void* read_file(const char* path, size_t* n) {
 
 int main(int argc, char** argv) {
     if (argc < 5 || argc > 6) {
-        fprintf(stderr, "usage: %s MODEL FRAMES HEIGHT WIDTH [bgr|nv12]\n", argv[0]);
+        fprintf(stderr, "usage: %s MODEL FRAMES HEIGHT WIDTH [bgr|gray|nv12]\n", argv[0]);
         return 2;
     }
     const int h = atoi(argv[3]), w = atoi(argv[4]);
     const int nv12 = argc == 6 && strcmp(argv[5], "nv12") == 0;
-    if (argc == 6 && !nv12 && strcmp(argv[5], "bgr") != 0) {
-        fprintf(stderr, "frame format must be bgr or nv12, got %s\n", argv[5]);
+    if (argc == 6 && !nv12 && strcmp(argv[5], "bgr") != 0 && strcmp(argv[5], "gray") != 0) {
+        fprintf(stderr, "frame format must be bgr, gray or nv12, got %s\n", argv[5]);
         return 2;
     }
     size_t model_bytes = 0, frames_bytes = 0;
@@ -74,12 +76,20 @@ int main(int argc, char** argv) {
     free(model);
     lfd_engine_desc d;
     CHECK_LFD(lfd_engine_info(engine, &d));
+    lfd_op image_op;   /* op 0 reads the frames: Cin = 3 (BGR) or 1 (gray) bytes per pixel of a uint8 frame */
+    int32_t src_op, level;
+    CHECK_LFD(lfd_engine_op(engine, 0, &image_op, &src_op, &level));
+    const size_t px = (size_t)image_op.Cin;
+    if (argc == 6 && !nv12 && (strcmp(argv[5], "gray") == 0) != (px == 1)) {
+        fprintf(stderr, "%s frames on a %s model\n", argv[5], px == 1 ? "gray" : "BGR");
+        return 2;
+    }
     if (h < 1 || w < 1 || h > d.H || w > d.W || (nv12 && ((h | w) & 1))) {
         fprintf(stderr, "frames of %dx%d do not fit the model's capacity %dx%d%s\n", h, w, d.H, d.W, nv12 ? " (NV12: even sizes)" : "");
         return 1;
     }
-    const size_t frame_bytes = nv12 ? (size_t)h * w * 3 / 2 : (size_t)h * w * 3;
-    const size_t image_bytes = nv12 ? (size_t)d.H * d.W * 3 / 2 : (size_t)d.H * d.W * 3;   /* one image in the capacity layout */
+    const size_t frame_bytes = nv12 ? (size_t)h * w * 3 / 2 : (size_t)h * w * px;
+    const size_t image_bytes = nv12 ? (size_t)d.H * d.W * 3 / 2 : (size_t)d.H * d.W * px;   /* one image in the capacity layout */
     const size_t n_frames = frames_bytes / frame_bytes;
     if (n_frames * frame_bytes != frames_bytes) {
         fprintf(stderr, "%s holds %zu bytes, not a whole number of %zu-byte frames\n", argv[2], frames_bytes, frame_bytes);
@@ -120,7 +130,7 @@ int main(int argc, char** argv) {
                 for (int r = 0; r < h; ++r) memcpy(img + (size_t)r * d.W, f + (size_t)r * w, (size_t)w);
                 for (int r = 0; r < h / 2; ++r) memcpy(img + (size_t)(d.H + r) * d.W, f + (size_t)(h + r) * w, (size_t)w);
             } else {
-                for (int r = 0; r < h; ++r) memcpy(img + (size_t)r * d.W * 3, f + (size_t)r * w * 3, (size_t)w * 3);
+                for (int r = 0; r < h; ++r) memcpy(img + (size_t)r * d.W * px, f + (size_t)r * w * px, (size_t)w * px);
             }
         }
         CHECK_CUDA(cudaMemcpyAsync(input, batch, d.N * image_bytes, cudaMemcpyHostToDevice, stream));

@@ -80,7 +80,12 @@ enum { LFD_INPUT_F32_NCHW = 0, LFD_INPUT_U8_NHWC = 1, LFD_INPUT_U8_NV12 = 2 };
  * lfd_plan_forward, lfd_plan_forward_extent, lfd_plan_profile and lfd_run_op check before anything is enqueued: an odd frame height or
  * width is LFD_ERR_INVALID, an NV12 frame on a plan (an image op) of odd capacity H or W is LFD_ERR_UNSUPPORTED.  lfd_train_plan_run,
  * lfd_train_plan_profile and lfd_run_top refuse NV12 with LFD_ERR_UNSUPPORTED.  Every entry point refuses a format other than these three
- * with LFD_ERR_INVALID. */
+ * with LFD_ERR_INVALID.
+ * GRAY (1-channel) PLANS: an image op (STEM0 / STEM4; lfd_top STEM0 / WGRAD_STEM) with Cin = 1 reads one value per pixel, and the same
+ * format numbers then mean: LFD_INPUT_F32_NCHW float[N][1][H][W]; LFD_INPUT_U8_NHWC uint8[N][H][W] (1 byte per pixel); LFD_INPUT_U8_NV12
+ * the usual NV12 buffer above, of which only the Y plane is read (the UV bytes are never touched): Y is the gray byte, as
+ * cv2.cvtColor(frame, cv2.COLOR_YUV2GRAY_NV12) defines it.  A gray model with stem weights W1 gives, bit for bit, what the 3-channel model
+ * with stem weights [W1, 0, 0] gives on a frame whose channel 0 is the gray frame. */
 enum { LFD_CONV_UMMA = 0, LFD_CONV_SIMT = 1 }; /* SIMT = cross-check kernel, validation only */
 /* 16-bit storage type of activations and packed weights (fp32 accumulation either way; same bytes, same tensor-core rate):
  * bf16 = the north-star dtype; fp16 = 3 more mantissa bits, the variant that meets 1e-3 END TO END (DESIGN.md "Parity") and the
@@ -95,17 +100,21 @@ enum { LFD_DTYPE_BF16 = 0, LFD_DTYPE_FP16 = 1 };
  * Pixels outside the image (conv padding, beyond a smaller frame's extent) are 0 after the transform.  ALL SEVEN FIELDS ZERO selects
  * simple_normalize on BGR, mean 127.5 and scale float32(1 / 127.5): a zero-filled struct behaves as the library always did.  Anything else
  * must be complete: in_swap_rb 0 or 1, every mean finite, every scale finite and non-zero; otherwise the op fails with LFD_ERR_INVALID when
- * it is planned, before anything is enqueued.  The LFD_INPUT_F32_NCHW input is taken as it is and ignores these fields. */
+ * it is planned, before anything is enqueued.  On a gray op (Cin = 1) the one channel is ((float) byte - in_mean[0]) * in_scale[0]: a
+ * nonzero in_swap_rb, or unequal in_mean / in_scale values, is LFD_ERR_INVALID there.  The LFD_INPUT_F32_NCHW input is taken as it is and
+ * ignores these fields. */
 
 /* One fused layer.  Activations are bf16 NHWC at byte offsets into the caller's workspace.
- *   STEM0      3x3/s2 conv on the 3-channel image + shift (+ReLU), scale folded into the weights like CONV; in_off ignored (reads the external input);
+ *   STEM0      3x3/s2 conv on the image + shift (+ReLU), Cin = 3 (BGR) or 1 (gray), scale folded into the weights like CONV; in_off ignored
+ *              (reads the external input);
  *              weight = bf16 packed [kh][2][Cout][8]: element (kh, kc, n, j) = weight of output n, input channel j % 4, filter
  *              column kw = 2*kc + j/4 (zero for kw = 3 and for the padded 4th channel): the kernel keeps the image patch as
- *              4-channel bf16 pixels and lets the wgmma address generator do the im2col (K = 16 per filter row).
+ *              4-channel bf16 pixels and lets the wgmma address generator do the im2col (K = 16 per filter row).  A gray op's weight is
+ *              packed the same way with its one channel in the channel-0 lanes and zeros in the others.
  *   STEM4      the four convolutions of a 'faster' stem in one kernel: stem0 3x3/s2 3->64 (weight / shift / relu, packed as STEM0),
  *              stem1 1x1 64->64 (tail_weight / tail_shift / tail_relu, tail_cout = 64), stem2 3x3/s2 64->64 (s2_weight = bf16 packed
  *              [9][8][64][8], i.e. the CONV packing with cc = 64; s2_shift / s2_relu) and stem3 1x1 64->64 (s3_weight = bf16 packed
- *              [8][64][8]; s3_shift / s3_relu).  Cin = 3, Cout = 64, ksize = 3, stride = 2; H x W = the image, Ho x Wo = the stem3
+ *              [8][64][8]; s3_shift / s3_relu).  Cin = 3 or 1, Cout = 64, ksize = 3, stride = 2; H x W = the image, Ho x Wo = the stem3
  *              output (two stride-2 steps); in_off ignored.  Every intermediate is rounded to bf16 exactly as the STEM0 + CONV pair
  *              path rounds it, so the output is bit-identical to it; the stem1 map never reaches HBM.  Sizes: lfd_stem4_query.
  *   CONV       ksize in {1,3}, stride in {1,2}, pad = ksize/2; y = conv(x) + shift (+res) (ReLU) -> bf16; Cout in {16, 32, 48, 64, 128}
@@ -386,7 +395,8 @@ int lfd_sigmoid_focal_loss_backward(const float* logits, const int64_t* targets,
  *   WGRAD            x        dz      -       -        -          dstage   -       -        -
  *   WGRAD_STEM       x27      dz      -       -        -          dstage   -       -        -          (x = the run-time input image; x27 >= 0: scratch
  *                                                                                                        bf16 [N][Ho][Wo][32] for the im2col + tensor-core path, dstage then has 32 rows;
- *                                                                                                        x27 = -1 or impl = SIMT: the SIMT kernel, 27 rows)
+ *                                                                                                        x27 = -1 or impl = SIMT: the SIMT kernel, 27 rows;
+ *                                                                                                        Cin = 1 (gray): 9 rows [tap][co], x27 zero past column 9)
  *   UNPACK           -        -       -       -        -          -        -       -        table (lfd_unpack_desc[n_desc], device)
  *   ZERO             begin    bytes   -       -        -          -        -       -        -          (cudaMemsetAsync of a workspace region)
  *   INFER            in       out     res     ds_out   -          -        -       -        op (const lfd_op*, HOST memory, read by lfd_train_plan_create)
@@ -444,7 +454,8 @@ typedef struct lfd_pack_desc {
     const float* src;         /* the parameter; SCALE_SHIFT: the bias [n] (or NULL) */
     const float* src2;        /* SCALE_SHIFT: the level's scalar Scale parameter (or NULL = 1) */
     void* dst;                /* CONV_FWD: bf16 [Cin/cc][k*k][cc/8][Cout][8]; CONV_DGRAD: the transposed conv's operand
-                                 bf16 [Cout/cc][k*k][cc/8][Cin][8] with flipped taps; STEM: bf16 [kh][2][Cout][8];
+                                 bf16 [Cout/cc][k*k][cc/8][Cin][8] with flipped taps; STEM: bf16 [kh][2][Cout][8] of a
+                                 [Cout][Cin][3][3] weight, Cin = 3 or 1 (gray: channel-0 lanes, zeros elsewhere);
                                  ROUND_F32: fp32 copy holding bf16-rounded values; SCALE_SHIFT: scale[n] */
     void* dst2;               /* SCALE_SHIFT: shift[n] = bias * scale */
     void* dst3;               /* SCALE_SHIFT: bias[n] */

@@ -317,9 +317,10 @@ extern "C" int lfd_stem4_query(int N, int H, int W, int* num_tiles, int64_t* sme
 }
 
 // The input transform of an op as the kernels take it (constants by byte position, kernels.cuh) from the C-ABI's fields (by network
-// channel, see lfd_op): all seven fields zero = simple_normalize on BGR; anything else has to be a complete transform.  One place for
-// lfd_op and lfd_top.
-static int input_transform_of(int32_t swap, const float* mean, const float* scale, InputTransform* out) {
+// channel, see lfd_op): all seven fields zero = simple_normalize; anything else has to be a complete transform.  One place for lfd_op
+// and lfd_top, and for both image kinds: BGR (cin 3) and gray (cin 1), whose one channel is (byte - mean[0]) * scale[0] -- it has no
+// channel swap and takes three equal constants, so every byte position of the resolved transform holds channel 0's.
+static int input_transform_of(int cin, int32_t swap, const float* mean, const float* scale, InputTransform* out) {
     bool zero = swap == 0;
     for (int c = 0; c < 3; ++c) zero = zero && mean[c] == 0.f && scale[c] == 0.f;
     if (zero) {
@@ -328,6 +329,10 @@ static int input_transform_of(int32_t swap, const float* mean, const float* scal
         return LFD_OK;
     }
     if (swap != 0 && swap != 1) return fail(LFD_ERR_INVALID, "input transform: in_swap_rb = %d (0 or 1)", swap);
+    if (cin == 1 && (swap || mean[1] != mean[0] || mean[2] != mean[0] || scale[1] != scale[0] || scale[2] != scale[0]))
+        return fail(LFD_ERR_INVALID, "input transform of a gray (1-channel) image: in_swap_rb must be 0 and the three in_mean / in_scale equal "
+                    "(got swap %d, mean %g %g %g, scale %g %g %g)", swap, (double)mean[0], (double)mean[1], (double)mean[2], (double)scale[0],
+                    (double)scale[1], (double)scale[2]);
     for (int c = 0; c < 3; ++c)
         if (!std::isfinite(mean[c]) || !std::isfinite(scale[c]) || scale[c] == 0.f)
             return fail(LFD_ERR_INVALID, "input transform: channel %d has mean %g, scale %g (set all of in_swap_rb / in_mean / in_scale with finite means and "
@@ -344,14 +349,15 @@ static int check_op(const lfd_op& o) {
     switch (o.kind) {
         case LFD_OP_STEM0:
             if (o.scale || o.tail_scale) return fail(LFD_ERR_INVALID, "conv scale must be folded into the packed weights (pass scale = NULL)");
-            if (o.Cin != 3 || o.ksize != 3 || o.stride != 2) return fail(LFD_ERR_UNSUPPORTED, "stem0 supports 3x3/s2 on 3 input channels only (got Cin=%d k=%d s=%d)", o.Cin, o.ksize, o.stride);
+            if ((o.Cin != 3 && o.Cin != 1) || o.ksize != 3 || o.stride != 2)
+                return fail(LFD_ERR_UNSUPPORTED, "stem0 supports 3x3/s2 on 3 (BGR) or 1 (gray) input channels only (got Cin=%d k=%d s=%d)", o.Cin, o.ksize, o.stride);
             if (o.Cout != 16 && o.Cout != 32 && o.Cout != 48 && o.Cout != 64) return fail(LFD_ERR_UNSUPPORTED, "stem0 Cout must be 16/32/48/64 (got %d)", o.Cout);
             if (o.Ho != eh || o.Wo != ew) return fail(LFD_ERR_INVALID, "stem0 output size mismatch");
             break;
         case LFD_OP_STEM4:
             if (o.scale || o.tail_scale) return fail(LFD_ERR_INVALID, "conv scale must be folded into the packed weights (pass scale = NULL)");
-            if (o.Cin != 3 || o.ksize != 3 || o.stride != 2 || o.Cout != 64 || o.tail_cout != 64 || o.ds_cout || o.res_off >= 0 || o.gn_groups)
-                return fail(LFD_ERR_UNSUPPORTED, "stem4 is 3x3/s2 3->64, 1x1 64->64, 3x3/s2 64->64, 1x1 64->64 without residual / statistics");
+            if ((o.Cin != 3 && o.Cin != 1) || o.ksize != 3 || o.stride != 2 || o.Cout != 64 || o.tail_cout != 64 || o.ds_cout || o.res_off >= 0 || o.gn_groups)
+                return fail(LFD_ERR_UNSUPPORTED, "stem4 is 3x3/s2 3->64 or 1->64 (got Cin=%d), 1x1 64->64, 3x3/s2 64->64, 1x1 64->64 without residual / statistics", o.Cin);
             if (!o.weight || !o.tail_weight || !o.s2_weight || !o.s3_weight) return fail(LFD_ERR_INVALID, "stem4 needs the weights of all four convs");
             if (o.Ho != (eh - 1) / 2 + 1 || o.Wo != (ew - 1) / 2 + 1) return fail(LFD_ERR_INVALID, "stem4 output size mismatch (expected the stem3 map)");
             break;
@@ -388,7 +394,7 @@ static int plan_op(const lfd_op& o, PlannedOp* out) {
     out->smem = 0;
     out->grid = 0;
     if (o.kind == LFD_OP_STEM0 || o.kind == LFD_OP_STEM4) {
-        rc = input_transform_of(o.in_swap_rb, o.in_mean, o.in_scale, &out->xf);
+        rc = input_transform_of(o.Cin, o.in_swap_rb, o.in_mean, o.in_scale, &out->xf);
         if (rc) return rc;
     }
     if (o.kind == LFD_OP_CONV || o.kind == LFD_OP_STEM0 || o.kind == LFD_OP_STEM4) {
@@ -416,12 +422,12 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
                 Stem0Params p;
                 p.in = input; p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off);
                 p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift;
-                p.input_format = input_format; p.N = o.N; p.H = o.H; p.W = o.W; p.Ho = o.Ho; p.Wo = o.Wo; p.Cout = o.Cout; p.relu = o.relu; p.f16 = o.dtype;
+                p.input_format = input_format; p.Cin = o.Cin; p.N = o.N; p.H = o.H; p.W = o.W; p.Ho = o.Ho; p.Wo = o.Wo; p.Cout = o.Cout; p.relu = o.relu; p.f16 = o.dtype;
                 p.xf = po.xf;
                 CUDA_TRY(stem0_launch(p, st));
             } else {
                 UmmaConvParams p = po.cp;
-                p.in_raw = input; p.input_format = input_format; p.in = nullptr;
+                p.in_raw = input; p.input_format = input_format; p.in_ch = o.Cin; p.in = nullptr;
                 p.xf = po.xf;
                 if (input_format == LFD_INPUT_F32_NCHW) p.xf.swap = 0;   // the loaders order the channels at the load: fp32 planes are taken as they are
                 p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off); p.res = nullptr;
@@ -438,11 +444,11 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
             if (!input) return fail(LFD_ERR_INVALID, "stem4 needs the external input pointer");
             if (conv_impl == LFD_CONV_SIMT) return fail(LFD_ERR_UNSUPPORTED, "the SIMT cross-check kernels do not implement the fused stem (plan its four convs)");
             UmmaConvParams p = po.cp;
-            p.in_raw = input; p.input_format = input_format; p.in = nullptr;
+            p.in_raw = input; p.input_format = input_format; p.in_ch = o.Cin; p.in = nullptr;
             p.xf = po.xf;
             if (input_format == LFD_INPUT_F32_NCHW) p.xf.swap = 0;
-            // the word loader: rows of whole aligned words (BGR: 3 words per 4 pixels; NV12: a Y word and a UV word, its image pitch
-            // H * W * 3 / 2 then being a multiple of 4 as well, since H is even)
+            // the word loader: rows of whole aligned words (BGR: 3 words per 4 pixels; gray: 1 word per 4 pixels; NV12: a Y word and a UV
+            // word, its image pitch H * W * 3 / 2 then being a multiple of 4 as well, since H is even)
             p.in_words = input_format != LFD_INPUT_F32_NCHW && o.W % 4 == 0 && (reinterpret_cast<uintptr_t>(input) & 3) == 0;
             p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off); p.res = nullptr; p.stats = nullptr;
             p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift; p.relu = o.relu;
@@ -1068,7 +1074,8 @@ static int plan_top(const lfd_top& t, int64_t ws_bytes, PlannedTop* out) {
         case LFD_TOP_NORM_BWD_REDUCE: case LFD_TOP_NORM_BWD_APPLY: case LFD_TOP_ZERO:
             break;
         case LFD_TOP_WGRAD_STEM:
-            return input_transform_of(t.in_swap_rb, t.in_mean, t.in_scale, &out->conv.xf);
+            if (t.Cin != 3 && t.Cin != 1) return fail(LFD_ERR_UNSUPPORTED, "wgrad_stem: 3 (BGR) or 1 (gray) input channels (got Cin=%d)", t.Cin);
+            return input_transform_of(t.Cin, t.in_swap_rb, t.in_mean, t.in_scale, &out->conv.xf);
         default:
             return fail(LFD_ERR_INVALID, "unknown training op kind %d", t.kind);
     }
@@ -1404,6 +1411,11 @@ static int check_model_op(const lfd_engine* e, int i) {
                                : o.in_swap_rb == 0 && !memcmp(o.in_mean, "\0\0\0\0\0\0\0\0\0\0\0\0", 12) &&
                                      !memcmp(o.in_scale, "\0\0\0\0\0\0\0\0\0\0\0\0", 12);
     if (!same_xf) return bad_file("op %d: input transform (in_swap_rb / in_mean / in_scale) %s", i, image ? "differs from the plan's" : "set on an op that does not read the image");
+    if (image) {
+        InputTransform xf;
+        if (o.Cin != 3 && o.Cin != 1) return bad_file("op 0: an image of %d channels (3: BGR, 1: gray)", o.Cin);
+        if (input_transform_of(o.Cin, o.in_swap_rb, o.in_mean, o.in_scale, &xf)) return bad_file("op 0: %s", g_err);
+    }
     const int32_t dims[] = {o.H, o.W, o.Ho, o.Wo};
     for (int32_t d : dims)
         if (!in_range(d, 1, kModelMaxSide)) return bad_file("op %d: H / W / Ho / Wo = %d / %d / %d / %d outside [1, %d]", i, o.H, o.W, o.Ho, o.Wo, kModelMaxSide);
@@ -1526,7 +1538,7 @@ static int parse_model(const uint8_t* b, size_t n, lfd_engine* e) {
     if (e->stats_off < 0 || e->stats_bytes < 0 || e->stats_bytes > e->ws_bytes || e->stats_off > e->ws_bytes - e->stats_bytes)
         return bad_file("stats_off / stats_bytes = %lld / %lld outside the workspace", (long long)e->stats_off, (long long)e->stats_bytes);
     InputTransform xf;
-    if (input_transform_of(swap, mean, scale, &xf)) return bad_file("input transform: %s", g_err);
+    if (input_transform_of(3, swap, mean, scale, &xf)) return bad_file("input transform: %s", g_err);   // op 0 checks it for its own image kind
     if (e->soft != 0 && e->soft != 1) return bad_file("nms_type = %d (0 greedy, 1 soft_nms)", e->soft);
     if (e->soft && ((e->soft_method != LFD_SOFT_NMS_LINEAR && e->soft_method != LFD_SOFT_NMS_GAUSSIAN) || !std::isfinite(e->soft_sigma) ||
                     !std::isfinite(e->soft_min_score)))

@@ -36,7 +36,7 @@ struct ConvGeom {
     int N, H, W, Cin, Ho, Wo, Cout, ksize, stride;
     int tail_cout;   // > 0: a 1x1/s1 conv (Cout -> tail_cout) is fused behind this conv (second GEMM in the same kernel)
     int ds_cout;     // > 0 (3x3/s2 only): the residual block's 1x1/s2 shortcut conv (Cin -> ds_cout == Cout) is fused: second output tensor
-    int stem;   // 1: 3x3/s2 conv on the raw 3-channel image (K = 27 padded to 32), operand built by the producers
+    int stem;   // 1: 3x3/s2 conv on the raw 3- or 1-channel image (K = 27 padded to 32), operand built by the producers
     int stem4;  // 1: the fused four-conv stem (MODE_STEM4); H x W = the image, Ho x Wo = the stem3 output, Cout = tail_cout = 64
 };
 
@@ -76,6 +76,7 @@ struct alignas(64) UmmaConvParams {
     uint32_t smem_table_off, smem_bias_off, smem_bias2_off, smem_staging_off;
     uint32_t smem_w_off, smem_ring_off;
     int input_format;
+    int in_ch;                  // MODE_STEM / MODE_STEM4: channels of the image, 3 (BGR) or 1 (gray: the loaders write (v, 0, 0, 0), see kStem*)
     InputTransform xf;          // MODE_STEM / MODE_STEM4, u8 NHWC image: byte -> network input (constant bank; xf.swap is 0 for fp32 input)
     int f16;                    // activation / weight type: 0 = bf16, 1 = IEEE fp16 (same bytes, same tensor-core rate)
     // MODE_STEM4: stem0 = w / shift / relu, stem1 = w2 / shift2 / relu2 (the tail fields), stem2 = its 3x3/s2 weights packed

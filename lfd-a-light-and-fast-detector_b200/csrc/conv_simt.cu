@@ -1,6 +1,6 @@
 // conv_simt.cu -- the bandwidth-bound / narrow kernels of the LFD forward that are not GEMM shaped, plus a
 // SIMT cross-check of the wgmma convolution:
-//   stem0_kernel       3x3 stride-2 conv on the 3-channel image (K = 27): direct, fused BN scale/shift + ReLU,
+//   stem0_kernel       3x3 stride-2 conv on the 3-channel (or gray) image (K = 27): direct, fused BN scale/shift + ReLU,
 //                      reads fp32 NCHW (reference `forward(x)` input) or uint8 HWC BGR with the
 //                      (x/255-0.5)/0.5 normalisation fused (reference predict path,
 //                      lfd/data_pipeline/augmentation/augmentation_pipeline.py:31-36); writes bf16 NHWC.
@@ -55,20 +55,20 @@ __global__ void __launch_bounds__(kS0Threads) stem0_kernel(const __grid_constant
         }
         const int y = iy0 + r, x = ix0 + c;
         float v = 0.f;
-        if (y >= 0 && y < p.H && x >= 0 && x < p.W) {
+        if (y >= 0 && y < p.H && x >= 0 && x < p.W && (ci == 0 || p.Cin == 3)) {   // gray: channel 0 only, channels 1 and 2 are 0
             if (p.input_format == 0) {
-                v = reinterpret_cast<const float*>(p.in)[(((size_t)n * 3 + ci) * p.H + y) * p.W + x];
+                v = reinterpret_cast<const float*>(p.in)[(((size_t)n * p.Cin + ci) * p.H + y) * p.W + x];
             } else if (p.input_format == 2) {   // NV12: Y plane, then the interleaved UV plane at the same pitch
                 const int m = p.xf.swap ? 2 - ci : ci;
                 const size_t plane = (size_t)p.H * p.W;
                 const uint8_t* img = reinterpret_cast<const uint8_t*>(p.in) + (size_t)n * (plane + plane / 2);
                 const uint8_t* uv = img + plane + (size_t)(y >> 1) * p.W + (x & ~1);
-                uint32_t bgr[3];
-                nv12_to_bgr(img[(size_t)y * p.W + x], uv[0], uv[1], bgr);
+                uint32_t bgr[3] = {img[(size_t)y * p.W + x], 0u, 0u};
+                if (p.Cin == 3) nv12_to_bgr(bgr[0], uv[0], uv[1], bgr);
                 v = p.xf.apply(m, bgr[m]);
             } else {
                 const int m = p.xf.swap ? 2 - ci : ci;
-                v = p.xf.apply(m, reinterpret_cast<const uint8_t*>(p.in)[(((size_t)n * p.H + y) * p.W + x) * 3 + m]);
+                v = p.xf.apply(m, reinterpret_cast<const uint8_t*>(p.in)[(((size_t)n * p.H + y) * p.W + x) * p.Cin + m]);
             }
             v = round16_rt(v, p.f16);
         }

@@ -20,11 +20,11 @@ struct InputTransform {
 };
 
 struct Stem0Params {
-    const void* in;            // fp32 NCHW (input_format 0) or u8 NHWC (1)
+    const void* in;            // fp32 NCHW (input_format 0), u8 NHWC (1) or NV12 (2), with Cin = 3 or 1 (gray) channels
     __nv_bfloat16* out;        // bf16 NHWC
     const __nv_bfloat16* w;    // packed [kh][2][Cout][8]: element (kh, kc, n, j) = weight (n, ci = j % 4, kh, kw = 2 kc + j / 4), 0 for kw = 3 or ci = 3
     const float* shift;        // fp32 [Cout] or null (BatchNorm scale is folded into w); applied as bf16
-    int input_format, N, H, W, Ho, Wo, Cout, relu;
+    int input_format, Cin, N, H, W, Ho, Wo, Cout, relu;
     int f16;                   // 16-bit type of weights / output: 0 = bf16, 1 = fp16
     InputTransform xf;         // u8 NHWC input only
 };

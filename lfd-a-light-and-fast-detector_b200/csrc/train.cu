@@ -8,6 +8,8 @@
 //   GroupNorm + ReLU lfd/model/head/lfd_head.py:85-135
 //   final convs      lfd/model/head/lfd_head.py:137-143,164-185 (Scale multiplies conv output AND bias, :177-180)
 //   optimizer step   lfd/execution/hooks/optimizer_hook.py:21-36 (clip_grad_norm_ then torch.optim.SGD.step)
+#include <type_traits>
+
 #include "train.cuh"
 
 #include "conv_common.cuh"
@@ -85,14 +87,14 @@ __global__ void __launch_bounds__(256) pack_kernel(const PackDesc* __restrict__ 
         else v = d.src[((size_t)kch * d.Cin + n) * kk + (kk - 1 - tap)];
         reinterpret_cast<__nv_bfloat16*>(d.dst)[idx] = __float2bfloat16_rn(v);
     } else if (d.kind == PACK_STEM) {
-        // [kh][2][Cout][8]: element (kh, kc, n, j) = W[n][ci = j % 4][kh][kw = 2 kc + j / 4], zero for kw = 3 or ci = 3
+        // [kh][2][Cout][8]: element (kh, kc, n, j) = W[n][ci = j % 4][kh][kw = 2 kc + j / 4], zero for kw = 3 or ci >= Cin (3, or 1: gray)
         const int j = idx & 7;
         int r = idx >> 3;
         const int n = r % d.Cout; r /= d.Cout;
         const int kc = r & 1;
         const int kh = r >> 1;
         const int ci = j & 3, kw = 2 * kc + (j >> 2);
-        const float v = (ci < 3 && kw < 3) ? d.src[(((size_t)n * 3 + ci) * 3 + kh) * 3 + kw] : 0.f;
+        const float v = (ci < d.Cin && kw < 3) ? d.src[(((size_t)n * d.Cin + ci) * 3 + kh) * 3 + kw] : 0.f;
         reinterpret_cast<__nv_bfloat16*>(d.dst)[idx] = __float2bfloat16_rn(v);
     } else if (d.kind == PACK_ROUND_F32) {
         reinterpret_cast<float*>(d.dst)[idx] = bf16_round(d.src[idx]);
@@ -714,10 +716,10 @@ cudaError_t head_final_bwd_launch(const HeadFinalBwdParams& p, int num_sms, cuda
 }
 
 // ===================================================================================================
-// weight gradient of the 3-channel stem conv (3x3/s2 on the raw image): K = 27, far too narrow for a tensor-core tile.
+// weight gradient of the stem conv (3x3/s2 on the raw image of Cin = 3 or 1 channels): K = 9 Cin, far too narrow for a tensor-core tile.
 // dstage[(kh*3+kw)][ci][co] += sum_{n,oy,ox} x(n, ci, 2oy+kh-1, 2ox+kw-1) * dz(n, oy, ox, co), x normalised and rounded to bf16 like
 // the forward kernel does (rounding point R0).  Persistent blocks walk 64-pixel output row segments; every thread owns one output
-// channel and up to 7 of the 27 (tap, ci) pairs, accumulates in registers and flushes once.
+// channel and up to 7 of the 9 Cin (tap, ci) pairs, accumulates in registers and flushes once.
 // ===================================================================================================
 static constexpr int kWsSeg = 64, kWsCols = 2 * kWsSeg + 1;
 
@@ -733,17 +735,18 @@ __global__ void __launch_bounds__(256) wgrad_stem_kernel(WgradGeom g, const void
     const int segs_x = (g.Wo + kWsSeg - 1) / kWsSeg;
     const int n_seg = g.N * g.Ho * segs_x;
     const size_t plane = (size_t)g.H * g.W;
+    const int K = 9 * g.Cin;
     for (int seg = blockIdx.x; seg < n_seg; seg += gridDim.x) {
         const int sx = seg % segs_x, oy = (seg / segs_x) % g.Ho, n = seg / (segs_x * g.Ho);
         const int ox0 = sx * kWsSeg, ix0 = 2 * ox0 - 1, iy0 = 2 * oy - 1;
         __syncthreads();
-        for (int i = threadIdx.x; i < 9 * kWsCols; i += 256) {
+        for (int i = threadIdx.x; i < 3 * g.Cin * kWsCols; i += 256) {
             const int c = i % kWsCols, kh = (i / kWsCols) % 3, ci = i / (3 * kWsCols);
             const int y = iy0 + kh, x = ix0 + c;
             float v = 0.f;
             if ((unsigned)y < (unsigned)g.H && (unsigned)x < (unsigned)g.W) {
-                if (input_format == 1) { const int m = xf.swap ? 2 - ci : ci; v = xf.apply(m, reinterpret_cast<const uint8_t*>(image)[((size_t)n * plane + (size_t)y * g.W + x) * 3 + m]); }
-                else v = reinterpret_cast<const float*>(image)[((size_t)n * 3 + ci) * plane + (size_t)y * g.W + x];
+                if (input_format == 1) { const int m = xf.swap ? 2 - ci : ci; v = xf.apply(m, reinterpret_cast<const uint8_t*>(image)[((size_t)n * plane + (size_t)y * g.W + x) * g.Cin + m]); }
+                else v = reinterpret_cast<const float*>(image)[((size_t)n * g.Cin + ci) * plane + (size_t)y * g.W + x];
                 v = bf16_round(v);
             }
             patch[ci][kh][c] = v;
@@ -755,9 +758,9 @@ __global__ void __launch_bounds__(256) wgrad_stem_kernel(WgradGeom g, const void
             const float d = __bfloat162float(dzp[(size_t)px * Cout]);
 #pragma unroll
             for (int i = 0; i < 7; ++i) {
-                const int q = grp + ngrp * i;   // (kh*3 + kw)*3 + ci
-                if (q < 27) {
-                    const int ci = q % 3, t = q / 3;
+                const int q = grp + ngrp * i;   // (kh*3 + kw)*Cin + ci
+                if (q < K) {
+                    const int ci = g.Cin == 3 ? q % 3 : 0, t = g.Cin == 3 ? q / 3 : q;      // (divisions by a constant)
                     acc[i] = fmaf(d, patch[ci][t / 3][2 * px + t % 3], acc[i]);
                 }
             }
@@ -766,12 +769,12 @@ __global__ void __launch_bounds__(256) wgrad_stem_kernel(WgradGeom g, const void
 #pragma unroll
     for (int i = 0; i < 7; ++i) {
         const int q = grp + ngrp * i;
-        if (q < 27) atomicAdd(dstage + (size_t)q * Cout + co, acc[i]);
+        if (q < K) atomicAdd(dstage + (size_t)q * Cout + co, acc[i]);
     }
 }
 
 cudaError_t wgrad_stem_launch(const WgradGeom& g, const void* image, int input_format, const InputTransform& xf, const __nv_bfloat16* dz, float* dstage, int num_sms, cudaStream_t st) {
-    if (g.Cin != 3 || g.ksize != 3 || g.stride != 2 || 256 % g.Cout || g.Cout < 16 || g.Cout > 64) return cudaErrorInvalidValue;
+    if ((g.Cin != 3 && g.Cin != 1) || g.ksize != 3 || g.stride != 2 || 256 % g.Cout || g.Cout < 16 || g.Cout > 64) return cudaErrorInvalidValue;
     const int n_seg = g.N * g.Ho * ((g.Wo + kWsSeg - 1) / kWsSeg);
     int blocks = 4 * num_sms;
     if (blocks > n_seg) blocks = n_seg;
@@ -779,38 +782,44 @@ cudaError_t wgrad_stem_launch(const WgradGeom& g, const void* image, int input_f
     return cudaGetLastError();
 }
 
-// im2col of the 3-channel stem conv for its weight gradient: X27[n][oy][ox][q] with q = (kh*3 + kw)*3 + ci (q >= 27: zero) as bf16, the
-// image normalised + rounded like the forward does (R0).  The weight gradient of the stem conv is then the weight gradient of a 1x1 conv
-// with 32 input channels over X27, i.e. one launch of the tensor-core wgrad kernel; its staging rows [q][co] ARE the [tap][ci][co] layout.
+// im2col of the stem conv for its weight gradient: X27[n][oy][ox][q] with q = (kh*3 + kw)*Cin + ci (q >= 9 Cin: zero; Cin = 3, or 1 for a
+// gray image: X9 padded to the same 32 columns) as bf16, the image normalised + rounded like the forward does (R0).  The weight gradient of
+// the stem conv is then the weight gradient of a 1x1 conv with 32 input channels over X27, i.e. one launch of the tensor-core wgrad kernel;
+// its staging rows [q][co] ARE the [tap][ci][co] layout.
 __global__ void __launch_bounds__(256) stem_im2col_kernel(WgradGeom g, const void* __restrict__ image, int input_format, const __grid_constant__ InputTransform xf,
                                                           __nv_bfloat16* __restrict__ x27) {
     const size_t total = (size_t)g.N * g.Ho * g.Wo * 4;          // one thread per (output pixel, 8-value chunk)
     const size_t plane = (size_t)g.H * g.W;
-    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (size_t)gridDim.x * 256) {
-        const int chunk = (int)(i & 3);
-        const size_t pix = i >> 2;
-        const int ox = (int)(pix % g.Wo), oy = (int)((pix / g.Wo) % g.Ho), n = (int)(pix / ((size_t)g.Wo * g.Ho));
-        float v[8];
+    auto body = [&](auto cin_c) {      // the channel count as a compile-time constant: (tap, ci) from q without a division by a variable
+        constexpr int CIN = decltype(cin_c)::value;
+        for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (size_t)gridDim.x * 256) {
+            const int chunk = (int)(i & 3);
+            const size_t pix = i >> 2;
+            const int ox = (int)(pix % g.Wo), oy = (int)((pix / g.Wo) % g.Ho), n = (int)(pix / ((size_t)g.Wo * g.Ho));
+            float v[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int q = chunk * 8 + j;
-            float f = 0.f;
-            if (q < 27) {
-                const int ci = q % 3, t = q / 3;
-                const int y = 2 * oy + t / 3 - 1, x = 2 * ox + t % 3 - 1;
-                if ((unsigned)y < (unsigned)g.H && (unsigned)x < (unsigned)g.W) {
-                    if (input_format == 1) { const int m = xf.swap ? 2 - ci : ci; f = xf.apply(m, reinterpret_cast<const uint8_t*>(image)[((size_t)n * plane + (size_t)y * g.W + x) * 3 + m]); }
-                    else f = reinterpret_cast<const float*>(image)[((size_t)n * 3 + ci) * plane + (size_t)y * g.W + x];
+            for (int j = 0; j < 8; ++j) {
+                const int q = chunk * 8 + j;
+                float f = 0.f;
+                if (q < 9 * CIN) {
+                    const int ci = q % CIN, t = q / CIN;
+                    const int y = 2 * oy + t / 3 - 1, x = 2 * ox + t % 3 - 1;
+                    if ((unsigned)y < (unsigned)g.H && (unsigned)x < (unsigned)g.W) {
+                        if (input_format == 1) { const int m = xf.swap ? 2 - ci : ci; f = xf.apply(m, reinterpret_cast<const uint8_t*>(image)[((size_t)n * plane + (size_t)y * g.W + x) * CIN + m]); }
+                        else f = reinterpret_cast<const float*>(image)[((size_t)n * CIN + ci) * plane + (size_t)y * g.W + x];
+                    }
                 }
+                v[j] = f;
             }
-            v[j] = f;
+            reinterpret_cast<uint4*>(x27)[i] = pack8f(v);
         }
-        reinterpret_cast<uint4*>(x27)[i] = pack8f(v);
-    }
+    };
+    if (g.Cin == 1) body(std::integral_constant<int, 1>());
+    else body(std::integral_constant<int, 3>());
 }
 
 cudaError_t stem_im2col_launch(const WgradGeom& g, const void* image, int input_format, const InputTransform& xf, __nv_bfloat16* x27, int num_sms, cudaStream_t st) {
-    if (g.Cin != 3 || g.ksize != 3 || g.stride != 2) return cudaErrorInvalidValue;
+    if ((g.Cin != 3 && g.Cin != 1) || g.ksize != 3 || g.stride != 2) return cudaErrorInvalidValue;
     const size_t total = (size_t)g.N * g.Ho * g.Wo * 4;
     size_t blocks = (total + 255) / 256;
     if (blocks > (size_t)num_sms * 16) blocks = (size_t)num_sms * 16;

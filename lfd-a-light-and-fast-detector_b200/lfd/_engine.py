@@ -52,12 +52,22 @@ def level_geometry(backbone, head, h, w):
     return level_sizes, acc, offs
 
 
-def check_input(x, N, H, W, contiguous):
-    """x: float32 [N,3,H,W] or uint8 [N,H,W,3] on a CUDA device -> its nat.INPUT_* format."""
+def image_channels(model):
+    """Channels of the image a model reads: its stem conv's in_channels (3: BGR, 1: gray)."""
+    return model._backbone.stem_layers()[0][0].in_channels
+
+
+def _u8_shape_ok(shape, N, h, w, channels):
+    """uint8 frames: [N,h,w,3] for BGR; [N,h,w] or [N,h,w,1] for gray."""
+    return shape == (N, h, w, channels) or (channels == 1 and shape == (N, h, w))
+
+
+def check_input(x, N, H, W, contiguous, channels=3):
+    """x: float32 [N,C,H,W] or uint8 [N,H,W,3] (gray, C = 1: [N,H,W] or [N,H,W,1]) on a CUDA device -> its nat.INPUT_* format."""
     if x.dtype == torch.float32:
-        fmt, ok = nat.INPUT_F32_NCHW, tuple(x.shape) == (N, 3, H, W)
+        fmt, ok = nat.INPUT_F32_NCHW, tuple(x.shape) == (N, channels, H, W)
     elif x.dtype == torch.uint8:
-        fmt, ok = nat.INPUT_U8_NHWC, tuple(x.shape) == (N, H, W, 3)
+        fmt, ok = nat.INPUT_U8_NHWC, _u8_shape_ok(tuple(x.shape), N, H, W, channels)
     else:
         raise TypeError('input must be float32 NCHW or uint8 NHWC, got %s' % (x.dtype,))
     if not ok or not x.is_cuda or (contiguous and not x.is_contiguous()):
@@ -66,13 +76,14 @@ def check_input(x, N, H, W, contiguous):
     return fmt
 
 
-def check_frame(x, N, H, W):
-    """x: float32 [N,3,h,w] or uint8 [N,h,w,3], contiguous, on a CUDA device, with h <= H and w <= W -> (its nat.INPUT_* format, h, w)."""
+def check_frame(x, N, H, W, channels=3):
+    """x: float32 [N,C,h,w] or uint8 [N,h,w,3] (gray, C = 1: [N,h,w] or [N,h,w,1]), contiguous, on a CUDA device, with h <= H and w <= W
+    -> (its nat.INPUT_* format, h, w)."""
     if x.dtype == torch.float32:
-        fmt, ok = nat.INPUT_F32_NCHW, x.dim() == 4 and x.shape[1] == 3
+        fmt, ok = nat.INPUT_F32_NCHW, x.dim() == 4 and x.shape[1] == channels
         h, w = (x.shape[2], x.shape[3]) if ok else (0, 0)
     elif x.dtype == torch.uint8:
-        fmt, ok = nat.INPUT_U8_NHWC, x.dim() == 4 and x.shape[3] == 3
+        fmt, ok = nat.INPUT_U8_NHWC, x.dim() >= 3 and _u8_shape_ok(tuple(x.shape), x.shape[0], x.shape[1], x.shape[2], channels)
         h, w = (x.shape[1], x.shape[2]) if ok else (0, 0)
     else:
         raise TypeError('input must be float32 NCHW or uint8 NHWC, got %s' % (x.dtype,))
@@ -147,13 +158,13 @@ def fold_scale(weight, scale):
 
 
 def pack_stem_weight(weight, dtype=torch.bfloat16):
-    """[Cout, 3, 3, 3] float -> bf16 [kh][2][Cout][8]: element (kh, kc, n, j) is the weight of output n for input channel
-    j % 4 and filter column kw = 2*kc + j // 4 (zero for kw = 3 and for the padded 4th channel) -- the B operand of the stem
+    """[Cout, Cin, 3, 3] float (Cin = 3, or 1 for a gray image) -> bf16 [kh][2][Cout][8]: element (kh, kc, n, j) is the weight of output n
+    for input channel j % 4 and filter column kw = 2*kc + j // 4 (zero for kw = 3 and for channels >= Cin) -- the B operand of the stem
     conv, whose K runs over the 4 pixels x 4 channels that follow a filter row's first input pixel (conv_umma.cu, kStem*)."""
-    cout = weight.shape[0]
+    cout, cin = weight.shape[0], weight.shape[1]
     w = weight.detach().float().cpu()                      # [n, ci, kh, kw]
     full = torch.zeros(3, 4, 4, cout)                      # [kh, pixel, channel, n]
-    full[:, :3, :3, :] = w.permute(2, 3, 1, 0)
+    full[:, :3, :cin, :] = w.permute(2, 3, 1, 0)
     return full.reshape(3, 2, 8, cout).permute(0, 1, 3, 2).contiguous().to(dtype)
 
 
@@ -324,12 +335,12 @@ class InferencePlan(object):
                 and ((conv.out_channels in (32, 64) and c2.out_channels in (32, 64, 128)) or (conv.out_channels == 48 and c2.out_channels == 48)))
 
     def _emit_stem0(self, conv, norm, relu, out_name, h, w, tail=None):
-        if conv.in_channels != 3 or conv.kernel_size != (3, 3) or conv.stride != (2, 2):
-            raise NotImplementedError('the H100 stem kernel handles the 3x3/s2 conv on a 3-channel image only')
+        if conv.in_channels not in (1, 3) or conv.kernel_size != (3, 3) or conv.stride != (2, 2):
+            raise NotImplementedError('the H100 stem kernel handles the 3x3/s2 conv on a 3-channel (BGR) or 1-channel (gray) image only')
         ho, wo = conv_out(h, 3, 2), conv_out(w, 3, 2)
         scale, shift = self._fold(conv, norm)
         wt = pack_stem_weight(fold_scale(conv.weight, scale), self.tdtype)
-        op = dict(kind=nat.OP_STEM0, H=h, W=w, Cin=3, Ho=ho, Wo=wo, Cout=conv.out_channels, ksize=3, stride=2, relu=int(relu),
+        op = dict(kind=nat.OP_STEM0, H=h, W=w, Cin=conv.in_channels, Ho=ho, Wo=wo, Cout=conv.out_channels, ksize=3, stride=2, relu=int(relu),
                   w_bf16=self._add_bf16(wt), shift=self._add_f32(shift), modules=(conv, norm))
         if tail is not None:
             op.update(self._tail_fields(tail, conv.out_channels))
@@ -344,7 +355,7 @@ class InferencePlan(object):
         return 50 << 20          # H100 SXM, as the 132-SM fallback assumes an H100
 
     def _use_stem4(self, layers):
-        """A 'faster' stem (3x3/s2 3->64, 1x1, 3x3/s2 64->64, 1x1, all 64 channels) runs as one kernel when its stem1 map -- the
+        """A 'faster' stem (3x3/s2 3->64 or 1->64, 1x1, 3x3/s2 64->64, 1x1, all 64 channels) runs as one kernel when its stem1 map -- the
         tensor the fusion keeps out of HBM -- would not stay in L2 between the two fused pairs (more than half of it).  Smaller
         plans have no HBM round trip to remove and keep the two-kernel path."""
         if not self.fuse or self.fuse_stem is False or len(layers) != 4:
@@ -354,8 +365,8 @@ class InferencePlan(object):
         def conv3s2(c, cin):
             return (c.in_channels == cin and c.out_channels == 64 and c.kernel_size == (3, 3) and c.stride == (2, 2)
                     and c.padding == (1, 1) and c.groups == 1 and c.dilation == (1, 1))
-        if not (conv3s2(c0, 3) and conv3s2(c2, 64) and self._can_tail(c0, layers[1]) and self._can_tail(c2, layers[3])
-                and c1.out_channels == 64 and c3.out_channels == 64):
+        if not (c0.in_channels in (1, 3) and conv3s2(c0, c0.in_channels) and conv3s2(c2, 64) and self._can_tail(c0, layers[1])
+                and self._can_tail(c2, layers[3]) and c1.out_channels == 64 and c3.out_channels == 64):
             return False
         if self.fuse_stem:
             return True
@@ -369,7 +380,7 @@ class InferencePlan(object):
         s0, b0 = self._fold(c0, n0)
         s2, b2 = self._fold(c2, n2)
         s3, b3 = self._fold(c3, n3)
-        op = dict(kind=nat.OP_STEM4, H=h, W=w, Cin=3, Ho=ho, Wo=wo, Cout=64, ksize=3, stride=2, relu=int(r0),
+        op = dict(kind=nat.OP_STEM4, H=h, W=w, Cin=c0.in_channels, Ho=ho, Wo=wo, Cout=64, ksize=3, stride=2, relu=int(r0),
                   w_bf16=self._add_bf16(pack_stem_weight(fold_scale(c0.weight, s0), self.tdtype)), shift=self._add_f32(b0), modules=(c0, n0),
                   s2_w=self._add_bf16(pack_conv_weight(fold_scale(c2.weight, s2), 64, self.tdtype)), s2_shift=self._add_f32(b2), s2_relu=int(r2),
                   s2_modules=(c2, n2),
@@ -423,6 +434,7 @@ class InferencePlan(object):
     # ------------------------------------------------------------------ graph walk
     def _emit_stem(self, layers, h, w):
         """The stem on the image -> (name of its output, h, w)."""
+        self.in_channels = layers[0][0].in_channels
         cur = None
         i = 0
         if self._use_stem4(layers):
@@ -684,7 +696,7 @@ class InferencePlan(object):
         if self.handle is None:
             raise nat.LfdError('this plan was built for host-side inspection only (create_native=False)')
         if x is None:
-            x = torch.zeros((self.N, self.H, self.W, 3), dtype=torch.uint8, device=self.device)
+            x = torch.zeros(self.u8_shape(self.H, self.W), dtype=torch.uint8, device=self.device)
         lib = nat.lib()
 
         def measure(caps):
@@ -778,14 +790,19 @@ class InferencePlan(object):
 
     def staging(self, fmt):
         """The plan-owned input of frames below the capacity, in the capacity layout of format fmt (uint8 [N,H,W,3], float32 [N,3,H,W] or
-        NV12 uint8 [N,3H/2,W])."""
+        NV12 uint8 [N,3H/2,W]; a gray plan: uint8 [N,H,W], float32 [N,1,H,W] or the same NV12 layout)."""
+        c = self.in_channels
         if self._stage is None:
             self._stage = torch.empty(self.N * 3 * self.H * self.W * 4, dtype=torch.uint8, device=self.device)
         if fmt == nat.INPUT_U8_NHWC:
-            return self._stage[:self.N * self.H * self.W * 3].view(self.N, self.H, self.W, 3)
+            return self._stage[:self.N * self.H * self.W * c].view(self.u8_shape(self.H, self.W))
         if fmt == nat.INPUT_U8_NV12:
             return self._stage[:self.N * self.H * self.W * 3 // 2].view(self.N, self.H * 3 // 2, self.W)
-        return self._stage.view(torch.float32).view(self.N, 3, self.H, self.W)
+        return self._stage.view(torch.float32)[:self.N * c * self.H * self.W].view(self.N, c, self.H, self.W)
+
+    def u8_shape(self, h, w):
+        """The shape of N uint8 frames of h x w on this plan: [N,h,w,3] (BGR) or [N,h,w] (gray)."""
+        return (self.N, h, w, 3) if self.in_channels == 3 else (self.N, h, w)
 
     def num_graphs(self):
         return nat.lib().lfd_plan_num_graphs(self.handle)
@@ -793,7 +810,8 @@ class InferencePlan(object):
     def forward(self, x, use_graph=True, slot=0, frame_format=None):
         """x: cuda float32 [N,3,h,w] (contiguous) or uint8 [N,h,w,3] with h <= H and w <= W; with frame_format='nv12', NV12 video frames
         uint8 [N,3h/2,w] of even h and w (include/lfd_b200.h, LFD_INPUT_U8_NV12), which give bit for bit what the uint8 path gives on
-        cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12).  Returns the frame's (cls, reg) in the
+        cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12).  A gray plan (in_channels 1) takes float32 [N,1,h,w] or uint8 [N,h,w] / [N,h,w,1], and
+        reads only the Y plane of NV12 frames: the uint8 path on cv2.cvtColor(frame, cv2.COLOR_YUV2GRAY_NV12).  Returns the frame's (cls, reg) in the
         plan-owned buffers of output `slot` (a second slot lets the post-process of one batch overlap the forward of the next,
         lfd/pipeline.py): (N, P, C') and (N, P, 4) for the frame's P points, laid out as a plan built for h x w lays them out;
         frame_level_sizes / frame_P describe them.  A frame of the full size is read in place; a smaller one is first copied into the
@@ -801,7 +819,9 @@ class InferencePlan(object):
         if self.handle is None:
             raise nat.LfdError('this plan was built for host-side inspection only (create_native=False)')
         if frame_format is None:
-            fmt, h, w = check_frame(x, self.N, self.H, self.W)
+            fmt, h, w = check_frame(x, self.N, self.H, self.W, self.in_channels)
+            if fmt == nat.INPUT_U8_NHWC and self.in_channels == 1:
+                x = x.view(self.N, h, w)
         elif frame_format == 'nv12':
             fmt, (h, w) = nat.INPUT_U8_NV12, check_nv12_frame(x, self.N, self.H, self.W)
         else:

@@ -26,7 +26,7 @@ import torch
 import torch.nn as nn
 
 from . import _native as nat
-from ._engine import PrefixEmitter, _Arena, check_input, conv_out, level_geometry, place_tensors, tune_branch_bounds
+from ._engine import PrefixEmitter, _Arena, check_input, conv_out, image_channels, level_geometry, place_tensors, tune_branch_bounds
 
 __all__ = ['FlatParameters', 'TrainPlan', 'train_forward']
 
@@ -119,6 +119,7 @@ class TrainPlan(object):
         self.N, self.H, self.W, self.device = N, H, W, device
         self.model = model
         self.input_transform = getattr(model, 'input_transform', None)    # of uint8 batches: the stem conv, its weight gradient, the frozen prefix's stem
+        self.in_channels = image_channels(model)         # 3: BGR batches, 1: gray (float32 [N,1,H,W] / uint8 [N,H,W])
         self.create_native = create_native               # False: host-side planning only (CPU tests of the planner)
         self.flat = flat_parameters(model, allow_cpu=not create_native)
         self._off, self._top = {}, 256                  # workspace regions: name -> byte offset
@@ -183,8 +184,10 @@ class TrainPlan(object):
         """fp32 staging [k*k][Cin][Cout] of a conv's weight gradient (shared by every use of the parameter)."""
         key = id(conv.weight)
         if key not in self._gstage:
-            # (the stem conv's staging has 32 rows: its tensor-core path pads the 27 (tap, ci) rows to a 32-channel 1x1 problem)
-            name = self._alloc('g%d' % len(self._gstage), (conv.weight.numel() if conv.in_channels != 3 else 32 * conv.out_channels) * 4)
+            # (the stem conv's staging has 32 rows: its tensor-core path pads the 27 (tap, ci) rows -- 9 on a gray image -- to a 32-channel
+            # 1x1 problem)
+            stem = conv.in_channels in (1, 3)
+            name = self._alloc('g%d' % len(self._gstage), (32 * conv.out_channels if stem else conv.weight.numel()) * 4)
             self._gstage[key] = name
             self._zero_bwd.append(name)
             kk = conv.kernel_size[0] ** 2
@@ -769,7 +772,7 @@ class TrainPlan(object):
 
     # ------------------------------------------------------------------ execution
     def forward(self, x, use_graph=False):
-        fmt = check_input(x, self.N, self.H, self.W, contiguous=False)
+        fmt = check_input(x, self.N, self.H, self.W, contiguous=False, channels=self.in_channels)
         # the backward reads the image again (stem weight gradient): keep it in a plan-owned buffer with a fixed address
         if self._input is None or self._input.dtype != x.dtype:
             self._input = torch.empty_like(x, memory_format=torch.contiguous_format)
@@ -803,7 +806,7 @@ class TrainPlan(object):
         grad = self.flat.grad.clone() if self.flat.grad is not None else None
         outs = [t.clone() for t in (self.cls_out, self.reg_out, self.gcls, self.greg)]
         if self._input is None:
-            self._input = torch.zeros((self.N, self.H, self.W, 3), dtype=torch.uint8, device=dev)
+            self._input = torch.zeros((self.N, self.H, self.W, 3) if self.in_channels == 3 else (self.N, self.H, self.W), dtype=torch.uint8, device=dev)
             self._fmt = nat.INPUT_U8_NHWC
         tuned = (nat.TOP_CONV, nat.TOP_WGRAD)
         result = {}

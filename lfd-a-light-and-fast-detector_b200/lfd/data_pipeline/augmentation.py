@@ -130,12 +130,27 @@ InputTransform = collections.namedtuple('InputTransform', 'swap_rb mean scale')
 __all__ += ['InputTransform', 'input_transform_of']
 
 
-def input_transform_of(pipeline, allow_flip=False):
-    """pipeline -> the InputTransform the stem kernels run in its place; None -> None (the kernels' default, simple_normalize on BGR); an
+def _gray_transform(swap, mean, scale):
+    """The transform of a gray (1-channel) model: (byte - mean) * scale with no channel swap, kept as three equal constants, which is what
+    the library takes for a 1-channel image (include/lfd_b200.h).  BGR2RGB, or unequal per-channel constants, have no meaning on one channel."""
+    mean, scale = tuple(float(v) for v in numpy.atleast_1d(mean)), tuple(float(v) for v in numpy.atleast_1d(scale))
+    if swap:
+        raise ValueError('a gray (1-channel) model has no channel order: BGR2RGB cannot run on its input')
+    if len(set(mean)) != 1 or len(set(scale)) != 1:
+        raise ValueError('a gray (1-channel) model takes a Normalize with one constant or three equal ones (got mean %r, scale %r)' % (mean, scale))
+    return InputTransform(False, (mean[0],) * 3, (scale[0],) * 3)
+
+
+def input_transform_of(pipeline, allow_flip=False, channels=3):
+    """pipeline -> the InputTransform the stem kernels run in its place; None -> None (the kernels' default, simple_normalize); an
     InputTransform is returned as it is.  Raises ValueError for a pipeline Compose.device_spec() cannot express, and for one with a
-    HorizontalFlip unless allow_flip (the training loader, whose input kernel does the flip before the stem sees the batch)."""
-    if pipeline is None or isinstance(pipeline, InputTransform):
-        return pipeline
+    HorizontalFlip unless allow_flip (the training loader, whose input kernel does the flip before the stem sees the batch).
+    channels=1: the transform of a gray model's one channel -- a final Normalize with one constant or three equal ones, no BGR2RGB
+    (ValueError otherwise)."""
+    if pipeline is None:
+        return None
+    if isinstance(pipeline, InputTransform):
+        return pipeline if channels == 3 else _gray_transform(pipeline.swap_rb, pipeline.mean, pipeline.scale)
     spec = pipeline_device_spec(pipeline, False)
     if spec is None:
         raise ValueError('the stem kernels cannot run this pipeline on uint8 frames: it must be a Compose (or a function that picks one by the '
@@ -143,6 +158,8 @@ def input_transform_of(pipeline, allow_flip=False):
     flip_p, swap, mean, scale = spec
     if flip_p is not None and not allow_flip:
         raise ValueError('the stem kernels cannot run a HorizontalFlip (p = %g): the input transform is a channel swap and a normalisation' % flip_p)
+    if channels == 1:
+        return _gray_transform(swap, mean, scale)
     return InputTransform(bool(swap), tuple(float(v) for v in mean), tuple(float(v) for v in scale))
 
 

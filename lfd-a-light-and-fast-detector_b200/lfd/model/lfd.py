@@ -148,9 +148,12 @@ class LFD(nn.Module):
         Normalize, or a function that picks such a Compose by the sample's keys), e.g. the TrafficLight val_pipeline or
         typical_coco_val_pipeline.  The kernels then build, per pixel, the 16-bit rounding of the very fp32 number the pipeline produces
         on the host, so uint8 frames give the results of the float32 NCHW batch the pipeline makes of them.  Raises ValueError for a
-        pipeline the kernels cannot run (a flip, another transform, an opaque function).  float32 input is unaffected."""
+        pipeline the kernels cannot run (a flip, another transform, an opaque function).  float32 input is unaffected.  A gray model (a
+        1-channel stem conv) takes None or a final Normalize with one constant or three equal ones, and raises ValueError for BGR2RGB or
+        unequal constants."""
         from ..data_pipeline.augmentation import input_transform_of
-        self.input_transform = input_transform_of(pipeline)
+        from .._engine import image_channels
+        self.input_transform = input_transform_of(pipeline, channels=image_channels(self))
 
     def train_plan_for(self, n, h, w, device):
         """The native training plan (forward + backward op lists) for one input shape (built on first use)."""
@@ -194,7 +197,7 @@ class LFD(nn.Module):
 
     def forward(self, x):
         """x: float32 [N,3,H,W] (reference contract) or uint8 [N,H,W,3] BGR (channel order and normalisation fused into the stem kernel:
-        set_input_transform), on CUDA.
+        set_input_transform), on CUDA.  A gray model (input_channels=1) takes float32 [N,1,H,W] or uint8 [N,H,W] / [N,H,W,1].
         -> (classification [N,P,C'], regression [N,P,4]) float32."""
         if not x.is_cuda:
             raise RuntimeError('lfd_b200 has no CPU path: move the model and the input to a CUDA (H100) device')
@@ -535,7 +538,9 @@ class LFD(nn.Module):
         own set_input_transform setting, by default simple_normalize, augmentation_pipeline.py:31-36), or BGR2RGB / a final Normalize of
         the declarative stand-ins.  The image then goes to the device as it is, 3 bytes per pixel, and is normalised inside the stem
         kernel to the same 16-bit values, so the rows are those of the host path.  Any other pipeline or image is processed on the host
-        exactly like the reference does."""
+        exactly like the reference does.
+        A gray model (input_channels=1) takes a uint8 HxW image (what cv2.imread(path, IMREAD_UNCHANGED) gives for a gray file), or HxWx1,
+        on the fused path only: a pipeline it cannot run, or an image of another shape or type, raises ValueError (no colour conversion)."""
         assert isinstance(image, str) or isinstance(image, numpy.ndarray)
         if isinstance(image, str):
             import cv2
@@ -543,12 +548,20 @@ class LFD(nn.Module):
             assert image is not None, 'image is None, confirm that the path is valid!'
         device = torch.device('cuda', cuda_device_index)
         from ..data_pipeline.augmentation import input_transform_of
-        fusable = image.dtype == numpy.uint8 and image.ndim == 3 and image.shape[2] == 3
+        from .._engine import image_channels
+        gray = image_channels(self) == 1
+        if gray:
+            if image.dtype != numpy.uint8 or not (image.ndim == 2 or (image.ndim == 3 and image.shape[2] == 1)):
+                raise ValueError('a gray (1-channel) model takes a uint8 HxW image, got %s %s' % (image.dtype, image.shape))
+            image = image.reshape(image.shape[0], image.shape[1])
+        fusable = image.dtype == numpy.uint8 and (gray or (image.ndim == 3 and image.shape[2] == 3))
         transform = self.input_transform
         if aug_pipeline is not None and fusable:
             try:
-                transform = input_transform_of(aug_pipeline)
+                transform = input_transform_of(aug_pipeline, channels=1 if gray else 3)
             except ValueError:
+                if gray:
+                    raise
                 fusable = False
         if aug_pipeline is None or fusable:
             if not fusable:

@@ -7,6 +7,7 @@ forward of batch i+1.  This is the serving-side
 counterpart of the reference's `predict_for_single_image` (lfd/model/lfd.py:544-655), which moves one image at a time
 and synchronises after every stage.
 """
+import math
 import os
 import torch
 
@@ -89,14 +90,20 @@ class StreamingDetector(object):
         val_pipeline.  A pipeline the kernels cannot run raises ValueError here: frames are never normalised other than asked.
         frame_format: 'bgr' -- host frames uint8 [N,H,W,3]; 'nv12' -- NV12 video frames uint8 [N,3H/2,W] (H and W even), half the bytes
         to copy, converted to BGR inside the stem kernel bit for bit as cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12) would, after which
-        input_pipeline applies as it does to BGR frames."""
-        if frame_format not in ('bgr', 'nv12'):
-            raise ValueError("frame_format must be 'bgr' or 'nv12', got %r" % (frame_format,))
+        input_pipeline applies as it does to BGR frames; 'gray' -- uint8 [N,H,W], for a gray model (a 1-channel stem conv).  A gray model
+        takes 'gray' or 'nv12', of which it reads the Y plane only (cv2.COLOR_YUV2GRAY_NV12), and raises ValueError for 'bgr'; a BGR model
+        raises ValueError for 'gray'."""
+        from ._engine import image_channels
+        if frame_format not in ('bgr', 'nv12', 'gray'):
+            raise ValueError("frame_format must be 'bgr' or 'nv12' ('gray' for a gray model), got %r" % (frame_format,))
         if frame_format == 'nv12' and (height % 2 or width % 2):
             raise ValueError('NV12 frames have an even height and width, got %dx%d' % (height, width))
+        gray = image_channels(model) == 1
+        if gray != (frame_format == 'gray') and frame_format != 'nv12':
+            raise ValueError("a %s model takes frame_format '%s' or 'nv12', got %r" % ('gray' if gray else 'BGR', 'gray' if gray else 'bgr', frame_format))
         self.frame_format = frame_format
         from .data_pipeline.augmentation import input_transform_of
-        self.input_transform = input_transform_of(input_pipeline)
+        self.input_transform = input_transform_of(input_pipeline, channels=1 if gray else 3)
         self.model = model
         self.depth = max(2, int(depth))     # batches in flight: copy of i+2 | forward of i+1 | post-process + read-back of i
         self.device = device if device is not None else next(model.parameters()).device
@@ -123,7 +130,7 @@ class StreamingDetector(object):
         self.post.set_meta([width] * batch, [height] * batch, [1.0] * batch)
         nv12 = frame_format == 'nv12'
         self.pipe = ForwardPostPipeline(model, self.plan, self.post, self.score_thr, self.iou_thr, frame_format='nv12' if nv12 else None)
-        frame_shape = (batch, height * 3 // 2, width) if nv12 else (batch, height, width, 3)
+        frame_shape = (batch, height * 3 // 2, width) if nv12 else self.plan.u8_shape(height, width)
         self.slots = []
         for _ in range(self.depth):
             self.slots.append(dict(
@@ -133,11 +140,11 @@ class StreamingDetector(object):
                 out_count=torch.empty((batch + 1,), dtype=torch.int32).pin_memory(),
                 h2d=torch.cuda.Event(), h2d_aux=[torch.cuda.Event() for _ in self.copy_streams[1:]], done=torch.cuda.Event(), busy=False))
         self.step = 0
-        self.h2d_bytes = batch * height * width * 3 // (2 if nv12 else 1)
+        self.h2d_bytes = math.prod(frame_shape)
         self.d2h_bytes = batch * self.max_out * (5 * 4 + 4) + (batch + 1) * 4
 
     def submit(self, frames_u8):
-        """frames_u8: pinned (or pageable) host uint8 [N,H,W,3] (frame_format 'nv12': [N,3H/2,W]).  Enqueues copy + compute; returns the
+        """frames_u8: pinned (or pageable) host uint8 [N,H,W,3] (frame_format 'nv12': [N,3H/2,W]; 'gray': [N,H,W]).  Enqueues copy + compute; returns the
         slot index."""
         s = self.slots[self.step % self.depth]
         if s['busy']:
