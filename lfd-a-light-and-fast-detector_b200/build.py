@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 OUT = os.environ.get('LFD_B200_OUT') or os.path.join(HERE, 'liblfd_b200.so')      # LFD_B200_OUT / LFD_B200_EXTRA_FLAGS: tuning experiments only
 SOURCES = ['api.cu', 'conv_umma.cu', 'conv_simt.cu', 'postprocess.cu', 'losses.cu', 'train.cu', 'wgrad_umma.cu', 'input.cu']
-HEADERS = ['ptx.cuh', 'conv_common.cuh', 'kernels.cuh', 'train.cuh', os.path.join('..', '..', 'include', 'lfd_b200.h')]
+HEADERS = ['ptx.cuh', 'image.cuh', 'conv_common.cuh', 'kernels.cuh', 'train.cuh', os.path.join('..', '..', 'include', 'lfd_b200.h')]
 INCLUDE = os.path.join(os.path.dirname(HERE), 'include')
 # the C program that runs a model file through the library and cudart alone (include/lfd_b200.h, lfd_engine_*), built next to the library
 EXAMPLE = os.path.join(os.path.dirname(HERE), 'examples', 'lfd_detect.c')

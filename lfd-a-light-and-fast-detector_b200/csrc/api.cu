@@ -407,6 +407,14 @@ static int plan_op(const lfd_op& o, PlannedOp* out) {
     return LFD_OK;
 }
 
+// The image a stem op reads: its format, its op's channel count and resolved transform.  fp32 planes are taken as they are, in the
+// order they lie: the transform and its channel swap apply to uint8 input only.
+static ImageIn image_in(const void* input, int format, int cin, int H, int W, const InputTransform& xf) {
+    ImageIn img = {input, format, cin, H, W, xf};
+    if (format == LFD_INPUT_F32_NCHW) img.xf.swap = 0;
+    return img;
+}
+
 // ext: null, or this op's row of a plan's device geometry table (lfd_plan_forward_extent), which the kernel reads when it starts
 static int launch_op(const PlannedOp& po, size_t index, const void* input, int input_format, uint8_t* ws, float* cls, float* reg, int P,
                      int cls_channels, int conv_impl, cudaStream_t st, const lfd_extent* ext = nullptr) {
@@ -420,16 +428,14 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
             if (conv_impl == LFD_CONV_SIMT) {
                 if (o.tail_cout) return fail(LFD_ERR_UNSUPPORTED, "the SIMT cross-check kernels do not implement fused tails");
                 Stem0Params p;
-                p.in = input; p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off);
+                p.img = image_in(input, input_format, o.Cin, o.H, o.W, po.xf);
+                p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off);
                 p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift;
-                p.input_format = input_format; p.Cin = o.Cin; p.N = o.N; p.H = o.H; p.W = o.W; p.Ho = o.Ho; p.Wo = o.Wo; p.Cout = o.Cout; p.relu = o.relu; p.f16 = o.dtype;
-                p.xf = po.xf;
+                p.N = o.N; p.Ho = o.Ho; p.Wo = o.Wo; p.Cout = o.Cout; p.relu = o.relu; p.f16 = o.dtype;
                 CUDA_TRY(stem0_launch(p, st));
             } else {
                 UmmaConvParams p = po.cp;
-                p.in_raw = input; p.input_format = input_format; p.in_ch = o.Cin; p.in = nullptr;
-                p.xf = po.xf;
-                if (input_format == LFD_INPUT_F32_NCHW) p.xf.swap = 0;   // the loaders order the channels at the load: fp32 planes are taken as they are
+                p.img = image_in(input, input_format, o.Cin, o.H, o.W, po.xf); p.in = nullptr;
                 p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off); p.res = nullptr;
                 p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift; p.stats = nullptr;
                 p.relu = o.relu; p.gn_groups = 0; p.trace = g_trace; p.tl = tl; p.f16 = o.dtype;
@@ -444,9 +450,7 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
             if (!input) return fail(LFD_ERR_INVALID, "stem4 needs the external input pointer");
             if (conv_impl == LFD_CONV_SIMT) return fail(LFD_ERR_UNSUPPORTED, "the SIMT cross-check kernels do not implement the fused stem (plan its four convs)");
             UmmaConvParams p = po.cp;
-            p.in_raw = input; p.input_format = input_format; p.in_ch = o.Cin; p.in = nullptr;
-            p.xf = po.xf;
-            if (input_format == LFD_INPUT_F32_NCHW) p.xf.swap = 0;
+            p.img = image_in(input, input_format, o.Cin, o.H, o.W, po.xf); p.in = nullptr;
             // the word loader: rows of whole aligned words (BGR: 3 words per 4 pixels; gray: 1 word per 4 pixels; NV12: a Y word and a UV
             // word, its image pitch H * W * 3 / 2 then being a multiple of 4 as well, since H is even)
             p.in_words = input_format != LFD_INPUT_F32_NCHW && o.W % 4 == 0 && (reinterpret_cast<uintptr_t>(input) & 3) == 0;
@@ -1193,15 +1197,16 @@ static int launch_top(const PlannedTop& pt, const void* input, int fmt, uint8_t*
         case LFD_TOP_WGRAD_STEM: {
             WgradGeom g = {t.N, t.H, t.W, t.Cin, t.Ho, t.Wo, t.Cout, t.ksize, t.stride};
             if (!input || t.off[1] < 0 || t.off[5] < 0) return fail(LFD_ERR_INVALID, "wgrad_stem: missing tensor");
+            const ImageIn img = image_in(input, fmt, t.Cin, t.H, t.W, pt.conv.xf);
             if (t.off[0] >= 0 && t.impl == LFD_WGRAD_UMMA) {
                 // tensor-core path: im2col into the scratch tensor X27 [N][Ho][Wo][32] at off[0], then the 1x1 wgrad (32 -> Cout) over it;
                 // the staging at off[5] must hold 32 rows of Cout floats (rows 27..31 stay zero)
                 __nv_bfloat16* x27 = at<__nv_bfloat16>(ws, t.off[0]);
-                CUDA_TRY(stem_im2col_launch(g, input, fmt, pt.conv.xf, x27, sms, st));
+                CUDA_TRY(stem_im2col_launch(g, img, x27, sms, st));
                 WgradGeom g1 = {t.N, t.Ho, t.Wo, 32, t.Ho, t.Wo, t.Cout, 1, 1};
                 CUDA_TRY(wgrad_umma_launch(g1, x27, at<const __nv_bfloat16>(ws, t.off[1]), at<float>(ws, t.off[5]), sms, st));
             } else {
-                CUDA_TRY(wgrad_stem_launch(g, input, fmt, pt.conv.xf, at<const __nv_bfloat16>(ws, t.off[1]), at<float>(ws, t.off[5]), sms, st));
+                CUDA_TRY(wgrad_stem_launch(g, img, at<const __nv_bfloat16>(ws, t.off[1]), at<float>(ws, t.off[5]), sms, st));
             }
             break;
         }

@@ -20,18 +20,6 @@ static constexpr int kSmemTableOff = 512;    // first per-layer region
 // from there, at offsets chosen per layer (UmmaConvParams::smem_*_off): halo pixel table (modes that need it), the fp32 shifts
 // of the conv and of the fused tail, then the 1024-byte aligned staging regions [warpgroup][buffer]
 
-// LFD_INPUT_U8_NV12: the three bytes (B, G, R) of a pixel from its Y byte and the (U, V) pair of its 2x2 block -- BT.601 limited
-// range in 20-bit fixed point, bit for bit what cv2.cvtColor(f, COLOR_YUV2BGR_NV12) gives.  The only code that knows the constants:
-// every loader of an NV12 frame calls it, then applies the input transform to the bytes as it does to BGR bytes.
-__host__ __device__ __forceinline__ uint32_t nv12_sat8(int v) { return (uint32_t)(v < 0 ? 0 : v > 255 ? 255 : v); }
-__host__ __device__ __forceinline__ void nv12_to_bgr(uint32_t Y, uint32_t U, uint32_t V, uint32_t bgr[3]) {
-    const int y = ((int)Y > 16 ? (int)Y - 16 : 0) * 1220542 + (1 << 19);     // max(0, Y - 16) * 1220542 + the rounding half
-    const int u = (int)U - 128, v = (int)V - 128;
-    bgr[0] = nv12_sat8((y + 2116026 * u) >> 20);                           // arithmetic shifts
-    bgr[1] = nv12_sat8((y - 852492 * v - 409993 * u) >> 20);
-    bgr[2] = nv12_sat8((y + 1673527 * v) >> 20);
-}
-
 struct ConvGeom {
     int N, H, W, Cin, Ho, Wo, Cout, ksize, stride;
     int tail_cout;   // > 0: a 1x1/s1 conv (Cout -> tail_cout) is fused behind this conv (second GEMM in the same kernel)
@@ -48,7 +36,6 @@ struct alignas(64) UmmaConvParams {
     int solo;                   // 1: conv_umma_solo_kernel (one consumer warpgroup per tile, see umma_conv_configure)
     const __nv_bfloat16* in;
     __nv_bfloat16* out;
-    const void* in_raw;         // MODE_STEM: the image, fp32 NCHW (input_format 0) or uint8 NHWC (1)
     const __nv_bfloat16* res;   // optional residual (same shape as out)
     const __nv_bfloat16* w;     // packed [cc][tap][kc][Cout][8]
     const float* shift;         // [Cout] fp32 or null; rounded to the 16-bit type and added to the accumulator (BatchNorm scale is folded into w)
@@ -75,9 +62,7 @@ struct alignas(64) UmmaConvParams {
     uint32_t a_stage_bytes, b_slice_bytes, stage_bytes, w_total_bytes;
     uint32_t smem_table_off, smem_bias_off, smem_bias2_off, smem_staging_off;
     uint32_t smem_w_off, smem_ring_off;
-    int input_format;
-    int in_ch;                  // MODE_STEM / MODE_STEM4: channels of the image, 3 (BGR) or 1 (gray: the loaders write (v, 0, 0, 0), see kStem*)
-    InputTransform xf;          // MODE_STEM / MODE_STEM4, u8 NHWC image: byte -> network input (constant bank; xf.swap is 0 for fp32 input)
+    ImageIn img;                // MODE_STEM / MODE_STEM4: the image (read from the constant bank)
     int f16;                    // activation / weight type: 0 = bf16, 1 = IEEE fp16 (same bytes, same tensor-core rate)
     // MODE_STEM4: stem0 = w / shift / relu, stem1 = w2 / shift2 / relu2 (the tail fields), stem2 = its 3x3/s2 weights packed
     // [9][8][64][8] + shift + ReLU, stem3 = its 1x1 weights packed [8][64][8] + shift + ReLU; H1 x W1 = the stem1 map

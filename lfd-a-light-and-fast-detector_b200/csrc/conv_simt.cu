@@ -45,35 +45,21 @@ __global__ void __launch_bounds__(kS0Threads) stem0_kernel(const __grid_constant
         const int kh = k / 9, kw = (k / 3) % 3, ci = k % 3;   // packed [kh][kw / 2][Cout][(kw % 2) * 4 + ci]
         wsm[i] = up_lo_rt((uint32_t)reinterpret_cast<const unsigned short*>(p.w)[(((kh * 2 + (kw >> 1)) * Cout + nn) * 8) + (kw & 1) * 4 + ci], p.f16);
     }
-    // input patch -> smem, rounded to bf16 (rounding point R0 of DESIGN.md)
-    for (int i = tid; i < 3 * kS0PatchH * kS0PatchW; i += kS0Threads) {
-        int ci, r, c;
-        if (p.input_format == 0) {  // fp32 NCHW: x fastest
-            c = i % kS0PatchW; r = (i / kS0PatchW) % kS0PatchH; ci = i / (kS0PatchW * kS0PatchH);
-        } else {                    // u8 NHWC: channel fastest
-            ci = i % 3; c = (i / 3) % kS0PatchW; r = i / (3 * kS0PatchW);
+    // input patch -> smem, rounded to bf16 (rounding point R0 of DESIGN.md); a gray image fills channels 1 and 2 with 0
+    image_dispatch(p.img, [&](auto ch_c, auto fmt_c) {
+        constexpr int CH = decltype(ch_c)::value, FMT = decltype(fmt_c)::value;
+        for (int i = tid; i < kS0PatchH * kS0PatchW; i += kS0Threads) {
+            const int r = i / kS0PatchW, c = i % kS0PatchW;
+            const int y = iy0 + r, x = ix0 + c;
+            const bool inside = y >= 0 && y < p.img.H && x >= 0 && x < p.img.W;
+            uint32_t raw[CH];
+            float f[3];
+            image_load<CH, FMT>(p.img, n, image_px<CH, FMT>(p.img, y, x), y, x, inside, raw);
+            image_decode<CH, FMT>(p.img, raw, inside, f);
+#pragma unroll
+            for (int ci = 0; ci < 3; ++ci) patch[(ci * kS0PatchH + r) * kS0PatchPitch + c] = round16_rt(f[ci], p.f16);
         }
-        const int y = iy0 + r, x = ix0 + c;
-        float v = 0.f;
-        if (y >= 0 && y < p.H && x >= 0 && x < p.W && (ci == 0 || p.Cin == 3)) {   // gray: channel 0 only, channels 1 and 2 are 0
-            if (p.input_format == 0) {
-                v = reinterpret_cast<const float*>(p.in)[(((size_t)n * p.Cin + ci) * p.H + y) * p.W + x];
-            } else if (p.input_format == 2) {   // NV12: Y plane, then the interleaved UV plane at the same pitch
-                const int m = p.xf.swap ? 2 - ci : ci;
-                const size_t plane = (size_t)p.H * p.W;
-                const uint8_t* img = reinterpret_cast<const uint8_t*>(p.in) + (size_t)n * (plane + plane / 2);
-                const uint8_t* uv = img + plane + (size_t)(y >> 1) * p.W + (x & ~1);
-                uint32_t bgr[3] = {img[(size_t)y * p.W + x], 0u, 0u};
-                if (p.Cin == 3) nv12_to_bgr(bgr[0], uv[0], uv[1], bgr);
-                v = p.xf.apply(m, bgr[m]);
-            } else {
-                const int m = p.xf.swap ? 2 - ci : ci;
-                v = p.xf.apply(m, reinterpret_cast<const uint8_t*>(p.in)[(((size_t)n * p.H + y) * p.W + x) * p.Cin + m]);
-            }
-            v = round16_rt(v, p.f16);
-        }
-        patch[(ci * kS0PatchH + r) * kS0PatchPitch + c] = v;
-    }
+    });
     __syncthreads();
     const int g = tid % NG, lp0 = tid / NG;
     float acc[PASSES][8];

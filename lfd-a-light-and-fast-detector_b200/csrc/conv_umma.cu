@@ -664,13 +664,13 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
         if (MODE == MODE_STEM) {
             // Raw image patch -> normalised bf16 [row][pixel][b g r 0] in the ring stage (see kStem* above).  Every thread owns
             // up to 5 patch pixels; the raw values of the NEXT tile are fetched into registers right after the current patch
-            // has been written, so the loads fly while the thread waits for the next free stage.  A gray image (p.in_ch == 1) has
+            // has been written, so the loads fly while the thread waits for the next free stage.  A gray image (p.img.ch == 1) has
             // one value per pixel (fp32 plane, uint8 byte, NV12's Y byte -- its UV plane is never read), written as (v, 0, 0, 0):
             // the body is specialised for it at compile time, so the BGR loaders are exactly what they are without it.
             auto stem_producer = [&](auto gray_c) LFD_LAMBDA_INLINE {
                 constexpr bool gray = decltype(gray_c)::value;
-                const bool u8 = p.input_format != 0;        // uint8 BGR (1) or NV12 (2): bytes, normalised by p.xf
-                const bool nv12 = p.input_format == 2;
+                const bool u8 = p.img.format != 0;        // uint8 BGR (1) or NV12 (2): bytes, normalised by p.img.xf
+                const bool nv12 = p.img.format == 2;
                 const int plane = p.H * p.W;
                 int rel[kStemPerThread];          // source offset of pixel j relative to the patch origin (bytes for BGR, elements for gray / fp32 / NV12's Y)
                 int prc[kStemPerThread];          // (row << 8) | col
@@ -679,7 +679,7 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
                     const int q = min(ptid + j * kProdThreads, kStemPix - 1);
                     const int r = q / kStemCols, c = q - r * kStemCols;
                     prc[j] = (r << 8) | c;
-                    rel[j] = p.input_format == 1 && !gray ? (r * p.W + c) * 3 : r * p.W + c;
+                    rel[j] = p.img.format == 1 && !gray ? (r * p.W + c) * 3 : r * p.W + c;
                 }
                 const bool last_ok = ptid + (kStemPerThread - 1) * kProdThreads < kStemPix;   // this thread owns a pixel in the last round
                 uint32_t raw[kStemPerThread][gray ? 1 : 3];
@@ -693,7 +693,7 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
                     if (nv12) {
                         // raw = (Y, U, V): the Y plane, then the interleaved UV plane at the same pitch, UV row = absolute row / 2 (the patch
                         // starts at an odd row), UV column = x & ~1
-                        const uint8_t* img = reinterpret_cast<const uint8_t*>(p.in_raw) + (size_t)n * (plane + (plane >> 1));
+                        const uint8_t* img = reinterpret_cast<const uint8_t*>(p.img.data) + (size_t)n * (plane + (plane >> 1));
                         const uint8_t* org = img + (ptrdiff_t)iy0 * p.W + ix0;
 #pragma unroll
                         for (int j = 0; j < kStemPerThread; ++j) {
@@ -709,7 +709,7 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
                         }
                     } else if (u8) {
                         const int bpp = gray ? 1 : 3;
-                        const uint8_t* img = reinterpret_cast<const uint8_t*>(p.in_raw) + (size_t)n * plane * bpp;
+                        const uint8_t* img = reinterpret_cast<const uint8_t*>(p.img.data) + (size_t)n * plane * bpp;
                         const uint8_t* org = img + ((ptrdiff_t)iy0 * p.W + ix0) * bpp;
 #pragma unroll
                         for (int j = 0; j < kStemPerThread; ++j) {
@@ -726,7 +726,7 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
                             if constexpr (!gray) { raw[j][1] = __ldg(src + 1); raw[j][2] = __ldg(src + 2); }
                         }
                     } else {
-                        const float* img = reinterpret_cast<const float*>(p.in_raw) + (size_t)n * plane * (gray ? 1 : 3);
+                        const float* img = reinterpret_cast<const float*>(p.img.data) + (size_t)n * plane * (gray ? 1 : 3);
                         const float* org = img + (ptrdiff_t)iy0 * p.W + ix0;
 #pragma unroll
                         for (int j = 0; j < kStemPerThread; ++j) {
@@ -758,7 +758,7 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
                         if (j == kStemPerThread - 1 && !last_ok) break;
                         uint32_t lo, hi;
                         if constexpr (gray) {
-                            float v = u8 ? p.xf.apply(0, raw[j][0]) : __uint_as_float(raw[j][0]);     // NV12: the Y byte as it is
+                            float v = u8 ? p.img.xf.apply(0, raw[j][0]) : __uint_as_float(raw[j][0]);     // NV12: the Y byte as it is
                             if (!((okmask >> j) & 1u)) v = 0.f;                                      // conv zero padding
                             lo = pack2<F16>(v, 0.f); hi = pack2<F16>(0.f, 0.f);                       // rounding point R0
                         } else {
@@ -766,10 +766,10 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
                             float f[3];
 #pragma unroll
                             for (int k = 0; k < 3; ++k) {
-                                f[k] = u8 ? p.xf.apply(k, raw[j][k]) : __uint_as_float(raw[j][k]);
+                                f[k] = u8 ? p.img.xf.apply(k, raw[j][k]) : __uint_as_float(raw[j][k]);
                                 if (!((okmask >> j) & 1u)) f[k] = 0.f;        // conv zero padding (of the normalised image)
                             }
-                            const bool sw = p.xf.swap;           // u8 BGR -> RGB: the normalised bytes 0 and 2 change places
+                            const bool sw = p.img.xf.swap;           // u8 BGR -> RGB: the normalised bytes 0 and 2 change places
                             lo = pack2<F16>(sw ? f[2] : f[0], f[1]); hi = pack2<F16>(sw ? f[0] : f[2], 0.f);   // rounding point R0
                         }
                         asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(dst0 + j * (kProdThreads * 8)), "r"(lo), "r"(hi) : "memory");
@@ -781,7 +781,7 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
                     if (ptid == 0) LFD_TRACE(0, it, 3);
                 }
             };
-            if (p.in_ch == 1) stem_producer(std::true_type());
+            if (p.img.ch == 1) stem_producer(std::true_type());
             else stem_producer(std::false_type());
         } else {
         // every thread owns ONE 16-byte channel chunk (cpc divides 128) and walks the halo pixels with a fixed stride
@@ -1202,15 +1202,10 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
         // ============================================================== PRODUCER: raw image patch -> normalised 16-bit [row][pixel][b g r 0]
         asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
         const int ptid = tid - kConsumerThreads;
-        // A gray image (p.in_ch == 1) has one value per pixel (fp32 plane, uint8 byte, NV12's Y byte -- its UV plane is never read),
-        // written as (v, 0, 0, 0): the body is specialised for it at compile time, so the BGR loaders are exactly what they are without it.
-        auto s4_producer = [&](auto gray_c) LFD_LAMBDA_INLINE {
-            constexpr bool gray = decltype(gray_c)::value;
-            constexpr int kCh = gray ? 1 : 3;    // values (and, for uint8, bytes) per pixel
-            const bool u8 = p.input_format != 0;    // uint8 BGR (1) or NV12 (2): bytes, normalised by p.xf
-            const bool nv12 = p.input_format == 2;
-            const bool sw = p.xf.swap;       // u8 BGR -> RGB: the normalised bytes 0 and 2 of a pixel change places
-            const int plane = p.H * p.W;
+        // A gray image (p.img.ch == 1) has one value per pixel, written as (v, 0, 0, 0): the body is specialised for it and for the format
+        // at compile time (image.cuh), so the BGR loaders are exactly what they are without it.
+        auto s4_producer = [&](auto ch_c, auto fmt_c) LFD_LAMBDA_INLINE {
+            constexpr int CH = decltype(ch_c)::value, FMT = decltype(fmt_c)::value;
             pdl_wait();
             int tile0, tile1;
             s4_run(lg.num_tiles, tile0, tile1);
@@ -1224,16 +1219,15 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                 mbar_wait(&empty[s], ph ^ 1);
                 if (ptid == 0) LFD_TRACE(0, lt, 1);
                 const uint32_t dst0 = smem_u32(smem + kS4Ring) + s * kS4PatchBytes;
-                if (p.in_words) {
-                    // ix0 = 1 (mod 4): group g of a patch row = image columns ix0 - 1 + 4g .. + 3 = patch columns 4g - 1 .. 4g + 2,
-                    // 12 bytes at a 4-byte aligned address (W % 4 == 0; NV12: the Y word and the UV word, both aligned since the image
-                    // pitch H * W * 3 / 2 is then a multiple of 4 too; gray: one word, NV12 gray: the Y word).  A group lies wholly
-                    // inside or wholly outside the tensor, so no load touches a byte outside it; a valid width that is not a multiple
-                    // of 4 ends inside a group, whose pixels past it are zeroed one by one.  Two batches of 3 groups: all loads of a
-                    // batch are issued before any is used (6 groups at once do not fit the producer's 56 registers).
+                if (FMT != LFD_INPUT_F32_NCHW && p.in_words) {
+                    // ix0 = 1 (mod 4): group g of a patch row = image columns ix0 - 1 + 4g .. + 3 = patch columns 4g - 1 .. 4g + 2, whole
+                    // aligned words (image_load_words).  A group lies wholly inside or wholly outside the tensor, so no load touches a byte
+                    // outside it; a valid width that is not a multiple of 4 ends inside a group, whose pixels past it are zeroed one by one.
+                    // Two batches of 3 groups: all loads of a batch are issued before any is used (6 groups at once do not fit the
+                    // producer's 56 registers).
 #pragma unroll 1
                     for (int j0 = 0; j0 < kS4GroupsPerThread; j0 += kS4GroupBatch) {
-                        uint32_t wd[kS4GroupBatch][kCh];
+                        uint32_t wd[kS4GroupBatch][CH];
                         bool ok[kS4GroupBatch];
 #pragma unroll
                         for (int j = 0; j < kS4GroupBatch; ++j) {
@@ -1241,22 +1235,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                             const int r = q / 10, g = q - r * 10;
                             const int y = iy0 + r, x = ix0 - 1 + 4 * g;
                             ok[j] = q < kS4Groups && (unsigned)y < (unsigned)lg.H && (unsigned)x < (unsigned)lg.W;
-                            if (nv12) {
-                                // two words: Y of pixels x .. x + 3 at (y, x), and U0 V0 U1 V1 of their two 2x2 blocks at UV row y / 2, column x
-                                const uint8_t* img = reinterpret_cast<const uint8_t*>(p.in_raw) + (ptrdiff_t)n * (plane + (plane >> 1));
-                                const uint32_t* ys = reinterpret_cast<const uint32_t*>(img + (ptrdiff_t)y * p.W + x);
-                                const uint32_t* uvs = reinterpret_cast<const uint32_t*>(img + plane + (ptrdiff_t)(y >> 1) * p.W + x);
-                                wd[j][0] = ok[j] ? __ldg(ys) : 0u;
-                                if constexpr (!gray) {
-                                    wd[j][1] = ok[j] ? __ldg(uvs) : 0u;
-                                    wd[j][2] = 0u;
-                                }
-                            } else {
-                                const uint32_t* src = reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint8_t*>(p.in_raw) +
-                                                                                        ((ptrdiff_t)n * plane + (ptrdiff_t)y * p.W + x) * kCh);
-#pragma unroll
-                                for (int k = 0; k < kCh; ++k) wd[j][k] = ok[j] ? __ldg(src + k) : 0u;
-                            }
+                            image_load_words<CH, FMT>(p.img, n, y, x, ok[j], wd[j]);
                         }
 #pragma unroll
                         for (int j = 0; j < kS4GroupBatch; ++j) {
@@ -1264,36 +1243,21 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                             if (q >= kS4Groups) break;
                             const int r = q / 10, g = q - r * 10;
                             const int in_cols = lg.W - (ix0 - 1 + 4 * g);    // pixels k < in_cols of the group lie inside the valid width
-                            uint32_t px[4][2];
+                            uint2 px[4];
 #pragma unroll
                             for (int k = 0; k < 4; ++k) {
-                                const bool okk = ok[j] && (!EXT || k < in_cols);
-                                if constexpr (gray) {
-                                    const float v = okk ? p.xf.apply(0, (wd[j][0] >> (8 * k)) & 0xffu) : 0.f;     // zero padding
-                                    px[k][0] = pack2<F16>(v, 0.f);                                              // rounding point R0
-                                    px[k][1] = pack2<F16>(0.f, 0.f);
-                                } else {
-                                    float f[3];
-                                    uint32_t bytes[3];
-                                    if (nv12) {
-                                        nv12_to_bgr((wd[j][0] >> (8 * k)) & 0xffu, (wd[j][1] >> (8 * (k & 2))) & 0xffu,
-                                                    (wd[j][1] >> (8 * (k & 2) + 8)) & 0xffu, bytes);
-                                    } else {
-#pragma unroll
-                                        for (int c = 0; c < 3; ++c) bytes[c] = (wd[j][(3 * k + c) >> 2] >> (8 * ((3 * k + c) & 3))) & 0xffu;
-                                    }
-#pragma unroll
-                                    for (int c = 0; c < 3; ++c) f[c] = okk ? p.xf.apply(c, bytes[c]) : 0.f;     // zero padding of the normalised image
-                                    px[k][0] = pack2<F16>(sw ? f[2] : f[0], f[1]);                           // rounding point R0
-                                    px[k][1] = pack2<F16>(sw ? f[0] : f[2], 0.f);
-                                }
+                                uint32_t raw[CH];
+                                float f[3];
+                                image_unpack_word<CH, FMT>(wd[j], k, raw);
+                                image_decode<CH, FMT>(p.img, raw, ok[j] && (!EXT || k < in_cols), f);
+                                px[k] = pack_px<F16>(f);
                             }
                             const uint32_t d = dst0 + (uint32_t)(r * kS4RowBytes + 32 * g);              // patch column 4g, 16-byte aligned
-                            if (g > 0) asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(d - 8u), "r"(px[0][0]), "r"(px[0][1]) : "memory");
+                            if (g > 0) asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(d - 8u), "r"(px[0].x), "r"(px[0].y) : "memory");
                             if (g < 9) {
-                                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(d), "r"(px[1][0]), "r"(px[1][1]), "r"(px[2][0]),
-                                             "r"(px[2][1]) : "memory");
-                                asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(d + 16u), "r"(px[3][0]), "r"(px[3][1]) : "memory");
+                                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(d), "r"(px[1].x), "r"(px[1].y), "r"(px[2].x),
+                                             "r"(px[2].y) : "memory");
+                                asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(d + 16u), "r"(px[3].x), "r"(px[3].y) : "memory");
                             }
                         }
                     }
@@ -1301,7 +1265,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                     // per-pixel loader: fp32 NCHW, or uint8 (BGR / gray / NV12) rows that are not whole aligned words
 #pragma unroll 1
                     for (int j0 = 0; j0 < kS4PerThread; j0 += kS4Batch) {
-                        uint32_t raw[kS4Batch][kCh];
+                        uint32_t raw[kS4Batch][CH];
                         bool ok[kS4Batch];
 #pragma unroll
                         for (int j = 0; j < kS4Batch; ++j) {
@@ -1309,44 +1273,16 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                             const int r = q / kS4Cols, c = q - r * kS4Cols;
                             const int y = iy0 + r, x = ix0 + c;
                             ok[j] = q < kS4Pix && (interior || ((unsigned)y < (unsigned)lg.H && (unsigned)x < (unsigned)lg.W));
-                            const ptrdiff_t pix = ok[j] ? (ptrdiff_t)n * plane + (ptrdiff_t)y * p.W + x : 0;
-                            if (nv12) {      // (Y, U, V); UV row = absolute row / 2, UV column = x & ~1
-                                const uint8_t* img = reinterpret_cast<const uint8_t*>(p.in_raw) + (ok[j] ? (ptrdiff_t)n * (plane + (plane >> 1)) : 0);
-                                raw[j][0] = __ldg(img + (ok[j] ? (ptrdiff_t)y * p.W + x : 0));
-                                if constexpr (!gray) {
-                                    const uint8_t* uv = img + plane + (ok[j] ? (ptrdiff_t)(y >> 1) * p.W + (x & ~1) : 0);
-                                    raw[j][1] = __ldg(uv); raw[j][2] = __ldg(uv + 1);
-                                }
-                            } else if (u8) {
-                                const uint8_t* src = reinterpret_cast<const uint8_t*>(p.in_raw) + pix * kCh;
-#pragma unroll
-                                for (int k = 0; k < kCh; ++k) raw[j][k] = __ldg(src + k);
-                            } else {
-                                const float* src = reinterpret_cast<const float*>(p.in_raw) + (ok[j] ? (ptrdiff_t)n * (kCh - 1) * plane + pix : 0);
-#pragma unroll
-                                for (int k = 0; k < kCh; ++k) raw[j][k] = __float_as_uint(__ldg(src + k * plane));
-                            }
+                            image_load<CH, FMT>(p.img, n, image_px<CH, FMT>(p.img, y, x), y, x, ok[j], raw[j]);
                         }
 #pragma unroll
                         for (int j = 0; j < kS4Batch; ++j) {
                             const int q = ptid + (j0 + j) * kProdThreads;
                             if (q >= kS4Pix) break;
-                            uint32_t lo, hi;
-                            if constexpr (gray) {
-                                float v = u8 ? p.xf.apply(0, raw[j][0]) : __uint_as_float(raw[j][0]);     // NV12: the Y byte as it is
-                                if (!ok[j]) v = 0.f;                                                     // conv zero padding
-                                lo = pack2<F16>(v, 0.f); hi = pack2<F16>(0.f, 0.f);                       // rounding point R0
-                            } else {
-                                if (nv12) nv12_to_bgr(raw[j][0], raw[j][1], raw[j][2], raw[j]);   // (Y, U, V) -> the bytes (B, G, R)
-                                float f[3];
-#pragma unroll
-                                for (int k = 0; k < 3; ++k) {
-                                    f[k] = u8 ? p.xf.apply(k, raw[j][k]) : __uint_as_float(raw[j][k]);
-                                    if (!ok[j]) f[k] = 0.f;             // conv zero padding (of the normalised image)
-                                }
-                                lo = pack2<F16>(sw ? f[2] : f[0], f[1]); hi = pack2<F16>(sw ? f[0] : f[2], 0.f);   // rounding point R0
-                            }
-                            asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(dst0 + q * 8), "r"(lo), "r"(hi) : "memory");
+                            float f[3];
+                            image_decode<CH, FMT>(p.img, raw[j], ok[j], f);
+                            const uint2 v = pack_px<F16>(f);
+                            asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(dst0 + q * 8), "r"(v.x), "r"(v.y) : "memory");
                         }
                     }
                 }
@@ -1355,8 +1291,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                 if (ptid == 0) LFD_TRACE(0, lt, 2);
             }
         };
-        if (p.in_ch == 1) s4_producer(std::true_type());
-        else s4_producer(std::false_type());
+        image_dispatch(p.img, s4_producer);
     }
     LFD_TL_END(p.tl);
 }

@@ -4,29 +4,19 @@
 #include <cuda_bf16.h>
 #include <stdint.h>
 
+#include "image.cuh"
+
 namespace lfd {
 
 static constexpr int kMaxLevels = 8;
 
-// What every kernel that reads a uint8 NHWC image makes of it: network input channel c of a pixel = apply(m, byte[m]) with
-// m = swap ? 2 - c : c, in fp32 one subtract, then one multiply: albumentations' Normalize after an optional BGR -> RGB, with the constants
-// Normalize itself computes.  mean / scale are indexed by the byte's position m IN MEMORY (api.cu permutes the C-ABI's per-network-channel
-// constants once), so a loader normalises the three bytes where they lie and a swap only exchanges two finished floats.  Pixels outside the
-// image are 0 AFTER this (the conv's zero padding), not the image of byte 0.  The fp32 NCHW input is taken as it is.
-struct InputTransform {
-    int swap;
-    float mean[3], scale[3];
-    __host__ __device__ __forceinline__ float apply(int m, uint32_t byte) const { return ((float)byte - mean[m]) * scale[m]; }
-};
-
 struct Stem0Params {
-    const void* in;            // fp32 NCHW (input_format 0), u8 NHWC (1) or NV12 (2), with Cin = 3 or 1 (gray) channels
+    ImageIn img;
     __nv_bfloat16* out;        // bf16 NHWC
     const __nv_bfloat16* w;    // packed [kh][2][Cout][8]: element (kh, kc, n, j) = weight (n, ci = j % 4, kh, kw = 2 kc + j / 4), 0 for kw = 3 or ci = 3
     const float* shift;        // fp32 [Cout] or null (BatchNorm scale is folded into w); applied as bf16
-    int input_format, Cin, N, H, W, Ho, Wo, Cout, relu;
+    int N, Ho, Wo, Cout, relu;
     int f16;                   // 16-bit type of weights / output: 0 = bf16, 1 = fp16
-    InputTransform xf;         // u8 NHWC input only
 };
 cudaError_t stem0_launch(const Stem0Params& p, cudaStream_t st);
 

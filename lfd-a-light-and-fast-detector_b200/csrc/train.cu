@@ -723,8 +723,8 @@ cudaError_t head_final_bwd_launch(const HeadFinalBwdParams& p, int num_sms, cuda
 // ===================================================================================================
 static constexpr int kWsSeg = 64, kWsCols = 2 * kWsSeg + 1;
 
-__global__ void __launch_bounds__(256) wgrad_stem_kernel(WgradGeom g, const void* __restrict__ image, int input_format, const __grid_constant__ InputTransform xf,
-                                                         const __nv_bfloat16* __restrict__ dz, float* __restrict__ dstage) {
+__global__ void __launch_bounds__(256) wgrad_stem_kernel(WgradGeom g, const __grid_constant__ ImageIn img, const __nv_bfloat16* __restrict__ dz,
+                                                         float* __restrict__ dstage) {
     __shared__ float patch[3][3][kWsCols + 3];   // [ci][kh][column]
     const int Cout = g.Cout;
     const int ngrp = 256 / Cout;                 // (tap, ci) groups
@@ -734,23 +734,25 @@ __global__ void __launch_bounds__(256) wgrad_stem_kernel(WgradGeom g, const void
     for (int i = 0; i < 7; ++i) acc[i] = 0.f;
     const int segs_x = (g.Wo + kWsSeg - 1) / kWsSeg;
     const int n_seg = g.N * g.Ho * segs_x;
-    const size_t plane = (size_t)g.H * g.W;
     const int K = 9 * g.Cin;
     for (int seg = blockIdx.x; seg < n_seg; seg += gridDim.x) {
         const int sx = seg % segs_x, oy = (seg / segs_x) % g.Ho, n = seg / (segs_x * g.Ho);
         const int ox0 = sx * kWsSeg, ix0 = 2 * ox0 - 1, iy0 = 2 * oy - 1;
         __syncthreads();
-        for (int i = threadIdx.x; i < 3 * g.Cin * kWsCols; i += 256) {
-            const int c = i % kWsCols, kh = (i / kWsCols) % 3, ci = i / (3 * kWsCols);
-            const int y = iy0 + kh, x = ix0 + c;
-            float v = 0.f;
-            if ((unsigned)y < (unsigned)g.H && (unsigned)x < (unsigned)g.W) {
-                if (input_format == 1) { const int m = xf.swap ? 2 - ci : ci; v = xf.apply(m, reinterpret_cast<const uint8_t*>(image)[((size_t)n * plane + (size_t)y * g.W + x) * g.Cin + m]); }
-                else v = reinterpret_cast<const float*>(image)[((size_t)n * g.Cin + ci) * plane + (size_t)y * g.W + x];
-                v = bf16_round(v);
+        image_dispatch(img, [&](auto ch_c, auto fmt_c) {
+            constexpr int CH = decltype(ch_c)::value, FMT = decltype(fmt_c)::value;
+            for (int i = threadIdx.x; i < 3 * kWsCols; i += 256) {
+                const int c = i % kWsCols, kh = i / kWsCols;
+                const int y = iy0 + kh, x = ix0 + c;
+                const bool inside = (unsigned)y < (unsigned)g.H && (unsigned)x < (unsigned)g.W;
+                uint32_t raw[CH];
+                float f[3];
+                image_load<CH, FMT>(img, n, image_px<CH, FMT>(img, y, x), y, x, inside, raw);
+                image_decode<CH, FMT>(img, raw, inside, f);
+#pragma unroll
+                for (int ci = 0; ci < CH; ++ci) patch[ci][kh][c] = bf16_round(f[ci]);
             }
-            patch[ci][kh][c] = v;
-        }
+        });
         __syncthreads();
         const int npx = min(kWsSeg, g.Wo - ox0);
         const __nv_bfloat16* dzp = dz + (((size_t)n * g.Ho + oy) * g.Wo + ox0) * Cout + co;
@@ -773,57 +775,51 @@ __global__ void __launch_bounds__(256) wgrad_stem_kernel(WgradGeom g, const void
     }
 }
 
-cudaError_t wgrad_stem_launch(const WgradGeom& g, const void* image, int input_format, const InputTransform& xf, const __nv_bfloat16* dz, float* dstage, int num_sms, cudaStream_t st) {
+cudaError_t wgrad_stem_launch(const WgradGeom& g, const ImageIn& img, const __nv_bfloat16* dz, float* dstage, int num_sms, cudaStream_t st) {
     if ((g.Cin != 3 && g.Cin != 1) || g.ksize != 3 || g.stride != 2 || 256 % g.Cout || g.Cout < 16 || g.Cout > 64) return cudaErrorInvalidValue;
     const int n_seg = g.N * g.Ho * ((g.Wo + kWsSeg - 1) / kWsSeg);
     int blocks = 4 * num_sms;
     if (blocks > n_seg) blocks = n_seg;
-    wgrad_stem_kernel<<<blocks, 256, 0, st>>>(g, image, input_format, xf, dz, dstage);
+    wgrad_stem_kernel<<<blocks, 256, 0, st>>>(g, img, dz, dstage);
     return cudaGetLastError();
 }
 
 // im2col of the stem conv for its weight gradient: X27[n][oy][ox][q] with q = (kh*3 + kw)*Cin + ci (q >= 9 Cin: zero; Cin = 3, or 1 for a
 // gray image: X9 padded to the same 32 columns) as bf16, the image normalised + rounded like the forward does (R0).  The weight gradient of
 // the stem conv is then the weight gradient of a 1x1 conv with 32 input channels over X27, i.e. one launch of the tensor-core wgrad kernel;
-// its staging rows [q][co] ARE the [tap][ci][co] layout.
-__global__ void __launch_bounds__(256) stem_im2col_kernel(WgradGeom g, const void* __restrict__ image, int input_format, const __grid_constant__ InputTransform xf,
-                                                          __nv_bfloat16* __restrict__ x27) {
-    const size_t total = (size_t)g.N * g.Ho * g.Wo * 4;          // one thread per (output pixel, 8-value chunk)
-    const size_t plane = (size_t)g.H * g.W;
-    auto body = [&](auto cin_c) {      // the channel count as a compile-time constant: (tap, ci) from q without a division by a variable
-        constexpr int CIN = decltype(cin_c)::value;
-        for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (size_t)gridDim.x * 256) {
-            const int chunk = (int)(i & 3);
-            const size_t pix = i >> 2;
+// its staging rows [q][co] ARE the [tap][ci][co] layout.  One thread per output pixel: its 9 taps are loaded and decoded once each.
+__global__ void __launch_bounds__(256) stem_im2col_kernel(WgradGeom g, const __grid_constant__ ImageIn img, __nv_bfloat16* __restrict__ x27) {
+    const size_t total = (size_t)g.N * g.Ho * g.Wo;
+    image_dispatch(img, [&](auto ch_c, auto fmt_c) {      // compile-time channel count: every q of a pixel is a fixed register
+        constexpr int CH = decltype(ch_c)::value, FMT = decltype(fmt_c)::value;
+        for (size_t pix = (size_t)blockIdx.x * 256 + threadIdx.x; pix < total; pix += (size_t)gridDim.x * 256) {
             const int ox = (int)(pix % g.Wo), oy = (int)((pix / g.Wo) % g.Ho), n = (int)(pix / ((size_t)g.Wo * g.Ho));
-            float v[8];
+            float v[32];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const int q = chunk * 8 + j;
-                float f = 0.f;
-                if (q < 9 * CIN) {
-                    const int ci = q % CIN, t = q / CIN;
-                    const int y = 2 * oy + t / 3 - 1, x = 2 * ox + t % 3 - 1;
-                    if ((unsigned)y < (unsigned)g.H && (unsigned)x < (unsigned)g.W) {
-                        if (input_format == 1) { const int m = xf.swap ? 2 - ci : ci; f = xf.apply(m, reinterpret_cast<const uint8_t*>(image)[((size_t)n * plane + (size_t)y * g.W + x) * CIN + m]); }
-                        else f = reinterpret_cast<const float*>(image)[((size_t)n * CIN + ci) * plane + (size_t)y * g.W + x];
-                    }
-                }
-                v[j] = f;
+            for (int t = 0; t < 9; ++t) {
+                const int y = 2 * oy + t / 3 - 1, x = 2 * ox + t % 3 - 1;
+                const bool inside = (unsigned)y < (unsigned)g.H && (unsigned)x < (unsigned)g.W;
+                uint32_t raw[CH];
+                float f[3];
+                image_load<CH, FMT>(img, n, image_px<CH, FMT>(img, y, x), y, x, inside, raw);
+                image_decode<CH, FMT>(img, raw, inside, f);
+#pragma unroll
+                for (int ci = 0; ci < CH; ++ci) v[t * CH + ci] = f[ci];
             }
-            reinterpret_cast<uint4*>(x27)[i] = pack8f(v);
+#pragma unroll
+            for (int q = 9 * CH; q < 32; ++q) v[q] = 0.f;
+#pragma unroll
+            for (int c = 0; c < 4; ++c) reinterpret_cast<uint4*>(x27)[pix * 4 + c] = pack8f(v + 8 * c);
         }
-    };
-    if (g.Cin == 1) body(std::integral_constant<int, 1>());
-    else body(std::integral_constant<int, 3>());
+    });
 }
 
-cudaError_t stem_im2col_launch(const WgradGeom& g, const void* image, int input_format, const InputTransform& xf, __nv_bfloat16* x27, int num_sms, cudaStream_t st) {
+cudaError_t stem_im2col_launch(const WgradGeom& g, const ImageIn& img, __nv_bfloat16* x27, int num_sms, cudaStream_t st) {
     if ((g.Cin != 3 && g.Cin != 1) || g.ksize != 3 || g.stride != 2) return cudaErrorInvalidValue;
-    const size_t total = (size_t)g.N * g.Ho * g.Wo * 4;
+    const size_t total = (size_t)g.N * g.Ho * g.Wo;
     size_t blocks = (total + 255) / 256;
     if (blocks > (size_t)num_sms * 16) blocks = (size_t)num_sms * 16;
-    stem_im2col_kernel<<<(int)blocks, 256, 0, st>>>(g, image, input_format, xf, x27);
+    stem_im2col_kernel<<<(int)blocks, 256, 0, st>>>(g, img, x27);
     return cudaGetLastError();
 }
 

@@ -109,10 +109,10 @@ int wgrad_umma_supported(const WgradGeom& g);
 cudaError_t wgrad_umma_launch(const WgradGeom& g, const __nv_bfloat16* x, const __nv_bfloat16* dz, float* dstage, int num_sms, cudaStream_t st);
 // SIMT cross-check (validation only)
 cudaError_t wgrad_simt_launch(const WgradGeom& g, const __nv_bfloat16* x, const __nv_bfloat16* dz, float* dstage, cudaStream_t st);
-// the 3-channel stem conv: x is the raw image (fp32 NCHW or u8 NHWC, normalised + rounded to bf16 like the forward does)
+// the stem conv: the raw image (image.cuh), normalised + rounded to bf16 like the forward does
 // im2col of the stem conv's input for the tensor-core path: X27 bf16 [N][Ho][Wo][32] (27 (tap, ci) values + 5 zeros per output pixel)
-cudaError_t stem_im2col_launch(const WgradGeom& g, const void* image, int input_format, const InputTransform& xf, __nv_bfloat16* x27, int num_sms, cudaStream_t st);
-cudaError_t wgrad_stem_launch(const WgradGeom& g, const void* image, int input_format, const InputTransform& xf, const __nv_bfloat16* dz, float* dstage, int num_sms, cudaStream_t st);
+cudaError_t stem_im2col_launch(const WgradGeom& g, const ImageIn& img, __nv_bfloat16* x27, int num_sms, cudaStream_t st);
+cudaError_t wgrad_stem_launch(const WgradGeom& g, const ImageIn& img, const __nv_bfloat16* dz, float* dstage, int num_sms, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------------
 // optimizer: clip_grad_norm_ + SGD(momentum, weight decay) over flat fp32 buffers

@@ -180,9 +180,9 @@ _STEM4 = re.compile(r'_ZN3lfd12stem4_kernelILb([01])ELb([01])EEEvNS_14UmmaConvPa
 
 
 def test_every_stem_instantiation_pipelines_its_wgmmas_without_a_stack_frame():
-    """The gray loaders are run-time branches of the stem producers: conv_umma.cu as build.py compiles it, with ptxas -v.  Every stem
-    instantiation (conv_umma_kernel MODE_STEM 16 / 32 / 64, conv_umma_c48_kernel MODE_STEM, stem4_kernel) has no stack frame and keeps
-    its wgmma pipeline."""
+    """The stem producers specialise gray and BGR at compile time (stem4_kernel through the shared decoder of image.cuh, the MODE_STEM
+    producer in its own loader): conv_umma.cu as build.py compiles it, with ptxas -v.  Every stem instantiation (conv_umma_kernel MODE_STEM 16 / 32 / 64,
+    conv_umma_c48_kernel MODE_STEM, stem4_kernel) has no stack frame and keeps its wgmma pipeline."""
     b = _build_module()
     cuobjdump = os.path.join(os.path.dirname(b.NVCC), 'cuobjdump')
     if not (os.path.exists(b.NVCC) and os.path.exists(cuobjdump)):

@@ -1,6 +1,6 @@
 # -*- coding: utf-8 -*-
 """The input transform of the uint8 path (BGR -> RGB and any Normalize inside the stem kernels), host side: lowering of the pipelines,
-the C structs and their all-zero default, where the planners put the transform, the plan caches, and the SASS of the new build."""
+the C structs and their all-zero default, where the planners put the transform and the plan caches."""
 import ctypes as C
 
 import numpy as np
@@ -225,26 +225,3 @@ def test_loader_exposes_the_transform_only_when_asked():
     with pytest.raises(ValueError):
         DataLoader(None, Sampler(), Region(), opaque(pipe), model_normalizes=True)
 
-
-def test_the_new_build_keeps_the_sass_counts():
-    """The counters of tests/test_conv_sass.py on conv_umma.cu as it is now: the three uint8 loaders read their constants from the
-    parameter block, and no instantiation may have gained a stack frame or lost its wgmma pipelining."""
-    import os
-    import subprocess
-    import tempfile
-    from test_conv_sass import _build_module, _sass_counts
-    b = _build_module()
-    cuobjdump = os.path.join(os.path.dirname(b.NVCC), 'cuobjdump')
-    if not (os.path.exists(b.NVCC) and os.path.exists(cuobjdump)):
-        pytest.skip('nvcc / cuobjdump not found at %s' % os.path.dirname(b.NVCC))
-    with tempfile.TemporaryDirectory() as tmp:
-        obj = os.path.join(tmp, 'conv_umma.o')
-        p = subprocess.run([b.NVCC] + [f for f in b.FLAGS if f != '-DLFD_B200_TRACE'] + ['-Xptxas', '-v', '-c', os.path.join(b.CSRC, 'conv_umma.cu'), '-o', obj],
-                           stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
-        log = p.stdout.decode()
-        assert p.returncode == 0, log
-        b._check_stack_frames(log, limit=0)           # not one byte of stack in conv_umma_kernel / conv_umma_c48_kernel / stem4_kernel
-        counts = _sass_counts(obj, cuobjdump)
-    stems = {n: c for n, c in counts.items() if 'stem4_kernel' in n or 'conv_umma_kernelILi4' in n or 'conv_umma_c48_kernelILi4' in n}
-    assert len(stems) >= 4 + 2 + 2, sorted(stems)
-    assert all(hgmma > 0 for hgmma, _ in stems.values())
