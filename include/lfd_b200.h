@@ -492,12 +492,13 @@ int lfd_sgd_step(float* params, float* grads, float* momentum_buf, int64_t n, fl
 /* ------------------------------------------------------------------------------------------ training input batch
  * One launch builds a batch of training crops from uint8 source windows, the pixel work of the reference's data loader
  * (RandomBBoxCropRegionSampler & co. lfd/data_pipeline/sampler/region_sampler.py, crop_from_image :280-300, the gray -> 3 channel
- * tile data_loader.py:122-124, HorizontalFlip / BGR2RGB / Normalize, _image_batch_postprocess data_loader.py:68-83):
+ * tile data_loader.py:122-124, HorizontalFlip / BGR2RGB / Normalize, _image_batch_postprocess data_loader.py:68-83), and the
+ * 1-channel batches of gray models (num_input_channels = 1):
  *   R = cv2.resize(S, (0, 0), fx = s, fy = s) (INTER_LINEAR on uint8, bit-exact; INTER_AREA when 1/s == 2; a copy when the size is kept),
  *   crop[y][x] = R[crop_y + y][crop_x + x] inside R, 0 outside; out[y][x] = crop[y][out_w - 1 - x] when flipped.
  * R is never materialised. */
 enum { LFD_RESIZE_COPY = 0, LFD_RESIZE_LINEAR = 1, LFD_RESIZE_AREA2 = 2 };
-enum { LFD_INPUT_OUT_U8_NHWC = 0, LFD_INPUT_OUT_F32_NCHW = 1 };
+enum { LFD_INPUT_OUT_U8_NHWC = 0, LFD_INPUT_OUT_F32_NCHW = 1, LFD_INPUT_OUT_U8_GRAY = 2, LFD_INPUT_OUT_F32_GRAY = 3 };
 typedef struct lfd_input_desc {
     int64_t src_off;          /* byte offset in src of the window's first pixel */
     double inv_scale;         /* 1 / s */
@@ -516,7 +517,12 @@ typedef struct lfd_input_desc {
  * out_mode LFD_INPUT_OUT_U8_NHWC: out uint8 [n, H, W, 3]; LFD_INPUT_OUT_F32_NCHW: out float32 [n, 3, H, W] with
  * out = (v - mean[c]) * scale[c] (albumentations' Normalize: mean[c] = mean * max_pixel, scale[c] = float32(1 / (std * max_pixel))).
  * Pixels outside an image's out_w x out_h are 0 in both modes (the zero padding of mixed-size batches).  swap_rb: BGR -> RGB; a
- * 1-channel source is replicated to 3.  mean / scale: host float[3], unused in the uint8 mode.  W <= 6144. */
+ * 1-channel source is replicated to 3.  mean / scale: host float[3], unused in the uint8 mode.  W <= 6144.
+ * The gray modes, for 1-channel models: LFD_INPUT_OUT_U8_GRAY: out uint8 [n, H, W]; LFD_INPUT_OUT_F32_GRAY: out float32 [n, 1, H, W]
+ * with out = (v - mean[0]) * scale[0].  A gray source is read as it is; a BGR source is converted first, as cv2.cvtColor(S,
+ * COLOR_BGR2GRAY) does on uint8 ((3735 B + 19235 G + 9798 R + 16384) >> 15), and R is cv2.resize of that gray image.  Padding is 0
+ * as above.  swap_rb != 0 with a gray mode is LFD_ERR_INVALID; only mean[0] and scale[0] are read.
+ * Every argument is checked before anything is enqueued: an invalid call writes nothing. */
 int lfd_input_batch(const lfd_input_desc* descs, int n, const uint8_t* src, void* out, int out_mode, int swap_rb, int H, int W,
                     const float* mean, const float* scale, lfd_stream stream);
 

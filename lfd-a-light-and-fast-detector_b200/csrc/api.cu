@@ -1293,8 +1293,11 @@ extern "C" int lfd_sgd_step(float* params, float* grads, float* momentum_buf, in
 extern "C" int lfd_input_batch(const lfd_input_desc* descs, int n, const uint8_t* src, void* out, int out_mode, int swap_rb, int H, int W,
                                const float* mean, const float* scale, lfd_stream stream) {
     if (n < 0 || H < 1 || W < 1 || (n > 0 && (!descs || !src || !out))) return fail(LFD_ERR_INVALID, "lfd_input_batch: bad arguments (n=%d H=%d W=%d)", n, H, W);
-    if (out_mode != LFD_INPUT_OUT_U8_NHWC && out_mode != LFD_INPUT_OUT_F32_NCHW) return fail(LFD_ERR_INVALID, "lfd_input_batch: out_mode %d", out_mode);
-    if (out_mode == LFD_INPUT_OUT_F32_NCHW && (!mean || !scale)) return fail(LFD_ERR_INVALID, "lfd_input_batch: the fp32 mode needs mean and scale");
+    if (out_mode < LFD_INPUT_OUT_U8_NHWC || out_mode > LFD_INPUT_OUT_F32_GRAY) return fail(LFD_ERR_INVALID, "lfd_input_batch: out_mode %d", out_mode);
+    const bool gray = out_mode == LFD_INPUT_OUT_U8_GRAY || out_mode == LFD_INPUT_OUT_F32_GRAY;
+    if ((out_mode == LFD_INPUT_OUT_F32_NCHW || out_mode == LFD_INPUT_OUT_F32_GRAY) && (!mean || !scale))
+        return fail(LFD_ERR_INVALID, "lfd_input_batch: the fp32 modes need mean and scale");
+    if (gray && swap_rb) return fail(LFD_ERR_INVALID, "lfd_input_batch: swap_rb=%d with the gray out_mode %d (one channel has no channel order)", swap_rb, out_mode);
     if (W > 6144) return fail(LFD_ERR_UNSUPPORTED, "lfd_input_batch: W=%d > 6144 (the column table lives in 48 KB of shared memory)", W);
     if (n > 65535) return fail(LFD_ERR_UNSUPPORTED, "lfd_input_batch: n=%d > 65535", n);
     if (n == 0) return LFD_OK;

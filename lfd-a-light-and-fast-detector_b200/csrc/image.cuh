@@ -39,6 +39,12 @@ __host__ __device__ __forceinline__ void nv12_to_bgr(uint32_t Y, uint32_t U, uin
     bgr[2] = nv12_sat8((y + 1673527 * v) >> 20);
 }
 
+// uint8 B, G, R -> gray in 15-bit fixed point, bit for bit what cv2.cvtColor(img, COLOR_BGR2GRAY) gives on uint8 (all 2^24 triples; the
+// often-quoted 14-bit constants 1868 / 9617 / 4899 differ on 43 864 of them).  The training input kernel's gray modes (input.cu).
+__host__ __device__ __forceinline__ uint32_t bgr_to_gray(uint32_t b, uint32_t g, uint32_t r) {
+    return (3735u * b + 19235u * g + 9798u * r + 16384u) >> 15;
+}
+
 // The input image of a batch: fp32 NCHW float[N][ch][H][W], uint8 NHWC uint8[N][H][W][ch], or NV12 (image n = an H x W Y plane, then the
 // interleaved (U, V) plane of H / 2 rows at the same pitch; ch = 1 reads the Y plane only).  H x W is the tensor's (the pitch); a smaller
 // frame lies in its top-left corner.  xf.swap is 0 for fp32 input: its planes are taken as they are.

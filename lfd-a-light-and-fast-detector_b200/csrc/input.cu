@@ -4,7 +4,8 @@
 // One CTA per (image, band of kBandRows output rows).  The CTA first builds a per-output-column table in shared memory (source
 // column and weights, or "zero" / "padding"), then each thread produces four consecutive pixels of a row: it reads their 2x2 source
 // neighbourhoods directly from the window (the resized image is never materialised) and writes 12 bytes (uint8 NHWC) or one float4
-// per channel plane (fp32 NCHW), so consecutive threads store consecutive addresses.
+// per channel plane (fp32 NCHW), so consecutive threads store consecutive addresses.  The gray modes (uint8 [n,H,W], fp32 [n,1,H,W])
+// convert a BGR source to gray at every tap they read, then resize the gray values; they store 4 bytes or one float4.
 #include "../../include/lfd_b200.h"
 #include "kernels.cuh"
 
@@ -74,6 +75,25 @@ __device__ RowInfo row_info(const lfd_input_desc& d, const uint8_t* win, int y) 
     return ri;
 }
 
+// one channel of one output pixel of the gray modes from its source taps: tap(row, x) is the value the resize reads at window column x
+// of a source row.  The same arithmetic as pixel() below, which the 3-channel modes run.
+template <class Tap>
+__device__ __forceinline__ int resample(const lfd_input_desc& d, const RowInfo& ri, int2 col, int x0, int x1, Tap tap) {
+    const int two = col.y >> 24 & 1;
+    const int p00 = tap(ri.r0, x0);
+    if (d.mode == LFD_RESIZE_COPY) return p00;
+    if (d.mode == LFD_RESIZE_AREA2) {
+        int sum = p00 + (two ? tap(ri.r0, x1) : 0);
+        if (ri.b1) sum += tap(ri.r1, x0) + (two ? tap(ri.r1, x1) : 0);
+        const int count = (1 + two) * (1 + ri.b1);
+        return count == 4 ? (sum + 2) >> 2 : __float2int_rn((float)sum / (float)count);   // partial blocks: sum / count, half to even
+    }
+    const int a0 = col.y & 0xfff, a1 = col.y >> 12 & 0xfff;
+    const int h0 = p00 * a0 + (two ? tap(ri.r0, x1) * a1 : 0);
+    const int h1 = tap(ri.r1, x0) * a0 + (two ? tap(ri.r1, x1) * a1 : 0);
+    return min((((h0 >> 4) * ri.b0 >> 16) + ((h1 >> 4) * ri.b1 >> 16) + 2) >> 2, 255);
+}
+
 // one output pixel: channel k of the source order in bits 8k..8k+7 (a gray source replicated)
 __device__ __forceinline__ uint32_t pixel(const lfd_input_desc& d, const RowInfo& ri, int2 col) {
     if (ri.kind != 0 || col.x < 0 || d.win_w <= 0) return 0u;
@@ -103,6 +123,17 @@ __device__ __forceinline__ uint32_t pixel(const lfd_input_desc& d, const RowInfo
     return C == 1 ? packed * 0x010101u : packed;
 }
 
+// one output pixel of a gray mode: the gray value, a BGR source converted tap by tap (bgr_to_gray) before the resize arithmetic of
+// pixel(), as cv2.resize of cv2.cvtColor(BGR2GRAY) computes it.  The 3-channel modes keep pixel() as it is, so their code does not change.
+__device__ __forceinline__ uint32_t gray_pixel(const lfd_input_desc& d, const RowInfo& ri, int2 col) {
+    if (ri.kind != 0 || col.x < 0 || d.win_w <= 0) return 0u;
+    const int wmax = d.win_w - 1;
+    const int x0 = min(max(col.x, 0), wmax);
+    const int x1 = min(max(col.x + 1, 0), wmax);
+    if (d.channels == 1) return resample(d, ri, col, x0, x1, [](const uint8_t* r, int x) { return (int)r[x]; });
+    return resample(d, ri, col, x0, x1, [](const uint8_t* r, int x) { return (int)bgr_to_gray(r[3 * x], r[3 * x + 1], r[3 * x + 2]); });
+}
+
 template <int OUT_MODE>
 __global__ void __launch_bounds__(kThreads) input_batch_kernel(const lfd_input_desc* __restrict__ descs, const uint8_t* __restrict__ src,
                                                                void* __restrict__ out, int swap_rb, int H, int W, float3 mean, float3 scale) {
@@ -118,14 +149,15 @@ __global__ void __launch_bounds__(kThreads) input_batch_kernel(const lfd_input_d
     for (int t = threadIdx.x; t < rows * groups; t += kThreads) {
         const int y = y_begin + t / groups, x = (t % groups) * 4;
         const RowInfo ri = row_info(d, win, y);
+        constexpr bool gray = OUT_MODE == LFD_INPUT_OUT_U8_GRAY || OUT_MODE == LFD_INPUT_OUT_F32_GRAY;
         uint32_t v[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            v[j] = x + j < W ? pixel(d, ri, cols[x + j]) : 0u;
-            if (swap_rb) v[j] = (v[j] & 0x00ff00u) | (v[j] >> 16 & 0xffu) | (v[j] & 0xffu) << 16;
+            v[j] = x + j < W ? (gray ? gray_pixel(d, ri, cols[x + j]) : pixel(d, ri, cols[x + j])) : 0u;
+            if (!gray && swap_rb) v[j] = (v[j] & 0x00ff00u) | (v[j] >> 16 & 0xffu) | (v[j] & 0xffu) << 16;
         }
         const int n = min(4, W - x);
-        if (OUT_MODE == LFD_INPUT_OUT_U8_NHWC) {
+        if constexpr (OUT_MODE == LFD_INPUT_OUT_U8_NHWC) {
             uint8_t* o = reinterpret_cast<uint8_t*>(out) + (((size_t)img * H + y) * W + x) * 3;
             if (n == 4 && (reinterpret_cast<uintptr_t>(o) & 3) == 0) {
                 uint32_t* ow = reinterpret_cast<uint32_t*>(o);
@@ -135,7 +167,7 @@ __global__ void __launch_bounds__(kThreads) input_batch_kernel(const lfd_input_d
             } else {
                 for (int j = 0; j < n * 3; ++j) o[j] = (uint8_t)(v[j / 3] >> (8 * (j % 3)));
             }
-        } else {
+        } else if constexpr (OUT_MODE == LFD_INPUT_OUT_F32_NCHW) {
             const float m[3] = {mean.x, mean.y, mean.z}, s[3] = {scale.x, scale.y, scale.z};
 #pragma unroll
             for (int c = 0; c < 3; ++c) {
@@ -152,6 +184,26 @@ __global__ void __launch_bounds__(kThreads) input_batch_kernel(const lfd_input_d
                     for (int j = 0; j < n; ++j) o[j] = f[j];
                 }
             }
+        } else if constexpr (OUT_MODE == LFD_INPUT_OUT_U8_GRAY) {
+            uint8_t* o = reinterpret_cast<uint8_t*>(out) + ((size_t)img * H + y) * W + x;
+            if (n == 4 && (reinterpret_cast<uintptr_t>(o) & 3) == 0) {
+                *reinterpret_cast<uint32_t*>(o) = v[0] | v[1] << 8 | v[2] << 16 | v[3] << 24;
+            } else {
+                for (int j = 0; j < n; ++j) o[j] = (uint8_t)v[j];
+            }
+        } else {   // LFD_INPUT_OUT_F32_GRAY: one plane, one constant pair (mean.x, scale.x)
+            float f[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int2 e = x + j < W ? cols[x + j] : make_int2(kPad, 0);
+                f[j] = (ri.kind == kPad || e.x == kPad) ? 0.f : __fmul_rn(__fsub_rn((float)v[j], mean.x), scale.x);
+            }
+            float* o = reinterpret_cast<float*>(out) + ((size_t)img * H + y) * W + x;
+            if (n == 4 && (reinterpret_cast<uintptr_t>(o) & 15) == 0) {
+                *reinterpret_cast<float4*>(o) = make_float4(f[0], f[1], f[2], f[3]);
+            } else {
+                for (int j = 0; j < n; ++j) o[j] = f[j];
+            }
         }
     }
 }
@@ -163,12 +215,17 @@ cudaError_t input_batch_launch(const void* descs, int n, const uint8_t* src, voi
     const dim3 grid((H + kBandRows - 1) / kBandRows, n);
     const size_t smem = (size_t)W * sizeof(int2);
     const lfd_input_desc* d = reinterpret_cast<const lfd_input_desc*>(descs);
+    const float3 zero = make_float3(0.f, 0.f, 0.f);
     if (out_mode == LFD_INPUT_OUT_U8_NHWC) {
-        input_batch_kernel<LFD_INPUT_OUT_U8_NHWC><<<grid, kThreads, smem, st>>>(d, src, out, swap_rb, H, W, make_float3(0.f, 0.f, 0.f),
-                                                                             make_float3(0.f, 0.f, 0.f));
-    } else {
+        input_batch_kernel<LFD_INPUT_OUT_U8_NHWC><<<grid, kThreads, smem, st>>>(d, src, out, swap_rb, H, W, zero, zero);
+    } else if (out_mode == LFD_INPUT_OUT_F32_NCHW) {
         input_batch_kernel<LFD_INPUT_OUT_F32_NCHW><<<grid, kThreads, smem, st>>>(d, src, out, swap_rb, H, W, make_float3(mean[0], mean[1], mean[2]),
                                                                               make_float3(scale[0], scale[1], scale[2]));
+    } else if (out_mode == LFD_INPUT_OUT_U8_GRAY) {
+        input_batch_kernel<LFD_INPUT_OUT_U8_GRAY><<<grid, kThreads, smem, st>>>(d, src, out, 0, H, W, zero, zero);
+    } else {
+        input_batch_kernel<LFD_INPUT_OUT_F32_GRAY><<<grid, kThreads, smem, st>>>(d, src, out, 0, H, W, make_float3(mean[0], 0.f, 0.f),
+                                                                              make_float3(scale[0], 0.f, 0.f));
     }
     return cudaGetLastError();
 }

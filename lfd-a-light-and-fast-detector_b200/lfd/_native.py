@@ -83,7 +83,7 @@ UNPACK_CONV, UNPACK_ADD = 0, 1
 MAX_BRANCHES = 8          # LFD_MAX_BRANCHES
 
 RESIZE_COPY, RESIZE_LINEAR, RESIZE_AREA2 = 0, 1, 2
-INPUT_OUT_U8_NHWC, INPUT_OUT_F32_NCHW = 0, 1
+INPUT_OUT_U8_NHWC, INPUT_OUT_F32_NCHW, INPUT_OUT_U8_GRAY, INPUT_OUT_F32_GRAY = 0, 1, 2, 3     # gray: uint8 [n,H,W], float32 [n,1,H,W]
 
 
 class InputDesc(C.Structure):

@@ -17,6 +17,10 @@ float32 NCHW normalised and zero-padded at the bottom-right like the reference's
 None, a Compose of the stand-ins in lfd.data_pipeline.augmentation, or a function choosing one by the sample's keys runs on the host
 exactly as the reference does, and the batch goes to the device as float32 NCHW.
 
+input_channels=1 feeds a gray (1-channel) model: the input kernel converts BGR sources to gray as cv2.cvtColor(COLOR_BGR2GRAY) at
+decode, then resizes, crops and flips the gray image, and image_batch is uint8 [n, H, W] or float32 [n, 1, H, W] under the same rule
+as above.  The draws, annotations and metas are those of input_channels=3.  Only the device path makes gray batches.
+
 Under torch.distributed every rank makes every draw but decodes, copies and resamples only its shard_range of the batch and yields a
 RankLocalBatch, which Executor.train / val use without slicing again.
 """
@@ -165,12 +169,18 @@ class _Slot(object):
 
 class DataLoader(object):
 
-    def __init__(self, dataset, dataset_sampler, region_sampler, augmentation_pipeline=None, num_workers=1, model_normalizes=False):
+    def __init__(self, dataset, dataset_sampler, region_sampler, augmentation_pipeline=None, num_workers=1, model_normalizes=False,
+                 input_channels=3):
         """model_normalizes: the model's stem kernels run the pipeline's channel swap and normalisation (LFD.set_input_transform with
         this loader's `input_transform`; Executor.train does that): batches of equal-size crops are then raw uint8 BGR NHWC, a quarter of
         the bytes, for every pipeline the input kernel can run.  The flip stays in the input kernel.  A batch with crops of different
         sizes is float32 NCHW, normalised here, as without the argument (its zero padding is zero AFTER normalisation, which no byte
-        expresses); the model takes float32 batches as they are."""
+        expresses); the model takes float32 batches as they are.
+        input_channels: 3 (BGR batches) or 1 (gray batches for a gray model: uint8 [n, H, W] or float32 [n, 1, H, W]).  With 1 the pipeline
+        must be one the input kernel runs, without BGR2RGB and with a Normalize of one constant or three equal ones (ValueError otherwise);
+        gray and BGR sources both become gray, BGR ones as cv2.cvtColor(COLOR_BGR2GRAY) before the resize."""
+        if input_channels not in (1, 3):
+            raise ValueError('input_channels must be 3 (BGR) or 1 (gray), got %r' % (input_channels,))
         self._dataset = dataset
         self._dataset_sampler = dataset_sampler
         self._loops = len(dataset_sampler)
@@ -187,9 +197,15 @@ class DataLoader(object):
         self._specs = specs if native else None
         if model_normalizes and not native:
             raise ValueError('model_normalizes needs a region sampler with draw() and a pipeline the input kernel can run (flip, BGR2RGB, a final Normalize)')
-        # what the model has to do to this loader's uint8 batches; None: simple_normalize on BGR, the only pipeline that gives uint8 batches
+        if input_channels == 1:
+            if not native:
+                raise ValueError('input_channels=1 needs a region sampler with draw() and a pipeline the input kernel can run (flip, a final '
+                                 'Normalize): gray batches are made on the device only')
+            input_transform_of(augmentation_pipeline, allow_flip=True, channels=1)     # ValueError for BGR2RGB or unequal constants
+        self.input_channels = input_channels
+        # what the model has to do to this loader's uint8 batches; None: simple_normalize, the only pipeline that gives uint8 batches
         # without model_normalizes
-        self.input_transform = input_transform_of(augmentation_pipeline, allow_flip=True) if model_normalizes else None
+        self.input_transform = input_transform_of(augmentation_pipeline, allow_flip=True, channels=input_channels) if model_normalizes else None
         self._slots = [_Slot(), _Slot()]
         self._stream = None
         self.last_stats = None   # host timings / bytes of the last native batch (tests/debug_input_timing.py)
@@ -309,17 +325,19 @@ class DataLoader(object):
             numpy.array_equal(scale, numpy.full(3, numpy.float32(1.0) / numpy.float32(127.5), numpy.float32))))
         if u8:
             swap = False     # raw BGR bytes: with model_normalizes the swap happens in the stem kernel
+        gray = self.input_channels == 1     # swap is False: the constructor refused BGR2RGB
         with torch.cuda.stream(self._stream):
             staged = torch.empty(off, dtype=torch.uint8, device=device)
             staged.copy_(buf[:off], non_blocking=True)
             if u8:
-                out = torch.empty((n, H, W, 3), dtype=torch.uint8, device=device)
+                out = torch.empty((n, H, W) if gray else (n, H, W, 3), dtype=torch.uint8, device=device)
+                mode = nat.INPUT_OUT_U8_GRAY if gray else nat.INPUT_OUT_U8_NHWC
             else:
-                out = torch.empty((n, 3, H, W), dtype=torch.float32, device=device)
+                out = torch.empty((n, 1, H, W) if gray else (n, 3, H, W), dtype=torch.float32, device=device)
+                mode = nat.INPUT_OUT_F32_GRAY if gray else nat.INPUT_OUT_F32_NCHW
             m, s = (C.c_float * 3)(*mean.tolist()), (C.c_float * 3)(*scale.tolist())
-            nat.check(nat.lib().lfd_input_batch(C.c_void_p(staged.data_ptr()), n, C.c_void_p(staged.data_ptr()), nat.ptr(out),
-                                                nat.INPUT_OUT_U8_NHWC if u8 else nat.INPUT_OUT_F32_NCHW, int(swap), H, W, m, s,
-                                                C.c_void_p(self._stream.cuda_stream)))
+            nat.check(nat.lib().lfd_input_batch(C.c_void_p(staged.data_ptr()), n, C.c_void_p(staged.data_ptr()), nat.ptr(out), mode,
+                                                int(swap), H, W, m, s, C.c_void_p(self._stream.cuda_stream)))
             slot.event = torch.cuda.Event()
             slot.event.record(self._stream)
         self.last_stats = dict(draw_decode_ms=(t1 - t0) * 1e3, copy_ms=(t2 - t1) * 1e3, h2d_bytes=off, images=n)

@@ -123,9 +123,22 @@ class Executor(object):
         """This rank's share of a batch: a RankLocalBatch already is one (the loader built only this rank's images)."""
         return tuple(data_batch) if isinstance(data_batch, RankLocalBatch) else shard_batch(data_batch)
 
+    def _check_input_channels(self, loader):
+        """A DataLoader's batches have its input_channels (3: BGR, 1: gray); the model must read that many (ValueError otherwise)."""
+        model = self.config_dict['model']
+        channels = getattr(loader, 'input_channels', None)
+        if channels is None or not hasattr(model, '_backbone'):
+            return
+        from .._engine import image_channels
+        if channels != image_channels(model):
+            raise ValueError('the data loader makes %d-channel batches (input_channels=%d) but the model reads %d-channel images'
+                             % (channels, channels, image_channels(model)))
+
     def _set_input_transform(self, loader):
         """A loader that leaves channel order and normalisation to the model (DataLoader(model_normalizes=True)) says which: its uint8
-        batches mean nothing without it.  A DataLoader without the argument resets the model to the default its uint8 batches assume."""
+        batches mean nothing without it.  A DataLoader without the argument resets the model to the default its uint8 batches assume.
+        Its channel count must be the model's (ValueError before the first step)."""
+        self._check_input_channels(loader)
         if hasattr(loader, 'input_transform') and hasattr(self.config_dict['model'], 'set_input_transform'):
             self.config_dict['model'].set_input_transform(loader.input_transform)
 
@@ -133,6 +146,7 @@ class Executor(object):
         cfg = self.config_dict
         cfg['mode'] = 'train'
         cfg['model'].train()
+        self._check_input_channels(cfg.get('val_data_loader'))     # the val loader too, so a mismatch stops the run before it trains
         self._set_input_transform(cfg['train_data_loader'])
         self._call_hooks('before_train_epoch')
         for i, data_batch in enumerate(cfg['train_data_loader']):
