@@ -16,6 +16,7 @@ import functools
 import torch
 
 from gpu_ops import DTYPES, conv_out, ref_conv64, stem_input
+from helpers import bits  # noqa: F401  (X.bits of test_gpu_extent_configs.py)
 from lfd import _native as nat
 from lfd._engine import fold_scale, pack_conv_weight, pack_stem_weight
 from nv12_oracle import nv12_frames, nv12_oracle
@@ -166,10 +167,6 @@ def _scratch_buf():
 
 def _scratch():
     return _scratch_buf()
-
-
-def bits(t):
-    return t.contiguous().view(torch.int16 if t.element_size() == 2 else torch.int32)
 
 
 def assert_poison(t, what):

@@ -1,6 +1,7 @@
 # -*- coding: utf-8 -*-
 """Helpers that drive single native ops through the C-ABI (lfd_run_op) for the GPU parity tests."""
 import ctypes as C
+import functools
 
 import torch
 import torch.nn.functional as F
@@ -25,13 +26,106 @@ def conv_out(size, k, s):
     return (size + 2 * (k // 2) - k) // s + 1
 
 
+GUARD = 4096          # bytes of poison before and after every tensor of the single-op runners
+
+
+class Workspace(object):
+    """Byte workspace with named, 256-byte aligned regions (what lfd_op / lfd_top offsets index).  By default zero-filled with the regions
+    back to back.  guard > 0 keeps that many bytes before and after every region; poison fills the workspace with 0xff bytes (NaN in bf16,
+    fp16, fp32 and fp64), so a kernel that reads outside its tensors carries a NaN and one that writes outside them is caught by
+    assert_guards().  A region added with zero=True starts at zero (the fused GroupNorm statistics accumulate with atomics)."""
+
+    def __init__(self, device, guard=0, poison=False):
+        self.device, self.guard, self.poison = device, guard, poison
+        self.top = max(256, guard)
+        self.items = {}          # name -> (offset, bytes, dtype, shape)
+        self.init = {}
+        self.zero = []
+        self.buf = None
+
+    def add(self, name, tensor=None, shape=None, dtype=None, zero=False):
+        if tensor is not None:
+            tensor = tensor.contiguous()
+            shape, dtype = tuple(tensor.shape), tensor.dtype
+            self.init[name] = tensor
+        nbytes = int(torch.empty(0, dtype=dtype).element_size())
+        for s in shape:
+            nbytes *= s
+        off = self.top
+        self.items[name] = (off, nbytes, dtype, tuple(shape))
+        self.top = ((off + nbytes + 255) & ~255) + self.guard
+        if zero:
+            self.zero.append(name)
+        return off
+
+    def finalize(self):
+        self.buf = torch.full((self.top + 256,), 0xff if self.poison else 0, dtype=torch.uint8, device=self.device)
+        for name in self.zero:
+            off, nbytes, _, _ = self.items[name]
+            self.buf[off:off + nbytes] = 0
+        for name, t in self.init.items():
+            off, nbytes, _, _ = self.items[name]
+            self.buf[off:off + nbytes] = t.to(self.device).view(torch.uint8).reshape(-1)
+        return self
+
+    def off(self, name):
+        return self.items[name][0] if name is not None else -1
+
+    def get(self, name):
+        off, nbytes, dtype, shape = self.items[name]
+        return self.buf[off:off + nbytes].view(dtype).view(shape).clone()
+
+    def assert_guards(self, what=''):
+        """Every byte outside the regions still holds the poison (one reduction on the device; the workspace stays there)."""
+        assert self.poison
+        outside = torch.ones_like(self.buf, dtype=torch.bool)
+        for off, nbytes, _, _ in self.items.values():
+            outside[off:off + nbytes] = False
+        written = (self.buf != 0xff) & outside
+        n = int(written.sum())
+        if n:
+            first = int(written.nonzero()[0])
+            end, name = max([(o + nb, k) for k, (o, nb, _, _) in self.items.items() if o + nb <= first], default=(0, 'the start'))
+            raise AssertionError('%s: %d bytes outside the tensors were written, the first at byte %d (%d bytes past the end of %s)'
+                                 % (what, n, first, first - end, name))
+
+
+def make_op(kind, dtype='bf16', transform=None, **fields):
+    """An lfd_op (nat.Op) of the 16-bit storage type `dtype`, every tensor offset -1 (none) unless given, the input transform set by
+    nat.set_input_transform."""
+    op = nat.Op()
+    op.kind, op.dtype = kind, DTYPES[dtype][3]
+    op.in_off = op.out_off = op.res_off = op.stats_off = op.ds_out_off = -1
+    for k, v in fields.items():
+        setattr(op, k, v)
+    nat.set_input_transform(op, transform)
+    return op
+
+
+def _set_tail(op, tail, cin, tdt, dev):
+    """The fused 1x1 tail (w [Cf, cin, 1, 1], scale, shift, relu) of op -> the device operands, to be kept until the launch"""
+    w2, sc2, sh2, relu2 = tail
+    keep = pack_conv_weight(fold_scale(w2, sc2), cin, tdt).to(dev), sh2.float().to(dev).contiguous()
+    op.tail_cout, op.tail_relu = w2.shape[0], int(relu2)
+    op.tail_weight, op.tail_shift = keep[0].data_ptr(), keep[1].data_ptr()
+    return keep
+
+
+def _run_op(op, ws, x=None, fmt=0, impl=nat.CONV_UMMA):
+    with torch.cuda.device(ws.device):
+        rc = nat.lib().lfd_run_op(C.byref(op), nat.ptr(x), fmt, nat.ptr(ws.buf), None, None, 0, 0, impl, nat.stream_ptr())
+        torch.cuda.synchronize()
+    return rc
+
+
 def run_conv(x_nhwc, weight, scale, shift, stride, relu, res=None, gn_groups=0, impl=nat.CONV_UMMA, tail=None, dtype='bf16', max_ctas=0,
-             ds=None):
+             ds=None, inplace=False):
     """x_nhwc: cuda bf16 / fp16 [N,H,W,Cin]; weight fp32 [Cout,Cin,k,k] (already representable in the 16-bit type).
     max_ctas: lfd_op.max_ctas (0 = one persistent CTA per SM).  ds = (w3 [Cout,Cin,1,1], scale3, shift3): the fused 1x1/s2
-    shortcut of a 3x3/s2 conv (lfd_op.ds_cout).
+    shortcut of a 3x3/s2 conv (lfd_op.ds_cout).  inplace: the residual is read from the output tensor (out == res).
+    Every tensor sits in a guarded, poisoned Workspace whose guards are checked after the launch.
     -> (out [N,Ho,Wo,Cf], stats double [N,groups,2] or None, conv_query dict), plus the shortcut output [N,Ho,Wo,Cout] with ds"""
-    tdt, _, _, code = DTYPES[dtype]
+    tdt = DTYPES[dtype][0]
     assert x_nhwc.dtype == tdt
     dev = x_nhwc.device
     N, H, W, Cin = x_nhwc.shape
@@ -41,46 +135,35 @@ def run_conv(x_nhwc, weight, scale, shift, stride, relu, res=None, gn_groups=0, 
     q = nat.conv_query(N, H, W, Cin, Ho, Wo, Cout, k, stride, Cf if tail is not None else 0, Cout if ds is not None else 0)
     wp = pack_conv_weight(fold_scale(weight, scale), q['cc'], tdt).to(dev)   # BatchNorm scale folded before the bf16 rounding
     sh = shift.float().to(dev).contiguous()
-    in_b = x_nhwc.numel() * 2
-    out_b = N * Ho * Wo * Cf * 2
-    al = lambda v: (v + 255) & ~255
-    off_in, off_out = 4096, 4096 + al(in_b)
-    off_res = off_out + al(out_b)
-    off_ds = off_res + al(out_b)
-    total = off_ds + al(out_b) + 256
-    ws = torch.zeros(total, dtype=torch.uint8, device=dev)
-    ws[off_in:off_in + in_b] = x_nhwc.contiguous().view(torch.uint8).reshape(-1)
-    if res is not None:
-        ws[off_res:off_res + out_b] = res.contiguous().view(torch.uint8).reshape(-1)
-    op = nat.Op()
-    op.kind = nat.OP_CONV
-    op.dtype = code
-    op.N, op.H, op.W, op.Cin, op.Ho, op.Wo, op.Cout = N, H, W, Cin, Ho, Wo, Cout
-    op.ksize, op.stride, op.relu, op.gn_groups, op.cc = k, stride, int(relu), gn_groups, q['cc']
-    op.in_off, op.out_off, op.res_off = off_in, off_out, (off_res if res is not None else -1)
-    op.stats_off = 0 if gn_groups else -1
-    op.max_ctas = max_ctas
-    op.weight, op.shift = wp.data_ptr(), sh.data_ptr()
-    if tail is not None:
-        w2, sc2, sh2, relu2 = tail
-        w2p = pack_conv_weight(fold_scale(w2, sc2), Cout, tdt).to(dev)
-        sh2d = sh2.float().to(dev).contiguous()
-        op.tail_cout, op.tail_relu = Cf, int(relu2)
-        op.tail_weight, op.tail_shift = w2p.data_ptr(), sh2d.data_ptr()
+    ws = Workspace(dev, guard=GUARD, poison=True)
+    ws.add('in', x_nhwc)
+    if inplace:
+        ws.add('out', res)
+    else:
+        ws.add('out', shape=(N, Ho, Wo, Cf), dtype=tdt)
+        if res is not None:
+            ws.add('res', res)
+    if gn_groups:
+        ws.add('stats', shape=(N, gn_groups, 2), dtype=torch.float64, zero=True)
+    if ds is not None:
+        ws.add('ds', shape=(N, Ho, Wo, Cout), dtype=tdt)
+    ws.finalize()
+    op = make_op(nat.OP_CONV, dtype, N=N, H=H, W=W, Cin=Cin, Ho=Ho, Wo=Wo, Cout=Cout, ksize=k, stride=stride, relu=int(relu),
+                 gn_groups=gn_groups, cc=q['cc'], max_ctas=max_ctas, in_off=ws.off('in'), out_off=ws.off('out'),
+                 res_off=ws.off('out' if inplace else 'res' if res is not None else None), stats_off=ws.off('stats' if gn_groups else None),
+                 weight=wp.data_ptr(), shift=sh.data_ptr())
+    keep = list(_set_tail(op, tail, Cout, tdt, dev)) if tail is not None else []
     if ds is not None:
         w3, sc3, sh3 = ds
-        w3p = pack_conv_weight(fold_scale(w3, sc3), Cin, tdt).to(dev)      # [Cin/8][Cout][8]
-        sh3d = sh3.float().to(dev).contiguous()
-        op.ds_cout, op.ds_out_off = Cout, off_ds
-        op.ds_weight, op.ds_shift = w3p.data_ptr(), sh3d.data_ptr()
-    with torch.cuda.device(dev):
-        nat.check(nat.lib().lfd_run_op(C.byref(op), None, 0, nat.ptr(ws), None, None, 0, 0, impl, nat.stream_ptr()))
-        torch.cuda.synchronize()
-    out = ws[off_out:off_out + out_b].view(tdt).view(N, Ho, Wo, Cf).clone()
-    stats = ws[0:N * gn_groups * 16].view(torch.float64).view(N, gn_groups, 2).clone() if gn_groups else None
+        keep += [pack_conv_weight(fold_scale(w3, sc3), Cin, tdt).to(dev), sh3.float().to(dev).contiguous()]     # [Cin/8][Cout][8]
+        op.ds_cout, op.ds_out_off = Cout, ws.off('ds')
+        op.ds_weight, op.ds_shift = keep[-2].data_ptr(), keep[-1].data_ptr()
+    nat.check(_run_op(op, ws, impl=impl))
+    ws.assert_guards('conv N%d %dx%d %d-%d k%ds%d' % (N, H, W, Cin, Cout, k, stride))
+    stats = ws.get('stats') if gn_groups else None
     if ds is not None:
-        return out, stats, q, ws[off_ds:off_ds + out_b].view(tdt).view(N, Ho, Wo, Cout).clone()
-    return out, stats, q
+        return ws.get('out'), stats, q, ws.get('ds')
+    return ws.get('out'), stats, q
 
 
 def ref_conv(x_nhwc, weight, scale, shift, stride, relu, res=None, dtype='bf16'):
@@ -113,44 +196,36 @@ def assert_bf16_close(out_bf16, ref_fp32, what='', dtype='bf16'):
                              % (what, int(bad.sum()), o.numel(), i, float(o[i]), float(r[i]), float((o - r).abs().max()), float(r.abs().max())))
 
 
-def run_stem0(img, fmt, w, shift, relu, tail=None, max_ctas=0, dtype='bf16'):
-    """LFD_OP_STEM0 through lfd_run_op: img = cuda uint8 [N,H,W,3] (fmt 'u8') or float32 [N,3,H,W] (fmt 'f32'); w fp32
-    [Cout,3,3,3] with the BatchNorm scale already folded in (rounded to the 16-bit type by the packing); tail as in run_conv.
-    -> (out [N,Ho,Wo,Cf], number of 16 x 8 output tiles)"""
-    tdt, _, _, code = DTYPES[dtype]
-    dev = img.device
-    if fmt == 'u8':
-        N, H, W, _ = img.shape
+def run_stem0(x, fmt, w, shift, *, cin=3, relu=True, tail=None, transform=None, dtype='bf16', impl=nat.CONV_UMMA, max_ctas=0, raw_rc=False):
+    """LFD_OP_STEM0 with Cin = cin through lfd_run_op.  x (fmt, a nat.INPUT_* code): float32 [N,cin,H,W], uint8 [N,H,W,cin] or gray
+    [N,H,W], NV12 [N,3H/2,W]; w fp32 [Cout,cin,3,3] with the BatchNorm scale already folded in (rounded to the 16-bit type by the
+    packing); tail as in run_conv.  The output sits in a guarded, poisoned Workspace whose guards are checked after the launch.
+    -> (out [N,Ho,Wo,Cf], number of 16 x 8 output tiles); raw_rc: -> (lfd_run_op's return code, the workspace bytes), unchecked"""
+    tdt = DTYPES[dtype][0]
+    dev = x.device
+    N = x.shape[0]
+    if fmt == nat.INPUT_F32_NCHW:
+        H, W = x.shape[2], x.shape[3]
+    elif fmt == nat.INPUT_U8_NV12:
+        H, W = x.shape[1] * 2 // 3, x.shape[2]
     else:
-        N, _, H, W = img.shape
+        H, W = x.shape[1], x.shape[2]
     Cout = w.shape[0]
     Ho, Wo = conv_out(H, 3, 2), conv_out(W, 3, 2)
     Cf = tail[0].shape[0] if tail is not None else Cout
-    wp = pack_stem_weight(w, tdt).to(dev)
-    sh = shift.float().to(dev).contiguous()
-    out_b = N * Ho * Wo * Cf * 2
-    ws = torch.zeros(4096 + ((out_b + 255) & ~255) + 256, dtype=torch.uint8, device=dev)
-    op = nat.Op()
-    op.kind = nat.OP_STEM0
-    op.dtype = code
-    op.N, op.H, op.W, op.Cin, op.Ho, op.Wo, op.Cout = N, H, W, 3, Ho, Wo, Cout
-    op.ksize, op.stride, op.relu = 3, 2, int(relu)
-    op.in_off, op.out_off, op.res_off, op.stats_off = -1, 4096, -1, -1
-    op.max_ctas = max_ctas
-    op.weight, op.shift = wp.data_ptr(), sh.data_ptr()
-    if tail is not None:
-        w2, sc2, sh2, relu2 = tail
-        w2p = pack_conv_weight(fold_scale(w2, sc2), Cout, tdt).to(dev)
-        sh2d = sh2.float().to(dev).contiguous()
-        op.tail_cout, op.tail_relu = Cf, int(relu2)
-        op.tail_weight, op.tail_shift = w2p.data_ptr(), sh2d.data_ptr()
-    x = img.contiguous()
-    with torch.cuda.device(dev):
-        nat.check(nat.lib().lfd_run_op(C.byref(op), nat.ptr(x), nat.INPUT_U8_NHWC if fmt == 'u8' else nat.INPUT_F32_NCHW, nat.ptr(ws), None,
-                                       None, 0, 0, nat.CONV_UMMA, nat.stream_ptr()))
-        torch.cuda.synchronize()
-    out = ws[4096:4096 + out_b].view(tdt).view(N, Ho, Wo, Cf).clone()
-    return out, N * ((Ho + 15) // 16) * ((Wo + 7) // 8)
+    wp, sh = pack_stem_weight(w, tdt).to(dev), shift.float().to(dev).contiguous()
+    ws = Workspace(dev, guard=GUARD, poison=True)
+    ws.add('out', shape=(N, Ho, Wo, Cf), dtype=tdt)
+    ws.finalize()
+    op = make_op(nat.OP_STEM0, dtype, transform, N=N, H=H, W=W, Cin=cin, Ho=Ho, Wo=Wo, Cout=Cout, ksize=3, stride=2, relu=int(relu),
+                 max_ctas=max_ctas, out_off=ws.off('out'), weight=wp.data_ptr(), shift=sh.data_ptr())
+    keep = _set_tail(op, tail, Cout, tdt, dev) if tail is not None else None    # noqa: F841  (alive until the launch)
+    rc = _run_op(op, ws, x.contiguous(), fmt, impl)
+    if raw_rc:
+        return rc, ws.buf
+    nat.check(rc)
+    ws.assert_guards('stem0 N%d %dx%d Cin %d Cout %d tail %d' % (N, H, W, cin, Cout, Cf if tail is not None else 0))
+    return ws.get('out'), N * ((Ho + 15) // 16) * ((Wo + 7) // 8)
 
 
 def stem_input(img, fmt, dtype='bf16'):
@@ -229,3 +304,77 @@ def assert_gn_stats(stats, out, groups, what=''):
     st = stats.cpu()
     assert bool(((st[..., 0] - s1).abs() <= 1e-5 * a1 + 1e-30).all()), '%s: sum off by %g' % (what, float((st[..., 0] - s1).abs().max()))
     assert bool(((st[..., 1] - s2).abs() <= 1e-5 * s2 + 1e-30).all()), '%s: sum of squares off by %g' % (what, float((st[..., 1] - s2).abs().max()))
+
+
+# ------------------------------------------------------------------------------------------------ op-level conv and stem cases
+# conv case: (N, H, W, Cin, Cout, k, s, relu, res, gn, tail, ds); stem case: (Cout, tail, fmt 'u8' / 'f32', H, W).  Each test module
+# passes its own seed, so its operands stay what they have always been.
+STEM_FMT = {'u8': nat.INPUT_U8_NHWC, 'f32': nat.INPUT_F32_NCHW}
+
+
+@functools.lru_cache(maxsize=None)
+def conv_operands(case, dtype, seed):
+    """-> (x, w, scale, shift, res or None, tail (w2, scale2, shift2, relu) or None, shortcut (w3, scale3, shift3) or None), drawn in
+    that order"""
+    N, H, W, Cin, Cout, k, s, relu, use_res, gn, tail, ds = case
+    tdt = DTYPES[dtype][0]
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn((N, H, W, Cin), generator=g).to(tdt)
+    w = torch.randn((Cout, Cin, k, k), generator=g) * (2.0 / (Cin * k * k)) ** 0.5
+    scale, shift = torch.rand((Cout,), generator=g) + 0.5, torch.randn((Cout,), generator=g) * 0.2
+    Cf = tail or Cout
+    Ho, Wo = conv_out(H, k, s), conv_out(W, k, s)
+    res = torch.randn((N, Ho, Wo, Cf), generator=g).to(tdt) if use_res else None
+    t = None
+    if tail:
+        t = (torch.randn((tail, Cout, 1, 1), generator=g) * (2.0 / Cout) ** 0.5, torch.rand((tail,), generator=g) + 0.5,
+             torch.randn((tail,), generator=g) * 0.2, bool(relu))
+    d = None
+    if ds:
+        d = (torch.randn((Cout, Cin, 1, 1), generator=g) * (1.0 / Cin) ** 0.5, torch.rand((Cout,), generator=g) + 0.5,
+             torch.randn((Cout,), generator=g) * 0.2)
+    return x, w, scale, shift, res, t, d
+
+
+@functools.lru_cache(maxsize=None)
+def conv_reference(case, dtype, seed):
+    """(ref64, S, K) of the stored output (tail: the two-layer chain with the 16-bit intermediate) and of the shortcut output (or None)."""
+    N, H, W, Cin, Cout, k, s, relu, use_res, gn, tail, ds = case
+    x, w, scale, shift, res, t, d = conv_operands(case, dtype, seed)
+    rnd = DTYPES[dtype][1]
+    if tail:
+        mid, _, _ = ref_conv64(x, w, scale, shift, s, relu, dtype=dtype)
+        main = ref_conv64(rnd(mid.float()), t[0], t[1], t[2], 1, t[3], res=res, dtype=dtype)
+    else:
+        main = ref_conv64(x, w, scale, shift, s, relu, res=res, dtype=dtype)
+    # the shortcut reads the conv's centre tap: a 1x1/s2 conv of the same input, stored without ReLU
+    short = ref_conv64(x[:, ::2, ::2, :], d[0], d[1], d[2], 1, False, dtype=dtype) if ds else None
+    return main, short
+
+
+def run_conv_case(case, dtype, seed, max_ctas=0, impl=nat.CONV_UMMA, inplace=False):
+    """run_conv on conv_operands(case, dtype, seed) -> (out, stats or None, conv_query, shortcut output or None)"""
+    N, H, W, Cin, Cout, k, s, relu, use_res, gn, tail, ds = case
+    x, w, scale, shift, res, t, d = conv_operands(case, dtype, seed)
+    r = run_conv(x.cuda(), w, scale, shift, s, bool(relu), res=None if res is None else res.cuda(), gn_groups=gn, impl=impl, tail=t,
+                 dtype=dtype, max_ctas=max_ctas, ds=d, inplace=inplace)
+    return r if ds else r + (None,)
+
+
+@functools.lru_cache(maxsize=None)
+def stem_operands(case, seed):
+    """-> (image, w with the BatchNorm scale folded in, shift, tail (w2, scale2, shift2, True) or None)"""
+    Cout, tail, fmt, H, W = case
+    N = 2
+    g = torch.Generator().manual_seed(seed)
+    if fmt == 'u8':
+        img = torch.randint(0, 256, (N, H, W, 3), generator=g, dtype=torch.uint8)
+    else:
+        img = torch.randn((N, 3, H, W), generator=g)
+    w = torch.randn((Cout, 3, 3, 3), generator=g) * (2.0 / 27) ** 0.5 * (torch.rand((Cout, 1, 1, 1), generator=g) + 0.5)
+    shift = torch.randn((Cout,), generator=g) * 0.2
+    t = None
+    if tail:
+        t = (torch.randn((tail, Cout, 1, 1), generator=g) * (2.0 / Cout) ** 0.5, torch.rand((tail,), generator=g) + 0.5,
+             torch.randn((tail,), generator=g) * 0.2, True)
+    return img, w, shift, t

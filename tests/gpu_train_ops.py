@@ -4,45 +4,8 @@ import ctypes as C
 
 import torch
 
+from gpu_ops import Workspace  # noqa: F401  (the training tests' workspace)
 from lfd import _native as nat
-
-
-class Workspace(object):
-    """Byte workspace with named, 256-byte aligned regions (what lfd_top.off[] indexes)."""
-
-    def __init__(self, device):
-        self.device = device
-        self.top = 256
-        self.items = {}          # name -> (offset, bytes, dtype, shape)
-        self.init = {}
-        self.buf = None
-
-    def add(self, name, tensor=None, shape=None, dtype=None):
-        if tensor is not None:
-            tensor = tensor.contiguous()
-            shape, dtype = tuple(tensor.shape), tensor.dtype
-            self.init[name] = tensor
-        nbytes = int(torch.empty(0, dtype=dtype).element_size())
-        for s in shape:
-            nbytes *= s
-        off = self.top
-        self.items[name] = (off, nbytes, dtype, tuple(shape))
-        self.top = (off + nbytes + 255) & ~255
-        return off
-
-    def finalize(self):
-        self.buf = torch.zeros(self.top + 256, dtype=torch.uint8, device=self.device)
-        for name, t in self.init.items():
-            off, nbytes, _, _ = self.items[name]
-            self.buf[off:off + nbytes] = t.to(self.device).view(torch.uint8).reshape(-1)
-        return self
-
-    def off(self, name):
-        return self.items[name][0] if name is not None else -1
-
-    def get(self, name):
-        off, nbytes, dtype, shape = self.items[name]
-        return self.buf[off:off + nbytes].view(dtype).view(shape).clone()
 
 
 def make_top(kind, **kw):
@@ -73,10 +36,6 @@ def desc_table(descs, device):
     arr = (type(descs[0]) * len(descs))(*descs)
     raw = bytes(memoryview(arr).cast('B'))
     return torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(device)
-
-
-def bf16r(t):
-    return t.to(torch.bfloat16).float()
 
 
 # ------------------------------------------------------------------------------------------------ grids of the SIMT training launches

@@ -1,10 +1,13 @@
 # -*- coding: utf-8 -*-
+import functools
 import os
 
 import numpy as np
 import torch
 
 import synth
+import tl_s
+from lfd import _native as nat
 from oracle import lfd_oracle as orc
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
@@ -112,3 +115,119 @@ def assert_same_detections_up_to_margins(got_src, want_src, scores, boxes, thr, 
         cascade = [int(u) for u, v in zip(same, ious) if int(u) in dset and int(u) != d and v > iou_thr - iou_tol]
         assert bool(near.any()) or cascade, (what, 'detection differs without a borderline decision', d, float(scores[d]))
     return len(diff)
+
+
+@functools.lru_cache(maxsize=None)
+def model_of(name, device='cpu'):
+    """The synthetic model of a config, TL_S included, in eval mode on `device` (one instance per name and device)."""
+    model = tl_s.synth_model()[0] if name == 'TL_S' else synth_model(name)[0]
+    return model.to(device).eval()
+
+
+def finetune_model(cfg, frozen_stages, cls_bias, seed=666):
+    """A synthetic model in training mode with its first `frozen_stages` stages frozen ('all': every stage)."""
+    model, _ = synth_model(cfg, cls_bias=cls_bias, seed=seed)
+    bb = model._backbone
+    bb._frozen_stages = len(bb.stages()) if frozen_stages == 'all' else frozen_stages
+    return model.train()                  # LFDResNet.train freezes the stem and stages 0..k-1 (eval mode, requires_grad False)
+
+
+class ListDataset(object):
+    """A dataset of the given samples, indexed 0..n-1."""
+
+    def __init__(self, samples):
+        self.samples = dict(enumerate(samples))
+
+    def __len__(self):
+        return len(self.samples)
+
+    def __getitem__(self, i):
+        return self.samples[i]
+
+    def get_indexes(self):
+        return list(self.samples.keys())
+
+
+def bits(t):
+    """The bits of a 16- or 32-bit tensor, as integers of the same width (on its device)."""
+    return t.contiguous().view(torch.int16 if t.element_size() == 2 else torch.int32)
+
+
+def same_bits(a, b, what):
+    bad = bits(a) != bits(b)
+    if bool(bad.any()):
+        i = tuple(bad.nonzero()[0].tolist())
+        raise AssertionError('%s: %d of %d elements differ, first at %s: %r vs %r' % (what, int(bad.sum()), bad.numel(), i, float(a[i]), float(b[i])))
+
+
+def misaligned(x):
+    """A device copy of uint8 x at a base address of 1 (mod 4)."""
+    raw = torch.empty(x.numel() + 1, dtype=torch.uint8, device='cuda')
+    y = raw[1:].view(x.shape)                        # base address 1 (mod 4): the fused stem's per-pixel loader
+    y.copy_(x)
+    assert y.data_ptr() % 4 == 1
+    return y
+
+
+def grids_agree(results, what):
+    """Results of one op on several grids: entries 0 and 1 (fp32 gradients) bit for bit, every later entry (fp64 sums) to 1e-12."""
+    g0 = results[0]
+    for r in results[1:]:
+        for a, b in zip(g0[:2], r[:2]):
+            assert torch.equal(a.view(torch.int32), b.view(torch.int32)), what + ': gradients differ between grids'
+        for a, b in zip(g0[2:], r[2:]):   # fp64 sums in another order: the same to ~1e-15
+            assert bool(((a - b).abs() <= 1e-12 * a.abs() + 1e-300).all()), (what, a, b)
+
+
+# ------------------------------------------------------------------------------------------------ probes of whole inference plans
+CONV_KINDS = (nat.OP_STEM0, nat.OP_CONV, nat.OP_STEM4)
+
+
+def conv_outputs(plan):
+    """(tensor name, op) of every output of the plan's conv ops (the shortcut outputs included)."""
+    return [(op[k], op) for op in plan._ops if op['kind'] in CONV_KINDS for k in ('out', 'out2') if op.get(k) is not None]
+
+
+def downstream_of_gn(plan):
+    """Names of the tensors that depend on a GroupNorm."""
+    tainted = set()
+    for op in plan._ops:
+        if op['kind'] == nat.OP_GN_APPLY or any(op.get(k) in tainted for k in ('inp', 'res')):
+            tainted |= {op[k] for k in ('out', 'out2') if op.get(k) is not None}
+    return tainted
+
+
+def close_downstream_of_gn(what, a, b):
+    """Results downstream of a GroupNorm, whose statistics come from fp64 atomics that add in another order on another grid: a flipped
+    last bit of one group's mean or rstd moves every value of the group, so the number of differing elements depends on the map size and
+    the 16-bit type; the largest difference keeps the bound of test_gpu_schedule_invariance.py.  A value read from outside the frame
+    would be NaN (or 255-based) instead."""
+    assert bool(torch.isfinite(a).all()), what
+    d = (a - b).abs()
+    assert float(d.max()) <= 2.0 ** -6 * float(b.abs().max()), (what, float(d.max()), int((d > 0).sum()))
+
+
+def poison(plan):
+    """0xff bytes (NaN in every float type, 255 in a uint8 staging) in the plan's workspace, input staging and outputs."""
+    plan.workspace.fill_(0xff)
+    if plan._stage is not None:
+        plan._stage.fill_(0xff)
+    for c, r in plan._outputs:
+        c.view(torch.uint8).fill_(0xff)
+        r.view(torch.uint8).fill_(0xff)
+
+
+def untouched(plan, call):
+    """call() must raise before anything reaches the device: the workspace, the outputs and the staging keep their bytes.
+    -> the message of the error"""
+    import pytest
+    plan.staging(nat.INPUT_U8_NHWC)
+    poison(plan)
+    torch.cuda.synchronize()
+    with pytest.raises((ValueError, nat.LfdError)) as e:
+        call()
+    torch.cuda.synchronize()
+    assert bool((plan.workspace == 0xff).all()) and bool((plan._stage == 0xff).all())
+    for c, r in plan._outputs:
+        assert bool((c.view(torch.uint8) == 0xff).all()) and bool((r.view(torch.uint8) == 0xff).all())
+    return str(e.value)

@@ -4,7 +4,8 @@
 mkdir -p gpurun_out
 nvidia-smi --query-gpu=name,clocks.sm,clocks.max.sm,memory.total --format=csv > gpurun_out/gpu.txt 2>&1
 rc_all=0
-for m in test_gpu_conv test_gpu_ops test_gpu_train_ops test_gpu_variants test_gpu_forward test_gpu_train test_gpu_executor test_gpu_fullsize; do
+for f in tests/test_gpu_*.py; do
+  m=$(basename "$f" .py)
   timeout 600 python -m pytest tests/$m.py -q -m gpu -x --tb=short -p no:cacheprovider "$@" > gpurun_out/$m.log 2>&1
   rc=$?
   echo "== $m rc=$rc"; tail -n 25 gpurun_out/$m.log

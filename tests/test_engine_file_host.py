@@ -3,15 +3,13 @@
 (lfd_engine_open / lfd_engine_info / lfd_engine_op) and compare it with the plan; the export is deterministic; and lfd_engine_open
 refuses corrupted files with the documented code and a message that names the field."""
 import ctypes as C
-import functools
 import struct
 import zlib
 
 import pytest
 import torch
 
-import tl_s
-from helpers import synth_model
+from helpers import model_of
 from lfd import _native as nat
 from lfd._engine import MODEL_FORMAT_VERSION
 from lfd.deployment import export_model
@@ -21,11 +19,6 @@ LFD_ERR_INVALID, LFD_ERR_UNSUPPORTED = 1, 3
 CONFIGS = ['WIDERFACE_XS', 'WIDERFACE_S', 'WIDERFACE_M', 'WIDERFACE_L', 'TT100K_S', 'TT100K_L', 'TL_L', 'TL_S']
 PTR_FIELDS = [n for n, t in nat.Op._fields_ if t is C.c_void_p]
 HEADER, PLAN = 48, 120
-
-
-@functools.lru_cache(maxsize=None)
-def model_of(name):
-    return tl_s.synth_model()[0] if name == 'TL_S' else synth_model(name)[0]
 
 
 def export(tmp_path, name, N=2, H=200, W=264, tag='a', **kw):

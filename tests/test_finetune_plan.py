@@ -6,21 +6,13 @@ import pytest
 import torch
 
 import lfd._native as nat
-from helpers import synth_model
+from helpers import finetune_model, synth_model
 from lfd._engine import InferencePlan
 from lfd._train import TrainPlan, flat_parameters
 from plan_order import check_every_conflict_ordered
 
 CPU = torch.device('cpu')
 CASES = [(cfg, k) for cfg in ('WIDERFACE_L', 'WIDERFACE_S', 'TT100K_L', 'TL_L') for k in (1, 2, 'all')]
-
-
-def finetune_model(cfg, frozen_stages):
-    model, _ = synth_model(cfg)
-    bb = model._backbone
-    bb._frozen_stages = len(bb.stages()) if frozen_stages == 'all' else frozen_stages
-    model.train()                  # LFDResNet.train freezes the stem and stages 0..k-1 (eval mode, requires_grad False)
-    return model
 
 
 def freeze_head_branch(model):
@@ -94,7 +86,7 @@ def _final_convs(model):
 
 @pytest.mark.parametrize('cfg,frozen_stages', CASES)
 def test_frozen_stage_plan(cfg, frozen_stages, shape=(2, 128, 160)):
-    model = finetune_model(cfg, frozen_stages)
+    model = finetune_model(cfg, frozen_stages, -1.0)
     frozen_ids = {id(p) for p in model.parameters() if not p.requires_grad}
     assert frozen_ids
     plan = TrainPlan(model, *shape, CPU, create_native=False)
@@ -124,7 +116,7 @@ def test_frozen_stage_plan(cfg, frozen_stages, shape=(2, 128, 160)):
 def test_prefix_ops_are_the_inference_plans(cfg, frozen_stages, shape):
     """Kinds, fusions (tails, fused shortcut, the four-conv stem where the inference plan picks it) and packed operand bytes of every
     prefix op equal those of the inference plan's op producing the same tensor."""
-    model = finetune_model(cfg, frozen_stages)
+    model = finetune_model(cfg, frozen_stages, -1.0)
     plan = TrainPlan(model, *shape, CPU, create_native=False)
     model.eval()
     ref = InferencePlan(model, *shape, CPU, create_native=False)
@@ -203,7 +195,7 @@ def test_fused_sgd_runs_skip_frozen_slots():
     """FusedSGD steps over runs of the flat buffer: a frozen parameter's slots are in none of them (torch.optim.SGD skips a parameter
     without gradient: no weight decay, no momentum), and (un)freezing rebuilds the runs."""
     from lfd.execution.optim import FusedSGD
-    model = finetune_model('WIDERFACE_L', 2)
+    model = finetune_model('WIDERFACE_L', 2, -1.0)
     flat = flat_parameters(model, allow_cpu=True)
     opt = FusedSGD(model, torch.optim.SGD(model.parameters(), lr=0.01, momentum=0.9, weight_decay=1e-4).param_groups)
     opt._flat = flat

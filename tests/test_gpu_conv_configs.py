@@ -9,8 +9,9 @@ import functools
 import pytest
 import torch
 
-from gpu_ops import (DTYPES, assert_faithful, assert_gn_stats, assert_tail_close, conv_out, ref_conv64, run_conv, run_stem0,
-                     stem_input)
+from gpu_ops import (DTYPES, STEM_FMT, assert_faithful, assert_gn_stats, assert_tail_close, conv_out, conv_reference, ref_conv64, run_conv,
+                     run_conv_case, run_stem0, stem_input, stem_operands)
+from helpers import bits
 from lfd import _native as nat
 
 MODE_FLAT, MODE_3X3S1, MODE_3X3S2, MODE_1X1S2, MODE_STEM = 'flat', '3x3s1', '3x3s2', '1x1s2', 'stem'
@@ -104,51 +105,8 @@ def test_case_table_covers_every_configuration():
     assert all(c[3] >= 64 and c[4] >= 33 for c in STEM_CASES)
 
 
-@functools.lru_cache(maxsize=None)
-def _operands(case, dtype):
-    N, H, W, Cin, Cout, k, s, relu, use_res, gn, tail, ds = case
-    tdt, rnd = DTYPES[dtype][0], DTYPES[dtype][1]
-    g = torch.Generator().manual_seed(hash(case) & 0xffff)
-    x = torch.randn((N, H, W, Cin), generator=g).to(tdt)
-    w = torch.randn((Cout, Cin, k, k), generator=g) * (2.0 / (Cin * k * k)) ** 0.5
-    scale, shift = torch.rand((Cout,), generator=g) + 0.5, torch.randn((Cout,), generator=g) * 0.2
-    Cf = tail or Cout
-    Ho, Wo = conv_out(H, k, s), conv_out(W, k, s)
-    res = torch.randn((N, Ho, Wo, Cf), generator=g).to(tdt) if use_res else None
-    t = None
-    if tail:
-        t = (torch.randn((tail, Cout, 1, 1), generator=g) * (2.0 / Cout) ** 0.5, torch.rand((tail,), generator=g) + 0.5,
-             torch.randn((tail,), generator=g) * 0.2, bool(relu))
-    d = None
-    if ds:
-        d = (torch.randn((Cout, Cin, 1, 1), generator=g) * (1.0 / Cin) ** 0.5, torch.rand((Cout,), generator=g) + 0.5,
-             torch.randn((Cout,), generator=g) * 0.2)
-    return x, w, scale, shift, res, t, d
-
-
-def _run(case, dtype, max_ctas):
-    N, H, W, Cin, Cout, k, s, relu, use_res, gn, tail, ds = case
-    x, w, scale, shift, res, t, d = _operands(case, dtype)
-    r = run_conv(x.cuda(), w, scale, shift, s, bool(relu), res=None if res is None else res.cuda(),
-                 gn_groups=gn, tail=t, dtype=dtype, max_ctas=max_ctas, ds=d)
-    out, stats, q = r[0], r[1], r[2]
-    return out, stats, q, (r[3] if ds else None)
-
-
-@functools.lru_cache(maxsize=None)
-def _reference(case, dtype):
-    """(ref64, S, K) of the stored output (tail: the two-layer chain with the 16-bit intermediate) and of the shortcut output."""
-    N, H, W, Cin, Cout, k, s, relu, use_res, gn, tail, ds = case
-    x, w, scale, shift, res, t, d = _operands(case, dtype)
-    rnd = DTYPES[dtype][1]
-    if tail:
-        mid, _, _ = ref_conv64(x, w, scale, shift, s, relu, dtype=dtype)
-        main = ref_conv64(rnd(mid.float()), t[0], t[1], t[2], 1, t[3], res=res, dtype=dtype)
-    else:
-        main = ref_conv64(x, w, scale, shift, s, relu, res=res, dtype=dtype)
-    # the shortcut reads the conv's centre tap: a 1x1/s2 conv of the same input, stored without ReLU
-    short = ref_conv64(x[:, ::2, ::2, :], d[0], d[1], d[2], 1, False, dtype=dtype) if ds else None
-    return main, short
+def _seed(case):
+    return hash(case) & 0xffff
 
 
 @pytest.mark.gpu
@@ -157,10 +115,10 @@ def _reference(case, dtype):
 @pytest.mark.parametrize('case', [c for c, _ in CASES], ids=_id)
 def test_conv_config_matches_fp64(case, dtype, max_ctas):
     N, H, W, Cin, Cout, k, s, relu, use_res, gn, tail, ds = case
-    out, stats, q, out3 = _run(case, dtype, max_ctas)
+    out, stats, q, out3 = run_conv_case(case, dtype, _seed(case), max_ctas)
     if max_ctas:
         assert q['num_tiles'] // max_ctas >= 4
-    (ref, S, K), short = _reference(case, dtype)
+    (ref, S, K), short = conv_reference(case, dtype, _seed(case))
     what = 'conv %s %s max_ctas=%d (plan %s)' % (_id(case), dtype, max_ctas, q)
     if tail:
         assert_tail_close(out, ref, dtype, what)
@@ -170,10 +128,6 @@ def test_conv_config_matches_fp64(case, dtype, max_ctas):
         assert_faithful(out3, short[0], short[1], short[2], dtype, what + ' shortcut')
     if gn:
         assert_gn_stats(stats, out, gn, what)
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int16).cpu()
 
 
 def _assert_stats_equal(a, b, out, what):
@@ -187,12 +141,12 @@ def _assert_stats_equal(a, b, out, what):
 def test_grid_does_not_change_the_output(case):
     """Tiles are strided by gridDim: any grid size gives the same stored bits (statistics: the same sums up to the order of the
     fp64 atomics)."""
-    runs = [_run(case, 'bf16', m) for m in (1, 2, 7, 0)]
+    runs = [run_conv_case(case, 'bf16', _seed(case), m) for m in (1, 2, 7, 0)]
     out0, st0, _, sc0 = runs[-1]
     for m, (out, st, _, sc) in zip((1, 2, 7), runs[:-1]):
-        assert torch.equal(_bits(out), _bits(out0)), 'max_ctas=%d changes %d output elements' % (m, int((out != out0).sum()))
+        assert torch.equal(bits(out), bits(out0)), 'max_ctas=%d changes %d output elements' % (m, int((out != out0).sum()))
         if sc is not None:
-            assert torch.equal(_bits(sc), _bits(sc0)), 'max_ctas=%d changes the shortcut output' % m
+            assert torch.equal(bits(sc), bits(sc0)), 'max_ctas=%d changes the shortcut output' % m
         if st is not None:
             _assert_stats_equal(st, st0, out0, 'max_ctas=%d statistics' % m)
 
@@ -227,28 +181,14 @@ def test_gn_statistics_conv_honours_relu_and_residual(impl, tail):
 
 
 # ------------------------------------------------------------------------------------------------ STEM0 as an op
-@functools.lru_cache(maxsize=None)
-def _stem_operands(case, dtype):
+def _stem_seed(case):
     Cout, tail, fmt, H, W = case
-    N = 2
-    g = torch.Generator().manual_seed(Cout * 1000 + tail * 10 + H + W)
-    if fmt == 'u8':
-        img = torch.randint(0, 256, (N, H, W, 3), generator=g, dtype=torch.uint8)
-    else:
-        img = torch.randn((N, 3, H, W), generator=g)
-    w = torch.randn((Cout, 3, 3, 3), generator=g) * (2.0 / 27) ** 0.5 * (torch.rand((Cout, 1, 1, 1), generator=g) + 0.5)
-    shift = torch.randn((Cout,), generator=g) * 0.2
-    t = None
-    if tail:
-        t = (torch.randn((tail, Cout, 1, 1), generator=g) * (2.0 / Cout) ** 0.5, torch.rand((tail,), generator=g) + 0.5,
-             torch.randn((tail,), generator=g) * 0.2, True)
-    return img, w, shift, t
+    return Cout * 1000 + tail * 10 + H + W
 
 
 def _run_stem(case, dtype, max_ctas):
-    Cout, tail, fmt, H, W = case
-    img, w, shift, t = _stem_operands(case, dtype)
-    return run_stem0(img.cuda(), fmt, w, shift, True, tail=t, max_ctas=max_ctas, dtype=dtype)
+    img, w, shift, t = stem_operands(case, _stem_seed(case))
+    return run_stem0(img.cuda(), STEM_FMT[case[2]], w, shift, tail=t, max_ctas=max_ctas, dtype=dtype)
 
 
 @pytest.mark.gpu
@@ -257,7 +197,7 @@ def _run_stem(case, dtype, max_ctas):
 @pytest.mark.parametrize('case', STEM_CASES, ids=_stem_id)
 def test_stem0_matches_fp64(case, dtype, max_ctas):
     Cout, tail, fmt, H, W = case
-    img, w, shift, t = _stem_operands(case, dtype)
+    img, w, shift, t = stem_operands(case, _stem_seed(case))
     out, num_tiles = _run_stem(case, dtype, max_ctas)
     if max_ctas:
         assert num_tiles // max_ctas >= 4
@@ -278,7 +218,7 @@ def test_stem0_matches_fp64(case, dtype, max_ctas):
 def test_stem0_grid_does_not_change_the_output(case):
     outs = [_run_stem(case, 'bf16', m)[0] for m in (1, 2, 7, 0)]
     for m, o in zip((1, 2, 7), outs[:-1]):
-        assert torch.equal(_bits(o), _bits(outs[-1])), 'max_ctas=%d changes %d stem elements' % (m, int((o != outs[-1]).sum()))
+        assert torch.equal(bits(o), bits(outs[-1])), 'max_ctas=%d changes %d stem elements' % (m, int((o != outs[-1]).sum()))
 
 
 # ------------------------------------------------------------------------------------------------ STEM4 as an op
@@ -321,7 +261,7 @@ def test_stem4_matches_fp64_chain_and_is_grid_invariant(h, w, fmt):
     q = nat.stem4_query(2, h, w)
     assert q['num_tiles'] >= 3
     for m, o in zip((1, 3), outs[:-1]):
-        assert torch.equal(_bits(o), _bits(outs[-1])), 'stem4 max_ctas=%d changes %d elements' % (m, int((o != outs[-1]).sum()))
+        assert torch.equal(bits(o), bits(outs[-1])), 'stem4 max_ctas=%d changes %d elements' % (m, int((o != outs[-1]).sum()))
     rnd = DTYPES[dtype][1]
     t = stem_input(img, fmt, dtype)
     for conv, norm, relu in model._backbone.stem_layers():

@@ -4,7 +4,6 @@ InferencePlan and PostPlan it was exported from give -- on float32, uint8 BGR an
 and replayed as a CUDA graph, with greedy NMS and Soft-NMS -- with the same launches; examples/lfd_detect prints the rows of
 predict_for_single_image; and a call the engine refuses enqueues nothing."""
 import ctypes as C
-import functools
 import os
 import subprocess
 
@@ -13,9 +12,8 @@ import pytest
 import torch
 
 import synth
-import tl_s
 from engine_file import Engine, rows
-from helpers import synth_model
+from helpers import model_of
 from lfd import _native as nat
 from lfd._engine import InferencePlan, PostPlan
 from lfd.data_pipeline.augmentation import input_transform_of
@@ -29,12 +27,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PROGRAM = os.path.join(ROOT, 'lfd-a-light-and-fast-detector_b200', 'lfd_detect')
 LFD_ERR_INVALID, LFD_ERR_CAPACITY = 1, 4
 SOFT = dict(type='soft_nms', iou_thr=0.3, method='linear', min_score=0.05)
-
-
-@functools.lru_cache(maxsize=None)
-def model_of(name):
-    model = tl_s.synth_model(cls_bias=-1.0)[0] if name == 'TL_S' else synth_model(name, cls_bias=-1.0)[0]
-    return model.cuda().eval()
 
 
 def pipeline_of(name):
@@ -73,7 +65,7 @@ CASES = [(name, 'bf16', None) for name in ('WIDERFACE_XS', 'WIDERFACE_S', 'WIDER
 
 @pytest.mark.parametrize('name,dtype,fuse', CASES)
 def test_engine_equals_the_plan(tmp_path, name, dtype, fuse):
-    model = model_of(name)
+    model = model_of(name, 'cuda')
     N, H, W = 2, 256, 320
     plan = InferencePlan(model, N, H, W, torch.device('cuda'), act_dtype=dtype, fuse_stem=fuse, input_transform=input_transform_of(pipeline_of(name)))
     if fuse is not None:
@@ -109,7 +101,7 @@ def test_engine_equals_the_plan(tmp_path, name, dtype, fuse):
 @pytest.mark.parametrize('name', ['WIDERFACE_S', 'TL_L', 'TL_S'])
 @pytest.mark.parametrize('soft', [False, True], ids=['nms', 'soft_nms'])
 def test_rows_equal_predict_for_single_image(tmp_path, name, soft):
-    model = model_of(name)
+    model = model_of(name, 'cuda')
     own = model._nms_cfg
     model._nms_cfg = dict(SOFT) if soft else dict(type='nms', iou_thr=0.4)
     try:
@@ -134,7 +126,7 @@ def test_rows_equal_predict_for_single_image(tmp_path, name, soft):
 def test_autotuned_export_replays_its_bounds(tmp_path):
     """The CTA bounds autotune picks are in the file, and the results do not depend on them (TL_L: no GroupNorm statistics, whose fp64
     atomics would add in another order under another grid)."""
-    model = model_of('TL_L')
+    model = model_of('TL_L', 'cuda')
     N, H, W = 2, 256, 320
     path = str(tmp_path / 'tuned.lfd')
     tuned, post = export_model(model, path, N, H, W, input_pipeline=tl_val_pipeline, autotune=True)
@@ -181,7 +173,7 @@ def _program_rows(out):
 @pytest.mark.parametrize('name', ['WIDERFACE_S', 'TL_S'])
 def test_c_program_prints_the_rows_of_predict_for_single_image(tmp_path, name):
     assert os.path.exists(PROGRAM), 'build() links examples/lfd_detect.c next to the library'
-    model = model_of(name)
+    model = model_of(name, 'cuda')
     h, w = 184, 248
     path = str(tmp_path / 'm.lfd')
     export_model(model, path, 1, h, w, input_pipeline=pipeline_of(name), classification_threshold=0.3, autotune=False)
@@ -206,7 +198,7 @@ def test_c_program_prints_the_rows_of_predict_for_single_image(tmp_path, name):
 
 def test_errors_launch_nothing(tmp_path):
     """Each refused call returns its code before anything reaches the device: every caller buffer keeps its bytes."""
-    model = model_of('WIDERFACE_S')
+    model = model_of('WIDERFACE_S', 'cuda')
     path = str(tmp_path / 'm.lfd')
     export_model(model, path, 2, 96, 160, autotune=False)
     data = open(path, 'rb').read()
@@ -257,7 +249,7 @@ def test_errors_launch_nothing(tmp_path):
 def test_a_call_on_another_stream_writes_the_image_sizes_again(tmp_path):
     """The per-image width / height the post-process reads are written on the stream of the call that writes them: a call of the same size
     on another stream writes them again, so its post-process is ordered after them (the region is overwritten here to show it)."""
-    model = model_of('TL_L')
+    model = model_of('TL_L', 'cuda')
     path = str(tmp_path / 'm.lfd')
     export_model(model, path, 2, 256, 320, input_pipeline=tl_val_pipeline, classification_threshold=0.3, autotune=False)
     eng = Engine(open(path, 'rb').read())

@@ -11,20 +11,13 @@ import pytest
 import torch
 
 import synth
-from helpers import synth_model
+from helpers import finetune_model, synth_model
 from lfd._engine import InferencePlan
 from lfd.execution.executor import Executor
 from lfd.execution.optim import FusedSGD
 from test_gpu_train_step_per_op import Replay
 
 pytestmark = pytest.mark.gpu
-
-
-def finetune_model(cfg, frozen_stages, cls_bias=-2.0, seed=666):
-    model, _ = synth_model(cfg, cls_bias=cls_bias, seed=seed)
-    bb = model._backbone
-    bb._frozen_stages = len(bb.stages()) if frozen_stages == 'all' else frozen_stages
-    return model.cuda().train()
 
 
 def _input(fmt, n, h, w, seed=0):
@@ -56,7 +49,7 @@ def _prefix_matches_inference(model, plan, x):
                                                            ('WIDERFACE_L', 'all', (2, 186, 252), None), ('TT100K_L', 2, (1, 186, 252), None)])
 @pytest.mark.parametrize('fmt', ['f32', 'u8'])
 def test_prefix_tensors_equal_the_inference_plans(cfg, frozen_stages, shape, stem4, fmt):
-    model = finetune_model(cfg, frozen_stages)
+    model = finetune_model(cfg, frozen_stages, -2.0).cuda()
     x = _input(fmt, *shape)
     plan = model.train_plan_for(*shape, x.device)
     kinds = {op['kind'] for _, op in plan._prefix['ops']}
@@ -83,8 +76,8 @@ def _frozen_state(model):
 def test_fused_sgd_steps_like_torch_sgd_with_frozen_parameters():
     """FusedSGD over the flat buffers vs torch.optim.SGD (momentum 0.9, weight decay 1e-4) on the same gradients: frozen parameters
     untouched and without momentum entry, trainable ones and their momentum buffers to the optimizer kernel test's bound."""
-    model = finetune_model('WIDERFACE_L', 2)
-    twin = finetune_model('WIDERFACE_L', 2)
+    model = finetune_model('WIDERFACE_L', 2, -2.0).cuda()
+    twin = finetune_model('WIDERFACE_L', 2, -2.0).cuda()
     opt = FusedSGD.from_torch(_sgd(model), model)
     topt = _sgd(twin)
     opt.zero_grad()
@@ -174,7 +167,7 @@ def test_executor_fine_tunes_with_frozen_stages_and_resumes(tmp_path):
 
 def test_fine_tuning_reduces_the_loss():
     from lfd.execution.hooks import OptimizerHook
-    model = finetune_model('WIDERFACE_S', 2)
+    model = finetune_model('WIDERFACE_S', 2, -2.0).cuda()
     n, h, w = 4, 256, 256
     x = synth.synth_input(n, h, w).cuda()
     ann = synth.synth_annotations(n, h, w, 1, seed=3)
@@ -195,7 +188,7 @@ def test_fine_tuning_reduces_the_loss():
 def test_new_prefix_weights_are_repacked_and_unfreezing_differentiates():
     """load_state_dict between two steps: the next step's prefix tensors equal a fresh InferencePlan's.  Unfreezing (frozen_stages -1 and
     train() again) gives a plan that differentiates the newly trainable layers, checked layer by layer."""
-    model = finetune_model('WIDERFACE_S', 2)
+    model = finetune_model('WIDERFACE_S', 2, -2.0).cuda()
     n, h, w = 2, 160, 192
     x = synth.synth_input(n, h, w).cuda()
     ann = synth.synth_annotations(n, h, w, 1, seed=3)
@@ -223,8 +216,8 @@ def test_new_prefix_weights_are_repacked_and_unfreezing_differentiates():
 
 
 def test_cuda_graph_fine_tuning_step_matches_eager():
-    model = finetune_model('WIDERFACE_S', 2)
-    ref = finetune_model('WIDERFACE_S', 2)
+    model = finetune_model('WIDERFACE_S', 2, -2.0).cuda()
+    ref = finetune_model('WIDERFACE_S', 2, -2.0).cuda()
     ref.use_cuda_graph_training = True
     n, h, w = 2, 128, 160
     x = synth.synth_input(n, h, w).cuda()

@@ -12,14 +12,15 @@ import torch
 
 import synth
 from engine_file import Engine, rows
-from gpu_ops import DTYPES, assert_faithful, conv_out, ref_conv64
+from gpu_ops import DTYPES, assert_faithful, conv_out, ref_conv64, run_stem0
 from gpu_train_ops import Workspace, assert_within, cdiv, make_top, run_top, stem_wgrad_grid
 from gray_models import gray_pair, twin_f32, twin_u8
+from helpers import misaligned, same_bits
 from lfd import _native as nat
-from lfd._engine import InferencePlan, fold_scale, pack_conv_weight, pack_stem_weight
+from lfd._engine import InferencePlan
 from lfd.data_pipeline.augmentation import Compose, Normalize, input_transform_of
 from nv12_oracle import nv12_frames
-from test_gpu_nv12 import compare, misaligned, same_bits, snapshot
+from test_gpu_nv12 import compare, snapshot
 
 pytestmark = pytest.mark.gpu
 
@@ -44,45 +45,11 @@ def luma(nv):
 
 
 # ------------------------------------------------------------------------------------------------------------------ single ops
-def run_stem0(x, fmt, cin, transform, w, shift, tail, dtype, impl=nat.CONV_UMMA, max_ctas=0, raw_rc=False):
-    """LFD_OP_STEM0 with Cin = cin through lfd_run_op.  x: uint8 [N,H,W] (gray) / [N,H,W,3], float32 [N,cin,H,W] or NV12 [N,3H/2,W]."""
-    tdt, code = DTYPES[dtype][0], DTYPES[dtype][3]
-    if fmt == nat.INPUT_F32_NCHW:
-        N, H, W = x.shape[0], x.shape[2], x.shape[3]
-    elif fmt == nat.INPUT_U8_NV12:
-        N, H, W = x.shape[0], x.shape[1] * 2 // 3, x.shape[2]
-    else:
-        N, H, W = x.shape[0], x.shape[1], x.shape[2]
-    Cout = w.shape[0]
-    Ho, Wo = conv_out(H, 3, 2), conv_out(W, 3, 2)
-    Cf = tail[0].shape[0] if tail is not None else Cout
-    keep = [pack_stem_weight(w, tdt).cuda(), shift.float().cuda()]
-    out_b = N * Ho * Wo * Cf * 2
-    ws = torch.full((4096 + ((out_b + 255) & ~255) + 256,), 0xff, dtype=torch.uint8, device='cuda')
-    op = nat.Op()
-    op.kind, op.dtype = nat.OP_STEM0, code
-    op.N, op.H, op.W, op.Cin, op.Ho, op.Wo, op.Cout = N, H, W, cin, Ho, Wo, Cout
-    op.ksize, op.stride, op.relu, op.max_ctas = 3, 2, 1, max_ctas
-    op.in_off, op.out_off, op.res_off, op.stats_off, op.ds_out_off = -1, 4096, -1, -1, -1
-    op.weight, op.shift = keep[0].data_ptr(), keep[1].data_ptr()
-    if tail is not None:
-        keep += [pack_conv_weight(fold_scale(tail[0], torch.ones(Cf)), Cout, tdt).cuda(), tail[1].float().cuda()]
-        op.tail_cout, op.tail_relu, op.tail_weight, op.tail_shift = Cf, 1, keep[2].data_ptr(), keep[3].data_ptr()
-    nat.set_input_transform(op, transform)
-    torch.cuda.synchronize()
-    rc = nat.lib().lfd_run_op(C.byref(op), nat.ptr(x), fmt, nat.ptr(ws), None, None, 0, 0, impl, nat.stream_ptr())
-    torch.cuda.synchronize()
-    if raw_rc:
-        return rc, ws
-    nat.check(rc)
-    return ws[4096:4096 + out_b].view(tdt).view(N, Ho, Wo, Cf).clone()
-
-
 def weights(cout):
     g = torch.Generator().manual_seed(cout)
     w1 = torch.randn((cout, 1, 3, 3), generator=g) * 0.1
     shift = torch.randn(cout, generator=g) * 0.1
-    tail = (torch.randn((cout, cout, 1, 1), generator=g) * 0.1, torch.randn(cout, generator=g) * 0.1)
+    tail = (torch.randn((cout, cout, 1, 1), generator=g) * 0.1, torch.ones(cout), torch.randn(cout, generator=g) * 0.1, True)
     return w1, torch.cat([w1, torch.zeros(cout, 2, 3, 3)], 1), shift, tail
 
 
@@ -108,10 +75,10 @@ def test_stem0_gray_equals_its_twin(cout, dtype, name):
             for t in (None, tail):
                 for ctas in (0, 3):
                     what = 'stem0 Cout=%d%s %s %s fmt=%d %dx%d max_ctas=%d' % (cout, ' + tail' if t else '', dtype, name, fg, h, wd, ctas)
-                    same_bits(run_stem0(xg, fg, 1, transform, w1, shift, t, dtype, max_ctas=ctas),
-                              run_stem0(xt, ft, 3, transform, w3, shift, t, dtype, max_ctas=ctas), what)
-            same_bits(run_stem0(xg, fg, 1, transform, w1, shift, None, dtype, impl=nat.CONV_SIMT),
-                      run_stem0(xt, ft, 3, transform, w3, shift, None, dtype, impl=nat.CONV_SIMT),
+                    same_bits(run_stem0(xg, fg, w1, shift, cin=1, tail=t, transform=transform, dtype=dtype, max_ctas=ctas)[0],
+                              run_stem0(xt, ft, w3, shift, tail=t, transform=transform, dtype=dtype, max_ctas=ctas)[0], what)
+            same_bits(run_stem0(xg, fg, w1, shift, cin=1, transform=transform, dtype=dtype, impl=nat.CONV_SIMT)[0],
+                      run_stem0(xt, ft, w3, shift, transform=transform, dtype=dtype, impl=nat.CONV_SIMT)[0],
                       'SIMT stem0 Cout=%d %s %s fmt=%d %dx%d' % (cout, dtype, name, fg, h, wd))
 
 
@@ -131,7 +98,7 @@ def test_gray_stem0_is_a_faithful_rounding_of_float64(cout, dtype):
         for x, inp, fmt in ((x8, g8, nat.INPUT_U8_NHWC), (xf, gf, nat.INPUT_F32_NCHW)):
             ref, S, K = ref_conv64(x, w1, torch.ones(cout), shift, 2, True, dtype=dtype)
             for impl in (nat.CONV_UMMA, nat.CONV_SIMT):
-                out = run_stem0(inp, fmt, 1, t, w1, shift, None, dtype, impl=impl)
+                out, _ = run_stem0(inp, fmt, w1, shift, cin=1, transform=t, dtype=dtype, impl=impl)
                 assert_faithful(out.float(), ref, S, K, dtype, 'gray stem0 Cout=%d %s fmt=%d impl=%d %dx%d' % (cout, dtype, fmt, impl, h, wd))
 
 
@@ -444,7 +411,7 @@ def test_refusals_launch_nothing():
                           (InputTransform(False, (1.0,) * 3, (0.5, 0.5, 0.25)), 1, LFD_ERR_INVALID),
                           (None, 2, LFD_ERR_UNSUPPORTED), (None, 4, LFD_ERR_UNSUPPORTED)):
         for impl in (nat.CONV_UMMA, nat.CONV_SIMT):
-            rc, ws = run_stem0(x, nat.INPUT_U8_NHWC, cin, tr, w1, shift, None, 'bf16', impl=impl, raw_rc=True)
+            rc, ws = run_stem0(x, nat.INPUT_U8_NHWC, w1, shift, cin=cin, transform=tr, impl=impl, raw_rc=True)
             assert rc == want and bool((ws == 0xff).all()), (tr, cin, impl, rc)
             if cin == 2:
                 assert '1' in nat.lib().lfd_last_error().decode() and '3' in nat.lib().lfd_last_error().decode()

@@ -19,6 +19,7 @@ import torch
 
 from gen_golden_input import synthetic_samples
 from gray_models import gray_pair
+from helpers import ListDataset
 from lfd import _native as nat
 from lfd.data_pipeline import sampler as S
 from lfd.data_pipeline.augmentation import Compose, HorizontalFlip, Normalize, bbox_param, pipeline_device_spec, simple_widerface_train_pipeline
@@ -177,20 +178,6 @@ def test_invalid_calls_write_nothing(case):
 
 
 # ------------------------------------------------------------------------------------------------------------------ loader
-class ListDataset(object):
-    def __init__(self, samples):
-        self.samples = dict(enumerate(samples))
-
-    def __len__(self):
-        return len(self.samples)
-
-    def __getitem__(self, i):
-        return self.samples[i]
-
-    def get_indexes(self):
-        return list(self.samples.keys())
-
-
 def _replay(ds, sampler, region, pipeline):
     """The loader's draws, in its order -> per batch the rule's items and the flipped annotations."""
     flip_p = {b: pipeline_device_spec(pipeline, b)[0] for b in (False, True)}

@@ -2,19 +2,16 @@
 """BGR -> RGB and any Normalize inside the stem kernels' uint8 path.  The defining property: the 16-bit value a loader builds for a
 pixel is the rounding of the fp32 number the host pipeline produces, so every op and every plan gives, on a uint8 frame under a
 transform, exactly what it gives on the float32 NCHW tensor the host stand-ins make of that frame."""
-import ctypes as C
-import functools
-
 import numpy as np
 import pytest
 import torch
 
 import synth
 import tl_s
-from gpu_ops import DTYPES, conv_out
-from helpers import synth_model
+from gpu_ops import DTYPES, conv_out, run_stem0
+from helpers import finetune_model, misaligned, model_of, same_bits, synth_model
 from lfd import _native as nat
-from lfd._engine import InferencePlan, fold_scale, pack_conv_weight, pack_stem_weight
+from lfd._engine import InferencePlan
 from lfd.data_pipeline.augmentation import (BGR2RGB, Compose, input_transform_of, simple_widerface_val_pipeline, standard_normalize,
                                             typical_coco_val_pipeline)
 from test_input_transform_host import opaque, tl_val_pipeline
@@ -54,41 +51,8 @@ def host_f32(pipeline, x_u8):
     return torch.from_numpy(np.ascontiguousarray(np.stack(out).transpose(0, 3, 1, 2)))
 
 
-def same_bits(a, b, what):
-    bad = a.view(torch.int16) != b.view(torch.int16)
-    if bool(bad.any()):
-        i = tuple(bad.nonzero()[0].tolist())
-        raise AssertionError('%s: %d of %d elements differ, first at %s: %r vs %r' % (what, int(bad.sum()), bad.numel(), i, float(a[i]), float(b[i])))
-
-
 # ------------------------------------------------------------------------------------------------------------------ single ops
-def run_stem0(x, transform, w, shift, tail, dtype, impl=nat.CONV_UMMA, max_ctas=0):
-    """LFD_OP_STEM0 through lfd_run_op on uint8 NHWC or float32 NCHW x -> [N, Ho, Wo, Cf]."""
-    tdt, code = DTYPES[dtype][0], DTYPES[dtype][3]
-    u8 = x.dtype == torch.uint8
-    N, H, W = (x.shape[0], x.shape[1], x.shape[2]) if u8 else (x.shape[0], x.shape[2], x.shape[3])
-    Cout = w.shape[0]
-    Ho, Wo = conv_out(H, 3, 2), conv_out(W, 3, 2)
-    Cf = tail[0].shape[0] if tail is not None else Cout
-    keep = [pack_stem_weight(w, tdt).cuda(), shift.float().cuda()]
-    out_b = N * Ho * Wo * Cf * 2
-    ws = torch.full((4096 + ((out_b + 255) & ~255) + 256,), 0xff, dtype=torch.uint8, device='cuda')
-    op = nat.Op()
-    op.kind, op.dtype = nat.OP_STEM0, code
-    op.N, op.H, op.W, op.Cin, op.Ho, op.Wo, op.Cout = N, H, W, 3, Ho, Wo, Cout
-    op.ksize, op.stride, op.relu, op.max_ctas = 3, 2, 1, max_ctas
-    op.in_off, op.out_off, op.res_off, op.stats_off, op.ds_out_off = -1, 4096, -1, -1, -1
-    op.weight, op.shift = keep[0].data_ptr(), keep[1].data_ptr()
-    if tail is not None:
-        keep += [pack_conv_weight(fold_scale(tail[0], torch.ones(Cf)), Cout, tdt).cuda(), tail[1].float().cuda()]
-        op.tail_cout, op.tail_relu, op.tail_weight, op.tail_shift = Cf, 1, keep[2].data_ptr(), keep[3].data_ptr()
-    nat.set_input_transform(op, transform)
-    nat.check(nat.lib().lfd_run_op(C.byref(op), nat.ptr(x), nat.INPUT_U8_NHWC if u8 else nat.INPUT_F32_NCHW, nat.ptr(ws), None, None, 0, 0,
-                                   impl, nat.stream_ptr()))
-    torch.cuda.synchronize()
-    return ws[4096:4096 + out_b].view(tdt).view(N, Ho, Wo, Cf).clone()
-
-
+U8, F32 = nat.INPUT_U8_NHWC, nat.INPUT_F32_NCHW
 SIZES = [(37, 40), (38, 41), (39, 42), (40, 43)]           # H and W = 0..3 (mod 4)
 
 
@@ -101,7 +65,7 @@ def test_stem0_on_u8_frames_equals_stem0_on_the_host_normalised_tensor(cout, dty
     g = torch.Generator().manual_seed(cout)
     w = torch.randn((cout, 3, 3, 3), generator=g) * 0.05
     shift = torch.randn(cout, generator=g) * 0.1
-    tail = (torch.randn((cout, cout, 1, 1), generator=g) * 0.1, torch.randn(cout, generator=g) * 0.1)
+    tail = (torch.randn((cout, cout, 1, 1), generator=g) * 0.1, torch.ones(cout), torch.randn(cout, generator=g) * 0.1, True)
     for h, wd in SIZES:
         x8 = frames(2, h, wd)
         xf = host_f32(host_pipe, x8).cuda()
@@ -109,11 +73,13 @@ def test_stem0_on_u8_frames_equals_stem0_on_the_host_normalised_tensor(cout, dty
         for t in (None, tail):
             for ctas in (0, 3):
                 what = 'stem0 Cout=%d%s %s %s %dx%d, max_ctas=%d' % (cout, ' + tail' if t else '', dtype, name, h, wd, ctas)
-                same_bits(run_stem0(x8, transform, w, shift, t, dtype, max_ctas=ctas), run_stem0(xf, None, w, shift, t, dtype, max_ctas=ctas), what)
-        ref = run_stem0(xf, None, w, shift, None, dtype, impl=nat.CONV_SIMT)
-        same_bits(run_stem0(x8, transform, w, shift, None, dtype, impl=nat.CONV_SIMT), ref, 'SIMT stem0 Cout=%d %s %s %dx%d' % (cout, dtype, name, h, wd))
+                same_bits(run_stem0(x8, U8, w, shift, tail=t, transform=transform, dtype=dtype, max_ctas=ctas)[0],
+                          run_stem0(xf, F32, w, shift, tail=t, dtype=dtype, max_ctas=ctas)[0], what)
+        ref = run_stem0(xf, F32, w, shift, dtype=dtype, impl=nat.CONV_SIMT)[0]
+        same_bits(run_stem0(x8, U8, w, shift, transform=transform, dtype=dtype, impl=nat.CONV_SIMT)[0], ref,
+                  'SIMT stem0 Cout=%d %s %s %dx%d' % (cout, dtype, name, h, wd))
         # the SIMT kernel stays the cross-check of the tensor-core path under every transform (one 16-bit spacing: fp32 summation order)
-        tc = run_stem0(x8, transform, w, shift, None, dtype).float()
+        tc = run_stem0(x8, U8, w, shift, transform=transform, dtype=dtype)[0].float()
         assert float((tc - ref.float()).abs().max()) <= DTYPES[dtype][2] * 2 * float(ref.float().abs().max()), (cout, dtype, name)
 
 
@@ -123,27 +89,13 @@ def test_zero_fields_are_the_simple_constants_and_todays_results():
     x8 = frames(2, 45, 61)
     xf = host_f32(simple_widerface_val_pipeline, x8).cuda()
     x8 = torch.from_numpy(x8).cuda()
-    zero = run_stem0(x8, None, w, shift, None, 'bf16')
-    same_bits(zero, run_stem0(x8, input_transform_of(simple_widerface_val_pipeline), w, shift, None, 'bf16'), 'zero fields vs explicit constants')
-    same_bits(zero, run_stem0(xf, None, w, shift, None, 'bf16'), 'zero fields vs fp32 simple_normalize')
-    same_bits(zero, run_stem0(xf, input_transform_of(tl_val_pipeline), w, shift, None, 'bf16'), 'the fp32 input ignores the transform')
+    zero = run_stem0(x8, U8, w, shift)[0]
+    same_bits(zero, run_stem0(x8, U8, w, shift, transform=input_transform_of(simple_widerface_val_pipeline))[0], 'zero fields vs explicit constants')
+    same_bits(zero, run_stem0(xf, F32, w, shift)[0], 'zero fields vs fp32 simple_normalize')
+    same_bits(zero, run_stem0(xf, F32, w, shift, transform=input_transform_of(tl_val_pipeline))[0], 'the fp32 input ignores the transform')
 
 
 # ------------------------------------------------------------------------------------------------------------------ plans
-@functools.lru_cache(maxsize=None)
-def model_of(name):
-    model = tl_s.synth_model()[0] if name == 'TL_S' else synth_model(name)[0]
-    return model.cuda().eval()
-
-
-def misaligned(x):
-    raw = torch.empty(x.numel() + 1, dtype=torch.uint8, device='cuda')
-    y = raw[1:].view(x.shape)                        # base address 1 (mod 4): the fused stem's per-pixel loader
-    y.copy_(x)
-    assert y.data_ptr() % 4 == 1
-    return y
-
-
 def run_plan(plan, x, graph=False):
     plan.workspace.fill_(0xff)
     with torch.no_grad():
@@ -168,7 +120,7 @@ def test_fused_stem_on_both_loaders(dtype, name):
     """STEM4 (WIDERFACE_S, forced): the word loader (W % 4 == 0, aligned base), the per-pixel loader (other widths, or a base address =
     1 mod 4): the stem3 map bit for bit, the head outputs up to the GroupNorm atomics."""
     kernel_pipe, host_pipe = TRANSFORMS[name]
-    model = model_of('WIDERFACE_S')
+    model = model_of('WIDERFACE_S', 'cuda')
     for h, w in ((186, 252), (185, 253), (187, 254), (184, 255)):
         plan = InferencePlan(model, 2, h, w, torch.device('cuda'), act_dtype=dtype, fuse_stem=True, input_transform=input_transform_of(kernel_pipe),
                              reuse=False)
@@ -194,7 +146,7 @@ def test_frames_below_the_capacity(cfg, fuse, name):
     """One 2 x 400 x 656 plan, frames of every width mod 4, every buffer pre-filled with 0xff: the frame's outputs on uint8 input are those
     of the same plan on the host-normalised tensor (columns past the width and rows past the height are zero AFTER normalisation)."""
     kernel_pipe, host_pipe = TRANSFORMS[name]
-    model = model_of(cfg)
+    model = model_of(cfg, 'cuda')
     plan = InferencePlan(model, 2, 400, 656, torch.device('cuda'), fuse_stem=fuse, input_transform=input_transform_of(kernel_pipe))
     assert plan._ops[0]['kind'] == (nat.OP_STEM4 if fuse else nat.OP_STEM0)
     for h, w in ((400, 656), (397, 652), (350, 653), (399, 654), (211, 655), (400, 329)):
@@ -287,7 +239,6 @@ def _step(model, x, ann):
 def test_training_step_on_u8_batches_equals_the_step_on_the_host_normalised_batch(cfg, frozen):
     """The stem conv, the im2col of its weight gradient and (fine-tuning) the frozen prefix's stem all read the uint8 batch under the
     transform: their outputs bit for bit, the loss and the flat gradient within the run-to-run tolerance of the fp32 atomics."""
-    from test_finetune_plan import finetune_model
     n, h, w = 2, 128, 160
     x8 = frames(n, h, w, seed=9)
     xf = host_f32(tl_val_pipeline, x8).cuda()
@@ -295,7 +246,7 @@ def test_training_step_on_u8_batches_equals_the_step_on_the_host_normalised_batc
     ann = synth.synth_annotations(n, h, w, 1, seed=5)
     res = []
     for x in (x8, xf):
-        model = (finetune_model(cfg, frozen) if frozen else synth_model(cfg, cls_bias=-2.0)[0]).cuda().train()
+        model = (finetune_model(cfg, frozen, -1.0) if frozen else synth_model(cfg, cls_bias=-2.0)[0]).cuda().train()
         model.set_input_transform(tl_val_pipeline)
         loss, grad = _step(model, x, ann)
         plan = model.train_plan_for(n, h, w, x.device)

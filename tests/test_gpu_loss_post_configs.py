@@ -17,6 +17,7 @@ import pytest
 import torch
 
 import loss_post_ref as ref
+from helpers import grids_agree
 from lfd import _native as nat
 from oracle import lfd_oracle as orc
 
@@ -266,14 +267,6 @@ def assert_within(got, want, S, K, what):
                                                                                             float(want[i]), float(tol[i])))
 
 
-def _grids_agree(results, what):
-    g0 = results[0]
-    for r in results[1:]:
-        for a, b in zip(g0[:2], r[:2]):
-            assert torch.equal(a.view(torch.int32), b.view(torch.int32)), what + ': gradients differ between grids'
-        assert bool(((r[2] - g0[2]).abs() <= 1e-12 * g0[2].abs() + 1e-300).all()), (what, r[2], g0[2])
-
-
 LOSS_LV = ref.level_table(LOSS_LEVELS)
 
 
@@ -289,7 +282,7 @@ def test_classification_loss_elementwise(case):
     cfg = dict(N=LOSS_N, P=P, C=C_, cls_mode=mode, bbox_mode=0, reg_loss=0, gamma=gamma, alpha=alpha, reg_eps=1e-6, smooth_l1_beta=1.0,
                cls_weight=1.7, reg_weight=1.0)
     res = [run_loss(cfg, LOSS_LV, x, reg, q, rt, lab, cnt, m) for m in GRIDS]
-    _grids_agree(res, _cls_id(case))
+    grids_agree(res, _cls_id(case))
     gc, _, sums = res[0]
     l, g, sl, sg = ref.cls_ref(mode, x, lab, C_, gamma, alpha, q)
     scale = 1.7 / (int(cnt[0]) + 1)
@@ -352,7 +345,7 @@ def test_regression_loss_elementwise(case):
     cfg = dict(N=LOSS_N, P=LOSS_LV['P'], C=1, cls_mode=0, bbox_mode=bbox, reg_loss=kind, gamma=2.0, alpha=0.25, reg_eps=eps, smooth_l1_beta=beta,
                cls_weight=1.0, reg_weight=1.3)
     res = [run_loss(cfg, LOSS_LV, x, raw, np.zeros((rows, 1), np.float32), t, lab, cnt, m) for m in GRIDS]
-    _grids_agree(res, _reg_id(case))
+    grids_agree(res, _reg_id(case))
     _, gr, sums = res[0]
     pos = np.nonzero(lab == 0)[0]
     px, py = np.tile(pt['px'], LOSS_N)[pos], np.tile(pt['py'], LOSS_N)[pos]

@@ -22,7 +22,7 @@ import loss_weighting_ref as wref
 import synth
 import test_gpu_loss_post_configs as lpc
 from aten_train_reference import train_forward as aten_train_forward
-from helpers import synth_model
+from helpers import grids_agree, synth_model
 from lfd import _native as nat
 from loss_weighting_ref import U, assert_close
 
@@ -61,15 +61,6 @@ def run_weighted(cfg_vals, lv, x, reg, q, rt, lab, cw, rw, max_ctas):
     return gc.cpu(), gr.cpu(), sums.cpu(), wsum.cpu()
 
 
-def _grids_agree(res, what):
-    g0 = res[0]
-    for r in res[1:]:
-        for a, b in zip(g0[:2], r[:2]):
-            assert torch.equal(a.view(torch.int32), b.view(torch.int32)), what + ': gradients differ between grids'
-        for a, b in zip(g0[2:], r[2:]):   # fp64 sums in another order: the same to ~1e-15
-            assert bool(((a - b).abs() <= 1e-12 * a.abs() + 1e-300).all()), (what, a, b)
-
-
 def _id(k):
     return '%s-%s-cw%d-rw%d-%s' % (k[0], k[1], k[2], k[3], k[4])
 
@@ -90,7 +81,7 @@ def test_golden_cases_per_element(key):
     cfg = dict(N=GOLDEN['N'], P=lv['P'], C=Cn, cls_mode=wref.CLS_CODES[cname], bbox_mode=wref.BBOX_CODES[case['bbox']], reg_loss=wref.REG_CODES[rname],
                gamma=gamma, alpha=alpha, reg_eps=eps, smooth_l1_beta=beta, cls_weight=clw, reg_weight=rlw)
     res = [run_weighted(cfg, lv, x, raw, ct, rt, lab, cw, rw, m) for m in GRIDS]
-    _grids_agree(res, _id(key))
+    grids_agree(res, _id(key))
     gc, gr, sums, wsum = res[0]
     r = wref.golden_case_ref(GOLDEN, key)
     assert abs(float(wsum[0]) - r['weight_sum']) <= 1e-12 * r['weight_sum']
@@ -184,7 +175,7 @@ def test_classification_weighting_under_forced_grids(mode):
     cfg = dict(N=lpc.LOSS_N, P=rows // lpc.LOSS_N, C=2, cls_mode=mode, bbox_mode=0, reg_loss=0, gamma=1.5, alpha=0.5, reg_eps=1e-6, smooth_l1_beta=1.0,
                cls_weight=1.7, reg_weight=1.0)
     res = [run_weighted(cfg, lpc.LOSS_LV, x, reg, q, rt, lab, 1, 0, m) for m in GRIDS]
-    _grids_agree(res, 'cls mode %d' % mode)
+    grids_agree(res, 'cls mode %d' % mode)
     # the weight sum is deterministic: the same bits on a repeated call
     assert torch.equal(run_weighted(cfg, lpc.LOSS_LV, x, reg, q, rt, lab, 1, 0, 1)[3], res[1][3])
     gc, _, sums, wsum = res[0]
@@ -207,7 +198,7 @@ def test_regression_weighting_under_forced_grids(kind, bbox):
     cfg = dict(N=lpc.LOSS_N, P=lpc.LOSS_LV['P'], C=1, cls_mode=0, bbox_mode=bbox, reg_loss=kind, gamma=2.0, alpha=0.25, reg_eps=1e-6,
                smooth_l1_beta=1.0, cls_weight=1.0, reg_weight=1.3)
     res = [run_weighted(cfg, lpc.LOSS_LV, x, raw, q, t, lab, 0, 1, m) for m in GRIDS]
-    _grids_agree(res, 'reg kind %d bbox %d' % (kind, bbox))
+    grids_agree(res, 'reg kind %d bbox %d' % (kind, bbox))
     _, gr, sums, wsum = res[0]
     pos = np.nonzero(lab == 0)[0]
     w = q[pos, 0].astype(np.float64)

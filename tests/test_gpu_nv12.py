@@ -3,17 +3,16 @@
 uint8 BGR path gives on cv2.cvtColor(f, cv2.COLOR_YUV2BGR_NV12) (tests/nv12_oracle.py) under the same input transform.  Every comparison
 here runs the same op or plan on the NV12 frames and on their oracle BGR frames."""
 import ctypes as C
-import functools
 
 import numpy as np
 import pytest
 import torch
 
-import tl_s
-from gpu_ops import DTYPES, conv_out
-from helpers import synth_model
+from gpu_ops import run_stem0
+from helpers import (CONV_KINDS, close_downstream_of_gn, downstream_of_gn, misaligned, model_of, poison, same_bits, synth_model,
+                     untouched)
 from lfd import _native as nat
-from lfd._engine import InferencePlan, fold_scale, pack_conv_weight, pack_stem_weight
+from lfd._engine import InferencePlan
 from lfd.data_pipeline.augmentation import BGR2RGB, Compose, input_transform_of, simple_widerface_val_pipeline, typical_coco_val_pipeline
 from nv12_oracle import nv12_frames, nv12_oracle
 from test_input_transform_host import tl_val_pipeline
@@ -38,52 +37,6 @@ def frames(n, h, w, seed=0):
     return torch.from_numpy(x).cuda(), torch.from_numpy(nv12_oracle(x)).cuda()
 
 
-def same_bits(a, b, what):
-    bad = a.view(torch.int16) != b.view(torch.int16)
-    if bool(bad.any()):
-        i = tuple(bad.nonzero()[0].tolist())
-        raise AssertionError('%s: %d of %d elements differ, first at %s: %r vs %r' % (what, int(bad.sum()), bad.numel(), i, float(a[i]), float(b[i])))
-
-
-def misaligned(x):
-    raw = torch.empty(x.numel() + 1, dtype=torch.uint8, device='cuda')
-    y = raw[1:].view(x.shape)                        # base address 1 (mod 4): the fused stem's per-pixel loader
-    y.copy_(x)
-    assert y.data_ptr() % 4 == 1
-    return y
-
-
-# ------------------------------------------------------------------------------------------------------------------ single ops
-def run_stem0(x, fmt, transform, w, shift, tail, dtype, impl=nat.CONV_UMMA, max_ctas=0, raw_rc=False):
-    """LFD_OP_STEM0 through lfd_run_op on uint8 BGR [N, H, W, 3] or NV12 [N, 3H/2, W] x -> [N, Ho, Wo, Cf]
-    (raw_rc: -> (lfd_run_op's return code, the workspace))."""
-    tdt, code = DTYPES[dtype][0], DTYPES[dtype][3]
-    N, H, W = (x.shape[0], x.shape[1], x.shape[2]) if fmt == nat.INPUT_U8_NHWC else (x.shape[0], x.shape[1] * 2 // 3, x.shape[2])
-    Cout = w.shape[0]
-    Ho, Wo = conv_out(H, 3, 2), conv_out(W, 3, 2)
-    Cf = tail[0].shape[0] if tail is not None else Cout
-    keep = [pack_stem_weight(w, tdt).cuda(), shift.float().cuda()]
-    out_b = N * Ho * Wo * Cf * 2
-    ws = torch.full((4096 + ((out_b + 255) & ~255) + 256,), 0xff, dtype=torch.uint8, device='cuda')
-    op = nat.Op()
-    op.kind, op.dtype = nat.OP_STEM0, code
-    op.N, op.H, op.W, op.Cin, op.Ho, op.Wo, op.Cout = N, H, W, 3, Ho, Wo, Cout
-    op.ksize, op.stride, op.relu, op.max_ctas = 3, 2, 1, max_ctas
-    op.in_off, op.out_off, op.res_off, op.stats_off, op.ds_out_off = -1, 4096, -1, -1, -1
-    op.weight, op.shift = keep[0].data_ptr(), keep[1].data_ptr()
-    if tail is not None:
-        keep += [pack_conv_weight(fold_scale(tail[0], torch.ones(Cf)), Cout, tdt).cuda(), tail[1].float().cuda()]
-        op.tail_cout, op.tail_relu, op.tail_weight, op.tail_shift = Cf, 1, keep[2].data_ptr(), keep[3].data_ptr()
-    nat.set_input_transform(op, transform)
-    torch.cuda.synchronize()
-    rc = nat.lib().lfd_run_op(C.byref(op), nat.ptr(x), fmt, nat.ptr(ws), None, None, 0, 0, impl, nat.stream_ptr())
-    torch.cuda.synchronize()
-    if raw_rc:
-        return rc, ws
-    nat.check(rc)
-    return ws[4096:4096 + out_b].view(tdt).view(N, Ho, Wo, Cf).clone()
-
-
 SIZES = [(40, 44), (42, 46), (40, 46), (42, 44)]           # H and W = 0 and 2 (mod 4)
 
 
@@ -95,53 +48,27 @@ def test_stem0_on_nv12_frames_equals_stem0_on_the_converted_frames(cout, dtype, 
     g = torch.Generator().manual_seed(cout)
     w = torch.randn((cout, 3, 3, 3), generator=g) * 0.05
     shift = torch.randn(cout, generator=g) * 0.1
-    tail = (torch.randn((cout, cout, 1, 1), generator=g) * 0.1, torch.randn(cout, generator=g) * 0.1)
+    tail = (torch.randn((cout, cout, 1, 1), generator=g) * 0.1, torch.ones(cout), torch.randn(cout, generator=g) * 0.1, True)
     for h, wd in SIZES:
         nv, bgr = frames(2, h, wd, seed=cout)
         for t in (None, tail):
             for ctas in (0, 3):
                 what = 'stem0 Cout=%d%s %s %s %dx%d, max_ctas=%d' % (cout, ' + tail' if t else '', dtype, name, h, wd, ctas)
-                same_bits(run_stem0(nv, nat.INPUT_U8_NV12, transform, w, shift, t, dtype, max_ctas=ctas),
-                          run_stem0(bgr, nat.INPUT_U8_NHWC, transform, w, shift, t, dtype, max_ctas=ctas), what)
-        same_bits(run_stem0(nv, nat.INPUT_U8_NV12, transform, w, shift, None, dtype, impl=nat.CONV_SIMT),
-                  run_stem0(bgr, nat.INPUT_U8_NHWC, transform, w, shift, None, dtype, impl=nat.CONV_SIMT),
+                same_bits(run_stem0(nv, nat.INPUT_U8_NV12, w, shift, tail=t, transform=transform, dtype=dtype, max_ctas=ctas)[0],
+                          run_stem0(bgr, nat.INPUT_U8_NHWC, w, shift, tail=t, transform=transform, dtype=dtype, max_ctas=ctas)[0], what)
+        same_bits(run_stem0(nv, nat.INPUT_U8_NV12, w, shift, transform=transform, dtype=dtype, impl=nat.CONV_SIMT)[0],
+                  run_stem0(bgr, nat.INPUT_U8_NHWC, w, shift, transform=transform, dtype=dtype, impl=nat.CONV_SIMT)[0],
                   'SIMT stem0 Cout=%d %s %s %dx%d' % (cout, dtype, name, h, wd))
 
 
 # ------------------------------------------------------------------------------------------------------------------ plans
-@functools.lru_cache(maxsize=None)
-def model_of(name):
-    model = tl_s.synth_model()[0] if name == 'TL_S' else synth_model(name)[0]
-    return model.cuda().eval()
-
-
-CONV_KINDS = (nat.OP_STEM0, nat.OP_CONV, nat.OP_STEM4)
-
-
-def _downstream_of_gn(plan):
-    tainted = set()
-    for op in plan._ops:
-        if op['kind'] == nat.OP_GN_APPLY or any(op.get(k) in tainted for k in ('inp', 'res')):
-            tainted |= {op[k] for k in ('out', 'out2') if op.get(k) is not None}
-    return tainted
-
-
 def _has_gn(plan):
     return any(op['kind'] == nat.OP_GN_APPLY or (op['kind'] == nat.OP_HEAD_FINAL and op.get('gn_groups')) for op in plan._ops)
 
 
-def _poison(plan):
-    plan.workspace.fill_(0xff)
-    if plan._stage is not None:
-        plan._stage.fill_(0xff)
-    for c, r in plan._outputs:
-        c.view(torch.uint8).fill_(0xff)
-        r.view(torch.uint8).fill_(0xff)
-
-
 def snapshot(plan, x, frame_format, graph, h, w):
     """Forward of x on a poisoned plan (built with reuse=False) -> (conv outputs cropped to the frame's valid region, cls, reg)."""
-    _poison(plan)
+    poison(plan)
     with torch.no_grad():
         for _ in range(2 if graph else 1):
             cls, reg = plan.forward(x, use_graph=graph, frame_format=frame_format)
@@ -156,28 +83,21 @@ def snapshot(plan, x, frame_format, graph, h, w):
     return tensors, cls.clone(), reg.clone()
 
 
-def _close(what, a, b):
-    """Downstream of a GroupNorm: its fp64 statistics atomics add in another order from run to run (test_gpu_schedule_invariance.py)."""
-    assert bool(torch.isfinite(a).all()), what
-    d = (a - b).abs()
-    assert float(d.max()) <= 2.0 ** -6 * float(b.abs().max()), (what, float(d.max()), int((d > 0).sum()))
-
-
 def compare(what, plan, got, ref):
     """Every conv output that does not depend on a GroupNorm bit for bit; the rest, and the heads of GroupNorm configs, up to the fp64
     atomics of the statistics; the heads of the other configs bit for bit."""
-    tainted = _downstream_of_gn(plan)
+    tainted = downstream_of_gn(plan)
     (gt, gc, gr), (rt, rc, rr) = got, ref
     assert sorted(gt) == sorted(rt)
     for name in rt:
         if name in tainted:
-            _close('%s: %s' % (what, name), gt[name].float(), rt[name].float())
+            close_downstream_of_gn('%s: %s' % (what, name), gt[name].float(), rt[name].float())
         else:
             same_bits(gt[name], rt[name], '%s: %s' % (what, name))
     assert gc.shape == rc.shape and gr.shape == rr.shape, what
     if _has_gn(plan):
-        _close(what + ': cls', gc, rc)
-        _close(what + ': reg', gr, rr)
+        close_downstream_of_gn(what + ': cls', gc, rc)
+        close_downstream_of_gn(what + ': reg', gr, rr)
     else:
         assert torch.equal(gc, rc) and torch.equal(gr, rr), '%s: head outputs differ' % what
 
@@ -188,7 +108,7 @@ def test_fused_stem_on_both_loaders(dtype, name):
     """STEM4 (WIDERFACE_S, forced): the word loader (W % 4 == 0 at an aligned base), the per-pixel loader (W % 4 == 2, or a base address
     = 1 mod 4); the default grid and the stem bounded to 1, 7 and 131 CTAs (runs that start mid-row and cross images): the stem3 map bit
     for bit against the same plan on the converted frames."""
-    model = model_of('WIDERFACE_S')
+    model = model_of('WIDERFACE_S', 'cuda')
     for h, w in ((186, 252), (186, 254), (188, 250)):
         plan = InferencePlan(model, 2, h, w, torch.device('cuda'), act_dtype=dtype, fuse_stem=True, input_transform=input_transform_of(TRANSFORMS[name]),
                              reuse=False)
@@ -214,7 +134,7 @@ PLANS = [('WIDERFACE_S', True, 'bf16'), ('WIDERFACE_S', False, 'bf16'), ('TL_L',
 
 @pytest.mark.parametrize('cfg,fuse,dtype', PLANS)
 def test_whole_plans(cfg, fuse, dtype):
-    model = model_of(cfg)
+    model = model_of(cfg, 'cuda')
     plan = InferencePlan(model, 2, 400, 656, torch.device('cuda'), act_dtype=dtype, fuse_stem=fuse,
                          input_transform=input_transform_of(tl_val_pipeline if cfg.startswith('TL') else None), reuse=False)
     assert (plan._ops[0]['kind'] == nat.OP_STEM4) == bool(fuse)
@@ -234,7 +154,7 @@ def test_frames_below_the_capacity(cfg, fuse):
     """One 2 x 400 x 656 plan, a scrambled sequence of even frame sizes, every buffer pre-filled with 0xff before each frame: each NV12
     frame gives what its converted BGR frame gives on the same plan; two graphs per format (the caller's tensor at the capacity, the
     plan's staging buffer below it)."""
-    model = model_of(cfg)
+    model = model_of(cfg, 'cuda')
     plan = InferencePlan(model, 2, 400, 656, torch.device('cuda'), fuse_stem=fuse, reuse=False,
                          input_transform=input_transform_of(tl_val_pipeline if cfg.startswith('TL') else None))
     assert (plan._ops[0]['kind'] == nat.OP_STEM4) == bool(fuse)
@@ -288,20 +208,6 @@ def test_streaming_detector_on_nv12_frames(cfg, pipeline):
 
 
 # ------------------------------------------------------------------------------------------------------------------ errors
-def _untouched(plan, call):
-    """call() must fail before anything reaches the device: the workspace, the outputs and the staging keep their bytes."""
-    plan.staging(nat.INPUT_U8_NHWC)
-    _poison(plan)
-    torch.cuda.synchronize()
-    with pytest.raises((ValueError, nat.LfdError)) as e:
-        call()
-    torch.cuda.synchronize()
-    assert bool((plan.workspace == 0xff).all()) and bool((plan._stage == 0xff).all())
-    for c, r in plan._outputs:
-        assert bool((c.view(torch.uint8) == 0xff).all()) and bool((r.view(torch.uint8) == 0xff).all())
-    return str(e.value)
-
-
 def _rc(plan, call):
     """The return code of a C entry point that must fail before anything is enqueued."""
     box = []
@@ -309,20 +215,20 @@ def _rc(plan, call):
     def run():
         box.append(call())
         nat.check(box[-1])
-    _untouched(plan, run)
+    untouched(plan, run)
     return box[0]
 
 
 def test_errors_launch_nothing():
-    model = model_of('TEST_FAST')
+    model = model_of('TEST_FAST', 'cuda')
     lib = nat.lib()
     plan = InferencePlan(model, 2, 96, 160, torch.device('cuda'))
     # the host checks
     for shape in [(2, 145, 160), (2, 144, 161), (2, 96, 160, 3), (3, 144, 160), (1, 144, 160), (2, 150, 160), (2, 144, 162)]:
         x = torch.zeros(shape, dtype=torch.uint8, device='cuda')
-        _untouched(plan, lambda: plan.forward(x, frame_format='nv12'))
+        untouched(plan, lambda: plan.forward(x, frame_format='nv12'))
     x = torch.zeros((2, 96, 160, 3), dtype=torch.uint8, device='cuda')
-    assert 'frame_format' in _untouched(plan, lambda: plan.forward(x, frame_format='i420'))
+    assert 'frame_format' in untouched(plan, lambda: plan.forward(x, frame_format='i420'))
     # the C entry points: an odd frame, a format outside 0..2
     stage = plan.staging(nat.INPUT_U8_NV12)
     ms = (C.c_float * lib.lfd_plan_num_launches(plan.handle))()
@@ -349,7 +255,7 @@ def test_errors_launch_nothing():
         # NV12 on a plan of odd capacity
         odd = InferencePlan(model, 2, 97, 160, torch.device('cuda'))
         x = torch.zeros((2, 97 * 3 // 2 + 1, 160), dtype=torch.uint8, device='cuda')
-        assert 'even' in _untouched(odd, lambda: odd.forward(x, frame_format='nv12'))
+        assert 'even' in untouched(odd, lambda: odd.forward(x, frame_format='nv12'))
         assert _rc(odd, forward(odd, nat.INPUT_U8_NV12, x)) == LFD_ERR_UNSUPPORTED
         assert _rc(odd, profile(odd, nat.INPUT_U8_NV12, x)) == LFD_ERR_UNSUPPORTED
         ostage = odd.staging(nat.INPUT_U8_NHWC)
@@ -361,7 +267,7 @@ def test_errors_launch_nothing():
     for H, W, fmt, want in ((40, 45, nat.INPUT_U8_NV12, LFD_ERR_UNSUPPORTED), (40, 44, 3, LFD_ERR_INVALID), (40, 44, -2, LFD_ERR_INVALID)):
         x = torch.zeros((2, H * 3 // 2, W), dtype=torch.uint8, device='cuda')
         for impl in (nat.CONV_UMMA, nat.CONV_SIMT):
-            rc, ws = run_stem0(x, fmt, None, w, torch.zeros(16), None, 'bf16', impl=impl, raw_rc=True)
+            rc, ws = run_stem0(x, fmt, w, torch.zeros(16), impl=impl, raw_rc=True)
             assert rc == want and bool((ws == 0xff).all()), (H, W, fmt, impl, rc)
     # training refuses NV12 (UNSUPPORTED) and any format outside 0..2 (INVALID), before anything is enqueued
     tm = synth_model('TL_L', cls_bias=-2.0)[0].cuda().train()

@@ -6,33 +6,20 @@ import pytest
 import torch
 
 import synth
-from helpers import synth_model
+from helpers import conv_outputs, downstream_of_gn, synth_model
 from lfd import _native as nat
 from lfd._engine import InferencePlan
 
 pytestmark = pytest.mark.gpu
 
 N, H, W = 2, 200, 328
-CONV_KINDS = (nat.OP_STEM0, nat.OP_CONV, nat.OP_STEM4)
-
-
-def _conv_outputs(plan):
-    return [op[k] for op in plan._ops if op['kind'] in CONV_KINDS for k in ('out', 'out2') if op.get(k) is not None]
-
-
-def _downstream_of_gn(plan):
-    tainted = set()
-    for op in plan._ops:
-        if op['kind'] == nat.OP_GN_APPLY or any(op.get(k) in tainted for k in ('inp', 'res')):
-            tainted |= {op[k] for k in ('out', 'out2') if op.get(k) is not None}
-    return tainted
 
 
 def _run(plan, x):
     with torch.no_grad():
         cls, reg = plan.forward(x, use_graph=False)
     torch.cuda.synchronize()
-    return {name: plan.tensor(name).clone() for name in _conv_outputs(plan)}, cls.clone(), reg.clone()
+    return {name: plan.tensor(name).clone() for name, _ in conv_outputs(plan)}, cls.clone(), reg.clone()
 
 
 def _bound_every_op(plan, m):
@@ -59,7 +46,7 @@ def test_plan_outputs_do_not_depend_on_the_grid(name, fuse_stem):
     if fuse_stem:
         assert plan._ops[0]['kind'] == nat.OP_STEM4
     has_gn = any(op['kind'] == nat.OP_GN_APPLY or (op['kind'] == nat.OP_HEAD_FINAL and op.get('gn_groups')) for op in plan._ops)
-    gn_tainted = _downstream_of_gn(plan)
+    gn_tainted = downstream_of_gn(plan)
     x = synth.synth_input(N, H, W, seed=3).cuda()
     base, cls0, reg0 = _run(plan, x)
     for m in (1, 5):

@@ -14,8 +14,8 @@ import math
 import pytest
 import torch
 
-from gpu_ops import DTYPES, conv_out, stem_input
-from gpu_train_ops import (Workspace, bf16r, cdiv, desc_table, elementwise_blocks, gn_bwd_blocks, grid_sms, head_bwd_grid, make_top,
+from gpu_ops import DTYPES, bf16r, conv_out, make_op, stem_input
+from gpu_train_ops import (Workspace, cdiv, desc_table, elementwise_blocks, gn_bwd_blocks, grid_sms, head_bwd_grid, make_top,
                            reduce_blocks, run_top, stem_wgrad_grid, assert_within)
 from train_op_ref import (bn_apply_ref, bn_bwd_ref, bn_running_ref, bn_stats_ref, check_amb, check_faithful, check_within, conv_pack_ref,
                           gn_bwd_ref, head_activation, head_backward_ref, head_forward_ref)
@@ -447,7 +447,7 @@ def test_head_final_forward_and_backward_match_fp64(case, max_ctas):
 @pytest.mark.gpu
 @pytest.mark.parametrize('dtype', ['bf16', 'fp16'])
 def test_inference_gn_apply_matches_fp64(dtype):
-    tdt, rnd, _, code = DTYPES[dtype]
+    tdt, rnd = DTYPES[dtype][:2]
     N, H, W, G = 3, 31, 33, 16
     C, HW = 8 * G, H * W
     g = torch.Generator().manual_seed(41)
@@ -463,10 +463,8 @@ def test_inference_gn_apply_matches_fp64(dtype):
     ws.add('out', torch.full((N, HW, C), float('nan')).to(tdt))
     ws.finalize()
     g_d, b_d = gamma.to(DEV), beta.to(DEV)
-    op = nat.Op()
-    op.kind, op.dtype, op.N, op.H, op.W, op.Cin, op.Cout, op.gn_groups = nat.OP_GN_APPLY, code, N, H, W, C, C, G
-    op.in_off, op.out_off, op.stats_off, op.res_off, op.ds_out_off = ws.off('in'), ws.off('out'), ws.off('stats'), -1, -1
-    op.gamma, op.beta, op.max_ctas = g_d.data_ptr(), b_d.data_ptr(), 1
+    op = make_op(nat.OP_GN_APPLY, dtype, N=N, H=H, W=W, Cin=C, Cout=C, gn_groups=G, in_off=ws.off('in'), out_off=ws.off('out'),
+                 stats_off=ws.off('stats'), gamma=g_d.data_ptr(), beta=b_d.data_ptr(), max_ctas=1)
     _run_op(op, ws)
     a, a_b, amb = _head_activation(x, gamma, beta, stats, 16, dtype)
     got = ws.get('out').cpu().double()
@@ -487,7 +485,7 @@ def _run_op(op, ws, cls=None, reg=None, P=0, cls_channels=0):
 @pytest.mark.parametrize('case', [c for c in HEAD_CASES if c[3] == 3 and c[1] + c[2] in (5, 6, 45, 64)], ids=_head_id)
 def test_inference_head_final_matches_fp64(case, dtype):
     groups, nc, nr, N, H, W = case
-    tdt, rnd, _, code = DTYPES[dtype]
+    tdt = DTYPES[dtype][0]
     C, HW, no = 128, H * W, nc + nr
     raw, gamma, beta, w, bias, scale, shift, gcls, greg, stats, point_off, cls_stride, P = _head_operands(case, dtype)
     tiles, bx = cdiv(HW, 128), min(cdiv(4, N), cdiv(HW, 128))           # head_final_launch with one SM
@@ -498,11 +496,9 @@ def test_inference_head_final_matches_fp64(case, dtype):
     ws.finalize()
     w_d, sc_d, sh_d, g_d, b_d = w.to(DEV), scale.to(DEV), shift.to(DEV), gamma.to(DEV), beta.to(DEV)
     cls_o, reg_o = torch.full((N, P, cls_stride), float('nan'), device=DEV), torch.full((N, P, 4), float('nan'), device=DEV)
-    op = nat.Op()
-    op.kind, op.dtype, op.N, op.H, op.W, op.Cin, op.Cout, op.gn_groups = nat.OP_HEAD_FINAL, code, N, H, W, C, no, groups
-    op.n_cls, op.n_reg, op.point_off = nc, nr, point_off
-    op.in_off, op.out_off, op.stats_off, op.res_off, op.ds_out_off = ws.off('in'), -1, ws.off('stats') if groups else -1, -1, -1
-    op.weight, op.scale, op.shift, op.max_ctas = w_d.data_ptr(), sc_d.data_ptr(), sh_d.data_ptr(), 1
+    op = make_op(nat.OP_HEAD_FINAL, dtype, N=N, H=H, W=W, Cin=C, Cout=no, gn_groups=groups, n_cls=nc, n_reg=nr, point_off=point_off,
+                 in_off=ws.off('in'), stats_off=ws.off('stats' if groups else None), weight=w_d.data_ptr(), scale=sc_d.data_ptr(),
+                 shift=sh_d.data_ptr(), max_ctas=1)
     if groups:
         op.gamma, op.beta = g_d.data_ptr(), b_d.data_ptr()
     _run_op(op, ws, cls_o, reg_o, P, cls_stride)

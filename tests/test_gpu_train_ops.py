@@ -10,14 +10,11 @@ import torch.nn.functional as F
 
 from lfd import _native as nat
 from lfd._engine import pack_conv_weight, pack_stem_weight
-from gpu_train_ops import Workspace, make_top, run_top, desc_table, bf16r
+from gpu_ops import bf16r, conv_out
+from gpu_train_ops import Workspace, make_top, run_top, desc_table
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
-
-
-def conv_out(size, k, s):
-    return (size + 2 * (k // 2) - k) // s + 1
 
 
 def rel(a, b):

@@ -13,14 +13,13 @@ import pytest
 import torch
 
 import synth
-from helpers import synth_model
+from helpers import close_downstream_of_gn, conv_outputs, downstream_of_gn, poison, synth_model, untouched
 from lfd import _native as nat
 from lfd._engine import InferencePlan
 
 pytestmark = pytest.mark.gpu
 
 N, H, W = 2, 400, 656
-CONV_KINDS = (nat.OP_STEM0, nat.OP_CONV, nat.OP_STEM4)
 # the capacity; every h mod 4 and w mod 4; deepest levels of 1 x 1 (100 x 120, 37 x 5); the smallest frame; widths with and without the
 # stem4 word loader's w % 4 == 0 (the capacity, 656, always has it)
 SIZES = [(400, 656), (399, 655), (398, 654), (397, 653), (396, 652), (257, 130), (130, 259), (100, 120), (37, 5), (1, 1)]
@@ -34,32 +33,11 @@ def _order(seed):
     return [SIZES[0]] + seq[:9] + [SIZES[0]] + seq[9:]
 
 
-def _conv_outputs(plan):
-    return [(op[k], op) for op in plan._ops if op['kind'] in CONV_KINDS for k in ('out', 'out2') if op.get(k) is not None]
-
-
-def _downstream_of_gn(plan):
-    tainted = set()
-    for op in plan._ops:
-        if op['kind'] == nat.OP_GN_APPLY or any(op.get(k) in tainted for k in ('inp', 'res')):
-            tainted |= {op[k] for k in ('out', 'out2') if op.get(k) is not None}
-    return tainted
-
-
 def _frames(h, w, seed):
     g = torch.Generator().manual_seed(seed)
     u8 = torch.randint(0, 256, (N, h, w, 3), dtype=torch.uint8, generator=g)
     f32 = synth.synth_input(N, h, w, seed=seed)
     return {nat.INPUT_U8_NHWC: u8.cuda(), nat.INPUT_F32_NCHW: f32.cuda().contiguous()}
-
-
-def _poison(plan):
-    plan.workspace.fill_(0xff)
-    if plan._stage is not None:
-        plan._stage.fill_(0xff)
-    for c, r in plan._outputs:
-        c.view(torch.uint8).fill_(0xff)
-        r.view(torch.uint8).fill_(0xff)
 
 
 class _Exact(object):
@@ -75,7 +53,7 @@ class _Exact(object):
             with torch.no_grad():
                 cls, reg = plan.forward(x, use_graph=False)
             torch.cuda.synchronize()
-            tensors = {name: plan.tensor(name).clone() for name, _ in _conv_outputs(plan)}
+            tensors = {name: plan.tensor(name).clone() for name, _ in conv_outputs(plan)}
             self.cache[key] = (tensors, cls.clone(), reg.clone(), plan.level_sizes, _stats(plan))
             del plan
         return self.cache[key]
@@ -100,30 +78,20 @@ def _compare(what, plan, exact, cls, reg, has_gn, tainted):
             s2, es2 = st[k * per_slot + 1:(k + 1) * per_slot:2], estats[k * per_slot + 1:(k + 1) * per_slot:2]
             assert bool(((s2 - es2).abs() <= 1e-5 * es2.abs()).all()), (what, op['out'], 'GroupNorm statistics',
                                                                         float(((s2 - es2).abs() / es2.abs()).max()))
-    for name, op in _conv_outputs(plan):
+    for name, op in conv_outputs(plan):
         want = tensors[name]
         got = plan.tensor(name)[:, :want.shape[1], :want.shape[2]]
         if name not in tainted:
             assert torch.equal(got.view(torch.int16), want.view(torch.int16)), '%s: %s differs in %d of %d elements' % (
                 what, name, int((got.view(torch.int16) != want.view(torch.int16)).sum()), want.numel())
         else:
-            _close(what + ': ' + name, got.float(), want.float())
+            close_downstream_of_gn(what + ': ' + name, got.float(), want.float())
     assert cls.shape == ecls.shape and reg.shape == ereg.shape, (what, cls.shape, ecls.shape)
     if not has_gn:
         assert torch.equal(cls, ecls) and torch.equal(reg, ereg), '%s: head outputs differ' % what
     else:
-        _close(what + ': cls', cls, ecls)
-        _close(what + ': reg', reg, ereg)
-
-
-def _close(what, a, b):
-    """Results downstream of a GroupNorm, whose statistics (checked above) come from fp64 atomics that add in another order on another
-    grid: a flipped last bit of one group's mean or rstd moves every value of the group, so the number of differing elements depends on
-    the map size and the 16-bit type; the largest difference keeps the bound of test_gpu_schedule_invariance.py.  A value read from
-    outside the frame would be NaN (or 255-based) instead."""
-    assert bool(torch.isfinite(a).all()), what
-    d = (a - b).abs()
-    assert float(d.max()) <= 2.0 ** -6 * float(b.abs().max()), (what, float(d.max()), int((d > 0).sum()))
+        close_downstream_of_gn(what + ': cls', cls, ecls)
+        close_downstream_of_gn(what + ': reg', reg, ereg)
 
 
 CASES = [('WIDERFACE_S', None, 'bf16'), ('WIDERFACE_S', True, 'bf16'), ('WIDERFACE_L', None, 'bf16'), ('TT100K_L', None, 'bf16'),
@@ -142,7 +110,7 @@ def test_capacity_plan_matches_exact_plans_tensor_by_tensor(name, fuse_stem, act
     exact = _Exact(model, stem4, act_dtype)
     has_gn = any(op['kind'] == nat.OP_GN_APPLY or (op['kind'] == nat.OP_HEAD_FINAL and op.get('gn_groups')) for op in plan._ops)
     assert has_gn == (name != 'TL_L')
-    tainted = _downstream_of_gn(plan)
+    tainted = downstream_of_gn(plan)
     frames = {s: _frames(s[0], s[1], seed=11 + i) for i, s in enumerate(SIZES)}
     graphs = 0
     for fmt in (nat.INPUT_U8_NHWC, nat.INPUT_F32_NCHW):
@@ -154,7 +122,7 @@ def test_capacity_plan_matches_exact_plans_tensor_by_tensor(name, fuse_stem, act
                     held.copy_(x)
                     x = held
                 else:
-                    _poison(plan)
+                    poison(plan)
                 with torch.no_grad():
                     cls, reg = plan.forward(x, use_graph=use_graph)
                 torch.cuda.synchronize()
@@ -218,27 +186,13 @@ def test_get_results_of_mixed_sizes_match_per_size_post_plans():
     assert len(model._plans) == 1
 
 
-def _untouched(plan, call):
-    """call() must raise before anything reaches the device: the workspace, the outputs and the staging keep their bytes."""
-    plan.staging(nat.INPUT_U8_NHWC)
-    _poison(plan)
-    torch.cuda.synchronize()
-    with pytest.raises((ValueError, nat.LfdError)) as e:
-        call()
-    torch.cuda.synchronize()
-    assert bool((plan.workspace == 0xff).all()) and bool((plan._stage == 0xff).all())
-    for c, r in plan._outputs:
-        assert bool((c.view(torch.uint8) == 0xff).all()) and bool((r.view(torch.uint8) == 0xff).all())
-    return str(e.value)
-
-
 def test_errors_launch_nothing():
     model, _ = synth_model('TEST_FAST')
     model.cuda()
     plan = InferencePlan(model, N, 96, 160, torch.device('cuda'))
     for shape in [(N, 97, 160, 3), (N, 96, 161, 3), (N + 1, 64, 64, 3), (N - 1, 96, 160, 3)]:
         x = torch.zeros(shape, dtype=torch.uint8, device='cuda')
-        msg = _untouched(plan, lambda: plan.forward(x))
+        msg = untouched(plan, lambda: plan.forward(x))
         assert 'capacity' in msg
     # the C entry point checks the frame and the table itself
     lib, stage = nat.lib(), plan.staging(nat.INPUT_U8_NHWC)
@@ -248,17 +202,17 @@ def test_errors_launch_nothing():
         with torch.cuda.device(plan.device):
             nat.check(lib.lfd_plan_forward_extent(plan.handle, nat.ptr(stage), nat.INPUT_U8_NHWC, h, w, t, nat.ptr(plan.workspace),
                                                   nat.ptr(plan.cls_out), nat.ptr(plan.reg_out), 1, nat.stream_ptr()))
-    assert 'capacity' in _untouched(plan, lambda: raw(97, 160, table))
-    assert 'capacity' in _untouched(plan, lambda: raw(64, 161, table))
-    assert 'frame' in _untouched(plan, lambda: raw(64, 96, table))          # a table of another frame
+    assert 'capacity' in untouched(plan, lambda: raw(97, 160, table))
+    assert 'capacity' in untouched(plan, lambda: raw(64, 161, table))
+    assert 'frame' in untouched(plan, lambda: raw(64, 96, table))          # a table of another frame
     bad = (nat.Extent * len(table))()
     C_ = __import__('ctypes')
     C_.memmove(bad, table, C_.sizeof(table))
     bad[3].Ho = 10 ** 4
-    assert 'outside' in _untouched(plan, lambda: raw(64, 100, bad))
+    assert 'outside' in untouched(plan, lambda: raw(64, 100, bad))
     simt = InferencePlan(model, N, 96, 160, torch.device('cuda'), conv_impl=nat.CONV_SIMT)
     x = torch.zeros((N, 64, 100, 3), dtype=torch.uint8, device='cuda')
-    assert 'SIMT' in _untouched(simt, lambda: simt.forward(x))
+    assert 'SIMT' in untouched(simt, lambda: simt.forward(x))
     with torch.cuda.device(simt.device):
         rc = lib.lfd_plan_forward_extent(simt.handle, nat.ptr(simt.staging(nat.INPUT_U8_NHWC)), nat.INPUT_U8_NHWC, 64, 100,
                                          simt._extent(64, 100)[0], nat.ptr(simt.workspace), nat.ptr(simt.cls_out), nat.ptr(simt.reg_out),

@@ -5,8 +5,8 @@ CPU gradients of the same 16-bit operands."""
 import pytest
 import torch
 
-from gpu_ops import assert_faithful, conv_out, ref_conv64
-from gpu_train_ops import Workspace, bf16r, desc_table, make_top, run_top
+from gpu_ops import assert_faithful, bf16r, conv_out, ref_conv64
+from gpu_train_ops import Workspace, desc_table, make_top, run_top
 from lfd import _native as nat
 
 DEV = 'cuda'

@@ -9,7 +9,7 @@ import pytest
 import torch
 
 from gray_models import gray_pair
-from helpers import synth_model
+from helpers import ListDataset, synth_model
 from lfd import _native as nat
 from lfd.data_pipeline import sampler as S
 from lfd.data_pipeline import simple_normalize_pipeline
@@ -31,24 +31,10 @@ def test_output_mode_constants_match_the_header():
         assert getattr(nat, 'INPUT_OUT_' + name) == v, name
 
 
-class ListDataset(object):
-    def __init__(self, n=6):
-        rng = np.random.default_rng(0)
-        self.samples = {i: {'image': rng.integers(0, 256, (60, 70, 3), dtype=np.uint8), 'bboxes': [[5, 6, 20, 22]], 'bbox_labels': [0],
-                            'image_id': i} for i in range(n)}
-
-    def __len__(self):
-        return len(self.samples)
-
-    def __getitem__(self, i):
-        return self.samples[i]
-
-    def get_indexes(self):
-        return list(self.samples.keys())
-
-
 def _loader(pipeline=simple_widerface_train_pipeline, region=None, **kw):
-    ds = ListDataset()
+    rng = np.random.default_rng(0)
+    ds = ListDataset([{'image': rng.integers(0, 256, (60, 70, 3), dtype=np.uint8), 'bboxes': [[5, 6, 20, 22]], 'bbox_labels': [0], 'image_id': i}
+                      for i in range(6)])
     return DataLoader(ds, S.RandomDatasetSampler(ds, batch_size=3), region or S.RandomBBoxCropRegionSampler(crop_size=32), pipeline, **kw)
 
 

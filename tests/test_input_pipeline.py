@@ -13,6 +13,7 @@ import torch
 
 import input_oracle as O
 from gen_golden_input import digest, synthetic_samples
+from helpers import ListDataset
 from lfd.data_pipeline import Dataset, Sample, simple_normalize_pipeline
 from lfd.data_pipeline import sampler as S
 from lfd.data_pipeline.augmentation import Compose, HorizontalFlip, bbox_param, pipeline_device_spec, simple_normalize, simple_widerface_train_pipeline
@@ -28,20 +29,6 @@ SAMPLES = synthetic_samples()     # the goldens keep digests of the images, not 
 def test_regenerated_samples_are_the_golden_ones():
     assert [digest(s['image']) for s in SAMPLES] == GOLDEN['source_digests']
     assert [{k: v for k, v in s.items() if k != 'image'} for s in SAMPLES] == GOLDEN['samples']
-
-
-class ListDataset(object):
-    def __init__(self, samples):
-        self.samples = dict(enumerate(samples))
-
-    def __len__(self):
-        return len(self.samples)
-
-    def __getitem__(self, i):
-        return self.samples[i]
-
-    def get_indexes(self):
-        return list(self.samples.keys())
 
 
 @pytest.mark.parametrize('k', range(len(GOLDEN['region'])))

@@ -8,7 +8,8 @@ import pytest
 import torch
 
 import tl_s
-from helpers import synth_model
+from gpu_ops import make_op
+from helpers import finetune_model, synth_model
 from lfd import _native as nat
 from lfd._engine import InferencePlan
 from lfd.data_pipeline.augmentation import (BGR2RGB, Compose, HorizontalFlip, InputTransform, Normalize, bbox_param,
@@ -83,13 +84,8 @@ def test_structs_have_the_library_sizes_and_the_new_fields():
 
 
 def _stem_op(transform=None, **over):
-    o = nat.Op()
-    o.kind, o.dtype = nat.OP_STEM0, nat.DTYPE_BF16
-    o.N, o.H, o.W, o.Cin, o.Ho, o.Wo, o.Cout = 1, 32, 32, 3, 16, 16, 64
-    o.ksize, o.stride, o.relu = 3, 2, 1
-    o.in_off, o.out_off, o.res_off, o.stats_off, o.ds_out_off = -1, 4096, -1, -1, -1
-    o.weight = 256
-    nat.set_input_transform(o, transform)
+    o = make_op(nat.OP_STEM0, transform=transform, N=1, H=32, W=32, Cin=3, Ho=16, Wo=16, Cout=64, ksize=3, stride=2, relu=1, out_off=4096,
+                weight=256)
     for k, v in over.items():
         if isinstance(v, tuple):
             getattr(o, k)[:] = v
@@ -194,8 +190,7 @@ def test_training_plan_and_frozen_prefix_carry_the_transform():
                 assert fields(o) == (0, (0.0,) * 3, (0.0,) * 3)
     assert seen == [nat.TOP_STEM0, nat.TOP_WGRAD_STEM]
     # fine-tuning: the frozen prefix's stem is an inference op inside the training plan
-    from test_finetune_plan import finetune_model
-    frozen = finetune_model('WIDERFACE_L', 1)
+    frozen = finetune_model('WIDERFACE_L', 1, -1.0)
     frozen.set_input_transform(tl_val_pipeline)
     plan = TrainPlan(frozen, 2, 128, 160, 'cpu', create_native=False)
     assert plan._prefix is not None
