@@ -15,7 +15,7 @@ import functools
 
 import torch
 
-from gpu_ops import DTYPES, conv_out, ref_conv64, stem_input
+from gpu_ops import DTYPES, conv_out, ref_conv64, stem_operand
 from helpers import bits  # noqa: F401  (X.bits of test_gpu_extent_configs.py)
 from lfd import _native as nat
 from lfd._engine import fold_scale, pack_conv_weight, pack_stem_weight
@@ -349,21 +349,6 @@ def transform_of(name):
     from lfd.data_pipeline.augmentation import input_transform_of, typical_coco_val_pipeline
     from test_input_transform_host import tl_val_pipeline
     return input_transform_of({'rgb-standard': tl_val_pipeline, 'caffe': typical_coco_val_pipeline}[name])
-
-
-def stem_operand(img, fmt, xf, dtype):
-    """The 16-bit stem operand [N, h, w, 3] a loader builds from the frame: img = float32 [N, 3, h, w] ('f32'), uint8 BGR [N, h, w, 3]
-    ('u8') or NV12 [N, 3h/2, w] ('nv12', converted by the cv2 oracle first).  A transform subtracts its fp32 mean and multiplies by its
-    fp32 scale, per network channel, after the optional BGR -> RGB."""
-    if fmt == 'nv12':
-        img, fmt = torch.from_numpy(nv12_oracle(img.numpy())), 'u8'
-    if fmt == 'f32' or xf is None:
-        return stem_input(img, fmt, dtype)
-    b = img.float()
-    if xf.swap_rb:
-        b = b.flip(-1)
-    mean, scale = torch.tensor(list(xf.mean), dtype=torch.float32), torch.tensor(list(xf.scale), dtype=torch.float32)
-    return DTYPES[dtype][1]((b - mean) * scale)
 
 
 class _ImageSpec(object):

@@ -237,6 +237,25 @@ def stem_input(img, fmt, dtype='bf16'):
     return rnd(img.float().permute(0, 2, 3, 1))
 
 
+def stem_operand(img, fmt, xf, dtype):
+    """The 16-bit stem operand [N, h, w, C] a loader builds from the frame: img = float32 [N, C, h, w] ('f32'), uint8 BGR [N, h, w, 3] or
+    gray [N, h, w] / [N, h, w, 1] ('u8'), or BGR NV12 [N, 3h/2, w] ('nv12', converted by the cv2 oracle first), on img's device.  A transform subtracts its fp32 mean and multiplies by its fp32 scale, per network channel, after the
+    optional BGR -> RGB."""
+    if fmt == 'nv12':
+        from nv12_oracle import nv12_oracle
+        img, fmt = torch.from_numpy(nv12_oracle(img.cpu().numpy())).to(img.device), 'u8'
+    if fmt == 'u8' and (img.dim() == 3 or img.shape[-1] == 1):
+        img = img.reshape(img.shape[:3] + (1,))                  # gray
+    if fmt == 'f32' or xf is None:
+        return stem_input(img, fmt, dtype)
+    b = img.float()
+    if xf.swap_rb:
+        b = b.flip(-1)
+    c = b.shape[-1]
+    mean, scale = (torch.tensor(list(v)[:c], dtype=torch.float32, device=b.device) for v in (xf.mean, xf.scale))
+    return DTYPES[dtype][1]((b - mean) * scale)
+
+
 def ref_conv64(x_nhwc, weight, scale, shift, stride, relu, res=None, dtype='bf16', device='cpu'):
     """float64 evaluation of the fused layer on exactly the operands the kernel sees: round16(weight * scale), round16(shift),
     the 16-bit input and residual, on `device` (the CPU, or the GPU for whole-network sizes).  -> (y [N,Ho,Wo,Cout] float64, not
@@ -296,7 +315,7 @@ def assert_tail_close(out, ref, dtype='bf16', what=''):
 
 def assert_gn_stats(stats, out, groups, what=''):
     """Fused GroupNorm statistics against float64 sums of the stored tensor: the kernel adds fp32 partial sums of at most a few
-    dozen values before its fp64 atomics, so 1e-5 of the sum of |terms| bounds the difference."""
+    dozen values before its fp64 atomics, so 1e-5 of the sum of |terms| bounds the difference.  -> max err / tol."""
     N, C = out.shape[0], out.shape[-1]
     o = out.cpu().double().reshape(N, -1, groups, C // groups)
     s1, s2 = o.sum(dim=(1, 3)), (o * o).sum(dim=(1, 3))
@@ -304,6 +323,7 @@ def assert_gn_stats(stats, out, groups, what=''):
     st = stats.cpu()
     assert bool(((st[..., 0] - s1).abs() <= 1e-5 * a1 + 1e-30).all()), '%s: sum off by %g' % (what, float((st[..., 0] - s1).abs().max()))
     assert bool(((st[..., 1] - s2).abs() <= 1e-5 * s2 + 1e-30).all()), '%s: sum of squares off by %g' % (what, float((st[..., 1] - s2).abs().max()))
+    return max(float(((st[..., 0] - s1).abs() / (1e-5 * a1 + 1e-30)).max()), float(((st[..., 1] - s2).abs() / (1e-5 * s2 + 1e-30)).max()))
 
 
 # ------------------------------------------------------------------------------------------------ op-level conv and stem cases

@@ -9,7 +9,7 @@ import lfd._native as nat
 from helpers import finetune_model, synth_model
 from lfd._engine import InferencePlan
 from lfd._train import TrainPlan, flat_parameters
-from plan_order import check_every_conflict_ordered
+from plan_order import check_training_ops
 
 CPU = torch.device('cpu')
 CASES = [(cfg, k) for cfg in ('WIDERFACE_L', 'WIDERFACE_S', 'TT100K_L', 'TL_L') for k in (1, 2, 'all')]
@@ -71,9 +71,9 @@ def _check_plan(plan, model, frozen_ids):
     for op in plan.bwd_ops:
         for v in op.get('ptr', {}).values():
             assert not (isinstance(v, tuple) and v[0] == 'grad' and id(v[1]) in frozen_ids)
-    # no backward op on a frozen-prefix layer, and the plan still orders every cross-branch conflict
-    assert check_every_conflict_ordered(plan.fwd_ops, 'fwd') >= 0
-    assert check_every_conflict_ordered(plan.bwd_ops, 'bwd') >= 0
+    # no backward op on a frozen-prefix layer, and the plan still orders every overlap, the recycled prefix scratch included
+    assert check_training_ops(plan, plan.fwd_ops, 'fwd') >= 0
+    assert check_training_ops(plan, plan.bwd_ops, 'bwd') >= 0
 
 
 def _final_convs(model):

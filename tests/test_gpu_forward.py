@@ -13,9 +13,9 @@ from oracle import lfd_oracle as orc
 pytestmark = pytest.mark.gpu
 FWD = ['WIDERFACE_XS', 'WIDERFACE_S', 'WIDERFACE_L', 'TT100K_L', 'TL_L', 'TEST_FAST', 'TEST_FASTEST']
 # Parity protocol (DESIGN.md "Parity"):
-#  Gate A/B  every fused layer, fed the tensors the CUDA path actually produced upstream ("teacher forced"), equals the
-#            fp32 CPU evaluation of that layer on the same bf16 operands to <= 1 bf16 ulp; the fp32 head outputs to 1e-4.
-#            This is the 1e-3 bar of BASELINE.json applied where it is attainable: per layer.
+#  Gate A/B  every op of the plan, fed the tensors the CUDA path actually produced upstream on the plan's own reused workspace,
+#            against float64 on the same 16-bit operands, per element (test_gpu_inference_per_op.py).  This is the 1e-3 bar of
+#            BASELINE.json applied where it is attainable: per op.
 #  Gate C    end to end, two bf16 pipelines that differ only in fp32 summation order (tensor core vs CPU) decorrelate
 #            to bf16-ulp level after a few layers (a 1-ulp flip is 4e-3; flips compound), exactly like the reference's own
 #            model.bfloat16() vs fp32 (SURVEY 7: 1.1e-2 .. 2.3e-2).  The drift is bounded here, not hidden.
@@ -198,80 +198,6 @@ def test_predict_for_single_image_runs_end_to_end():
     model.act_dtype = 'bf16'
     rows3 = model.predict_for_single_image(img, None, classification_threshold=0.2, nms_threshold=0.4)
     assert abs(len(rows3) - len(rows)) <= max(2, len(rows) // 50)
-
-
-@pytest.mark.parametrize('name', FWD)
-def test_every_layer_within_one_bf16_ulp_teacher_forced_without_reuse(name):
-    """Gate A/B: each fused layer of the real network, evaluated in fp32 on the CPU from the inputs the CUDA path itself
-    produced, matches the stored CUDA output to 1 bf16 ulp (final fp32 cls / reg: 2e-4 rms, 2e-3 max relative)."""
-    import torch.nn.functional as F
-    from gpu_ops import ref_conv, assert_bf16_close, bf16r
-    from lfd._engine import InferencePlan
-    g = load_golden('forward_%s.pt' % name)
-    model, sd = synth_model(name, cls_bias=g['cls_bias'], seed=g['seed'])
-    model.cuda()
-    x = synth.synth_input(g['N'], g['H'], g['W'])
-    # the plan model(x) builds, with reuse=False: every intermediate stays alive for inspection
-    plan = InferencePlan(model, g['N'], g['H'], g['W'], torch.device('cuda'), model.conv_impl, act_dtype=model.act_dtype,
-                         input_transform=model.input_transform, reuse=False)
-    cls, reg = (t.cpu() for t in plan.forward(x.cuda(), use_graph=False))
-    checked = 0
-    for op in plan._ops:
-        kind = op['kind']
-        if kind in (nat.OP_STEM0, nat.OP_CONV):
-            conv, norm = op['modules']
-            scale, shift = InferencePlan._fold(conv, norm)
-            src = bf16r(x).permute(0, 2, 3, 1) if kind == nat.OP_STEM0 else plan.tensor(op['inp'])
-            res = plan.tensor(op['res']) if op.get('res') is not None else None
-            if not op.get('tail_cout'):
-                ref = ref_conv(src, conv.weight.detach().cpu(), scale, shift, op['stride'], bool(op['relu']), res=res)
-                assert_bf16_close(plan.tensor(op['out']), ref, 'conv %s' % op['out'])
-                if op.get('ds_cout'):     # fused 1x1/s2 shortcut conv: second output of the same launch
-                    sconv, snorm = op['ds_modules']
-                    sscale, sshift = InferencePlan._fold(sconv, snorm)
-                    ref2 = ref_conv(src, sconv.weight.detach().cpu(), sscale, sshift, 2, False)
-                    assert_bf16_close(plan.tensor(op['out2']), ref2, 'fused shortcut %s' % op['out2'])
-            else:   # conv + fused 1x1 tail: the intermediate (bf16) only exists inside the kernel
-                conv2, norm2 = op['tail_modules']
-                scale2, shift2 = InferencePlan._fold(conv2, norm2)
-                mid = bf16r(ref_conv(src, conv.weight.detach().cpu(), scale, shift, op['stride'], bool(op['relu'])))
-                ref = ref_conv(mid, conv2.weight.detach().cpu(), scale2, shift2, 1, bool(op['tail_relu']), res=res)
-                got = plan.tensor(op['out']).float().cpu()
-                tol = ref.abs() * 2.0 ** -7 + 2e-3 * float(ref.abs().max())   # 1-ulp flips of the in-kernel intermediate
-                assert bool(((got - ref).abs() <= tol).all()), ('fused tail', op['out'], float((got - ref).abs().max()))
-                assert rel_err(got, ref)[1] < 3e-3
-        elif kind in (nat.OP_GN_APPLY, nat.OP_HEAD_FINAL):
-            tnorm = op['modules'][0]
-            raw = plan.tensor(op['inp']).float().cpu()                      # [N,H,W,C] stored conv output
-            n, h, w, c = raw.shape
-            if tnorm is None:            # head without norm layers: the stored tensor is already conv + bias + ReLU
-                y = raw
-            else:
-                grp = raw.reshape(n, h * w, tnorm.num_groups, c // tnorm.num_groups).double()
-                mean = grp.mean(dim=(1, 3))
-                var = grp.var(dim=(1, 3), unbiased=False)
-                rstd = (1.0 / torch.sqrt(var + tnorm.eps)).float()
-                y = (raw.reshape(n, h * w, tnorm.num_groups, -1) - mean.float()[:, None, :, None]) * rstd[:, None, :, None]
-                y = y.reshape(n, h, w, c) * tnorm.weight.detach().cpu().float() + tnorm.bias.detach().cpu().float()
-                y = F.relu(y)
-            if kind == nat.OP_GN_APPLY:
-                assert_bf16_close(plan.tensor(op['out']), y, 'gn_apply %s' % op['out'])
-            else:
-                a = bf16r(y).reshape(n, h * w, c)
-                convs, scales = op['modules'][1], op['modules'][2]
-                outs = []
-                for fc, sc in zip(convs, scales):
-                    wt = bf16r(fc.weight.detach().cpu().reshape(fc.out_channels, -1))
-                    outs.append((a @ wt.t() + fc.bias.detach().cpu().float()) * sc)
-                o = torch.cat(outs, dim=-1)
-                p0, p1 = op['point_off'], op['point_off'] + h * w
-                got = torch.cat(([cls[:, p0:p1]] if op['n_cls'] else []) + ([reg[:, p0:p1]] if op['n_reg'] else []), dim=-1)
-                # the 128 normalised inputs are re-rounded to bf16 (Rg): fp32 round-off next to a rounding boundary flips
-                # single inputs by one bf16 ulp, which shows up as a few 1e-4 on isolated outputs
-                e = rel_err(got, o)
-                assert e[0] < 2e-3 and e[1] < 2e-4, ('head_final', op['inp'], e)
-        checked += 1
-    assert checked == len(plan._ops)
 
 
 def test_streaming_detector_matches_synchronous_path():

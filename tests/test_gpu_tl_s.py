@@ -249,67 +249,6 @@ def test_tl_s_training_is_not_implemented():
         TrainPlan(model, 2, 256, 320, torch.device('cuda', 0))
 
 
-@pytest.mark.parametrize('impl', [nat.CONV_UMMA, nat.CONV_SIMT], ids=['umma', 'simt'])
-def test_tl_s_every_layer_within_one_bf16_ulp_teacher_forced_without_reuse(impl):
-    """Gate A/B of test_gpu_forward.py for TL_S: each fused layer of the real network (the 3 -> 48 stem with its fused 48 tail, the
-    stage-0 3x3/s2 conv with its fused 48 shortcut, the 48-channel blocks, the neck conv from 48 channels, ...), evaluated in fp32 on
-    the CPU from the inputs the CUDA path itself produced, matches the stored CUDA output to 1 bf16 ulp; the head outputs to 2e-4 rms."""
-    from gpu_ops import ref_conv, assert_bf16_close, bf16r
-    from lfd._engine import InferencePlan
-    g, model, sd = _model('bf16', impl)
-    x = synth.synth_input(g['N'], g['H'], g['W'])
-    # the plan model(x) builds, with reuse=False: every intermediate stays alive for inspection
-    plan = InferencePlan(model, g['N'], g['H'], g['W'], torch.device('cuda'), model.conv_impl, act_dtype=model.act_dtype,
-                         input_transform=model.input_transform, reuse=False)
-    cls, reg = (t.cpu() for t in plan.forward(x.cuda(), use_graph=False))
-    seen = set()
-    for op in plan._ops:
-        kind = op['kind']
-        if kind in (nat.OP_STEM0, nat.OP_CONV):
-            conv, norm = op['modules']
-            scale, shift = InferencePlan._fold(conv, norm)
-            src = bf16r(x).permute(0, 2, 3, 1) if kind == nat.OP_STEM0 else plan.tensor(op['inp'])
-            res = plan.tensor(op['res']) if op.get('res') is not None else None
-            seen.add((kind, op['Cin'], op['Cout'], op['ksize'], op['stride'], op.get('tail_cout', 0), op.get('ds_cout', 0)))
-            if not op.get('tail_cout'):
-                ref = ref_conv(src, conv.weight.detach().cpu(), scale, shift, op['stride'], bool(op['relu']), res=res)
-                assert_bf16_close(plan.tensor(op['out']), ref, 'conv %s' % op['out'])
-                if op.get('ds_cout'):
-                    sconv, snorm = op['ds_modules']
-                    sscale, sshift = InferencePlan._fold(sconv, snorm)
-                    ref2 = ref_conv(src, sconv.weight.detach().cpu(), sscale, sshift, 2, False)
-                    assert_bf16_close(plan.tensor(op['out2']), ref2, 'fused shortcut %s' % op['out2'])
-            else:
-                conv2, norm2 = op['tail_modules']
-                scale2, shift2 = InferencePlan._fold(conv2, norm2)
-                mid = bf16r(ref_conv(src, conv.weight.detach().cpu(), scale, shift, op['stride'], bool(op['relu'])))
-                ref = ref_conv(mid, conv2.weight.detach().cpu(), scale2, shift2, 1, bool(op['tail_relu']), res=res)
-                got = plan.tensor(op['out']).float().cpu()
-                tol = ref.abs() * 2.0 ** -7 + 2e-3 * float(ref.abs().max())   # 1-ulp flips of the in-kernel intermediate
-                assert bool(((got - ref).abs() <= tol).all()), ('fused tail', op['out'], float((got - ref).abs().max()))
-                assert rel_err(got, ref)[1] < 3e-3
-        else:
-            assert kind == nat.OP_HEAD_FINAL and op['modules'][0] is None      # TL heads: no norm layers
-            raw = plan.tensor(op['inp']).float().cpu()
-            n, h, w, c = raw.shape
-            a = bf16r(raw).reshape(n, h * w, c)
-            outs = []
-            for fc, sc in zip(op['modules'][1], op['modules'][2]):
-                wt = bf16r(fc.weight.detach().cpu().reshape(fc.out_channels, -1))
-                outs.append((a @ wt.t() + fc.bias.detach().cpu().float()) * sc)
-            o = torch.cat(outs, dim=-1)
-            p0, p1 = op['point_off'], op['point_off'] + h * w
-            got = torch.cat(([cls[:, p0:p1]] if op['n_cls'] else []) + ([reg[:, p0:p1]] if op['n_reg'] else []), dim=-1)
-            e = rel_err(got, o)
-            assert e[0] < 2e-3 and e[1] < 2e-4, ('head_final', op['inp'], e)
-    if impl == nat.CONV_UMMA:     # the layers the 48-wide kernel runs in this plan
-        assert (nat.OP_STEM0, 3, 48, 3, 2, 48, 0) in seen and (nat.OP_CONV, 48, 48, 3, 2, 0, 48) in seen
-        assert (nat.OP_CONV, 48, 48, 3, 1, 0, 0) in seen and (nat.OP_CONV, 48, 64, 3, 2, 0, 64) in seen
-        assert any(k[1] == 48 and k[2] == 128 and k[3] == 1 for k in seen)        # the neck conv from 48 channels
-    else:
-        assert (nat.OP_STEM0, 3, 48, 3, 2, 0, 0) in seen and (nat.OP_CONV, 48, 48, 1, 2, 0, 0) in seen
-
-
 def test_tl_s_streaming_detector_matches_synchronous_path():
     """lfd.pipeline.StreamingDetector (batches in flight on copy / forward / post-process streams) returns, batch by batch, exactly what
     the synchronous forward + detect returns for TL_S, as test_gpu_forward.py checks for WIDERFACE_XS."""

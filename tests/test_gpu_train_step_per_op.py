@@ -28,10 +28,10 @@ import synth
 from gpu_train_ops import gn_bwd_blocks, grid_sms, head_bwd_grid, reduce_blocks
 from helpers import synth_model
 from lfd import _native as nat
-from gpu_ops import assert_tail_close, ref_conv64, stem_input, ulp16
-from lfd._engine import InferencePlan, pack_stem_weight
-from train_op_ref import (U, bn_apply_ref, bn_bwd_ref, bn_running_ref, bn_stats_ref, check_amb, check_faithful, check_within, conv_pack_ref,
-                          gn_bwd_ref, head_activation, head_backward_ref, head_forward_ref)
+from gpu_ops import ref_conv64, stem_operand, ulp16
+from lfd._engine import pack_stem_weight
+from train_op_ref import (U, bf, bn_apply_ref, bn_bwd_ref, bn_running_ref, bn_stats_ref, check_amb, check_conv_op, check_faithful, check_within, conv_pack_ref,
+                          gn_bwd_ref, head_activation, head_backward_ref, head_forward_ref, layer_relu)
 
 DEV = 'cuda'
 WGRAD_K = 1e-5 / U          # the wgrad config test's bound 1e-5 * S: a tile lost or counted twice moves an element by about S / tiles
@@ -42,10 +42,6 @@ KIND_NAMES = {v: k[4:] for k, v in vars(nat).items() if k.startswith('TOP_') and
 WORST = {}          # largest err / tol per (kind, output) over the replays of a session
 
 
-def _bf(t):
-    return t.to(torch.bfloat16).double()
-
-
 def _conv64(x, w, shift, stride, relu=False, res=None):
     """gpu_ops.ref_conv64 on the GPU for a conv whose 16-bit weights w are given as they are (no BatchNorm fold); shift None: none."""
     cout = w.shape[0]
@@ -53,17 +49,9 @@ def _conv64(x, w, shift, stride, relu=False, res=None):
     return ref_conv64(x, w.float().cpu(), torch.ones(cout), sh, stride, relu, res=res, device=DEV)
 
 
-def _folded64(x, mods, relu, res=None, stride=None):
-    """gpu_ops.ref_conv64 on the GPU of a conv + BatchNorm folded as the inference plan folds it (InferencePlan._fold, fold_scale): the
-    same host code that stages the frozen prefix, so this checks the kernels on those operands, not the folding itself."""
-    conv, norm = mods
-    scale, shift = InferencePlan._fold(conv, norm)
-    return ref_conv64(x, conv.weight, scale, shift, conv.stride[0] if stride is None else stride, relu, res=res, device=DEV)
-
-
 def _image(x):
     """The stem's 16-bit operand (rounding point R0), on the GPU."""
-    return stem_input(x, 'u8' if x.dtype == torch.uint8 else 'f32').to(torch.bfloat16)
+    return stem_operand(x, 'u8' if x.dtype == torch.uint8 else 'f32', None, 'bf16')
 
 
 class Replay(object):
@@ -74,6 +62,7 @@ class Replay(object):
         n = x.shape[0]
         h, w = (x.shape[1], x.shape[2]) if x.dtype == torch.uint8 else (x.shape[2], x.shape[3])
         self.bn = [m for m in model.modules() if isinstance(m, nn.BatchNorm2d)]
+        self.relu = layer_relu(model)          # the frozen prefix's ReLUs, from the layer records
         self.bn0 = [(m.running_mean.clone(), m.running_var.clone()) for m in self.bn]
         out = model(x)
         model.get_loss(out, ann)['loss'].backward()
@@ -309,7 +298,7 @@ class Replay(object):
         z = self.name_at(t.off[1])
         self.nan_fill(z)
         self.run(t)
-        ref, S, K = _conv64(_image(self.x), _bf(conv.weight.detach()), None, 2)
+        ref, S, K = _conv64(_image(self.x), bf(conv.weight.detach()), None, 2)
         self.note(t.kind, 'z', check_faithful(self.view(z), ref, S, K, self.what + ' z'))
 
     def op_conv(self, t):
@@ -326,7 +315,7 @@ class Replay(object):
             st0 = self.view(st).clone()
         self.nan_fill(z)
         self.run(t)
-        ref, S, K = _conv64(self.view(x), _bf(conv.weight.detach()), None, conv.stride[0])
+        ref, S, K = _conv64(self.view(x), bf(conv.weight.detach()), None, conv.stride[0])
         out = self.view(z)
         self.note(t.kind, 'z', check_faithful(out, ref, S, K, self.what + ' z'))
         if st is not None:       # fused GroupNorm statistics of the stored output: fp32 partials of a few dozen values, fp64 atomics
@@ -351,7 +340,7 @@ class Replay(object):
         if not acc:
             self.nan_fill(dx)
         self.run(t)
-        wt = _bf(conv.weight.detach()).permute(1, 0, 2, 3).flip(2, 3)
+        wt = bf(conv.weight.detach()).permute(1, 0, 2, 3).flip(2, 3)
         ref, S, K = _conv64(self.view(src), wt, None, 1, res=prev)
         self.note(t.kind, 'dx', check_faithful(self.view(dx), ref, S, K, self.what + ' dx'))
         self.written.add(dx)
@@ -690,22 +679,8 @@ class Replay(object):
             x = _image(self.x)
         else:
             x = tensor(op['inp'], t.off[0]).view(N, op['H'], op['W'], op['Cin'])
-        if op['kind'] == nat.OP_STEM4:      # stem0 + 1x1 tail, stem2 3x3/s2, stem3 1x1: three 16-bit intermediates inside the kernel
-            mid = _bf(_folded64(x, op['modules'], bool(op['relu']))[0])
-            mid = _bf(_folded64(mid, op['tail_modules'], bool(op['tail_relu']))[0])
-            mid = _bf(_folded64(mid, op['s2_modules'], bool(op['s2_relu']))[0])
-            ref = _folded64(mid, op['s3_modules'], bool(op['s3_relu']))[0]
-            self.note(t.kind, 'stem4 (fused-tail bound)', assert_tail_close(out, ref, what=self.what + ' stem4'))
-        elif op.get('tail_cout'):
-            mid = _bf(_folded64(x, op['modules'], bool(op['relu']))[0])
-            ref = _folded64(mid, op['tail_modules'], bool(op['tail_relu']), res=res)[0]
-            self.note(t.kind, 'fused tail (fused-tail bound)', assert_tail_close(out, ref, what=self.what + ' tail'))
-        else:
-            ref, S, K = _folded64(x, op['modules'], bool(op['relu']), res=res)
-            self.note(t.kind, 'out', check_faithful(out, ref, S, K, self.what + ' out'))
-        if out2 is not None:
-            ref, S, K = _folded64(x, op['ds_modules'], False, stride=2)
-            self.note(t.kind, 'shortcut', check_faithful(out2.view(ref.shape), ref, S, K, self.what + ' shortcut'))
+        for name, ratio in check_conv_op(op, x, out, out2, res, 'bf16', self.what, self.relu):
+            self.note(t.kind, name, ratio)
 
     # ------------------------------------------------------------------ the executor on the same step
     def executor_matches(self):

@@ -92,36 +92,13 @@ def test_planner_builds_expected_graph(name, n_conv):
     merged = name.startswith('WIDERFACE')
     assert kinds.count('head_final') == (levels if merged else 2 * levels)
     assert kinds.count('gn_apply') == (levels if merged else 2 * levels)
-    # live ranges never overlap in the workspace
+    # (the workspace placement and the ordering of every overlap: test_inference_plans_order_every_overlap)
+    # branches: the per-level neck + head chains, and the shortcut convs on branch 7 where they cannot be fused into the block's first conv
     ops = plan._ops
-    last_use = {}
-    for i, op in enumerate(ops):
-        for k in ('inp', 'res'):
-            if op.get(k) is not None:
-                last_use[op[k]] = i
-    born = {op['out']: i for i, op in enumerate(ops) if op.get('out') is not None}
-    names = list(born)
-    for a in names:
-        for b in names:
-            if a >= b:
-                continue
-            if born[a] <= last_use.get(b, born[b]) and born[b] <= last_use.get(a, born[a]):   # lifetimes intersect
-                oa, ob = plan.offsets[a], plan.offsets[b]
-                assert oa + plan._tensors[a] <= ob or ob + plan._tensors[b] <= oa, (a, b)
-    assert plan.workspace_bytes < plan.activation_bytes + plan.stats_bytes + 65536
-    # branches (per-level neck + head chains) run concurrently with the backbone: their buffers must be disjoint from
-    # every other branch's, and a tap read across branches is never recycled
-    # (shortcut convs are fused into the block's first 3x3/s2 conv; where they cannot be, they run on branch 7)
     fused_sc = [o for o in ops if o.get('ds_cout')]
     branches = sorted(set(plan.tensor_branch.values()))
     assert branches == list(range(len(plan.level_sizes) + 1)) + ([] if fused_sc else [7])
     assert all(o['ksize'] == 3 and o['stride'] == 2 and o.get('out2') in plan.offsets for o in fused_sc)
-    for a in names:
-        for b in names:
-            if a < b and (plan.tensor_branch[a] != plan.tensor_branch[b] or a in plan.shared_tensors or b in plan.shared_tensors):
-                oa, ob = plan.offsets[a], plan.offsets[b]
-                if plan.tensor_branch[a] != plan.tensor_branch[b] or born[b] >= born[a] and a in plan.shared_tensors or born[a] >= born[b] and b in plan.shared_tensors:
-                    assert oa + plan._tensors[a] <= ob or ob + plan._tensors[b] <= oa, (a, b)
     # shared = the level taps + per stage the block input read by the shortcut branch and the shortcut's output
     n_short = len([o for o in ops if o['branch'] == 7])
     assert n_short > 0 or fused_sc
@@ -188,16 +165,17 @@ def test_build_guard_rejects_large_stack_frames():
 def test_training_plan_level_chains_order_every_conflict(name):
     """The training planner puts every level's neck + head chain on its own branch (side stream) and derives the wait masks from the
     read / write / accumulate role of each operand.  Replay the fork / wait protocol of lfd_train_plan_run with vector clocks and check
-    that every pair of ops that conflict on a workspace tensor (write vs anything, accumulate vs read) is ordered."""
+    that every pair of ops that conflict on workspace bytes (write vs anything, accumulate vs read) is ordered, and that no read bytes are
+    overwritten before their reader (plan_order.py)."""
     from lfd._train import TrainPlan
-    from plan_order import check_every_conflict_ordered
+    from plan_order import check_training_ops
     model, _ = synth_model(name)
     model.train()
     plan = TrainPlan(model, 2, 128, 160, torch.device('cpu'), create_native=False)
     for which, ops in (('fwd', plan.fwd_ops), ('bwd', plan.bwd_ops)):
         branches = sorted({op.get('branch', 0) for op in ops})
         assert branches[0] == 0 and len(branches) == 1 + len(plan.level_sizes) and branches[-1] < nat.MAX_BRANCHES
-        n_pairs = check_every_conflict_ordered(ops, (name, which))
+        n_pairs = check_training_ops(plan, ops, (name, which))
         if which == 'bwd':
             assert n_pairs >= len(plan.level_sizes)                  # at least the taps' gradients: level chain writes, backbone accumulates
     # the backward starts every level chain before the backbone
@@ -280,3 +258,37 @@ def test_tune_branch_bounds_descent(monkeypatch):
     clock[0] = 0.0
     caps, log = eng.tune_branch_bounds(work, measure, (64, 32), 2.5)       # trials start at t = 1 and 2 only
     assert caps == {1: 0, 2: 64, 3: 0} and [l for l, _ in log] == ['all SMs', 'branch 2 <= 64 CTAs', 'branch 2 <= 32 CTAs']
+
+
+def _inference_plans():
+    """Every config, TL_S and the gray TL_S, at a small, an odd and the 8 x 720 x 1280 shape (WIDERFACE_S there plans a STEM4 op), with the
+    fused stem forced on and off and on the SIMT cross-check (its shortcut convs run on branch 7)."""
+    import tl_s
+    from gray_models import gray_pair
+    from oracle import lfd_oracle as orc
+    models = [(name, synth_model(name)[0]) for name in sorted(orc.CONFIGS)] + [('TL_S', tl_s.synth_model()[0]), ('gray TL_S', gray_pair('TL_S')[0])]
+    for name, model in models:
+        # (below the STEM4 gate fuse_stem=False plans what the default plans; at 8 x 720 x 1280 the default fuses a 'faster' stem)
+        for shape, variants in (((2, 184, 248), (dict(), dict(fuse_stem=True))), ((2, 186, 250), (dict(), dict(fuse_stem=True), dict(conv_impl=nat.CONV_SIMT))),
+                                ((8, 720, 1280), (dict(), dict(fuse_stem=False)))):
+            for kw in variants:
+                yield '%s %s %s' % (name, shape, kw), model, InferencePlan(model, *shape, torch.device('cpu'), create_native=False, **kw)
+
+
+def test_inference_plans_order_every_overlap():
+    """plan_order.check_inference_plan on every plan of _inference_plans: the workspace bytes of every op record inside the workspace and
+    aligned, every cross-branch overlap ordered by the executor's fork / wait rules, no bytes overwritten between their producer and a
+    reader, disjoint GroupNorm statistics slots read from their producer, and the head's point ranges as level_geometry lays them out."""
+    from plan_order import check_inference_plan
+    seen_stem4 = False
+    for what, model, plan in _inference_plans():
+        n_pairs = check_inference_plan(plan, model, what)
+        if len({o.branch for o in plan._op_array}) > 1:
+            assert n_pairs > 0, what
+        print('%-60s %3d ordered cross-branch overlapping pairs' % (what, n_pairs))
+        seen_stem4 |= plan._op_array[0].kind == nat.OP_STEM4
+        if what.startswith('WIDERFACE_S (2, 184, 248) {}'):
+            caps = {b: 16 for b in range(1, len(plan.level_sizes) + 1)}
+            plan._set_side_ctas(caps)
+            assert check_inference_plan(plan, model, what + ' side CTAs') == n_pairs
+    assert seen_stem4

@@ -17,7 +17,7 @@ from fractions import Fraction
 
 import torch
 
-from gpu_ops import ulp16
+from gpu_ops import DTYPES, ref_conv64, ulp16
 
 U = 2.0 ** -24          # one fp32 rounding
 
@@ -325,3 +325,116 @@ def conv_pack_ref(w, cc, dgrad):
     wf = w.reshape(-1)
     v = wf[(kch * Cin + n) * kk + (kk - 1 - tap)] if dgrad else wf[(n * Cin + kch) * kk + tap]
     return v.to(torch.bfloat16)
+
+
+# ------------------------------------------------------------------------------------------------ inference ops (LFD_TOP_INFER, lfd_op)
+def bf(t, dtype='bf16'):
+    """t rounded to the 16-bit type, as float64."""
+    return t.to(DTYPES[dtype][0]).double()
+
+
+def folded64(x, mods, relu, res=None, stride=None, dtype='bf16', device='cuda'):
+    """gpu_ops.ref_conv64 of a conv + BatchNorm folded as the inference plan folds it (InferencePlan._fold, fold_scale): the same host code
+    that stages the plans, so this checks the kernels on those operands, not the folding itself."""
+    from lfd._engine import InferencePlan
+    conv, norm = mods
+    scale, shift = InferencePlan._fold(conv, norm)
+    return ref_conv64(x, conv.weight, scale, shift, conv.stride[0] if stride is None else stride, relu, res=res, dtype=dtype, device=device)
+
+
+def layer_relu(model):
+    """id(conv) -> whether a ReLU follows the conv, from the model's layer records: the stem's (conv, norm, relu) triples; every conv of a
+    residual block (the last one after the residual add); not the 1x1/s2 shortcut; every neck conv; a head tower conv without norm layers,
+    not one followed by a GroupNorm (its ReLU comes after the normalisation)."""
+    bb, neck, head = model._backbone, model._neck, model._head
+    relu = {id(c): bool(r) for c, _, r in bb.stem_layers()}
+    for stage in bb.stages():
+        for block in stage:
+            relu.update((id(c), True) for c, _ in block.conv_norm_pairs())
+            if block._downsample is not None:
+                relu[id(list(block._downsample)[0])] = False
+    for l in range(head._num_heads):
+        relu[id(neck.level(l)[0])] = True
+        cls_tower, reg_tower, _, _ = head.level_paths(l)
+        relu.update((id(c), n is None) for c, n in list(cls_tower) + list(reg_tower))
+    return relu
+
+
+def rn16_bound(t, dtype, d):
+    """The kernels store round-to-nearest-even 16-bit values of fp32 results (cvt.rn, ptx.cuh).  For fp32 values v >= t (d = -1) resp.
+    v <= t (d = +1), t float64: the bound RN16(v) >= RN16(RD32(t)) resp. <= RN16(RU32(t)) -- both roundings are monotone -- as float64."""
+    f = t.float()
+    off = (f.double() > t) if d < 0 else (f.double() < t)
+    f = torch.where(off, torch.nextafter(f, torch.full_like(f, float('inf') * d)), f)
+    return f.to(DTYPES[dtype][0]).double()
+
+
+def chain_interval(x, layers, res, dtype, device):
+    """A chain of convs run by one kernel whose outputs, the last one included, are stored as 16-bit values (a fused 1x1 tail behind a
+    conv, the four convs of STEM4): layers = [(modules, relu)], res added to the last.  -> (ref, lo, hi): the float64 chain on the
+    reference's round-to-nearest intermediates, and per element the 16-bit values a correct kernel may store.
+
+    Each conv accumulates in fp32 within K 2^-24 S of its exact value (ref_conv64's bound) and stores the round-to-nearest 16-bit value
+    of its fp32 result (ReLU fused into the conversion).  So the kernel's value lies in [RN(relu(y - P - d)), RN(relu(y + P + d))] (rn16_bound),
+    where y is the exact value on the reference's input, d = K 2^-24 S and P = |W| * (how far the kernel's input may lie from the
+    reference's), propagated from the previous layer (ReLU and rounding are monotone).  Where no rounding midpoint lies within P + d of y
+    -- almost everywhere -- the interval is one 16-bit value; where one does, the next layer widens by |W| times that one step only around
+    it.  (A faithful rounding, either neighbour, would widen every element by one step at every layer.)"""
+    import torch.nn.functional as F
+    from lfd._engine import InferencePlan, fold_scale
+    rnd = DTYPES[dtype][1]
+    t, reach = x.to(device).double(), None          # reach: how far the kernel's input may lie from the reference's, per element
+    for li, (mods, relu) in enumerate(layers):
+        r = res if li == len(layers) - 1 else None
+        pre, S, K = folded64(t, mods, False, res=r, dtype=dtype, device=device)
+        P = torch.zeros_like(pre)
+        if reach is not None:
+            conv = mods[0]
+            _, S, K = folded64(t.abs() + reach, mods, False, res=r, dtype=dtype, device=device)   # S over the widest input the kernel may see
+            w = rnd(fold_scale(conv.weight, InferencePlan._fold(*mods)[0])).double().to(device).abs()
+            P = F.conv2d(reach.permute(0, 3, 1, 2), w, None, stride=conv.stride[0], padding=conv.kernel_size[0] // 2).permute(0, 2, 3, 1)
+        d = P + K * U * S
+        y, lo, hi = pre, pre - d, pre + d
+        if relu:
+            y, lo, hi = y.clamp(min=0), lo.clamp(min=0), hi.clamp(min=0)
+        lo, hi = rn16_bound(lo, dtype, -1), rn16_bound(hi, dtype, 1)
+        if r is not None or li == len(layers) - 1:
+            return y, lo, hi
+        t = rnd(y.float()).double()                                                             # the reference's intermediate
+        reach = torch.maximum(hi - t, t - lo)
+
+
+def check_conv_op(op, x, out, out2, res, dtype, what, relu):
+    """The outputs of a STEM0 / CONV / STEM4 op of the inference planner against float64 on the 16-bit input x [N, H, W, Cin] (the stem
+    operand for the stems) and residual res.  Convs, folding and strides come from the op's modules, ReLU from the layer records
+    (relu = layer_relu(model)).  One layer: a faithful rounding (check_faithful); behind 16-bit intermediates inside the kernel (a fused
+    1x1 tail, the four convs of STEM4): the interval chain_interval propagates through the chain.  -> [(output, max err / tol)]."""
+    import lfd._native as nat
+    dev = out.device
+    mods = [op['modules']] + [op[k] for k in ('tail_modules', 's2_modules', 's3_modules') if k in op]
+    assert len(mods) == (4 if op['kind'] == nat.OP_STEM4 else 2 if op.get('tail_cout') else 1), what
+    layers = [(m, relu[id(m[0])]) for m in mods]
+    if len(layers) == 1:
+        ref, S, K = folded64(x, layers[0][0], layers[0][1], res=res, dtype=dtype, device=dev)
+        got = [('out', check_faithful(out, ref, S, K, what + ' out', dtype))]
+    else:
+        name = 'stem4' if op['kind'] == nat.OP_STEM4 else 'fused tail'
+        ref, lo, hi = chain_interval(x, layers, res, dtype, dev)
+        got = [(name, check_interval(out, ref, lo, hi, '%s %s' % (what, name)))]
+    if out2 is not None:               # the fused 1x1/s2 shortcut reads the block input, stored without ReLU
+        sconv = op['ds_modules'][0]
+        assert not relu[id(sconv)], what
+        ref, S, K = folded64(x, op['ds_modules'], False, stride=2, dtype=dtype, device=dev)
+        got.append(('shortcut', check_faithful(out2.view(ref.shape), ref, S, K, what + ' shortcut', dtype)))
+    return got
+
+
+def check_interval(out, ref, lo, hi, what):
+    """lo <= out <= hi per element.  -> max |out - ref| / (the interval's reach from ref on that side)."""
+    o = out.to(ref.device).double()
+    ok = (o >= lo) & (o <= hi)
+    _report(what, o, ref, torch.maximum(hi - ref, ref - lo), ok)
+    reach = torch.where(o >= ref, hi - ref, ref - lo)
+    e = (o - ref).abs()
+    r = torch.where(e == 0, torch.zeros_like(e), e / reach.clamp(min=1e-300))
+    return float(r.max()) if r.numel() else 0.0
