@@ -526,6 +526,30 @@ typedef struct lfd_input_desc {
 int lfd_input_batch(const lfd_input_desc* descs, int n, const uint8_t* src, void* out, int out_mode, int swap_rb, int H, int W,
                     const float* mean, const float* scale, lfd_stream stream);
 
+/* ------------------------------------------------------------------------------------------ resized inference input
+ * Frames of any size run at the network's: R = cv2.resize(frame, (0, 0), fx = s, fy = s) on uint8, bit for bit, the rule of the
+ * reference's TypicalCOCOTrainingRegionSampler:
+ *   dh = round-half-even(src_h * s), dw = round-half-even(src_w * s) (in double);
+ *   LFD_RESIZE_COPY when dh x dw is src_h x src_w, LFD_RESIZE_AREA2 when 1 / s is 2 (within DBL_EPSILON), LFD_RESIZE_LINEAR otherwise
+ *   (upscaling included); the arithmetic of lfd_input_batch.
+ * lfd_resize_query (host only, no device needed): that rule -> *dh, *dw, *mode.  Source sides below 1, a scale that is not finite or not
+ * > 0, or an empty result: LFD_ERR_INVALID.  A side beyond the int range is reported as INT_MAX. */
+int lfd_resize_query(int src_h, int src_w, double scale, int* dh, int* dw, int* mode);
+/* Resizes n device frames of src_h x src_w by scale s into the top-left dh x dw corner of each image of dst, a capacity-layout uint8
+ * buffer [n][H][W][channels] (what lfd_plan_forward_extent reads as LFD_INPUT_U8_NHWC).  Bytes of dst outside the dh x dw extents are not
+ * written.  One launch, no host synchronisation, nothing allocated: it may precede a graph replay on the same stream.
+ *   src_format LFD_INPUT_U8_NHWC: channels = 3, BGR frames uint8 [n][src_h][src_w][3] -> BGR; channels = 1, gray frames [n][src_h][src_w]
+ *              -> gray (cv2.resize of the gray image).
+ *   src_format LFD_INPUT_U8_NV12: frames uint8 [n][3 src_h / 2][src_w] (LFD_INPUT_U8_NV12; src_h, src_w even); channels = 3: each tap is
+ *              converted to B, G, R before the resize arithmetic, which is cv2.resize(cv2.cvtColor(f, COLOR_YUV2BGR_NV12)); channels = 1:
+ *              the Y plane is resized (COLOR_YUV2GRAY_NV12) and the UV bytes are never read.
+ * src needs no alignment.  Every argument is checked before anything is enqueued, and a refused call writes nothing: a null pointer, a
+ * format other than these, channels other than 1 / 3, n, H or W < 1, an odd NV12 size, or what lfd_resize_query refuses is
+ * LFD_ERR_INVALID; dh > H or dw > W is LFD_ERR_CAPACITY; float32 frames (LFD_INPUT_F32_NCHW) are LFD_ERR_UNSUPPORTED, as are dw > 6144
+ * and n > 65535.  A BGR source for a gray model has no call here: colour to gray is not an inference input path. */
+int lfd_resize_frames(const void* src, int src_format, int channels, int n, int src_h, int src_w, double scale, uint8_t* dst, int H, int W,
+                      lfd_stream stream);
+
 /* ------------------------------------------------------------------------------------------ model files
  * A model file (written by lfd/_engine.py InferencePlan.export, lfd.deployment.export_model) is one inference plan with its weights and
  * its post-process, so that a program that links only this library and cudart runs a trained model: the same kernels, launches and
@@ -578,6 +602,18 @@ int lfd_engine_bind(lfd_engine* engine, void* weights, size_t weights_bytes, voi
  * or events between streams), as for one lfd_plan. */
 int lfd_engine_detect(lfd_engine* engine, const void* input, int input_format, int h, int w, float* dets, int32_t* labels, int32_t* count,
                       float* cls_out, float* reg_out, int use_graph, lfd_stream stream);
+/* One batch of N frames of any size src_h x src_w (uint8 BGR or gray, as op 0's Cin, or NV12: input_format LFD_INPUT_U8_NHWC /
+ * LFD_INPUT_U8_NV12, as lfd_resize_frames takes them) run at the network's size:
+ *   1. lfd_resize_frames by `scale` into `frames`, a caller-owned device buffer of the capacity layout uint8 [N][H][W][Cin], 256-byte
+ *      aligned (what cudaMalloc returns), whose bytes outside the resized dh x dw extent are never read;
+ *   2. the forward of lfd_engine_detect at dh x dw (lfd_plan_forward at the capacity, lfd_plan_forward_extent below it);
+ *   3. the post-process with the reference's meta of a resized image (lfd/model/lfd.py get_results): image size int(src_w * scale) x
+ *      int(src_h * scale), taken in double, and resize_scale = scale, so that dets are in source-frame coordinates.
+ * Every argument is checked before anything is enqueued, with lfd_resize_frames's codes (dh > H or dw > W: LFD_ERR_CAPACITY; float32
+ * frames: LFD_ERR_UNSUPPORTED); frames not 256-byte aligned or an unbound engine is LFD_ERR_INVALID.  Outputs, cls_out / reg_out, use_graph
+ * and streams as lfd_engine_detect. */
+int lfd_engine_detect_resized(lfd_engine* engine, const void* input, int input_format, int src_h, int src_w, double scale, uint8_t* frames,
+                              float* dets, int32_t* labels, int32_t* count, float* cls_out, float* reg_out, int use_graph, lfd_stream stream);
 int lfd_engine_num_launches(const lfd_engine* engine); /* lfd_plan_num_launches of the bound plan (0 before lfd_engine_bind) */
 
 #ifdef __cplusplus

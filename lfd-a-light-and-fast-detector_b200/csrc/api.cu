@@ -1,5 +1,7 @@
 // api.cu -- the extern "C" boundary of liblfd_b200.so (declared in include/lfd_b200.h).
 #include <stdarg.h>
+#include <cfloat>
+#include <climits>
 #include <cmath>
 #include <stdio.h>
 #include <string.h>
@@ -1306,6 +1308,81 @@ extern "C" int lfd_input_batch(const lfd_input_desc* descs, int n, const uint8_t
     return LFD_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ resized inference input
+// The size and interpolation of cv2.resize(frame, (0, 0), fx = s, fy = s) on uint8, stated once (region_sampler.resize_plan is the same
+// rule in Python): each side round-half-even(side * s) (nearbyint in the default rounding mode, as cv2's saturate_cast), a copy when the
+// size is kept, INTER_AREA when 1 / s is 2 (cv2: within DBL_EPSILON of the integer 2), INTER_LINEAR otherwise, upscaling included.
+// A side too large for an int is reported as INT_MAX: it exceeds every capacity.
+static int resize_rule(const char* fn, int h, int w, double s, int* dh, int* dw, int* mode) {
+    if (h < 1 || w < 1) return fail(LFD_ERR_INVALID, "%s: source frames of %dx%d", fn, h, w);
+    if (!std::isfinite(s) || s <= 0.0) return fail(LFD_ERR_INVALID, "%s: resize scale %g (finite and > 0)", fn, s);
+    const double rh = std::nearbyint((double)h * s), rw = std::nearbyint((double)w * s);
+    if (rh < 1.0 || rw < 1.0) return fail(LFD_ERR_INVALID, "%s: resize scale %.17g makes a %dx%d frame empty", fn, s, h, w);
+    *dh = rh >= (double)INT_MAX ? INT_MAX : (int)rh;
+    *dw = rw >= (double)INT_MAX ? INT_MAX : (int)rw;
+    const double inv = 1.0 / s, iinv = std::nearbyint(inv);
+    if (*dh == h && *dw == w) *mode = LFD_RESIZE_COPY;
+    else if (std::fabs(inv - iinv) < DBL_EPSILON && iinv == 2.0) *mode = LFD_RESIZE_AREA2;
+    else *mode = LFD_RESIZE_LINEAR;
+    return LFD_OK;
+}
+
+extern "C" int lfd_resize_query(int src_h, int src_w, double scale, int* dh, int* dw, int* mode) {
+    if (!dh || !dw || !mode) return fail(LFD_ERR_INVALID, "lfd_resize_query: null argument");
+    return resize_rule("lfd_resize_query", src_h, src_w, scale, dh, dw, mode);
+}
+
+// One resize launch, checked: the geometry every frame of the batch shares and where the frames lie
+struct ResizeCall {
+    lfd_input_desc d;
+    size_t src_stride;   // bytes from one source frame to the next
+    int nv12_bgr;        // NV12 frames to BGR (d: the Y plane); an NV12 frame on a gray model is its Y plane, a gray frame
+};
+
+// Every argument of lfd_resize_frames, before anything is enqueued
+static int check_resize(const char* fn, const void* src, int fmt, int channels, int n, int h, int w, double s, const void* dst, int H, int W,
+                        ResizeCall* out) {
+    if (!src || !dst) return fail(LFD_ERR_INVALID, "%s: null argument", fn);
+    if (fmt == LFD_INPUT_F32_NCHW) return fail(LFD_ERR_UNSUPPORTED, "%s: float32 frames are not resized (uint8 BGR, gray or NV12 frames are)", fn);
+    if (fmt != LFD_INPUT_U8_NHWC && fmt != LFD_INPUT_U8_NV12)
+        return fail(LFD_ERR_INVALID, "%s: input format %d (1 = uint8 NHWC, 2 = uint8 NV12)", fn, fmt);
+    if (channels != 1 && channels != 3) return fail(LFD_ERR_INVALID, "%s: channels = %d (3 = BGR, 1 = gray)", fn, channels);
+    if (n < 1 || H < 1 || W < 1) return fail(LFD_ERR_INVALID, "%s: bad arguments (n=%d H=%d W=%d)", fn, n, H, W);
+    if (fmt == LFD_INPUT_U8_NV12 && ((h | w) & 1)) return fail(LFD_ERR_INVALID, "%s: an NV12 frame has an even height and width, got %dx%d", fn, h, w);
+    int dh = 0, dw = 0, mode = 0;
+    int rc = resize_rule(fn, h, w, s, &dh, &dw, &mode);
+    if (rc) return rc;
+    if (dh > H || dw > W)
+        return fail(LFD_ERR_CAPACITY, "%s: %dx%d frames at scale %.17g are %dx%d, beyond the destination's %dx%d", fn, h, w, s, dh, dw, H, W);
+    if (dw > 6144) return fail(LFD_ERR_UNSUPPORTED, "%s: resized width %d > 6144 (the column table lives in 48 KB of shared memory)", fn, dw);
+    if (n > 65535) return fail(LFD_ERR_UNSUPPORTED, "%s: n=%d > 65535", fn, n);
+    const bool nv12 = fmt == LFD_INPUT_U8_NV12;
+    const int c = nv12 ? 1 : channels;   // bytes per pixel of the plane the taps read
+    lfd_input_desc d{};
+    d.inv_scale = 1.0 / s;
+    d.pitch = w * c;
+    d.channels = c;
+    d.win_w = d.src_w = w;
+    d.win_h = d.src_h = h;
+    d.out_w = d.dw = dw;
+    d.out_h = d.dh = dh;
+    d.mode = mode;
+    out->d = d;
+    out->src_stride = nv12 ? (size_t)h * w * 3 / 2 : (size_t)h * w * c;
+    out->nv12_bgr = nv12 && channels == 3;
+    return LFD_OK;
+}
+
+extern "C" int lfd_resize_frames(const void* src, int src_format, int channels, int n, int src_h, int src_w, double scale, uint8_t* dst, int H,
+                                 int W, lfd_stream stream) {
+    ResizeCall rs;
+    int rc = check_resize("lfd_resize_frames", src, src_format, channels, n, src_h, src_w, scale, dst, H, W, &rs);
+    if (rc) return rc;
+    if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_resize_frames: no CUDA device (there is no CPU fallback)");
+    CUDA_TRY(resize_frames_launch(rs.d, static_cast<const uint8_t*>(src), rs.src_stride, n, rs.nv12_bgr, dst, H, W, st_of(stream)));
+    return LFD_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ model files (lfd_engine_*)
 // The layout is documented in include/lfd_b200.h and DESIGN.md "Model files"; lfd/_engine.py InferencePlan.export is the writer.
 static constexpr size_t kModelHeaderBytes = 48, kModelPlanBytes = 120;
@@ -1328,7 +1405,8 @@ struct lfd_engine {
     lfd_plan* plan = nullptr;
     uint8_t *weights = nullptr, *ws = nullptr, *post_ws = nullptr;
     std::vector<lfd_extent> ext;              // the geometry table of the last frame below the capacity
-    int meta_h = 0, meta_w = 0;               // the frame size the post-process workspace holds (0: none yet), written on meta_stream
+    int meta_h = 0, meta_w = 0;               // the image size the post-process workspace holds (0: none yet), written on meta_stream
+    float meta_s = 0.f;                       // and the resize scale
     cudaStream_t meta_stream = nullptr;
     ~lfd_engine() { lfd_plan_destroy(plan); }
 };
@@ -1659,6 +1737,7 @@ extern "C" int lfd_engine_bind(lfd_engine* e, void* weights, size_t weights_byte
     e->ws = reinterpret_cast<uint8_t*>(workspace);
     e->post_ws = reinterpret_cast<uint8_t*>(post_workspace);
     e->meta_h = e->meta_w = 0;
+    e->meta_s = 0.f;
     return LFD_OK;
 }
 
@@ -1684,12 +1763,13 @@ static int fill_f32(float* dst, float v, size_t n, cudaStream_t st) {
     return LFD_OK;
 }
 
-extern "C" int lfd_engine_detect(lfd_engine* e, const void* input, int input_format, int h, int w, float* dets, int32_t* labels, int32_t* count,
-                                 float* cls_out, float* reg_out, int use_graph, lfd_stream stream) {
-    if (!e || !input || !dets || !labels || !count) return fail(LFD_ERR_INVALID, "lfd_engine_detect: null argument");
-    if (!e->plan) return fail(LFD_ERR_INVALID, "lfd_engine_detect: the engine is not bound (lfd_engine_bind)");
-    if (h < 1 || w < 1 || h > e->H || w > e->W) return fail(LFD_ERR_INVALID, "lfd_engine_detect: frame %dx%d outside the capacity %dx%d", h, w, e->H, e->W);
-    int rc = check_input_format("lfd_engine_detect", input_format, &e->ops[0], h, w);
+// lfd_engine_detect on an h x w frame with the post-process's image size img_w x img_h and resize scale
+static int engine_detect(lfd_engine* e, const char* fn, const void* input, int input_format, int h, int w, int img_w, int img_h, float scale,
+                         float* dets, int32_t* labels, int32_t* count, float* cls_out, float* reg_out, int use_graph, lfd_stream stream) {
+    if (!e || !input || !dets || !labels || !count) return fail(LFD_ERR_INVALID, "%s: null argument", fn);
+    if (!e->plan) return fail(LFD_ERR_INVALID, "%s: the engine is not bound (lfd_engine_bind)", fn);
+    if (h < 1 || w < 1 || h > e->H || w > e->W) return fail(LFD_ERR_INVALID, "%s: frame %dx%d outside the capacity %dx%d", fn, h, w, e->H, e->W);
+    int rc = check_input_format(fn, input_format, &e->ops[0], h, w);
     if (rc) return rc;
     const int n_ops = (int)e->ops.size();
     // the frame's geometry: every op's extent follows from its producer's, as a plan built for h x w has it (lfd/_engine.py extent_table)
@@ -1727,13 +1807,15 @@ extern "C" int lfd_engine_detect(lfd_engine* e, const void* input, int input_for
     if (rc) return rc;
     float* meta = reinterpret_cast<float*>(e->post_ws + engine_meta_off(e));
     const size_t N = (size_t)e->N;
-    // written once per frame size and stream: the post-process workspace is the engine's alone, and a call on another stream writes it
-    // again so that its post-process is ordered after the values it reads
-    if (h != e->meta_h || w != e->meta_w || st != e->meta_stream) {
+    // written once per image size, scale and stream: the post-process workspace is the engine's alone, and a call on another stream writes
+    // it again so that its post-process is ordered after the values it reads
+    if (img_h != e->meta_h || img_w != e->meta_w || scale != e->meta_s || st != e->meta_stream) {
         e->meta_h = e->meta_w = 0;
-        if ((rc = fill_f32(meta, (float)w, N, st)) || (rc = fill_f32(meta + N, (float)h, N, st)) || (rc = fill_f32(meta + 2 * N, 1.0f, N, st))) return rc;
-        e->meta_h = h;
-        e->meta_w = w;
+        if ((rc = fill_f32(meta, (float)img_w, N, st)) || (rc = fill_f32(meta + N, (float)img_h, N, st)) || (rc = fill_f32(meta + 2 * N, scale, N, st)))
+            return rc;
+        e->meta_h = img_h;
+        e->meta_w = img_w;
+        e->meta_s = scale;
         e->meta_stream = st;
     }
     int32_t* src = reinterpret_cast<int32_t*>(e->post_ws + engine_src_off(e));
@@ -1741,4 +1823,25 @@ extern "C" int lfd_engine_detect(lfd_engine* e, const void* input, int input_for
         return lfd_postprocess_soft_nms(&cfg, cls, reg, meta, meta + N, meta + 2 * N, e->post_ws, dets, labels, src, count, count + N, e->soft_method,
                                         e->soft_sigma, e->soft_min_score, stream);
     return lfd_postprocess(&cfg, cls, reg, meta, meta + N, meta + 2 * N, e->post_ws, dets, labels, src, count, count + N, stream);
+}
+
+extern "C" int lfd_engine_detect(lfd_engine* e, const void* input, int input_format, int h, int w, float* dets, int32_t* labels, int32_t* count,
+                                 float* cls_out, float* reg_out, int use_graph, lfd_stream stream) {
+    return engine_detect(e, "lfd_engine_detect", input, input_format, h, w, w, h, 1.0f, dets, labels, count, cls_out, reg_out, use_graph, stream);
+}
+
+extern "C" int lfd_engine_detect_resized(lfd_engine* e, const void* input, int input_format, int src_h, int src_w, double scale, uint8_t* frames,
+                                         float* dets, int32_t* labels, int32_t* count, float* cls_out, float* reg_out, int use_graph,
+                                         lfd_stream stream) {
+    const char* fn = "lfd_engine_detect_resized";
+    if (!e || !input || !frames || !dets || !labels || !count) return fail(LFD_ERR_INVALID, "%s: null argument", fn);
+    if (!e->plan) return fail(LFD_ERR_INVALID, "%s: the engine is not bound (lfd_engine_bind)", fn);
+    if ((uintptr_t)frames & 255) return fail(LFD_ERR_INVALID, "%s: frames %p must be 256-byte aligned (as cudaMalloc returns)", fn, (void*)frames);
+    ResizeCall rs;
+    int rc = check_resize(fn, input, input_format, e->ops[0].Cin, e->N, src_h, src_w, scale, frames, e->H, e->W, &rs);
+    if (rc) return rc;
+    CUDA_TRY(resize_frames_launch(rs.d, static_cast<const uint8_t*>(input), rs.src_stride, e->N, rs.nv12_bgr, frames, e->H, e->W, st_of(stream)));
+    // the reference's meta of a resized image: resized_width = int(w * s), resized_height = int(h * s) in double, resize_scale = s
+    return engine_detect(e, fn, frames, LFD_INPUT_U8_NHWC, rs.d.dh, rs.d.dw, (int)((double)src_w * scale), (int)((double)src_h * scale), (float)scale,
+                         dets, labels, count, cls_out, reg_out, use_graph, stream);
 }

@@ -6,8 +6,14 @@
 // neighbourhoods directly from the window (the resized image is never materialised) and writes 12 bytes (uint8 NHWC) or one float4
 // per channel plane (fp32 NCHW), so consecutive threads store consecutive addresses.  The gray modes (uint8 [n,H,W], fp32 [n,1,H,W])
 // convert a BGR source to gray at every tap they read, then resize the gray values; they store 4 bytes or one float4.
+//
+// lfd_resize_frames (resize_frames_kernel) runs the same per-tap code on N whole frames of one size and scale: one geometry for the
+// batch, passed by value, and only the resized h x w extent of each destination image is written.  An NV12 source is converted to
+// B, G, R at every tap it reads (nv12_to_bgr), then resized, as cv2.resize of cv2.cvtColor(COLOR_YUV2BGR_NV12) computes it.
 #include "../../include/lfd_b200.h"
 #include "kernels.cuh"
+
+#include <type_traits>
 
 namespace lfd {
 namespace {
@@ -47,9 +53,17 @@ struct RowInfo {
     int b0, b1;          // LINEAR: vertical weights; AREA2: b1 = 1 when the block has two rows
     int kind;            // 0 = pixel row, kZero, kPad
 };
+// an NV12 source's rows: r0 / r1 in the Y plane, and the interleaved (U, V) rows that go with them
+struct Nv12RowInfo : RowInfo {
+    const uint8_t* u0;
+    const uint8_t* u1;
+};
 
-__device__ RowInfo row_info(const lfd_input_desc& d, const uint8_t* win, int y) {
-    RowInfo ri{nullptr, nullptr, 2048, 0, 0};
+// NV12 (RI = Nv12RowInfo): the window is a whole frame's Y plane (win_y = 0, win_h = its rows), followed by its UV plane at the same pitch
+template <class RI = RowInfo>
+__device__ RI row_info(const lfd_input_desc& d, const uint8_t* win, int y) {
+    RI ri{};
+    ri.b0 = 2048;
     if (y >= d.out_h) { ri.kind = kPad; return ri; }
     const int r = d.crop_y + y;
     if (r < 0 || r >= d.dh || d.win_h <= 0) { ri.kind = kZero; return ri; }
@@ -72,6 +86,10 @@ __device__ RowInfo row_info(const lfd_input_desc& d, const uint8_t* win, int y) 
     y1 = min(max(y1 - d.win_y, 0), d.win_h - 1);
     ri.r0 = win + (size_t)y0 * d.pitch;
     ri.r1 = win + (size_t)y1 * d.pitch;
+    if constexpr (std::is_same<RI, Nv12RowInfo>::value) {
+        ri.u0 = win + ((size_t)d.win_h + (y0 >> 1)) * d.pitch;
+        ri.u1 = win + ((size_t)d.win_h + (y1 >> 1)) * d.pitch;
+    }
     return ri;
 }
 
@@ -92,6 +110,28 @@ __device__ __forceinline__ int resample(const lfd_input_desc& d, const RowInfo& 
     const int h0 = p00 * a0 + (two ? tap(ri.r0, x1) * a1 : 0);
     const int h1 = tap(ri.r1, x0) * a0 + (two ? tap(ri.r1, x1) * a1 : 0);
     return min((((h0 >> 4) * ri.b0 >> 16) + ((h1 >> 4) * ri.b1 >> 16) + 2) >> 2, 255);
+}
+
+// channel k (0 = B, 1 = G, 2 = R) of the NV12 pixel at column x of Y row r (ri.r0 or ri.r1): its Y byte and the (U, V) pair of its 2x2
+// block, from the UV row of r (when r0 and r1 are one row, so are u0 and u1)
+__device__ __forceinline__ int nv12_tap(const Nv12RowInfo& ri, const uint8_t* r, int x, int k) {
+    const uint8_t* uv = (r == ri.r0 ? ri.u0 : ri.u1) + (x & ~1);
+    uint32_t bgr[3];
+    nv12_to_bgr(r[x], uv[0], uv[1], bgr);
+    return (int)bgr[k];
+}
+
+// one output pixel of an NV12 source: B, G, R in bits 0..23, each tap converted (nv12_tap) before the resize arithmetic of pixel()
+__device__ __forceinline__ uint32_t nv12_pixel(const lfd_input_desc& d, const Nv12RowInfo& ri, int2 col) {
+    if (ri.kind != 0 || col.x < 0 || d.win_w <= 0) return 0u;
+    const int wmax = d.win_w - 1;
+    const int x0 = min(max(col.x, 0), wmax);
+    const int x1 = min(max(col.x + 1, 0), wmax);
+    uint32_t packed = 0u;
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+        packed |= (uint32_t)resample(d, ri, col, x0, x1, [&](const uint8_t* r, int x) { return nv12_tap(ri, r, x, k); }) << (8 * k);
+    return packed;
 }
 
 // one output pixel: channel k of the source order in bits 8k..8k+7 (a gray source replicated)
@@ -134,6 +174,25 @@ __device__ __forceinline__ uint32_t gray_pixel(const lfd_input_desc& d, const Ro
     return resample(d, ri, col, x0, x1, [](const uint8_t* r, int x) { return (int)bgr_to_gray(r[3 * x], r[3 * x + 1], r[3 * x + 2]); });
 }
 
+// the n <= 4 pixels v[0..n) of a uint8 output row at o: BGR 3 bytes each (three aligned words when n == 4 and o allows), gray 1 byte
+__device__ __forceinline__ void store_u8_bgr(uint8_t* o, const uint32_t (&v)[4], int n) {
+    if (n == 4 && (reinterpret_cast<uintptr_t>(o) & 3) == 0) {
+        uint32_t* ow = reinterpret_cast<uint32_t*>(o);
+        ow[0] = v[0] | v[1] << 24;
+        ow[1] = v[1] >> 8 | v[2] << 16;
+        ow[2] = v[2] >> 16 | v[3] << 8;
+    } else {
+        for (int j = 0; j < n * 3; ++j) o[j] = (uint8_t)(v[j / 3] >> (8 * (j % 3)));
+    }
+}
+__device__ __forceinline__ void store_u8_gray(uint8_t* o, const uint32_t (&v)[4], int n) {
+    if (n == 4 && (reinterpret_cast<uintptr_t>(o) & 3) == 0) {
+        *reinterpret_cast<uint32_t*>(o) = v[0] | v[1] << 8 | v[2] << 16 | v[3] << 24;
+    } else {
+        for (int j = 0; j < n; ++j) o[j] = (uint8_t)v[j];
+    }
+}
+
 template <int OUT_MODE>
 __global__ void __launch_bounds__(kThreads) input_batch_kernel(const lfd_input_desc* __restrict__ descs, const uint8_t* __restrict__ src,
                                                                void* __restrict__ out, int swap_rb, int H, int W, float3 mean, float3 scale) {
@@ -158,15 +217,7 @@ __global__ void __launch_bounds__(kThreads) input_batch_kernel(const lfd_input_d
         }
         const int n = min(4, W - x);
         if constexpr (OUT_MODE == LFD_INPUT_OUT_U8_NHWC) {
-            uint8_t* o = reinterpret_cast<uint8_t*>(out) + (((size_t)img * H + y) * W + x) * 3;
-            if (n == 4 && (reinterpret_cast<uintptr_t>(o) & 3) == 0) {
-                uint32_t* ow = reinterpret_cast<uint32_t*>(o);
-                ow[0] = v[0] | v[1] << 24;
-                ow[1] = v[1] >> 8 | v[2] << 16;
-                ow[2] = v[2] >> 16 | v[3] << 8;
-            } else {
-                for (int j = 0; j < n * 3; ++j) o[j] = (uint8_t)(v[j / 3] >> (8 * (j % 3)));
-            }
+            store_u8_bgr(reinterpret_cast<uint8_t*>(out) + (((size_t)img * H + y) * W + x) * 3, v, n);
         } else if constexpr (OUT_MODE == LFD_INPUT_OUT_F32_NCHW) {
             const float m[3] = {mean.x, mean.y, mean.z}, s[3] = {scale.x, scale.y, scale.z};
 #pragma unroll
@@ -185,12 +236,7 @@ __global__ void __launch_bounds__(kThreads) input_batch_kernel(const lfd_input_d
                 }
             }
         } else if constexpr (OUT_MODE == LFD_INPUT_OUT_U8_GRAY) {
-            uint8_t* o = reinterpret_cast<uint8_t*>(out) + ((size_t)img * H + y) * W + x;
-            if (n == 4 && (reinterpret_cast<uintptr_t>(o) & 3) == 0) {
-                *reinterpret_cast<uint32_t*>(o) = v[0] | v[1] << 8 | v[2] << 16 | v[3] << 24;
-            } else {
-                for (int j = 0; j < n; ++j) o[j] = (uint8_t)v[j];
-            }
+            store_u8_gray(reinterpret_cast<uint8_t*>(out) + ((size_t)img * H + y) * W + x, v, n);
         } else {   // LFD_INPUT_OUT_F32_GRAY: one plane, one constant pair (mean.x, scale.x)
             float f[4];
 #pragma unroll
@@ -208,7 +254,60 @@ __global__ void __launch_bounds__(kThreads) input_batch_kernel(const lfd_input_d
     }
 }
 
+// lfd_resize_frames: N frames of one size, one geometry.  d describes every frame as a whole-image window (crop 0, out = the resized
+// dh x dw); frame n starts at src + n * src_stride; destination image n is uint8 [H][W][3] (BGR) or [H][W] (GRAY) at dst + n * H * W * ch.
+struct ResizeArgs {
+    lfd_input_desc d;
+    const uint8_t* src;
+    size_t src_stride;
+    uint8_t* dst;
+    int H, W;
+};
+
+// One CTA per (frame, band of kBandRows resized rows), as input_batch_kernel; rows and columns beyond dh x dw are not written.
+// GRAY: a gray source or an NV12 frame's Y plane (d.channels = 1); NV12: 3-channel output from NV12 taps.
+template <bool GRAY, bool NV12>
+__global__ void __launch_bounds__(kThreads) resize_frames_kernel(const __grid_constant__ ResizeArgs a) {
+    extern __shared__ int2 cols[];   // [dw]
+    const lfd_input_desc& d = a.d;
+    const int dw = d.out_w;
+    for (int x = threadIdx.x; x < dw; x += kThreads) cols[x] = column_entry(d, x);
+    __syncthreads();
+    const int img = blockIdx.y;
+    const uint8_t* win = a.src + img * a.src_stride;
+    const int groups = (dw + 3) >> 2;
+    const int y_begin = blockIdx.x * kBandRows;
+    const int rows = min(kBandRows, d.out_h - y_begin);
+    for (int t = threadIdx.x; t < rows * groups; t += kThreads) {
+        const int y = y_begin + t / groups, x = (t % groups) * 4;
+        using RI = std::conditional_t<NV12, Nv12RowInfo, RowInfo>;
+        const RI ri = row_info<RI>(d, win, y);
+        uint32_t v[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if (x + j >= dw) v[j] = 0u;
+            else if constexpr (NV12) v[j] = nv12_pixel(d, ri, cols[x + j]);
+            else v[j] = GRAY ? gray_pixel(d, ri, cols[x + j]) : pixel(d, ri, cols[x + j]);
+        }
+        const int n = min(4, dw - x);
+        const size_t o = ((size_t)img * a.H + y) * a.W + x;
+        if constexpr (GRAY) store_u8_gray(a.dst + o, v, n);
+        else store_u8_bgr(a.dst + o * 3, v, n);
+    }
+}
+
 }  // namespace
+
+cudaError_t resize_frames_launch(const lfd_input_desc& d, const uint8_t* src, size_t src_stride, int n, int nv12_bgr, uint8_t* dst, int H,
+                                 int W, cudaStream_t st) {
+    const ResizeArgs a{d, src, src_stride, dst, H, W};
+    const dim3 grid((d.out_h + kBandRows - 1) / kBandRows, n);
+    const size_t smem = (size_t)d.out_w * sizeof(int2);
+    if (nv12_bgr) resize_frames_kernel<false, true><<<grid, kThreads, smem, st>>>(a);
+    else if (d.channels == 1) resize_frames_kernel<true, false><<<grid, kThreads, smem, st>>>(a);
+    else resize_frames_kernel<false, false><<<grid, kThreads, smem, st>>>(a);
+    return cudaGetLastError();
+}
 
 cudaError_t input_batch_launch(const void* descs, int n, const uint8_t* src, void* out, int out_mode, int swap_rb, int H, int W,
                                const float* mean, const float* scale, cudaStream_t st) {

@@ -111,6 +111,24 @@ def check_nv12_frame(x, N, H, W):
     return h, w
 
 
+def check_source(x, N, channels, nv12):
+    """x: N source frames of any size for a resized forward -- uint8 [N,h,w,3] (BGR), [N,h,w] or [N,h,w,1] (gray, channels = 1), or with nv12
+    NV12 frames uint8 [N,3h/2,w] of even h and w -- contiguous, on a CUDA device -> (its nat.INPUT_* format, h, w).  float32 frames are
+    refused: the resize reads uint8."""
+    if x.dtype != torch.uint8:
+        raise ValueError('resized frames are uint8 (BGR, gray or NV12), got %s' % (x.dtype,))
+    if nv12:
+        ok = x.dim() == 3 and x.shape[1] % 3 == 0 and x.shape[2] % 2 == 0     # 3h/2 rows of an even h
+        fmt, h, w = nat.INPUT_U8_NV12, (int(x.shape[1]) // 3 * 2 if ok else 0), (int(x.shape[2]) if ok else 0)
+    else:
+        ok = x.dim() >= 3 and _u8_shape_ok(tuple(x.shape), x.shape[0], x.shape[1], x.shape[2], channels)
+        fmt, h, w = nat.INPUT_U8_NHWC, (int(x.shape[1]) if ok else 0), (int(x.shape[2]) if ok else 0)
+    if not ok or x.shape[0] != N or h < 1 or w < 1 or not x.is_cuda or not x.is_contiguous():
+        want = 'NV12 frames uint8 [N, 3h/2, w] of even h and w' if nv12 else ('uint8 [N, h, w, 3]' if channels == 3 else 'uint8 [N, h, w]')
+        raise ValueError('resized input must be N=%d contiguous CUDA frames, %s; got %s' % (N, want, tuple(x.shape)))
+    return fmt, h, w
+
+
 def stage_nv12(stage, x, h, w):
     """Copies NV12 frames x [N, 3h/2, w] into the capacity layout stage [N, 3H/2, W]: the Y rows into the top-left corner of the H x W Y
     plane, the UV rows into the top-left corner of the H/2 x W UV plane."""
@@ -807,7 +825,7 @@ class InferencePlan(object):
     def num_graphs(self):
         return nat.lib().lfd_plan_num_graphs(self.handle)
 
-    def forward(self, x, use_graph=True, slot=0, frame_format=None):
+    def forward(self, x, use_graph=True, slot=0, frame_format=None, resize_scale=None):
         """x: cuda float32 [N,3,h,w] (contiguous) or uint8 [N,h,w,3] with h <= H and w <= W; with frame_format='nv12', NV12 video frames
         uint8 [N,3h/2,w] of even h and w (include/lfd_b200.h, LFD_INPUT_U8_NV12), which give bit for bit what the uint8 path gives on
         cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12).  A gray plan (in_channels 1) takes float32 [N,1,h,w] or uint8 [N,h,w] / [N,h,w,1], and
@@ -815,17 +833,23 @@ class InferencePlan(object):
         plan-owned buffers of output `slot` (a second slot lets the post-process of one batch overlap the forward of the next,
         lfd/pipeline.py): (N, P, C') and (N, P, 4) for the frame's P points, laid out as a plan built for h x w lays them out;
         frame_level_sizes / frame_P describe them.  A frame of the full size is read in place; a smaller one is first copied into the
-        top-left corner of a plan-owned input, so that every frame size replays the same CUDA graph (one per input format)."""
+        top-left corner of a plan-owned input, so that every frame size replays the same CUDA graph (one per input format).
+        resize_scale=s: x holds N uint8 frames of any size h x w (above the capacity too; BGR [N,h,w,3], gray [N,h,w], or NV12 with
+        frame_format='nv12'), resized on the device into the plan-owned input exactly as cv2.resize(frame, (0, 0), fx=s, fy=s) resizes them
+        (lfd_resize_frames; NV12 as cv2.resize of the converted frame), and the forward runs at the resized size (nat.resize_query), which
+        must fit the capacity."""
         if self.handle is None:
             raise nat.LfdError('this plan was built for host-side inspection only (create_native=False)')
+        if frame_format not in (None, 'nv12'):
+            raise ValueError("frame_format must be None (float32 NCHW or uint8 BGR, by dtype) or 'nv12', got %r" % (frame_format,))
+        if resize_scale is not None:
+            return self._forward_resized(x, use_graph, slot, frame_format == 'nv12', float(resize_scale))
         if frame_format is None:
             fmt, h, w = check_frame(x, self.N, self.H, self.W, self.in_channels)
             if fmt == nat.INPUT_U8_NHWC and self.in_channels == 1:
                 x = x.view(self.N, h, w)
-        elif frame_format == 'nv12':
-            fmt, (h, w) = nat.INPUT_U8_NV12, check_nv12_frame(x, self.N, self.H, self.W)
         else:
-            raise ValueError("frame_format must be None (float32 NCHW or uint8 BGR, by dtype) or 'nv12', got %r" % (frame_format,))
+            fmt, (h, w) = nat.INPUT_U8_NV12, check_nv12_frame(x, self.N, self.H, self.W)
         cls_out, reg_out = self.outputs(slot)
         lib = nat.lib()
         if (h, w) == (self.H, self.W):
@@ -847,9 +871,36 @@ class InferencePlan(object):
                 stage[:, :, :h, :w].copy_(x)
             nat.check(lib.lfd_plan_forward_extent(self.handle, nat.ptr(stage), fmt, h, w, table, nat.ptr(self.workspace), nat.ptr(cls_out),
                                                   nat.ptr(reg_out), int(bool(use_graph)), nat.stream_ptr()))
+        return self._frame_outputs(cls_out, reg_out, level_sizes, P)
+
+    def _frame_outputs(self, cls_out, reg_out, level_sizes, P):
         self.frame_level_sizes, self.frame_P = level_sizes, P
         n, c = self.N, self.cls_channels
         return cls_out.view(-1)[:n * P * c].view(n, P, c), reg_out.view(-1)[:n * P * 4].view(n, P, 4)
+
+    def _forward_resized(self, x, use_graph, slot, nv12, s):
+        """forward(x, resize_scale=s): the resize into the uint8 staging input, then the forward at the resized extent on that input (one
+        CUDA graph for the capacity, one for every size below it, as for frames staged by copy)."""
+        if self.conv_impl != nat.CONV_UMMA:
+            raise nat.LfdError('the SIMT cross-check plan does not take resized frames')
+        fmt, h, w = check_source(x, self.N, self.in_channels, nv12)
+        _, dh, dw = nat.resize_query(h, w, s)
+        if dh > self.H or dw > self.W:
+            raise ValueError('%dx%d frames at resize scale %r are %dx%d, beyond the plan\'s capacity %dx%d' % (h, w, s, dh, dw, self.H, self.W))
+        cls_out, reg_out = self.outputs(slot)
+        lib = nat.lib()
+        with torch.cuda.device(self.device):
+            stage = self.staging(nat.INPUT_U8_NHWC)
+            st = nat.stream_ptr()
+            nat.check(lib.lfd_resize_frames(nat.ptr(x), fmt, self.in_channels, self.N, h, w, s, nat.ptr(stage), self.H, self.W, st))
+            if (dh, dw) == (self.H, self.W):
+                nat.check(lib.lfd_plan_forward(self.handle, nat.ptr(stage), nat.INPUT_U8_NHWC, nat.ptr(self.workspace), nat.ptr(cls_out),
+                                               nat.ptr(reg_out), int(bool(use_graph)), st))
+                return self._frame_outputs(cls_out, reg_out, self.level_sizes, self.P)
+            table, level_sizes, P = self._extent(dh, dw)
+            nat.check(lib.lfd_plan_forward_extent(self.handle, nat.ptr(stage), nat.INPUT_U8_NHWC, dh, dw, table, nat.ptr(self.workspace),
+                                                  nat.ptr(cls_out), nat.ptr(reg_out), int(bool(use_graph)), st))
+        return self._frame_outputs(cls_out, reg_out, level_sizes, P)
 
     def tensor(self, name):
         """Debug view of an intermediate activation as NHWC bf16 / fp16 (valid right after an eager forward only if

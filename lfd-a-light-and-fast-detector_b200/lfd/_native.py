@@ -186,12 +186,15 @@ SYMBOLS = {
     'lfd_grad_sqnorm': (_i, [_vp, _i64, _vp, _vp]),
     'lfd_sgd_step': (_i, [_vp, _vp, _vp, _i64, _f, _f, _f, _f, _i, _f, _f, _vp, _vp]),
     'lfd_input_batch': (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, C.POINTER(_f), C.POINTER(_f), _vp]),
+    'lfd_resize_query': (_i, [_i, _i, C.c_double, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i)]),
+    'lfd_resize_frames': (_i, [_vp, _i, _i, _i, _i, _i, C.c_double, _vp, _i, _i, _vp]),
     'lfd_engine_open': (_i, [_vp, C.c_size_t, C.POINTER(_vp)]),
     'lfd_engine_close': (_i, [_vp]),
     'lfd_engine_info': (_i, [_vp, C.POINTER(EngineDesc)]),
     'lfd_engine_op': (_i, [_vp, _i, C.POINTER(Op), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     'lfd_engine_bind': (_i, [_vp, _vp, C.c_size_t, _vp, C.c_size_t, _vp, C.c_size_t, _vp]),
     'lfd_engine_detect': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
+    'lfd_engine_detect_resized': (_i, [_vp, _vp, _i, _i, _i, C.c_double, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
     'lfd_engine_num_launches': (_i, [_vp]),
 }
 
@@ -263,3 +266,12 @@ def stem4_query(N, H, W):
     smem = C.c_int64()
     check(lib().lfd_stem4_query(N, H, W, C.byref(nt), C.byref(smem), C.byref(ho), C.byref(wo)))
     return dict(num_tiles=nt.value, smem_bytes=smem.value, Ho=ho.value, Wo=wo.value)
+
+
+def resize_query(src_h, src_w, scale):
+    """(mode, resized height, resized width) of cv2.resize(frame, (0, 0), fx=scale, fy=scale) on uint8 frames of src_h x src_w, as the
+    library resizes them (lfd_resize_query: the one statement of the rule that lfd_resize_frames and lfd_engine_detect_resized follow).
+    Raises LfdError for a scale that is not finite or not > 0, or an empty result."""
+    dh, dw, mode = C.c_int(), C.c_int(), C.c_int()
+    check(lib().lfd_resize_query(int(src_h), int(src_w), float(scale), C.byref(dh), C.byref(dw), C.byref(mode)))
+    return mode.value, dh.value, dw.value

@@ -44,10 +44,11 @@ class ForwardPostPipeline(object):
     slot is rewritten only after its post-process has finished.  The post-process buffers are single: `consume(results)`
     is called with the post stream current, enqueue device->host copies (or anything else that reads them) there."""
 
-    def __init__(self, model, plan, post, score_thr, iou_thr, frame_format=None):
-        """frame_format: of the device inputs, passed to plan.forward (None: float32 NCHW or uint8 BGR by dtype, 'nv12': NV12 frames)."""
+    def __init__(self, model, plan, post, score_thr, iou_thr, frame_format=None, resize_scale=None):
+        """frame_format: of the device inputs, passed to plan.forward (None: float32 NCHW or uint8 BGR by dtype, 'nv12': NV12 frames);
+        resize_scale: passed to plan.forward as well (the inputs are frames of another size, resized on the forward stream)."""
         self.model, self.plan, self.post = model, plan, post
-        self.frame_format = frame_format
+        self.frame_format, self.resize_scale = frame_format, resize_scale
         self.score_thr, self.iou_thr = float(score_thr), float(iou_thr)
         dev = plan.device
         with torch.cuda.device(dev):
@@ -69,7 +70,8 @@ class ForwardPostPipeline(object):
                 self.fwd_stream.wait_event(wait_for)
             if self.k >= self.n_slots:
                 self.fwd_stream.wait_event(self.post_done[slot])
-            cls, reg = self.plan.forward(x, use_graph=self.model.use_cuda_graph, slot=slot, frame_format=self.frame_format)
+            cls, reg = self.plan.forward(x, use_graph=self.model.use_cuda_graph, slot=slot, frame_format=self.frame_format,
+                                         resize_scale=self.resize_scale)
             self.fwd_done[slot].record(self.fwd_stream)
         with torch.cuda.stream(self.post_stream):
             self.post_stream.wait_event(self.fwd_done[slot])
@@ -84,7 +86,7 @@ class ForwardPostPipeline(object):
 class StreamingDetector(object):
 
     def __init__(self, model, batch, height, width, score_thr, iou_thr, max_out=1024, device=None, depth=3, copy_streams=4,
-                 input_pipeline=None, frame_format='bgr'):
+                 input_pipeline=None, frame_format='bgr', source_size=None, resize_scale=None):
         """input_pipeline: the model's val pipeline, run on the uint8 frames inside the stem kernel -- None: simple_normalize on BGR;
         else BGR2RGB / a final Normalize of the declarative stand-ins (lfd/data_pipeline/augmentation.py), e.g. the TrafficLight
         val_pipeline.  A pipeline the kernels cannot run raises ValueError here: frames are never normalised other than asked.
@@ -92,12 +94,33 @@ class StreamingDetector(object):
         to copy, converted to BGR inside the stem kernel bit for bit as cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12) would, after which
         input_pipeline applies as it does to BGR frames; 'gray' -- uint8 [N,H,W], for a gray model (a 1-channel stem conv).  A gray model
         takes 'gray' or 'nv12', of which it reads the Y plane only (cv2.COLOR_YUV2GRAY_NV12), and raises ValueError for 'bgr'; a BGR model
-        raises ValueError for 'gray'."""
+        raises ValueError for 'gray'.
+        source_size=(h, w): the host frames are h x w (any size, in frame_format) and height x width stays the network's input size (the
+        plan's capacity).  Each batch goes up at source size and is resized on the device, on the forward stream, exactly as
+        cv2.resize(frame, (0, 0), fx=s, fy=s) would (NV12: cv2.resize of the converted frame); the network runs at the resized size, and the
+        detections are in source-frame coordinates: the post-process takes the reference's meta of a resized image, int(w * s) x int(h * s)
+        and resize_scale s.  resize_scale=None takes the largest s whose result fits: min(height / h, width / w); an explicit scale whose
+        result does not fit raises ValueError."""
         from ._engine import image_channels
         if frame_format not in ('bgr', 'nv12', 'gray'):
             raise ValueError("frame_format must be 'bgr' or 'nv12' ('gray' for a gray model), got %r" % (frame_format,))
-        if frame_format == 'nv12' and (height % 2 or width % 2):
-            raise ValueError('NV12 frames have an even height and width, got %dx%d' % (height, width))
+        if source_size is None and resize_scale is not None:
+            raise ValueError('resize_scale needs source_size: the size of the frames it resizes')
+        src_h, src_w = (height, width) if source_size is None else (int(source_size[0]), int(source_size[1]))
+        if frame_format == 'nv12' and (src_h % 2 or src_w % 2):
+            raise ValueError('NV12 frames have an even height and width, got %dx%d' % (src_h, src_w))
+        self.source_size, self.resize_scale = None, None
+        meta, (dh, dw) = (width, height, 1.0), (height, width)
+        if source_size is not None:
+            s = min(height / src_h, width / src_w) if resize_scale is None else float(resize_scale)
+            try:
+                _, dh, dw = nat.resize_query(src_h, src_w, s)
+            except nat.LfdError as e:
+                raise ValueError(str(e))
+            if dh > height or dw > width:
+                raise ValueError('%dx%d frames at resize scale %r are %dx%d, beyond the network size %dx%d' % (src_h, src_w, s, dh, dw, height, width))
+            self.source_size, self.resize_scale = (src_h, src_w), s
+            meta = (int(src_w * s), int(src_h * s), s)       # the reference's resized_width / resized_height / resize_scale
         gray = image_channels(model) == 1
         if gray != (frame_format == 'gray') and frame_format != 'nv12':
             raise ValueError("a %s model takes frame_format '%s' or 'nv12', got %r" % ('gray' if gray else 'BGR', 'gray' if gray else 'bgr', frame_format))
@@ -124,13 +147,16 @@ class StreamingDetector(object):
             model.input_transform = own
         if getattr(model, 'use_cuda_graph', True) and not self.plan.autotuned:
             self.plan.autotune()
-        for i, hw in enumerate(self.plan.level_sizes):
+        # the level geometry of the frames the network runs on: the capacity's, or that of the resized extent below it
+        level_sizes = self.plan.level_sizes if (dh, dw) == (height, width) else self.plan.extent_table(dh, dw)[1]
+        for i, hw in enumerate(level_sizes):
             model._head_indexes_to_feature_map_sizes[i] = hw
-        self.post = model.post_plan(batch, self.plan.level_sizes, dev)   # greedy NMS or Soft-NMS: model._nms_cfg as of now
-        self.post.set_meta([width] * batch, [height] * batch, [1.0] * batch)
+        self.post = model.post_plan(batch, level_sizes, dev)   # greedy NMS or Soft-NMS: model._nms_cfg as of now
+        self.post.set_meta([meta[0]] * batch, [meta[1]] * batch, [meta[2]] * batch)
         nv12 = frame_format == 'nv12'
-        self.pipe = ForwardPostPipeline(model, self.plan, self.post, self.score_thr, self.iou_thr, frame_format='nv12' if nv12 else None)
-        frame_shape = (batch, height * 3 // 2, width) if nv12 else self.plan.u8_shape(height, width)
+        self.pipe = ForwardPostPipeline(model, self.plan, self.post, self.score_thr, self.iou_thr, frame_format='nv12' if nv12 else None,
+                                        resize_scale=self.resize_scale)
+        frame_shape = (batch, src_h * 3 // 2, src_w) if nv12 else self.plan.u8_shape(src_h, src_w)
         self.slots = []
         for _ in range(self.depth):
             self.slots.append(dict(
@@ -144,8 +170,8 @@ class StreamingDetector(object):
         self.d2h_bytes = batch * self.max_out * (5 * 4 + 4) + (batch + 1) * 4
 
     def submit(self, frames_u8):
-        """frames_u8: pinned (or pageable) host uint8 [N,H,W,3] (frame_format 'nv12': [N,3H/2,W]; 'gray': [N,H,W]).  Enqueues copy + compute; returns the
-        slot index."""
+        """frames_u8: pinned (or pageable) host uint8 [N,H,W,3] (frame_format 'nv12': [N,3H/2,W]; 'gray': [N,H,W]); H x W is source_size
+        when given.  Enqueues copy + compute; returns the slot index."""
         s = self.slots[self.step % self.depth]
         if s['busy']:
             s['done'].synchronize()
