@@ -64,7 +64,8 @@ int lfd_device_sm_count(void);
 
 /* ------------------------------------------------------------------------------------------ forward plan */
 enum { LFD_OP_STEM0 = 0, LFD_OP_CONV = 1, LFD_OP_GN_APPLY = 2, LFD_OP_HEAD_FINAL = 3, LFD_OP_STEM4 = 4 };
-enum { LFD_INPUT_F32_NCHW = 0, LFD_INPUT_U8_NHWC = 1, LFD_INPUT_U8_NV12 = 2 };
+enum { LFD_INPUT_F32_NCHW = 0, LFD_INPUT_U8_NHWC = 1, LFD_INPUT_U8_NV12 = 2, LFD_INPUT_U8_YUY2 = 4, LFD_INPUT_U8_UYVY = 5, LFD_INPUT_U8_BGRA = 6,
+       LFD_INPUT_U8_RGBA = 7 };
 /* LFD_INPUT_U8_NV12 (inference only): YUV 4:2:0 video frames, one contiguous uint8 buffer without row padding.  Image n starts at byte
  * n * H * W * 3 / 2 and holds a Y plane of H rows x W bytes, then an interleaved UV plane of H / 2 rows x W bytes (U at even bytes, V at
  * odd bytes): the bytes of a uint8 [N][3H/2][W] tensor.  H and W are even.  A pixel (y, x) is turned into the three bytes (B, G, R) from
@@ -79,8 +80,19 @@ enum { LFD_INPUT_F32_NCHW = 0, LFD_INPUT_U8_NHWC = 1, LFD_INPUT_U8_NV12 = 2 };
  * Y rows in the top-left corner of the H x W Y plane, its h / 2 UV rows in the top-left corner of the H / 2 x W UV plane.
  * lfd_plan_forward, lfd_plan_forward_extent, lfd_plan_profile and lfd_run_op check before anything is enqueued: an odd frame height or
  * width is LFD_ERR_INVALID, an NV12 frame on a plan (an image op) of odd capacity H or W is LFD_ERR_UNSUPPORTED.  lfd_train_plan_run,
- * lfd_train_plan_profile and lfd_run_top refuse NV12 with LFD_ERR_UNSUPPORTED.  Every entry point refuses a format other than these three
- * with LFD_ERR_INVALID.
+ * lfd_train_plan_profile and lfd_run_top refuse NV12 with LFD_ERR_UNSUPPORTED.  Every entry point refuses a format other than these
+ * and the packed formats below (3, negative values, ...) with LFD_ERR_INVALID.
+ * PACKED CAMERA FRAMES (inference only): one contiguous uint8 buffer without row padding, the frame of a smaller extent in the top-left
+ * corner of the capacity layout, as for uint8 BGR.
+ *   LFD_INPUT_U8_YUY2 / LFD_INPUT_U8_UYVY: YUV 4:2:2, uint8 [N][H][W][2] (W even), each pair of pixels 2k, 2k + 1 in 4 bytes: YUY2
+ *     Y0 U Y1 V (USB / UVC webcams, V4L2), UYVY U Y0 V Y1 (HDMI / SDI capture).  Pixel x takes its Y byte and the (U, V) of its pair
+ *     x & ~1, through the NV12 formula above: bit for bit cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_YUY2 / _UYVY).
+ *   LFD_INPUT_U8_BGRA / LFD_INPUT_U8_RGBA: 4-byte pixels, uint8 [N][H][W][4]; the fourth (alpha) byte is never read.  The pixel is the
+ *     BGR bytes (B, G, R) = (b0, b1, b2) for BGRA and (b2, b1, b0) for RGBA: cv2.cvtColor(frame, cv2.COLOR_BGRA2BGR / _RGBA2BGR).
+ * From there, as for NV12, every op and plan gives exactly what it gives on the converted uint8 BGR frame under the same input transform.
+ * Checked before anything is enqueued: an odd 4:2:2 frame width is LFD_ERR_INVALID, a 4:2:2 frame on an image op of odd capacity W is
+ * LFD_ERR_UNSUPPORTED, BGRA / RGBA on a gray image op (Cin = 1) is LFD_ERR_UNSUPPORTED; lfd_train_plan_run, lfd_train_plan_profile and
+ * lfd_run_top refuse all four with LFD_ERR_UNSUPPORTED.  A gray op reads the Y bytes of a 4:2:2 frame (cv2.COLOR_YUV2GRAY_YUY2 / _UYVY).
  * GRAY (1-channel) PLANS: an image op (STEM0 / STEM4; lfd_top STEM0 / WGRAD_STEM) with Cin = 1 reads one value per pixel, and the same
  * format numbers then mean: LFD_INPUT_F32_NCHW float[N][1][H][W]; LFD_INPUT_U8_NHWC uint8[N][H][W] (1 byte per pixel); LFD_INPUT_U8_NV12
  * the usual NV12 buffer above, of which only the Y plane is read (the UV bytes are never touched): Y is the gray byte, as

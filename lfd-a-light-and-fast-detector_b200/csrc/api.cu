@@ -322,11 +322,13 @@ extern "C" int lfd_stem4_query(int N, int H, int W, int* num_tiles, int64_t* sme
 // channel, see lfd_op): all seven fields zero = simple_normalize; anything else has to be a complete transform.  One place for lfd_op
 // and lfd_top, and for both image kinds: BGR (cin 3) and gray (cin 1), whose one channel is (byte - mean[0]) * scale[0] -- it has no
 // channel swap and takes three equal constants, so every byte position of the resolved transform holds channel 0's.
-static int input_transform_of(int cin, int32_t swap, const float* mean, const float* scale, InputTransform* out) {
+// rgba: the transform of the same op on LFD_INPUT_U8_RGBA frames, whose bytes 0..2 are R, G, B: the byte positions of the BGR transform
+// mirrored, which is the BGR transform with the channel swap toggled.  The kernels then read RGBA as BGRA.
+static int input_transform_of(int cin, int32_t swap, const float* mean, const float* scale, InputTransform* out, bool rgba = false) {
     bool zero = swap == 0;
     for (int c = 0; c < 3; ++c) zero = zero && mean[c] == 0.f && scale[c] == 0.f;
     if (zero) {
-        out->swap = 0;
+        out->swap = rgba;
         for (int c = 0; c < 3; ++c) { out->mean[c] = 127.5f; out->scale[c] = 1.0f / 127.5f; }
         return LFD_OK;
     }
@@ -339,8 +341,9 @@ static int input_transform_of(int cin, int32_t swap, const float* mean, const fl
         if (!std::isfinite(mean[c]) || !std::isfinite(scale[c]) || scale[c] == 0.f)
             return fail(LFD_ERR_INVALID, "input transform: channel %d has mean %g, scale %g (set all of in_swap_rb / in_mean / in_scale with finite means and "
                         "finite non-zero scales, or none of them)", c, (double)mean[c], (double)scale[c]);
-    out->swap = swap;
-    for (int m = 0; m < 3; ++m) { out->mean[m] = mean[swap ? 2 - m : m]; out->scale[m] = scale[swap ? 2 - m : m]; }   // by byte position
+    const int sw = swap ^ (int)rgba;
+    out->swap = sw;
+    for (int m = 0; m < 3; ++m) { out->mean[m] = mean[sw ? 2 - m : m]; out->scale[m] = scale[sw ? 2 - m : m]; }   // by byte position
     return LFD_OK;
 }
 
@@ -423,6 +426,9 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
     const lfd_op& o = po.op;
     unsigned long long* tl = g_timeline ? g_timeline + 2 * index : nullptr;
     const int* ext_row = ext ? &ext->H : nullptr;
+    // RGBA frames are read as BGRA, under the op's transform resolved for their byte order (plan_op validated the op's fields)
+    InputTransform xf = po.xf;
+    if (input_format == LFD_INPUT_U8_RGBA) input_transform_of(o.Cin, o.in_swap_rb, o.in_mean, o.in_scale, &xf, true);
     if (ext && conv_impl == LFD_CONV_SIMT) return fail(LFD_ERR_UNSUPPORTED, "the SIMT cross-check kernels run full-size frames only");
     switch (o.kind) {
         case LFD_OP_STEM0: {
@@ -430,14 +436,14 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
             if (conv_impl == LFD_CONV_SIMT) {
                 if (o.tail_cout) return fail(LFD_ERR_UNSUPPORTED, "the SIMT cross-check kernels do not implement fused tails");
                 Stem0Params p;
-                p.img = image_in(input, input_format, o.Cin, o.H, o.W, po.xf);
+                p.img = image_in(input, input_format, o.Cin, o.H, o.W, xf);
                 p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off);
                 p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift;
                 p.N = o.N; p.Ho = o.Ho; p.Wo = o.Wo; p.Cout = o.Cout; p.relu = o.relu; p.f16 = o.dtype;
                 CUDA_TRY(stem0_launch(p, st));
             } else {
                 UmmaConvParams p = po.cp;
-                p.img = image_in(input, input_format, o.Cin, o.H, o.W, po.xf); p.in = nullptr;
+                p.img = image_in(input, input_format, o.Cin, o.H, o.W, xf); p.in = nullptr;
                 p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off); p.res = nullptr;
                 p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift; p.stats = nullptr;
                 p.relu = o.relu; p.gn_groups = 0; p.trace = g_trace; p.tl = tl; p.f16 = o.dtype;
@@ -452,9 +458,9 @@ static int launch_op(const PlannedOp& po, size_t index, const void* input, int i
             if (!input) return fail(LFD_ERR_INVALID, "stem4 needs the external input pointer");
             if (conv_impl == LFD_CONV_SIMT) return fail(LFD_ERR_UNSUPPORTED, "the SIMT cross-check kernels do not implement the fused stem (plan its four convs)");
             UmmaConvParams p = po.cp;
-            p.img = image_in(input, input_format, o.Cin, o.H, o.W, po.xf); p.in = nullptr;
+            p.img = image_in(input, input_format, o.Cin, o.H, o.W, xf); p.in = nullptr;
             // the word loader: rows of whole aligned words (BGR: 3 words per 4 pixels; gray: 1 word per 4 pixels; NV12: a Y word and a UV
-            // word, its image pitch H * W * 3 / 2 then being a multiple of 4 as well, since H is even)
+            // word, its image pitch H * W * 3 / 2 then being a multiple of 4 as well, since H is even; 4:2:2: 2 words; 4-byte pixels: 4)
             p.in_words = input_format != LFD_INPUT_F32_NCHW && o.W % 4 == 0 && (reinterpret_cast<uintptr_t>(input) & 3) == 0;
             p.out = reinterpret_cast<__nv_bfloat16*>(ws + o.out_off); p.res = nullptr; p.stats = nullptr;
             p.w = reinterpret_cast<const __nv_bfloat16*>(o.weight); p.shift = o.shift; p.relu = o.relu;
@@ -565,15 +571,27 @@ extern "C" int lfd_plan_destroy(lfd_plan* plan) {
 
 extern "C" int lfd_plan_num_launches(const lfd_plan* plan) { return plan ? (int)plan->ops.size() : 0; }
 
-// The input format of an inference entry point, before anything is enqueued: 0, 1 or 2.  An NV12 frame (h x w) has an even height and
-// width, on an image op whose capacity (H x W: the UV plane's pitch and twice its rows) is even too.
+static bool is_yuv422(int fmt) { return fmt == LFD_INPUT_U8_YUY2 || fmt == LFD_INPUT_U8_UYVY; }
+static bool is_px4(int fmt) { return fmt == LFD_INPUT_U8_BGRA || fmt == LFD_INPUT_U8_RGBA; }
+static bool is_packed(int fmt) { return is_yuv422(fmt) || is_px4(fmt); }
+
+// The input format of an inference entry point, before anything is enqueued: 0, 1, 2 or a packed format (4..7).  An NV12 frame (h x w)
+// has an even height and width, on an image op whose capacity (H x W: the UV plane's pitch and twice its rows) is even too; a 4:2:2 frame
+// an even width, on an even capacity width; 4-byte pixels are colour only.
 static int check_input_format(const char* fn, int fmt, const lfd_op* img, int h, int w) {
-    if (fmt != LFD_INPUT_F32_NCHW && fmt != LFD_INPUT_U8_NHWC && fmt != LFD_INPUT_U8_NV12)
-        return fail(LFD_ERR_INVALID, "%s: input format %d (0 = float32 NCHW, 1 = uint8 NHWC, 2 = uint8 NV12)", fn, fmt);
+    if (fmt != LFD_INPUT_F32_NCHW && fmt != LFD_INPUT_U8_NHWC && fmt != LFD_INPUT_U8_NV12 && !is_packed(fmt))
+        return fail(LFD_ERR_INVALID, "%s: input format %d (0 = float32 NCHW, 1 = uint8 NHWC, 2 = uint8 NV12, 4 = YUY2, 5 = UYVY, 6 = BGRA, "
+                    "7 = RGBA)", fn, fmt);
     if (fmt == LFD_INPUT_U8_NV12 && img) {
         if ((img->H | img->W) & 1) return fail(LFD_ERR_UNSUPPORTED, "%s: NV12 frames need an even capacity, the plan's is %dx%d", fn, img->H, img->W);
         if ((h | w) & 1) return fail(LFD_ERR_INVALID, "%s: an NV12 frame has an even height and width, got %dx%d", fn, h, w);
     }
+    if (is_yuv422(fmt) && img) {
+        if (img->W & 1) return fail(LFD_ERR_UNSUPPORTED, "%s: 4:2:2 frames need an even capacity width, the plan's is %d", fn, img->W);
+        if (w & 1) return fail(LFD_ERR_INVALID, "%s: a 4:2:2 frame has an even width, got %d", fn, w);
+    }
+    if (is_px4(fmt) && img && img->Cin != 3)
+        return fail(LFD_ERR_UNSUPPORTED, "%s: BGRA / RGBA frames are colour input, the image op reads %d channel(s)", fn, img->Cin);
     return LFD_OK;
 }
 
@@ -586,6 +604,7 @@ static const lfd_op* image_op(const lfd_plan* pl) {
 // Training reads float32 NCHW or uint8 NHWC only
 static int check_train_format(const char* fn, int fmt) {
     if (fmt == LFD_INPUT_U8_NV12) return fail(LFD_ERR_UNSUPPORTED, "%s: NV12 input is for inference plans only", fn);
+    if (is_packed(fmt)) return fail(LFD_ERR_UNSUPPORTED, "%s: 4:2:2 and 4-byte pixel input is for inference plans only", fn);
     if (fmt != LFD_INPUT_F32_NCHW && fmt != LFD_INPUT_U8_NHWC)
         return fail(LFD_ERR_INVALID, "%s: input format %d (0 = float32 NCHW, 1 = uint8 NHWC)", fn, fmt);
     return LFD_OK;
@@ -1334,21 +1353,23 @@ extern "C" int lfd_resize_query(int src_h, int src_w, double scale, int* dh, int
 
 // One resize launch, checked: the geometry every frame of the batch shares and where the frames lie
 struct ResizeCall {
-    lfd_input_desc d;
+    lfd_input_desc d;    // the plane the taps read: an NV12 frame's Y plane, the frame otherwise (d.channels: its bytes per pixel)
     size_t src_stride;   // bytes from one source frame to the next
-    int nv12_bgr;        // NV12 frames to BGR (d: the Y plane); an NV12 frame on a gray model is its Y plane, a gray frame
+    int fmt, channels;   // the frame format and the output channels (resize_frames_launch)
 };
 
 // Every argument of lfd_resize_frames, before anything is enqueued
 static int check_resize(const char* fn, const void* src, int fmt, int channels, int n, int h, int w, double s, const void* dst, int H, int W,
                         ResizeCall* out) {
     if (!src || !dst) return fail(LFD_ERR_INVALID, "%s: null argument", fn);
-    if (fmt == LFD_INPUT_F32_NCHW) return fail(LFD_ERR_UNSUPPORTED, "%s: float32 frames are not resized (uint8 BGR, gray or NV12 frames are)", fn);
-    if (fmt != LFD_INPUT_U8_NHWC && fmt != LFD_INPUT_U8_NV12)
-        return fail(LFD_ERR_INVALID, "%s: input format %d (1 = uint8 NHWC, 2 = uint8 NV12)", fn, fmt);
+    if (fmt == LFD_INPUT_F32_NCHW) return fail(LFD_ERR_UNSUPPORTED, "%s: float32 frames are not resized (uint8 BGR, gray, NV12 or packed frames are)", fn);
+    if (fmt != LFD_INPUT_U8_NHWC && fmt != LFD_INPUT_U8_NV12 && !is_packed(fmt))
+        return fail(LFD_ERR_INVALID, "%s: input format %d (1 = uint8 NHWC, 2 = uint8 NV12, 4 = YUY2, 5 = UYVY, 6 = BGRA, 7 = RGBA)", fn, fmt);
     if (channels != 1 && channels != 3) return fail(LFD_ERR_INVALID, "%s: channels = %d (3 = BGR, 1 = gray)", fn, channels);
     if (n < 1 || H < 1 || W < 1) return fail(LFD_ERR_INVALID, "%s: bad arguments (n=%d H=%d W=%d)", fn, n, H, W);
     if (fmt == LFD_INPUT_U8_NV12 && ((h | w) & 1)) return fail(LFD_ERR_INVALID, "%s: an NV12 frame has an even height and width, got %dx%d", fn, h, w);
+    if (is_yuv422(fmt) && (w & 1)) return fail(LFD_ERR_INVALID, "%s: a 4:2:2 frame has an even width, got %d", fn, w);
+    if (is_px4(fmt) && channels != 3) return fail(LFD_ERR_UNSUPPORTED, "%s: BGRA / RGBA frames are colour input, not gray", fn);
     int dh = 0, dw = 0, mode = 0;
     int rc = resize_rule(fn, h, w, s, &dh, &dw, &mode);
     if (rc) return rc;
@@ -1357,7 +1378,7 @@ static int check_resize(const char* fn, const void* src, int fmt, int channels, 
     if (dw > 6144) return fail(LFD_ERR_UNSUPPORTED, "%s: resized width %d > 6144 (the column table lives in 48 KB of shared memory)", fn, dw);
     if (n > 65535) return fail(LFD_ERR_UNSUPPORTED, "%s: n=%d > 65535", fn, n);
     const bool nv12 = fmt == LFD_INPUT_U8_NV12;
-    const int c = nv12 ? 1 : channels;   // bytes per pixel of the plane the taps read
+    const int c = nv12 ? 1 : is_yuv422(fmt) ? 2 : is_px4(fmt) ? 4 : channels;   // bytes per pixel of the plane the taps read
     lfd_input_desc d{};
     d.inv_scale = 1.0 / s;
     d.pitch = w * c;
@@ -1369,7 +1390,8 @@ static int check_resize(const char* fn, const void* src, int fmt, int channels, 
     d.mode = mode;
     out->d = d;
     out->src_stride = nv12 ? (size_t)h * w * 3 / 2 : (size_t)h * w * c;
-    out->nv12_bgr = nv12 && channels == 3;
+    out->fmt = fmt;
+    out->channels = channels;
     return LFD_OK;
 }
 
@@ -1379,7 +1401,7 @@ extern "C" int lfd_resize_frames(const void* src, int src_format, int channels, 
     int rc = check_resize("lfd_resize_frames", src, src_format, channels, n, src_h, src_w, scale, dst, H, W, &rs);
     if (rc) return rc;
     if (sm_count() <= 0) return fail(LFD_ERR_CUDA, "lfd_resize_frames: no CUDA device (there is no CPU fallback)");
-    CUDA_TRY(resize_frames_launch(rs.d, static_cast<const uint8_t*>(src), rs.src_stride, n, rs.nv12_bgr, dst, H, W, st_of(stream)));
+    CUDA_TRY(resize_frames_launch(rs.d, static_cast<const uint8_t*>(src), rs.src_stride, n, rs.fmt, rs.channels, dst, H, W, st_of(stream)));
     return LFD_OK;
 }
 
@@ -1840,7 +1862,7 @@ extern "C" int lfd_engine_detect_resized(lfd_engine* e, const void* input, int i
     ResizeCall rs;
     int rc = check_resize(fn, input, input_format, e->ops[0].Cin, e->N, src_h, src_w, scale, frames, e->H, e->W, &rs);
     if (rc) return rc;
-    CUDA_TRY(resize_frames_launch(rs.d, static_cast<const uint8_t*>(input), rs.src_stride, e->N, rs.nv12_bgr, frames, e->H, e->W, st_of(stream)));
+    CUDA_TRY(resize_frames_launch(rs.d, static_cast<const uint8_t*>(input), rs.src_stride, e->N, rs.fmt, rs.channels, frames, e->H, e->W, st_of(stream)));
     // the reference's meta of a resized image: resized_width = int(w * s), resized_height = int(h * s) in double, resize_scale = s
     return engine_detect(e, fn, frames, LFD_INPUT_U8_NHWC, rs.d.dh, rs.d.dw, (int)((double)src_w * scale), (int)((double)src_h * scale), (float)scale,
                          dets, labels, count, cls_out, reg_out, use_graph, stream);

@@ -665,21 +665,28 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
             // Raw image patch -> normalised bf16 [row][pixel][b g r 0] in the ring stage (see kStem* above).  Every thread owns
             // up to 5 patch pixels; the raw values of the NEXT tile are fetched into registers right after the current patch
             // has been written, so the loads fly while the thread waits for the next free stage.  A gray image (p.img.ch == 1) has
-            // one value per pixel (fp32 plane, uint8 byte, NV12's Y byte -- its UV plane is never read), written as (v, 0, 0, 0):
-            // the body is specialised for it at compile time, so the BGR loaders are exactly what they are without it.
+            // one value per pixel (fp32 plane, uint8 byte, NV12's Y byte -- its UV plane is never read -- or a 4:2:2 pixel's Y byte),
+            // written as (v, 0, 0, 0): the body is specialised for it at compile time, so the BGR loaders are exactly what they are
+            // without it.  The packed formats (4:2:2, 4-byte pixels) have fetch branches of their own, taken once per tile.
             auto stem_producer = [&](auto gray_c) LFD_LAMBDA_INLINE {
                 constexpr bool gray = decltype(gray_c)::value;
-                const bool u8 = p.img.format != 0;        // uint8 BGR (1) or NV12 (2): bytes, normalised by p.img.xf
-                const bool nv12 = p.img.format == 2;
+                const int fmt = p.img.format;
+                const bool u8 = fmt != LFD_INPUT_F32_NCHW;   // bytes, normalised by p.img.xf
+                const bool nv12 = fmt == LFD_INPUT_U8_NV12;
+                const bool yuv422 = fmt == LFD_INPUT_U8_YUY2 || fmt == LFD_INPUT_U8_UYVY;
+                const bool px4 = fmt == LFD_INPUT_U8_BGRA || fmt == LFD_INPUT_U8_RGBA;   // RGBA: api.cu permuted p.img.xf
                 const int plane = p.H * p.W;
-                int rel[kStemPerThread];          // source offset of pixel j relative to the patch origin (bytes for BGR, elements for gray / fp32 / NV12's Y)
+                // source offset of pixel j relative to the patch origin: bytes for BGR, 4:2:2 and 4-byte pixels, elements for gray / fp32 /
+                // NV12's Y
+                const int bpp = fmt == LFD_INPUT_U8_NHWC && !gray ? 3 : yuv422 ? 2 : px4 ? 4 : 1;
+                int rel[kStemPerThread];
                 int prc[kStemPerThread];          // (row << 8) | col
 #pragma unroll
                 for (int j = 0; j < kStemPerThread; ++j) {
                     const int q = min(ptid + j * kProdThreads, kStemPix - 1);
                     const int r = q / kStemCols, c = q - r * kStemCols;
                     prc[j] = (r << 8) | c;
-                    rel[j] = p.img.format == 1 && !gray ? (r * p.W + c) * 3 : r * p.W + c;
+                    rel[j] = (r * p.W + c) * bpp;
                 }
                 const bool last_ok = ptid + (kStemPerThread - 1) * kProdThreads < kStemPix;   // this thread owns a pixel in the last round
                 uint32_t raw[kStemPerThread][gray ? 1 : 3];
@@ -707,24 +714,48 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
                             raw[j][0] = __ldg(src);
                             if constexpr (!gray) { raw[j][1] = __ldg(uv); raw[j][2] = __ldg(uv + 1); }
                         }
-                    } else if (u8) {
-                        const int bpp = gray ? 1 : 3;
-                        const uint8_t* img = reinterpret_cast<const uint8_t*>(p.img.data) + (size_t)n * plane * bpp;
-                        const uint8_t* org = img + ((ptrdiff_t)iy0 * p.W + ix0) * bpp;
+                    } else if (yuv422) {
+                        // raw = (Y, U, V): the Y byte at byte l of the pixel's 2 (l = 1 for UYVY), U and V at bytes 1 - l and 3 - l of its
+                        // pair x & ~1
+                        const int l = fmt == LFD_INPUT_U8_UYVY;
+                        const uint8_t* img = reinterpret_cast<const uint8_t*>(p.img.data) + (size_t)n * plane * 2;
+                        const uint8_t* org = img + ((ptrdiff_t)iy0 * p.W + ix0) * 2;
 #pragma unroll
                         for (int j = 0; j < kStemPerThread; ++j) {
                             if (j == kStemPerThread - 1 && !last_ok) break;
+                            const int y = iy0 + (prc[j] >> 8), x = ix0 + (prc[j] & 255);
                             const uint8_t* src = org + rel[j];
-                            bool ok = true;
-                            if (!interior) {
-                                const int y = iy0 + (prc[j] >> 8), x = ix0 + (prc[j] & 255);
-                                ok = (unsigned)y < (unsigned)lg.H && (unsigned)x < (unsigned)lg.W;
-                                if (!ok) src = img;
-                            }
+                            const uint8_t* pair = src - 2 * (x & 1);
+                            const bool ok = interior || ((unsigned)y < (unsigned)lg.H && (unsigned)x < (unsigned)lg.W);
+                            if (!ok) src = pair = img;
                             okmask |= (ok ? 1u : 0u) << j;
-                            raw[j][0] = __ldg(src);
-                            if constexpr (!gray) { raw[j][1] = __ldg(src + 1); raw[j][2] = __ldg(src + 2); }
+                            raw[j][0] = __ldg(src + l);
+                            if constexpr (!gray) { raw[j][1] = __ldg(pair + 1 - l); raw[j][2] = __ldg(pair + 3 - l); }
                         }
+                    } else if (u8) {
+                        // uint8 BGR / gray (BPP 3 / 1) or 4-byte pixels (BPP 4: bytes 0..2, the alpha byte is never read)
+                        auto fetch_bytes = [&](auto bpp_c) LFD_LAMBDA_INLINE {
+                            constexpr int BPP = decltype(bpp_c)::value;
+                            const uint8_t* img = reinterpret_cast<const uint8_t*>(p.img.data) + (size_t)n * plane * BPP;
+                            const uint8_t* org = img + ((ptrdiff_t)iy0 * p.W + ix0) * BPP;
+#pragma unroll
+                            for (int j = 0; j < kStemPerThread; ++j) {
+                                if (j == kStemPerThread - 1 && !last_ok) break;
+                                const uint8_t* src = org + rel[j];
+                                bool ok = true;
+                                if (!interior) {
+                                    const int y = iy0 + (prc[j] >> 8), x = ix0 + (prc[j] & 255);
+                                    ok = (unsigned)y < (unsigned)lg.H && (unsigned)x < (unsigned)lg.W;
+                                    if (!ok) src = img;
+                                }
+                                okmask |= (ok ? 1u : 0u) << j;
+                                raw[j][0] = __ldg(src);
+                                if constexpr (!gray) { raw[j][1] = __ldg(src + 1); raw[j][2] = __ldg(src + 2); }
+                            }
+                        };
+                        if constexpr (gray) fetch_bytes(std::integral_constant<int, 1>());
+                        else if (px4) fetch_bytes(std::integral_constant<int, 4>());
+                        else fetch_bytes(std::integral_constant<int, 3>());
                     } else {
                         const float* img = reinterpret_cast<const float*>(p.img.data) + (size_t)n * plane * (gray ? 1 : 3);
                         const float* org = img + (ptrdiff_t)iy0 * p.W + ix0;
@@ -758,11 +789,11 @@ LFD_DEVINL void conv_umma_body(const UmmaConvParams& p) {
                         if (j == kStemPerThread - 1 && !last_ok) break;
                         uint32_t lo, hi;
                         if constexpr (gray) {
-                            float v = u8 ? p.img.xf.apply(0, raw[j][0]) : __uint_as_float(raw[j][0]);     // NV12: the Y byte as it is
+                            float v = u8 ? p.img.xf.apply(0, raw[j][0]) : __uint_as_float(raw[j][0]);     // NV12 / 4:2:2: the Y byte as it is
                             if (!((okmask >> j) & 1u)) v = 0.f;                                      // conv zero padding
                             lo = pack2<F16>(v, 0.f); hi = pack2<F16>(0.f, 0.f);                       // rounding point R0
                         } else {
-                            if (nv12) nv12_to_bgr(raw[j][0], raw[j][1], raw[j][2], raw[j]);   // (Y, U, V) -> the bytes (B, G, R)
+                            if (nv12 || yuv422) nv12_to_bgr(raw[j][0], raw[j][1], raw[j][2], raw[j]);   // (Y, U, V) -> the bytes (B, G, R)
                             float f[3];
 #pragma unroll
                             for (int k = 0; k < 3; ++k) {
@@ -1227,7 +1258,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                     // producer's 56 registers).
 #pragma unroll 1
                     for (int j0 = 0; j0 < kS4GroupsPerThread; j0 += kS4GroupBatch) {
-                        uint32_t wd[kS4GroupBatch][CH];
+                        uint32_t wd[kS4GroupBatch][kImageWords<CH, FMT>];
                         bool ok[kS4GroupBatch];
 #pragma unroll
                         for (int j = 0; j < kS4GroupBatch; ++j) {
@@ -1262,7 +1293,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) stem4_kernel(const __grid_con
                         }
                     }
                 } else {
-                    // per-pixel loader: fp32 NCHW, or uint8 (BGR / gray / NV12) rows that are not whole aligned words
+                    // per-pixel loader: fp32 NCHW, or uint8 (BGR / gray / NV12 / 4:2:2 / 4-byte) rows that are not whole aligned words
 #pragma unroll 1
                     for (int j0 = 0; j0 < kS4PerThread; j0 += kS4Batch) {
                         uint32_t raw[kS4Batch][CH];

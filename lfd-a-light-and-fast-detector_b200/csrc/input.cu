@@ -9,7 +9,8 @@
 //
 // lfd_resize_frames (resize_frames_kernel) runs the same per-tap code on N whole frames of one size and scale: one geometry for the
 // batch, passed by value, and only the resized h x w extent of each destination image is written.  An NV12 source is converted to
-// B, G, R at every tap it reads (nv12_to_bgr), then resized, as cv2.resize of cv2.cvtColor(COLOR_YUV2BGR_NV12) computes it.
+// B, G, R at every tap it reads (nv12_to_bgr), then resized, as cv2.resize of cv2.cvtColor(COLOR_YUV2BGR_NV12) computes it; a 4:2:2
+// (YUY2 / UYVY) or 4-byte (BGRA / RGBA) source the same way (packed_pixel).
 #include "../../include/lfd_b200.h"
 #include "kernels.cuh"
 
@@ -132,6 +133,35 @@ __device__ __forceinline__ uint32_t nv12_pixel(const lfd_input_desc& d, const Nv
     for (int k = 0; k < 3; ++k)
         packed |= (uint32_t)resample(d, ri, col, x0, x1, [&](const uint8_t* r, int x) { return nv12_tap(ri, r, x, k); }) << (8 * k);
     return packed;
+}
+
+// one output pixel of a 4:2:2 (SRC = LFD_INPUT_U8_YUY2) or 4-byte (SRC = LFD_INPUT_U8_BGRA) source: B, G, R in bits 0..23, each tap
+// converted before the resize arithmetic of pixel(); GRAY: the Y byte of a 4:2:2 source.  order: the Y byte of a 4:2:2 pair (0 YUY2
+// Y0 U Y1 V, 1 UYVY U Y0 V Y1), or 1 for RGBA, whose B is byte 2.
+template <int SRC, bool GRAY>
+__device__ __forceinline__ uint32_t packed_pixel(const lfd_input_desc& d, const RowInfo& ri, int2 col, int order) {
+    if (ri.kind != 0 || col.x < 0 || d.win_w <= 0) return 0u;
+    const int wmax = d.win_w - 1;
+    const int x0 = min(max(col.x, 0), wmax);
+    const int x1 = min(max(col.x + 1, 0), wmax);
+    if constexpr (GRAY) {
+        return resample(d, ri, col, x0, x1, [&](const uint8_t* r, int x) { return (int)r[2 * x + order]; });
+    } else {
+        uint32_t packed = 0u;
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+            packed |= (uint32_t)resample(d, ri, col, x0, x1, [&](const uint8_t* r, int x) {
+                if constexpr (SRC == LFD_INPUT_U8_YUY2) {
+                    const uint8_t* pair = r + 4 * (x >> 1);
+                    uint32_t bgr[3];
+                    nv12_to_bgr(r[2 * x + order], pair[1 - order], pair[3 - order], bgr);
+                    return (int)bgr[k];
+                } else {
+                    return (int)r[4 * x + (order ? 2 - k : k)];
+                }
+            }) << (8 * k);
+        return packed;
+    }
 }
 
 // one output pixel: channel k of the source order in bits 8k..8k+7 (a gray source replicated)
@@ -262,11 +292,13 @@ struct ResizeArgs {
     size_t src_stride;
     uint8_t* dst;
     int H, W;
+    int order;   // packed_pixel's
 };
 
 // One CTA per (frame, band of kBandRows resized rows), as input_batch_kernel; rows and columns beyond dh x dw are not written.
-// GRAY: a gray source or an NV12 frame's Y plane (d.channels = 1); NV12: 3-channel output from NV12 taps.
-template <bool GRAY, bool NV12>
+// SRC = LFD_INPUT_U8_NHWC: GRAY a gray source or an NV12 frame's Y plane (d.channels = 1), else a BGR source; LFD_INPUT_U8_NV12:
+// 3-channel output from NV12 taps; LFD_INPUT_U8_YUY2 / _BGRA: packed_pixel.
+template <bool GRAY, int SRC>
 __global__ void __launch_bounds__(kThreads) resize_frames_kernel(const __grid_constant__ ResizeArgs a) {
     extern __shared__ int2 cols[];   // [dw]
     const lfd_input_desc& d = a.d;
@@ -280,13 +312,14 @@ __global__ void __launch_bounds__(kThreads) resize_frames_kernel(const __grid_co
     const int rows = min(kBandRows, d.out_h - y_begin);
     for (int t = threadIdx.x; t < rows * groups; t += kThreads) {
         const int y = y_begin + t / groups, x = (t % groups) * 4;
-        using RI = std::conditional_t<NV12, Nv12RowInfo, RowInfo>;
+        using RI = std::conditional_t<SRC == LFD_INPUT_U8_NV12, Nv12RowInfo, RowInfo>;
         const RI ri = row_info<RI>(d, win, y);
         uint32_t v[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             if (x + j >= dw) v[j] = 0u;
-            else if constexpr (NV12) v[j] = nv12_pixel(d, ri, cols[x + j]);
+            else if constexpr (SRC == LFD_INPUT_U8_NV12) v[j] = nv12_pixel(d, ri, cols[x + j]);
+            else if constexpr (SRC == LFD_INPUT_U8_YUY2 || SRC == LFD_INPUT_U8_BGRA) v[j] = packed_pixel<SRC, GRAY>(d, ri, cols[x + j], a.order);
             else v[j] = GRAY ? gray_pixel(d, ri, cols[x + j]) : pixel(d, ri, cols[x + j]);
         }
         const int n = min(4, dw - x);
@@ -298,14 +331,18 @@ __global__ void __launch_bounds__(kThreads) resize_frames_kernel(const __grid_co
 
 }  // namespace
 
-cudaError_t resize_frames_launch(const lfd_input_desc& d, const uint8_t* src, size_t src_stride, int n, int nv12_bgr, uint8_t* dst, int H,
-                                 int W, cudaStream_t st) {
-    const ResizeArgs a{d, src, src_stride, dst, H, W};
+cudaError_t resize_frames_launch(const lfd_input_desc& d, const uint8_t* src, size_t src_stride, int n, int fmt, int channels, uint8_t* dst,
+                                 int H, int W, cudaStream_t st) {
+    const bool yuv422 = fmt == LFD_INPUT_U8_YUY2 || fmt == LFD_INPUT_U8_UYVY, px4 = fmt == LFD_INPUT_U8_BGRA || fmt == LFD_INPUT_U8_RGBA;
+    const ResizeArgs a{d, src, src_stride, dst, H, W, fmt == LFD_INPUT_U8_UYVY || fmt == LFD_INPUT_U8_RGBA};
     const dim3 grid((d.out_h + kBandRows - 1) / kBandRows, n);
     const size_t smem = (size_t)d.out_w * sizeof(int2);
-    if (nv12_bgr) resize_frames_kernel<false, true><<<grid, kThreads, smem, st>>>(a);
-    else if (d.channels == 1) resize_frames_kernel<true, false><<<grid, kThreads, smem, st>>>(a);
-    else resize_frames_kernel<false, false><<<grid, kThreads, smem, st>>>(a);
+    if (fmt == LFD_INPUT_U8_NV12 && channels == 3) resize_frames_kernel<false, LFD_INPUT_U8_NV12><<<grid, kThreads, smem, st>>>(a);
+    else if (yuv422 && channels == 3) resize_frames_kernel<false, LFD_INPUT_U8_YUY2><<<grid, kThreads, smem, st>>>(a);
+    else if (yuv422) resize_frames_kernel<true, LFD_INPUT_U8_YUY2><<<grid, kThreads, smem, st>>>(a);
+    else if (px4) resize_frames_kernel<false, LFD_INPUT_U8_BGRA><<<grid, kThreads, smem, st>>>(a);
+    else if (d.channels == 1) resize_frames_kernel<true, LFD_INPUT_U8_NHWC><<<grid, kThreads, smem, st>>>(a);
+    else resize_frames_kernel<false, LFD_INPUT_U8_NHWC><<<grid, kThreads, smem, st>>>(a);
     return cudaGetLastError();
 }
 

@@ -167,9 +167,11 @@ cudaError_t box_loss_launch(int kind, const float* pred, const float* target, in
 // input.cu: descs = device lfd_input_desc[n] (include/lfd_b200.h, lfd_input_batch)
 cudaError_t input_batch_launch(const void* descs, int n, const uint8_t* src, void* out, int out_mode, int swap_rb, int H, int W,
                                const float* mean, const float* scale, cudaStream_t st);
-// input.cu: lfd_resize_frames -- n frames of one geometry d (host, passed by value), frame i at src + i * src_stride; nv12_bgr: the frames
-// are NV12 and the output BGR (d describes the Y plane, channels 1); else d.channels 1 = gray -> gray, 3 = BGR -> BGR
-cudaError_t resize_frames_launch(const lfd_input_desc& d, const uint8_t* src, size_t src_stride, int n, int nv12_bgr, uint8_t* dst, int H,
-                                 int W, cudaStream_t st);
+// input.cu: lfd_resize_frames -- n frames of one geometry d (host, passed by value), frame i at src + i * src_stride, in the frame format
+// fmt (LFD_INPUT_U8_*; d describes the plane the taps read, d.channels its bytes per pixel), to `channels` (3 = BGR, 1 = gray) output
+// channels: uint8 BGR / gray -> itself, NV12 -> BGR (or its Y plane, d then being that plane with channels 1 -> gray), 4:2:2 -> BGR or
+// its Y bytes, BGRA / RGBA -> BGR
+cudaError_t resize_frames_launch(const lfd_input_desc& d, const uint8_t* src, size_t src_stride, int n, int fmt, int channels, uint8_t* dst,
+                                 int H, int W, cudaStream_t st);
 
 }  // namespace lfd

@@ -739,7 +739,7 @@ __global__ void __launch_bounds__(256) wgrad_stem_kernel(WgradGeom g, const __gr
         const int sx = seg % segs_x, oy = (seg / segs_x) % g.Ho, n = seg / (segs_x * g.Ho);
         const int ox0 = sx * kWsSeg, ix0 = 2 * ox0 - 1, iy0 = 2 * oy - 1;
         __syncthreads();
-        image_dispatch(img, [&](auto ch_c, auto fmt_c) {
+        image_dispatch<false>(img, [&](auto ch_c, auto fmt_c) {
             constexpr int CH = decltype(ch_c)::value, FMT = decltype(fmt_c)::value;
             for (int i = threadIdx.x; i < 3 * kWsCols; i += 256) {
                 const int c = i % kWsCols, kh = i / kWsCols;
@@ -790,7 +790,7 @@ cudaError_t wgrad_stem_launch(const WgradGeom& g, const ImageIn& img, const __nv
 // its staging rows [q][co] ARE the [tap][ci][co] layout.  One thread per output pixel: its 9 taps are loaded and decoded once each.
 __global__ void __launch_bounds__(256) stem_im2col_kernel(WgradGeom g, const __grid_constant__ ImageIn img, __nv_bfloat16* __restrict__ x27) {
     const size_t total = (size_t)g.N * g.Ho * g.Wo;
-    image_dispatch(img, [&](auto ch_c, auto fmt_c) {      // compile-time channel count: every q of a pixel is a fixed register
+    image_dispatch<false>(img, [&](auto ch_c, auto fmt_c) {      // compile-time channel count: every q of a pixel is a fixed register
         constexpr int CH = decltype(ch_c)::value, FMT = decltype(fmt_c)::value;
         for (size_t pix = (size_t)blockIdx.x * 256 + threadIdx.x; pix < total; pix += (size_t)gridDim.x * 256) {
             const int ox = (int)(pix % g.Wo), oy = (int)((pix / g.Wo) % g.Ho), n = (int)(pix / ((size_t)g.Wo * g.Ho));

@@ -129,6 +129,32 @@ def check_source(x, N, channels, nv12):
     return fmt, h, w
 
 
+# the packed camera-frame formats of InferencePlan.forward / StreamingDetector: name -> (nat.INPUT_* code, bytes per pixel)
+PACKED_FORMATS = {'yuy2': (nat.INPUT_U8_YUY2, 2), 'uyvy': (nat.INPUT_U8_UYVY, 2), 'bgra': (nat.INPUT_U8_BGRA, 4), 'rgba': (nat.INPUT_U8_RGBA, 4)}
+
+
+def check_packed(x, frame_format, N, channels, H=None, W=None):
+    """x: packed camera frames (include/lfd_b200.h), contiguous, on a CUDA device -- 'yuy2' / 'uyvy': YUV 4:2:2 uint8 [N,h,w,2] of an
+    even w; 'bgra' / 'rgba': uint8 [N,h,w,4] -- for a model that reads `channels` image channels (a gray model takes 4:2:2 only, of
+    which it reads the Y bytes); with a capacity H x W, h <= H and w <= W on an even W for 4:2:2 -> (its nat.INPUT_* format, h, w)."""
+    fmt, bpp = PACKED_FORMATS[frame_format]
+    if channels == 1 and bpp == 4:
+        raise ValueError("a gray model reads 4:2:2 frames ('yuy2' / 'uyvy'); %r frames are colour, got frame_format %r" % (frame_format, frame_format))
+    if bpp == 2 and W is not None and W % 2:
+        raise ValueError('4:2:2 frames need a plan of even width, this plan\'s capacity is %dx%d' % (H, W))
+    if x.dtype != torch.uint8 or x.dim() != 4 or x.shape[3] != bpp:
+        raise ValueError('%s frames are a uint8 [N, h, w, %d] tensor, got %s %s' % (frame_format.upper(), bpp, x.dtype, tuple(x.shape)))
+    n, h, w = (int(v) for v in x.shape[:3])
+    if bpp == 2 and w % 2:
+        raise ValueError('4:2:2 frames have an even width, got %dx%d' % (h, w))
+    if n != N or h < 1 or w < 1 or (H is not None and not (h <= H and w <= W)):
+        cap = ' of at most H=%d x W=%d (the plan\'s capacity)' % (H, W) if H is not None else ''
+        raise ValueError('input must be N=%d %s frames%s, got %d frames of %dx%d' % (N, frame_format.upper(), cap, n, h, w))
+    if not x.is_cuda or not x.is_contiguous():
+        raise ValueError('%s frames must be a contiguous CUDA tensor' % (frame_format.upper(),))
+    return fmt, h, w
+
+
 def stage_nv12(stage, x, h, w):
     """Copies NV12 frames x [N, 3h/2, w] into the capacity layout stage [N, 3H/2, W]: the Y rows into the top-left corner of the H x W Y
     plane, the UV rows into the top-left corner of the H/2 x W UV plane."""
@@ -807,8 +833,9 @@ class InferencePlan(object):
         return self._extents[(h, w)]
 
     def staging(self, fmt):
-        """The plan-owned input of frames below the capacity, in the capacity layout of format fmt (uint8 [N,H,W,3], float32 [N,3,H,W] or
-        NV12 uint8 [N,3H/2,W]; a gray plan: uint8 [N,H,W], float32 [N,1,H,W] or the same NV12 layout)."""
+        """The plan-owned input of frames below the capacity, in the capacity layout of format fmt (uint8 [N,H,W,3], float32 [N,3,H,W],
+        NV12 uint8 [N,3H/2,W], 4:2:2 uint8 [N,H,W,2] or BGRA / RGBA uint8 [N,H,W,4]; a gray plan: uint8 [N,H,W], float32 [N,1,H,W] or the
+        same NV12 and 4:2:2 layouts)."""
         c = self.in_channels
         if self._stage is None:
             self._stage = torch.empty(self.N * 3 * self.H * self.W * 4, dtype=torch.uint8, device=self.device)
@@ -816,6 +843,9 @@ class InferencePlan(object):
             return self._stage[:self.N * self.H * self.W * c].view(self.u8_shape(self.H, self.W))
         if fmt == nat.INPUT_U8_NV12:
             return self._stage[:self.N * self.H * self.W * 3 // 2].view(self.N, self.H * 3 // 2, self.W)
+        for code, bpp in PACKED_FORMATS.values():
+            if fmt == code:
+                return self._stage[:self.N * self.H * self.W * bpp].view(self.N, self.H, self.W, bpp)
         return self._stage.view(torch.float32)[:self.N * c * self.H * self.W].view(self.N, c, self.H, self.W)
 
     def u8_shape(self, h, w):
@@ -837,19 +867,26 @@ class InferencePlan(object):
         resize_scale=s: x holds N uint8 frames of any size h x w (above the capacity too; BGR [N,h,w,3], gray [N,h,w], or NV12 with
         frame_format='nv12'), resized on the device into the plan-owned input exactly as cv2.resize(frame, (0, 0), fx=s, fy=s) resizes them
         (lfd_resize_frames; NV12 as cv2.resize of the converted frame), and the forward runs at the resized size (nat.resize_query), which
-        must fit the capacity."""
+        must fit the capacity.
+        frame_format='yuy2' / 'uyvy' (YUV 4:2:2 uint8 [N,h,w,2], w even) or 'bgra' / 'rgba' (uint8 [N,h,w,4], the alpha byte never read):
+        packed camera frames, read by the stem kernels (and by the resize, with resize_scale) as the uint8 BGR path reads
+        cv2.cvtColor(frame, cv2.COLOR_{YUY2,UYVY,BGRA,RGBA}2BGR), bit for bit.  A gray plan takes 4:2:2 frames, of which it reads the Y
+        bytes (cv2.COLOR_YUV2GRAY_YUY2 / _UYVY), and raises ValueError for 'bgra' / 'rgba'."""
         if self.handle is None:
             raise nat.LfdError('this plan was built for host-side inspection only (create_native=False)')
-        if frame_format not in (None, 'nv12'):
-            raise ValueError("frame_format must be None (float32 NCHW or uint8 BGR, by dtype) or 'nv12', got %r" % (frame_format,))
+        if frame_format not in (None, 'nv12') and frame_format not in PACKED_FORMATS:
+            raise ValueError("frame_format must be None (float32 NCHW or uint8 BGR, by dtype) or 'nv12', got %r (packed camera frames: 'yuy2', "
+                             "'uyvy', 'bgra', 'rgba')" % (frame_format,))
         if resize_scale is not None:
-            return self._forward_resized(x, use_graph, slot, frame_format == 'nv12', float(resize_scale))
+            return self._forward_resized(x, use_graph, slot, frame_format, float(resize_scale))
         if frame_format is None:
             fmt, h, w = check_frame(x, self.N, self.H, self.W, self.in_channels)
             if fmt == nat.INPUT_U8_NHWC and self.in_channels == 1:
                 x = x.view(self.N, h, w)
-        else:
+        elif frame_format == 'nv12':
             fmt, (h, w) = nat.INPUT_U8_NV12, check_nv12_frame(x, self.N, self.H, self.W)
+        else:
+            fmt, h, w = check_packed(x, frame_format, self.N, self.in_channels, self.H, self.W)
         cls_out, reg_out = self.outputs(slot)
         lib = nat.lib()
         if (h, w) == (self.H, self.W):
@@ -865,10 +902,10 @@ class InferencePlan(object):
             stage = self.staging(fmt)
             if fmt == nat.INPUT_U8_NV12:
                 stage_nv12(stage, x, h, w)
-            elif fmt == nat.INPUT_U8_NHWC:
-                stage[:, :h, :w].copy_(x)
-            else:
+            elif fmt == nat.INPUT_F32_NCHW:
                 stage[:, :, :h, :w].copy_(x)
+            else:
+                stage[:, :h, :w].copy_(x)
             nat.check(lib.lfd_plan_forward_extent(self.handle, nat.ptr(stage), fmt, h, w, table, nat.ptr(self.workspace), nat.ptr(cls_out),
                                                   nat.ptr(reg_out), int(bool(use_graph)), nat.stream_ptr()))
         return self._frame_outputs(cls_out, reg_out, level_sizes, P)
@@ -878,12 +915,15 @@ class InferencePlan(object):
         n, c = self.N, self.cls_channels
         return cls_out.view(-1)[:n * P * c].view(n, P, c), reg_out.view(-1)[:n * P * 4].view(n, P, 4)
 
-    def _forward_resized(self, x, use_graph, slot, nv12, s):
+    def _forward_resized(self, x, use_graph, slot, frame_format, s):
         """forward(x, resize_scale=s): the resize into the uint8 staging input, then the forward at the resized extent on that input (one
         CUDA graph for the capacity, one for every size below it, as for frames staged by copy)."""
         if self.conv_impl != nat.CONV_UMMA:
             raise nat.LfdError('the SIMT cross-check plan does not take resized frames')
-        fmt, h, w = check_source(x, self.N, self.in_channels, nv12)
+        if frame_format in PACKED_FORMATS:
+            fmt, h, w = check_packed(x, frame_format, self.N, self.in_channels)
+        else:
+            fmt, h, w = check_source(x, self.N, self.in_channels, frame_format == 'nv12')
         _, dh, dw = nat.resize_query(h, w, s)
         if dh > self.H or dw > self.W:
             raise ValueError('%dx%d frames at resize scale %r are %dx%d, beyond the plan\'s capacity %dx%d' % (h, w, s, dh, dw, self.H, self.W))

@@ -16,6 +16,8 @@ ABI_VERSION = 5           # LFD_B200_ABI_VERSION
 
 OP_STEM0, OP_CONV, OP_GN_APPLY, OP_HEAD_FINAL, OP_STEM4 = 0, 1, 2, 3, 4
 INPUT_F32_NCHW, INPUT_U8_NHWC, INPUT_U8_NV12 = 0, 1, 2     # NV12: inference only, uint8 [N, 3H/2, W] (include/lfd_b200.h)
+# packed camera frames, inference only: 4:2:2 uint8 [N, H, W, 2] (W even), 4-byte pixels uint8 [N, H, W, 4] (include/lfd_b200.h)
+INPUT_U8_YUY2, INPUT_U8_UYVY, INPUT_U8_BGRA, INPUT_U8_RGBA = 4, 5, 6, 7
 CONV_UMMA, CONV_SIMT = 0, 1
 DTYPE_BF16, DTYPE_FP16 = 0, 1
 CLS_SIGMOID, CLS_SOFTMAX, CLS_BCE, CLS_QFL = 0, 1, 2, 3

@@ -45,7 +45,8 @@ class ForwardPostPipeline(object):
     is called with the post stream current, enqueue device->host copies (or anything else that reads them) there."""
 
     def __init__(self, model, plan, post, score_thr, iou_thr, frame_format=None, resize_scale=None):
-        """frame_format: of the device inputs, passed to plan.forward (None: float32 NCHW or uint8 BGR by dtype, 'nv12': NV12 frames);
+        """frame_format: of the device inputs, passed to plan.forward (None: float32 NCHW or uint8 BGR by dtype, 'nv12': NV12 frames,
+        'yuy2' / 'uyvy' / 'bgra' / 'rgba': packed camera frames);
         resize_scale: passed to plan.forward as well (the inputs are frames of another size, resized on the forward stream)."""
         self.model, self.plan, self.post = model, plan, post
         self.frame_format, self.resize_scale = frame_format, resize_scale
@@ -94,21 +95,26 @@ class StreamingDetector(object):
         to copy, converted to BGR inside the stem kernel bit for bit as cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12) would, after which
         input_pipeline applies as it does to BGR frames; 'gray' -- uint8 [N,H,W], for a gray model (a 1-channel stem conv).  A gray model
         takes 'gray' or 'nv12', of which it reads the Y plane only (cv2.COLOR_YUV2GRAY_NV12), and raises ValueError for 'bgr'; a BGR model
-        raises ValueError for 'gray'.
+        raises ValueError for 'gray'.  'yuy2' / 'uyvy' -- YUV 4:2:2 camera frames uint8 [N,H,W,2] (W even; a gray model reads their Y
+        bytes, cv2.COLOR_YUV2GRAY_YUY2 / _UYVY) and 'bgra' / 'rgba' -- uint8 [N,H,W,4] (BGR models only, the alpha byte is never read):
+        converted inside the stem kernels (or the resize) bit for bit as cv2.cvtColor(frame, cv2.COLOR_{YUY2,UYVY,BGRA,RGBA}2BGR) would.
         source_size=(h, w): the host frames are h x w (any size, in frame_format) and height x width stays the network's input size (the
         plan's capacity).  Each batch goes up at source size and is resized on the device, on the forward stream, exactly as
         cv2.resize(frame, (0, 0), fx=s, fy=s) would (NV12: cv2.resize of the converted frame); the network runs at the resized size, and the
         detections are in source-frame coordinates: the post-process takes the reference's meta of a resized image, int(w * s) x int(h * s)
         and resize_scale s.  resize_scale=None takes the largest s whose result fits: min(height / h, width / w); an explicit scale whose
         result does not fit raises ValueError."""
-        from ._engine import image_channels
-        if frame_format not in ('bgr', 'nv12', 'gray'):
-            raise ValueError("frame_format must be 'bgr' or 'nv12' ('gray' for a gray model), got %r" % (frame_format,))
+        from ._engine import image_channels, PACKED_FORMATS
+        if frame_format not in ('bgr', 'nv12', 'gray') and frame_format not in PACKED_FORMATS:
+            raise ValueError("frame_format must be 'bgr' or 'nv12' ('gray' for a gray model), got %r (packed camera frames: 'yuy2', 'uyvy', "
+                             "'bgra', 'rgba')" % (frame_format,))
         if source_size is None and resize_scale is not None:
             raise ValueError('resize_scale needs source_size: the size of the frames it resizes')
         src_h, src_w = (height, width) if source_size is None else (int(source_size[0]), int(source_size[1]))
         if frame_format == 'nv12' and (src_h % 2 or src_w % 2):
             raise ValueError('NV12 frames have an even height and width, got %dx%d' % (src_h, src_w))
+        if frame_format in ('yuy2', 'uyvy') and src_w % 2:
+            raise ValueError('4:2:2 frames have an even width, got %dx%d' % (src_h, src_w))
         self.source_size, self.resize_scale = None, None
         meta, (dh, dw) = (width, height, 1.0), (height, width)
         if source_size is not None:
@@ -122,7 +128,9 @@ class StreamingDetector(object):
             self.source_size, self.resize_scale = (src_h, src_w), s
             meta = (int(src_w * s), int(src_h * s), s)       # the reference's resized_width / resized_height / resize_scale
         gray = image_channels(model) == 1
-        if gray != (frame_format == 'gray') and frame_format != 'nv12':
+        if gray and frame_format in ('bgra', 'rgba'):
+            raise ValueError("a gray model takes frame_format 'gray', 'nv12', 'yuy2' or 'uyvy'; %r frames are colour" % (frame_format,))
+        if gray != (frame_format == 'gray') and frame_format not in ('nv12', 'yuy2', 'uyvy', 'bgra', 'rgba'):
             raise ValueError("a %s model takes frame_format '%s' or 'nv12', got %r" % ('gray' if gray else 'BGR', 'gray' if gray else 'bgr', frame_format))
         self.frame_format = frame_format
         from .data_pipeline.augmentation import input_transform_of
@@ -153,10 +161,15 @@ class StreamingDetector(object):
             model._head_indexes_to_feature_map_sizes[i] = hw
         self.post = model.post_plan(batch, level_sizes, dev)   # greedy NMS or Soft-NMS: model._nms_cfg as of now
         self.post.set_meta([meta[0]] * batch, [meta[1]] * batch, [meta[2]] * batch)
-        nv12 = frame_format == 'nv12'
-        self.pipe = ForwardPostPipeline(model, self.plan, self.post, self.score_thr, self.iou_thr, frame_format='nv12' if nv12 else None,
+        device_format = frame_format if frame_format == 'nv12' or frame_format in PACKED_FORMATS else None
+        self.pipe = ForwardPostPipeline(model, self.plan, self.post, self.score_thr, self.iou_thr, frame_format=device_format,
                                         resize_scale=self.resize_scale)
-        frame_shape = (batch, src_h * 3 // 2, src_w) if nv12 else self.plan.u8_shape(src_h, src_w)
+        if frame_format == 'nv12':
+            frame_shape = (batch, src_h * 3 // 2, src_w)
+        elif frame_format in PACKED_FORMATS:
+            frame_shape = (batch, src_h, src_w, PACKED_FORMATS[frame_format][1])
+        else:
+            frame_shape = self.plan.u8_shape(src_h, src_w)
         self.slots = []
         for _ in range(self.depth):
             self.slots.append(dict(
@@ -170,7 +183,8 @@ class StreamingDetector(object):
         self.d2h_bytes = batch * self.max_out * (5 * 4 + 4) + (batch + 1) * 4
 
     def submit(self, frames_u8):
-        """frames_u8: pinned (or pageable) host uint8 [N,H,W,3] (frame_format 'nv12': [N,3H/2,W]; 'gray': [N,H,W]); H x W is source_size
+        """frames_u8: pinned (or pageable) host uint8 [N,H,W,3] (frame_format 'nv12': [N,3H/2,W]; 'gray': [N,H,W]; 'yuy2' / 'uyvy':
+        [N,H,W,2]; 'bgra' / 'rgba': [N,H,W,4]); H x W is source_size
         when given.  Enqueues copy + compute; returns the slot index."""
         s = self.slots[self.step % self.depth]
         if s['busy']:
